@@ -1,5 +1,5 @@
 # Development / CI image for adapm_b200 (the reference ships an ubuntu + sshd + gdbserver dev image; this is the
-# B200 equivalent). Build:  docker build -t adapm_b200 .     Run:  docker run --gpus all --ipc=host -it adapm_b200
+# H100 equivalent). Build:  docker build -t adapm_b200 .     Run:  docker run --gpus all --ipc=host -it adapm_b200
 # --ipc=host (or a large --shm-size) is required: ranks rendezvous through a POSIX-shm control block and exchange
 # CUDA IPC handles.
 FROM nvidia/cuda:12.9.0-devel-ubuntu24.04
@@ -15,6 +15,6 @@ RUN pip install --no-cache-dir torch --index-url https://download.pytorch.org/wh
 
 WORKDIR /workspace/adapm_b200
 COPY . .
-# nvcc cross-compiles sm_100a without a GPU: the extension is built into the image
+# nvcc cross-compiles sm_90a without a GPU: the extension is built into the image
 RUN python -m adapm_b200._build
 CMD ["python", "-m", "pytest", "tests", "-q", "-m", "not gpu"]

@@ -1,4 +1,4 @@
-"""adapm_b200 - a Blackwell-native, intent-driven parameter manager.
+"""adapm_b200 - a GPU-native (Hopper, sm_90a), intent-driven parameter manager.
 
 Python API with the reference's method names (``bindings/bindings.cc:79-374`` of
 alexrenz/AdaPM): ``setup``, ``scheduler``, ``Server``, ``Worker`` with
@@ -6,7 +6,7 @@ alexrenz/AdaPM): ``setup``, ``scheduler``, ``Server``, ``Worker`` with
 pull_sample / begin_setup / end_setup / wait_sync / barrier / wait / waitall /
 finalize / get_key_size / num_keys``.
 
-Differences that follow from the B200-first design:
+Differences that follow from the GPU-first design:
 
 * one process per GPU (``torchrun``); there is no scheduler process - ``scheduler()``
   returns immediately and exists only so that reference launch scripts keep working;

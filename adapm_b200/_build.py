@@ -1,8 +1,8 @@
 """In-tree build of the native extension ``adapm_b200/_C*.so``.
 
-Everything is compiled explicitly for sm_100a (``-gencode arch=compute_100a,code=sm_100a
+Everything is compiled explicitly for sm_90a (``-gencode arch=compute_90a,code=sm_90a
 -lineinfo``); nvcc cross-compiles without a GPU. The resulting ``.so`` sits next to the
-Python sources so that it travels with the repository snapshot to the GPU box.
+Python sources, so the package imports straight from the repository tree.
 
     python -m adapm_b200._build            # incremental (ninja)
     python -m adapm_b200._build --force    # rebuild everything
@@ -54,7 +54,7 @@ def _ninja_file() -> str:
     incs = f"-I{CSRC} -I{pybind11.get_include()} -I{py_inc} -I{CUDA_HOME}/include"
     cxxflags = f"-O3 -g1 -std=c++17 -fPIC -fvisibility=hidden -Wall -Wno-unused-function -pthread {incs}"
     nvflags = (
-        "-O3 -std=c++17 -lineinfo -gencode arch=compute_100a,code=[sm_100a,compute_100a] "
+        "-O3 -std=c++17 -lineinfo -gencode arch=compute_90a,code=[sm_90a,compute_90a] "
         "--expt-relaxed-constexpr -Xcompiler -fPIC,-fvisibility=hidden,-pthread "
         f"-Xptxas -v {incs}"
     )

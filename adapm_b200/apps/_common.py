@@ -22,7 +22,7 @@ def add_system_options(ap: argparse.ArgumentParser) -> None:
         g.add_argument("--" + f, dest=f, default=None)
     g.add_argument("--backend", default=None, choices=["cpu", "cuda"])
     g.add_argument("--value_type", default="float", choices=["float", "double"],
-                   help="type of the parameter values: float (fused sm_100a kernels) or double (the reference's ValT for kge "
+                   help="type of the parameter values: float (fused sm_90a kernels) or double (the reference's ValT for kge "
                         "and mf; trains through Pull / Push with the same update rule on either backend)")
 
 

@@ -149,7 +149,7 @@ def main(argv=None) -> int:
             break
     if rank == 0:
         if model.cuda and cfg.algorithm == "ComplEx" and cfg.embed_dim % 4 == 0:
-            # fused gather + tcgen05 GEMM + rank count: entity rows are read from every GPU's HBM in-kernel
+            # fused gather + wgmma GEMM + rank count: entity rows are read from every GPU's HBM in-kernel
             print(f"[kge] test (fused gather-GEMM eval): {evaluate_fused(model, te, known)}", flush=True)
     ev = model.evaluate_distributed(te, known)
     if rank == 0:

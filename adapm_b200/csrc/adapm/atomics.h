@@ -1,8 +1,8 @@
-// Memory primitives shared by the CPU executor and the sm_100a kernels.
+// Memory primitives shared by the CPU executor and the sm_90a kernels.
 //
 // The parameter manager talks to peers through *memory semantics*: a peer's heap
 // is mapped into this address space (POSIX shm on CPU, CUDA IPC / NVLink peer
-// mapping on B200) and every protocol step is a load, store, or reduction on such
+// mapping on the GPU) and every protocol step is a load, store, or reduction on such
 // a pointer. On the device all cross-rank accesses use system scope so that they
 // are coherent over NVLink; on the host they are __atomic builtins.
 #pragma once
@@ -16,7 +16,7 @@ namespace adapm {
 namespace mem {
 
 #if defined(__CUDA_ARCH__)
-// ---------------------------------------------------------------- device (sm_100a)
+// ---------------------------------------------------------------- device (sm_90a)
 ADAPM_D uint32_t ld_acquire(const uint32_t* p) {
   uint32_t v;
   asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");

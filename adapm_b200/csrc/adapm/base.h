@@ -1,4 +1,4 @@
-// Base types of the B200-native parameter manager.
+// Base types of the GPU-native parameter manager.
 //
 // Parity with the reference's include/ps/base.h:1-65 (Key, Clock, CLOCK_MAX,
 // WORKER_FINISHED, WINDOW_MAX, Version, MgmtTechniques, LOCAL). The reference

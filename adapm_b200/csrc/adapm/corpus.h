@@ -3,7 +3,7 @@
 //
 // Capability parity with the corpus handling of the reference application (apps/word2vec.cc:147-364 vocabulary hash /
 // sort / min_count pruning, :563-606 reading sentences ahead, :672-690 window shrinking, frequent-word subsampling),
-// re-shaped for a GPU consumer: a B200 trains 32 768 pairs in 0.74 ms, i.e. the loader has to deliver ~45 M pairs/s per
+// re-shaped for a GPU consumer: a GPU trains 32 768 pairs in a few ms, i.e. the loader has to deliver millions of pairs/s per
 // GPU, so batches are produced by a C++ thread into a bounded ring of buffers while the previous batches train.
 #pragma once
 #include <atomic>

@@ -10,7 +10,7 @@
 //           support it; cudaMalloc + CUDA IPC is the fallback. Peers read and write the
 //           heaps directly over NVLink/NVSwitch.
 //
-// This is the B200-native stand-in for ZMQVan + Van + Postoffice node management
+// This is the GPU-native stand-in for ZMQVan + Van + Postoffice node management
 // (include/zmq_van.h:30-250, src/van.cc:267-357): no data ever travels through a socket
 // and there is no message (de)serialisation anywhere.
 #pragma once

@@ -1,7 +1,7 @@
 // Symmetric-heap layout of one rank's parameter store.
 //
 // Every rank allocates ONE heap with the SAME layout; peers map each other's heaps
-// (POSIX shm on CPU, CUDA-IPC/NVLink on B200), so any per-key or per-slot field of
+// (POSIX shm on CPU, CUDA-IPC/NVLink on the GPUs), so any per-key or per-slot field of
 // any rank is `heap[rank] + offset`. This replaces the reference's
 // vector<unique_ptr<Parameter>> + 16384 mutexes (coloc_kv_server_handle.h:122-152,
 // :1069-1083) and its Addressbook (addressbook.h:30-176): the ownership directory

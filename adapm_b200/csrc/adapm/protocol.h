@@ -2,8 +2,8 @@
 //
 // Every function here is a per-key / per-slot step executed by a "group" of lanes:
 // one CPU thread (HostGroup) or one 32-wide warp (WarpGroup, see cuda/group.cuh).
-// The CPU executor and the sm_100a kernels both instantiate this file, so the CPU
-// contract tests exercise the exact state machine that runs on B200.
+// The CPU executor and the sm_90a kernels both instantiate this file, so the CPU
+// contract tests exercise the exact state machine that runs on the GPU.
 //
 // What it replaces in the reference (studied, not copied):
 //   worker fast path       coloc_kv_worker.h:120-318, coloc_kv_server_handle.h:346-478

@@ -283,8 +283,8 @@ void SyncEngine::round(bool sweep) {
 // within a step or two, so that set saturates and a round costs the same whether it comes after 2 steps or after 20.
 // Under load the rounds pace themselves (a round takes longer than min_clocks steps), but after any gap in the step
 // stream (barrier, checkpoint, loader stall) the engine would otherwise restart with a burst of short-interval rounds,
-// each refreshing the whole hot set again - measured at 8 GPUs: 2 x the refresh traffic per step and 20 % slower steps in
-// the 20 steps after a barrier (profiles/README.md). Requests that wait for rounds (WaitSync, shutdown) are served at
+// each refreshing the whole hot set again (more refresh traffic per step and slower steps right after the gap).
+// Requests that wait for rounds (WaitSync, shutdown) are served at
 // once, and without clock progress a round starts every min_clocks_wait_ms so that intents and evictions never starve.
 void SyncEngine::pace(bool device_round) {
   ADAPM_NVTX("adapm::sync::pace");

@@ -1,4 +1,4 @@
-// Generic parameter-manager kernels for sm_100a and their host driver.
+// Generic parameter-manager kernels for sm_90a and their host driver.
 //
 // Kernel inventory (SURVEY 2.5 numbering):
 //   K1  pull_kernel        batched gather: in-kernel directory lookup, local HBM rows or
@@ -228,11 +228,11 @@ __global__ void __launch_bounds__(kThreads) phase_scan_kernel(const __grid_const
 //   global (local HBM or NVLink peer) --cp.async.bulk--> shared memory --(warp: LDS, subtract, STS)-->
 //   --cp.reduce.async.bulk.add.f32 / cp.async.bulk--> global
 // and every warp keeps kRowStages operations in flight in a ring of shared-memory stages, without occupying the
-// load / store slots of the SM. MEASURED (2 GPUs, next to the SGNS step, profiles/README.md): the pass takes 3 x LONGER
-// than the register variant (C.row 11.3 vs 3.3 ms, A.row 2.5 vs 0.9 ms per round) - the training kernel keeps the SM's
-// TMA unit busy (27 bulk loads + 27 bulk reductions per pair), so the round's bulk operations queue behind it, while
-// the LSU path it leaves alone is comparatively idle. Steps that overlap the pass are slightly faster (0.996 vs
-// 1.072 ms) and the end-to-end rate is the same within noise (2.00 vs 1.97 G updates/s), but rounds that take three
+// load / store slots of the SM. Next to the SGNS step this pass was measured to take longer than the register variant
+// (on the previous hardware target; not re-measured on H100) - the training kernel keeps the SM's TMA unit busy
+// (27 bulk loads + 27 bulk reductions per pair), so the round's bulk operations queue behind it, while the LSU path
+// it leaves alone is comparatively idle. Steps that overlap the pass were slightly faster and the end-to-end rate the
+// same within noise, but rounds that take three
 // times as long mean staler replicas, so the register variant stays the default.
 constexpr int kRowWarps = 2;        // warps per block
 constexpr int kRowStages = 3;       // operations in flight per warp
@@ -596,6 +596,27 @@ CudaBackend::CudaBackend(const Options& opt, const Layout& L, std::shared_ptr<Fa
   dev_timeout_ns_ = (unsigned long long)(std::min(opt.wait_timeout_s, 20.0) * 1e9);
 }
 
+CudaBackend::FxScratch& CudaBackend::fx_scratch(size_t rows, int row_len) {
+  use_device();
+  if (!fx_.cidx) {
+    const size_t nk = (size_t)ctx_.L.num_keys;
+    ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.cidx, nk * sizeof(int)));
+    ADAPM_CUDA_CHECK(cudaMemset(fx_.cidx, 0xff, nk * sizeof(int)));
+    ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.count, sizeof(unsigned int)));
+    ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.loss, sizeof(unsigned long long)));
+    ADAPM_CUDA_CHECK(cudaMemset(fx_.loss, 0, sizeof(unsigned long long)));
+  }
+  if (rows > fx_.rows || row_len != fx_.row_len) {
+    if (fx_.acc) { ADAPM_CUDA_CHECK(cudaFree(fx_.acc)); ADAPM_CUDA_CHECK(cudaFree(fx_.keys)); }
+    ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.acc, rows * row_len * sizeof(long long)));
+    ADAPM_CUDA_CHECK(cudaMemset(fx_.acc, 0, rows * row_len * sizeof(long long)));
+    ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.keys, rows * sizeof(Key)));
+    fx_.rows = rows;
+    fx_.row_len = row_len;
+  }
+  return fx_;
+}
+
 CudaBackend::~CudaBackend() {
   cudaSetDevice(device_);
   cudaDeviceSynchronize();
@@ -611,6 +632,11 @@ CudaBackend::~CudaBackend() {
   if (recs_host_) cudaFreeHost(recs_host_);
   if (status_dev_) cudaFree(status_dev_);
   if (status_host_) cudaFreeHost(status_host_);
+  if (fx_.acc) cudaFree(fx_.acc);
+  if (fx_.cidx) cudaFree(fx_.cidx);
+  if (fx_.keys) cudaFree(fx_.keys);
+  if (fx_.count) cudaFree(fx_.count);
+  if (fx_.loss) cudaFree(fx_.loss);
   if (round_done_) cudaEventDestroy(round_done_);
   for (auto& kv : tickets_) cudaEventDestroy(kv.second);
   for (auto e : event_pool_) cudaEventDestroy(e);

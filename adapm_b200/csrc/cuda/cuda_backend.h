@@ -1,4 +1,4 @@
-// CudaBackend: the B200 executor of the protocol. One instance per rank = per GPU.
+// CudaBackend: the GPU executor of the protocol. One instance per rank = per GPU.
 // Heaps are peer-mapped device allocations (VMM handles + NVLS multicast or CUDA IPC across
 // processes - fabric.cc; peer access inside one process); every kernel receives the Ctx by value and dereferences peer heaps
 // directly, so Pull = NVLink loads, Push = NVLink reductions (REDG), directory updates =
@@ -74,6 +74,18 @@ class CudaBackend : public Backend {
     return s;
   }
   int num_sms() const { return num_sms_; }
+  // device scratch of the deterministic one-GPU SGNS step (ops_sgns_tma.cu), owned by the backend, grown on demand:
+  // fixed-point accumulator rows, the compact row index of every key touched by the step (-1 = none) and its inverse
+  struct FxScratch {
+    long long* acc = nullptr;          // [rows][row_len]
+    size_t rows = 0;
+    int row_len = 0;
+    int* cidx = nullptr;               // [num_keys]
+    Key* keys = nullptr;               // [rows]
+    unsigned int* count = nullptr;     // number of compact rows of the current step
+    unsigned long long* loss = nullptr;
+  };
+  FxScratch& fx_scratch(size_t rows, int row_len);
 
   // ---- kernel timeline: CUDA events around every sync-round kernel plus user marks, all relative to one base
   // event, so that the round's kernels and the training kernels of other streams land on one time axis
@@ -99,7 +111,7 @@ class CudaBackend : public Backend {
   Ctx ctx_;
   bool int_rows_ = false;   // Options::dtype == int64 (8-byte rows are float64 otherwise)
   int device_ = 0;
-  int num_sms_ = 148;
+  int num_sms_ = 132;
   // grid sizes of the sync-round kernels, in blocks per SM. The round runs on a high-priority stream next to the
   // training kernels: a small footprint lets it share the SMs with them instead of displacing them.
   struct TraceRec { const char* name; cudaEvent_t a, b; };
@@ -140,6 +152,7 @@ class CudaBackend : public Backend {
   uint64_t fused_rounds_ = 0;          // barrier sequence numbers derive from it (same on every rank)
   unsigned long long dev_timeout_ns_ = 20ull * 1000000000ull;
   std::vector<uint32_t> key_len_;   // host mirror of per-key lengths (mixed-length stores only)
+  FxScratch fx_;
 };
 
 }  // namespace adapm

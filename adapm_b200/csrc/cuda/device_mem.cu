@@ -198,7 +198,7 @@ uint64_t vmm_granularity(int dev, int world, bool multicast) {
     mp.size = g;
     mp.handleTypes = CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR;
     size_t mg = 0;
-    // (the RECOMMENDED multicast granularity is 512 MB on B200; the minimum - 2 MB - is what binding requires)
+    // (the RECOMMENDED multicast granularity can be far larger; the minimum - 2 MB - is what binding requires)
     ADAPM_CU_CHECK(drv().MulticastGetGranularity(&mg, &mp, CU_MULTICAST_GRANULARITY_MINIMUM));
     if (mg > g) g = mg;
   }

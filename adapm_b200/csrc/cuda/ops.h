@@ -17,7 +17,7 @@ void sgns_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const K
 bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, const Key* negatives,
                    int n_pairs, int neg, int d, float alpha, float* loss_out, unsigned long long* stats);
 
-// word2vec SGNS with shared negatives on the tensor cores (ops_sgns_shared.cu): three tcgen05 GEMMs + three elementwise
+// word2vec SGNS with shared negatives on the tensor cores (ops_sgns_shared.cu): three wgmma GEMMs + three elementwise
 // kernels between ONE Pull and ONE Push of the rows [centers | contexts | shared negatives].
 size_t sgns_shared_workspace_bytes(int B, int Nn, int d);
 void sgns_shared_core(cudaStream_t stream, const float* R, const Key* contexts, const Key* negs, int B, int Nn, int d,
@@ -47,14 +47,14 @@ void mf_step(CudaBackend& be, cudaStream_t stream, const Key* row_keys, const Ke
              const int* row_nnz, const int* col_nnz, int n, int rank, float eps, float lambda, float* loss_out,
              unsigned long long* stats);
 
-// tcgen05/TMEM/TMA GEMM: C[M,N] fp32 = A[M,K] bf16 x B[N,K]^T bf16 (ops_gemm_tcgen05.cu)
+// wgmma/TMA GEMM: C[M,N] fp32 = A[M,K] bf16 x B[N,K]^T bf16 (ops_gemm_wgmma.cu)
 void gemm_nt_bf16(cudaStream_t stream, const void* A, const void* B, int M, int N, int K, float* C, int ldc);
 void gemm_nt_e4m3(cudaStream_t stream, const void* A, const void* B, int M, int N, int K, float* C, int ldc, float alpha);
 // same GEMM with the ranking epilogue: rank_out[row] += #{col != true_col[row] : score > true_score[row]}
 void gemm_nt_bf16_rank_count(cudaStream_t stream, const void* A, const void* B, int M, int N, int K,
                              const float* true_score, const int* true_col, int* rank_out);
 
-// fused gather (local HBM / NVLink peers, through the directory) + tcgen05 GEMM (ops_gather_gemm.cu):
+// fused gather (local HBM / NVLink peers, through the directory) + wgmma GEMM (ops_gather_gemm.cu):
 // C[M,N] = Q[M,K] (bf16, row pitch ldq) x rows(keys[0..N))[0..K)^T, rows read from the parameter store
 void gather_gemm(CudaBackend& be, cudaStream_t stream, const void* Q, const Key* keys, int M, int N, int K, int ldq, float* C,
                  int ldc, unsigned long long* stats);

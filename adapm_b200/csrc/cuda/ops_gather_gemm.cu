@@ -1,19 +1,19 @@
-// Fused parameter gather + tensor-core GEMM (sm_100a): the "Intent-prefetch all-gather (+) consumer GEMM"
+// Fused parameter gather + tensor-core GEMM (sm_90a): the "Intent-prefetch all-gather (+) consumer GEMM"
 // hot path of the north star. Scores C[M, N] = Q[M, K] x E[keys[0..N), 0..K)^T where the rows of E are
 // NOT a dense matrix: they live in the parameter store, spread over the HBM of all GPUs. Producer warps
 // resolve each key through the replicated directory, read the fp32 embedding rows straight from the local
 // slab / local replica / a peer GPU over NVLink (16-byte loads on peer-mapped pointers), convert to bf16
-// and write them into the 128-byte-swizzled K-major shared-memory layout that tcgen05.mma consumes - in the
-// same kernel as the UTCHMMA tiles, overlapped with them through an mbarrier ring. The query tile arrives
+// and write them into the 128-byte-swizzled K-major shared-memory layout that wgmma consumes - in the
+// same kernel as the wgmma tiles, overlapped with them through an mbarrier ring. The query tile arrives
 // through TMA. Epilogues: STORE (fp32 scores) or RANK_COUNT (filtered-ranking evaluation of the KGE models:
 // the [M x N] score matrix and the gathered entity matrix never exist in HBM).
 //
-// Warp roles (384 threads): 0 TMA(Q) | 1 MMA issuer | 2 TMEM alloc | 4-7 epilogue | 8-11 row gatherers.
+// Warpgroup roles (384 threads): 0 row gatherers (thread 0 also issues the TMA of Q) | 1-2 wgmma consumers + epilogue.
 #include <cuda_runtime.h>
 
 #include "ops.h"
 #include "pm_kernels.cuh"
-#include "tcgen05_utils.cuh"
+#include "wgmma_utils.cuh"
 
 namespace adapm {
 namespace cudaops {
@@ -22,7 +22,6 @@ namespace {
 
 using namespace tc;
 
-constexpr int kGatherThreads = 384;
 constexpr int BK_ELEMS = 64;  // bf16 elements per 128-byte K-block row
 
 enum GEpilogue : int { G_STORE = 0, G_RANK_COUNT = 1 };
@@ -33,7 +32,7 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
 }
 
 template <int EPI>
-__global__ void __launch_bounds__(kGatherThreads, 1)
+__global__ void __launch_bounds__(kGemmThreads, 1)
 gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ Ctx c,
                    const Key* __restrict__ keys, int M, int N, int K, float* __restrict__ C, int ldc,
                    const float* __restrict__ true_score, const int* __restrict__ true_col, int* __restrict__ rank_out,
@@ -46,56 +45,18 @@ gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
   const int num_kb = (K + BK_ELEMS - 1) / BK_ELEMS;
   dev::cta_enter(c);   // the gather warps read store rows through the directory: count this CTA in the grace epoch
 
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     // full: 1 arrival (TMA expect_tx for the Q tile) + 4 arrivals (one per gather warp)
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&sm.full_bar[s], 5); mbar_init(&sm.empty_bar[s], 1); }
-    mbar_init(&sm.tmem_full_bar, 1);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&sm.full_bar[s], 5); mbar_init(&sm.empty_bar[s], kConsumerWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_q) : "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm.tmem_base)), "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  if (warp == 0 && lane == 0) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_q) : "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = sm.tmem_base;
 
-  if (warp == 0) {
-    // ===================== TMA producer: query tile =====================
-    if (lane == 0) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (uint32_t)(kb / STAGES) & 1u;
-        mbar_wait(&sm.empty_bar[s], ph ^ 1u);
-        mbar_expect_tx(&sm.full_bar[s], A_BYTES);
-        tma_load_2d(sm.a[s], &tmap_q, &sm.full_bar[s], kb * BK_ELEMS, tile_m * BM);
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc(KIND_BF16, BM, BN);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (uint32_t)(kb / STAGES) & 1u;
-        mbar_wait(&sm.full_bar[s], ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t a_addr = smem_u32(sm.a[s]);
-        const uint32_t b_addr = smem_u32(sm.b[s]);
-#pragma unroll
-        for (int k = 0; k < ROW_BYTES / MMA_K_BYTES; ++k)
-          umma<KIND_BF16>(tmem_base, umma_desc(a_addr + k * MMA_K_BYTES), umma_desc(b_addr + k * MMA_K_BYTES), idesc,
-                          (kb | k) != 0 ? 1u : 0u);
-        umma_commit(&sm.empty_bar[s]);
-      }
-      umma_commit(&sm.tmem_full_bar);
-    }
-  } else if (warp >= 8) {
-    // ===================== gatherers: store rows (local HBM / NVLink peers) -> swizzled smem =====================
-    const int t = threadIdx.x - 256;          // tile row handled by this thread (0..127)
+  if (warp < 4) {
+    // ===================== gatherers: store rows (local HBM / NVLink peers) -> swizzled smem; thread 0 also TMAs Q ==
+    const int t = threadIdx.x;                // tile row handled by this thread (0..127)
     const int n = tile_n * BN + t;
     const float* row = nullptr;
     unsigned nl = 0, nr = 0;
@@ -112,6 +73,10 @@ gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
       const int s = kb % STAGES;
       const uint32_t ph = (uint32_t)(kb / STAGES) & 1u;
       mbar_wait(&sm.empty_bar[s], ph ^ 1u);
+      if (t == 0) {
+        mbar_expect_tx(&sm.full_bar[s], A_BYTES);
+        tma_load_2d(sm.a[s], &tmap_q, &sm.full_bar[s], kb * BK_ELEMS, tile_m * BM);
+      }
       unsigned char* dst_row = sm.b[s] + (size_t)t * ROW_BYTES;
       const int k0 = kb * BK_ELEMS;
       // 64 floats of this row -> 8 chunks of 8 bf16; chunk c goes to position c ^ (t & 7)  (128B swizzle)
@@ -132,9 +97,7 @@ gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor core
       __syncwarp();
-      if (lane == 0) {
-        asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&sm.full_bar[s])) : "memory");
-      }
+      if (lane == 0) mbar_arrive(&sm.full_bar[s]);
     }
     if (stats) {
 #pragma unroll
@@ -144,38 +107,15 @@ gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
         if (nr) atomicAdd(stats + 1, (unsigned long long)nr);
       }
     }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    const int q = warp & 3;
-    mbar_wait(&sm.tmem_full_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int row = tile_m * BM + q * 32 + lane;
-    float ts = 0.f;
-    int tcol = -1, cnt = 0;
-    if (EPI == G_RANK_COUNT && row < M) { ts = true_score[row]; tcol = true_col[row]; }
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-      uint32_t r[32];
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
-      const int col0 = tile_n * BN + c0;
-      if (EPI == G_STORE) {
-        store_chunk_coalesced(r, sm.epi[q], 1.f, C, ldc, tile_m * BM + q * 32, col0, M, N, lane);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int col = col0 + j;
-          cnt += (col < N && col != tcol && __uint_as_float(r[j]) > ts) ? 1 : 0;
-        }
-      }
-    }
-    if (EPI == G_RANK_COUNT && row < M && cnt) atomicAdd(rank_out + row, cnt);
-  }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
+  } else {
+    // ===================== consumers: wgmma -> registers -> C / counts =====================
+    const int wg = (warp >> 2) - 1;
+    float d[64];
+    consume_ring<KIND_BF16>(sm, num_kb, wg, lane, d);
+    const int row0 = tile_m * BM + wg * 64 + (warp & 3) * 16;
+    const int col0 = tile_n * BN;
+    if (EPI == G_STORE) store_fragment(d, 1.f, C, ldc, row0, col0, M, N, lane, false);
+    else rank_count_fragment(d, true_score, true_col, rank_out, row0, col0, M, N, lane);
   }
   dev::cta_exit(c);
 }
@@ -195,7 +135,7 @@ void launch_gather(CudaBackend& be, cudaStream_t stream, const void* Q, const Ke
     attr_set = true;
   }
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
-  gather_gemm_kernel<EPI><<<grid, kGatherThreads, smem, stream>>>(mq, be.ctx(), keys, M, N, K, C, ldc, true_score, true_col,
+  gather_gemm_kernel<EPI><<<grid, kGemmThreads, smem, stream>>>(mq, be.ctx(), keys, M, N, K, C, ldc, true_score, true_col,
                                                                   rank_out, stats);
   ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cudaGetLastError());

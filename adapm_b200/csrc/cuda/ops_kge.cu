@@ -1,4 +1,4 @@
-// Fused knowledge-graph-embedding training step (ComplEx) for sm_100a: Pull(s, r, o) + score +
+// Fused knowledge-graph-embedding training step (ComplEx) for sm_90a: Pull(s, r, o) + score +
 // BCE gradient + L2 + AdaGrad + Push(s, r, o) in one kernel over local HBM / NVLink peers
 // (SURVEY K1 + K8 + K9 + K2 + K14).
 //

@@ -1,4 +1,4 @@
-// Fused matrix-factorisation SGD step for sm_100a: Pull(w_i, h_j) + error + L2 + AdaGrad + Push
+// Fused matrix-factorisation SGD step for sm_90a: Pull(w_i, h_j) + error + L2 + AdaGrad + Push
 // in one kernel over local HBM / NVLink peers (SURVEY K1 + K10 + K9 + K2).
 //
 // Update rule = the reference's UpdateNsqlL2Adagrad (apps/mf/update.h:32-70):

@@ -1,4 +1,4 @@
-// Fused word2vec SGNS step for sm_100a: Pull + dot/sigmoid + AdaGrad + Push in ONE kernel,
+// Fused word2vec SGNS step for sm_90a: Pull + dot/sigmoid + AdaGrad + Push in ONE kernel,
 // reading rows from and reducing updates into whichever HBM currently holds each key
 // (local slab, local replica, or a peer GPU over NVLink) - SURVEY K1+K7+K9+K2.
 //

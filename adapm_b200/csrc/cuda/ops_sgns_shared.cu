@@ -10,8 +10,8 @@
 //     dE0 [B, d]  = G x En        + gpos * Ec    center gradient (gpos = 1 - sigmoid(<e0, ec>), the positive target)
 //     dEn [Nn, d] = G^T x E0                     negative gradient
 //
-// i.e. B * Nn sample pairs for 2 B + Nn rows of traffic. All three contractions run on the hand-written tcgen05 / TMEM /
-// TMA GEMM of this package (ops_gemm_tcgen05.cu; bf16 operands, fp32 accumulation); the pieces around them are the
+// i.e. B * Nn sample pairs for 2 B + Nn rows of traffic. All three contractions run on the hand-written wgmma /
+// TMA GEMM of this package (ops_gemm_wgmma.cu; bf16 operands, fp32 accumulation); the pieces around them are the
 // three kernels of this file:
 //   shared_prep_kernel    rows (fp32, as pulled from the store) -> bf16 operand + its transpose (tile transposition
 //                         through shared memory), positive-target gradient gpos and its loss

@@ -1,4 +1,4 @@
-// SGNS step, TMA-prefetch variant (sm_100a): same semantics as ops_sgns.cu, but the target rows of a
+// SGNS step, TMA-prefetch variant (sm_90a): same semantics as ops_sgns.cu, but the target rows of a
 // pair stream through a per-warp shared-memory ring that is filled by the TMA engine
 // (cp.async.bulk global -> shared, completion on an mbarrier) several targets ahead of the math.
 //
@@ -71,6 +71,29 @@ template <int N> __device__ __forceinline__ void bulk_wait_read() {   // all but
 }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
+// dev::mark_pushed on the packed (mark pointer, kind bit) form of a Target
+__device__ __forceinline__ void mark_pushed(void* mark, int bits) {
+  if (!mark) return;
+  if (bits & 2) *static_cast<uint8_t*>(mark) = (uint8_t)1;
+  else mem::red_add(static_cast<uint32_t*>(mark), 1u);
+}
+
+// Deterministic accumulation (one GPU): updates are added as 64-bit fixed-point integers into an accumulator row per
+// key touched by the step instead of into the store rows, so the step reads only start-of-step values and the sums do
+// not depend on the order in which warps add them; sgns_fx_apply_kernel then adds each row's sum to the store once.
+// |embedding update| <= alpha per contribution (AdaGrad normalises it), AdaGrad increments are squared gradients:
+// 2^40 / 2^36 leave 2^23 / 2^27 of range. Within each half of an accumulator row, element 4j + c sits at c * d/4 + j,
+// so that one warp-wide atomic over the lanes' j covers contiguous memory.
+constexpr float kFxEmb = 1099511627776.f;     // 2^40
+constexpr float kFxAda = 68719476736.f;       // 2^36
+constexpr float kFxLoss = 4294967296.f;       // 2^32
+__device__ __forceinline__ void fx_add4(long long* half, int j, int nvec, float4 v, float scale) {
+  atomicAdd(reinterpret_cast<unsigned long long*>(half + j), (unsigned long long)__float2ll_rn(v.x * scale));
+  atomicAdd(reinterpret_cast<unsigned long long*>(half + nvec + j), (unsigned long long)__float2ll_rn(v.y * scale));
+  atomicAdd(reinterpret_cast<unsigned long long*>(half + 2 * nvec + j), (unsigned long long)__float2ll_rn(v.z * scale));
+  atomicAdd(reinterpret_cast<unsigned long long*>(half + 3 * nvec + j), (unsigned long long)__float2ll_rn(v.w * scale));
+}
+
 struct WarpSmem {
   unsigned long long bar[RING];
 };
@@ -84,19 +107,23 @@ struct WarpSmem {
 // BULK (ADAPM_SGNS_BULKRED=1): the updates of a target leave as ONE TMA bulk reduction per row: the warp overwrites the
 // consumed ring slot with [embedding update | AdaGrad update] and lane 0 issues cp.reduce.async.bulk from it; the slot is
 // reloaded one target later, after the reduction has read it (prefetch distance RING - 1).
-template <int VPL, int MAXREG, bool BULK>
-__global__ void __maxnreg__(MAXREG)
-sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
-                     const Key* __restrict__ negatives, int n_pairs, int neg, int d, float alpha,
-                     float* __restrict__ loss_out, unsigned long long* __restrict__ stats, int tma_remote) {
+// FX: deterministic one-GPU variant (fixed-point accumulation, see kFxEmb); instantiated as its own kernel
+// (sgns_step_tma_fx_kernel) so that the in-place variants keep their register allocation.
+template <int VPL, bool BULK, bool FX>
+__device__ __forceinline__ void
+sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
+                   const Key* __restrict__ negatives, int n_pairs, int neg, int d, float alpha,
+                   float* __restrict__ loss_out, unsigned long long* __restrict__ stats, int tma_remote,
+                   long long* __restrict__ fx_acc, const int* __restrict__ fx_cidx,
+                   unsigned long long* __restrict__ fx_loss) {
   // per warp: RING row buffers of 2*d floats (16-byte aligned) | generic-path scratch is carved from the ring
   extern __shared__ __align__(128) unsigned char smem_raw[];
   __shared__ WarpSmem wsm[kWarps];
   dev::cta_enter(c);
   const int lane = threadIdx.x & 31;
   const int wib = threadIdx.x >> 5;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  const int warp = blockIdx.x * kWarps + wib;       // launched with kThreads threads: the compile-time warp count lets
+  const int nwarps = gridDim.x * kWarps;             // ptxas rematerialise the grid stride instead of spilling it
   const int nvec = d >> 2;
   const uint32_t row_bytes = (uint32_t)(2 * d * sizeof(float));
   const size_t buf_floats = ((size_t)2 * d + 31) & ~(size_t)31;  // keep every ring slot 128-byte aligned
@@ -119,23 +146,28 @@ sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ cent
     const Key pos_key = contexts[p];
     // ---- resolve center (lane 0) + up to 31 targets (lanes 1..31) with one dependent-load chain
     Key my_key = -1;
-    Target my_t;
-    my_t.row = nullptr; my_t.version = nullptr; my_t.flag = nullptr;
-    int my_remote = 0;
+    // what this lane resolved: the row, and what marks a completed push of it - resolve_fast sets at most one of the
+    // version counter (owned row) and the dirty byte (replica), so one pointer + a kind bit hold it (frees registers)
+    float* my_row = nullptr;
+    void* my_mark = nullptr;
+    int my_bits = 0;                     // bit 0: the row lives on a peer GPU, bit 1: my_mark is a replica dirty byte,
+                                         // bits 2..: the key's accumulator row (deterministic mode)
     if (lane == 0) my_key = ckey;
     else if (lane - 1 < n_targets) my_key = (lane == 1) ? pos_key : negatives[(size_t)p * neg + (lane - 2)];
     if (my_key >= 0) {
       unsigned r0 = n_remote;
-      my_t = dev::resolve_fast(c, my_key, 0, &n_local, &n_remote);
-      my_remote = (n_remote != r0) ? 1 : 0;
+      const Target tg = dev::resolve_fast(c, my_key, 0, &n_local, &n_remote);
+      my_row = tg.row;
+      my_mark = tg.flag ? (void*)tg.flag : (void*)tg.version;
+      my_bits = ((n_remote != r0) ? 1 : 0) | (tg.flag ? 2 : 0) | (FX ? __ldg(fx_cidx + my_key) << 2 : 0);
     }
     // target t (0-based) -> lane t+1 (only pairs with <= 31 targets use this kernel)
     auto issue = [&](int t) {
       const int b = issued % RING;
       float* buf = ring + (size_t)b * buf_floats;
       const Key tkey = (Key)__shfl_sync(0xffffffffu, (unsigned long long)my_key, t + 1);
-      float* row = (float*)__shfl_sync(0xffffffffu, (unsigned long long)my_t.row, t + 1);
-      const int remote = __shfl_sync(0xffffffffu, my_remote, t + 1);
+      float* row = (float*)__shfl_sync(0xffffffffu, (unsigned long long)my_row, t + 1);
+      const int remote = __shfl_sync(0xffffffffu, my_bits, t + 1) & 1;
       const bool skip = (t > 0 && tkey == pos_key) || row == nullptr;
       if (skip) {
         if (lane == 0) mbar_arrive(&bars[b]);            // nothing to load: complete the phase
@@ -158,7 +190,7 @@ sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ cent
     };
 
     // ---- center row (registers)
-    float* c_row = (float*)__shfl_sync(0xffffffffu, (unsigned long long)my_t.row, 0);
+    float* c_row = (float*)__shfl_sync(0xffffffffu, (unsigned long long)my_row, 0);
     const bool c_slow = (c_row == nullptr);
     float4 e0[VPL], g0[VPL];
     // prefetch the first RING (BULK: RING - 1) targets before touching the center row
@@ -197,7 +229,9 @@ sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ cent
       const int b = consumed % RING;
       float* buf = ring + (size_t)b * buf_floats;
       const Key tkey = (Key)__shfl_sync(0xffffffffu, (unsigned long long)my_key, t + 1);
-      float* t_row = (float*)__shfl_sync(0xffffffffu, (unsigned long long)my_t.row, t + 1);
+      float* t_row = (float*)__shfl_sync(0xffffffffu, (unsigned long long)my_row, t + 1);
+      // (shuffled here, with the whole warp converged: the update loop below runs on a subset of the lanes)
+      long long* fx_t = FX ? fx_acc + (size_t)(__shfl_sync(0xffffffffu, my_bits, t + 1) >> 2) * (2 * d) : nullptr;
       mbar_wait(&bars[b], (consumed / RING) & 1u);
       ++consumed;
       const float label = (t == 0) ? 1.f : 0.f;
@@ -252,7 +286,10 @@ sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ cent
             ue.y = alpha * gr.y * rsqrtf(a1.y + ua.y);
             ue.z = alpha * gr.z * rsqrtf(a1.z + ua.z);
             ue.w = alpha * gr.w * rsqrtf(a1.w + ua.w);
-            if (BULK) {                   // stage the update in place of the consumed row
+            if (FX) {                     // deterministic mode: fixed-point sums, applied after the step
+              fx_add4(fx_t, j, nvec, ue, kFxEmb);
+              fx_add4(fx_t + d, j, nvec, ua, kFxAda);
+            } else if (BULK) {            // stage the update in place of the consumed row
               reinterpret_cast<float4*>(buf)[j] = ue;
               reinterpret_cast<float4*>(buf + d)[j] = ua;
             } else {
@@ -261,14 +298,14 @@ sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ cent
             }
           }
         }
-        if (BULK) {
+        if (BULK && !FX) {
           __syncwarp();
           if (lane == 0) {
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the staged update is visible to the TMA engine
             bulk_red_s2g(t_row, buf, row_bytes);
           }
         }
-        if (lane == t + 1) dev::mark_pushed(my_t);
+        if (lane == t + 1) mark_pushed(my_mark, my_bits);
         ++n_upd;
       }
       // exactly one bulk group per target (empty for skipped / generic-path targets): "all but the youngest group"
@@ -313,6 +350,7 @@ sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ cent
         if (dev::slow_push(c, ckey, stage)) ++n_upd;
       }
     } else {
+      long long* fx_c = FX ? fx_acc + (size_t)(__shfl_sync(0xffffffffu, my_bits, 0) >> 2) * (2 * d) : nullptr;
 #pragma unroll
       for (int v = 0; v < VPL; ++v) {
         int j = lane + v * 32;
@@ -324,7 +362,10 @@ sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ cent
           ue.y = alpha * g0[v].y * rsqrtf(a0.y + ua.y);
           ue.z = alpha * g0[v].z * rsqrtf(a0.z + ua.z);
           ue.w = alpha * g0[v].w * rsqrtf(a0.w + ua.w);
-          if (BULK) {
+          if (FX) {
+            fx_add4(fx_c, j, nvec, ue, kFxEmb);
+            fx_add4(fx_c + d, j, nvec, ua, kFxAda);
+          } else if (BULK) {
             reinterpret_cast<float4*>(scratch)[j] = ue;
             reinterpret_cast<float4*>(scratch + d)[j] = ua;
           } else {
@@ -333,7 +374,7 @@ sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ cent
           }
         }
       }
-      if (BULK) {
+      if (BULK && !FX) {
         __syncwarp();
         if (lane == 0) {
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -341,7 +382,7 @@ sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ cent
           bulk_commit();
         }
       }
-      if (lane == 0) dev::mark_pushed(my_t);
+      if (lane == 0) mark_pushed(my_mark, my_bits);
       ++n_upd;
     }
     __syncwarp();
@@ -349,7 +390,8 @@ sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ cent
   if (BULK) { if (lane == 0) bulk_wait_all(); __syncwarp(); }   // every bulk reduction has been performed before the CTA leaves
 
   __syncwarp();
-  if (lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
+  if (FX && lane == 0) atomicAdd(fx_loss, (unsigned long long)__float2ll_rn(loss_acc * kFxLoss));
+  else if (lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
   unsigned sum_local = n_local, sum_remote = n_remote;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -365,6 +407,85 @@ sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ cent
   dev::cta_exit(c);
 }
 
+template <int VPL, int MAXREG, bool BULK>
+__global__ void __maxnreg__(MAXREG)
+sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
+                     const Key* __restrict__ negatives, int n_pairs, int neg, int d, float alpha,
+                     float* __restrict__ loss_out, unsigned long long* __restrict__ stats, int tma_remote) {
+  sgns_step_tma_body<VPL, BULK, false>(c, centers, contexts, negatives, n_pairs, neg, d, alpha, loss_out, stats,
+                                       tma_remote, nullptr, nullptr, nullptr);
+}
+
+template <int VPL>
+__global__ void __maxnreg__(128)
+sgns_step_tma_fx_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
+                        const Key* __restrict__ negatives, int n_pairs, int neg, int d, float alpha,
+                        unsigned long long* __restrict__ stats, long long* __restrict__ fx_acc,
+                        const int* __restrict__ fx_cidx, unsigned long long* __restrict__ fx_loss) {
+  sgns_step_tma_body<VPL, false, true>(c, centers, contexts, negatives, n_pairs, neg, d, alpha, nullptr, stats, 1,
+                                       fx_acc, fx_cidx, fx_loss);
+}
+
+// key of update source i of a step: centers [0, B), contexts [B, 2B), negatives [2B, 2B + B * neg)
+__device__ __forceinline__ Key fx_key(const Key* centers, const Key* contexts, const Key* negatives, int n_pairs, long i) {
+  if (i < n_pairs) return centers[i];
+  if (i < 2L * n_pairs) return contexts[i - n_pairs];
+  return negatives[i - 2L * n_pairs];
+}
+
+// Gives every key touched by the step a compact accumulator row (which row a key gets may vary from run to run;
+// what is summed into it does not).
+__global__ void sgns_fx_index_kernel(const Key* __restrict__ centers, const Key* __restrict__ contexts,
+                                     const Key* __restrict__ negatives, int n_pairs, int neg, int* __restrict__ cidx,
+                                     Key* __restrict__ keys, unsigned int* __restrict__ count) {
+  const long n = (long)n_pairs * (neg + 2);
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const Key k = fx_key(centers, contexts, negatives, n_pairs, i);
+    if (k >= 0 && atomicCAS(cidx + k, -1, -2) == -1) {
+      const unsigned r = atomicAdd(count, 1u);
+      keys[r] = k;
+      cidx[k] = (int)r;
+    }
+  }
+}
+
+// One warp per accumulator row: adds its fixed-point sums to the key's store row (one writer per row), clears the
+// row and the key's index; thread 0 moves the step's fixed-point loss into loss_out.
+__global__ void sgns_fx_apply_kernel(const __grid_constant__ Ctx c, int d, const Key* __restrict__ keys,
+                                     const unsigned int* __restrict__ count, int* __restrict__ cidx,
+                                     long long* __restrict__ fx_acc, unsigned long long* __restrict__ fx_loss,
+                                     float* __restrict__ loss_out) {
+  dev::cta_enter(c);
+  const int lane = threadIdx.x & 31;
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    const long long v = (long long)*fx_loss;
+    *fx_loss = 0ull;
+    if (loss_out) *loss_out += (float)((double)v / (double)kFxLoss);
+  }
+  const unsigned n = *count;
+  const int nvec = d >> 2;
+  const unsigned nwarps = (gridDim.x * blockDim.x) >> 5;
+  for (unsigned r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n; r += nwarps) {
+    const Key k = keys[r];
+    const int32_t slot = __ldcg(slot_of(c, c.rank) + k);
+    long long* a = fx_acc + (size_t)r * (2 * d);
+    float* row = slot >= 0 ? row_ptr<float>(c, c.rank, 0, (uint32_t)slot) : nullptr;
+    for (int h = 0; h < 2; ++h) {
+      const double inv = 1.0 / (double)(h ? kFxAda : kFxEmb);
+      for (int i = lane; i < d; i += 32) {
+        const long long v = a[h * d + i];
+        if (v) {
+          const int e = 4 * (i % nvec) + i / nvec;
+          if (row) row[h * d + e] += (float)((double)v * inv);
+          a[h * d + i] = 0;
+        }
+      }
+    }
+    if (lane == 0) cidx[k] = -1;
+  }
+  dev::cta_exit(c);
+}
+
 }  // namespace
 
 // Returns false if this variant does not support the shape (the caller falls back to the LDG kernel).
@@ -374,11 +495,8 @@ bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   const Ctx& c = be.ctx();
   const int vpl = (d / 4 + 31) / 32;
   const size_t buf_floats = ((size_t)2 * d + 31) & ~(size_t)31;
-  // Block shape: 256 threads x 2 blocks = 16 warps per SM. Measured alternatives at the headline config (1 GPU,
-  // profiles/README.md): 192 threads x 3 blocks = 18 warps per SM at 112 / 104 registers: -7 % / -8 % (the registers
-  // cost more than the warps bring); L2 prefetch of the next pair's keys and of the center's AdaGrad half: +-0.2 %.
-  // ncu at this config: DRAM 4.54 TB/s = 69 % of the measured copy bandwidth with random 2400-byte rows - the
-  // kernel is at the memory system, not at an issue or occupancy limit.
+  // Block shape: 256 threads x 2 blocks = 16 warps per SM (two blocks of 128 registers fill the register file; the
+  // ring of 5 row buffers per warp keeps enough 2400-byte rows in flight to be memory-bound).
   const int threads = kThreads;
   const int warps = threads / 32;
   const size_t smem = (size_t)warps * (RING + 1) * buf_floats * sizeof(float) + 128;
@@ -393,6 +511,23 @@ bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   // target t+1 during the update of target t - was measured too: no gain at 128 registers, -5 % at 104: the kernel is
   // not bound by the per-warp dependency chain.)
   static const bool bulk = [] { const char* e = getenv("ADAPM_SGNS_BULKRED"); return !e || atoi(e) != 0; }();
+  // One GPU: deterministic step (fixed-point accumulation + apply pass), so that the same inputs give the same rows
+  // and loss in every run; ADAPM_SGNS_DETERMINISTIC=0 selects in-place (Hogwild) updates. Several GPUs: rows move
+  // between ranks during the step and are updated in place.
+  static const bool det_env = [] { const char* e = getenv("ADAPM_SGNS_DETERMINISTIC"); return !e || atoi(e) != 0; }();
+  const long n_src = (long)n_pairs * (neg + 2);
+  ADAPM_CHECK(n_src < (1L << 29), "sgns_step: too many keys in one step");   // (row index << 2 fits an int)
+  CudaBackend::FxScratch* fx =
+      det_env && c.L.world == 1 ? &be.fx_scratch((size_t)std::min<long>(n_src, c.L.num_keys), 2 * d) : nullptr;
+  long long* fx_acc = fx ? fx->acc : nullptr;
+  const int* fx_cidx = fx ? fx->cidx : nullptr;
+  unsigned long long* fx_loss = fx ? fx->loss : nullptr;
+  if (fx) {
+    ADAPM_CUDA_CHECK(cudaMemsetAsync(fx->count, 0, sizeof(unsigned int), stream));
+    sgns_fx_index_kernel<<<(int)std::min<long>((n_src + 255) / 256, be.num_sms() * 8L), 256, 0, stream>>>(
+        centers, contexts, negatives, n_pairs, neg, fx->cidx, fx->keys, fx->count);
+    ADAPM_COUNT_LAUNCH();
+  }
 #define ADAPM_LAUNCH_TMA3(V, T, B)                                                                              \
   do {                                                                                                          \
     static bool attr_set = false;                                                                               \
@@ -410,13 +545,37 @@ bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, con
     else if (lean) ADAPM_LAUNCH_TMA3(V, 104, false);                     \
     else ADAPM_LAUNCH_TMA3(V, 128, false);                               \
   } while (0)
-  switch (vpl) {
-    case 1: ADAPM_LAUNCH_TMA(1); break;
-    case 2: ADAPM_LAUNCH_TMA(2); break;
-    default: ADAPM_LAUNCH_TMA(3); break;
+#define ADAPM_LAUNCH_TMA_FX(V)                                                                                  \
+  do {                                                                                                          \
+    static bool attr_set = false;                                                                               \
+    if (!attr_set) {                                                                                            \
+      cudaFuncSetAttribute(sgns_step_tma_fx_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024); \
+      attr_set = true;                                                                                          \
+    }                                                                                                           \
+    sgns_step_tma_fx_kernel<V><<<blocks, threads, smem, stream>>>(c, centers, contexts, negatives, n_pairs, neg, d, \
+                                                                  alpha, stats, fx_acc, fx_cidx, fx_loss);      \
+  } while (0)
+  if (fx) {
+    switch (vpl) {
+      case 1: ADAPM_LAUNCH_TMA_FX(1); break;
+      case 2: ADAPM_LAUNCH_TMA_FX(2); break;
+      default: ADAPM_LAUNCH_TMA_FX(3); break;
+    }
+  } else {
+    switch (vpl) {
+      case 1: ADAPM_LAUNCH_TMA(1); break;
+      case 2: ADAPM_LAUNCH_TMA(2); break;
+      default: ADAPM_LAUNCH_TMA(3); break;
+    }
   }
   ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cudaGetLastError());
+  if (fx) {
+    sgns_fx_apply_kernel<<<(int)std::min<long>((n_src + 7) / 8, be.num_sms() * 16L), 256, 0, stream>>>(
+        c, d, fx->keys, fx->count, fx->cidx, fx->acc, fx->loss, loss_out);
+    ADAPM_COUNT_LAUNCH();
+    ADAPM_CUDA_CHECK(cudaGetLastError());
+  }
   return true;
 }
 

@@ -8,7 +8,7 @@ DMLC_ROLE / DMLC_RANK / DMLC_PS_ROOT_URI / DMLC_PS_ROOT_PORT`` for scripts that 
 scheduler process: ranks rendezvous through a POSIX-shm control block. A rank that exits with
 code 254 is restarted (``keepalive`` of tracker/dmlc_local.py:15-26). ``torchrun`` and ``mpirun``
 work too - the package also reads ``OMPI_COMM_WORLD_*``, ``PMI_*`` and ``SLURM_*``.
-The fabric is single-node (shm control block + peer-mapped heaps over NVLink/NVSwitch): one 8xB200 box is the target.
+The fabric is single-node (shm control block + peer-mapped heaps over NVLink/NVSwitch): one 8-GPU NVSwitch box is the target.
 """
 from __future__ import annotations
 

@@ -10,7 +10,7 @@ reference's PyTorch bindings would:
   fused gather kernel, NVLink loads for remote rows), DeepFM forward/backward in PyTorch, worker-side
   AdaGrad, ``push`` the additive updates (device path: REDs into the owners' rows);
 * the dense MLP is replicated; its gradients are all-reduced with ``torch.distributed`` when available.
-  On a CUDA server the MLP's linear layers can run on the hand-written tcgen05 GEMM
+  On a CUDA server the MLP's linear layers can run on the hand-written wgmma GEMM
   (``ops.gemm_nt_bf16``; ``precision='fp8'`` uses the e4m3 tensor-core path with per-tensor scales).
 """
 from __future__ import annotations
@@ -49,7 +49,7 @@ class DeepFMConfig:
 
 
 class TensorCoreLinear(torch.autograd.Function):
-    """y = x @ W^T on the hand-written tcgen05 GEMM (bf16 or fp8 operands, fp32 accumulate)."""
+    """y = x @ W^T on the hand-written wgmma GEMM (bf16 or fp8 operands, fp32 accumulate)."""
 
     @staticmethod
     def forward(ctx, x, w, precision):

@@ -286,7 +286,7 @@ class KGE:
         out = {k: [] for k in ("rank_s", "rank_r", "rank_o", "rank_s_raw", "rank_o_raw")}
 
         def count_better(q, cand, true_score, true_idx):
-            if tc:   # tcgen05 GEMM with the rank-count epilogue: the [B, candidates] scores never reach HBM
+            if tc:   # wgmma GEMM with the rank-count epilogue: the [B, candidates] scores never reach HBM
                 return gemm_nt_rank_count(q, cand, true_score, true_idx).long() + 1
             scores = q @ cand.t()
             scores.scatter_(1, true_idx.view(-1, 1), float("-inf"))
@@ -401,8 +401,8 @@ def complex_query(a: torch.Tensor, r: torch.Tensor, conj: bool) -> torch.Tensor:
 
 
 def score_all(q: torch.Tensor, E: torch.Tensor, server=None) -> torch.Tensor:
-    """1-vs-all scores [B, ne] = q @ E^T. With a CUDA server the hand-written tcgen05 GEMM is used
-    (bf16 operands, fp32 accumulation in TMEM); otherwise a plain fp32 matmul."""
+    """1-vs-all scores [B, ne] = q @ E^T. With a CUDA server the hand-written wgmma GEMM is used
+    (bf16 operands, fp32 accumulation in registers); otherwise a plain fp32 matmul."""
     if server is not None:
         from ..ops import gemm_nt_bf16
 
@@ -471,7 +471,7 @@ def kge_reference_step(kv, S, R, O, L, cfg: KGEConfig, masks=None) -> float:
 def evaluate_fused(model: "KGE", triples: torch.Tensor, known: torch.Tensor, batch: int = 2048) -> dict:
     """Filtered ranking without ever pulling the model: per batch only the rows of the queries, of the true
     answers and of the known answers are pulled (device Pull); the 1-vs-all scoring against ALL entities runs in
-    the fused gather + tcgen05 GEMM + rank-count kernel (``ops.gather_gemm_rank_count``), which reads the entity
+    the fused gather + wgmma GEMM + rank-count kernel (``ops.gather_gemm_rank_count``), which reads the entity
     rows from whichever GPU's HBM holds them. Works on any number of GPUs; every rank may evaluate its own share
     of the test triples concurrently."""
     from ..ops import gather_gemm_rank_count

@@ -14,7 +14,7 @@ Behavioural parity with the reference application ``apps/word2vec.cc``:
 * checkpoint: ``"<vocab> <dim>\\n"`` then per word ``"<word> "`` + ``dim`` raw float32 + ``"\\n"``
   (word2vec.cc:367-416).
 
-B200-first differences: the per-pair loop of the reference is one batched kernel
+GPU-first differences: the per-pair loop of the reference is one batched kernel
 (``ops.sgns_step``) that fuses pull, scoring, AdaGrad and push over local HBM / NVLink peers.
 """
 from __future__ import annotations

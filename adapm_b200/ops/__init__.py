@@ -1,4 +1,4 @@
-"""Torch-facing wrappers of the hand-written sm_100a kernels (csrc/cuda/ops_*.cu).
+"""Torch-facing wrappers of the hand-written sm_90a kernels (csrc/cuda/ops_*.cu).
 
 All ops take CUDA tensors, run on the current CUDA stream and operate directly on the
 parameter store of a ``Server`` with ``backend='cuda'`` (local HBM and NVLink-mapped peers).
@@ -51,7 +51,7 @@ class SgnsSharedStep:
     (csrc/cuda/ops_sgns_shared.cu; SURVEY K7's GEMM formulation, an option next to the reference-faithful fused step).
 
     Per step: ONE Pull of the rows ``[centers | contexts | shared negatives]`` through the store (any protocol state,
-    local HBM or NVLink), three tcgen05 GEMMs (scores, center gradient, negative gradient; bf16 operands, fp32
+    local HBM or NVLink), three wgmma GEMMs (scores, center gradient, negative gradient; bf16 operands, fp32
     accumulation) with three elementwise kernels around them, ONE Push of the additive ``[embedding | AdaGrad]`` updates.
     ``B`` pairs x ``Nn`` negatives = B * Nn sample pairs for 2 B + Nn rows of traffic.
     """
@@ -258,7 +258,7 @@ def _bf16_k8(t: torch.Tensor) -> torch.Tensor:
 
 
 def gemm_nt_bf16(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
-    """C[M,N] fp32 = a[M,K] x b[N,K]^T on the 5th-gen tensor cores (hand-written tcgen05/TMEM/TMA kernel,
+    """C[M,N] fp32 = a[M,K] x b[N,K]^T on the Hopper tensor cores (hand-written wgmma/TMA kernel,
     bf16 operands, fp32 accumulation)."""
     if not (a.is_cuda and b.is_cuda and a.dim() == 2 and b.dim() == 2 and a.shape[1] == b.shape[1]):
         raise ValueError("gemm_nt_bf16 expects CUDA matrices a[M,K], b[N,K]")
@@ -270,7 +270,7 @@ def gemm_nt_bf16(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
 
 
 def gemm_nt_fp8(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
-    """C = a @ b^T with e4m3 operands on the fp8 tensor-core path (tcgen05.mma kind::f8f6f4), per-tensor scales
+    """C = a @ b^T with e4m3 operands on the fp8 tensor-core path (wgmma e4m3), per-tensor scales
     chosen from the absolute maxima, fp32 accumulation; the scale product is applied in the epilogue."""
     if not (a.is_cuda and b.is_cuda and a.shape[1] == b.shape[1]):
         raise ValueError("gemm_nt_fp8 expects CUDA matrices a[M,K], b[N,K]")
@@ -290,7 +290,7 @@ def gemm_nt_fp8(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
 
 def gemm_nt_rank_count(q: torch.Tensor, e: torch.Tensor, true_score: torch.Tensor, true_col: torch.Tensor) -> torch.Tensor:
     """counts[i] = #{j != true_col[i] : <q[i], e[j]> > true_score[i]} without materialising the score matrix
-    (rank-count epilogue of the tcgen05 GEMM)."""
+    (rank-count epilogue of the wgmma GEMM)."""
     q16, e16 = _bf16_k8(q), _bf16_k8(e)
     M, N, K = q16.shape[0], e16.shape[0], q16.shape[1]
     ts = true_score.to(torch.float32).contiguous()
@@ -304,7 +304,7 @@ def gemm_nt_rank_count(q: torch.Tensor, e: torch.Tensor, true_score: torch.Tenso
 def gather_gemm(server, q: torch.Tensor, keys: torch.Tensor, k: int, stats: Optional[torch.Tensor] = None) -> torch.Tensor:
     """scores[M, N] = q[M, k] @ E^T where row n of E is the first ``k`` values of store row ``keys[n]`` - the rows
     are gathered inside the GEMM kernel from the local slab, local replicas or peer GPUs over NVLink (fused
-    gather + tcgen05 GEMM); the gathered matrix never exists in HBM."""
+    gather + wgmma GEMM); the gathered matrix never exists in HBM."""
     _i64(keys, "keys")
     q16 = _bf16_k8(q)
     M, N = q16.shape[0], keys.numel()

@@ -1,12 +1,12 @@
 """Block-scaled fp8 (MX-style) codec for embedding rows: e4m3 values with one UE8M0 (power-of-two, 8-bit exponent) scale
-per block of 32 values - the operand format of Blackwell's `tcgen05.mma ... kind::mxf8f6f4.block_scale` and the storage
+per block of 32 values - the OCP microscaling (MX) fp8 layout and the storage
 format BASELINE config #5 asks for (1 byte per value + 1 byte per 32 values = 1.03 B instead of 4 B).
 
 This module is the *format definition* and its numerics (quantise / dequantise / fake-quantise, error bounds), in plain
 PyTorch so that it runs on any backend. `models/deepfm.py` uses it for `table_precision="fp8_block"`: the model trains on
 the values an fp8 table would deliver while the parameter manager keeps fp32 master rows (delta accumulation and AdaGrad
 stay fp32, the "requantise at sync" scheme); a table that actually STORES one byte per value needs a 1-byte row type in
-the store and is not implemented (ROADMAP "Config #5")."""
+the store and is not implemented."""
 from __future__ import annotations
 
 import torch

@@ -3,8 +3,8 @@
 Capability parity with the reference's (unused) ``include/ps/internal/parallel_sort.h:23-55``,
 ``parallel_kv_match.h:29-120`` and ``assign_op.h:12-68``: sort a key array, and for two ascending key lists
 combine the values of the keys present in both (``dst[k] op= src[k]``). The reference forks threads recursively;
-here both are data-parallel tensor programs that run on whichever device the tensors live on (a B200 sorts
-and matches hundreds of millions of keys per second, so there is nothing to hand-thread).
+here both are data-parallel tensor programs that run on whichever device the tensors live on (a GPU sorts
+and matches keys far faster than hand-threaded host code).
 """
 from __future__ import annotations
 

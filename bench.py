@@ -59,11 +59,15 @@ def parse_args():
                     help="experimental: device-side Intent for keys that are already local (ops.IntentPrepass)")
     ap.add_argument("--opt", action="append", default=[], metavar="KEY=VALUE",
                     help="extra server option (e.g. --opt sys.sync.idle_period=1); repeatable")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy: its loss and "
+                         "the rows of a fixed, seeded sample of keys (rank 0; word2vec only). On one GPU the same "
+                         "arguments give the same inputs and the same outputs in every run")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """Samples SM clocks / throttle reasons with nvidia-smi DURING the timed region (B200_PROFILING.md)."""
+    """Samples SM clocks / throttle reasons with nvidia-smi DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -115,8 +119,32 @@ def reference_arm(args):
     return 0
 
 
+def dump_outputs(out_dir, model, worker, last_batch, cfg, rank):
+    """What the last timed step computed, as a caller of the step sees it: the step's summed logistic loss and the
+    [embedding | AdaGrad] rows of 2048 keys of that step's batch plus 2048 keys of the whole table (fixed seed)."""
+    import numpy as np
+    import torch
+
+    loss = float(model.loss.item())
+    g = torch.Generator().manual_seed(0)
+    batch_keys = torch.unique(last_batch.view(-1).cpu())
+    keys = torch.cat([batch_keys[torch.randperm(batch_keys.numel(), generator=g)[:2048]],
+                      torch.randint(0, cfg.num_keys, (2048,), generator=g)])
+    keys = torch.unique(keys)
+    rows = torch.empty(keys.numel(), cfg.row_len, dtype=torch.float32)
+    worker.pull(keys, rows)
+    if rank != 0:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([loss], dtype=np.float64))
+    np.save(os.path.join(out_dir, "row_keys.npy"), keys.numpy().astype(np.float64))
+    np.save(os.path.join(out_dir, "rows.npy"), rows.numpy())
+
+
 def main():
     args = parse_args()
+    if args.dump_outputs and (args.impl != "native" or args.config != "word2vec"):
+        sys.exit("--dump-outputs is implemented for the native word2vec run")
     if args.impl == "reference":
         return reference_arm(args)
 
@@ -281,6 +309,8 @@ def main():
     counters1 = server.counters()
     stats1 = model.stats.tolist()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, model, worker, batches[P + W + 2 * K + 2], cfg, rank)
     if rank == 0 and sampler.p is None:
         clocks = {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["clock sampling disabled (ADAPM_BENCH_NO_SMI)"]}
 
@@ -400,7 +430,7 @@ def main():
             hbm = peaks["hbm_gbs"]
             denom = "measured"
         except Exception:
-            hbm, denom = 6650.0, "fallback"
+            hbm, denom = 3350.0, "H100 SXM data sheet"
         # same-box anchor: the NCCL-only arm (bench.py --impl nccl, stock PyTorch ops + all_to_all), measured on this pool
         # and recorded in baseline/nccl_arm.json by N (BASELINE.md section 6); the reference itself cannot be built
         vs_baseline, anchor = None, None
@@ -418,7 +448,7 @@ def main():
         nv_step = (2 * dstat[1] * row_bytes                                             # fused step: remote row load + reduction
                    + (dcnt.get("refreshes", 0) + dcnt.get("relocations", 0)) * row_bytes  # round: owner row reads
                    + dcnt.get("deltas_shipped", 0) * row_bytes) / n_steps_win            # round: replica deltas (reductions)
-        link_gbs = 770.0   # measured peer copy, one direction, per GPU (B200_PROFILING.md)
+        link_gbs = 450.0   # NVLink 4 data-sheet rate, one direction, per H100 SXM (not a measured copy rate)
         nv_time_ms = nv_step / (link_gbs * 1e9) * 1e3
         hbm_time_ms = cfg.batch_pairs * cfg.updates_per_pair * bytes_per_update / (hbm * 1e9) * 1e3
         out = {
@@ -454,7 +484,7 @@ def main():
                          "roofline_ms_per_step": max(nv_time_ms, hbm_time_ms),
                          "fraction_of_roofline": max(nv_time_ms, hbm_time_ms) / (dev_ms / K),
                          "note": "roofline = slower of (algorithmic HBM bytes / measured copy bandwidth) and (bytes that "
-                                 "crossed NVLink / 770 GB/s measured peer copy); rank 0's counters over both timed loops"},
+                                 "crossed NVLink / 450 GB/s data-sheet rate); rank 0's counters over both timed loops"},
             "locality": {"rows_local": dstat[0], "rows_remote": dstat[1], "rows_slow_path": dstat[2]},
             "pm": {k: dcnt.get(k, 0) for k in ("relocations", "replica_setups", "replica_drops", "refreshes",
                                                 "deltas_shipped", "sync_rounds", "protocol_errors")},

@@ -296,7 +296,7 @@ def run_ctr(ctx: Ctx):
         upd_step = ctx.world * float(model.rows_pushed) / max(1, model.step_no)
         out = _line(ctx, "CTR DeepFM sparse updates/sec (device-timed, max over ranks)",
                     f"DeepFM, {cfg.num_features} feature keys x {cfg.row_len} fp32 (emb 16 + AdaGrad), 26 fields, MLP 400x3 "
-                    f"(dense GEMMs: tcgen05 {cfg.precision})",
+                    f"(dense GEMMs: wgmma {cfg.precision})",
                     {"batch_examples_per_gpu": cfg.batch_size, "global_batch": ctx.world * cfg.batch_size, "intent_read_ahead": RA,
                      "placement_steps": P, "examples_per_s": ctx.world * cfg.batch_size * K / (t["dev_ms"] * 1e-3),
                      "updates_per_step": "distinct feature rows of the batch (mean over the run)"},

@@ -1,6 +1,6 @@
 // Probe: does this box support NVLS multicast objects (cuMulticastCreate) between 2+ GPUs, and do multimem.st /
 // multimem.ld_reduce / multimem.red work on them? Single process, one context per device.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -o mc_probe mc_probe.cu -lcuda
+//   nvcc -gencode arch=compute_90a,code=sm_90a -o mc_probe mc_probe.cu -lcuda
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstdio>

@@ -11,7 +11,7 @@ os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on an H100)")
     config.addinivalue_line("markers", "slow: long-running stress variant")
 
 

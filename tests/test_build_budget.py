@@ -20,7 +20,7 @@ def _kernels():
         _build.build()
         logs = glob.glob(os.path.join(LOGS, "*.cu.o.log"))
     out = {}
-    pat = re.compile(r"Compiling entry function '([^']+)' for 'sm_100a'\n(?:ptxas info\s*:\s*Function properties[^\n]*\n"
+    pat = re.compile(r"Compiling entry function '([^']+)' for 'sm_90a'\n(?:ptxas info\s*:\s*Function properties[^\n]*\n"
                      r"\s*(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n)?"
                      r"ptxas info\s*:\s*Used (\d+) registers")
     for f in logs:
@@ -56,13 +56,13 @@ def test_hot_kernels_stay_within_their_register_budget():
     assert k["phase_row_tma_kernel"]["regs"] * 64 <= room, k["phase_row_tma_kernel"]
     # tensor-core kernels: no spills, enough room for 1 CTA/SM with large smem tiles
     for name, v in k.items():
-        if name.startswith(("gemm_nt_tcgen05", "gather_gemm_kernel")):
+        if name.startswith(("gemm_nt_wgmma", "gather_gemm_kernel")):
             assert v["spill"] == 0, (name, v)
 
 
-def test_blackwell_instructions_are_in_the_built_extension():
-    """SASS / PTX of the in-tree extension (cuobjdump, no GPU needed): the kernels that are documented to use the 5th-gen
-    tensor cores, TMA, clusters and NVLS multimem really contain those instructions - a refactoring that silently drops
+def test_hopper_instructions_are_in_the_built_extension():
+    """SASS / PTX of the in-tree extension (cuobjdump, no GPU needed): the kernels that are documented to use the Hopper
+    tensor cores (wgmma), TMA, mbarriers and NVLS multimem really contain those instructions - a refactoring that silently drops
     one of them (e.g. a fallback path becoming the only path) fails here, not in a benchmark weeks later."""
     import shutil
 
@@ -89,15 +89,14 @@ def test_blackwell_instructions_are_in_the_built_extension():
             out |= h
         return out
 
-    gemm = ops_of("gemm_nt_tcgen05_kernel")
-    assert {"UTCHMMA", "LDTM", "UTMALDG"} <= gemm, sorted(gemm)
-    assert "UTCQMMA" in gemm                                                     # fp8 (kind::f8f6f4) instantiation
-    pair = ops_of("gemm_nt_tcgen05_pair_kernel")
-    assert {"UTCHMMA", "LDTM", "UTMALDG", "UCGABAR_ARV", "UCGABAR_WAIT"} <= pair, sorted(pair)     # cta_group::2 + cluster
-    assert {"UTCHMMA", "LDTM"} <= ops_of("gather_gemm_kernel")
+    gemm = ops_of("gemm_nt_wgmma_kernel")
+    assert {"HGMMA", "UTMALDG", "SYNCS", "WARPGROUP"} <= gemm, sorted(gemm)   # wgmma bf16, TMA ring, mbarriers
+    assert "QGMMA" in gemm                                                       # fp8 (e4m3) instantiation
+    gather = ops_of("gather_gemm_kernel")
+    assert {"HGMMA", "UTMALDG", "SYNCS"} <= gather, sorted(gather)
     sgns = ops_of("sgns_step_tma_kernel")
     assert {"UBLKCP.S", "UBLKRED.G", "SYNCS"} <= sgns, sorted(sgns)              # TMA ring in, TMA bulk reductions out
     assert {"LDGMC.E"} <= ops_of("xbar_kernel")                                   # multimem.ld_reduce (NVLS)
     ptx = subprocess.run(["cuobjdump", "-ptx", so[0]], capture_output=True, text=True).stdout
     assert "multimem.st.release.sys.global" in ptx and "multimem.ld_reduce" in ptx
-    assert "tcgen05.mma.cta_group::2" in ptx and "cp.reduce.async.bulk" in ptx
+    assert "wgmma.mma_async" in ptx and "cp.reduce.async.bulk" in ptx

@@ -1,5 +1,5 @@
 """The CPU contract tests re-run on the CUDA backend: several logical ranks share one GPU
-(inproc fabric), so the full relocation/replication protocol runs through the sm_100a kernels
+(inproc fabric), so the full relocation/replication protocol runs through the sm_90a kernels
 with peer pointers that happen to live on the same device."""
 import pytest
 

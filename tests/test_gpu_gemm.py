@@ -1,4 +1,4 @@
-"""tcgen05/TMEM/TMA GEMM (ops_gemm_tcgen05.cu) against torch.matmul on the same bf16-rounded operands."""
+"""wgmma/TMA GEMM (ops_gemm_wgmma.cu) against torch.matmul on the same bf16-rounded operands."""
 import pytest
 import torch
 
@@ -82,7 +82,7 @@ def test_kge_eval_tensor_core_path_matches_fp32():
 
 @pytest.mark.parametrize("M,N,K", [(128, 128, 128), (300, 500, 416), (64, 1000, 80), (2048, 4096, 256)])
 def test_gemm_nt_fp8_matches_torch(M, N, K):
-    """e4m3 operands on the kind::f8f6f4 tensor-core path vs the same quantised operands multiplied in fp32."""
+    """e4m3 operands on the fp8 wgmma tensor-core path vs the same quantised operands multiplied in fp32."""
     from adapm_b200.ops import gemm_nt_fp8
 
     g = torch.Generator(device="cuda").manual_seed(K)

@@ -1,4 +1,4 @@
-"""Numerics of the hand-written sm_100a kernels against plain PyTorch fp32 references."""
+"""Numerics of the hand-written sm_90a kernels against plain PyTorch fp32 references."""
 import numpy as np
 import pytest
 import torch
@@ -141,6 +141,63 @@ def test_sgns_step_matches_pytorch_reference(cluster1, d, neg, impl):
     assert s[1] == 0 and s[2] == 0 and s[3] == int(valid.sum()) + B
 
 
+@pytest.mark.parametrize("d,neg", [(300, 25), (128, 5), (64, 2)])
+def test_sgns_steps_with_repeated_keys_match_start_of_step_reference(cluster1, d, neg):
+    """Few distinct keys, so every row is updated by many pairs of a step, over several steps: on one GPU every pair
+    reads the state at the start of the step and the step adds all pairs' updates, which the fp64 formula below
+    computes exactly (an accumulator that is not cleared, or an update applied twice, shows up in the next step)."""
+    from adapm_b200.ops import sgns_step
+
+    B, words = 256, 40
+    n_keys = 2 * words
+    server, kv = cluster1(2 * d, n_keys)
+    dev = server.device
+    g = torch.Generator().manual_seed(d + neg)
+    rows = torch.empty(n_keys, 2 * d, dtype=torch.float64)
+    rows[:, :d] = torch.randn(n_keys, d, generator=g, dtype=torch.float64) * 0.3
+    rows[:, d:] = torch.rand(n_keys, d, generator=g, dtype=torch.float64) + 1e-3
+    allk = torch.arange(n_keys)
+    kv.set(allk, rows.float().clone().view(-1))
+    ref = rows.float().double()
+    alpha = 0.05
+    for step in range(3):
+        centers = 2 * torch.randint(0, words, (B,), generator=g)
+        tk = 2 * torch.randint(0, words, (B, neg + 1), generator=g) + 1
+        contexts, negatives = tk[:, 0].clone(), tk[:, 1:].contiguous()
+        loss = torch.zeros(1, device=dev)
+        stats = torch.zeros(4, dtype=torch.int64, device=dev)
+        sgns_step(server, centers.to(dev), contexts.to(dev), negatives.to(dev), d, alpha, loss, stats, impl="tma")
+        torch.cuda.synchronize()
+
+        e0, a0 = ref[centers, :d], ref[centers, d:]
+        e1, a1 = ref[tk][:, :, :d], ref[tk][:, :, d:]
+        label = torch.zeros(B, neg + 1, dtype=torch.float64); label[:, 0] = 1
+        f = (e0.unsqueeze(1) * e1).sum(-1)
+        gr = label - torch.sigmoid(f)
+        gr = torch.where(f > 6, label - 1, gr)
+        gr = torch.where(f < -6, label, gr)
+        valid = torch.ones(B, neg + 1, dtype=torch.bool)
+        valid[:, 1:] = negatives != contexts.view(B, 1)
+        gr = gr * valid
+        grad0 = (gr.unsqueeze(-1) * e1).sum(1)
+        grad1 = gr.unsqueeze(-1) * e0.unsqueeze(1)
+        new = ref.clone()
+        new[:, :d].index_add_(0, centers, alpha * grad0 / torch.sqrt(a0 + grad0 ** 2))
+        new[:, d:].index_add_(0, centers, grad0 ** 2)
+        new[:, :d].index_add_(0, tk.view(-1), (alpha * grad1 / torch.sqrt(a1 + grad1 ** 2)).view(-1, d))
+        new[:, d:].index_add_(0, tk.view(-1), (grad1 ** 2).view(-1, d))
+        ref = new
+        z = torch.where(label > 0.5, f, -f).clamp(-6, 6)
+        ref_loss = (torch.log1p(torch.exp(-z)) * valid).sum()
+        torch.testing.assert_close(loss.cpu()[0].double(), ref_loss, rtol=1e-4, atol=1e-3)
+
+        got = torch.empty(n_keys * 2 * d)
+        kv.pull(allk, got)
+        got = got.view(n_keys, 2 * d).double()
+        torch.testing.assert_close(got, ref, rtol=2e-4, atol=2e-5)
+        ref = got      # the next step starts from the stored float32 state
+
+
 def test_device_sampler_distribution(cluster1):
     from adapm_b200.ops import DeviceSampler
 
@@ -175,6 +232,32 @@ def test_word2vec_training_reduces_loss(cluster1):
         model.step(data.batch(s % 3))
         losses.append(model.loss.item())
     assert losses[-1] < 0.9 * losses[0]
+
+
+def test_word2vec_steps_are_deterministic_on_one_gpu(cluster1):
+    """Zipf batches touch hot rows from many pairs of the same step; on one GPU the step still computes the same rows
+    and losses, bit for bit, in every run."""
+    from adapm_b200.models.word2vec import SyntheticPairs, Word2Vec, Word2VecConfig, zipf_counts
+
+    cfg = Word2VecConfig(vocab_size=5000, embed_dim=64, negative=5, batch_pairs=2048)
+    counts = zipf_counts(cfg.vocab_size)
+    runs = []
+    for _ in range(2):
+        server, kv = cluster1(cfg.row_len, cfg.num_keys)
+        model = Word2Vec(server, kv, cfg, counts)
+        model.init_model()
+        data = SyntheticPairs(cfg, counts, 0)
+        losses = []
+        for s in range(20):
+            model.loss.zero_()
+            model.step(data.batch(s))
+            losses.append(model.loss.item())
+        torch.cuda.synchronize()
+        rows = torch.empty(cfg.num_keys, cfg.row_len)
+        kv.pull(torch.arange(cfg.num_keys), rows)
+        runs.append((losses, rows))
+    assert runs[0][0] == runs[1][0]
+    assert torch.equal(runs[0][1], runs[1][1])
 
 
 def test_native_step_driver_matches_python_loop(cluster1):
@@ -359,7 +442,7 @@ def test_mf_step_matches_pytorch_reference(cluster1, rank):
 
 @pytest.mark.parametrize("d,B,Nn", [(300, 256, 128), (128, 512, 256), (64, 64, 32)])
 def test_sgns_shared_negatives_tensor_core_step(cluster1, d, B, Nn):
-    """Shared-negative SGNS on the tcgen05 GEMMs (ops_sgns_shared.cu) against the fp32 PyTorch reference of the same
+    """Shared-negative SGNS on the wgmma GEMMs (ops_sgns_shared.cu) against the fp32 PyTorch reference of the same
     op: the contractions run with bf16 operands (fp32 accumulation), so gradients agree to bf16 rounding; the AdaGrad
     accumulator update g^2 and the embedding update are compared on the rows after ONE step."""
     from adapm_b200.ops import SgnsSharedStep, sgns_shared_reference_step
