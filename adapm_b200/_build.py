@@ -35,6 +35,7 @@ CXX_SOURCES = [
 CUDA_SOURCES = [
     "cuda/device_mem.cu",
     "cuda/cuda_backend.cu",
+    "cuda/fx_accum.cu",
 ]
 
 

@@ -56,9 +56,13 @@ def main(argv=None) -> int:
     ap.add_argument("--max_N", type=int, default=-1, help="artificial maximum of training triples per worker (fast tests)")
     ap.add_argument("--read_partitioned_dataset", type=int, default=0,
                     help="read train.partitioned.<servers>x<threads>.del: block b of the file is trained by worker b")
+    ap.add_argument("--deterministic", type=int, default=0, choices=[0, 1],
+                    help="one GPU: every call of a batch reads the start-of-batch state, bit-identical runs")
     add_ablation_options(ap)
     add_system_options(ap)
     args = ap.parse_args(strip_dashes(argv if argv is not None else sys.argv[1:]))
+    if args.deterministic and int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        ap.error("--deterministic 1 needs a single GPU (WORLD_SIZE=1): on several GPUs rows move between ranks during a step")
 
     if args.batch_triples <= 0:
         args.batch_triples = min(4096, max(32, args.num_entities // 4))
@@ -67,7 +71,8 @@ def main(argv=None) -> int:
                     gamma_relation=args.gamma_relation, dropout_entity=args.dropout_entity,
                     dropout_relation=args.dropout_relation, batch_triples=args.batch_triples,
                     read_ahead=args.signal_intent_ahead, sampling_scheme=getattr(args, "sampling.scheme") or "local",
-                    signal_initial_relations_intent=bool(args.signal_initial_relations_intent), model_seed=args.model_seed)
+                    signal_initial_relations_intent=bool(args.signal_initial_relations_intent), model_seed=args.model_seed,
+                    deterministic=bool(args.deterministic))
     if args.write_embeddings and not args.model_path:
         os.makedirs(args.write_embeddings, exist_ok=True)
         args.model_path = os.path.join(args.write_embeddings, "")

@@ -50,10 +50,14 @@ def main(argv=None) -> int:
     ap.add_argument("--prevent_full_model_pull", type=int, default=0,
                     help="accepted for parity: losses are accumulated inside the step, the model is never pulled in full")
     ap.add_argument("--write_generated_factors", default="", help="path prefix to write the initial factors to")
+    ap.add_argument("--deterministic", type=int, default=0, choices=[0, 1],
+                    help="one GPU: every non-zero of a batch reads the start-of-batch state, bit-identical runs")
     add_ablation_options(ap)
     add_system_options(ap)
     args = ap.parse_args(strip_dashes(argv if argv is not None else sys.argv[1:]))
     world = int(__import__("os").environ.get("WORLD_SIZE", "1"))
+    if args.deterministic and world > 1:
+        ap.error("--deterministic 1 needs a single GPU (WORLD_SIZE=1): on several GPUs rows move between ranks during a step")
     rank = int(__import__("os").environ.get("RANK", "0"))
     test = None
     if args.dataset:
@@ -75,7 +79,7 @@ def main(argv=None) -> int:
                    batch_nnz=args.batch_nnz, signal_intent_cols=args.signal_intent_cols, bold_driver=bool(args.bold_driver),
                    model_seed=args.model_seed, eps_inc=args.increase_step_factor, eps_dec=args.decrease_step_factor,
                    signal_intent_rows=bool(args.signal_intent_rows), wor_blocks=bool(args.wor_blocks),
-                   wor_points=bool(args.wor_points), early_stop=args.early_stop)
+                   wor_points=bool(args.wor_points), early_stop=args.early_stop, deterministic=bool(args.deterministic))
     ad.setup(cfg.num_keys(world), 1)   # one worker per rank: the per-thread loops of the reference are batched kernels here
     server = ad.Server(cfg.row_len, backend=args.backend, options=system_options(args),
                        dtype={"float": "float32", "double": "float64"}[args.value_type])

@@ -596,25 +596,43 @@ CudaBackend::CudaBackend(const Options& opt, const Layout& L, std::shared_ptr<Fa
   dev_timeout_ns_ = (unsigned long long)(std::min(opt.wait_timeout_s, 20.0) * 1e9);
 }
 
-CudaBackend::FxScratch& CudaBackend::fx_scratch(size_t rows, int row_len) {
+CudaBackend::FxScratch& CudaBackend::fx_scratch(size_t acc_len, size_t rows, size_t calls) {
   use_device();
   if (!fx_.cidx) {
     const size_t nk = (size_t)ctx_.L.num_keys;
     ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.cidx, nk * sizeof(int)));
     ADAPM_CUDA_CHECK(cudaMemset(fx_.cidx, 0xff, nk * sizeof(int)));
-    ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.count, sizeof(unsigned int)));
+    ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.count, 2 * sizeof(unsigned int)));
     ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.loss, sizeof(unsigned long long)));
     ADAPM_CUDA_CHECK(cudaMemset(fx_.loss, 0, sizeof(unsigned long long)));
   }
-  if (rows > fx_.rows || row_len != fx_.row_len) {
-    if (fx_.acc) { ADAPM_CUDA_CHECK(cudaFree(fx_.acc)); ADAPM_CUDA_CHECK(cudaFree(fx_.keys)); }
-    ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.acc, rows * row_len * sizeof(long long)));
-    ADAPM_CUDA_CHECK(cudaMemset(fx_.acc, 0, rows * row_len * sizeof(long long)));
+  // (the regions are all zero between steps, so a larger buffer replaces the old one without a copy)
+  if (acc_len > fx_.acc_len) {
+    if (fx_.acc) ADAPM_CUDA_CHECK(cudaFree(fx_.acc));
+    ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.acc, acc_len * sizeof(long long)));
+    ADAPM_CUDA_CHECK(cudaMemset(fx_.acc, 0, acc_len * sizeof(long long)));
+    fx_.acc_len = acc_len;
+  }
+  if (rows > fx_.rows_cap) {
+    if (fx_.keys) { ADAPM_CUDA_CHECK(cudaFree(fx_.keys)); ADAPM_CUDA_CHECK(cudaFree(fx_.rows)); }
     ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.keys, rows * sizeof(Key)));
-    fx_.rows = rows;
-    fx_.row_len = row_len;
+    ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.rows, rows * sizeof(int2)));
+    fx_.rows_cap = rows;
+  }
+  if (calls > fx_.calls_cap) {
+    if (fx_.call_loss) ADAPM_CUDA_CHECK(cudaFree(fx_.call_loss));
+    ADAPM_CUDA_CHECK(cudaMalloc((void**)&fx_.call_loss, calls * sizeof(float)));
+    fx_.calls_cap = calls;
   }
   return fx_;
+}
+
+size_t CudaBackend::keys_with_len(uint32_t len) {
+  if (key_len_.empty()) return (size_t)ctx_.L.num_keys;
+  if (keys_by_len_.empty())
+    for (uint32_t l : key_len_) ++keys_by_len_[l];
+  auto it = keys_by_len_.find(len);
+  return it == keys_by_len_.end() ? 0 : it->second;
 }
 
 CudaBackend::~CudaBackend() {
@@ -635,6 +653,8 @@ CudaBackend::~CudaBackend() {
   if (fx_.acc) cudaFree(fx_.acc);
   if (fx_.cidx) cudaFree(fx_.cidx);
   if (fx_.keys) cudaFree(fx_.keys);
+  if (fx_.rows) cudaFree(fx_.rows);
+  if (fx_.call_loss) cudaFree(fx_.call_loss);
   if (fx_.count) cudaFree(fx_.count);
   if (fx_.loss) cudaFree(fx_.loss);
   if (round_done_) cudaEventDestroy(round_done_);

@@ -74,18 +74,24 @@ class CudaBackend : public Backend {
     return s;
   }
   int num_sms() const { return num_sms_; }
-  // device scratch of the deterministic one-GPU SGNS step (ops_sgns_tma.cu), owned by the backend, grown on demand:
-  // fixed-point accumulator rows, the compact row index of every key touched by the step (-1 = none) and its inverse
+  // device scratch of the deterministic one-GPU steps (fx_accum.cuh), owned by the backend, grown on demand: fixed-point
+  // accumulator regions, the region offset of every key touched by the step (-1 = none) and the step's regions
   struct FxScratch {
-    long long* acc = nullptr;          // [rows][row_len]
-    size_t rows = 0;
-    int row_len = 0;
-    int* cidx = nullptr;               // [num_keys]
-    Key* keys = nullptr;               // [rows]
-    unsigned int* count = nullptr;     // number of compact rows of the current step
-    unsigned long long* loss = nullptr;
+    long long* acc = nullptr;          // [acc_len], zero between steps
+    size_t acc_len = 0;
+    int* cidx = nullptr;               // [num_keys] region offset in units
+    Key* keys = nullptr;               // [rows] key of region r
+    int2* rows = nullptr;              // [rows] (offset, length) of region r, in units
+    size_t rows_cap = 0;
+    size_t step_rows = 0;              // bound on the regions of the current step
+    unsigned int* count = nullptr;     // [2]: regions of the current step, units handed out
+    unsigned long long* loss = nullptr;   // fixed-point loss (SGNS)
+    float* call_loss = nullptr;        // [calls] loss of every call of the step (KGE, MF)
+    size_t calls_cap = 0;
   };
-  FxScratch& fx_scratch(size_t rows, int row_len);
+  FxScratch& fx_scratch(size_t acc_len, size_t rows, size_t calls);
+  // number of keys whose rows have `len` values (every key for a store of one row length)
+  size_t keys_with_len(uint32_t len);
 
   // ---- kernel timeline: CUDA events around every sync-round kernel plus user marks, all relative to one base
   // event, so that the round's kernels and the training kernels of other streams land on one time axis
@@ -153,6 +159,7 @@ class CudaBackend : public Backend {
   unsigned long long dev_timeout_ns_ = 20ull * 1000000000ull;
   std::vector<uint32_t> key_len_;   // host mirror of per-key lengths (mixed-length stores only)
   FxScratch fx_;
+  std::unordered_map<uint32_t, size_t> keys_by_len_;   // keys_with_len cache (mixed-length stores)
 };
 
 }  // namespace adapm

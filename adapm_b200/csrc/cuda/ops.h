@@ -33,19 +33,24 @@ void sample_keys(CudaBackend& be, cudaStream_t stream, int kind, const float* pr
 void intent_prepass(CudaBackend& be, cudaStream_t stream, const Key* keys, int64_t n, Clock end, int worker, Key* out_keys,
                     unsigned int* out_count);
 
+// deterministic = true (one GPU only): every call reads the state at the start of the step and the updates are summed
+// in fixed point and applied once per row after the step (fx_accum.cuh), so the same inputs give the same rows and
+// loss in every run; false: one kernel that adds the updates in place (default).
 // knowledge-graph embeddings, ComplEx: fused pull + score + BCE/L2 gradient + AdaGrad + push (ops_kge.cu)
 void kge_complex_step(CudaBackend& be, cudaStream_t stream, const Key* subj, const Key* rel, const Key* obj,
                       const float* labels, int n_calls, int nh, float eta, float gamma_e, float gamma_r, float* loss_out,
-                      unsigned long long* stats, float dropout_e = 0.f, float dropout_r = 0.f, uint64_t seed = 0);
+                      unsigned long long* stats, float dropout_e = 0.f, float dropout_r = 0.f, uint64_t seed = 0,
+                      bool deterministic = false);
 // RESCAL: fused pull + s^T R o + rank-1 relation gradient + AdaGrad + push (ops_kge.cu); relation rows are 2*D*D floats
 void kge_rescal_step(CudaBackend& be, cudaStream_t stream, const Key* subj, const Key* rel, const Key* obj,
                      const float* labels, int n_calls, int D, float eta, float gamma_e, float gamma_r, float* loss_out,
-                     unsigned long long* stats, float dropout_e = 0.f, float dropout_r = 0.f, uint64_t seed = 0);
+                     unsigned long long* stats, float dropout_e = 0.f, float dropout_r = 0.f, uint64_t seed = 0,
+                     bool deterministic = false);
 
 // matrix factorisation: fused pull + error + L2 + AdaGrad + push (ops_mf.cu)
 void mf_step(CudaBackend& be, cudaStream_t stream, const Key* row_keys, const Key* col_keys, const float* xs,
              const int* row_nnz, const int* col_nnz, int n, int rank, float eps, float lambda, float* loss_out,
-             unsigned long long* stats);
+             unsigned long long* stats, bool deterministic = false);
 
 // wgmma/TMA GEMM: C[M,N] fp32 = A[M,K] bf16 x B[N,K]^T bf16 (ops_gemm_wgmma.cu)
 void gemm_nt_bf16(cudaStream_t stream, const void* A, const void* B, int M, int N, int K, float* C, int ldc);

@@ -38,23 +38,24 @@ void bind(py::module_& m) {
   });
   m.def("kge_complex_step", [](uintptr_t be, uintptr_t stream, uintptr_t s, uintptr_t r, uintptr_t o, uintptr_t labels,
                                int n, int nh, float eta, float gamma_e, float gamma_r, uintptr_t loss, uintptr_t stats,
-                               float dropout_e, float dropout_r, uint64_t seed) {
+                               float dropout_e, float dropout_r, uint64_t seed, bool deterministic) {
     kge_complex_step(backend_of(be), (cudaStream_t)stream, ptr<const Key>(s), ptr<const Key>(r), ptr<const Key>(o),
                      ptr<const float>(labels), n, nh, eta, gamma_e, gamma_r, ptr<float>(loss),
-                     ptr<unsigned long long>(stats), dropout_e, dropout_r, seed);
+                     ptr<unsigned long long>(stats), dropout_e, dropout_r, seed, deterministic);
   });
   m.def("kge_rescal_step", [](uintptr_t be, uintptr_t stream, uintptr_t s, uintptr_t r, uintptr_t o, uintptr_t labels,
                               int n, int D, float eta, float gamma_e, float gamma_r, uintptr_t loss, uintptr_t stats,
-                              float dropout_e, float dropout_r, uint64_t seed) {
+                              float dropout_e, float dropout_r, uint64_t seed, bool deterministic) {
     kge_rescal_step(backend_of(be), (cudaStream_t)stream, ptr<const Key>(s), ptr<const Key>(r), ptr<const Key>(o),
                     ptr<const float>(labels), n, D, eta, gamma_e, gamma_r, ptr<float>(loss),
-                    ptr<unsigned long long>(stats), dropout_e, dropout_r, seed);
+                    ptr<unsigned long long>(stats), dropout_e, dropout_r, seed, deterministic);
   });
   m.def("mf_step", [](uintptr_t be, uintptr_t stream, uintptr_t rows, uintptr_t cols, uintptr_t xs, uintptr_t rn,
-                      uintptr_t cn, int n, int rank, float eps, float lambda, uintptr_t loss, uintptr_t stats) {
+                      uintptr_t cn, int n, int rank, float eps, float lambda, uintptr_t loss, uintptr_t stats,
+                      bool deterministic) {
     mf_step(backend_of(be), (cudaStream_t)stream, ptr<const Key>(rows), ptr<const Key>(cols), ptr<const float>(xs),
             ptr<const int>(rn), ptr<const int>(cn), n, rank, eps, lambda, ptr<float>(loss),
-            ptr<unsigned long long>(stats));
+            ptr<unsigned long long>(stats), deterministic);
   });
   m.def("sgns_shared_workspace_bytes", [](int B, int Nn, int d) { return sgns_shared_workspace_bytes(B, Nn, d); });
   m.def("sgns_shared_core", [](uintptr_t stream, uintptr_t R, uintptr_t contexts, uintptr_t negs, int B, int Nn, int d, float alpha,

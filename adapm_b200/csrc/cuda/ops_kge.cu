@@ -10,12 +10,17 @@
 //   push(x, [-eta * d_x / sqrt(acc_x + d_x^2) | d_x^2])        for x in {s, r, o}
 // Row layout [embedding(nh) | AdaGrad(nh)], embedding = [real(nh/2) | imag(nh/2)].
 // One warp per training call; the three directory lookups are issued by three lanes at once.
+//
+// Deterministic one-GPU variants (kge_step_fx_kernel, kge_rescal_fx_kernel): every call reads the state at the start of
+// the step and adds its updates as fixed-point integers into per-key accumulator regions (fx_accum.cuh), which one
+// apply pass adds to the rows; each call's loss goes to its own slot and is summed in a fixed order.
 #include <cuda_runtime.h>
 
 #include <cstdlib>
 #include <map>
 #include <mutex>
 
+#include "fx_accum.cuh"
 #include "ops.h"
 #include "pm_kernels.cuh"
 
@@ -55,6 +60,12 @@ struct Dropout {
   }
 };
 
+// Fixed-point scales of the deterministic mode. |value update| <= eta per call (AdaGrad normalises it): 2^40 leaves
+// 2^23 / eta calls per element and step. AdaGrad increments are g^2 with g = dl * (sum of products of two embedding
+// values) + gamma * x and |dl| < 1: 2^36 leaves 2^27 of summed g^2 per element and step (resolution 1.5e-11).
+constexpr float kFxVal = 1099511627776.f;     // 2^40
+constexpr float kFxAda = 68719476736.f;       // 2^36
+
 // g = dl * d + (reg ? gamma * x : 0); returns AdaGrad update pair and issues the reductions.
 __device__ __forceinline__ void adagrad_push4(float* emb_ptr, float* acc_ptr, float4 d, float4 x, float dl, float gamma,
                                               float eta) {
@@ -67,11 +78,31 @@ __device__ __forceinline__ void adagrad_push4(float* emb_ptr, float* acc_ptr, fl
   dev::red_row4(emb_ptr, ue);
   dev::red_row4(acc_ptr, ua);
 }
+// deterministic mode: the same update, added to float4 jj of the key's accumulator region (halves of h values)
+__device__ __forceinline__ void adagrad_fx4(const float* acc_ptr, long long* region, int jj, int h, float4 d, float4 x,
+                                            float dl, float gamma, float eta) {
+  float4 g = make_float4(fmaf(gamma, x.x, dl * d.x), fmaf(gamma, x.y, dl * d.y), fmaf(gamma, x.z, dl * d.z),
+                         fmaf(gamma, x.w, dl * d.w));
+  float4 a = dev::ld_row4(acc_ptr);
+  float4 ua = f4_mul(g, g);
+  float4 ue = make_float4(-eta * g.x * rsqrtf(a.x + ua.x), -eta * g.y * rsqrtf(a.y + ua.y),
+                          -eta * g.z * rsqrtf(a.z + ua.z), -eta * g.w * rsqrtf(a.w + ua.w));
+  fx::add4(region, jj, h >> 2, ue, kFxVal);
+  fx::add4(region + h, jj, h >> 2, ua, kFxAda);
+}
+// deterministic mode: adds a staged row of updates [value update (h) | AdaGrad update (h)] to the key's region
+__device__ __forceinline__ void fx_add_staged(long long* region, const float* stage, int h) {
+  for (int i = threadIdx.x & 31; i < 2 * h; i += 32) {
+    const int hf = i >= h;
+    fx::add1(region + hf * h, i - hf * h, h, stage[i], hf ? kFxAda : kFxVal);
+  }
+}
 
 // scalar generic path (any nh; also used when a row is in a transitional state): rows staged in smem
+template <bool FX>
 __device__ __noinline__ float kge_call_generic(const Ctx& c, Key ks, Key kr, Key ko, float label, int nh, float eta,
                                                float gamma_e, float gamma_r, float* stage, bool* applied, uint32_t call,
-                                               Dropout de, Dropout dr) {
+                                               Dropout de, Dropout dr, long long* fx_acc, const int* fx_cidx) {
   const int lane = threadIdx.x & 31;
   float* S = stage; float* R = stage + 2 * nh; float* O = stage + 4 * nh;
   *applied = false;
@@ -108,10 +139,17 @@ __device__ __noinline__ float kge_call_generic(const Ctx& c, Key ks, Key kr, Key
     }
   }
   __syncwarp();
-  bool ok = dev::slow_push(c, ks, S);
-  ok = dev::slow_push(c, kr, R) && ok;
-  ok = dev::slow_push(c, ko, O) && ok;
-  *applied = ok;
+  if (FX) {
+    fx_add_staged(fx::region(fx_acc, fx_cidx, ks, 2 * nh), S, nh);
+    fx_add_staged(fx::region(fx_acc, fx_cidx, kr, 2 * nh), R, nh);
+    fx_add_staged(fx::region(fx_acc, fx_cidx, ko, 2 * nh), O, nh);
+    *applied = true;
+  } else {
+    bool ok = dev::slow_push(c, ks, S);
+    ok = dev::slow_push(c, kr, R) && ok;
+    ok = dev::slow_push(c, ko, O) && ok;
+    *applied = ok;
+  }
   float z = label > 0.5f ? sc : -sc;
   return __logf(1.f + __expf(-fminf(fmaxf(z, -30.f), 30.f)));
 }
@@ -119,12 +157,13 @@ __device__ __noinline__ float kge_call_generic(const Ctx& c, Key ks, Key kr, Key
 // VPLH = float4 vectors per lane per half-embedding (nh/8 float4 per half); VPLH = 0 -> generic only
 // MAXREG = register budget (2 blocks of 256 threads per SM): 128 uses the whole register file; 104 leaves room for one
 // block of the sync-round kernels per SM (see ops_sgns_tma.cu). ADAPM_KGE_REGS=104 selects the lean variant.
-template <int VPLH, int MAXREG>
-__global__ void __maxnreg__(MAXREG)
-kge_step_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, const Key* __restrict__ rel,
-                const Key* __restrict__ obj, const float* __restrict__ labels, int n_calls, int nh, float eta,
-                float gamma_e, float gamma_r, float* __restrict__ loss_out, unsigned long long* __restrict__ stats,
-                Dropout de, Dropout dr) {
+// FX: deterministic mode (kge_step_fx_kernel): start-of-step reads, fixed-point sums into fx_acc, call losses.
+template <int VPLH, bool FX>
+__device__ __forceinline__ void
+kge_step_body(const Ctx& c, const Key* __restrict__ subj, const Key* __restrict__ rel, const Key* __restrict__ obj,
+              const float* __restrict__ labels, int n_calls, int nh, float eta, float gamma_e, float gamma_r,
+              float* __restrict__ loss_out, unsigned long long* __restrict__ stats, Dropout de, Dropout dr,
+              long long* __restrict__ fx_acc, const int* __restrict__ fx_cidx, float* __restrict__ call_loss) {
   extern __shared__ float smem_f[];  // generic path: per warp 6*nh floats
   dev::cta_enter(c);
   const int lane = threadIdx.x & 31;
@@ -152,7 +191,10 @@ kge_step_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, con
     if (VPLH == 0 || !ps || !pr || !po) {
       ++n_slow;
       bool applied;
-      loss_acc += kge_call_generic(c, ks, kr, ko, label, nh, eta, gamma_e, gamma_r, stage, &applied, (uint32_t)p, de, dr);
+      const float l = kge_call_generic<FX>(c, ks, kr, ko, label, nh, eta, gamma_e, gamma_r, stage, &applied,
+                                           (uint32_t)p, de, dr, fx_acc, fx_cidx);
+      if (FX) { if (lane == 0) call_loss[p] = l; }
+      else loss_acc += l;
       if (applied) n_upd += 3;
       continue;
     }
@@ -186,12 +228,33 @@ kge_step_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, con
     const float ge = pos ? gamma_e : 0.f, gr = pos ? gamma_r : 0.f;
     {
       float z = pos ? sc : -sc;
-      loss_acc += __logf(1.f + __expf(-fminf(fmaxf(z, -30.f), 30.f)));
+      const float l = __logf(1.f + __expf(-fminf(fmaxf(z, -30.f), 30.f)));
+      if (FX) { if (lane == 0) call_loss[p] = l; }
+      else loss_acc += l;
+    }
+    long long *fs = nullptr, *fr = nullptr, *fo = nullptr;
+    if (FX) {
+      fs = fx::region(fx_acc, fx_cidx, ks, 2 * nh); fr = fx::region(fx_acc, fx_cidx, kr, 2 * nh);
+      fo = fx::region(fx_acc, fx_cidx, ko, 2 * nh);
     }
 #pragma unroll
     for (int v = 0; v < V; ++v) {
       const int j = lane + 32 * v;
-      if (j < nvh) {
+      if (FX && j < nvh) {
+        float4 ds_re = f4_fma(rre[v], ore[v], f4_mul(rim[v], oim[v]));
+        float4 ds_im = f4_sub(f4_mul(rre[v], oim[v]), f4_mul(rim[v], ore[v]));
+        float4 dr_re = f4_fma(sre[v], ore[v], f4_mul(sim[v], oim[v]));
+        float4 dr_im = f4_sub(f4_mul(sre[v], oim[v]), f4_mul(sim[v], ore[v]));
+        float4 do_re = f4_sub(f4_mul(rre[v], sre[v]), f4_mul(rim[v], sim[v]));
+        float4 do_im = f4_fma(rre[v], sim[v], f4_mul(rim[v], sre[v]));
+        // float4 j of the real half, float4 nvh + j of the imaginary half
+        adagrad_fx4(ps + nh + 4 * j, fs, j, nh, ds_re, sre[v], dl, ge, eta);
+        adagrad_fx4(ps + nh + H + 4 * j, fs, nvh + j, nh, ds_im, sim[v], dl, ge, eta);
+        adagrad_fx4(pr + nh + 4 * j, fr, j, nh, dr_re, rre[v], dl, gr, eta);
+        adagrad_fx4(pr + nh + H + 4 * j, fr, nvh + j, nh, dr_im, rim[v], dl, gr, eta);
+        adagrad_fx4(po + nh + 4 * j, fo, j, nh, do_re, ore[v], dl, ge, eta);
+        adagrad_fx4(po + nh + H + 4 * j, fo, nvh + j, nh, do_im, oim[v], dl, ge, eta);
+      } else if (j < nvh) {
         // gradients of the trilinear score (reference score_grad)
         float4 ds_re = f4_fma(rre[v], ore[v], f4_mul(rim[v], oim[v]));
         float4 ds_im = f4_sub(f4_mul(rre[v], oim[v]), f4_mul(rim[v], ore[v]));
@@ -212,7 +275,7 @@ kge_step_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, con
   }
 
   __syncwarp();
-  if (lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
+  if (!FX && lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
   unsigned sl = n_local, sr = n_remote;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -228,6 +291,26 @@ kge_step_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, con
   dev::cta_exit(c);
 }
 
+template <int VPLH, int MAXREG>
+__global__ void __maxnreg__(MAXREG)
+kge_step_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, const Key* __restrict__ rel,
+                const Key* __restrict__ obj, const float* __restrict__ labels, int n_calls, int nh, float eta,
+                float gamma_e, float gamma_r, float* __restrict__ loss_out, unsigned long long* __restrict__ stats,
+                Dropout de, Dropout dr) {
+  kge_step_body<VPLH, false>(c, subj, rel, obj, labels, n_calls, nh, eta, gamma_e, gamma_r, loss_out, stats, de, dr,
+                             nullptr, nullptr, nullptr);
+}
+
+template <int VPLH>
+__global__ void __maxnreg__(128)
+kge_step_fx_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, const Key* __restrict__ rel,
+                   const Key* __restrict__ obj, const float* __restrict__ labels, int n_calls, int nh, float eta,
+                   float gamma_e, float gamma_r, unsigned long long* __restrict__ stats, Dropout de, Dropout dr,
+                   long long* __restrict__ fx_acc, const int* __restrict__ fx_cidx, float* __restrict__ call_loss) {
+  kge_step_body<VPLH, true>(c, subj, rel, obj, labels, n_calls, nh, eta, gamma_e, gamma_r, nullptr, stats, de, dr,
+                            fx_acc, fx_cidx, call_loss);
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // RESCAL (reference kge.cc:895-922): score = s^T R o with a D x D relation matrix (relation row = [R | AdaGrad] of
 // 2 D^2 floats), gradients d_s = R o, d_o = R^T s, d_R = s o^T (rank 1). One warp per training call:
@@ -241,18 +324,27 @@ __device__ __noinline__ bool rescal_slow_rows(const Ctx& c, Key ks, Key kr, Key 
   return dev::slow_pull(c, ks, gs) && dev::slow_pull(c, kr, gr) && dev::slow_pull(c, ko, go);
 }
 
-__global__ void __launch_bounds__(kThreads)
-kge_rescal_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, const Key* __restrict__ rel,
-                  const Key* __restrict__ obj, const float* __restrict__ labels, int n_calls, int D, float eta,
-                  float gamma_e, float gamma_r, float* __restrict__ loss_out, unsigned long long* __restrict__ stats,
-                  Dropout de, Dropout dr, float* __restrict__ scratch) {
-  extern __shared__ float smem_f[];   // per warp: s[D] | o[D] | ds[D] | do[D]
+// Deterministic mode (FX, kge_rescal_fx_kernel): pass 1 forms ds and do in a fixed order instead of with shared-memory
+// atomics - the G = D/4 float4 of a matrix row are read by G consecutive lanes, 32/G rows per round; ds[i] is the sum of
+// its G partial dots (shuffle tree for G a power of two, else lane-ordered), each lane keeps its four do partial sums in
+// registers over its rows, and do[j] sums those in row-group order. Updates go to fixed-point accumulator regions
+// (relation region [D^2 | D^2], entity regions [D | D]) and each call's loss to its own slot.
+constexpr int kRescalFxSmem = 32 + 128;   // extra floats per warp: ds partials [32] | do partials [32/G][D]
+
+template <bool FX>
+__device__ __forceinline__ void
+kge_rescal_body(const Ctx& c, const Key* __restrict__ subj, const Key* __restrict__ rel, const Key* __restrict__ obj,
+                const float* __restrict__ labels, int n_calls, int D, float eta, float gamma_e, float gamma_r,
+                float* __restrict__ loss_out, unsigned long long* __restrict__ stats, Dropout de, Dropout dr,
+                float* __restrict__ scratch, long long* __restrict__ fx_acc, const int* __restrict__ fx_cidx,
+                float* __restrict__ call_loss) {
+  extern __shared__ float smem_f[];   // per warp: s[D] | o[D] | ds[D] | do[D] (| FX partials)
   dev::cta_enter(c);
   const int lane = threadIdx.x & 31;
   const int wib = threadIdx.x >> 5;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  float* sv = smem_f + (size_t)wib * 4 * D;
+  float* sv = smem_f + (size_t)wib * (FX ? 4 * D + kRescalFxSmem : 4 * D);
   float* ov = sv + D; float* dsv = ov + D; float* dov = dsv + D;
   const int DD = D * D;
   const int nv = DD >> 2;          // float4 of the relation matrix
@@ -276,7 +368,10 @@ kge_rescal_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, c
     if (slow) {   // stage the three rows in global scratch and run the same math on the copies
       ++n_slow;
       float* gr_ = my_scratch; float* gs_ = my_scratch + 2 * DD; float* go_ = gs_ + 2 * D;
-      if (!rescal_slow_rows(c, ks, kr, ko, gs_, gr_, go_)) continue;
+      if (!rescal_slow_rows(c, ks, kr, ko, gs_, gr_, go_)) {
+        if (FX && lane == 0) call_loss[p] = 0.f;
+        continue;
+      }
       ps = gs_; pr = gr_; po = go_;
     }
     const uint32_t cp = (uint32_t)p;
@@ -288,14 +383,58 @@ kge_rescal_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, c
     }
     __syncwarp();
     // ---- pass 1: ds = R o, do = R^T s
-    for (int q = lane; q < nv; q += 32) {
-      const int e = 4 * q, i = e / D, j = e - i * D;
-      float4 r4 = dev::ld_row4(pr + e);
-      if (dr.p > 0.f) r4 = dr.apply4(r4, cp, 1, (uint32_t)e);
-      const float si = sv[i];
-      atomicAdd(dsv + i, r4.x * ov[j] + r4.y * ov[j + 1] + r4.z * ov[j + 2] + r4.w * ov[j + 3]);
-      atomicAdd(dov + j, si * r4.x); atomicAdd(dov + j + 1, si * r4.y);
-      atomicAdd(dov + j + 2, si * r4.z); atomicAdd(dov + j + 3, si * r4.w);
+    if (FX) {
+      const int G = D >> 2, rpr = 32 / G;           // float4 per matrix row, rows per round
+      const int rg = lane / G, j = 4 * (lane - rg * G);
+      const bool pow2 = (G & (G - 1)) == 0;
+      float* dsp = dov + D;                         // [32] partial dots
+      float* dop = dsp + 32;                        // [rpr][D] partial do sums
+      float4 dacc = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int i0 = 0; i0 < D; i0 += rpr) {
+        const int i = i0 + rg;
+        float part = 0.f;
+        if (rg < rpr && i < D) {
+          const int e = i * D + j;
+          float4 r4 = dev::ld_row4(pr + e);
+          if (dr.p > 0.f) r4 = dr.apply4(r4, cp, 1, (uint32_t)e);
+          part = r4.x * ov[j] + r4.y * ov[j + 1] + r4.z * ov[j + 2] + r4.w * ov[j + 3];
+          const float si = sv[i];
+          dacc.x += si * r4.x; dacc.y += si * r4.y; dacc.z += si * r4.z; dacc.w += si * r4.w;
+        }
+        if (pow2) {                                 // G | 32: fixed shuffle tree inside each group of G lanes
+          for (int o = G >> 1; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+          if (lane - rg * G == 0 && i < D) dsv[i] = part;
+        } else {
+          dsp[lane] = part;
+          __syncwarp();
+          if (lane < rpr && i0 + lane < D) {
+            float t = 0.f;
+            for (int q = 0; q < G; ++q) t += dsp[lane * G + q];
+            dsv[i0 + lane] = t;
+          }
+          __syncwarp();
+        }
+      }
+      if (rg < rpr) {
+        float* d4 = dop + rg * D + j;
+        d4[0] = dacc.x; d4[1] = dacc.y; d4[2] = dacc.z; d4[3] = dacc.w;
+      }
+      __syncwarp();
+      for (int jj = lane; jj < D; jj += 32) {
+        float t = 0.f;
+        for (int r = 0; r < rpr; ++r) t += dop[r * D + jj];
+        dov[jj] = t;
+      }
+    } else {
+      for (int q = lane; q < nv; q += 32) {
+        const int e = 4 * q, i = e / D, j = e - i * D;
+        float4 r4 = dev::ld_row4(pr + e);
+        if (dr.p > 0.f) r4 = dr.apply4(r4, cp, 1, (uint32_t)e);
+        const float si = sv[i];
+        atomicAdd(dsv + i, r4.x * ov[j] + r4.y * ov[j + 1] + r4.z * ov[j + 2] + r4.w * ov[j + 3]);
+        atomicAdd(dov + j, si * r4.x); atomicAdd(dov + j + 1, si * r4.y);
+        atomicAdd(dov + j + 2, si * r4.z); atomicAdd(dov + j + 3, si * r4.w);
+      }
     }
     __syncwarp();
     float sc = 0.f;
@@ -306,14 +445,24 @@ kge_rescal_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, c
     const float ge = pos ? gamma_e : 0.f, grr = pos ? gamma_r : 0.f;
     {
       float z = pos ? sc : -sc;
-      loss_acc += __logf(1.f + __expf(-fminf(fmaxf(z, -30.f), 30.f)));
+      const float l = __logf(1.f + __expf(-fminf(fmaxf(z, -30.f), 30.f)));
+      if (FX) { if (lane == 0) call_loss[p] = l; }
+      else loss_acc += l;
+    }
+    long long *fs = nullptr, *fr = nullptr, *fo = nullptr;
+    if (FX) {   // regions in units of an entity row (2 D): relation regions are D units
+      fs = fx::region(fx_acc, fx_cidx, ks, 2 * D); fr = fx::region(fx_acc, fx_cidx, kr, 2 * D);
+      fo = fx::region(fx_acc, fx_cidx, ko, 2 * D);
     }
     // ---- entity rows
     for (int i = lane; i < D; i += 32) {
       const float g_s = fmaf(ge, sv[i], dl * dsv[i]), g_o = fmaf(ge, ov[i], dl * dov[i]);
       const float a_s = reinterpret_cast<const volatile float*>(ps)[D + i], a_o = reinterpret_cast<const volatile float*>(po)[D + i];
       const float us = -eta * g_s * rsqrtf(a_s + g_s * g_s), uo = -eta * g_o * rsqrtf(a_o + g_o * g_o);
-      if (slow) { ps[i] = us; ps[D + i] = g_s * g_s; po[i] = uo; po[D + i] = g_o * g_o; }
+      if (FX) {
+        fx::add1(fs, i, D, us, kFxVal); fx::add1(fs + D, i, D, g_s * g_s, kFxAda);
+        fx::add1(fo, i, D, uo, kFxVal); fx::add1(fo + D, i, D, g_o * g_o, kFxAda);
+      } else if (slow) { ps[i] = us; ps[D + i] = g_s * g_s; po[i] = uo; po[D + i] = g_o * g_o; }
       else { mem::red_add(ps + i, us); mem::red_add(ps + D + i, g_s * g_s); mem::red_add(po + i, uo); mem::red_add(po + D + i, g_o * g_o); }
     }
     // ---- pass 2: relation matrix update (rank-1 gradient)
@@ -328,10 +477,14 @@ kge_rescal_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, c
       const float4 ua = f4_mul(g, g);
       const float4 ue = make_float4(-eta * g.x * rsqrtf(a4.x + ua.x), -eta * g.y * rsqrtf(a4.y + ua.y),
                                     -eta * g.z * rsqrtf(a4.z + ua.z), -eta * g.w * rsqrtf(a4.w + ua.w));
-      if (slow) { *reinterpret_cast<float4*>(pr + e) = ue; *reinterpret_cast<float4*>(pr + DD + e) = ua; }
+      if (FX) { fx::add4(fr, q, nv, ue, kFxVal); fx::add4(fr + DD, q, nv, ua, kFxAda); }
+      else if (slow) { *reinterpret_cast<float4*>(pr + e) = ue; *reinterpret_cast<float4*>(pr + DD + e) = ua; }
       else { dev::red_row4(pr + e, ue); dev::red_row4(pr + DD + e, ua); }
     }
-    if (slow) {
+    if (FX) {
+      if (lane < 3 && !slow) dev::mark_pushed(t);
+      n_upd += 3;
+    } else if (slow) {
       __syncwarp();
       bool ok = dev::slow_push(c, ks, ps);
       ok = dev::slow_push(c, kr, pr) && ok;
@@ -345,7 +498,7 @@ kge_rescal_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, c
   }
 
   __syncwarp();
-  if (lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
+  if (!FX && lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
   unsigned sl = n_local, sr = n_remote;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -359,6 +512,25 @@ kge_rescal_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, c
     if (n_upd) atomicAdd(stats + 3, (unsigned long long)n_upd);
   }
   dev::cta_exit(c);
+}
+
+__global__ void __launch_bounds__(kThreads)
+kge_rescal_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, const Key* __restrict__ rel,
+                  const Key* __restrict__ obj, const float* __restrict__ labels, int n_calls, int D, float eta,
+                  float gamma_e, float gamma_r, float* __restrict__ loss_out, unsigned long long* __restrict__ stats,
+                  Dropout de, Dropout dr, float* __restrict__ scratch) {
+  kge_rescal_body<false>(c, subj, rel, obj, labels, n_calls, D, eta, gamma_e, gamma_r, loss_out, stats, de, dr, scratch,
+                         nullptr, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(kThreads)
+kge_rescal_fx_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, const Key* __restrict__ rel,
+                     const Key* __restrict__ obj, const float* __restrict__ labels, int n_calls, int D, float eta,
+                     float gamma_e, float gamma_r, unsigned long long* __restrict__ stats, Dropout de, Dropout dr,
+                     float* __restrict__ scratch, long long* __restrict__ fx_acc, const int* __restrict__ fx_cidx,
+                     float* __restrict__ call_loss) {
+  kge_rescal_body<true>(c, subj, rel, obj, labels, n_calls, D, eta, gamma_e, gamma_r, nullptr, stats, de, dr, scratch,
+                        fx_acc, fx_cidx, call_loss);
 }
 
 }  // namespace
@@ -375,7 +547,7 @@ static Dropout make_dropout(float p, uint64_t seed, uint32_t salt) {
 
 void kge_complex_step(CudaBackend& be, cudaStream_t stream, const Key* subj, const Key* rel, const Key* obj,
                       const float* labels, int n_calls, int nh, float eta, float gamma_e, float gamma_r, float* loss_out,
-                      unsigned long long* stats, float dropout_e, float dropout_r, uint64_t seed) {
+                      unsigned long long* stats, float dropout_e, float dropout_r, uint64_t seed, bool deterministic) {
   if (n_calls == 0) return;
   const Dropout de = make_dropout(dropout_e, seed, 0x11u), dr = make_dropout(dropout_r, seed, 0x22u);
   ADAPM_CHECK(nh % 2 == 0, "ComplEx needs an even embedding size");
@@ -406,6 +578,31 @@ void kge_complex_step(CudaBackend& be, cudaStream_t stream, const Key* subj, con
     if (lean) ADAPM_LAUNCH_KGE2(V, 104); \
     else ADAPM_LAUNCH_KGE2(V, 128);      \
   } while (0)
+#define ADAPM_LAUNCH_KGE_FX(V)                                                                                 \
+  do {                                                                                                         \
+    static bool attr_set = false;                                                                              \
+    if (!attr_set) {                                                                                           \
+      cudaFuncSetAttribute(kge_step_fx_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);    \
+      attr_set = true;                                                                                         \
+    }                                                                                                          \
+    kge_step_fx_kernel<V><<<blocks, kThreads, smem, stream>>>(c, subj, rel, obj, labels, n_calls, nh, eta,     \
+                                                              gamma_e, gamma_r, stats, de, dr, fxs->acc,       \
+                                                              fxs->cidx, fxs->call_loss);                      \
+  } while (0)
+  if (deterministic) {
+    // one GPU, start-of-step reads: every key gets a [nh | nh] accumulator region (entity and relation rows alike)
+    const fx::Source src[3] = {{subj, n_calls, 1}, {rel, n_calls, 1}, {obj, n_calls, 1}};
+    CudaBackend::FxScratch* fxs = &fx::begin(be, stream, src, 3, 2 * nh, n_calls);
+    switch (vplh) {
+      case 1: ADAPM_LAUNCH_KGE_FX(1); break;
+      case 2: ADAPM_LAUNCH_KGE_FX(2); break;
+      default: ADAPM_LAUNCH_KGE_FX(0); break;
+    }
+    ADAPM_COUNT_LAUNCH();
+    ADAPM_CUDA_CHECK(cudaGetLastError());
+    fx::apply(be, stream, 2 * nh, kFxVal, kFxAda, 0.f, n_calls, loss_out);
+    return;
+  }
   switch (vplh) {
     case 1: ADAPM_LAUNCH_KGE(1); break;
     case 2: ADAPM_LAUNCH_KGE(2); break;
@@ -418,7 +615,7 @@ void kge_complex_step(CudaBackend& be, cudaStream_t stream, const Key* subj, con
 // RESCAL training calls: entity rows 2*D floats, relation rows 2*D*D floats (D % 4 == 0, D <= 128).
 void kge_rescal_step(CudaBackend& be, cudaStream_t stream, const Key* subj, const Key* rel, const Key* obj,
                      const float* labels, int n_calls, int D, float eta, float gamma_e, float gamma_r, float* loss_out,
-                     unsigned long long* stats, float dropout_e, float dropout_r, uint64_t seed) {
+                     unsigned long long* stats, float dropout_e, float dropout_r, uint64_t seed, bool deterministic) {
   if (n_calls == 0) return;
   ADAPM_CHECK(D % 4 == 0 && D >= 4 && D <= 128, "kge_rescal_step: embedding size must be a multiple of 4 in [4, 128]");
   ADAPM_CHECK(be.ctx().L.val_bytes == 4, "the fused ops need float32 rows (Options::dtype)");
@@ -427,7 +624,7 @@ void kge_rescal_step(CudaBackend& be, cudaStream_t stream, const Key* subj, cons
   const Dropout de = make_dropout(dropout_e, seed, 0x11u), dr = make_dropout(dropout_r, seed, 0x22u);
   const int warps_per_block = kThreads / 32;
   const int blocks = std::min((n_calls + warps_per_block - 1) / warps_per_block, be.num_sms() * 4);
-  const size_t smem = (size_t)warps_per_block * 4 * D * sizeof(float);
+  const size_t smem = (size_t)warps_per_block * (deterministic ? 4 * D + kRescalFxSmem : 4 * D) * sizeof(float);
   // generic-path scratch (rows in a transitional protocol state): one relation row + two entity rows per warp
   static std::mutex mu;
   static std::map<int, std::pair<float*, size_t>> scratch_by_dev;
@@ -442,6 +639,18 @@ void kge_rescal_step(CudaBackend& be, cudaStream_t stream, const Key* subj, cons
       e.second = need;
     }
     scratch = e.first;
+  }
+  if (deterministic) {
+    // one GPU, start-of-step reads: entity regions [D | D] (one unit), relation regions [D^2 | D^2] (D units)
+    const fx::Source src[3] = {{subj, n_calls, 1}, {obj, n_calls, 1}, {rel, n_calls, D}};
+    CudaBackend::FxScratch& fxs = fx::begin(be, stream, src, 3, 2 * D, n_calls);
+    kge_rescal_fx_kernel<<<blocks, kThreads, smem, stream>>>(c, subj, rel, obj, labels, n_calls, D, eta, gamma_e,
+                                                             gamma_r, stats, de, dr, scratch, fxs.acc, fxs.cidx,
+                                                             fxs.call_loss);
+    ADAPM_COUNT_LAUNCH();
+    ADAPM_CUDA_CHECK(cudaGetLastError());
+    fx::apply(be, stream, 2 * D, kFxVal, kFxAda, 0.f, n_calls, loss_out);
+    return;
   }
   kge_rescal_kernel<<<blocks, kThreads, smem, stream>>>(c, subj, rel, obj, labels, n_calls, D, eta, gamma_e, gamma_r,
                                                         loss_out, stats, de, dr, scratch);

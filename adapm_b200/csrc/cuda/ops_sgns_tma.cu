@@ -14,6 +14,7 @@
 
 #include <cstdlib>
 
+#include "fx_accum.cuh"
 #include "ops.h"
 #include "pm_kernels.cuh"
 #include "sgns_common.cuh"
@@ -78,21 +79,13 @@ __device__ __forceinline__ void mark_pushed(void* mark, int bits) {
   else mem::red_add(static_cast<uint32_t*>(mark), 1u);
 }
 
-// Deterministic accumulation (one GPU): updates are added as 64-bit fixed-point integers into an accumulator row per
-// key touched by the step instead of into the store rows, so the step reads only start-of-step values and the sums do
-// not depend on the order in which warps add them; sgns_fx_apply_kernel then adds each row's sum to the store once.
-// |embedding update| <= alpha per contribution (AdaGrad normalises it), AdaGrad increments are squared gradients:
-// 2^40 / 2^36 leave 2^23 / 2^27 of range. Within each half of an accumulator row, element 4j + c sits at c * d/4 + j,
-// so that one warp-wide atomic over the lanes' j covers contiguous memory.
+// Deterministic accumulation (one GPU, fx_accum.cuh): |embedding update| <= alpha per contribution (AdaGrad normalises
+// it), AdaGrad increments are squared gradients: 2^40 / 2^36 leave 2^23 / 2^27 of range per element and step. The
+// loss is a fixed-point sum too: 2^32 leaves 2^31 of summed loss per step.
 constexpr float kFxEmb = 1099511627776.f;     // 2^40
 constexpr float kFxAda = 68719476736.f;       // 2^36
 constexpr float kFxLoss = 4294967296.f;       // 2^32
-__device__ __forceinline__ void fx_add4(long long* half, int j, int nvec, float4 v, float scale) {
-  atomicAdd(reinterpret_cast<unsigned long long*>(half + j), (unsigned long long)__float2ll_rn(v.x * scale));
-  atomicAdd(reinterpret_cast<unsigned long long*>(half + nvec + j), (unsigned long long)__float2ll_rn(v.y * scale));
-  atomicAdd(reinterpret_cast<unsigned long long*>(half + 2 * nvec + j), (unsigned long long)__float2ll_rn(v.z * scale));
-  atomicAdd(reinterpret_cast<unsigned long long*>(half + 3 * nvec + j), (unsigned long long)__float2ll_rn(v.w * scale));
-}
+using fx::add4;
 
 struct WarpSmem {
   unsigned long long bar[RING];
@@ -287,8 +280,8 @@ sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __r
             ue.z = alpha * gr.z * rsqrtf(a1.z + ua.z);
             ue.w = alpha * gr.w * rsqrtf(a1.w + ua.w);
             if (FX) {                     // deterministic mode: fixed-point sums, applied after the step
-              fx_add4(fx_t, j, nvec, ue, kFxEmb);
-              fx_add4(fx_t + d, j, nvec, ua, kFxAda);
+              add4(fx_t, j, nvec, ue, kFxEmb);
+              add4(fx_t + d, j, nvec, ua, kFxAda);
             } else if (BULK) {            // stage the update in place of the consumed row
               reinterpret_cast<float4*>(buf)[j] = ue;
               reinterpret_cast<float4*>(buf + d)[j] = ua;
@@ -363,8 +356,8 @@ sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __r
           ue.z = alpha * g0[v].z * rsqrtf(a0.z + ua.z);
           ue.w = alpha * g0[v].w * rsqrtf(a0.w + ua.w);
           if (FX) {
-            fx_add4(fx_c, j, nvec, ue, kFxEmb);
-            fx_add4(fx_c + d, j, nvec, ua, kFxAda);
+            add4(fx_c, j, nvec, ue, kFxEmb);
+            add4(fx_c + d, j, nvec, ua, kFxAda);
           } else if (BULK) {
             reinterpret_cast<float4*>(scratch)[j] = ue;
             reinterpret_cast<float4*>(scratch + d)[j] = ua;
@@ -426,66 +419,6 @@ sgns_step_tma_fx_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ c
                                        fx_acc, fx_cidx, fx_loss);
 }
 
-// key of update source i of a step: centers [0, B), contexts [B, 2B), negatives [2B, 2B + B * neg)
-__device__ __forceinline__ Key fx_key(const Key* centers, const Key* contexts, const Key* negatives, int n_pairs, long i) {
-  if (i < n_pairs) return centers[i];
-  if (i < 2L * n_pairs) return contexts[i - n_pairs];
-  return negatives[i - 2L * n_pairs];
-}
-
-// Gives every key touched by the step a compact accumulator row (which row a key gets may vary from run to run;
-// what is summed into it does not).
-__global__ void sgns_fx_index_kernel(const Key* __restrict__ centers, const Key* __restrict__ contexts,
-                                     const Key* __restrict__ negatives, int n_pairs, int neg, int* __restrict__ cidx,
-                                     Key* __restrict__ keys, unsigned int* __restrict__ count) {
-  const long n = (long)n_pairs * (neg + 2);
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
-    const Key k = fx_key(centers, contexts, negatives, n_pairs, i);
-    if (k >= 0 && atomicCAS(cidx + k, -1, -2) == -1) {
-      const unsigned r = atomicAdd(count, 1u);
-      keys[r] = k;
-      cidx[k] = (int)r;
-    }
-  }
-}
-
-// One warp per accumulator row: adds its fixed-point sums to the key's store row (one writer per row), clears the
-// row and the key's index; thread 0 moves the step's fixed-point loss into loss_out.
-__global__ void sgns_fx_apply_kernel(const __grid_constant__ Ctx c, int d, const Key* __restrict__ keys,
-                                     const unsigned int* __restrict__ count, int* __restrict__ cidx,
-                                     long long* __restrict__ fx_acc, unsigned long long* __restrict__ fx_loss,
-                                     float* __restrict__ loss_out) {
-  dev::cta_enter(c);
-  const int lane = threadIdx.x & 31;
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    const long long v = (long long)*fx_loss;
-    *fx_loss = 0ull;
-    if (loss_out) *loss_out += (float)((double)v / (double)kFxLoss);
-  }
-  const unsigned n = *count;
-  const int nvec = d >> 2;
-  const unsigned nwarps = (gridDim.x * blockDim.x) >> 5;
-  for (unsigned r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n; r += nwarps) {
-    const Key k = keys[r];
-    const int32_t slot = __ldcg(slot_of(c, c.rank) + k);
-    long long* a = fx_acc + (size_t)r * (2 * d);
-    float* row = slot >= 0 ? row_ptr<float>(c, c.rank, 0, (uint32_t)slot) : nullptr;
-    for (int h = 0; h < 2; ++h) {
-      const double inv = 1.0 / (double)(h ? kFxAda : kFxEmb);
-      for (int i = lane; i < d; i += 32) {
-        const long long v = a[h * d + i];
-        if (v) {
-          const int e = 4 * (i % nvec) + i / nvec;
-          if (row) row[h * d + e] += (float)((double)v * inv);
-          a[h * d + i] = 0;
-        }
-      }
-    }
-    if (lane == 0) cidx[k] = -1;
-  }
-  dev::cta_exit(c);
-}
-
 }  // namespace
 
 // Returns false if this variant does not support the shape (the caller falls back to the LDG kernel).
@@ -517,17 +450,14 @@ bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   static const bool det_env = [] { const char* e = getenv("ADAPM_SGNS_DETERMINISTIC"); return !e || atoi(e) != 0; }();
   const long n_src = (long)n_pairs * (neg + 2);
   ADAPM_CHECK(n_src < (1L << 29), "sgns_step: too many keys in one step");   // (row index << 2 fits an int)
-  CudaBackend::FxScratch* fx =
-      det_env && c.L.world == 1 ? &be.fx_scratch((size_t)std::min<long>(n_src, c.L.num_keys), 2 * d) : nullptr;
-  long long* fx_acc = fx ? fx->acc : nullptr;
-  const int* fx_cidx = fx ? fx->cidx : nullptr;
-  unsigned long long* fx_loss = fx ? fx->loss : nullptr;
-  if (fx) {
-    ADAPM_CUDA_CHECK(cudaMemsetAsync(fx->count, 0, sizeof(unsigned int), stream));
-    sgns_fx_index_kernel<<<(int)std::min<long>((n_src + 255) / 256, be.num_sms() * 8L), 256, 0, stream>>>(
-        centers, contexts, negatives, n_pairs, neg, fx->cidx, fx->keys, fx->count);
-    ADAPM_COUNT_LAUNCH();
+  CudaBackend::FxScratch* fxs = nullptr;
+  if (det_env && c.L.world == 1) {   // every key of the step gets an accumulator region of 2 d (one unit)
+    const fx::Source src[3] = {{centers, n_pairs, 1}, {contexts, n_pairs, 1}, {negatives, (long)n_pairs * neg, 1}};
+    fxs = &fx::begin(be, stream, src, 3, 2 * d);
   }
+  long long* fx_acc = fxs ? fxs->acc : nullptr;
+  const int* fx_cidx = fxs ? fxs->cidx : nullptr;
+  unsigned long long* fx_loss = fxs ? fxs->loss : nullptr;
 #define ADAPM_LAUNCH_TMA3(V, T, B)                                                                              \
   do {                                                                                                          \
     static bool attr_set = false;                                                                               \
@@ -555,7 +485,7 @@ bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, con
     sgns_step_tma_fx_kernel<V><<<blocks, threads, smem, stream>>>(c, centers, contexts, negatives, n_pairs, neg, d, \
                                                                   alpha, stats, fx_acc, fx_cidx, fx_loss);      \
   } while (0)
-  if (fx) {
+  if (fxs) {
     switch (vpl) {
       case 1: ADAPM_LAUNCH_TMA_FX(1); break;
       case 2: ADAPM_LAUNCH_TMA_FX(2); break;
@@ -570,12 +500,7 @@ bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   }
   ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cudaGetLastError());
-  if (fx) {
-    sgns_fx_apply_kernel<<<(int)std::min<long>((n_src + 7) / 8, be.num_sms() * 16L), 256, 0, stream>>>(
-        c, d, fx->keys, fx->count, fx->cidx, fx->acc, fx->loss, loss_out);
-    ADAPM_COUNT_LAUNCH();
-    ADAPM_CUDA_CHECK(cudaGetLastError());
-  }
+  if (fxs) fx::apply(be, stream, 2 * d, kFxEmb, kFxAda, kFxLoss, 0, loss_out);
   return true;
 }
 

@@ -23,6 +23,9 @@ hash, reproducible by ``ops.kge_dropout_mask``). The evaluation ranks subject, r
 triple (kge.cc:716-774) and aggregates the reference's 19 metrics over the ranks through ``eval_key``
 (kge.cc:592-709). The CPU backend runs the same calls through the public Pull/Push API with PyTorch math
 (``kge_reference_step``, also the numerics oracle of the GPU tests).
+
+``KGEConfig.deterministic`` selects the deterministic one-GPU variant of the fused kernels (start-of-step reads,
+fixed-point sums, bit-identical runs); the CPU backend accepts it and already follows the start-of-step rule.
 """
 from __future__ import annotations
 
@@ -54,6 +57,7 @@ class KGEConfig:
     signal_initial_relations_intent: bool = False
     init_std: float = 0.1
     model_seed: int = 134827
+    deterministic: bool = False      # one GPU: start-of-step reads, bit-identical runs (ops.kge_complex_step)
 
     @property
     def entity_len(self) -> int:
@@ -215,7 +219,7 @@ class KGE:
             S, R, O, L = self._expand(tr, neg)
             fused = kge_complex_step if cfg.algorithm == "ComplEx" else kge_rescal_step
             fused(self.server, S, R, O, L, cfg.embed_dim, cfg.eta, cfg.gamma_entity, cfg.gamma_relation, self.loss,
-                  self.stats, cfg.dropout_entity, cfg.dropout_relation, seed)
+                  self.stats, cfg.dropout_entity, cfg.dropout_relation, seed, deterministic=cfg.deterministic)
             self.step_no += 1
             return self.loss
         neg = torch.randint(0, cfg.num_entities, (B, 2 * cfg.neg_ratio), generator=self._gen)

@@ -45,6 +45,8 @@ class MFConfig:
     wor_blocks: bool = True          # WOR schedule for the DSGD blocks (else the fixed rotation (rank + sub-epoch) % W)
     wor_points: bool = True          # WOR schedule for the data points within a block / epoch (else file order)
     early_stop: int = 0              # stop an epoch after N data points (debugging)
+    deterministic: bool = False      # one GPU: start-of-step reads, bit-identical runs (ops.mf_step); the CPU backend
+                                     # accepts it and already follows the start-of-step rule
 
     def first_col_key(self, num_workers: int) -> int:
         return ((self.num_rows + num_workers - 1) // num_workers) * num_workers
@@ -150,7 +152,7 @@ class MatrixFactorization:
             ck = (torch.from_numpy(np.ascontiguousarray(j)) + self.fck).to(dev, non_blocking=True)
             mf_step(self.server, rk, ck, torch.from_numpy(np.ascontiguousarray(x)).to(dev, non_blocking=True),
                     torch.from_numpy(rn).to(dev, non_blocking=True), torch.from_numpy(cn).to(dev, non_blocking=True),
-                    cfg.rank, self.eps, cfg.lam, self.loss, self.stats)
+                    cfg.rank, self.eps, cfg.lam, self.loss, self.stats, deterministic=cfg.deterministic)
             self.step_no += 1
             return self.loss
         loss = mf_reference_step(self.worker, torch.from_numpy(i.astype(np.int64)),

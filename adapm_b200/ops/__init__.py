@@ -176,36 +176,51 @@ def _f32(t: torch.Tensor, name: str) -> torch.Tensor:
     return t
 
 
+def _check_deterministic(server, deterministic: bool) -> bool:
+    if deterministic and server.num_servers() > 1:
+        raise ValueError("deterministic=True needs a single-GPU server: on several GPUs rows move between ranks "
+                         "during the step")
+    return bool(deterministic)
+
+
 def kge_complex_step(server, subj: torch.Tensor, rel: torch.Tensor, obj: torch.Tensor, labels: torch.Tensor,
                      embed_dim: int, eta: float, gamma_entity: float, gamma_relation: float, loss: torch.Tensor,
                      stats: Optional[torch.Tensor] = None, dropout_entity: float = 0.0, dropout_relation: float = 0.0,
-                     seed: int = 0) -> None:
+                     seed: int = 0, deterministic: bool = False) -> None:
     """Fused ComplEx training calls: for every i, one Model::train(s[i], r[i], o[i], label[i]) of the
     reference (pull 3 rows, optional dropout on the pulled copies, score, BCE gradient, L2 on positives, AdaGrad,
-    push 3 rows). The dropout mask is ``kge_dropout_mask(seed, ...)``."""
+    push 3 rows). The dropout mask is ``kge_dropout_mask(seed, ...)``.
+
+    ``deterministic=True`` (single-GPU servers only, else ``ValueError``): every call reads the state at the start of
+    the step, the updates are summed in fixed point and applied once per row after the step, so that the same inputs
+    give bit-identical rows and loss in every run (three kernel launches instead of one). The default adds the updates
+    in place."""
     _i64(subj, "subj"); _i64(rel, "rel"); _i64(obj, "obj"); _f32(labels, "labels"); _f32(loss, "loss")
     n = subj.numel()
     if not (rel.numel() == n and obj.numel() == n and labels.numel() == n):
         raise ValueError("subj, rel, obj and labels must have the same length")
+    det = _check_deterministic(server, deterministic)
     _C.kge_complex_step(server._impl.backend_handle(), _stream(subj), subj.data_ptr(), rel.data_ptr(), obj.data_ptr(),
                         labels.data_ptr(), n, int(embed_dim), float(eta), float(gamma_entity), float(gamma_relation),
                         loss.data_ptr(), stats.data_ptr() if stats is not None else 0, float(dropout_entity),
-                        float(dropout_relation), int(seed) & 0xFFFFFFFFFFFFFFFF)
+                        float(dropout_relation), int(seed) & 0xFFFFFFFFFFFFFFFF, det)
 
 
 def kge_rescal_step(server, subj: torch.Tensor, rel: torch.Tensor, obj: torch.Tensor, labels: torch.Tensor,
                     embed_dim: int, eta: float, gamma_entity: float, gamma_relation: float, loss: torch.Tensor,
                     stats: Optional[torch.Tensor] = None, dropout_entity: float = 0.0, dropout_relation: float = 0.0,
-                    seed: int = 0) -> None:
-    """Fused RESCAL training calls (score s^T R o, rank-1 relation gradient; relation rows are 2*d*d floats)."""
+                    seed: int = 0, deterministic: bool = False) -> None:
+    """Fused RESCAL training calls (score s^T R o, rank-1 relation gradient; relation rows are 2*d*d floats).
+    ``deterministic``: as for :func:`kge_complex_step`."""
     _i64(subj, "subj"); _i64(rel, "rel"); _i64(obj, "obj"); _f32(labels, "labels"); _f32(loss, "loss")
     n = subj.numel()
     if not (rel.numel() == n and obj.numel() == n and labels.numel() == n):
         raise ValueError("subj, rel, obj and labels must have the same length")
+    det = _check_deterministic(server, deterministic)
     _C.kge_rescal_step(server._impl.backend_handle(), _stream(subj), subj.data_ptr(), rel.data_ptr(), obj.data_ptr(),
                        labels.data_ptr(), n, int(embed_dim), float(eta), float(gamma_entity), float(gamma_relation),
                        loss.data_ptr(), stats.data_ptr() if stats is not None else 0, float(dropout_entity),
-                       float(dropout_relation), int(seed) & 0xFFFFFFFFFFFFFFFF)
+                       float(dropout_relation), int(seed) & 0xFFFFFFFFFFFFFFFF, det)
 
 
 def _mix32(x: torch.Tensor) -> torch.Tensor:
@@ -236,16 +251,19 @@ def kge_dropout_mask(seed: int, n_calls: int, which: int, n_elems: int, p: float
 
 def mf_step(server, row_keys: torch.Tensor, col_keys: torch.Tensor, x: torch.Tensor, row_nnz: torch.Tensor,
             col_nnz: torch.Tensor, rank: int, eps: float, lam: float, loss: torch.Tensor,
-            stats: Optional[torch.Tensor] = None) -> None:
-    """Fused matrix-factorisation SGD/AdaGrad step over a batch of non-zeros (reference apps/mf/update.h)."""
+            stats: Optional[torch.Tensor] = None, deterministic: bool = False) -> None:
+    """Fused matrix-factorisation SGD/AdaGrad step over a batch of non-zeros (reference apps/mf/update.h).
+    ``deterministic``: as for :func:`kge_complex_step` (single-GPU servers only; the summed squared error is reduced in
+    a fixed order)."""
     _i64(row_keys, "row_keys"); _i64(col_keys, "col_keys"); _f32(x, "x"); _f32(loss, "loss")
     for t, nm in ((row_nnz, "row_nnz"), (col_nnz, "col_nnz")):
         if not (t.is_cuda and t.dtype == torch.int32 and t.is_contiguous()):
             raise TypeError(f"{nm} must be a contiguous CUDA int32 tensor")
     n = row_keys.numel()
+    det = _check_deterministic(server, deterministic)
     _C.mf_step(server._impl.backend_handle(), _stream(x), row_keys.data_ptr(), col_keys.data_ptr(), x.data_ptr(),
                row_nnz.data_ptr(), col_nnz.data_ptr(), n, int(rank), float(eps), float(lam), loss.data_ptr(),
-               stats.data_ptr() if stats is not None else 0)
+               stats.data_ptr() if stats is not None else 0, det)
 
 
 def _bf16_k8(t: torch.Tensor) -> torch.Tensor:
