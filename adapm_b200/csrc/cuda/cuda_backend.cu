@@ -224,153 +224,6 @@ __global__ void __launch_bounds__(kThreads) phase_scan_kernel(const __grid_const
   }
 }
 
-// ---- row pass on the TMA engine (float32 rows; opt-in: ADAPM_ROW_TMA=1): the rows of an operation travel as bulk copies
-//   global (local HBM or NVLink peer) --cp.async.bulk--> shared memory --(warp: LDS, subtract, STS)-->
-//   --cp.reduce.async.bulk.add.f32 / cp.async.bulk--> global
-// and every warp keeps kRowStages operations in flight in a ring of shared-memory stages, without occupying the
-// load / store slots of the SM. Next to the SGNS step this pass was measured to take longer than the register variant
-// (on the previous hardware target; not re-measured on H100) - the training kernel keeps the SM's TMA unit busy
-// (27 bulk loads + 27 bulk reductions per pair), so the round's bulk operations queue behind it, while the LSU path
-// it leaves alone is comparatively idle. Steps that overlap the pass were slightly faster and the end-to-end rate the
-// same within noise, but rounds that take three
-// times as long mean staler replicas, so the register variant stays the default.
-constexpr int kRowWarps = 2;        // warps per block
-constexpr int kRowStages = 3;       // operations in flight per warp
-__device__ __forceinline__ uint32_t rsm_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void rmbar_init(unsigned long long* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(rsm_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void rmbar_expect_tx(unsigned long long* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(rsm_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void rmbar_arrive(unsigned long long* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(rsm_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void rmbar_wait(unsigned long long* bar, uint32_t parity) {
-  const uint32_t addr = rsm_u32(bar);
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok) : "r"(addr), "r"(parity) : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ void rbulk_g2s(void* dst, const void* src, uint32_t bytes, unsigned long long* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(rsm_u32(dst)), "l"(src), "r"(bytes), "r"(rsm_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void rbulk_red_s2g(void* dst, const void* src, uint32_t bytes) {
-  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;"
-               ::"l"(dst), "r"(rsm_u32(src)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void rbulk_st_s2g(void* dst, const void* src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(rsm_u32(src)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool row_op_bulk_ok(const SlotWork& w) {
-  return (w.op == OP_SHIP || w.op == OP_REFRESH || w.op == OP_DROP) && (w.len & 3u) == 0 &&
-         ((((uintptr_t)w.dst) | ((uintptr_t)w.ref) | ((uintptr_t)w.src)) & 15u) == 0;
-}
-
-__global__ void __launch_bounds__(kRowWarps * 32, 10) phase_row_tma_kernel(const __grid_constant__ Ctx c,
-                                                                       const RoundDev* __restrict__ rd,
-                                                                       SlotWork* __restrict__ worklist,
-                                                                       const unsigned int* __restrict__ count,
-                                                                       uint32_t stage_floats) {
-  if (rd->stop) return;
-  extern __shared__ __align__(128) unsigned char row_smem[];
-  __shared__ unsigned long long bars[kRowWarps][kRowStages];
-  WarpGroup g;
-  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  const unsigned n = *count;
-  const unsigned warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const unsigned nwarps = (gridDim.x * blockDim.x) >> 5;
-  float* stage0 = reinterpret_cast<float*>(row_smem) + (size_t)wib * kRowStages * 2 * stage_floats;
-  if (lane == 0) {
-    for (int s = 0; s < kRowStages; ++s) rmbar_init(&bars[wib][s], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  __syncwarp();
-  const unsigned my_n = warp < n ? (n - warp + nwarps - 1) / nwarps : 0u;   // operations of this warp: warp + k * nwarps
-  auto issue = [&](unsigned k) {    // start the loads of my k-th operation into stage k % kRowStages (lane 0)
-    if (lane != 0) return;
-    const int st = (int)(k % kRowStages);
-    float* S = stage0 + (size_t)st * 2 * stage_floats;
-    float* R = S + stage_floats;
-    const SlotWork& w = worklist[warp + k * nwarps];
-    // the stage's previous user (operation k - kRowStages) committed its stores two groups ago at the latest
-    asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-    if (row_op_bulk_ok(w)) {
-      const uint32_t bytes = w.len * 4u;
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      rmbar_expect_tx(&bars[wib][st], 2u * bytes);
-      rbulk_g2s(S, w.src, bytes, &bars[wib][st]);      // SHIP / DROP: local row          REFRESH: owner row (NVLink)
-      rbulk_g2s(R, w.ref, bytes, &bars[wib][st]);      // local base row
-    } else {
-      rmbar_arrive(&bars[wib][st]);                    // nothing to load: register path below
-    }
-  };
-  for (unsigned k = 0; k + 1 < (unsigned)kRowStages && k < my_n; ++k) issue(k);
-  for (unsigned k = 0; k < my_n; ++k) {
-    const int st = (int)(k % kRowStages);
-    float* S = stage0 + (size_t)st * 2 * stage_floats;
-    float* R = S + stage_floats;
-    SlotWork& w = worklist[warp + k * nwarps];
-    rmbar_wait(&bars[wib][st], (k / kRowStages) & 1u);
-    if (w.op != OP_NONE) {
-      if (row_op_bulk_ok(w)) {
-        const uint32_t nv = w.len >> 2, bytes = w.len * 4u;
-        bool nz = false;
-        bool go = true;
-        if (w.op == OP_SHIP && w.thresh2 > 0.f) {     // ship only if the delta is large enough (sys.sync.threshold)
-          float a = 0.f;
-          for (uint32_t j = lane; j < nv; j += 32) {
-            const float4 s4 = reinterpret_cast<const float4*>(S)[j], r4 = reinterpret_cast<const float4*>(R)[j];
-            const float dx = s4.x - r4.x, dy = s4.y - r4.y, dz = s4.z - r4.z, dw = s4.w - r4.w;
-            a += dx * dx + dy * dy + dz * dz + dw * dw;
-          }
-          go = (float)g.sum((double)a) >= w.thresh2;
-        }
-        if (go) {
-          for (uint32_t j = lane; j < nv; j += 32) {   // R := S - R (the delta), S stays the new base
-            const float4 s4 = reinterpret_cast<const float4*>(S)[j];
-            float4 r4 = reinterpret_cast<const float4*>(R)[j];
-            r4.x = s4.x - r4.x; r4.y = s4.y - r4.y; r4.z = s4.z - r4.z; r4.w = s4.w - r4.w;
-            nz = nz || r4.x != 0.f || r4.y != 0.f || r4.z != 0.f || r4.w != 0.f;
-            reinterpret_cast<float4*>(R)[j] = r4;
-          }
-          nz = g.any(nz);
-        }
-        if (w.op == OP_DROP && go) {                  // the slot returns to the pool with all-zero rows: S := 0
-          for (uint32_t j = lane; j < nv; j += 32) reinterpret_cast<float4*>(S)[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // my stage writes -> the bulk stores below
-        __syncwarp();
-        if (lane == 0) {
-          if (w.op == OP_SHIP) {
-            if (nz) { rbulk_red_s2g(w.dst, R, bytes); rbulk_st_s2g(w.ref, S, bytes); w.flags |= W_NZ; }
-          } else if (w.op == OP_REFRESH) {
-            if (nz) { rbulk_red_s2g(w.dst, R, bytes); rbulk_st_s2g(w.ref, S, bytes); }
-          } else {   // OP_DROP: residual delta to the owner, then clear row and base
-            if (nz) { rbulk_red_s2g(w.dst, R, bytes); w.flags |= W_NZ; }
-            rbulk_st_s2g(const_cast<void*>(w.src), S, bytes);
-            rbulk_st_s2g(w.ref, S, bytes);
-          }
-        }
-      } else {
-        row_op_execute<float>(c, g, w);               // FINALIZE / CLEAR / odd shapes: register path
-      }
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.commit_group;" ::: "memory");   // exactly one group per operation
-    __syncwarp();
-    if (k + kRowStages - 1 < my_n) issue(k + kRowStages - 1);
-  }
-  if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");    // everything is performed before the commit pass
-  __syncwarp();
-}
-
 // resolve / commit: one thread per worklist entry (all the metadata work, including the NVLink metadata loads: a
 // thread-per-slot pass keeps as many of them in flight as there are entries). STEP 0 = resolve, 1 = commit.
 template <class Val, int PHASE, int STEP>
@@ -393,14 +246,12 @@ __global__ void __launch_bounds__(kThreads) phase_meta_kernel(const __grid_const
 // fits into the registers a lean training kernel (104 x 512) leaves free per SM, so the pass runs NEXT to the
 // training kernels instead of taking one of their two block slots.
 constexpr int kWorkThreads = 128;
-#ifndef ADAPM_WORK_MINB
-#define ADAPM_WORK_MINB 6   // <= 80 registers x 128 threads = 10 K of the 12 K registers a lean training kernel leaves free per SM
-#endif
+constexpr int kWorkMinBlocks = 6;   // <= 80 registers x 128 threads = 10 K of the 12 K registers a lean training kernel leaves free per SM
 template <class Val>
-__global__ void __launch_bounds__(kWorkThreads, ADAPM_WORK_MINB) phase_row_kernel(const __grid_constant__ Ctx c,
-                                                                               const RoundDev* __restrict__ rd,
-                                                                               SlotWork* __restrict__ worklist,
-                                                                               const unsigned int* __restrict__ count) {
+__global__ void __launch_bounds__(kWorkThreads, kWorkMinBlocks) phase_row_kernel(const __grid_constant__ Ctx c,
+                                                                              const RoundDev* __restrict__ rd,
+                                                                              SlotWork* __restrict__ worklist,
+                                                                              const unsigned int* __restrict__ count) {
   if (rd->stop) return;
   WarpGroup g;
   const unsigned n = *count;
@@ -564,9 +415,6 @@ CudaBackend::CudaBackend(const Options& opt, const Layout& L, std::shared_ptr<Fa
   ADAPM_CUDA_CHECK(cudaGetDeviceProperties(&prop, device_));
   num_sms_ = prop.multiProcessorCount;
   if (const char* e = getenv("ADAPM_SYNC_TRACE")) trace_on_ = atoi(e) != 0;
-  if (const char* e = getenv("ADAPM_SYNC_SCAN_BLOCKS")) scan_blocks_per_sm_ = std::max(1, atoi(e));
-  if (const char* e = getenv("ADAPM_SYNC_WORK_BLOCKS")) work_blocks_per_sm_ = std::max(1, atoi(e));
-  if (const char* e = getenv("ADAPM_SYNC_META_BLOCKS")) meta_blocks_per_sm_ = std::max(1, atoi(e));
   int lo = 0, hi = 0;
   ADAPM_CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
   ADAPM_CUDA_CHECK(cudaStreamCreateWithPriority(&sync_stream_, cudaStreamNonBlocking, hi));
@@ -980,36 +828,18 @@ void CudaBackend::register_intents(const IntentRec* recs, size_t n, const RoundP
   memcpy(status, st.host + o_st, n);
 }
 
-// The row pass of phase A / C: register variant by default; ADAPM_ROW_TMA=1 selects the TMA-engine variant for float32
-// rows whose staging fits into shared memory (measured slower next to the SGNS step, see phase_row_tma_kernel).
-void CudaBackend::launch_row_pass(unsigned int* wc) {
-  const Layout& L = ctx_.L;
-  uint32_t max_len = 0;
-  for (int k = 0; k < L.num_classes; ++k) max_len = std::max(max_len, L.cls[k].len);
-  const uint32_t stage_floats = (max_len + 31u) & ~31u;
-  const size_t smem = (size_t)kRowWarps * kRowStages * 2 * stage_floats * sizeof(float);
-  static const bool tma_env = [] { const char* e = getenv("ADAPM_ROW_TMA"); return e && atoi(e) != 0; }();
-  if (tma_env && L.val_bytes == 4 && !int_rows_ && smem <= 30 * 1024) {
-    phase_row_tma_kernel<<<num_sms_ * work_blocks_per_sm_, kRowWarps * 32, smem, sync_stream_>>>(ctx_, round_dev_, worklist_, wc,
-                                                                                               stage_floats);
-    return;
-  }
-  const int gw = num_sms_ * work_blocks_per_sm_;
-  ADAPM_DISPATCH_VAL(int_rows_, ctx_.L.val_bytes, phase_row_kernel<Val><<<gw, kWorkThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc));
-}
-
 void CudaBackend::launch_phase(int phase) {
   if (phase == 1) {
     unsigned int* wc = work_count_ + 2;
     ADAPM_CUDA_CHECK(cudaMemsetAsync(wc, 0, sizeof(unsigned int), sync_stream_));
     {
       TraceScope t_(this, "B.scan", sync_stream_);
-      phase_b_scan_kernel<<<num_sms_ * scan_blocks_per_sm_, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc);
+      phase_b_scan_kernel<<<num_sms_, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc);
     }
     // one thread per candidate: the grid is sized for the worst case seen so far (the count lives on the device)
     {
       TraceScope t_(this, "B.decide", sync_stream_);
-      phase_b_kernel<<<num_sms_ * meta_blocks_per_sm_ * 4, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc);
+      phase_b_kernel<<<num_sms_ * 4, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc);
     }
     ADAPM_COUNT_LAUNCH();
     ADAPM_COUNT_LAUNCH();
@@ -1018,32 +848,39 @@ void CudaBackend::launch_phase(int phase) {
   }
   unsigned int* wc = work_count_ + (phase == 0 ? 0 : 1);   // one counter per phase (read back by the kernel timeline)
   ADAPM_CUDA_CHECK(cudaMemsetAsync(wc, 0, sizeof(unsigned int), sync_stream_));
-  const int gs = num_sms_ * scan_blocks_per_sm_, gm = num_sms_ * meta_blocks_per_sm_;
   if (phase == 0) {
-    { TraceScope t_(this, "A.scan", sync_stream_); phase_scan_kernel<0><<<gs, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc); }
+    { TraceScope t_(this, "A.scan", sync_stream_); phase_scan_kernel<0><<<num_sms_, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc); }
     {
       TraceScope t_(this, "A.resolve", sync_stream_);
       ADAPM_DISPATCH_VAL(int_rows_, ctx_.L.val_bytes,
-                         phase_meta_kernel<Val, 0, 0><<<gm, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc));
+                         phase_meta_kernel<Val, 0, 0><<<num_sms_, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc));
     }
-    { TraceScope t_(this, "A.row", sync_stream_); launch_row_pass(wc); }
+    {
+      TraceScope t_(this, "A.row", sync_stream_);
+      ADAPM_DISPATCH_VAL(int_rows_, ctx_.L.val_bytes,
+                         phase_row_kernel<Val><<<num_sms_, kWorkThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc));
+    }
     {
       TraceScope t_(this, "A.commit", sync_stream_);
       ADAPM_DISPATCH_VAL(int_rows_, ctx_.L.val_bytes,
-                         phase_meta_kernel<Val, 0, 1><<<gm, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc));
+                         phase_meta_kernel<Val, 0, 1><<<num_sms_, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc));
     }
   } else {
-    { TraceScope t_(this, "C.scan", sync_stream_); phase_scan_kernel<1><<<gs, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc); }
+    { TraceScope t_(this, "C.scan", sync_stream_); phase_scan_kernel<1><<<num_sms_, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc); }
     {
       TraceScope t_(this, "C.resolve", sync_stream_);
       ADAPM_DISPATCH_VAL(int_rows_, ctx_.L.val_bytes,
-                         phase_meta_kernel<Val, 1, 0><<<gm, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc));
+                         phase_meta_kernel<Val, 1, 0><<<num_sms_, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc));
     }
-    { TraceScope t_(this, "C.row", sync_stream_); launch_row_pass(wc); }
+    {
+      TraceScope t_(this, "C.row", sync_stream_);
+      ADAPM_DISPATCH_VAL(int_rows_, ctx_.L.val_bytes,
+                         phase_row_kernel<Val><<<num_sms_, kWorkThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc));
+    }
     {
       TraceScope t_(this, "C.commit", sync_stream_);
       ADAPM_DISPATCH_VAL(int_rows_, ctx_.L.val_bytes,
-                         phase_meta_kernel<Val, 1, 1><<<gm, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc));
+                         phase_meta_kernel<Val, 1, 1><<<num_sms_, kThreads, 0, sync_stream_>>>(ctx_, round_dev_, worklist_, wc));
     }
   }
   for (int i = 0; i < 4; ++i) ADAPM_COUNT_LAUNCH();

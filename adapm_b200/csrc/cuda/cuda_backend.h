@@ -117,18 +117,15 @@ class CudaBackend : public Backend {
   Ctx ctx_;
   bool int_rows_ = false;   // Options::dtype == int64 (8-byte rows are float64 otherwise)
   int device_ = 0;
+  // The sync-round kernels run one block per SM. The round runs on a high-priority stream next to the training
+  // kernels: a small footprint lets it share the SMs with them instead of displacing them.
   int num_sms_ = 132;
-  // grid sizes of the sync-round kernels, in blocks per SM. The round runs on a high-priority stream next to the
-  // training kernels: a small footprint lets it share the SMs with them instead of displacing them.
   struct TraceRec { const char* name; cudaEvent_t a, b; };
   bool trace_on_ = false;        // ADAPM_SYNC_TRACE
   cudaEvent_t trace_base_ = nullptr;
   std::vector<TraceRec> trace_;
   std::vector<std::array<uint32_t, 3>> trace_counts_;
   std::mutex trace_mu_;
-  int scan_blocks_per_sm_ = 1;   // ADAPM_SYNC_SCAN_BLOCKS
-  int work_blocks_per_sm_ = 1;   // ADAPM_SYNC_WORK_BLOCKS (row pass: blocks of 128 threads)
-  int meta_blocks_per_sm_ = 1;   // ADAPM_SYNC_META_BLOCKS (resolve / commit passes: blocks of 256 threads)
   cudaStream_t sync_stream_ = nullptr;
   std::vector<cudaStream_t> worker_streams_;
   std::vector<std::unique_ptr<Staging>> staging_;  // per worker
@@ -144,7 +141,6 @@ class CudaBackend : public Backend {
   // device-resident round (default for world > 1; ADAPM_HOST_ROUND=1 selects the host-sequenced round)
   void upload_round(const RoundParams& rp, uint32_t n_recs, uint32_t flags);
   void launch_phase(int phase);   // 0 = A, 1 = B, 2 = C
-  void launch_row_pass(unsigned int* work_count);
   bool fused_round_ = false;
   RoundDev* round_dev_ = nullptr;      // device
   RoundDev* round_host_ = nullptr;     // pinned: [0] = upload staging, [1] = results

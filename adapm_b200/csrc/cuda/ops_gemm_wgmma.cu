@@ -18,7 +18,6 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cstdlib>
 
 #include "ops.h"
 #include "wgmma_utils.cuh"
@@ -104,15 +103,13 @@ void launch(cudaStream_t stream, const void* A, const void* B, int M, int N, int
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
   // split-K: few output tiles and a long K extent (e.g. the G^T E0 gradient GEMM of the shared-negative SGNS step:
   // 1024 x 304 x 32768 = 24 tiles) - spread the k-blocks of a tile over gridDim.z CTAs that add their partial tiles
-  // into the zeroed C. ADAPM_GEMM_SPLITK=<n> forces n splits (1 = off).
+  // into the zeroed C.
   if (EPI == EPI_STORE) {
-    static const int split_env = [] { const char* e = getenv("ADAPM_GEMM_SPLITK"); return e ? atoi(e) : 0; }();
     const int BKh = KIND == KIND_BF16 ? 64 : 128;
     const int total_kb = (K + BKh - 1) / BKh;
     const long tiles = (long)grid.x * grid.y;
     int splits = 1;
-    if (split_env > 0) splits = split_env;
-    else if (tiles * 2 <= num_sms && total_kb >= 32) splits = (int)std::min<long>(num_sms / tiles, total_kb / 8);
+    if (tiles * 2 <= num_sms && total_kb >= 32) splits = (int)std::min<long>(num_sms / tiles, total_kb / 8);
     splits = std::max(1, std::min(splits, std::min(total_kb, 64)));
     if (splits > 1) {
       const int kb_per = (total_kb + splits - 1) / splits;

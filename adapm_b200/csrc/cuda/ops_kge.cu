@@ -16,7 +16,6 @@
 // apply pass adds to the rows; each call's loss goes to its own slot and is summed in a fixed order.
 #include <cuda_runtime.h>
 
-#include <cstdlib>
 #include <map>
 #include <mutex>
 
@@ -155,8 +154,7 @@ __device__ __noinline__ float kge_call_generic(const Ctx& c, Key ks, Key kr, Key
 }
 
 // VPLH = float4 vectors per lane per half-embedding (nh/8 float4 per half); VPLH = 0 -> generic only
-// MAXREG = register budget (2 blocks of 256 threads per SM): 128 uses the whole register file; 104 leaves room for one
-// block of the sync-round kernels per SM (see ops_sgns_tma.cu). ADAPM_KGE_REGS=104 selects the lean variant.
+// The kernels run 2 blocks of 256 threads per SM at 128 registers, which use the whole register file.
 // FX: deterministic mode (kge_step_fx_kernel): start-of-step reads, fixed-point sums into fx_acc, call losses.
 template <int VPLH, bool FX>
 __device__ __forceinline__ void
@@ -291,8 +289,8 @@ kge_step_body(const Ctx& c, const Key* __restrict__ subj, const Key* __restrict_
   dev::cta_exit(c);
 }
 
-template <int VPLH, int MAXREG>
-__global__ void __maxnreg__(MAXREG)
+template <int VPLH>
+__global__ void __maxnreg__(128)
 kge_step_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, const Key* __restrict__ rel,
                 const Key* __restrict__ obj, const float* __restrict__ labels, int n_calls, int nh, float eta,
                 float gamma_e, float gamma_r, float* __restrict__ loss_out, unsigned long long* __restrict__ stats,
@@ -561,22 +559,15 @@ void kge_complex_step(CudaBackend& be, cudaStream_t stream, const Key* subj, con
   const int nvh = nh / 8;
   int vplh = (nh % 8 == 0) ? (nvh + 31) / 32 : 0;
   if (vplh > 2) vplh = 0;
-  static const int regs_env = [] { const char* e = getenv("ADAPM_KGE_REGS"); return e ? atoi(e) : 0; }();
-  const bool lean = regs_env > 0 && regs_env < 128;
-#define ADAPM_LAUNCH_KGE2(V, R)                                                                                 \
+#define ADAPM_LAUNCH_KGE(V)                                                                                    \
   do {                                                                                                         \
     static bool attr_set = false;                                                                              \
     if (!attr_set) {                                                                                           \
-      cudaFuncSetAttribute(kge_step_kernel<V, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);    \
+      cudaFuncSetAttribute(kge_step_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);       \
       attr_set = true;                                                                                         \
     }                                                                                                          \
-    kge_step_kernel<V, R><<<blocks, kThreads, smem, stream>>>(c, subj, rel, obj, labels, n_calls, nh, eta,     \
-                                                              gamma_e, gamma_r, loss_out, stats, de, dr);      \
-  } while (0)
-#define ADAPM_LAUNCH_KGE(V)              \
-  do {                                   \
-    if (lean) ADAPM_LAUNCH_KGE2(V, 104); \
-    else ADAPM_LAUNCH_KGE2(V, 128);      \
+    kge_step_kernel<V><<<blocks, kThreads, smem, stream>>>(c, subj, rel, obj, labels, n_calls, nh, eta,        \
+                                                           gamma_e, gamma_r, loss_out, stats, de, dr);         \
   } while (0)
 #define ADAPM_LAUNCH_KGE_FX(V)                                                                                 \
   do {                                                                                                         \

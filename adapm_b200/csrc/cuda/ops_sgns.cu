@@ -17,8 +17,6 @@
 // loads and 16-byte vector reductions (red.global.add.v4.f32).
 #include <cuda_runtime.h>
 
-#include <cstdlib>
-
 #include "ops.h"
 #include "pm_kernels.cuh"
 #include "sgns_common.cuh"
@@ -44,8 +42,9 @@ using dev::slow_pull;
 using dev::slow_push;
 
 // VPL = float4 vectors per lane covering d floats: VPL = ceil(d / 128)
-template <int VPL, int MINB>
-__global__ void __launch_bounds__(kThreads, MINB)
+// 2 blocks/SM: 128 registers and no spills (3 blocks/SM would cap the kernel at 80 registers, and it spills there)
+template <int VPL>
+__global__ void __launch_bounds__(kThreads, 2)
 sgns_step_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
                  const Key* __restrict__ negatives, int n_pairs, int neg, int d, float alpha,
                  float* __restrict__ loss_out, unsigned long long* __restrict__ stats) {
@@ -278,32 +277,26 @@ void sgns_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const K
   if (n_pairs == 0) return;
   ADAPM_CHECK(be.ctx().L.val_bytes == 4, "the fused ops need float32 rows (Options::dtype)");
   be.track_stream(stream);
-  static const int env_impl = [] { const char* e = getenv("ADAPM_SGNS_IMPL"); return e ? (e[0] == 't' ? 2 : 1) : 0; }();
-  if (impl == 0) impl = env_impl ? env_impl : 2;
-  if (impl == 2 && sgns_step_tma(be, stream, centers, contexts, negatives, n_pairs, neg, d, alpha, loss_out, stats)) return;
+  if ((impl == 0 || impl == 2) && sgns_step_tma(be, stream, centers, contexts, negatives, n_pairs, neg, d, alpha, loss_out, stats)) return;
   const int vpl = (d / 4 + 31) / 32;
   const int warps_per_block = kThreads / 32;
   int blocks = std::min((n_pairs + warps_per_block - 1) / warps_per_block, be.num_sms() * 8);
   size_t smem = (size_t)warps_per_block * 4 * d * sizeof(float);
-  // occupancy variant: 2 blocks/SM (128 regs, no spills) or 3 blocks/SM (80 regs, small spills)
-  static const int minb = [] { const char* e = getenv("ADAPM_SGNS_MINB"); return e ? atoi(e) : 2; }();
-#define ADAPM_LAUNCH_SGNS(V, M)                                                                          \
+#define ADAPM_LAUNCH_SGNS(V)                                                                             \
   do {                                                                                                   \
     static bool attr_set = false;                                                                        \
     if (!attr_set) {                                                                                     \
-      cudaFuncSetAttribute(sgns_step_kernel<V, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024); \
+      cudaFuncSetAttribute(sgns_step_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024); \
       attr_set = true;                                                                                   \
     }                                                                                                    \
-    sgns_step_kernel<V, M><<<blocks, kThreads, smem, stream>>>(c, centers, contexts, negatives, n_pairs, neg, d, \
-                                                              alpha, loss_out, stats);                  \
+    sgns_step_kernel<V><<<blocks, kThreads, smem, stream>>>(c, centers, contexts, negatives, n_pairs, neg, d, \
+                                                           alpha, loss_out, stats);                     \
   } while (0)
-#define ADAPM_LAUNCH_SGNS_V(V) \
-  do { if (minb >= 3) ADAPM_LAUNCH_SGNS(V, 3); else ADAPM_LAUNCH_SGNS(V, 2); } while (0)
   switch (vpl) {
-    case 1: ADAPM_LAUNCH_SGNS_V(1); break;
-    case 2: ADAPM_LAUNCH_SGNS_V(2); break;
-    case 3: ADAPM_LAUNCH_SGNS_V(3); break;
-    default: ADAPM_LAUNCH_SGNS_V(4); break;
+    case 1: ADAPM_LAUNCH_SGNS(1); break;
+    case 2: ADAPM_LAUNCH_SGNS(2); break;
+    case 3: ADAPM_LAUNCH_SGNS(3); break;
+    default: ADAPM_LAUNCH_SGNS(4); break;
   }
   ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cudaGetLastError());

@@ -5,10 +5,12 @@
 // Why: the LDG variant keeps one target (2 x 1200 B per warp) in flight per warp and is register
 // limited to 16 warps/SM -> ~48 KB in flight per SM, latency bound (ncu: DRAM 42 %, L2 49 %).
 // Here rows never occupy registers while in flight: 16 warps/SM x RING (4) rows x 2400 B = 150 KB per SM.
-//   lane 0      : mbarrier.arrive.expect_tx + cp.async.bulk (UBLKCP) for target t + RING
+//   lane 0      : mbarrier.arrive.expect_tx + cp.async.bulk (UBLKCP) for target t + RING - 1
 //   whole warp  : mbarrier.try_wait, LDS.128 the row from shared memory, dot / sigmoid / AdaGrad,
-//                 RED.128 the update to the row's home (local HBM or NVLink peer)
-// Rows that live on a peer GPU are staged with ordinary 16-byte loads into the same ring slot;
+//                 the update overwrites the consumed ring slot
+//   lane 0      : cp.reduce.async.bulk (UBLKRED) of that slot into the row's home (local HBM or NVLink peer)
+// (The deterministic one-GPU kernel adds its updates to fixed-point accumulators instead and prefetches RING targets.)
+// The TMA engine reads rows that live on a peer GPU through their NVLink-mapped addresses as well;
 // rows in a transitional protocol state take the generic out-of-line path.
 #include <cuda_runtime.h>
 
@@ -97,18 +99,19 @@ struct WarpSmem {
 // (A variant that summed rows whose relocation to this rank is in flight inside the kernel - local row + source row -
 // instead of taking the out-of-line generic path for them was measured on 2 GPUs and removed: no gain, 2 x the
 // instantiations.)
-// BULK (ADAPM_SGNS_BULKRED=1): the updates of a target leave as ONE TMA bulk reduction per row: the warp overwrites the
-// consumed ring slot with [embedding update | AdaGrad update] and lane 0 issues cp.reduce.async.bulk from it; the slot is
-// reloaded one target later, after the reduction has read it (prefetch distance RING - 1).
+// In place (BULK): the updates of a target leave as ONE TMA bulk reduction per row: the warp overwrites the consumed ring
+// slot with [embedding update | AdaGrad update] and lane 0 issues cp.reduce.async.bulk from it; the slot is reloaded one
+// target later, after the reduction has read it (prefetch distance RING - 1).
 // FX: deterministic one-GPU variant (fixed-point accumulation, see kFxEmb); instantiated as its own kernel
 // (sgns_step_tma_fx_kernel) so that the in-place variants keep their register allocation.
-template <int VPL, bool BULK, bool FX>
+template <int VPL, bool FX>
 __device__ __forceinline__ void
 sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
                    const Key* __restrict__ negatives, int n_pairs, int neg, int d, float alpha,
-                   float* __restrict__ loss_out, unsigned long long* __restrict__ stats, int tma_remote,
+                   float* __restrict__ loss_out, unsigned long long* __restrict__ stats,
                    long long* __restrict__ fx_acc, const int* __restrict__ fx_cidx,
                    unsigned long long* __restrict__ fx_loss) {
+  constexpr bool BULK = !FX;
   // per warp: RING row buffers of 2*d floats (16-byte aligned) | generic-path scratch is carved from the ring
   extern __shared__ __align__(128) unsigned char smem_raw[];
   __shared__ WarpSmem wsm[kWarps];
@@ -143,16 +146,15 @@ sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __r
     // version counter (owned row) and the dirty byte (replica), so one pointer + a kind bit hold it (frees registers)
     float* my_row = nullptr;
     void* my_mark = nullptr;
-    int my_bits = 0;                     // bit 0: the row lives on a peer GPU, bit 1: my_mark is a replica dirty byte,
+    int my_bits = 0;                     // bit 1: my_mark is a replica dirty byte,
                                          // bits 2..: the key's accumulator row (deterministic mode)
     if (lane == 0) my_key = ckey;
     else if (lane - 1 < n_targets) my_key = (lane == 1) ? pos_key : negatives[(size_t)p * neg + (lane - 2)];
     if (my_key >= 0) {
-      unsigned r0 = n_remote;
       const Target tg = dev::resolve_fast(c, my_key, 0, &n_local, &n_remote);
       my_row = tg.row;
       my_mark = tg.flag ? (void*)tg.flag : (void*)tg.version;
-      my_bits = ((n_remote != r0) ? 1 : 0) | (tg.flag ? 2 : 0) | (FX ? __ldg(fx_cidx + my_key) << 2 : 0);
+      my_bits = (tg.flag ? 2 : 0) | (FX ? __ldg(fx_cidx + my_key) << 2 : 0);
     }
     // target t (0-based) -> lane t+1 (only pairs with <= 31 targets use this kernel)
     auto issue = [&](int t) {
@@ -160,24 +162,15 @@ sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __r
       float* buf = ring + (size_t)b * buf_floats;
       const Key tkey = (Key)__shfl_sync(0xffffffffu, (unsigned long long)my_key, t + 1);
       float* row = (float*)__shfl_sync(0xffffffffu, (unsigned long long)my_row, t + 1);
-      const int remote = __shfl_sync(0xffffffffu, my_bits, t + 1) & 1;
       const bool skip = (t > 0 && tkey == pos_key) || row == nullptr;
       if (skip) {
         if (lane == 0) mbar_arrive(&bars[b]);            // nothing to load: complete the phase
-      } else if (!remote || tma_remote) {
+      } else if (lane == 0) {
         // local HBM row - or a peer's row: the TMA engine reads NVLink-mapped addresses as well
-        if (lane == 0) {
-          if (BULK) bulk_wait_read<1>();   // the reduction that used this slot (issued one target ago) has read it
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // order earlier LDS of this slot before the TMA write
-          mbar_expect_tx(&bars[b], row_bytes);
-          bulk_g2s(buf, row, row_bytes, &bars[b]);
-        }
-      } else {
-        // NVLink peer row staged with 16-byte loads (ADAPM_TMA_REMOTE=0)
-        if (BULK) { if (lane == 0) bulk_wait_read<1>(); __syncwarp(); }
-        for (int j = lane; j < 2 * nvec; j += 32) reinterpret_cast<float4*>(buf)[j] = dev::ld_row4(row + 4 * j);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars[b]);
+        if (BULK) bulk_wait_read<1>();   // the reduction that used this slot (issued one target ago) has read it
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // order earlier LDS of this slot before the TMA write
+        mbar_expect_tx(&bars[b], row_bytes);
+        bulk_g2s(buf, row, row_bytes, &bars[b]);
       }
       ++issued;
     };
@@ -282,16 +275,13 @@ sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __r
             if (FX) {                     // deterministic mode: fixed-point sums, applied after the step
               add4(fx_t, j, nvec, ue, kFxEmb);
               add4(fx_t + d, j, nvec, ua, kFxAda);
-            } else if (BULK) {            // stage the update in place of the consumed row
+            } else {                      // stage the update in place of the consumed row
               reinterpret_cast<float4*>(buf)[j] = ue;
               reinterpret_cast<float4*>(buf + d)[j] = ua;
-            } else {
-              dev::red_row4(t_row + 4 * j, ue);
-              dev::red_row4(t_row + d + 4 * j, ua);
             }
           }
         }
-        if (BULK && !FX) {
+        if (BULK) {
           __syncwarp();
           if (lane == 0) {
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the staged update is visible to the TMA engine
@@ -358,16 +348,13 @@ sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __r
           if (FX) {
             add4(fx_c, j, nvec, ue, kFxEmb);
             add4(fx_c + d, j, nvec, ua, kFxAda);
-          } else if (BULK) {
+          } else {
             reinterpret_cast<float4*>(scratch)[j] = ue;
             reinterpret_cast<float4*>(scratch + d)[j] = ua;
-          } else {
-            dev::red_row4(c_row + 4 * j, ue);
-            dev::red_row4(c_row + d + 4 * j, ua);
           }
         }
       }
-      if (BULK && !FX) {
+      if (BULK) {
         __syncwarp();
         if (lane == 0) {
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -400,13 +387,13 @@ sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __r
   dev::cta_exit(c);
 }
 
-template <int VPL, int MAXREG, bool BULK>
+template <int VPL, int MAXREG>
 __global__ void __maxnreg__(MAXREG)
 sgns_step_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
                      const Key* __restrict__ negatives, int n_pairs, int neg, int d, float alpha,
-                     float* __restrict__ loss_out, unsigned long long* __restrict__ stats, int tma_remote) {
-  sgns_step_tma_body<VPL, BULK, false>(c, centers, contexts, negatives, n_pairs, neg, d, alpha, loss_out, stats,
-                                       tma_remote, nullptr, nullptr, nullptr);
+                     float* __restrict__ loss_out, unsigned long long* __restrict__ stats) {
+  sgns_step_tma_body<VPL, false>(c, centers, contexts, negatives, n_pairs, neg, d, alpha, loss_out, stats, nullptr,
+                                 nullptr, nullptr);
 }
 
 template <int VPL>
@@ -415,8 +402,8 @@ sgns_step_tma_fx_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ c
                         const Key* __restrict__ negatives, int n_pairs, int neg, int d, float alpha,
                         unsigned long long* __restrict__ stats, long long* __restrict__ fx_acc,
                         const int* __restrict__ fx_cidx, unsigned long long* __restrict__ fx_loss) {
-  sgns_step_tma_body<VPL, false, true>(c, centers, contexts, negatives, n_pairs, neg, d, alpha, nullptr, stats, 1,
-                                       fx_acc, fx_cidx, fx_loss);
+  sgns_step_tma_body<VPL, true>(c, centers, contexts, negatives, n_pairs, neg, d, alpha, nullptr, stats, fx_acc, fx_cidx,
+                                fx_loss);
 }
 
 }  // namespace
@@ -435,15 +422,12 @@ bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   const size_t smem = (size_t)warps * (RING + 1) * buf_floats * sizeof(float) + 128;
   if (smem > 110 * 1024) return false;  // keep 2 blocks per SM
   int blocks = std::min((n_pairs + warps - 1) / warps, be.num_sms() * 12);
-  static const int tma_remote = [] { const char* e = getenv("ADAPM_TMA_REMOTE"); return e ? atoi(e) : 1; }();
-  // register budget: 128 (single GPU: nothing to share the SMs with) or 104 (multi GPU); ADAPM_SGNS_REGS overrides
-  static const int regs_env = [] { const char* e = getenv("ADAPM_SGNS_REGS"); return e ? atoi(e) : 0; }();
-  const bool lean = regs_env ? (regs_env < 128) : (c.L.world > 1);
-  // TMA bulk reductions are the default (measured +2.6 % on one GPU, and the warp's LSU slots stay free for the sync
-  // round's kernels); ADAPM_SGNS_BULKRED=0 selects the RED.128 variants. (A software-pipelined target loop - score of
-  // target t+1 during the update of target t - was measured too: no gain at 128 registers, -5 % at 104: the kernel is
-  // not bound by the per-warp dependency chain.)
-  static const bool bulk = [] { const char* e = getenv("ADAPM_SGNS_BULKRED"); return !e || atoi(e) != 0; }();
+  // register budget: 128 (single GPU: nothing to share the SMs with) or 104 (multi GPU)
+  const bool lean = c.L.world > 1;
+  // In-place updates leave as TMA bulk reductions: measured +2.6 % on one GPU against RED.128 from the warp, and the
+  // warp's LSU slots stay free for the sync round's kernels. (A software-pipelined target loop - score of target t+1
+  // during the update of target t - was measured too: no gain at 128 registers, -5 % at 104: the kernel is not bound by
+  // the per-warp dependency chain.)
   // One GPU: deterministic step (fixed-point accumulation + apply pass), so that the same inputs give the same rows
   // and loss in every run; ADAPM_SGNS_DETERMINISTIC=0 selects in-place (Hogwild) updates. Several GPUs: rows move
   // between ranks during the step and are updated in place.
@@ -458,22 +442,20 @@ bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   long long* fx_acc = fxs ? fxs->acc : nullptr;
   const int* fx_cidx = fxs ? fxs->cidx : nullptr;
   unsigned long long* fx_loss = fxs ? fxs->loss : nullptr;
-#define ADAPM_LAUNCH_TMA3(V, T, B)                                                                              \
+#define ADAPM_LAUNCH_TMA2(V, R)                                                                                 \
   do {                                                                                                          \
     static bool attr_set = false;                                                                               \
     if (!attr_set) {                                                                                            \
-      cudaFuncSetAttribute(sgns_step_tma_kernel<V, T, B>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024); \
+      cudaFuncSetAttribute(sgns_step_tma_kernel<V, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);  \
       attr_set = true;                                                                                          \
     }                                                                                                           \
-    sgns_step_tma_kernel<V, T, B><<<blocks, threads, smem, stream>>>(c, centers, contexts, negatives, n_pairs, neg, \
-                                                                        d, alpha, loss_out, stats, tma_remote);   \
+    sgns_step_tma_kernel<V, R><<<blocks, threads, smem, stream>>>(c, centers, contexts, negatives, n_pairs, neg, d, \
+                                                                  alpha, loss_out, stats);                      \
   } while (0)
-#define ADAPM_LAUNCH_TMA(V)                                              \
-  do {                                                                   \
-    if (bulk && lean) ADAPM_LAUNCH_TMA3(V, 104, true);                   \
-    else if (bulk) ADAPM_LAUNCH_TMA3(V, 128, true);                      \
-    else if (lean) ADAPM_LAUNCH_TMA3(V, 104, false);                     \
-    else ADAPM_LAUNCH_TMA3(V, 128, false);                               \
+#define ADAPM_LAUNCH_TMA(V)              \
+  do {                                   \
+    if (lean) ADAPM_LAUNCH_TMA2(V, 104); \
+    else ADAPM_LAUNCH_TMA2(V, 128);      \
   } while (0)
 #define ADAPM_LAUNCH_TMA_FX(V)                                                                                  \
   do {                                                                                                          \

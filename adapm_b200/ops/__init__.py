@@ -32,7 +32,7 @@ def sgns_step(server, centers: torch.Tensor, contexts: torch.Tensor, negatives: 
     ``loss``: float32[1] accumulated (+=) with the summed logistic loss;
     ``stats``: optional int64[4] accumulated with (local rows, remote rows, slow-path rows, updates).
     ``impl``: ``tma`` (rows prefetched by the TMA engine into a shared-memory ring), ``ldg`` (register
-    variant) or ``auto`` (tma when the shape fits, else ldg; ``ADAPM_SGNS_IMPL`` overrides).
+    variant) or ``auto`` (tma when the shape fits, else ldg).
     """
     _i64(centers, "centers"); _i64(contexts, "contexts"); _i64(negatives, "negatives")
     B = centers.numel()

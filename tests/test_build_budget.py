@@ -32,28 +32,26 @@ def _kernels():
     return out
 
 
-def test_hot_kernels_stay_within_their_register_budget():
+def test_hot_kernel_instantiations_stay_within_their_register_budget():
     k = _kernels()
     if not k:
         pytest.skip("no ptxas logs (extension was not built in-tree)")
     # full-register variants of the fused steps: 2 blocks x 256 threads x 128 registers = the register file, no spills
-    # (sgns_step_tma_kernel<VPL, MAXREG, BULK>: the bulk-reduction variant is the default)
-    for name in ("sgns_step_tma_kernel<3, 128, true>", "sgns_step_tma_kernel<2, 128, true>",
-                 "sgns_step_tma_kernel<1, 128, true>",
-                 "sgns_step_kernel<3, 2>", "kge_step_kernel<2, 128>", "kge_step_kernel<2, 104>", "mf_step_kernel<1>"):
+    # (sgns_step_tma_kernel<VPL, MAXREG>)
+    for name in ("sgns_step_tma_kernel<3, 128>", "sgns_step_tma_kernel<2, 128>", "sgns_step_tma_kernel<1, 128>",
+                 "sgns_step_kernel<3>", "kge_step_kernel<2>", "mf_step_kernel<1>"):
         assert name in k, sorted(k)
         assert k[name]["regs"] <= 128 and k[name]["spill"] == 0, (name, k[name])
     # lean multi-GPU variant: 104 registers leave 12 K registers per SM for one block of the round kernels
-    lean = k["sgns_step_tma_kernel<3, 104, true>"]
+    lean = k["sgns_step_tma_kernel<3, 104>"]
     assert lean["regs"] <= 104 and lean["spill"] <= 256, lean
     # the round's kernels must fit NEXT to two lean training blocks: meta passes (128-thread blocks, no spills) and
-    # the row passes (register variant: 128 threads, TMA-engine variant: 64 threads)
+    # the row pass (128 threads)
     room = 65536 - 2 * 256 * 104
     for name, v in k.items():
         if name.startswith(("phase_meta_kernel", "phase_scan_kernel", "phase_b_")):
             assert v["regs"] * 128 <= room and v["spill"] == 0, (name, v)
     assert k["phase_row_kernel<float>"]["regs"] * 128 <= room, k["phase_row_kernel<float>"]
-    assert k["phase_row_tma_kernel"]["regs"] * 64 <= room, k["phase_row_tma_kernel"]
     # tensor-core kernels: no spills, enough room for 1 CTA/SM with large smem tiles
     for name, v in k.items():
         if name.startswith(("gemm_nt_wgmma", "gather_gemm_kernel")):
