@@ -475,6 +475,18 @@ CudaBackend::FxScratch& CudaBackend::fx_scratch(size_t acc_len, size_t rows, siz
   return fx_;
 }
 
+void* CudaBackend::step_buffer(int i, size_t bytes) {
+  auto& b = step_bufs_.at((size_t)i);
+  if (bytes > b.second) {
+    use_device();
+    if (b.first) ADAPM_CUDA_CHECK(cudaFree(b.first));
+    ADAPM_CUDA_CHECK(cudaMalloc(&b.first, bytes));
+    ADAPM_CUDA_CHECK(cudaMemset(b.first, 0, bytes));
+    b.second = bytes;
+  }
+  return b.first;
+}
+
 size_t CudaBackend::keys_with_len(uint32_t len) {
   if (key_len_.empty()) return (size_t)ctx_.L.num_keys;
   if (keys_by_len_.empty())
@@ -505,6 +517,7 @@ CudaBackend::~CudaBackend() {
   if (fx_.call_loss) cudaFree(fx_.call_loss);
   if (fx_.count) cudaFree(fx_.count);
   if (fx_.loss) cudaFree(fx_.loss);
+  for (auto& b : step_bufs_) if (b.first) cudaFree(b.first);
   if (round_done_) cudaEventDestroy(round_done_);
   for (auto& kv : tickets_) cudaEventDestroy(kv.second);
   for (auto e : event_pool_) cudaEventDestroy(e);

@@ -92,6 +92,10 @@ class CudaBackend : public Backend {
   FxScratch& fx_scratch(size_t acc_len, size_t rows, size_t calls);
   // number of keys whose rows have `len` values (every key for a store of one row length)
   size_t keys_with_len(uint32_t len);
+  // device buffer i (< kStepBuffers) of at least `bytes`, grown on demand and zero-filled when it grows (a buffer that
+  // its user leaves zero stays zero); scratch of the deterministic one-GPU SGNS step (ops_sgns_tma.cu)
+  static constexpr int kStepBuffers = 12;
+  void* step_buffer(int i, size_t bytes);
 
   // ---- kernel timeline: CUDA events around every sync-round kernel plus user marks, all relative to one base
   // event, so that the round's kernels and the training kernels of other streams land on one time axis
@@ -155,6 +159,7 @@ class CudaBackend : public Backend {
   unsigned long long dev_timeout_ns_ = 20ull * 1000000000ull;
   std::vector<uint32_t> key_len_;   // host mirror of per-key lengths (mixed-length stores only)
   FxScratch fx_;
+  std::array<std::pair<void*, size_t>, kStepBuffers> step_bufs_{};
   std::unordered_map<uint32_t, size_t> keys_by_len_;   // keys_with_len cache (mixed-length stores)
 };
 

@@ -1,4 +1,5 @@
-// Deterministic accumulation of the fused training steps on one GPU (SGNS, ComplEx, RESCAL, MF).
+// Deterministic accumulation of the fused training steps on one GPU (ComplEx, RESCAL, MF). The SGNS step groups its
+// contributions by key instead (ops_sgns_tma.cu) and shares only FxScratch's key map, id list, counters and loss word.
 //
 // A deterministic step adds its updates as 64-bit fixed-point integers into an accumulator region per key touched by
 // the step instead of into the store rows, so every call reads only start-of-step values and the sums do not depend on
