@@ -66,6 +66,20 @@ void gather_gemm(CudaBackend& be, cudaStream_t stream, const void* Q, const Key*
 void gather_gemm_rank_count(CudaBackend& be, cudaStream_t stream, const void* Q, const Key* keys, int M, int N, int K, int ldq,
                             const float* true_score, const int* true_col, int* rank_out, unsigned long long* stats);
 
+// top-k retrieval on the tensor cores (ops_topk.cu): per query row the k best columns of Q x E^T (fp32 wgmma scores,
+// times col_scale[j] when given; score descending, ties to the smaller column; columns in the row's CSR exclusion list
+// ex_cols[ex_off[i] .. ex_off[i+1]) skipped; (-inf, -1) padding). The tile kernels write sorted partial lists of S
+// N-slices into part_v / part_c [M, S, k]; a merge kernel writes out_v [M, k] and out_i [M, k].
+constexpr int kTopkMax = 64;
+int topk_num_slices(int M, int N, int max_tiles_per_cta);   // S for the grid; max_tiles_per_cta <= 0: unbounded
+void gemm_nt_topk(cudaStream_t stream, const void* A, const void* B, int M, int N, int K, int k, int S,
+                  const float* col_scale, const int64_t* ex_off, const int64_t* ex_cols, float* part_v, int* part_c,
+                  float* out_v, int64_t* out_i);
+// the same with E = rows(keys[0..N))[0..K) gathered from the parameter store (as gather_gemm); out_i are positions in keys
+void gather_gemm_topk(CudaBackend& be, cudaStream_t stream, const void* Q, const Key* keys, int M, int N, int K, int ldq,
+                      int k, int S, const float* col_scale, const int64_t* ex_off, const int64_t* ex_cols, float* part_v,
+                      int* part_c, float* out_v, int64_t* out_i, unsigned long long* stats);
+
 // Native step driver of the word2vec SGNS loop (ops_train_loop.cu)
 struct SgnsLoopConfig {
   int batch_pairs = 0, negative = 0, embed_dim = 0, read_ahead = 0, max_inflight = 3, rank = 0;

@@ -84,6 +84,22 @@ void bind(py::module_& m) {
     gather_gemm_rank_count(backend_of(be), (cudaStream_t)stream, ptr<const void>(Q), ptr<const Key>(keys), M, N, K, ldq,
                            ptr<const float>(ts), ptr<const int>(tc), ptr<int>(rank), ptr<unsigned long long>(stats));
   });
+  m.attr("topk_max_k") = kTopkMax;
+  m.def("topk_num_slices", [](int M, int N, int max_tiles_per_cta) { return topk_num_slices(M, N, max_tiles_per_cta); });
+  m.def("gemm_nt_topk", [](uintptr_t stream, uintptr_t A, uintptr_t B, int M, int N, int K, int k, int S, uintptr_t col_scale,
+                           uintptr_t ex_off, uintptr_t ex_cols, uintptr_t part_v, uintptr_t part_c, uintptr_t out_v,
+                           uintptr_t out_i) {
+    gemm_nt_topk((cudaStream_t)stream, ptr<const void>(A), ptr<const void>(B), M, N, K, k, S, ptr<const float>(col_scale),
+                 ptr<const int64_t>(ex_off), ptr<const int64_t>(ex_cols), ptr<float>(part_v), ptr<int>(part_c),
+                 ptr<float>(out_v), ptr<int64_t>(out_i));
+  });
+  m.def("gather_gemm_topk", [](uintptr_t be, uintptr_t stream, uintptr_t Q, uintptr_t keys, int M, int N, int K, int ldq,
+                               int k, int S, uintptr_t col_scale, uintptr_t ex_off, uintptr_t ex_cols, uintptr_t part_v,
+                               uintptr_t part_c, uintptr_t out_v, uintptr_t out_i, uintptr_t stats) {
+    gather_gemm_topk(backend_of(be), (cudaStream_t)stream, ptr<const void>(Q), ptr<const Key>(keys), M, N, K, ldq, k, S,
+                     ptr<const float>(col_scale), ptr<const int64_t>(ex_off), ptr<const int64_t>(ex_cols), ptr<float>(part_v),
+                     ptr<int>(part_c), ptr<float>(out_v), ptr<int64_t>(out_i), ptr<unsigned long long>(stats));
+  });
   py::class_<SgnsLoop>(m, "SgnsLoop")
       .def(py::init([](uintptr_t worker, uintptr_t be, int batch_pairs, int negative, int embed_dim, int read_ahead,
                        int max_inflight, int rank, bool signal_intent, bool local_only, int64_t model_seed, int sampler_kind,

@@ -392,6 +392,83 @@ class KGE:
         kv.barrier()
         return self._finish_metrics(row[:19].double(), N)
 
+    # ------------------------------------------------------------------ link prediction
+    def _query(self, ent_rows: torch.Tensor, rel_rows: torch.Tensor, side: str) -> torch.Tensor:
+        """The query vector of ``rank_triples``: score(candidate) = <q, E[candidate]>."""
+        if self.cfg.algorithm == "ComplEx":
+            return complex_query(ent_rows, rel_rows, conj=(side == "subject"))
+        Rm = rel_rows.reshape(-1, self.cfg.embed_dim, self.cfg.embed_dim)
+        if side == "object":
+            return torch.einsum("bi,bij->bj", ent_rows, Rm)
+        return torch.einsum("bij,bj->bi", Rm, ent_rows)
+
+    def _known_answers(self, ents: torch.Tensor, rels: torch.Tensor, side: str, known: torch.Tensor):
+        """CSR ``(offsets [n + 1], cols)`` of the known answers of each query, ascending per row."""
+        ne, nr = self.cfg.num_entities, self.cfg.num_relations
+        dev = ents.device
+        known = torch.as_tensor(known, dtype=torch.int64).to(dev).view(-1, 3)
+        given, ans = (known[:, 0], known[:, 2]) if side == "object" else (known[:, 2], known[:, 0])
+        comp = torch.unique((given * nr + known[:, 1]) * ne + ans)        # sorted (query, answer) pairs, no duplicates
+        qkey = (ents * nr + rels) * ne
+        lo = torch.searchsorted(comp, qkey)
+        cnt = torch.searchsorted(comp, qkey + ne) - lo
+        offsets = torch.zeros(ents.numel() + 1, dtype=torch.int64, device=dev)
+        offsets[1:] = torch.cumsum(cnt, 0)
+        rows = torch.repeat_interleave(torch.arange(ents.numel(), device=dev), cnt)
+        pos = torch.arange(rows.numel(), device=dev) - offsets[:-1][rows] + lo[rows]
+        return offsets, comp[pos] % ne
+
+    def predict(self, entities, relations, side: str = "object", k: int = 10, known=None):
+        """The ``k`` most likely completions of each query: objects of ``(entities[i], relations[i], ?)`` for
+        ``side="object"``, subjects of ``(?, relations[i], entities[i])`` for ``side="subject"``.
+
+        Returns ``(entity ids int64 [n, k], scores float32 [n, k])``, best first; equal scores go to the smaller entity
+        id. ``known``: triples [m, 3] (e.g. train + valid + test); every known answer of a query is left out (the
+        filtered setting). A query with fewer than ``k`` candidates left is padded with ``(-1, -inf)``.
+        ``1 <= k <= 64``. The query vector is the one of ``rank_triples``.
+
+        CUDA backend (float32 rows): only the rows of the queries are pulled; the scores against all entities are
+        computed from bf16-rounded operands in the fused gather + top-k kernel (``ops.gather_gemm_topk``), which reads
+        the entity rows wherever they live, on any number of GPUs. CPU backend: fp32 PyTorch over ``pull_embeddings()``
+        with the same order (``ops.topk_reference``)."""
+        if side not in ("object", "subject"):
+            raise ValueError(f"side must be 'object' or 'subject', got {side!r}")
+        cfg = self.cfg
+        d, ne = cfg.embed_dim, cfg.num_entities
+        ents = torch.as_tensor(entities, dtype=torch.int64).reshape(-1)
+        rels = torch.as_tensor(relations, dtype=torch.int64).reshape(-1)
+        if ents.numel() != rels.numel():
+            raise ValueError("entities and relations must have the same length")
+        if self.cuda:
+            from ..ops import gather_gemm_topk
+
+            dev, kv = self.server.device, self.worker
+            ents, rels = ents.to(dev), rels.to(dev)
+
+            def pull_rows(keys, ln):
+                buf = torch.empty(keys.numel() * ln, dtype=torch.float32, device=dev)
+                kv.wait(kv.pull(keys.contiguous(), buf, True))
+                return buf.view(-1, ln)[:, : ln // 2]
+
+            q = self._query(pull_rows(ents, cfg.entity_len), pull_rows(rels + ne, cfg.relation_len), side)
+            excl = self._known_answers(ents, rels, side, known) if known is not None else None
+            vals, idx = gather_gemm_topk(self.server, q, torch.arange(ne, dtype=torch.int64, device=dev), d, k,
+                                         exclude=excl)
+            return idx, vals
+        from ..ops import _check_topk, topk_reference
+
+        _check_topk(ents.numel(), ne, k, None, None)
+        E, _, R, _ = self.pull_embeddings()
+        E, R = E.float(), R.float()
+        q = self._query(E[ents], R[rels], side)
+        excluded = None
+        if known is not None:
+            off, cols = self._known_answers(ents, rels, side, known)
+            excluded = torch.zeros(ents.numel(), ne, dtype=torch.bool)
+            excluded[torch.repeat_interleave(torch.arange(ents.numel()), off[1:] - off[:-1]), cols] = True
+        vals, idx = topk_reference(q @ E.t(), int(k), excluded)
+        return idx, vals
+
 
 def complex_query(a: torch.Tensor, r: torch.Tensor, conj: bool) -> torch.Tensor:
     """Query vector q such that score(s, r, e) = <q, E[e]> for all e (object side), or the subject-side

@@ -307,6 +307,59 @@ class Word2Vec:
         """Linear decay like the reference (word2vec.cc:551-559)."""
         self.alpha = max(self.cfg.starting_alpha * (1.0 - progress), self.cfg.starting_alpha * 1e-4)
 
+    # ------------------------------------------------------------------ nearest neighbours
+    def syn0_norms(self, chunk: int = 1 << 16) -> torch.Tensor:
+        """``1 / ||syn0[w]||`` for every word (float32 [vocab], on the server's device; ``inf`` for a zero row), read
+        with a chunked Pull. Pass it to :meth:`most_similar` to reuse it across calls."""
+        cfg, d, kv = self.cfg, self.cfg.embed_dim, self.worker
+        dev = self.server.device if self.cuda else torch.device("cpu")
+        out = torch.empty(cfg.vocab_size, dtype=torch.float32, device=dev)
+        for i in range(0, cfg.vocab_size, chunk):
+            w = torch.arange(i, min(cfg.vocab_size, i + chunk), dtype=torch.int64, device=dev)
+            rows = torch.empty(w.numel() * 2 * d, dtype=torch.float32, device=dev)
+            kv.wait(kv.pull(syn0_key(w), rows, self.cuda))
+            out[i:i + w.numel()] = 1.0 / rows.view(-1, 2 * d)[:, :d].norm(dim=1)
+        return out
+
+    def most_similar(self, words, k: int = 10, norms: Optional[torch.Tensor] = None):
+        """The ``k`` nearest words of each word in ``words`` by cosine similarity of the syn0 embeddings; the query
+        word itself is never returned. Returns ``(word ids int64 [n, k], cosine float32 [n, k])``, best first; equal
+        scores go to the smaller word id; ``(-1, -inf)`` pads a row when fewer than ``k`` words qualify (zero rows
+        give NaN scores and never qualify). ``norms``: the output of :meth:`syn0_norms` (computed here when omitted).
+        ``1 <= k <= 64``.
+
+        CUDA backend: the query rows are pulled and normalised, and ``ops.gather_gemm_topk`` scores them against all
+        syn0 rows of the store (bf16 operands, fp32 accumulation, times ``norms`` as the column scale) without
+        pulling the model. CPU backend: fp32 PyTorch with the same order (``ops.topk_reference``)."""
+        cfg, d, kv = self.cfg, self.cfg.embed_dim, self.worker
+        V = cfg.vocab_size
+        w = torch.as_tensor(words, dtype=torch.int64).reshape(-1)
+        n = w.numel()
+        dev = self.server.device if self.cuda else torch.device("cpu")
+        w = w.to(dev)
+        if norms is None:
+            norms = self.syn0_norms()
+        rows = torch.empty(n * 2 * d, dtype=torch.float32, device=dev)
+        kv.wait(kv.pull(syn0_key(w), rows, self.cuda))
+        q = rows.view(n, 2 * d)[:, :d] * norms[w].view(-1, 1)
+        if self.cuda:
+            from ..ops import gather_gemm_topk
+
+            excl = (torch.arange(n + 1, dtype=torch.int64, device=dev), w.contiguous())
+            vals, idx = gather_gemm_topk(self.server, q, syn0_key(torch.arange(V, dtype=torch.int64, device=dev)), d, k,
+                                         exclude=excl, col_scale=norms)
+            return idx, vals
+        from ..ops import _check_topk, topk_reference
+
+        _check_topk(n, V, k, None, None)
+        E = torch.empty(V * 2 * d, dtype=torch.float32)
+        kv.wait(kv.pull(syn0_key(torch.arange(V, dtype=torch.int64)), E))
+        scores = (q @ E.view(V, 2 * d)[:, :d].t()) * norms.view(1, -1)
+        excluded = torch.zeros(n, V, dtype=torch.bool)
+        excluded[torch.arange(n), w] = True
+        vals, idx = topk_reference(scores, int(k), excluded)
+        return idx, vals
+
     # ------------------------------------------------------------------ checkpoint
     def write_checkpoint(self, path: str, words=None, write_syn1: bool = False, chunk: int = 1 << 15) -> None:
         """Binary word2vec format of the reference (word2vec.cc:367-416); rank 0 pulls the model."""

@@ -348,6 +348,139 @@ def gather_gemm_rank_count(server, q: torch.Tensor, keys: torch.Tensor, k: int, 
     return out
 
 
+TOPK_MAX_K = 64
+# gather_gemm_topk on several GPUs: each CTA stays registered in the sync round's grace epoch for all its tiles, so the
+# slice count is chosen to keep a CTA at no more than this many 128-column tiles
+_TOPK_GRACE_TILES = 64
+
+
+def _check_topk(M: int, N: int, k: int, exclude, col_scale):
+    """Validates the top-k arguments (shapes, dtypes and the exclusion CSR) before anything touches the device."""
+    if isinstance(k, bool) or int(k) != k or not 1 <= int(k) <= TOPK_MAX_K:
+        raise ValueError(f"k must be an integer in [1, {TOPK_MAX_K}], got {k}")
+    if col_scale is not None:
+        if col_scale.dtype != torch.float32:
+            raise TypeError("col_scale must be float32")
+        if col_scale.dim() != 1 or col_scale.numel() != N:
+            raise ValueError(f"col_scale must have one entry per column ({N}), got shape {tuple(col_scale.shape)}")
+    if exclude is not None:
+        if not (isinstance(exclude, (tuple, list)) and len(exclude) == 2):
+            raise ValueError("exclude must be a CSR pair (offsets int64 [M + 1], cols int64 [nnz])")
+        off, cols = exclude
+        if off.dtype != torch.int64 or cols.dtype != torch.int64:
+            raise TypeError("exclude offsets and cols must be int64")
+        if off.dim() != 1 or off.numel() != M + 1 or cols.dim() != 1:
+            raise ValueError(f"exclude offsets must have M + 1 = {M + 1} entries and cols must be 1-D")
+        if int(off[0]) != 0 or int(off[-1]) != cols.numel() or bool((off[1:] < off[:-1]).any()):
+            raise ValueError("exclude offsets must start at 0, be monotone and end at nnz")
+
+
+def _topk_operands(dev, exclude, col_scale):
+    for t, nm in ((col_scale, "col_scale"),) + (((exclude[0], "exclude offsets"), (exclude[1], "exclude cols"))
+                                                 if exclude is not None else ()):
+        if t is not None and not (t.is_cuda and t.device == dev and t.is_contiguous()):
+            raise TypeError(f"{nm} must be a contiguous CUDA tensor on {dev}")
+    return (col_scale.data_ptr() if col_scale is not None else 0,
+            exclude[0].data_ptr() if exclude is not None else 0,
+            exclude[1].data_ptr() if exclude is not None else 0)
+
+
+def _topk_outputs(M: int, S: int, k: int, dev):
+    part_v = torch.empty(M * S * k, dtype=torch.float32, device=dev)
+    part_c = torch.empty(M * S * k, dtype=torch.int32, device=dev)
+    vals = torch.empty(M, k, dtype=torch.float32, device=dev)
+    idx = torch.empty(M, k, dtype=torch.int64, device=dev)
+    return part_v, part_c, vals, idx
+
+
+def _topk_empty(M: int, k: int, dev):
+    return (torch.full((M, k), float("-inf"), dtype=torch.float32, device=dev),
+            torch.full((M, k), -1, dtype=torch.int64, device=dev))
+
+
+def gemm_nt_topk(q: torch.Tensor, e: torch.Tensor, k: int, exclude=None, col_scale: Optional[torch.Tensor] = None):
+    """Per row i of ``q`` the ``k`` best columns j of ``score(i, j) = <q_i, e_j>``, without an [M, N] score matrix.
+
+    Returns ``(values fp32 [M, k], indices int64 [M, k])``. Scores are the fp32 wgmma accumulation of the bf16-rounded
+    operands (bit-identical to ``gemm_nt_bf16(q, e)`` wherever that GEMM does not split K), multiplied once by
+    ``col_scale[j]`` when ``col_scale`` (float32 [N]) is given. Order: score descending, ties to the smaller column;
+    the result does not depend on how the work is split, and repeated calls are bit-identical.
+    ``exclude = (offsets int64 [M + 1], cols int64 [nnz])``: columns ``cols[offsets[i]:offsets[i + 1]]`` (sorted
+    ascending within each row) never appear in row i. NaN scores are never selected; a row with fewer than ``k``
+    eligible columns is padded with ``(-inf, -1)``. ``1 <= k <= 64``. Extra device memory is O(M * S * k) for S column
+    slices (S is chosen from the SM count)."""
+    if not (q.dim() == 2 and e.dim() == 2 and q.shape[1] == e.shape[1]):
+        raise ValueError("gemm_nt_topk expects matrices q[M, K], e[N, K]")
+    M, N = q.shape[0], e.shape[0]
+    _check_topk(M, N, k, exclude, col_scale)
+    if not (q.is_cuda and e.is_cuda and q.device == e.device):
+        raise TypeError("gemm_nt_topk expects CUDA tensors on one device")
+    k = int(k)
+    if M == 0 or N == 0:
+        return _topk_empty(M, k, q.device)
+    cs, eo, ec = _topk_operands(q.device, exclude, col_scale)
+    q16, e16 = _bf16_k8(q), _bf16_k8(e)
+    S = _C.topk_num_slices(M, N, 0)
+    part_v, part_c, vals, idx = _topk_outputs(M, S, k, q.device)
+    _C.gemm_nt_topk(_stream(q16), q16.data_ptr(), e16.data_ptr(), M, N, q16.shape[1], k, S, cs, eo, ec, part_v.data_ptr(),
+                    part_c.data_ptr(), vals.data_ptr(), idx.data_ptr())
+    return vals, idx
+
+
+def gather_gemm_topk(server, q: torch.Tensor, keys: torch.Tensor, dim: int, k: int, exclude=None,
+                     col_scale: Optional[torch.Tensor] = None, stats: Optional[torch.Tensor] = None):
+    """:func:`gemm_nt_topk` against parameter-store rows: column n is the first ``dim`` values of store row
+    ``keys[n]``, gathered inside the kernel from local HBM, local replicas or peer GPUs over NVLink (as
+    :func:`gather_gemm`, whose scores it reproduces bit for bit). ``indices`` are positions into ``keys``. ``stats``:
+    optional int64[2] accumulated with (rows gathered locally, rows gathered from peers).
+
+    On several GPUs every CTA of the kernel counts in the grace period of the sync rounds for all of its column tiles
+    (at most 64), so a long retrieval delays the relocations of a concurrent sync round."""
+    _i64(keys, "keys")
+    if q.dim() != 2 or q.shape[1] != int(dim):
+        raise ValueError(f"q must be a matrix [M, dim = {dim}]")
+    M, N = q.shape[0], keys.numel()
+    _check_topk(M, N, k, exclude, col_scale)
+    if not (q.is_cuda and q.device == keys.device):
+        raise TypeError("q must be a CUDA tensor on the device of keys")
+    if stats is not None and not (stats.is_cuda and stats.dtype == torch.int64 and stats.numel() >= 2):
+        raise TypeError("stats must be a CUDA int64 tensor with 2 entries")
+    k = int(k)
+    if M == 0 or N == 0:
+        return _topk_empty(M, k, q.device)
+    cs, eo, ec = _topk_operands(q.device, exclude, col_scale)
+    q16 = _bf16_k8(q)
+    S = _C.topk_num_slices(M, N, _TOPK_GRACE_TILES if server.num_servers() > 1 else 0)
+    part_v, part_c, vals, idx = _topk_outputs(M, S, k, q.device)
+    _C.gather_gemm_topk(server._impl.backend_handle(), _stream(q16), q16.data_ptr(), keys.data_ptr(), M, N, int(dim),
+                        q16.shape[1], k, S, cs, eo, ec, part_v.data_ptr(), part_c.data_ptr(), vals.data_ptr(),
+                        idx.data_ptr(), stats.data_ptr() if stats is not None else 0)
+    return vals, idx
+
+
+def topk_reference(scores: torch.Tensor, k: int, excluded: Optional[torch.Tensor] = None):
+    """Plain PyTorch top-k with the rule of the top-k kernels (tests, CPU backends): per row the ``k`` best columns of
+    ``scores`` [M, N], score descending, ties to the smaller column, ``excluded`` (bool [M, N]) and NaN columns never
+    selected, ``(-inf, -1)`` padding. Returns ``(values [M, k], indices int64 [M, k])`` in the dtype of ``scores``."""
+    M, N = scores.shape
+    ok = ~torch.isnan(scores)
+    if excluded is not None:
+        ok &= ~excluded
+    s = torch.where(ok, scores, torch.full_like(scores, float("-inf")))
+    order = torch.sort(s, dim=1, descending=True, stable=True).indices          # ties keep the column order
+    order = order.gather(1, torch.sort(ok.gather(1, order).to(torch.int8), dim=1, descending=True, stable=True).indices)
+    kk = min(int(k), N)
+    idx = order[:, :kk]
+    vals = scores.gather(1, idx)
+    valid = ok.gather(1, idx)
+    vals = torch.where(valid, vals, torch.full_like(vals, float("-inf")))
+    idx = torch.where(valid, idx, torch.full_like(idx, -1))
+    if kk < k:
+        vals = torch.cat([vals, vals.new_full((M, k - kk), float("-inf"))], 1)
+        idx = torch.cat([idx, idx.new_full((M, k - kk), -1)], 1)
+    return vals, idx
+
+
 class IntentPrepass:
     """Device-side pre-pass for ``Worker.intent`` (experimental; ``csrc/cuda/ops_intent.cu``).
 
