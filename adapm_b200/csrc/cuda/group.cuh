@@ -22,7 +22,20 @@ struct WarpGroup {
   }
 };
 
-#define ADAPM_CUDA_CHECK(expr)                                                                  \
+// LaneGroup: one thread on its own (the per-row gather threads of the GEMM kernels).
+struct LaneGroup {
+  __device__ __forceinline__ int lane() const { return 0; }
+  __device__ __forceinline__ int size() const { return 1; }
+  __device__ __forceinline__ bool any(bool p) const { return p; }
+  __device__ __forceinline__ void sync() const {}
+  __device__ __forceinline__ uint32_t bcast(uint32_t v) const { return v; }
+  __device__ __forceinline__ int32_t bcast(int32_t v) const { return v; }
+  __device__ __forceinline__ uint64_t bcast(uint64_t v) const { return v; }
+  __device__ __forceinline__ uint32_t bcast_from(uint32_t v, int) const { return v; }
+  __device__ __forceinline__ double sum(double v) const { return v; }
+};
+
+#define ADAPM_CUDA_CHECK(expr)                                                                 \
   do {                                                                                          \
     cudaError_t _e = (expr);                                                                    \
     if (_e != cudaSuccess) {                                                                    \

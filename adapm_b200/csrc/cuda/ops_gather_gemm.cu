@@ -58,15 +58,14 @@ gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
     // ===================== gatherers: store rows (local HBM / NVLink peers) -> swizzled smem; thread 0 also TMAs Q ==
     const int t = threadIdx.x;                // tile row handled by this thread (0..127)
     const int n = tile_n * BN + t;
-    const float* row = nullptr;
-    unsigned nl = 0, nr = 0;
+    const Key key = n < N ? keys[n] : 0;
+    dev::GatherRow row = {nullptr, nullptr, nullptr, nullptr, 0u, false};
+    unsigned nl = 0, nr = 0, nu = 0;
     if (n < N) {
-      const Key key = keys[n];
-      const int cls = class_of_key(c, key);
-      for (int attempt = 0; attempt < 4096 && !row; ++attempt) {
-        dev::Target tg = dev::resolve_fast(c, key, cls, &nl, &nr);
-        row = tg.row;
-        if (!row) __nanosleep(256);            // transitional slot (relocation in flight): retry
+      row.row = dev::resolve_fast(c, key, class_of_key(c, key), &nl, &nr).row;
+      if (!row.row) {                          // transitional slot (relocation in flight)
+        row = dev::gather_locate(c, key);
+        if (!row.row) ++nu; else if (row.local) ++nl; else ++nr;
       }
     }
     for (int kb = 0; kb < num_kb; ++kb) {
@@ -81,11 +80,13 @@ gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
       const int k0 = kb * BK_ELEMS;
       // 64 floats of this row -> 8 chunks of 8 bf16; chunk c goes to position c ^ (t & 7)  (128B swizzle)
       float4 v[16];
+      do {
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int k = k0 + 4 * j;
-        v[j] = (row && k < K) ? dev::ld_row4(row + k) : make_float4(0.f, 0.f, 0.f, 0.f);  // K % 4 == 0
-      }
+        for (int j = 0; j < 16; ++j) {
+          const int k = k0 + 4 * j;
+          v[j] = (row.row && k < K) ? dev::ld_gather4(row, k) : make_float4(0.f, 0.f, 0.f, 0.f);  // K % 4 == 0
+        }
+      } while (dev::gather_reread(c, key, row));
 #pragma unroll
       for (int ch = 0; ch < 8; ++ch) {
         uint4 o;
@@ -101,10 +102,14 @@ gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
     }
     if (stats) {
 #pragma unroll
-      for (int o = 16; o > 0; o >>= 1) { nl += __shfl_xor_sync(0xffffffffu, nl, o); nr += __shfl_xor_sync(0xffffffffu, nr, o); }
+      for (int o = 16; o > 0; o >>= 1) {
+        nl += __shfl_xor_sync(0xffffffffu, nl, o); nr += __shfl_xor_sync(0xffffffffu, nr, o);
+        nu += __shfl_xor_sync(0xffffffffu, nu, o);
+      }
       if (lane == 0) {
         if (nl) atomicAdd(stats + 0, (unsigned long long)nl);
         if (nr) atomicAdd(stats + 1, (unsigned long long)nr);
+        if (nu) atomicAdd(stats + 2, (unsigned long long)nu);   // unresolved rows, staged as zeros
       }
     }
   } else {

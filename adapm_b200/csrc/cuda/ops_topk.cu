@@ -70,14 +70,17 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&v);
 }
-__device__ __forceinline__ void stage_row_bf16(unsigned char* tile, const float* row, int t, int k0, int K) {
+__device__ __forceinline__ void stage_row_bf16(unsigned char* tile, const Ctx& c, Key key, dev::GatherRow& row, int t,
+                                               int k0, int K) {
   unsigned char* dst_row = tile + (size_t)t * ROW_BYTES;
   float4 v[16];
+  do {
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    const int k = k0 + 4 * j;
-    v[j] = (row && k < K) ? dev::ld_row4(row + k) : make_float4(0.f, 0.f, 0.f, 0.f);
-  }
+    for (int j = 0; j < 16; ++j) {
+      const int k = k0 + 4 * j;
+      v[j] = (row.row && k < K) ? dev::ld_gather4(row, k) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  } while (dev::gather_reread(c, key, row));
   // 8 chunks of 8 bf16; chunk c goes to position c ^ (t & 7)  (128-byte swizzle)
 #pragma unroll
   for (int ch = 0; ch < 8; ++ch) {
@@ -318,18 +321,17 @@ gather_gemm_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
   if (warp < 4) {
     // ===================== gatherers: store rows -> swizzled smem, tile after tile; thread 0 also TMAs Q ============
     const int t = threadIdx.x;                // tile row handled by this thread (0..127)
-    unsigned nl = 0, nr = 0;
+    unsigned nl = 0, nr = 0, nu = 0;
     uint32_t it = 0;
     for (int tn = slice; tn < n_tiles; tn += a.S) {
       const int n = tn * BN + t;
-      const float* row = nullptr;
+      const Key key = n < a.N ? keys[n] : 0;
+      dev::GatherRow row = {nullptr, nullptr, nullptr, nullptr, 0u, false};
       if (n < a.N) {
-        const Key key = keys[n];
-        const int cls = class_of_key(c, key);
-        for (int attempt = 0; attempt < 4096 && !row; ++attempt) {
-          dev::Target tg = dev::resolve_fast(c, key, cls, &nl, &nr);
-          row = tg.row;
-          if (!row) __nanosleep(256);            // transitional slot (relocation in flight): retry
+        row.row = dev::resolve_fast(c, key, class_of_key(c, key), &nl, &nr).row;
+        if (!row.row) {                          // transitional slot (relocation in flight)
+          row = dev::gather_locate(c, key);
+          if (!row.row) ++nu; else if (row.local) ++nl; else ++nr;
         }
       }
       for (int kb = 0; kb < num_kb; ++kb, ++it) {
@@ -339,7 +341,7 @@ gather_gemm_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
           mbar_expect_tx(&sm.full_bar[s], A_BYTES);
           tma_load_2d(sm.a[s], &tmap_q, &sm.full_bar[s], kb * BK_ELEMS, tile_m * BM);
         }
-        stage_row_bf16(sm.b[s], row, t, kb * BK_ELEMS, a.K);
+        stage_row_bf16(sm.b[s], c, key, row, t, kb * BK_ELEMS, a.K);
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor core
         __syncwarp();
         if (lane == 0) mbar_arrive(&sm.full_bar[s]);
@@ -347,10 +349,14 @@ gather_gemm_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
     }
     if (stats) {
 #pragma unroll
-      for (int o = 16; o > 0; o >>= 1) { nl += __shfl_xor_sync(0xffffffffu, nl, o); nr += __shfl_xor_sync(0xffffffffu, nr, o); }
+      for (int o = 16; o > 0; o >>= 1) {
+        nl += __shfl_xor_sync(0xffffffffu, nl, o); nr += __shfl_xor_sync(0xffffffffu, nr, o);
+        nu += __shfl_xor_sync(0xffffffffu, nu, o);
+      }
       if (lane == 0) {
         if (nl) atomicAdd(stats + 0, (unsigned long long)nl);
         if (nr) atomicAdd(stats + 1, (unsigned long long)nr);
+        if (nu) atomicAdd(stats + 2, (unsigned long long)nu);   // unresolved rows, staged as zeros
       }
     }
   } else {

@@ -155,6 +155,49 @@ __device__ __forceinline__ Target resolve_fast(const Ctx& c, Key key, int cls, u
   return t;
 }
 
+// Rows for the gather threads of the GEMM kernels (one thread per row: ops_gather_gemm.cu, ops_topk.cu). `base` set: the
+// key's relocation is in flight and its value is row - base + row2 (locate_pull's three-way read), valid while
+// *meta_ptr still holds meta_val. row == nullptr: the key could not be resolved.
+struct GatherRow {
+  const float* row;
+  const float* base;
+  const float* row2;
+  const uint32_t* meta_ptr;
+  uint32_t meta_val;
+  bool local;
+};
+
+// For keys that resolve_fast leaves open: protocol.h's locate_pull with a one-lane group follows a relocation source to
+// the new owner, reads an INCOMING slot three ways and waits out FINALIZING - none of which needs the sync round to
+// progress, so a CTA that the round's grace period waits for cannot wait for the round.
+static __device__ __noinline__ GatherRow gather_locate(const Ctx& c, Key key) {
+  LaneGroup g;
+  const PullLoc<float> l = locate_pull<float>(c, g, key, false);
+  GatherRow r;
+  r.row = l.kind == LOC_FAIL ? nullptr : l.row;
+  r.base = l.kind == LOC_SUM3 ? l.base : nullptr;
+  r.row2 = l.row2; r.meta_ptr = l.meta_ptr; r.meta_val = l.meta_val; r.local = l.local;
+  return r;
+}
+
+__device__ __forceinline__ float4 ld_gather4(const GatherRow& r, int k) {
+  float4 v = ld_row4(r.row + k);
+  if (r.base) {
+    const float4 b = ld_row4(r.base + k), s = ld_row4(r.row2 + k);
+    v.x = v.x - b.x + s.x; v.y = v.y - b.y + s.y; v.z = v.z - b.z + s.z; v.w = v.w - b.w + s.w;
+  }
+  return v;
+}
+
+// After a three-way read: did the transfer complete in between (the values read may mix both sides)? Then re-locate.
+__device__ __forceinline__ bool gather_reread(const Ctx& c, Key key, GatherRow& r) {
+  if (!r.base) return false;
+  mem::fence();
+  if (mem::ld_acquire(r.meta_ptr) == r.meta_val) return false;
+  r = gather_locate(c, key);
+  return true;
+}
+
 // lane 0 marks a completed fast-path push
 __device__ __forceinline__ void mark_pushed(const Target& t) {
   if (t.version) mem::red_add(t.version, 1u);

@@ -319,32 +319,58 @@ def gemm_nt_rank_count(q: torch.Tensor, e: torch.Tensor, true_score: torch.Tenso
     return out
 
 
+def _gather_stats(server, stats: Optional[torch.Tensor], dev):
+    """The stats buffer of a gather launch. On several ranks a private int64[3] - (local rows, peer rows, rows that could
+    not be resolved and were staged as zeros) - that :func:`_gathered` checks after the launch."""
+    if server.num_servers() == 1:      # every row is a local owned row
+        return stats
+    return torch.zeros(3, dtype=torch.int64, device=dev)
+
+
+def _gathered(op: str, own: Optional[torch.Tensor], stats: Optional[torch.Tensor]) -> None:
+    if own is None or own is stats:
+        return
+    if stats is not None:
+        n = min(stats.numel(), 3)
+        stats[:n] += own[:n]
+    bad = int(own[2])                  # (waits for the launch)
+    if bad:
+        raise RuntimeError(f"{op}: {bad} store rows could not be resolved and were read as zeros")
+
+
 def gather_gemm(server, q: torch.Tensor, keys: torch.Tensor, k: int, stats: Optional[torch.Tensor] = None) -> torch.Tensor:
     """scores[M, N] = q[M, k] @ E^T where row n of E is the first ``k`` values of store row ``keys[n]`` - the rows
     are gathered inside the GEMM kernel from the local slab, local replicas or peer GPUs over NVLink (fused
-    gather + wgmma GEMM); the gathered matrix never exists in HBM."""
+    gather + wgmma GEMM); the gathered matrix never exists in HBM. ``stats``: optional int64 tensor accumulated with
+    (rows gathered locally, rows gathered from peers[, rows that could not be resolved]). On several ranks the call
+    waits for the kernel and raises ``RuntimeError`` if a row could not be resolved."""
     _i64(keys, "keys")
     q16 = _bf16_k8(q)
     M, N = q16.shape[0], keys.numel()
     c = torch.empty(M, N, dtype=torch.float32, device=q.device)
+    own = _gather_stats(server, stats, q.device)
     _C.gather_gemm(server._impl.backend_handle(), _stream(q16), q16.data_ptr(), keys.data_ptr(), M, N, int(k), q16.shape[1],
-                   c.data_ptr(), N, stats.data_ptr() if stats is not None else 0)
+                   c.data_ptr(), N, own.data_ptr() if own is not None else 0)
+    _gathered("gather_gemm", own, stats)
     return c
 
 
 def gather_gemm_rank_count(server, q: torch.Tensor, keys: torch.Tensor, k: int, true_score: torch.Tensor,
                            true_col: torch.Tensor, stats: Optional[torch.Tensor] = None) -> torch.Tensor:
     """counts[i] = #{n != true_col[i] : <q[i], row(keys[n])[:k]> > true_score[i]}: fused gather + GEMM + ranking
-    epilogue - neither the gathered rows nor the [M, N] scores are materialised."""
+    epilogue - neither the gathered rows nor the [M, N] scores are materialised. ``stats``: as for
+    :func:`gather_gemm`."""
     _i64(keys, "keys")
     q16 = _bf16_k8(q)
     M, N = q16.shape[0], keys.numel()
     out = torch.zeros(M, dtype=torch.int32, device=q.device)
     ts = true_score.to(torch.float32).contiguous()
     tc = true_col.to(torch.int32).contiguous()
+    own = _gather_stats(server, stats, q.device)
     _C.gather_gemm_rank_count(server._impl.backend_handle(), _stream(q16), q16.data_ptr(), keys.data_ptr(), M, N, int(k),
                               q16.shape[1], ts.data_ptr(), tc.data_ptr(), out.data_ptr(),
-                              stats.data_ptr() if stats is not None else 0)
+                              own.data_ptr() if own is not None else 0)
+    _gathered("gather_gemm_rank_count", own, stats)
     return out
 
 
@@ -432,7 +458,9 @@ def gather_gemm_topk(server, q: torch.Tensor, keys: torch.Tensor, dim: int, k: i
     """:func:`gemm_nt_topk` against parameter-store rows: column n is the first ``dim`` values of store row
     ``keys[n]``, gathered inside the kernel from local HBM, local replicas or peer GPUs over NVLink (as
     :func:`gather_gemm`, whose scores it reproduces bit for bit). ``indices`` are positions into ``keys``. ``stats``:
-    optional int64[2] accumulated with (rows gathered locally, rows gathered from peers).
+    optional int64[2] accumulated with (rows gathered locally, rows gathered from peers), and with the rows that could
+    not be resolved in a third entry if it has one; on several ranks the call waits for the kernels and raises
+    ``RuntimeError`` if a row could not be resolved.
 
     On several GPUs every CTA of the kernel counts in the grace period of the sync rounds for all of its column tiles
     (at most 64), so a long retrieval delays the relocations of a concurrent sync round."""
@@ -452,9 +480,11 @@ def gather_gemm_topk(server, q: torch.Tensor, keys: torch.Tensor, dim: int, k: i
     q16 = _bf16_k8(q)
     S = _C.topk_num_slices(M, N, _TOPK_GRACE_TILES if server.num_servers() > 1 else 0)
     part_v, part_c, vals, idx = _topk_outputs(M, S, k, q.device)
+    own = _gather_stats(server, stats, q.device)
     _C.gather_gemm_topk(server._impl.backend_handle(), _stream(q16), q16.data_ptr(), keys.data_ptr(), M, N, int(dim),
                         q16.shape[1], k, S, cs, eo, ec, part_v.data_ptr(), part_c.data_ptr(), vals.data_ptr(),
-                        idx.data_ptr(), stats.data_ptr() if stats is not None else 0)
+                        idx.data_ptr(), own.data_ptr() if own is not None else 0)
+    _gathered("gather_gemm_topk", own, stats)
     return vals, idx
 
 
