@@ -2,6 +2,7 @@
 
     python -m adapm_b200.launch -s 8 --backend cuda -m adapm_b200.apps.ctr -- --num_features 100000000
     python -m adapm_b200.apps.ctr --backend cpu --num_features 20000 --steps 30 --batch_size 512
+    python -m adapm_b200.apps.ctr --backend cpu --num_features 20000 --steps 30 --batch_size 512 --multi_hot 3
 """
 from __future__ import annotations
 
@@ -11,7 +12,7 @@ import time
 
 import adapm_b200 as ad
 from adapm_b200.apps._common import add_system_options, strip_dashes, system_options
-from adapm_b200.models.deepfm import DeepFM, DeepFMConfig, synthetic_ctr_batch
+from adapm_b200.models.deepfm import DeepFM, DeepFMConfig, synthetic_ctr_batch, synthetic_multi_hot_batch
 
 
 def main(argv=None) -> int:
@@ -25,11 +26,14 @@ def main(argv=None) -> int:
     ap.add_argument("--precision", default="bf16", choices=["fp32", "bf16", "fp8"])
     ap.add_argument("--table_precision", default="fp32", choices=["fp32", "fp8_block"],
                     help="fp8_block: train on the values a block-scaled e4m3 embedding table would deliver (fp32 master rows)")
+    ap.add_argument("--multi_hot", type=int, default=0,
+                    help="> 0: every field holds a bag of 1..L ids, pooled into one embedding (fused kernels on CUDA)")
+    ap.add_argument("--pooling", default="sum", choices=["sum", "mean"], help="pooling of multi-hot bags")
     add_system_options(ap)
     args = ap.parse_args(strip_dashes(argv if argv is not None else sys.argv[1:]))
     cfg = DeepFMConfig(num_features=args.num_features, num_fields=args.num_fields, embed_dim=args.embed_dim,
                        batch_size=args.batch_size, read_ahead=args.read_ahead, precision=args.precision,
-                       table_precision=args.table_precision)
+                       table_precision=args.table_precision, multi_hot=args.multi_hot, pooling=args.pooling)
     ad.setup(cfg.num_features, 1)
     server = ad.Server(cfg.row_len, backend=args.backend, options=system_options(args))
     kv = ad.Worker(0, server)
@@ -43,7 +47,7 @@ def main(argv=None) -> int:
 
     def batch(b):
         if b not in batches:
-            batches[b] = synthetic_ctr_batch(cfg, b, rank)
+            batches[b] = synthetic_multi_hot_batch(cfg, b, rank) if cfg.multi_hot else synthetic_ctr_batch(cfg, b, rank)
         return batches[b]
 
     look = LookaheadIntents(kv, args.steps + cfg.read_ahead, cfg.read_ahead, lambda b: batch(b)[0]) if server.num_servers() > 1 else None
@@ -53,9 +57,14 @@ def main(argv=None) -> int:
     for s in range(args.steps):
         if look:
             look.signal(s)
-        ids, y = batch(s)
-        batches.pop(s - 1, None)
-        losses.append(model.step(ids, y))
+        if cfg.multi_hot:
+            ids, off, y = batch(s)
+            batches.pop(s - 1, None)
+            losses.append(model.step(ids, y, offsets=off))
+        else:
+            ids, y = batch(s)
+            batches.pop(s - 1, None)
+            losses.append(model.step(ids, y))
         kv.advance_clock()
         if rank == 0 and (s + 1) % max(1, args.steps // 5) == 0:
             print(f"[ctr] step {s + 1}: loss {sum(losses[-10:]) / len(losses[-10:]):.4f} "

@@ -80,6 +80,22 @@ void gather_gemm_topk(CudaBackend& be, cudaStream_t stream, const void* Q, const
                       int k, int S, const float* col_scale, const int64_t* ex_off, const int64_t* ex_cols, float* part_v,
                       int* part_c, float* out_v, int64_t* out_i, unsigned long long* stats);
 
+// multi-hot embedding bags over rows [embedding (E) | AdaGrad (E)] (ops_embbag.cu). CSR bags: keys[nnz],
+// offsets[nbags + 1], optional weights[nnz]; mean: divide by the bag length. stats: int64[5] accumulated with (local
+// rows, peer rows, slow-path rows, rows updated, rows that could not be resolved).
+// forward (1 launch): out[nbags, E] = pooled rows, each bag summed in fp32 in key order.
+// backward (4 launches, the radix sort counted as one): G_k = grad_scale * sum over the occurrences of k of
+// c_i * grad_out[bag(i)] in position order, then push [-lr G / sqrt(acc + G^2) | G^2] once per distinct key.
+constexpr int kEmbBagMaxDim = 512;
+size_t embedding_bag_workspace_bytes(int64_t nnz, int64_t nbags, int E);
+void embedding_bag_forward(CudaBackend& be, cudaStream_t stream, const Key* keys, const int64_t* offsets,
+                           const float* weights, int64_t nnz, int nbags, int E, bool mean, float* out,
+                           unsigned long long* stats);
+void embedding_bag_backward(CudaBackend& be, cudaStream_t stream, const Key* keys, const int64_t* offsets,
+                            const float* weights, int64_t nnz, int nbags, int E, bool mean, const float* grad_out,
+                            float lr, float grad_scale, void* workspace, size_t workspace_bytes,
+                            unsigned long long* stats);
+
 // Native step driver of the word2vec SGNS loop (ops_train_loop.cu)
 struct SgnsLoopConfig {
   int batch_pairs = 0, negative = 0, embed_dim = 0, read_ahead = 0, max_inflight = 3, rank = 0;

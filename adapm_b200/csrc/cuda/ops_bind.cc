@@ -100,6 +100,22 @@ void bind(py::module_& m) {
                      ptr<const float>(col_scale), ptr<const int64_t>(ex_off), ptr<const int64_t>(ex_cols), ptr<float>(part_v),
                      ptr<int>(part_c), ptr<float>(out_v), ptr<int64_t>(out_i), ptr<unsigned long long>(stats));
   });
+  m.attr("embedding_bag_max_dim") = kEmbBagMaxDim;
+  m.def("embedding_bag_workspace_bytes", [](int64_t nnz, int64_t nbags, int E) {
+    return embedding_bag_workspace_bytes(nnz, nbags, E);
+  });
+  m.def("embedding_bag_forward", [](uintptr_t be, uintptr_t stream, uintptr_t keys, uintptr_t offsets, uintptr_t weights,
+                                    int64_t nnz, int nbags, int E, bool mean, uintptr_t out, uintptr_t stats) {
+    embedding_bag_forward(backend_of(be), (cudaStream_t)stream, ptr<const Key>(keys), ptr<const int64_t>(offsets),
+                          ptr<const float>(weights), nnz, nbags, E, mean, ptr<float>(out), ptr<unsigned long long>(stats));
+  });
+  m.def("embedding_bag_backward", [](uintptr_t be, uintptr_t stream, uintptr_t keys, uintptr_t offsets, uintptr_t weights,
+                                     int64_t nnz, int nbags, int E, bool mean, uintptr_t grad_out, float lr,
+                                     float grad_scale, uintptr_t ws, size_t ws_bytes, uintptr_t stats) {
+    embedding_bag_backward(backend_of(be), (cudaStream_t)stream, ptr<const Key>(keys), ptr<const int64_t>(offsets),
+                           ptr<const float>(weights), nnz, nbags, E, mean, ptr<const float>(grad_out), lr, grad_scale,
+                           ptr<void>(ws), ws_bytes, ptr<unsigned long long>(stats));
+  });
   py::class_<SgnsLoop>(m, "SgnsLoop")
       .def(py::init([](uintptr_t worker, uintptr_t be, int batch_pairs, int negative, int embed_dim, int read_ahead,
                        int max_inflight, int rank, bool signal_intent, bool local_only, int64_t model_seed, int sampler_kind,

@@ -38,6 +38,9 @@ class DeepFMConfig:
                                         # (UE8M0 scale per 32 values, utils/blockscale.py) would deliver; the parameter
                                         # manager keeps fp32 master rows (deltas and AdaGrad accumulate in fp32)
     model_seed: int = 1
+    multi_hot: int = 0                  # > 0: up to this many ids per field, pooled into one [w | v] per field
+                                        # (synthetic_multi_hot_batch, DeepFM.step(..., offsets=)); 0: one id per field
+    pooling: str = "sum"                # sum | mean (multi-hot fields)
 
     @property
     def emb_len(self) -> int:           # [w | v] padded to a multiple of 4 floats (16-byte vector row accesses)
@@ -100,6 +103,13 @@ class DeepFM:
         self.opt = torch.optim.Adam(self.net.parameters(), lr=cfg.lr_dense)
         self.step_no = 0
         self.rows_pushed = 0      # (key,row) updates applied so far (distinct feature rows per batch)
+        self.bag = None
+        if cfg.multi_hot:
+            from ..ops import StoreEmbeddingBag
+
+            if cfg.table_precision != "fp32":
+                raise ValueError("multi_hot needs table_precision='fp32'")
+            self.bag = StoreEmbeddingBag(server, worker, cfg.emb_len, mode=cfg.pooling, lr=cfg.lr_sparse)
 
     def init_model(self, chunk: int = 1 << 18) -> None:
         """v ~ N(0, 0.01), w = 0, accumulators 1e-6; every rank initialises the keys it is home for."""
@@ -121,9 +131,16 @@ class DeepFM:
         if self.server.num_servers() > 1:
             self.worker.intent(feat_ids.reshape(-1), clock, clock + 1)
 
-    def step(self, feat_ids: torch.Tensor, labels: torch.Tensor, return_tensor: bool = False):
+    def step(self, feat_ids: torch.Tensor, labels: torch.Tensor, return_tensor: bool = False,
+             offsets: Optional[torch.Tensor] = None):
         """feat_ids [B, F] int64 (global feature ids), labels [B] float (CPU / pinned / device tensors). Returns the
-        batch loss (a float, or the device tensor with ``return_tensor`` - no host synchronisation then)."""
+        batch loss (a float, or the device tensor with ``return_tensor`` - no host synchronisation then).
+
+        Multi-hot (``cfg.multi_hot > 0``): ``feat_ids`` is the flat int64 [nnz] list of all bags and ``offsets`` int64
+        [B * F + 1] delimits them, bag ``b * F + f`` holding the ids of field f of example b (see
+        :func:`synthetic_multi_hot_batch`)."""
+        if offsets is not None or self.bag is not None:
+            return self._step_multi_hot(feat_ids, labels, offsets, return_tensor)
         cfg, kv = self.cfg, self.worker
         B, F, k = feat_ids.shape[0], cfg.num_fields, cfg.embed_dim
         ids = feat_ids.to(self.dev, non_blocking=True).reshape(-1).contiguous()
@@ -159,6 +176,39 @@ class DeepFM:
         self.rows_pushed += int(uniq.numel())
         return loss.detach() if return_tensor else float(loss.detach())
 
+    def _step_multi_hot(self, feat_ids, labels, offsets, return_tensor):
+        """Every (example, field) bag is pooled by ``StoreEmbeddingBag`` (fused kernels on a CUDA server, pull +
+        ``embedding_bag`` + push on a CPU server); the pooled ``[w | v]`` of a field takes the place of its row: first
+        order ``sum_f w_f``, FM over the pooled ``v_f``, MLP on their concatenation. ``loss.backward()`` pushes the
+        AdaGrad updates of the batch's distinct ids (``grad_scale = B``, the single-hot rule). The step waits for the
+        device once even with ``return_tensor`` (the offsets check and the count of rows pushed)."""
+        if self.bag is None or offsets is None:
+            raise ValueError("multi-hot batches need DeepFMConfig.multi_hot > 0 and offsets")
+        cfg = self.cfg
+        F, k, el = cfg.num_fields, cfg.embed_dim, cfg.emb_len
+        ids = feat_ids.to(self.dev, non_blocking=True).reshape(-1).contiguous()
+        off = offsets.to(self.dev, non_blocking=True).reshape(-1).contiguous()
+        if (off.numel() - 1) % F:
+            raise ValueError(f"offsets must delimit B * {F} bags")
+        B = (off.numel() - 1) // F
+        y = labels.to(self.dev, non_blocking=True).float()
+        self.bag.grad_scale = float(B)          # sum over examples, like per-example SGD
+        e = self.bag(ids, off).view(B, F, el)
+        w1, v = e[:, :, 0], e[:, :, 1:1 + k]
+        fm = w1.sum(1) + 0.5 * ((v.sum(1) ** 2) - (v ** 2).sum(1)).sum(1)
+        logit = fm + self.net(v.reshape(B, F * k))
+        loss = torch.nn.functional.binary_cross_entropy_with_logits(logit, y)
+        self.opt.zero_grad(set_to_none=True)
+        loss.backward()
+        if torch.distributed.is_available() and torch.distributed.is_initialized() and self.server.num_servers() > 1:
+            for p in self.net.parameters():
+                torch.distributed.all_reduce(p.grad)
+                p.grad /= self.server.num_servers()
+        self.opt.step()
+        self.step_no += 1
+        self.rows_pushed += self.bag.take_rows_updated()
+        return loss.detach() if return_tensor else float(loss.detach())
+
 
 def synthetic_ctr_batch(cfg: DeepFMConfig, step: int, rank: int = 0):
     """Criteo-shaped synthetic batch: one id per field, ids Zipf-skewed within each field's range; the label
@@ -171,3 +221,25 @@ def synthetic_ctr_batch(cfg: DeepFMConfig, step: int, rank: int = 0):
     score = (((local % 7) - 3) * (1.0 / cfg.num_fields)).sum(1)
     labels = (rng.random(cfg.batch_size) < 1 / (1 + np.exp(-3 * score))).astype(np.float32)
     return torch.from_numpy(ids), torch.from_numpy(labels)
+
+
+def synthetic_multi_hot_batch(cfg: DeepFMConfig, step: int, rank: int = 0):
+    """Multi-hot batch in CSR form: ``(ids int64 [nnz], offsets int64 [B * F + 1], labels float32 [B])``. Bag
+    ``b * F + f`` holds the ids of field f of example b; its length is uniform in ``[1, cfg.multi_hot]``; ids are
+    skewed within each field's range as in :func:`synthetic_ctr_batch`. The label depends on a hidden linear model of
+    the bags' mean id scores, so that training has signal."""
+    if cfg.multi_hot < 1:
+        raise ValueError("synthetic_multi_hot_batch needs cfg.multi_hot >= 1")
+    rng = np.random.default_rng([cfg.model_seed, rank, step, cfg.multi_hot])
+    B, F = cfg.batch_size, cfg.num_fields
+    per_field = cfg.num_features // F
+    lens = rng.integers(1, cfg.multi_hot + 1, size=B * F)
+    bag = np.repeat(np.arange(B * F, dtype=np.int64), lens)
+    u = rng.random(bag.size)
+    local = np.minimum((per_field * u ** 3).astype(np.int64), per_field - 1)   # skewed towards small ids
+    ids = local + (bag % F) * per_field
+    offsets = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+    contrib = ((local % 7) - 3) * (1.0 / F) / lens[bag]
+    score = np.bincount(bag // F, weights=contrib, minlength=B)
+    labels = (rng.random(B) < 1 / (1 + np.exp(-3 * score))).astype(np.float32)
+    return torch.from_numpy(ids), torch.from_numpy(offsets), torch.from_numpy(labels)

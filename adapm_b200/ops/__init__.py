@@ -511,6 +511,208 @@ def topk_reference(scores: torch.Tensor, k: int, excluded: Optional[torch.Tensor
     return vals, idx
 
 
+EMBEDDING_BAG_MAX_DIM = 512
+_NNZ_LIMIT = 1 << 31
+
+
+class _EmbeddingBagFn(torch.autograd.Function):
+    """Autograd node of :class:`StoreEmbeddingBag`: the forward pools rows of the store, the backward pushes the
+    AdaGrad updates into the store (it returns no gradient: the rows are not tensors of the graph)."""
+
+    @staticmethod
+    def forward(ctx, anchor, bag, keys, offsets, weights):
+        ctx.bag = bag
+        out, ctx.state = bag._forward(keys, offsets, weights)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        ctx.bag._backward(ctx.state, grad)
+        ctx.state = None
+        return None, None, None, None, None
+
+
+class StoreEmbeddingBag:
+    """Multi-hot embedding bags over the rows of a parameter store: ``torch.nn.functional.embedding_bag`` with
+    ``include_last_offset=True`` whose table is the store, trained by worker-side AdaGrad.
+
+    Rows are ``[embedding (dim) | AdaGrad accumulator (dim)]`` (the server's value length must be ``2 * dim``).
+    ``bag(keys, offsets, per_sample_weights=None)`` returns ``out [nbags, dim]`` with
+    ``out[b] = sum_{i in [offsets[b], offsets[b + 1])} w_i * row(keys[i])[:dim]`` (``w_i`` = 1 without weights), divided
+    by the bag length for ``mode="mean"``; an empty bag gives zeros. ``keys`` int64 ``[nnz]``, ``offsets`` int64
+    ``[nbags + 1]`` (starts at 0, ends at nnz), ``per_sample_weights`` float32 ``[nnz]`` (``sum`` only, as in torch).
+    Weights are data: they get no gradient.
+
+    The result takes part in autograd: ``loss.backward()`` updates the rows in the store. For every distinct key ``k``
+    ``G = grad_scale * sum_{occurrences i of k} w_i (/ len of i's bag with mean) * grad_out[bag of i]`` and the row
+    gets ``[-lr * G / sqrt(acc + G^2) | G^2]`` added (``acc`` read when the update runs; 0 where ``G == 0``). Autograd
+    runs a backward only if some input requires grad: the op passes :attr:`anchor`, an empty tensor that requires grad,
+    so that the backward runs even when nothing else before the bag does.
+
+    ``impl``: ``fused`` (CUDA servers; csrc/cuda/ops_embbag.cu) - the forward is one kernel that reads the rows through
+    the directory (local HBM, replicas, peers over NVLink), the backward four launches (key/position prep, radix sort,
+    per-tile sums, finish) that push one update per distinct key. Each bag and each key's gradient is summed in fp32
+    in a fixed order, so on one GPU the same inputs give bit-identical outputs and rows. ``torch``: distinct keys ->
+    ``worker.pull`` -> ``F.embedding_bag`` over the pulled rows -> autograd -> AdaGrad -> ``worker.push``; the path of
+    CPU servers (``auto`` picks ``fused`` on CUDA servers, ``torch`` on CPU servers).
+
+    ``stats`` (fused): int64[4] accumulated with (rows read or updated locally, on peers, through the slow path of keys
+    in a transitional state, rows updated). Calls on one object must not overlap (one CUDA stream): the backward's
+    scratch is owned by the object and grows on demand."""
+
+    def __init__(self, server, worker, dim: int, mode: str = "sum", lr: float = 0.05, grad_scale: float = 1.0,
+                 impl: str = "auto"):
+        if isinstance(dim, bool) or int(dim) != dim or not (4 <= int(dim) <= EMBEDDING_BAG_MAX_DIM and int(dim) % 4 == 0):
+            raise ValueError(f"dim must be a multiple of 4 in [4, {EMBEDDING_BAG_MAX_DIM}], got {dim}")
+        if mode not in ("sum", "mean"):
+            raise ValueError(f"mode must be 'sum' or 'mean', got {mode!r}")
+        if impl not in ("auto", "fused", "torch"):
+            raise ValueError(f"impl must be 'auto', 'fused' or 'torch', got {impl!r}")
+        self.dim = int(dim)
+        row_len = getattr(server, "_uniform_len", None)
+        if row_len != 2 * self.dim:
+            raise ValueError(f"rows must be [embedding (dim) | AdaGrad (dim)]: the server's value length is {row_len}, "
+                             f"expected 2 * dim = {2 * self.dim}")
+        if impl == "auto":
+            impl = "fused" if server.backend == "cuda" else "torch"
+        if impl == "fused" and server.backend != "cuda":
+            raise ValueError("impl='fused' needs a server with backend='cuda'")
+        self.server, self.worker, self.mode, self.impl = server, worker, mode, impl
+        self.lr, self.grad_scale = float(lr), float(grad_scale)
+        self.device = server.device
+        self.anchor = torch.zeros(0, device=self.device, requires_grad=True)
+        self._stats = torch.zeros(5, dtype=torch.int64, device=self.device) if impl == "fused" else None
+        self._ws = None
+        self._rows_updated = 0          # torch route
+        self._rows_taken = 0
+
+    @property
+    def stats(self) -> Optional[torch.Tensor]:
+        return self._stats[:4] if self._stats is not None else None
+
+    def take_rows_updated(self) -> int:
+        """Rows updated since the previous call (one per distinct key and backward)."""
+        total = int(self._stats[3]) if self._stats is not None else self._rows_updated
+        n, self._rows_taken = total - self._rows_taken, total
+        return n
+
+    def __call__(self, keys: torch.Tensor, offsets: torch.Tensor,
+                 per_sample_weights: Optional[torch.Tensor] = None) -> torch.Tensor:
+        keys, offsets, per_sample_weights = self._check(keys, offsets, per_sample_weights)
+        return _EmbeddingBagFn.apply(self.anchor, self, keys, offsets, per_sample_weights)
+
+    def _check(self, keys, offsets, weights):
+        dev = self.device
+        for t, nm in ((keys, "keys"), (offsets, "offsets")):
+            if not isinstance(t, torch.Tensor) or t.dtype != torch.int64 or t.dim() != 1:
+                raise TypeError(f"{nm} must be a 1-D int64 tensor")
+            if t.device != dev:
+                raise TypeError(f"{nm} must be on the store's device {dev}, got {t.device}")
+        nnz = keys.numel()
+        if nnz >= _NNZ_LIMIT:
+            raise ValueError(f"at most 2^31 - 1 keys per call, got {nnz}")
+        if offsets.numel() < 1:
+            raise ValueError("offsets must have nbags + 1 entries (include_last_offset form)")
+        if weights is not None:
+            if self.mode != "sum":
+                raise ValueError("per_sample_weights are only supported with mode='sum'")
+            if not isinstance(weights, torch.Tensor) or weights.dtype != torch.float32:
+                raise TypeError("per_sample_weights must be a float32 tensor")
+            if weights.device != dev:
+                raise TypeError(f"per_sample_weights must be on the store's device {dev}, got {weights.device}")
+            if weights.shape != keys.shape:
+                raise ValueError(f"per_sample_weights must have one entry per key ({nnz}), got {tuple(weights.shape)}")
+            weights = weights.contiguous()
+        bad = (offsets[0] != 0) | (offsets[-1] != nnz)
+        if offsets.numel() > 1:
+            bad = bad | (offsets[1:] < offsets[:-1]).any()
+        if bool(bad):
+            raise ValueError(f"offsets must start at 0, be non-decreasing and end at nnz = {nnz}")
+        return keys.contiguous(), offsets.contiguous(), weights
+
+    # ---- fused route (CUDA servers)
+    def _check_resolved(self, op):
+        if self.server.num_servers() > 1 and int(self._stats[4]):   # (waits for the kernel)
+            raise RuntimeError(f"StoreEmbeddingBag {op}: {int(self._stats[4])} store rows could not be resolved")
+
+    def _forward(self, keys, offsets, weights):
+        if self.impl == "torch":
+            return self._forward_torch(keys, offsets, weights)
+        nbags = offsets.numel() - 1
+        out = torch.empty(nbags, self.dim, dtype=torch.float32, device=self.device)
+        _C.embedding_bag_forward(self.server._impl.backend_handle(), _stream(keys), keys.data_ptr(), offsets.data_ptr(),
+                                 weights.data_ptr() if weights is not None else 0, keys.numel(), nbags, self.dim,
+                                 self.mode == "mean", out.data_ptr(), self._stats.data_ptr())
+        self._check_resolved("forward")
+        return out, (keys, offsets, weights)
+
+    def _backward(self, state, grad):
+        if self.impl == "torch":
+            return self._backward_torch(state, grad)
+        keys, offsets, weights = state
+        nnz, nbags = keys.numel(), offsets.numel() - 1
+        g = grad.to(torch.float32).contiguous()
+        need = _C.embedding_bag_workspace_bytes(nnz, nbags, self.dim)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(max(need, 1), dtype=torch.uint8, device=self.device)
+        _C.embedding_bag_backward(self.server._impl.backend_handle(), _stream(g), keys.data_ptr(), offsets.data_ptr(),
+                                  weights.data_ptr() if weights is not None else 0, nnz, nbags, self.dim,
+                                  self.mode == "mean", g.data_ptr(), self.lr, self.grad_scale, self._ws.data_ptr(),
+                                  self._ws.numel(), self._stats.data_ptr())
+        self._check_resolved("backward")
+
+    # ---- torch route (CPU servers; the comparison arm of benchmarks/embbag_bench.py on CUDA servers)
+    def _forward_torch(self, keys, offsets, weights):
+        kv, d = self.worker, self.dim
+        uniq, inv = torch.unique(keys, return_inverse=True)
+        rows = torch.empty(uniq.numel() * 2 * d, dtype=self.server.dtype, device=self.device)
+        kv.wait(kv.pull(uniq, rows, True))
+        rows = rows.view(-1, 2 * d)
+        with torch.enable_grad():
+            emb = rows[:, :d].detach().clone().requires_grad_(True)
+            out = torch.nn.functional.embedding_bag(inv, emb, offsets, mode=self.mode, per_sample_weights=weights,
+                                                    include_last_offset=True)
+        return out.detach(), (uniq, emb, rows[:, d:], out)
+
+    def _backward_torch(self, state, grad):
+        uniq, emb, acc, out = state
+        (g,) = torch.autograd.grad(out, emb, grad.to(out.dtype))
+        g = g * self.grad_scale
+        upd = torch.where(g != 0, -self.lr * g / torch.sqrt(acc + g * g), torch.zeros_like(g))
+        self.worker.push(uniq, torch.cat([upd, g * g], 1).contiguous().view(-1), True)
+        self._rows_updated += int(uniq.numel())
+
+
+def embedding_bag_reference(table: torch.Tensor, keys: torch.Tensor, offsets: torch.Tensor,
+                            per_sample_weights: Optional[torch.Tensor] = None, mode: str = "sum",
+                            grad_out: Optional[torch.Tensor] = None, lr: float = 0.05, grad_scale: float = 1.0):
+    """The rule of :class:`StoreEmbeddingBag` in float64 on a dense table ``[num_keys, 2 * dim]`` (tests). Returns
+    ``(out [nbags, dim], new_table)``; ``new_table`` is the table after the update for ``grad_out`` ``[nbags, dim]``
+    (None without ``grad_out``)."""
+    t = table.detach().to(torch.float64).cpu()
+    d = t.shape[1] // 2
+    keys, offsets = keys.cpu(), offsets.cpu()
+    nb = offsets.numel() - 1
+    lens = offsets[1:] - offsets[:-1]
+    bag = torch.repeat_interleave(torch.arange(nb), lens)
+    c = per_sample_weights.detach().cpu().double() if per_sample_weights is not None else torch.ones(keys.numel(),
+                                                                                                    dtype=torch.float64)
+    if mode == "mean":
+        c = c / lens[bag].double()
+    out = torch.zeros(nb, d, dtype=torch.float64).index_add_(0, bag, c[:, None] * t[keys, :d])
+    if grad_out is None:
+        return out, None
+    uniq, inv = torch.unique(keys, return_inverse=True)
+    G = torch.zeros(uniq.numel(), d, dtype=torch.float64).index_add_(
+        0, inv, c[:, None] * grad_out.detach().cpu().double()[bag]) * grad_scale
+    acc = t[uniq, d:]
+    upd = torch.where(G != 0, -lr * G / torch.sqrt(acc + G * G), torch.zeros_like(G))
+    new = t.clone()
+    new[uniq, :d] += upd
+    new[uniq, d:] += G * G
+    return out, new
+
+
 class IntentPrepass:
     """Device-side pre-pass for ``Worker.intent`` (experimental; ``csrc/cuda/ops_intent.cu``).
 
