@@ -102,6 +102,7 @@ constexpr float kNoEntry = __builtin_huge_valf();
 struct ScoreOut {
   float* g0;                     // [n_pairs x d] the pair's center gradient
   float* snap;                   // [distinct centers x d] start-of-step embedding of each center, by compact id
+                                 // (the deterministic step keeps it right after g0 in one buffer)
   int* pcid;                     // [n_pairs] compact id of the pair's center
 };
 
@@ -484,13 +485,22 @@ __global__ void sgns_det_index_kernel(const __grid_constant__ Ctx c, const Key* 
   }
 }
 
-// SCATTER = false: cnt[id] = entries of key id. SCATTER = true: list / kid of CSR position off[id] + i, i < cnt[id],
-// hold the entries of key id; counts cnt back down to zero.
+// What one contribution (CSR position) adds to its key's row: g times vector vec of the step's vector buffer, which holds
+// the pairs' center gradients g0 (rows 0 .. n_pairs - 1) followed by the centers' start-of-step embeddings (rows
+// n_pairs + compact id). g is 1 for a center (its gradient is g0 itself), gs for a target, kNoEntry for nothing.
+struct alignas(8) GatherDesc {
+  float g;
+  int vec;
+};
+
+// SCATTER = false: cnt[id] = entries of key id. SCATTER = true: desc / kid of CSR position off[id] + i, i < cnt[id],
+// describe the entries of key id (from the score pass's gs and pcid); counts cnt back down to zero.
 template <bool SCATTER>
 __global__ void sgns_det_group_kernel(const Key* __restrict__ centers, const Key* __restrict__ contexts,
                                       const Key* __restrict__ negatives, int n_pairs, int neg,
                                       const int* __restrict__ cidx, int* __restrict__ cnt, const int* __restrict__ off,
-                                      int* __restrict__ list, int* __restrict__ kid) {
+                                      int* __restrict__ kid, const float* __restrict__ gsb,
+                                      const int* __restrict__ pcid, GatherDesc* __restrict__ desc) {
   const int n = n_pairs * (neg + 2);
   for (int x = blockIdx.x * blockDim.x + threadIdx.x; x < n; x += gridDim.x * blockDim.x) {
     const int p = x / (neg + 2), s = x - p * (neg + 2);
@@ -501,7 +511,16 @@ __global__ void sgns_det_group_kernel(const Key* __restrict__ centers, const Key
       atomicAdd(cnt + id, 1);
     } else {
       const int q = __ldg(off + id) + atomicSub(cnt + id, 1) - 1;
-      list[q] = x;
+      const float gx = __ldg(gsb + x);
+      GatherDesc e;
+      if (s == 0) {
+        e.g = gx == kNoEntry ? kNoEntry : 1.f;
+        e.vec = p;
+      } else {
+        e.g = gx;
+        e.vec = gx == kNoEntry ? 0 : n_pairs + __ldg(pcid + p);
+      }
+      desc[q] = e;
       kid[q] = id;
     }
   }
@@ -521,136 +540,203 @@ __device__ __forceinline__ void fx_terms(float gr, float a, float alpha, long lo
 // key is shared by the warps whose ranges it spans: each adds its int64 partial sums to the key's partial row - the
 // one of the first range boundary inside the key's entries - and sgns_det_finish_kernel applies it.
 // Within each half of a partial row, element 4j + c sits at c * d/4 + j (fx::pos), so a warp's atomics are contiguous.
+//
+// The warp first finds all keys of its range at once: the CSR is ordered by compact id, so a lane per position sees
+// where a key starts, and the keys' extents and rows are looked up together. It stages them and the range's entry
+// descriptors in shared memory. Rows and vectors then stream through two per-warp rings that the TMA engine fills
+// (cp.async.bulk, completion on an mbarrier) ahead of the math, as in the score pass: while the warp sums one key, the
+// rows of the next kGatherRows - 1 keys and the vectors of the next kGatherVecs entries are in flight. A light key's
+// update is written back from registers.
+// Little's law at d = 300 (2400-byte rows, 1200-byte vectors): 2 rows + 4 vectors = 9.6 KB in flight per warp, and
+// 16 warps per SM (2 blocks of 256 threads, 110 KB of shared memory and at most 128 registers each) keep about 150 KB
+// in flight per SM, 77 KB of it rows from HBM; 3.35 TB/s over 132 SMs needs about 25 KB per microsecond of latency.
+// Two blocks fit per SM up to d = 308; wider rows (up to d = 336, the widest the deterministic step takes) run one.
 constexpr int kGatherRange = 64;
-constexpr int kGatherUnroll = 2;   // entries whose loads are in flight together
+constexpr int kGatherRows = 3;                   // row ring slots
+constexpr int kGatherVecs = 4;                   // vector ring slots
+constexpr int kGatherDescs = 2 * kGatherRange;   // staged descriptors: the range and the rest of its last light key
+
+// shared memory of one gather warp: row ring | vector ring | descriptors | per key: row, start if heavy, end
+__host__ __device__ constexpr size_t gather_warp_bytes(int d) {
+  return ((size_t)kGatherRows * 2 * d + (size_t)kGatherVecs * d) * sizeof(float) + kGatherDescs * sizeof(GatherDesc) +
+         kGatherRange * (sizeof(float*) + 2 * sizeof(int));
+}
 
 template <int VPL>
 __global__ void __launch_bounds__(256, 2)
 sgns_det_gather_kernel(const __grid_constant__ Ctx c, float* const* __restrict__ rowp, const int* __restrict__ off,
-                       int n_ids, const int* __restrict__ list, const int* __restrict__ kid,
-                       const float* __restrict__ gsb, const float* __restrict__ g0b, const float* __restrict__ snap,
-                       const int* __restrict__ pcid, int neg, int d, float alpha, long long* __restrict__ part) {
-  constexpr int R = kGatherRange, U = kGatherUnroll;
+                       int n_ids, const int* __restrict__ kid, const GatherDesc* __restrict__ desc,
+                       const float* __restrict__ vecs, int d, float alpha, long long* __restrict__ part) {
+  constexpr int R = kGatherRange, NR = kGatherRows, NV = kGatherVecs;
+  constexpr unsigned kAll = 0xffffffffu;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  __shared__ unsigned long long bars[kWarps][NR + NV];
   dev::cta_enter(c);
   const int lane = threadIdx.x & 31;
+  const int wib = threadIdx.x >> 5;
   const int nvec = d >> 2;
   const int total = off[n_ids];
-  const int q0 = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * R;
+  const int q0 = (int)(blockIdx.x * kWarps + wib) * R;
   if (q0 < total) {
     const int q1 = min(q0 + R, total);
-    int q = q0;
-    {
-      const int id = kid[q];
-      const int s = off[id], e = off[id + 1];
-      if (s < q0 && e - s <= R) q = e;          // the rest of a light key that an earlier range owns
+    float* rring = reinterpret_cast<float*>(smem_raw + (size_t)wib * gather_warp_bytes(d));
+    float* vring = rring + (size_t)NR * 2 * d;
+    GatherDesc* dsm = reinterpret_cast<GatherDesc*>(vring + (size_t)NV * d);   // dsm[i]: CSR position q0 + i
+    float** krow = reinterpret_cast<float**>(dsm + kGatherDescs);              // key k of the warp: its row,
+    int* kheavy = reinterpret_cast<int*>(krow + R);                            // its first entry if heavy, else -1,
+    int* kend = kheavy + R;                                                    // and the end of its entries here
+    unsigned long long* rbar = bars[wib];
+    unsigned long long* vbar = rbar + NR;
+    if (lane == 0) {
+      for (int r = 0; r < NR + NV; ++r) mbar_init(&rbar[r], 1);
+      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
-    // lane l describes entry qc + l: factor g (1 for a center: its gradient is g0 itself) and the vector it scales
-    auto describe = [&](int qc, int n, float& g, const float*& vec) {
-      g = kNoEntry;
-      vec = snap;
-      if (lane < n) {
-        const int x = list[qc + lane];
-        const int p = x / (neg + 2);
-        const float gx = gsb[x];
-        if (x == p * (neg + 2)) {
-          g = gx == kNoEntry ? kNoEntry : 1.f;
-          vec = g0b + (size_t)p * d;
-        } else {
-          g = gx;
-          if (gx != kNoEntry) vec = snap + (size_t)pcid[p] * d;
-        }
-      }
-    };
-    while (q < q1) {
-      const int id = kid[q];
-      const int s = off[id], e = off[id + 1];
+
+    // ---- the keys of the range: lane l looks at positions q0 + l and q0 + 32 + l
+    const int ida = q0 + lane < q1 ? __ldg(kid + q0 + lane) : -1;
+    const int idb = q0 + 32 + lane < q1 ? __ldg(kid + q0 + 32 + lane) : -1;
+    for (int i = lane; i < kGatherDescs && q0 + i < total; i += 32) dsm[i] = desc[q0 + i];
+    const int prev_a = __shfl_up_sync(kAll, ida, 1), last_a = __shfl_sync(kAll, ida, 31);
+    const int prev_b = __shfl_up_sync(kAll, idb, 1);
+    // a key that starts at this position: its row, where its entries end in this warp, its first entry if heavy;
+    // false for the rest of a light key that an earlier range owns
+    auto key_at = [&](int id, bool start, float*& row, int& end, int& heavy_start) {
+      if (!start) return false;
+      const int s = __ldg(off + id), e = __ldg(off + id + 1);
+      row = rowp[id];
       const bool heavy = e - s > R;
-      const int qe = heavy ? min(e, q1) : e;
-      float* row = rowp[id];
-      // (the first chunk's descriptions load together with the row: they do not depend on it)
-      int n = min(32, qe - q);
-      float g;
-      const float* vec;
-      describe(q, n, g, vec);
-      float4 a[VPL];
-      long long se[VPL][4], sa[VPL][4];
+      end = heavy ? min(e, q1) : e;
+      heavy_start = heavy ? s : -1;
+      return heavy || s >= q0;
+    };
+    float *row_a = nullptr, *row_b = nullptr;
+    int end_a = 0, end_b = 0, hs_a = -1, hs_b = -1;
+    const bool in_a = key_at(ida, ida >= 0 && (lane == 0 || ida != prev_a), row_a, end_a, hs_a);
+    const bool in_b = key_at(idb, idb >= 0 && idb != (lane == 0 ? last_a : prev_b), row_b, end_b, hs_b);
+    const int qa = __shfl_sync(kAll, in_a ? q0 : end_a, 0);   // the first entry of the warp's first key
+    const unsigned ma = __ballot_sync(kAll, in_a), mb = __ballot_sync(kAll, in_b);
+    const unsigned below = (1u << lane) - 1u;
+    const int nk = __popc(ma) + __popc(mb);
+    if (in_a) {
+      const int k = __popc(ma & below);
+      krow[k] = row_a; kheavy[k] = hs_a; kend[k] = end_a;
+    }
+    if (in_b) {
+      const int k = __popc(ma) + __popc(mb & below);
+      krow[k] = row_b; kheavy[k] = hs_b; kend[k] = end_b;
+    }
+    __syncwarp();
+
+    if (nk > 0) {
+      // entries i = 0 .. ne - 1 of the warp are CSR positions qa + i, key after key
+      const int ne = kend[nk - 1] - qa;
+      const GatherDesc* dw = dsm + (qa - q0);
+      auto issue_row = [&](int k) {      // the row of key k into row slot k % NR (a heavy key: its AdaGrad half only)
+        if (lane != 0) return;
+        const int b = k % NR;
+        const float* row = krow[k];
+        if (!row) {
+          mbar_arrive(&rbar[b]);           // nothing to load: complete the phase
+          return;
+        }
+        const int h = kheavy[k] >= 0 ? d : 0;
+        const uint32_t bytes = (uint32_t)((2 * d - h) * sizeof(float));
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // earlier LDS of the slot before the TMA write
+        mbar_expect_tx(&rbar[b], bytes);
+        bulk_g2s(rring + (size_t)b * 2 * d + h, row + h, bytes, &rbar[b]);
+      };
+      auto issue_vec = [&](int i) {      // the vector of entry i into vector slot i % NV
+        if (lane != 0) return;
+        const int b = i % NV;
+        const GatherDesc e = dw[i];
+        if (e.g == kNoEntry) {
+          mbar_arrive(&vbar[b]);
+          return;
+        }
+        const uint32_t bytes = (uint32_t)(d * sizeof(float));
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        mbar_expect_tx(&vbar[b], bytes);
+        bulk_g2s(vring + (size_t)b * d, vecs + (size_t)e.vec * d, bytes, &vbar[b]);
+      };
+      for (int k = 0; k < min(nk, NR); ++k) issue_row(k);
+      for (int i = 0; i < min(ne, NV); ++i) issue_vec(i);
+
+      int i = 0;
+      for (int k = 0; k < nk; ++k) {
+        const int b = k % NR;
+        const float* rs = rring + (size_t)b * 2 * d;
+        float* row = krow[k];
+        const int heavy_start = kheavy[k];
+        const int ie_end = kend[k] - qa;
+        mbar_wait(&rbar[b], (uint32_t)(k / NR) & 1u);
+        float4 a[VPL];
+        long long se[VPL][4], sa[VPL][4];
 #pragma unroll
-      for (int v = 0; v < VPL; ++v) {
-        const int j = lane + v * 32;
-        a[v] = (j < nvec && row) ? dev::ld_row4_weak(row + d + 4 * j) : make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int v = 0; v < VPL; ++v) {
+          const int j = lane + v * 32;
+          a[v] = (j < nvec && row) ? reinterpret_cast<const float4*>(rs + d)[j] : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) se[v][k] = sa[v][k] = 0;
-      }
-      for (int qc = q;;) {
-        for (int k0 = 0; k0 < n; k0 += U) {
-          float gk[U];
-          float4 ev[U][VPL];
-#pragma unroll
-          for (int u = 0; u < U; ++u) {
-            gk[u] = __shfl_sync(0xffffffffu, g, (k0 + u) & 31);
-            const float* vk = (const float*)__shfl_sync(0xffffffffu, (unsigned long long)vec, (k0 + u) & 31);
-            if (k0 + u >= n) gk[u] = kNoEntry;
+          for (int q = 0; q < 4; ++q) se[v][q] = sa[v][q] = 0;
+        }
+        for (; i < ie_end; ++i) {
+          const int vb = i % NV;
+          const float g = dw[i].g;
+          mbar_wait(&vbar[vb], (uint32_t)(i / NV) & 1u);
+          if (g != kNoEntry) {
+            const float4* vs = reinterpret_cast<const float4*>(vring + (size_t)vb * d);
 #pragma unroll
             for (int v = 0; v < VPL; ++v) {
               const int j = lane + v * 32;
-              ev[u][v] = (j < nvec && gk[u] != kNoEntry) ? __ldg(reinterpret_cast<const float4*>(vk) + j)
-                                                          : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-          }
-#pragma unroll
-          for (int u = 0; u < U; ++u) {
-            if (gk[u] == kNoEntry) continue;
-#pragma unroll
-            for (int v = 0; v < VPL; ++v) {
-              if (lane + v * 32 < nvec) {
-                fx_terms(gk[u] * ev[u][v].x, a[v].x, alpha, se[v][0], sa[v][0]);
-                fx_terms(gk[u] * ev[u][v].y, a[v].y, alpha, se[v][1], sa[v][1]);
-                fx_terms(gk[u] * ev[u][v].z, a[v].z, alpha, se[v][2], sa[v][2]);
-                fx_terms(gk[u] * ev[u][v].w, a[v].w, alpha, se[v][3], sa[v][3]);
+              if (j < nvec) {
+                const float4 ev = vs[j];
+                fx_terms(g * ev.x, a[v].x, alpha, se[v][0], sa[v][0]);
+                fx_terms(g * ev.y, a[v].y, alpha, se[v][1], sa[v][1]);
+                fx_terms(g * ev.z, a[v].z, alpha, se[v][2], sa[v][2]);
+                fx_terms(g * ev.w, a[v].w, alpha, se[v][3], sa[v][3]);
               }
             }
           }
+          __syncwarp();                    // every lane has read vector slot vb
+          if (i + NV < ne) issue_vec(i + NV);
         }
-        qc += 32;
-        if (qc >= qe) break;
-        n = min(32, qe - qc);
-        describe(qc, n, g, vec);
-      }
-      if (heavy) {
-        unsigned long long* pr = reinterpret_cast<unsigned long long*>(part + (size_t)(s / R + 1) * (2 * d));
+        if (heavy_start >= 0) {
+          unsigned long long* pr = reinterpret_cast<unsigned long long*>(part + (size_t)(heavy_start / R + 1) * (2 * d));
 #pragma unroll
-        for (int v = 0; v < VPL; ++v) {
-          const int j = lane + v * 32;
-          if (j < nvec) {
+          for (int v = 0; v < VPL; ++v) {
+            const int j = lane + v * 32;
+            if (j < nvec) {
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              if (se[v][k]) atomicAdd(pr + k * nvec + j, (unsigned long long)se[v][k]);
-              if (sa[v][k]) atomicAdd(pr + d + k * nvec + j, (unsigned long long)sa[v][k]);
+              for (int q = 0; q < 4; ++q) {
+                if (se[v][q]) atomicAdd(pr + q * nvec + j, (unsigned long long)se[v][q]);
+                if (sa[v][q]) atomicAdd(pr + d + q * nvec + j, (unsigned long long)sa[v][q]);
+              }
+            }
+          }
+        } else if (row) {
+          // row += sum / scale; a zero sum leaves the element as it is (a -0.0 stays -0.0)
+          const double ie = 1.0 / (double)kFxEmb, ia = 1.0 / (double)kFxAda;
+#pragma unroll
+          for (int v = 0; v < VPL; ++v) {
+            const int j = lane + v * 32;
+            if (j < nvec) {
+              float4 r = reinterpret_cast<const float4*>(rs)[j];
+              float4 na = a[v];
+              float* rp = &r.x;
+              float* ap = &na.x;
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                if (se[v][q]) rp[q] += (float)((double)se[v][q] * ie);
+                if (sa[v][q]) ap[q] += (float)((double)sa[v][q] * ia);
+              }
+              reinterpret_cast<float4*>(row)[j] = r;
+              reinterpret_cast<float4*>(row + d)[j] = na;
             }
           }
         }
-      } else if (row) {
-        // row += sum / scale; a zero sum leaves the element as it is (a -0.0 stays -0.0)
-        const double ie = 1.0 / (double)kFxEmb, ia = 1.0 / (double)kFxAda;
-#pragma unroll
-        for (int v = 0; v < VPL; ++v) {
-          const int j = lane + v * 32;
-          if (j < nvec) {
-            float4 r = dev::ld_row4_weak(row + 4 * j);
-            float4 na = a[v];
-            float* rp = &r.x;
-            float* ap = &na.x;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              if (se[v][k]) rp[k] += (float)((double)se[v][k] * ie);
-              if (sa[v][k]) ap[k] += (float)((double)sa[v][k] * ia);
-            }
-            reinterpret_cast<float4*>(row)[j] = r;
-            reinterpret_cast<float4*>(row + d)[j] = na;
-          }
-        }
+        __syncwarp();                      // every lane has read row slot b
+        if (k + NR < nk) issue_row(k + NR);
       }
-      q = qe;
     }
   }
   dev::cta_exit(c);
@@ -697,7 +783,7 @@ __global__ void sgns_det_finish_kernel(const __grid_constant__ Ctx c, const Key*
 }
 
 // the backend's step buffers (CudaBackend::step_buffer) that the deterministic step uses
-enum StepBuf { kBufGs, kBufG0, kBufSnap, kBufPcid, kBufCnt, kBufOff, kBufList, kBufKid, kBufPart, kBufScan, kBufRowp };
+enum StepBuf { kBufGs, kBufVec, kBufPcid, kBufCnt, kBufOff, kBufDesc, kBufKid, kBufPart, kBufScan, kBufRowp };
 static_assert(kBufRowp < CudaBackend::kStepBuffers, "step buffers");
 
 // The deterministic one-GPU step: index -> score -> count, scan, scatter -> gather -> finish, all on `stream`.
@@ -713,12 +799,13 @@ void sgns_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   CudaBackend::FxScratch& fx = be.fx_scratch(0, (size_t)n_ids, 0);
   float* gsb = static_cast<float*>(be.step_buffer(kBufGs, (size_t)n_entries * sizeof(float)));
   ScoreOut so;
-  so.g0 = static_cast<float*>(be.step_buffer(kBufG0, (size_t)n_pairs * d * sizeof(float)));
-  so.snap = static_cast<float*>(be.step_buffer(kBufSnap, n_centers * d * sizeof(float)));
+  // one vector buffer: g0 of every pair, then the centers' snapshots (GatherDesc::vec is a row of it)
+  so.g0 = static_cast<float*>(be.step_buffer(kBufVec, ((size_t)n_pairs + n_centers) * d * sizeof(float)));
+  so.snap = so.g0 + (size_t)n_pairs * d;
   so.pcid = static_cast<int*>(be.step_buffer(kBufPcid, (size_t)n_pairs * sizeof(int)));
   int* cnt = static_cast<int*>(be.step_buffer(kBufCnt, ((size_t)n_ids + 1) * sizeof(int)));    // zero between steps
   int* off = static_cast<int*>(be.step_buffer(kBufOff, ((size_t)n_ids + 1) * sizeof(int)));
-  int* list = static_cast<int*>(be.step_buffer(kBufList, (size_t)n_entries * sizeof(int)));
+  GatherDesc* desc = static_cast<GatherDesc*>(be.step_buffer(kBufDesc, (size_t)n_entries * sizeof(GatherDesc)));
   int* kid = static_cast<int*>(be.step_buffer(kBufKid, (size_t)n_entries * sizeof(int)));
   long long* part = static_cast<long long*>(                                            // zero between steps
       be.step_buffer(kBufPart, ((size_t)n_ranges + 1) * 2 * d * sizeof(long long)));
@@ -755,18 +842,24 @@ void sgns_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, con
 #undef ADAPM_LAUNCH_SCORE
   ADAPM_COUNT_LAUNCH();
   sgns_det_group_kernel<false><<<blocks_for(n_entries), 256, 0, stream>>>(centers, contexts, negatives, n_pairs, neg,
-                                                                           fx.cidx, cnt, off, list, kid);
+                                                                           fx.cidx, cnt, off, kid, gsb, so.pcid, desc);
   ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, cnt, off, n_ids + 1, stream));
   ADAPM_COUNT_LAUNCH();
   ADAPM_COUNT_LAUNCH();   // (the scan is two kernels)
   sgns_det_group_kernel<true><<<blocks_for(n_entries), 256, 0, stream>>>(centers, contexts, negatives, n_pairs, neg,
-                                                                          fx.cidx, cnt, off, list, kid);
+                                                                          fx.cidx, cnt, off, kid, gsb, so.pcid, desc);
   ADAPM_COUNT_LAUNCH();
   const int gather_blocks = (n_ranges + kWarps - 1) / kWarps;
   const auto gather = vpl == 1 ? sgns_det_gather_kernel<1> : vpl == 2 ? sgns_det_gather_kernel<2> : sgns_det_gather_kernel<3>;
-  gather<<<gather_blocks, kThreads, 0, stream>>>(c, rowp, off, n_ids, list, kid, gsb, so.g0, so.snap, so.pcid, neg, d,
-                                                 alpha, part);
+  static bool gather_attr_set[4] = {};
+  if (!gather_attr_set[vpl]) {          // room for the largest row of this VPL (d = 128 VPL)
+    ADAPM_CUDA_CHECK(cudaFuncSetAttribute(gather, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)(kWarps * gather_warp_bytes(128 * vpl))));
+    gather_attr_set[vpl] = true;
+  }
+  gather<<<gather_blocks, kThreads, kWarps * gather_warp_bytes(d), stream>>>(c, rowp, off, n_ids, kid, desc, so.g0, d,
+                                                                             alpha, part);
   ADAPM_COUNT_LAUNCH();
   sgns_det_finish_kernel<<<blocks_for(n_entries), 256, 0, stream>>>(c, fx.keys, rowp, off, n_ids, kid, d, part, fx.cidx,
                                                                      fx.count, fx.loss, loss_out);

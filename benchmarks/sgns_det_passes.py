@@ -64,8 +64,9 @@ def pass_bytes(kc, d, neg):
         # gather-based step
         "index": slots * key + U * (key + 4),
         "score": U * half + P * half + C * half + slots * 4,                 # rows' embedding halves; g0, snapshot, gs
-        "group": 2 * slots * key + 2 * E * 8 + 3 * U * 4,                   # keys twice; list + kid; counts and scan
-        "gather": 2 * U * row + P * half + C * half + E * 12,               # rows read + written; g0, snapshot, gs/list/kid
+        "group": 2 * slots * key + 2 * E * 8 + E * 12 + 3 * U * 4,          # keys twice; descriptors + kid, gs + pcid
+                                                                            # read for them; counts and scan
+        "gather": 2 * U * row + P * half + C * half + E * 8,                # rows read + written; g0, snapshot; descriptors
         "finish": U * 12,
         # accumulator-based step
         "step": U * row + P * half + 2 * U * 2 * row,                       # rows; 8-byte accumulators read + written
