@@ -93,7 +93,8 @@ class CudaBackend : public Backend {
   // number of keys whose rows have `len` values (every key for a store of one row length)
   size_t keys_with_len(uint32_t len);
   // device buffer i (< kStepBuffers) of at least `bytes`, grown on demand and zero-filled when it grows (a buffer that
-  // its user leaves zero stays zero); scratch of the deterministic one-GPU SGNS step (ops_sgns_tma.cu)
+  // its user leaves zero stays zero); scratch of the deterministic one-GPU SGNS step (ops_sgns_tma.cu, buffers 0 - 9)
+  // and of the TransE step's generic path (ops_transe.cu, buffer 11)
   static constexpr int kStepBuffers = 12;
   void* step_buffer(int i, size_t bytes);
 

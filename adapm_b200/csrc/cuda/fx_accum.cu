@@ -12,19 +12,21 @@ namespace fx {
 namespace {
 
 struct Sources {
-  Source s[3];
+  Source s[4];
 };
 
 // Gives every key of the step a region of its own length: region offset = running total of the units handed out, or
 // r * units when every source has the same row length (uniform > 0: no second atomic on one counter).
 __global__ void fx_index_kernel(Sources src, int uniform, int* __restrict__ cidx, Key* __restrict__ keys,
                                 int2* __restrict__ rows, unsigned int* __restrict__ count) {
-  const long n0 = src.s[0].n, n1 = n0 + src.s[1].n, n = n1 + src.s[2].n;
+  const long n0 = src.s[0].n, n1 = n0 + src.s[1].n, n2 = n1 + src.s[2].n, n = n2 + src.s[3].n;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
     // (selected with conditionals: an indexed access would copy the sources to local memory)
-    const Key k = i < n0 ? src.s[0].keys[i] : (i < n1 ? src.s[1].keys[i - n0] : src.s[2].keys[i - n1]);
+    const Key k = i < n0 ? src.s[0].keys[i]
+                : (i < n1 ? src.s[1].keys[i - n0] : (i < n2 ? src.s[2].keys[i - n1] : src.s[3].keys[i - n2]));
     if (k >= 0 && atomicCAS(cidx + k, -1, -2) == -1) {
-      const int units = i < n0 ? src.s[0].units : (i < n1 ? src.s[1].units : src.s[2].units);
+      const int units = i < n0 ? src.s[0].units
+                      : (i < n1 ? src.s[1].units : (i < n2 ? src.s[2].units : src.s[3].units));
       const unsigned r = atomicAdd(count, 1u);
       const unsigned off = uniform ? r * (unsigned)uniform : atomicAdd(count + 1, (unsigned)units);
       keys[r] = k;
@@ -92,7 +94,7 @@ __global__ void fx_apply_kernel(const __grid_constant__ Ctx c, int unit, const K
 
 CudaBackend::FxScratch& begin(CudaBackend& be, cudaStream_t stream, const Source* src, int n_src, int unit,
                               long n_calls) {
-  ADAPM_CHECK(n_src >= 1 && n_src <= 3, "fx::begin: 1 to 3 key sources");
+  ADAPM_CHECK(n_src >= 1 && n_src <= 4, "fx::begin: 1 to 4 key sources");
   ADAPM_CHECK(be.ctx().L.world == 1, "deterministic steps need a single-GPU server (world == 1)");
   // scratch bound: per row length, min(keys of the step, keys of that length in the store)
   std::map<int, long> by_units;

@@ -53,7 +53,7 @@ struct Source {
   int units;
 };
 
-// Sizes the backend's scratch for a step over `src` (at most 3 sources; unit = row length in values of a 1-unit key)
+// Sizes the backend's scratch for a step over `src` (at most 4 sources; unit = row length in values of a 1-unit key)
 // and launches the index kernel on `stream`. n_calls > 0 also provides a per-call loss buffer (fx::apply reduces it).
 CudaBackend::FxScratch& begin(CudaBackend& be, cudaStream_t stream, const Source* src, int n_src, int unit,
                               long n_calls = 0);

@@ -47,6 +47,16 @@ void kge_rescal_step(CudaBackend& be, cudaStream_t stream, const Key* subj, cons
                      unsigned long long* stats, float dropout_e = 0.f, float dropout_r = 0.f, uint64_t seed = 0,
                      bool deterministic = false);
 
+// TransE: fused pull + L1/L2 distance + margin-ranking gradient + AdaGrad + push (ops_transe.cu). One positive triple
+// per (subj[i], rel[i], obj[i]) with neg[i * n_neg .. (i + 1) * n_neg) entity keys: the first half replaces the object,
+// the second the subject. Entity and relation rows are [embedding (d) | AdaGrad (d)], d % 4 == 0, 4 <= d <= 512;
+// entity rows are normalised on read. p = 1 or 2, n_neg <= 64. stats[3] counts the pushes issued.
+constexpr int kTransEMaxDim = 512;
+constexpr int kTransEMaxNeg = 64;
+void kge_transe_step(CudaBackend& be, cudaStream_t stream, const Key* subj, const Key* rel, const Key* obj,
+                     const Key* neg, int B, int n_neg, int d, int p, float margin, float eta, float gamma_e,
+                     float gamma_r, float* loss_out, unsigned long long* stats, bool deterministic = false);
+
 // matrix factorisation: fused pull + error + L2 + AdaGrad + push (ops_mf.cu)
 void mf_step(CudaBackend& be, cudaStream_t stream, const Key* row_keys, const Key* col_keys, const float* xs,
              const int* row_nnz, const int* col_nnz, int n, int rank, float eps, float lambda, float* loss_out,
@@ -78,6 +88,27 @@ void gemm_nt_topk(cudaStream_t stream, const void* A, const void* B, int M, int 
 // the same with E = rows(keys[0..N))[0..K) gathered from the parameter store (as gather_gemm); out_i are positions in keys
 void gather_gemm_topk(CudaBackend& be, cudaStream_t stream, const void* Q, const Key* keys, int M, int N, int K, int ldq,
                       int k, int S, const float* col_scale, const int64_t* ex_off, const int64_t* ex_cols, float* part_v,
+                      int* part_c, float* out_v, int64_t* out_i, unsigned long long* stats);
+// merges S sorted partial lists per row (part_v / part_c [M, S, k], column -1 = padding) into out_v / out_i [M, k]
+// with the order above
+void topk_merge(cudaStream_t stream, const float* part_v, const int* part_c, int M, int S, int k, float* out_v,
+                int64_t* out_i);
+
+// distance ranking and top-k against parameter-store rows on the CUDA cores (ops_dist.cu): D(i, j) = |q_i - e_j|_p,
+// p = 1 or 2, e_j = the first dim values of store row keys[j] (dim % 4 == 0), divided by max(|e_j|_2, 1e-12) when
+// normalize; each distance is an fp32 sum over the dim elements in order, bit-identical whichever CTA computes it.
+// Grid (M / 64 tiles) x S column slices. stats: (local rows, peer rows, rows that could not be resolved), accumulated.
+int dist_num_slices(CudaBackend& be, int M, int N, int max_tiles_per_cta);   // max_tiles_per_cta <= 0: unbounded
+// dtrue[i] = D(i, true_col[i]); raw[i] += #{j != true_col[i] : D(i, j) < dtrue[i]}; filt[i] the same without the
+// columns ex_cols[ex_off[i] .. ex_off[i + 1]) (raw, filt zeroed by the caller). 2 launches.
+void gather_dist_rank_count(CudaBackend& be, cudaStream_t stream, const float* q, const Key* keys, int M, int N, int dim,
+                            int p, bool normalize, int S, const int64_t* true_col, const int64_t* ex_off,
+                            const int64_t* ex_cols, float* dtrue, int64_t* raw, int64_t* filt,
+                            unsigned long long* stats);
+// per row the k (<= 64) columns of smallest distance: out_v = -D, out_i = column; ties to the smaller column, NaN never
+// selected, (-inf, -1) padding; exclusions as above. 2 launches (tiles, merge).
+void gather_dist_topk(CudaBackend& be, cudaStream_t stream, const float* q, const Key* keys, int M, int N, int dim, int p,
+                      bool normalize, int k, int S, const int64_t* ex_off, const int64_t* ex_cols, float* part_v,
                       int* part_c, float* out_v, int64_t* out_i, unsigned long long* stats);
 
 // multi-hot embedding bags over rows [embedding (E) | AdaGrad (E)] (ops_embbag.cu). CSR bags: keys[nnz],

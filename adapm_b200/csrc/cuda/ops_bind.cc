@@ -100,6 +100,33 @@ void bind(py::module_& m) {
                      ptr<const float>(col_scale), ptr<const int64_t>(ex_off), ptr<const int64_t>(ex_cols), ptr<float>(part_v),
                      ptr<int>(part_c), ptr<float>(out_v), ptr<int64_t>(out_i), ptr<unsigned long long>(stats));
   });
+  m.attr("transe_max_dim") = kTransEMaxDim;
+  m.attr("transe_max_neg") = kTransEMaxNeg;
+  m.def("kge_transe_step", [](uintptr_t be, uintptr_t stream, uintptr_t s, uintptr_t r, uintptr_t o, uintptr_t neg, int B,
+                              int n_neg, int d, int p, float margin, float eta, float gamma_e, float gamma_r, uintptr_t loss,
+                              uintptr_t stats, bool deterministic) {
+    kge_transe_step(backend_of(be), (cudaStream_t)stream, ptr<const Key>(s), ptr<const Key>(r), ptr<const Key>(o),
+                    ptr<const Key>(neg), B, n_neg, d, p, margin, eta, gamma_e, gamma_r, ptr<float>(loss),
+                    ptr<unsigned long long>(stats), deterministic);
+  });
+  m.def("dist_num_slices", [](uintptr_t be, int M, int N, int max_tiles_per_cta) {
+    return dist_num_slices(backend_of(be), M, N, max_tiles_per_cta);
+  });
+  m.def("gather_dist_rank_count", [](uintptr_t be, uintptr_t stream, uintptr_t q, uintptr_t keys, int M, int N, int dim,
+                                     int p, bool normalize, int S, uintptr_t true_col, uintptr_t ex_off, uintptr_t ex_cols,
+                                     uintptr_t dtrue, uintptr_t raw, uintptr_t filt, uintptr_t stats) {
+    gather_dist_rank_count(backend_of(be), (cudaStream_t)stream, ptr<const float>(q), ptr<const Key>(keys), M, N, dim, p,
+                           normalize, S, ptr<const int64_t>(true_col), ptr<const int64_t>(ex_off),
+                           ptr<const int64_t>(ex_cols), ptr<float>(dtrue), ptr<int64_t>(raw), ptr<int64_t>(filt),
+                           ptr<unsigned long long>(stats));
+  });
+  m.def("gather_dist_topk", [](uintptr_t be, uintptr_t stream, uintptr_t q, uintptr_t keys, int M, int N, int dim, int p,
+                               bool normalize, int k, int S, uintptr_t ex_off, uintptr_t ex_cols, uintptr_t part_v,
+                               uintptr_t part_c, uintptr_t out_v, uintptr_t out_i, uintptr_t stats) {
+    gather_dist_topk(backend_of(be), (cudaStream_t)stream, ptr<const float>(q), ptr<const Key>(keys), M, N, dim, p,
+                     normalize, k, S, ptr<const int64_t>(ex_off), ptr<const int64_t>(ex_cols), ptr<float>(part_v),
+                     ptr<int>(part_c), ptr<float>(out_v), ptr<int64_t>(out_i), ptr<unsigned long long>(stats));
+  });
   m.attr("embedding_bag_max_dim") = kEmbBagMaxDim;
   m.def("embedding_bag_workspace_bytes", [](int64_t nnz, int64_t nbags, int E) {
     return embedding_bag_workspace_bytes(nnz, nbags, E);

@@ -479,6 +479,13 @@ void gemm_nt_topk(cudaStream_t stream, const void* A, const void* B, int M, int 
   launch_merge(stream, a, out_v, out_i);
 }
 
+void topk_merge(cudaStream_t stream, const float* part_v, const int* part_c, int M, int S, int k, float* out_v,
+                int64_t* out_i) {
+  if (M == 0) return;
+  const TopkArgs a = make_args(M, 1, 1, k, S, nullptr, nullptr, nullptr, const_cast<float*>(part_v), const_cast<int*>(part_c));
+  launch_merge(stream, a, out_v, out_i);
+}
+
 void gather_gemm_topk(CudaBackend& be, cudaStream_t stream, const void* Q, const Key* keys, int M, int N, int K, int ldq,
                       int k, int S, const float* col_scale, const int64_t* ex_off, const int64_t* ex_cols, float* part_v,
                       int* part_c, float* out_v, int64_t* out_i, unsigned long long* stats) {

@@ -1,4 +1,4 @@
-"""Knowledge-graph embeddings (ComplEx, RESCAL) on the parameter manager.
+"""Knowledge-graph embeddings (ComplEx, RESCAL, TransE) on the parameter manager.
 
 Behavioural parity with the reference application ``apps/knowledge_graph_embeddings.cc``:
 
@@ -24,6 +24,12 @@ triple (kge.cc:716-774) and aggregates the reference's 19 metrics over the ranks
 (kge.cc:592-709). The CPU backend runs the same calls through the public Pull/Push API with PyTorch math
 (``kge_reference_step``, also the numerics oracle of the GPU tests).
 
+TransE (``algorithm="TransE"``, L1 or L2 by ``p_norm``) is the translational model of the reference's toy-data README:
+entity rows are normalised on read, a positive triple and its ``2 * neg_ratio`` negatives form margin-ranking pairs
+(``margin``), and one fused kernel per batch (``ops.kge_transe_step``) streams the negatives; the CPU route and the
+numerics oracle is ``ops.transe_reference_step``. Evaluation and prediction rank by distance: ``ops.gather_dist_rank_count``
+and ``ops.gather_dist_topk`` on the GPU, ``torch.cdist`` on the CPU.
+
 ``KGEConfig.deterministic`` selects the deterministic one-GPU variant of the fused kernels (start-of-step reads,
 fixed-point sums, bit-identical runs); the CPU backend accepts it and already follows the start-of-step rule.
 """
@@ -43,7 +49,7 @@ class KGEConfig:
     num_entities: int = 14951
     num_relations: int = 1345
     embed_dim: int = 512            # ComplEx: real half + imaginary half
-    algorithm: str = "ComplEx"      # ComplEx | RESCAL
+    algorithm: str = "ComplEx"      # ComplEx | RESCAL | TransE
     neg_ratio: int = 6
     eta: float = 0.1
     gamma_entity: float = 1e-3
@@ -58,6 +64,8 @@ class KGEConfig:
     init_std: float = 0.1
     model_seed: int = 134827
     deterministic: bool = False      # one GPU: start-of-step reads, bit-identical runs (ops.kge_complex_step)
+    p_norm: int = 1                  # TransE only: L1 or L2 distance
+    margin: float = 1.0              # TransE only: margin of the ranking loss
 
     @property
     def entity_len(self) -> int:
@@ -89,6 +97,7 @@ class KGEConfig:
 
     @property
     def updates_per_triple(self) -> int:
+        """ComplEx / RESCAL; a TransE triple pushes 3 rows plus one per active negative pair (count them instead)."""
         return 3 * (1 + 2 * self.neg_ratio)
 
 
@@ -125,6 +134,7 @@ class KGE:
         self.cuda = server.backend == "cuda" and server.dtype == torch.float32
         self.dtype = server.dtype
         self.step_no = 0
+        self.pushes = 0                 # TransE on the CPU route: rows pushed so far (3 per triple + active negatives)
         dev = server.device
         self._gen = torch.Generator().manual_seed(cfg.model_seed + 31 * server.my_rank())
         if self.cuda:
@@ -209,6 +219,8 @@ class KGE:
         """One batch of positive triples ([B,3] int64 CPU tensor, pinned for the e2e path)."""
         cfg = self.cfg
         B = triples_host.shape[0]
+        if cfg.algorithm == "TransE":
+            return self._step_transe(triples_host)
         if self.cuda:
             from ..ops import kge_complex_step, kge_rescal_step
 
@@ -225,6 +237,33 @@ class KGE:
         neg = torch.randint(0, cfg.num_entities, (B, 2 * cfg.neg_ratio), generator=self._gen)
         S, R, O, L = self._expand(triples_host, neg)
         loss = kge_reference_step(self.worker, S, R, O, L, cfg)
+        self.step_no += 1
+        return torch.tensor([loss], dtype=torch.float32)
+
+    def _step_transe(self, triples_host: torch.Tensor) -> torch.Tensor:
+        """TransE: one fused launch per batch on CUDA (``ops.kge_transe_step``), else ``ops.transe_reference_step``;
+        negatives ``[B, 2 * neg_ratio]`` in the layout of ``_expand`` (corrupted objects first)."""
+        from ..ops import kge_transe_step, transe_reference_step
+
+        cfg = self.cfg
+        if cfg.dropout_entity > 0 or cfg.dropout_relation > 0:
+            raise ValueError("dropout is not defined for TransE")
+        B, ne = triples_host.shape[0], cfg.num_entities
+        if self.cuda:
+            tr = triples_host.to(self.server.device, non_blocking=True)
+            local_only = cfg.sampling_scheme == "local" and self.server.num_servers() > 1
+            seed = (cfg.model_seed * 7 + self.server.my_rank() * 7919 + self.step_no) & 0xFFFFFFFFFFFF
+            neg = self.sampler.sample(B * 2 * cfg.neg_ratio, seed, local_only=local_only).view(B, 2 * cfg.neg_ratio)
+            kge_transe_step(self.server, tr[:, 0].contiguous(), (tr[:, 1] + ne).contiguous(), tr[:, 2].contiguous(), neg,
+                            cfg.embed_dim, cfg.p_norm, cfg.margin, cfg.eta, cfg.gamma_entity, cfg.gamma_relation,
+                            self.loss, self.stats, deterministic=cfg.deterministic)
+            self.step_no += 1
+            return self.loss
+        neg = torch.randint(0, ne, (B, 2 * cfg.neg_ratio), generator=self._gen)
+        loss, pushes = transe_reference_step(self.worker, triples_host[:, 0], triples_host[:, 1] + ne, triples_host[:, 2],
+                                             neg, cfg.embed_dim, cfg.p_norm, cfg.margin, cfg.eta, cfg.gamma_entity,
+                                             cfg.gamma_relation)
+        self.pushes += pushes
         self.step_no += 1
         return torch.tensor([loss], dtype=torch.float32)
 
@@ -268,6 +307,8 @@ class KGE:
         the relation rank unfiltered like in the reference. Returns a dict of int64 tensors
         ``rank_s, rank_r, rank_o, rank_s_raw, rank_o_raw``. ``known``: all true triples (train+valid+test)."""
         cfg = self.cfg
+        if cfg.algorithm == "TransE":
+            return self._rank_transe(triples, known, batch)
         dev = self.server.device if self.cuda else torch.device("cpu")
         E, _, R, _ = self.pull_embeddings(dev)
         triples = triples.to(dev)
@@ -333,6 +374,62 @@ class KGE:
             qr = bf(qr)
             true_score = (qr * R_s[t[:, 1]]).sum(1)
             out["rank_r"].append(count_better(qr, R_s, true_score, t[:, 1]))
+        return {k: torch.cat(v) if v else torch.zeros(0, dtype=torch.int64, device=dev) for k, v in out.items()}
+
+    def _transe_queries(self, Es, Rr, Eo):
+        """TransE queries from raw rows: (object side q = s^ + r, subject side q = o^ - r, relation side q = o^ - s^);
+        D(candidate) = |q - candidate|_p against normalised entities, or raw relations for the relation side."""
+        sh, oh = normalize_rows(Es), normalize_rows(Eo)
+        return (sh + Rr).contiguous(), (oh - Rr).contiguous(), (oh - sh).contiguous()
+
+    def _rank_transe(self, triples: torch.Tensor, known: torch.Tensor, batch: int) -> dict:
+        """``rank_triples`` for TransE: ranks by distance (a candidate is better when strictly closer), filtered by the
+        known answers. CUDA: ``ops.gather_dist_rank_count`` over the store rows with the exclusion CSR of
+        ``_known_answers``; CPU: ``torch.cdist`` over the pulled rows with the same rule."""
+        cfg = self.cfg
+        ne, nr, p = cfg.num_entities, cfg.num_relations, cfg.p_norm
+        out = {k: [] for k in ("rank_s", "rank_r", "rank_o", "rank_s_raw", "rank_o_raw")}
+        if self.cuda:
+            from ..ops import gather_dist_rank_count
+
+            dev, kv, d = self.server.device, self.worker, cfg.embed_dim
+            triples = triples.to(dev)
+            all_ent = torch.arange(ne, dtype=torch.int64, device=dev)
+            all_rel = torch.arange(ne, ne + nr, dtype=torch.int64, device=dev)
+
+            def pull_rows(keys):
+                buf = torch.empty(keys.numel() * 2 * d, dtype=torch.float32, device=dev)
+                kv.wait(kv.pull(keys.contiguous(), buf, True))
+                return buf.view(-1, 2 * d)[:, :d]
+
+            for i in range(0, triples.shape[0], batch):
+                t = triples[i:i + batch]
+                qo, qs, qr = self._transe_queries(pull_rows(t[:, 0]), pull_rows(t[:, 1] + ne), pull_rows(t[:, 2]))
+                for side, q, true_e, given in ((0, qo, t[:, 2], t[:, 0]), (1, qs, t[:, 0], t[:, 2])):
+                    excl = self._known_answers(given, t[:, 1], "object" if side == 0 else "subject", known)
+                    raw, filt = gather_dist_rank_count(self.server, q, all_ent, d, p, True, true_e.contiguous(), excl)
+                    out["rank_o_raw" if side == 0 else "rank_s_raw"].append(raw + 1)
+                    out["rank_o" if side == 0 else "rank_s"].append(filt + 1)
+                raw, _ = gather_dist_rank_count(self.server, qr, all_rel, d, p, False, t[:, 1].contiguous())
+                out["rank_r"].append(raw + 1)
+        else:
+            from ..ops import dist_rank_reference
+
+            E, _, R, _ = self.pull_embeddings()
+            E, R = E.double(), R.double()
+            En = normalize_rows(E)
+            for i in range(0, triples.shape[0], batch):
+                t = triples[i:i + batch]
+                qo, qs, qr = self._transe_queries(E[t[:, 0]], R[t[:, 1]], E[t[:, 2]])
+                for side, q, true_e, given in ((0, qo, t[:, 2], t[:, 0]), (1, qs, t[:, 0], t[:, 2])):
+                    off, cols = self._known_answers(given, t[:, 1], "object" if side == 0 else "subject", known)
+                    excluded = torch.zeros(t.shape[0], ne, dtype=torch.bool)
+                    excluded[torch.repeat_interleave(torch.arange(t.shape[0]), off[1:] - off[:-1]), cols] = True
+                    raw, filt = dist_rank_reference(q, En, p, true_e, excluded)
+                    out["rank_o_raw" if side == 0 else "rank_s_raw"].append(raw + 1)
+                    out["rank_o" if side == 0 else "rank_s"].append(filt + 1)
+                out["rank_r"].append(dist_rank_reference(qr, R, p, t[:, 1])[0] + 1)
+        dev = self.server.device if self.cuda else torch.device("cpu")
         return {k: torch.cat(v) if v else torch.zeros(0, dtype=torch.int64, device=dev) for k, v in out.items()}
 
     @staticmethod
@@ -439,6 +536,8 @@ class KGE:
         rels = torch.as_tensor(relations, dtype=torch.int64).reshape(-1)
         if ents.numel() != rels.numel():
             raise ValueError("entities and relations must have the same length")
+        if cfg.algorithm == "TransE":
+            return self._predict_transe(ents, rels, side, k, known)
         if self.cuda:
             from ..ops import gather_gemm_topk
 
@@ -468,6 +567,48 @@ class KGE:
             excluded[torch.repeat_interleave(torch.arange(ents.numel()), off[1:] - off[:-1]), cols] = True
         vals, idx = topk_reference(q @ E.t(), int(k), excluded)
         return idx, vals
+
+    def _predict_transe(self, ents, rels, side, k, known):
+        """``predict`` for TransE: the ``k`` nearest entities to ``s^ + r`` (objects) or ``o^ - r`` (subjects);
+        scores are ``-distance``. CUDA: ``ops.gather_dist_topk``; CPU: ``torch.cdist`` + ``ops.topk_reference``."""
+        cfg = self.cfg
+        d, ne, p = cfg.embed_dim, cfg.num_entities, cfg.p_norm
+        if self.cuda:
+            from ..ops import gather_dist_topk
+
+            dev, kv = self.server.device, self.worker
+            ents, rels = ents.to(dev), rels.to(dev)
+
+            def pull_rows(keys):
+                buf = torch.empty(keys.numel() * 2 * d, dtype=torch.float32, device=dev)
+                kv.wait(kv.pull(keys.contiguous(), buf, True))
+                return buf.view(-1, 2 * d)[:, :d]
+
+            e, r = pull_rows(ents), pull_rows(rels + ne)
+            q = (normalize_rows(e) + r) if side == "object" else (normalize_rows(e) - r)
+            excl = self._known_answers(ents, rels, side, known) if known is not None else None
+            vals, idx = gather_dist_topk(self.server, q.contiguous(), torch.arange(ne, dtype=torch.int64, device=dev), d,
+                                         k, p, True, exclude=excl)
+            return idx, vals
+        from ..ops import _check_topk, topk_reference
+
+        _check_topk(ents.numel(), ne, k, None, None)
+        E, _, R, _ = self.pull_embeddings()
+        E, R = E.float(), R.float()
+        En = normalize_rows(E)
+        q = (En[ents] + R[rels]) if side == "object" else (En[ents] - R[rels])
+        excluded = None
+        if known is not None:
+            off, cols = self._known_answers(ents, rels, side, known)
+            excluded = torch.zeros(ents.numel(), ne, dtype=torch.bool)
+            excluded[torch.repeat_interleave(torch.arange(ents.numel()), off[1:] - off[:-1]), cols] = True
+        vals, idx = topk_reference(-torch.cdist(q, En, p=float(p)), int(k), excluded)
+        return idx, vals
+
+
+def normalize_rows(e: torch.Tensor) -> torch.Tensor:
+    """e / max(|e|_2, 1e-12) per row: the entity rows TransE scores with."""
+    return e / e.norm(dim=-1, keepdim=True).clamp(min=1e-12)
 
 
 def complex_query(a: torch.Tensor, r: torch.Tensor, conj: bool) -> torch.Tensor:
@@ -557,6 +698,13 @@ def evaluate_fused(model: "KGE", triples: torch.Tensor, known: torch.Tensor, bat
     of the test triples concurrently."""
     from ..ops import gather_gemm_rank_count
 
+    if model.cfg.algorithm == "TransE":   # distance ranks from the store rows (ops.gather_dist_rank_count)
+        ranks = model.rank_triples(triples, known, batch)
+        rf = torch.cat([ranks["rank_o"], ranks["rank_s"]]).double()
+        rr = torch.cat([ranks["rank_o_raw"], ranks["rank_s_raw"]]).double()
+        return {"mrr": float((1 / rf).mean()), "mrr_raw": float((1 / rr).mean()),
+                "hits@1": float((rf <= 1).double().mean()), "hits@3": float((rf <= 3).double().mean()),
+                "hits@10": float((rf <= 10).double().mean()), "n": int(rf.numel() // 2)}
     cfg, kv, dev = model.cfg, model.worker, model.server.device
     d, ne = cfg.embed_dim, cfg.num_entities
     triples = triples.to(dev)

@@ -223,6 +223,213 @@ def kge_rescal_step(server, subj: torch.Tensor, rel: torch.Tensor, obj: torch.Te
                        float(dropout_relation), int(seed) & 0xFFFFFFFFFFFFFFFF, det)
 
 
+TRANSE_MAX_DIM = 512
+TRANSE_MAX_NEG = 64
+_NORM_EPS = 1e-12
+
+
+def _check_transe_shape(embed_dim: int, p: int) -> None:
+    if isinstance(embed_dim, bool) or int(embed_dim) != embed_dim or not (
+            4 <= int(embed_dim) <= TRANSE_MAX_DIM and int(embed_dim) % 4 == 0):
+        raise ValueError(f"embed_dim must be a multiple of 4 in [4, {TRANSE_MAX_DIM}], got {embed_dim}")
+    if p not in (1, 2) or isinstance(p, bool):
+        raise ValueError(f"p must be 1 or 2, got {p}")
+
+
+def kge_transe_step(server, subj: torch.Tensor, rel: torch.Tensor, obj: torch.Tensor, neg: torch.Tensor, embed_dim: int,
+                    p: int, margin: float, eta: float, gamma_entity: float, gamma_relation: float, loss: torch.Tensor,
+                    stats: Optional[torch.Tensor] = None, deterministic: bool = False) -> None:
+    """Fused TransE training step (csrc/cuda/ops_transe.cu) on ``server``'s store: one warp per positive triple
+    ``(subj[i], rel[i], obj[i])`` (store keys) with the entity keys ``neg[i]`` ([B, 2n]; the first n replace the object,
+    the last n the subject). Rows are ``[embedding (embed_dim) | AdaGrad (embed_dim)]``; entity rows are normalised on
+    read (``e / max(|e|_2, 1e-12)``), the store rows are never rescaled. The rule is :func:`transe_reference_step`'s:
+    margin-ranking loss ``sum_j max(0, margin + D_pos - D_neg_j)`` with ``D = |s^ + r - o^|_p``, one AdaGrad push per
+    row of the positive and one per negative of an active pair. ``loss``: float32[1], accumulated (+=); ``stats``:
+    optional int64[4] accumulated with (local rows, peer rows, slow-path rows, pushes issued).
+
+    ``deterministic=True`` (single-GPU servers only): start-of-step reads, fixed-point sums, bit-identical runs (three
+    launches instead of one); the AdaGrad increment of one push is clamped to 2^24 there (see ops_transe.cu)."""
+    _i64(subj, "subj"); _i64(rel, "rel"); _i64(obj, "obj"); _i64(neg, "neg"); _f32(loss, "loss")
+    _check_transe_shape(embed_dim, p)
+    B = subj.numel()
+    if not (rel.numel() == B and obj.numel() == B):
+        raise ValueError("subj, rel and obj must have the same length")
+    if neg.dim() != 2 or neg.shape[0] != B or neg.shape[1] % 2 or neg.shape[1] > TRANSE_MAX_NEG:
+        raise ValueError(f"neg must be [B, 2n] with 2n <= {TRANSE_MAX_NEG}, got {tuple(neg.shape)}")
+    if stats is not None and not (stats.is_cuda and stats.dtype == torch.int64 and stats.numel() >= 4):
+        raise TypeError("stats must be a CUDA int64 tensor with 4 entries")
+    det = _check_deterministic(server, deterministic)
+    _C.kge_transe_step(server._impl.backend_handle(), _stream(subj), subj.data_ptr(), rel.data_ptr(), obj.data_ptr(),
+                       neg.data_ptr(), B, int(neg.shape[1]), int(embed_dim), int(p), float(margin), float(eta),
+                       float(gamma_entity), float(gamma_relation), loss.data_ptr(),
+                       stats.data_ptr() if stats is not None else 0, det)
+
+
+def transe_reference_step(kv, subj: torch.Tensor, rel: torch.Tensor, obj: torch.Tensor, neg: torch.Tensor, embed_dim: int,
+                          p: int, margin: float, eta: float, gamma_entity: float, gamma_relation: float):
+    """The TransE rule of :func:`kge_transe_step` in float64 through Pull / Push (CPU servers, float64 rows, and the
+    oracle of the tests). Every row is read at the start of the step. Returns ``(loss, pushes)``.
+
+    Per positive triple with x = s^ + r - o^, D = |x|_p and u = dD/dx (sign(x) for p = 1, x / |x| for p = 2, 0 at 0):
+    a negative pair j is active when ``margin + D_pos - D_neg_j > 0``. The gradients of an active pair: object
+    corrupted - s^ and r get ``u - u_j``, o^ ``-u``, the negative's o'^ ``+u_j``; subject corrupted - s^ ``u``, r
+    ``u - u_j``, o^ ``u_j - u``, s'^ ``-u_j``. Through the normalisation ``g_e = (g_e^ - e^ (e^ . g_e^)) / max(|e|, 1e-12)``;
+    L2 adds ``gamma_entity * s``, ``gamma_relation * r``, ``gamma_entity * o`` on the raw rows. Pushes
+    ``[-eta g / sqrt(acc + g^2) | g^2]`` (0 where g == 0) with the pulled accumulator: s, r and o once per triple with their
+    summed gradients, every negative of an active pair once."""
+    _check_transe_shape(embed_dim, p)
+    d = int(embed_dim)
+    subj, rel, obj = (t.reshape(-1).cpu() for t in (subj, rel, obj))
+    neg = neg.cpu()
+    B, nn = neg.shape
+    n = nn // 2
+    f64 = torch.float64
+
+    def pull(keys):
+        v = torch.empty(keys.numel() * 2 * d, dtype=kv.server.dtype)
+        if keys.numel():
+            kv.wait(kv.pull(keys.contiguous(), v))
+        v = v.view(-1, 2 * d).to(f64)
+        return v[:, :d], v[:, d:]
+
+    def nrm(e):
+        inv = 1.0 / e.norm(dim=-1, keepdim=True).clamp(min=_NORM_EPS)
+        return e * inv, inv
+
+    def dist(x):
+        return x.abs().sum(-1) if p == 1 else x.norm(dim=-1)
+
+    def ddx(x, D):
+        if p == 1:
+            return torch.sign(x)
+        return torch.where(D.unsqueeze(-1) > 0, x / D.clamp(min=1e-300).unsqueeze(-1), torch.zeros_like(x))
+
+    def back(g_hat, e_hat, inv):
+        return (g_hat - e_hat * (e_hat * g_hat).sum(-1, keepdim=True)) * inv
+
+    Es, As = pull(subj)
+    Er, Ar = pull(rel)
+    Eo, Ao = pull(obj)
+    En, An = pull(neg.reshape(-1))
+    En, An = En.view(B, nn, d), An.view(B, nn, d)
+    sh, inv_s = nrm(Es)
+    oh, inv_o = nrm(Eo)
+    nh, inv_n = nrm(En)
+    x = sh + Er - oh
+    Dp = dist(x)
+    xn = torch.cat([(sh + Er).unsqueeze(1) - nh[:, :n], nh[:, n:] + (Er - oh).unsqueeze(1)], 1)
+    Dn = dist(xn)
+    term = margin + Dp.unsqueeze(1) - Dn
+    act = term > 0
+    loss = float(term.clamp(min=0).sum())
+    u = ddx(x, Dp)
+    un = ddx(xn, Dn) * act.unsqueeze(-1)
+    k = act.sum(1, keepdim=True).to(f64)
+    Uo, Us = un[:, :n].sum(1), un[:, n:].sum(1)
+    gs = back(k * u - Uo, sh, inv_s) + gamma_entity * Es
+    gr = k * u - Uo - Us + gamma_relation * Er
+    go = back(Us - k * u, oh, inv_o) + gamma_entity * Eo
+    gn = back(torch.cat([un[:, :n], -un[:, n:]], 1), nh, inv_n)
+
+    def upd(g, a):
+        ue = torch.where(g != 0, -eta * g / torch.sqrt(a + g * g), torch.zeros_like(g))
+        return torch.cat([ue, g * g], -1).to(kv.server.dtype).contiguous().view(-1)
+
+    kv.wait(kv.push(subj.contiguous(), upd(gs, As)))
+    kv.wait(kv.push(rel.contiguous(), upd(gr, Ar)))
+    kv.wait(kv.push(obj.contiguous(), upd(go, Ao)))
+    sel = act.reshape(-1)
+    if bool(sel.any()):
+        kv.wait(kv.push(neg.reshape(-1)[sel].contiguous(), upd(gn.reshape(-1, d)[sel], An.reshape(-1, d)[sel])))
+    return loss, 3 * B + int(sel.sum())
+
+
+def _dist_operands(server, q, keys, dim, p, exclude, stats, M):
+    _i64(keys, "keys")
+    _check_transe_shape(dim, p)
+    if q.dim() != 2 or q.shape[1] != int(dim):
+        raise ValueError(f"q must be a matrix [M, dim = {dim}]")
+    if not (q.is_cuda and q.device == keys.device):
+        raise TypeError("q must be a CUDA tensor on the device of keys")
+    _f32(q, "q")
+    if stats is not None and not (stats.is_cuda and stats.dtype == torch.int64 and stats.numel() >= 2):
+        raise TypeError("stats must be a CUDA int64 tensor with 2 entries")
+    _check_topk(M, keys.numel(), 1, exclude, None)
+    _, eo, ec = _topk_operands(q.device, exclude, None)
+    if q.data_ptr() % 16:              # the kernels read q in 16-byte vectors: a view at an odd offset is copied
+        q = q.clone()
+    return q, eo, ec
+
+
+def _dist_slices(server, M, N):
+    return _C.dist_num_slices(server._impl.backend_handle(), M, N, _TOPK_GRACE_TILES if server.num_servers() > 1 else 0)
+
+
+def gather_dist_rank_count(server, q: torch.Tensor, keys: torch.Tensor, dim: int, p: int, normalize: bool,
+                           true_col: torch.Tensor, exclude=None, stats: Optional[torch.Tensor] = None):
+    """Rank counts by distance against parameter-store rows (csrc/cuda/ops_dist.cu): with ``D(i, j) = |q_i - e_j|_p``
+    (fp32 on the CUDA cores, ``e_j`` = the first ``dim`` values of store row ``keys[j]``, divided by
+    ``max(|e_j|_2, 1e-12)`` when ``normalize``), returns int64 ``(raw, filtered)`` [M] with
+    ``raw[i] = #{j != true_col[i] : D(i, j) < D(i, true_col[i])}`` and ``filtered`` the same without the columns of the
+    CSR ``exclude = (offsets int64 [M + 1], cols int64 [nnz])`` (ascending per row, as for :func:`gather_gemm_topk`).
+    The true distance comes from the kernel's own distance function, bit-identical to the column's. ``stats``: as for
+    :func:`gather_gemm`; on several ranks the call waits and raises ``RuntimeError`` if a row could not be resolved."""
+    M = q.shape[0] if q.dim() == 2 else 0
+    q, eo, ec = _dist_operands(server, q, keys, dim, p, exclude, stats, M)
+    _i64(true_col, "true_col")
+    if true_col.numel() != M:
+        raise ValueError(f"true_col must have M = {M} entries")
+    N = keys.numel()
+    raw = torch.zeros(M, dtype=torch.int64, device=q.device)
+    filt = torch.zeros(M, dtype=torch.int64, device=q.device)
+    if M == 0:
+        return raw, filt
+    if N == 0 or bool(((true_col < 0) | (true_col >= N)).any()):
+        raise ValueError("true_col entries must be column indices in [0, N)")
+    dtrue = torch.empty(M, dtype=torch.float32, device=q.device)
+    own = _gather_stats(server, stats, q.device)
+    _C.gather_dist_rank_count(server._impl.backend_handle(), _stream(q), q.data_ptr(), keys.data_ptr(), M, N, int(dim),
+                              int(p), bool(normalize), _dist_slices(server, M, N), true_col.data_ptr(), eo, ec,
+                              dtrue.data_ptr(), raw.data_ptr(), filt.data_ptr(), own.data_ptr() if own is not None else 0)
+    _gathered("gather_dist_rank_count", own, stats)
+    return raw, filt
+
+
+def gather_dist_topk(server, q: torch.Tensor, keys: torch.Tensor, dim: int, k: int, p: int, normalize: bool,
+                     exclude=None, stats: Optional[torch.Tensor] = None):
+    """The ``k`` columns of smallest distance per query (the distances of :func:`gather_dist_rank_count`): returns
+    ``(values = -D fp32 [M, k], indices int64 [M, k])`` with :func:`gather_gemm_topk`'s conventions - smallest distance
+    first, ties to the smaller column, NaN never selected, ``(-inf, -1)`` padding, ``1 <= k <= 64``, exclusions as a
+    CSR; indices are positions into ``keys``. Per-slice lists are merged by the top-k merge kernel."""
+    M = q.shape[0] if q.dim() == 2 else 0
+    if isinstance(k, bool) or int(k) != k or not 1 <= int(k) <= TOPK_MAX_K:
+        raise ValueError(f"k must be an integer in [1, {TOPK_MAX_K}], got {k}")
+    q, eo, ec = _dist_operands(server, q, keys, dim, p, exclude, stats, M)
+    k, N = int(k), keys.numel()
+    if M == 0 or N == 0:
+        return _topk_empty(M, k, q.device)
+    S = _dist_slices(server, M, N)
+    part_v, part_c, vals, idx = _topk_outputs(M, S, k, q.device)
+    own = _gather_stats(server, stats, q.device)
+    _C.gather_dist_topk(server._impl.backend_handle(), _stream(q), q.data_ptr(), keys.data_ptr(), M, N, int(dim), int(p),
+                        bool(normalize), k, S, eo, ec, part_v.data_ptr(), part_c.data_ptr(), vals.data_ptr(),
+                        idx.data_ptr(), own.data_ptr() if own is not None else 0)
+    _gathered("gather_dist_topk", own, stats)
+    return vals, idx
+
+
+def dist_rank_reference(q: torch.Tensor, e: torch.Tensor, p: int, true_col: torch.Tensor, excluded=None):
+    """PyTorch ``cdist`` ranking with the rule of :func:`gather_dist_rank_count` on dense candidates ``e`` [N, dim]
+    (already normalised if wanted): ``(raw, filtered)`` int64 [M]; ``excluded``: bool [M, N] or None."""
+    D = torch.cdist(q, e, p=float(p))
+    dt = D.gather(1, true_col.view(-1, 1))
+    better = D < dt
+    better.scatter_(1, true_col.view(-1, 1), False)
+    raw = better.sum(1)
+    filt = (better & ~excluded).sum(1) if excluded is not None else raw.clone()
+    return raw, filt
+
+
 def _mix32(x: torch.Tensor) -> torch.Tensor:
     m = 0xFFFFFFFF
     x = x & m
