@@ -24,9 +24,12 @@ def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--dataset", default=None, help="directory with train.del / valid.del / test.del (s r o per line)")
     ap.add_argument("--synthetic", type=int, default=0, help="number of synthetic training triples")
-    ap.add_argument("--algorithm", default="ComplEx", choices=["ComplEx", "RESCAL", "TransE"])
+    ap.add_argument("--algorithm", default="ComplEx", choices=["ComplEx", "RESCAL", "TransE", "RotatE"])
     ap.add_argument("--transe_norm", type=int, default=1, choices=[1, 2], help="TransE: L1 or L2 distance")
-    ap.add_argument("--margin", type=float, default=1.0, help="TransE: margin of the ranking loss")
+    ap.add_argument("--margin", type=float, default=1.0,
+                    help="TransE: margin of the ranking loss; RotatE: gamma of the sigmoid loss")
+    ap.add_argument("--adversarial_temperature", type=float, default=1.0,
+                    help="RotatE: temperature alpha of the self-adversarial negative weights (0: uniform weights)")
     ap.add_argument("--embed_dim", type=int, default=10)
     ap.add_argument("--num_threads", "-t", type=int, default=1)
     ap.add_argument("--num_epochs", type=int, default=10)
@@ -74,7 +77,8 @@ def main(argv=None) -> int:
                     dropout_relation=args.dropout_relation, batch_triples=args.batch_triples,
                     read_ahead=args.signal_intent_ahead, sampling_scheme=getattr(args, "sampling.scheme") or "local",
                     signal_initial_relations_intent=bool(args.signal_initial_relations_intent), model_seed=args.model_seed,
-                    deterministic=bool(args.deterministic), p_norm=args.transe_norm, margin=args.margin)
+                    deterministic=bool(args.deterministic), p_norm=args.transe_norm, margin=args.margin,
+                    adversarial_temperature=args.adversarial_temperature)
     if args.write_embeddings and not args.model_path:
         os.makedirs(args.write_embeddings, exist_ok=True)
         args.model_path = os.path.join(args.write_embeddings, "")
@@ -144,7 +148,7 @@ def main(argv=None) -> int:
         kv.barrier()
         total = ps_allreduce(kv, cfg.loss_key, torch.tensor([bce, 0.0]))     # loss all-reduce through the PS
         if rank == 0:
-            kind = "margin" if cfg.algorithm == "TransE" else "bce"
+            kind = {"TransE": "margin", "RotatE": "self-adversarial"}.get(cfg.algorithm, "bce")
             print(f"[kge] epoch {epoch}: {kind} loss {float(total[0]):.4f} ({time.time() - t0:.1f}s)", flush=True)
         if args.eval_freq > 0 and epoch % args.eval_freq == 0:
             ev = model.evaluate_distributed(va, known)
@@ -156,8 +160,8 @@ def main(argv=None) -> int:
         if time.time() - t0 > args.max_runtime:
             break
     if rank == 0:
-        if model.cuda and cfg.algorithm in ("ComplEx", "TransE") and cfg.embed_dim % 4 == 0:
-            # fused gather + wgmma GEMM (ComplEx) or distance kernel (TransE) + rank count: entity rows are read from
+        if model.cuda and cfg.algorithm in ("ComplEx", "TransE", "RotatE") and cfg.embed_dim % 4 == 0:
+            # fused gather + wgmma GEMM (ComplEx) or distance kernel (TransE, RotatE) + rank count: entity rows are read from
             # every GPU's HBM in-kernel
             print(f"[kge] test (fused gather-GEMM eval): {evaluate_fused(model, te, known)}", flush=True)
     ev = model.evaluate_distributed(te, known)

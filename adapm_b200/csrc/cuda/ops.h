@@ -57,6 +57,16 @@ void kge_transe_step(CudaBackend& be, cudaStream_t stream, const Key* subj, cons
                      const Key* neg, int B, int n_neg, int d, int p, float margin, float eta, float gamma_e,
                      float gamma_r, float* loss_out, unsigned long long* stats, bool deterministic = false);
 
+// RotatE: fused pull + complex rotation + sigmoid loss with self-adversarial negative weights + AdaGrad + push
+// (ops_rotate.cu). Triples and negatives as for TransE. Entity rows are [z (d) | AdaGrad (d)] with z interleaved
+// (re, im), relation rows [phases (d / 2) | AdaGrad (d / 2)]; d % 8 == 0, 8 <= d <= 512, 2 <= n_neg <= 256.
+// stats[3] counts the pushes issued (3 + n_neg per triple).
+constexpr int kRotatEMaxDim = 512;
+constexpr int kRotatEMaxNeg = 256;
+void kge_rotate_step(CudaBackend& be, cudaStream_t stream, const Key* subj, const Key* rel, const Key* obj,
+                     const Key* neg, int B, int n_neg, int d, float margin, float alpha, float eta, float gamma_e,
+                     float* loss_out, unsigned long long* stats, bool deterministic = false);
+
 // matrix factorisation: fused pull + error + L2 + AdaGrad + push (ops_mf.cu)
 void mf_step(CudaBackend& be, cudaStream_t stream, const Key* row_keys, const Key* col_keys, const float* xs,
              const int* row_nnz, const int* col_nnz, int n, int rank, float eps, float lambda, float* loss_out,
@@ -96,8 +106,10 @@ void topk_merge(cudaStream_t stream, const float* part_v, const int* part_c, int
 
 // distance ranking and top-k against parameter-store rows on the CUDA cores (ops_dist.cu): D(i, j) = |q_i - e_j|_p,
 // p = 1 or 2, e_j = the first dim values of store row keys[j] (dim % 4 == 0), divided by max(|e_j|_2, 1e-12) when
-// normalize; each distance is an fp32 sum over the dim elements in order, bit-identical whichever CTA computes it.
+// normalize; p = kDistComplex: the sum of complex moduli sum_k |(q - e)_{2k} + i (q - e)_{2k+1}| (never normalised);
+// each distance is an fp32 sum over the dim elements in order, bit-identical whichever CTA computes it.
 // Grid (M / 64 tiles) x S column slices. stats: (local rows, peer rows, rows that could not be resolved), accumulated.
+constexpr int kDistComplex = 3;
 int dist_num_slices(CudaBackend& be, int M, int N, int max_tiles_per_cta);   // max_tiles_per_cta <= 0: unbounded
 // dtrue[i] = D(i, true_col[i]); raw[i] += #{j != true_col[i] : D(i, j) < dtrue[i]}; filt[i] the same without the
 // columns ex_cols[ex_off[i] .. ex_off[i + 1]) (raw, filt zeroed by the caller). 2 launches.

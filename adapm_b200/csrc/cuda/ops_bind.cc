@@ -109,6 +109,15 @@ void bind(py::module_& m) {
                     ptr<const Key>(neg), B, n_neg, d, p, margin, eta, gamma_e, gamma_r, ptr<float>(loss),
                     ptr<unsigned long long>(stats), deterministic);
   });
+  m.attr("rotate_max_dim") = kRotatEMaxDim;
+  m.attr("rotate_max_neg") = kRotatEMaxNeg;
+  m.def("kge_rotate_step", [](uintptr_t be, uintptr_t stream, uintptr_t s, uintptr_t r, uintptr_t o, uintptr_t neg, int B,
+                              int n_neg, int d, float margin, float alpha, float eta, float gamma_e, uintptr_t loss,
+                              uintptr_t stats, bool deterministic) {
+    kge_rotate_step(backend_of(be), (cudaStream_t)stream, ptr<const Key>(s), ptr<const Key>(r), ptr<const Key>(o),
+                    ptr<const Key>(neg), B, n_neg, d, margin, alpha, eta, gamma_e, ptr<float>(loss),
+                    ptr<unsigned long long>(stats), deterministic);
+  });
   m.def("dist_num_slices", [](uintptr_t be, int M, int N, int max_tiles_per_cta) {
     return dist_num_slices(backend_of(be), M, N, max_tiles_per_cta);
   });

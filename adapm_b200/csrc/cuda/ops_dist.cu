@@ -1,9 +1,13 @@
-// Distance ranking and top-k against parameter-store rows on the CUDA cores (sm_90a), for translational models (TransE):
+// Distance ranking and top-k against parameter-store rows on the CUDA cores (sm_90a), for translational models (TransE,
+// RotatE):
 //     D(i, j) = |q_i - e_j|_p,  p = 1 or 2,  e_j = first `dim` values of store row keys[j]  [/ max(|e_j|_2, 1e-12)]
+//     D(i, j) = sum_k sqrt((q_2k - e_2k)^2 + (q_2k+1 - e_2k+1)^2)  (p = kDistComplex: complex moduli of interleaved
+//               (re, im) rows, never normalised)
 // without an [M, N] distance matrix. L1 has no tensor-core form, and the L2 expansion |q|^2 - 2 q.e + |e|^2 loses too
 // much in bf16 to count ranks, so the distances are fp32 sums on the CUDA cores.
 //
-// Every distance is summed by one thread over k = 0 .. dim-1 in order with explicitly rounded operations, and every row
+// Every distance is summed by one thread over k = 0 .. dim-1 (pairs k = 0 .. dim/2-1) in order with explicitly rounded
+// operations, and every row
 // norm by four threads in a fixed pattern, so D(i, j) is bit-identical whichever CTA (or the true-distance kernel)
 // computes it.
 //
@@ -99,7 +103,12 @@ __device__ __forceinline__ float dterm(float acc, float q, float e) {
   return P == 1 ? __fadd_rn(acc, fabsf(df)) : __fmaf_rn(df, df, acc);
 }
 template <int P>
-__device__ __forceinline__ float dfinish(float acc) { return P == 1 ? acc : __fsqrt_rn(acc); }
+__device__ __forceinline__ float dfinish(float acc) { return P == 2 ? __fsqrt_rn(acc) : acc; }
+// one term of a complex-modulus sum: acc + |(q0 - e0) + i (q1 - e1)|
+__device__ __forceinline__ float cterm(float acc, float q0, float e0, float q1, float e1) {
+  const float d0 = __fsub_rn(q0, e0), d1 = __fsub_rn(q1, e1);
+  return __fadd_rn(acc, __fsqrt_rn(__fmaf_rn(d0, d0, __fmul_rn(d1, d1))));
+}
 
 __device__ __forceinline__ bool beats(float v, uint32_t c, float tv, uint32_t tc) {
   return v > tv || (v == tv && c < tc);
@@ -158,6 +167,21 @@ __device__ __forceinline__ void dist_tile(DistSmem& sm, const Ctx& c, const Dist
     sm.es[8 * g + 4][r] = v1.x; sm.es[8 * g + 5][r] = v1.y; sm.es[8 * g + 6][r] = v1.z; sm.es[8 * g + 7][r] = v1.w;
     __syncthreads();
     const int kn = min(DKC, a.dim - k0);
+    if (P == kDistComplex) {
+      for (int kk = 0; kk < kn; kk += 2) {
+        const float4 q0 = *reinterpret_cast<const float4*>(&sm.qs[kk][4 * ty]);
+        const float4 e0 = *reinterpret_cast<const float4*>(&sm.es[kk][4 * tx]);
+        const float4 q1 = *reinterpret_cast<const float4*>(&sm.qs[kk + 1][4 * ty]);
+        const float4 e1 = *reinterpret_cast<const float4*>(&sm.es[kk + 1][4 * tx]);
+        const float qa[4] = {q0.x, q0.y, q0.z, q0.w}, ea[4] = {e0.x, e0.y, e0.z, e0.w};
+        const float qb[4] = {q1.x, q1.y, q1.z, q1.w}, eb[4] = {e1.x, e1.y, e1.z, e1.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) d[i][j] = cterm(d[i][j], qa[i], ea[j], qb[i], eb[j]);
+      }
+      continue;
+    }
     for (int kk = 0; kk < kn; ++kk) {
       const float4 qv = *reinterpret_cast<const float4*>(&sm.qs[kk][4 * ty]);
       const float4 ev = *reinterpret_cast<const float4*>(&sm.es[kk][4 * tx]);
@@ -190,9 +214,8 @@ __device__ __forceinline__ void flush_stats(unsigned long long* stats, unsigned 
 
 // Dt[i] = D(i, true_col[i]) with the distance function of the tiles: four threads per query, thread 0 of the group sums
 template <int P>
-__global__ void __launch_bounds__(128)
-dist_true_kernel(const __grid_constant__ Ctx c, const __grid_constant__ DistArgs a, float* __restrict__ dtrue,
-                 unsigned long long* __restrict__ stats) {
+__device__ __forceinline__ void dist_true_run(const Ctx& c, const DistArgs& a, float* __restrict__ dtrue,
+                                              unsigned long long* __restrict__ stats) {
   dev::cta_enter(c);
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 2, g = threadIdx.x & 3;
   unsigned nl = 0, nr = 0, nu = 0;
@@ -210,8 +233,12 @@ dist_true_kernel(const __grid_constant__ Ctx c, const __grid_constant__ DistArgs
         if (a.normalize)
           v = make_float4(__fmul_rn(v.x, inv), __fmul_rn(v.y, inv), __fmul_rn(v.z, inv), __fmul_rn(v.w, inv));
         const float4 qv = __ldg(reinterpret_cast<const float4*>(a.q + (size_t)i * a.dim + k));
-        acc = dterm<P>(acc, qv.x, v.x); acc = dterm<P>(acc, qv.y, v.y);
-        acc = dterm<P>(acc, qv.z, v.z); acc = dterm<P>(acc, qv.w, v.w);
+        if (P == kDistComplex) {
+          acc = cterm(acc, qv.x, v.x, qv.y, v.y); acc = cterm(acc, qv.z, v.z, qv.w, v.w);
+        } else {
+          acc = dterm<P>(acc, qv.x, v.x); acc = dterm<P>(acc, qv.y, v.y);
+          acc = dterm<P>(acc, qv.z, v.z); acc = dterm<P>(acc, qv.w, v.w);
+        }
       }
     } while (dev::gather_reread(c, key, row));
     dtrue[i] = dfinish<P>(acc);
@@ -221,8 +248,7 @@ dist_true_kernel(const __grid_constant__ Ctx c, const __grid_constant__ DistArgs
 }
 
 template <int P>
-__global__ void __launch_bounds__(kDistThreads, 1)
-dist_rank_kernel(const __grid_constant__ Ctx c, const __grid_constant__ DistArgs a, unsigned long long* __restrict__ stats) {
+__device__ __forceinline__ void dist_rank_run(const Ctx& c, const DistArgs& a, unsigned long long* __restrict__ stats) {
   __shared__ __align__(16) DistSmem sm;
   dev::cta_enter(c);
   const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
@@ -285,8 +311,7 @@ __device__ __forceinline__ void list_insert(TopkLists& L, int k, int r, float v,
 }
 
 template <int P>
-__global__ void __launch_bounds__(kDistThreads, 1)
-dist_topk_kernel(const __grid_constant__ Ctx c, const __grid_constant__ DistArgs a, unsigned long long* __restrict__ stats) {
+__device__ __forceinline__ void dist_topk_run(const Ctx& c, const DistArgs& a, unsigned long long* __restrict__ stats) {
   extern __shared__ __align__(16) unsigned char dist_smem[];
   DistSmem& sm = *reinterpret_cast<DistSmem*>(dist_smem);
   TopkLists& L = *reinterpret_cast<TopkLists*>(dist_smem + sizeof(DistSmem));
@@ -349,10 +374,42 @@ dist_topk_kernel(const __grid_constant__ Ctx c, const __grid_constant__ DistArgs
   dev::cta_exit(c);
 }
 
+// The kernels: L1 / L2 (P = 1, 2) and the complex metric (cdist_*)
+template <int P>
+__global__ void __launch_bounds__(128)
+dist_true_kernel(const __grid_constant__ Ctx c, const __grid_constant__ DistArgs a, float* __restrict__ dtrue,
+                 unsigned long long* __restrict__ stats) {
+  dist_true_run<P>(c, a, dtrue, stats);
+}
+template <int P>
+__global__ void __launch_bounds__(kDistThreads, 1)
+dist_rank_kernel(const __grid_constant__ Ctx c, const __grid_constant__ DistArgs a, unsigned long long* __restrict__ stats) {
+  dist_rank_run<P>(c, a, stats);
+}
+template <int P>
+__global__ void __launch_bounds__(kDistThreads, 1)
+dist_topk_kernel(const __grid_constant__ Ctx c, const __grid_constant__ DistArgs a, unsigned long long* __restrict__ stats) {
+  dist_topk_run<P>(c, a, stats);
+}
+__global__ void __launch_bounds__(128)
+cdist_true_kernel(const __grid_constant__ Ctx c, const __grid_constant__ DistArgs a, float* __restrict__ dtrue,
+                  unsigned long long* __restrict__ stats) {
+  dist_true_run<kDistComplex>(c, a, dtrue, stats);
+}
+__global__ void __launch_bounds__(kDistThreads, 1)
+cdist_rank_kernel(const __grid_constant__ Ctx c, const __grid_constant__ DistArgs a, unsigned long long* __restrict__ stats) {
+  dist_rank_run<kDistComplex>(c, a, stats);
+}
+__global__ void __launch_bounds__(kDistThreads, 1)
+cdist_topk_kernel(const __grid_constant__ Ctx c, const __grid_constant__ DistArgs a, unsigned long long* __restrict__ stats) {
+  dist_topk_run<kDistComplex>(c, a, stats);
+}
+
 DistArgs make_args(const float* q, const Key* keys, int M, int N, int dim, int p, bool normalize, int S,
                    const int64_t* ex_off, const int64_t* ex_cols) {
   ADAPM_CHECK(dim >= 4 && dim % 4 == 0, "gather_dist: dim must be a positive multiple of 4");
-  ADAPM_CHECK(p == 1 || p == 2, "gather_dist: p must be 1 or 2");
+  ADAPM_CHECK(p == 1 || p == 2 || p == kDistComplex, "gather_dist: p must be 1, 2 or kDistComplex");
+  ADAPM_CHECK(p != kDistComplex || !normalize, "gather_dist: the complex metric does not normalise rows");
   ADAPM_CHECK(S >= 1 && S <= kMaxSlices, "gather_dist: bad slice count " << S);
   DistArgs a{};
   a.q = q; a.keys = keys; a.M = M; a.N = N; a.dim = dim; a.p = p; a.S = S; a.normalize = normalize;
@@ -382,12 +439,14 @@ void gather_dist_rank_count(CudaBackend& be, cudaStream_t stream, const float* q
   be.track_stream(stream);
   const int tb = (M * 4 + 127) / 128;
   if (p == 1) dist_true_kernel<1><<<tb, 128, 0, stream>>>(be.ctx(), a, dtrue, stats);
-  else dist_true_kernel<2><<<tb, 128, 0, stream>>>(be.ctx(), a, dtrue, stats);
+  else if (p == 2) dist_true_kernel<2><<<tb, 128, 0, stream>>>(be.ctx(), a, dtrue, stats);
+  else cdist_true_kernel<<<tb, 128, 0, stream>>>(be.ctx(), a, dtrue, stats);
   ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cudaGetLastError());
   const dim3 grid((M + DB - 1) / DB, S);
   if (p == 1) dist_rank_kernel<1><<<grid, kDistThreads, 0, stream>>>(be.ctx(), a, stats);
-  else dist_rank_kernel<2><<<grid, kDistThreads, 0, stream>>>(be.ctx(), a, stats);
+  else if (p == 2) dist_rank_kernel<2><<<grid, kDistThreads, 0, stream>>>(be.ctx(), a, stats);
+  else cdist_rank_kernel<<<grid, kDistThreads, 0, stream>>>(be.ctx(), a, stats);
   ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cudaGetLastError());
 }
@@ -407,11 +466,14 @@ void gather_dist_topk(CudaBackend& be, cudaStream_t stream, const float* q, cons
   if (!attr_set) {
     ADAPM_CUDA_CHECK(cudaFuncSetAttribute(dist_topk_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     ADAPM_CUDA_CHECK(cudaFuncSetAttribute(dist_topk_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    ADAPM_CUDA_CHECK(
+        cudaFuncSetAttribute(cdist_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
   const dim3 grid((M + DB - 1) / DB, S);
   if (p == 1) dist_topk_kernel<1><<<grid, kDistThreads, smem, stream>>>(be.ctx(), a, stats);
-  else dist_topk_kernel<2><<<grid, kDistThreads, smem, stream>>>(be.ctx(), a, stats);
+  else if (p == 2) dist_topk_kernel<2><<<grid, kDistThreads, smem, stream>>>(be.ctx(), a, stats);
+  else cdist_topk_kernel<<<grid, kDistThreads, smem, stream>>>(be.ctx(), a, stats);
   ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cudaGetLastError());
   topk_merge(stream, part_v, part_c, M, S, k, out_v, out_i);

@@ -26,6 +26,7 @@
 #include <algorithm>
 
 #include "fx_accum.cuh"
+#include "kge_step.cuh"
 #include "ops.h"
 #include "pm_kernels.cuh"
 
@@ -49,23 +50,10 @@ constexpr float kFxVal = 1099511627776.f;     // 2^40
 constexpr float kFxAda = 268435456.f;         // 2^28
 constexpr float kFxAdaMax = 16777216.f;       // 2^24
 
-__device__ __forceinline__ float4 f4(float v) { return make_float4(v, v, v, v); }
-__device__ __forceinline__ float4 add4(float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
-__device__ __forceinline__ float4 sub4(float4 a, float4 b) { return make_float4(a.x - b.x, a.y - b.y, a.z - b.z, a.w - b.w); }
-__device__ __forceinline__ float4 mul4(float4 a, float s) { return make_float4(a.x * s, a.y * s, a.z * s, a.w * s); }
-__device__ __forceinline__ float dot4(float4 a, float4 b) { return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w; }
-__device__ __forceinline__ float4 ld4(const float* p, int j) { return *reinterpret_cast<const float4*>(p + 4 * j); }
-__device__ __forceinline__ void st4(float* p, int j, float4 v) { *reinterpret_cast<float4*>(p + 4 * j) = v; }
+using namespace kge;
+
 __device__ __forceinline__ float sgn(float v) { return v > 0.f ? 1.f : (v < 0.f ? -1.f : 0.f); }
 
-template <int VPL>
-__device__ __forceinline__ void load_row(const float* row, int nv, int lane, float4 (&v)[VPL]) {
-#pragma unroll
-  for (int i = 0; i < VPL; ++i) {
-    const int j = lane + 32 * i;
-    v[i] = j < nv ? dev::ld_row4(row + 4 * j) : f4(0.f);
-  }
-}
 // 1 / max(|v|_2, eps)
 template <int VPL>
 __device__ __forceinline__ float inv_norm(const float4 (&v)[VPL]) {
@@ -88,31 +76,6 @@ template <int P>
 __device__ __forceinline__ float4 ddx(float4 x, float inv_d) {
   if (P == 1) return make_float4(sgn(x.x), sgn(x.y), sgn(x.z), sgn(x.w));
   return mul4(x, inv_d);
-}
-
-// AdaGrad push of gradient g onto float4 j of a row [emb (d) | acc (d)]: in place (REDs), onto a staged copy (the
-// generic path pushes it afterwards) or into the key's fixed-point region.
-template <bool FX>
-__device__ __forceinline__ void push4(float* row, int d, int j, float4 g, bool staged, long long* region, int nv,
-                                      float eta) {
-  const float4 a = dev::ld_row4(row + d + 4 * j);
-  const float4 ua = make_float4(g.x * g.x, g.y * g.y, g.z * g.z, g.w * g.w);
-  const float4 ue = make_float4(g.x != 0.f ? -eta * g.x * rsqrtf(a.x + ua.x) : 0.f,
-                                g.y != 0.f ? -eta * g.y * rsqrtf(a.y + ua.y) : 0.f,
-                                g.z != 0.f ? -eta * g.z * rsqrtf(a.z + ua.z) : 0.f,
-                                g.w != 0.f ? -eta * g.w * rsqrtf(a.w + ua.w) : 0.f);
-  if (FX) {
-    fx::add4(region, j, nv, ue, kFxVal);
-    fx::add4(region + d, j, nv,
-             make_float4(fminf(ua.x, kFxAdaMax), fminf(ua.y, kFxAdaMax), fminf(ua.z, kFxAdaMax), fminf(ua.w, kFxAdaMax)),
-             kFxAda);
-  } else if (staged) {
-    *reinterpret_cast<float4*>(row + 4 * j) = ue;
-    *reinterpret_cast<float4*>(row + d + 4 * j) = ua;
-  } else {
-    dev::red_row4(row + 4 * j, ue);
-    dev::red_row4(row + d + 4 * j, ua);
-  }
 }
 
 // gradient of a raw entity row from the gradient gh of its normalised copy eh = e * inv: (gh - eh (eh . gh)) * inv
@@ -220,7 +183,7 @@ __device__ __forceinline__ TripleOut triple_body(const Ctx& c, const Args& A, in
 #pragma unroll
     for (int i = 0; i < VPL; ++i) {
       const int j = lane + 32 * i;
-      if (j < nv) push4<FX>(pn, d, j, v[i], GEN && nslow, rg, nv, A.eta);
+      if (j < nv) push4<FX>(pn, d, j, v[i], GEN && nslow, rg, nv, A.eta, kFxVal, kFxAda, kFxAdaMax);
     }
     if (GEN && nslow && !FX) {
       if (dev::slow_push(c, kn, pn)) ++out.upd;
@@ -251,7 +214,7 @@ __device__ __forceinline__ TripleOut triple_body(const Ctx& c, const Args& A, in
 #pragma unroll
   for (int i = 0; i < VPL; ++i) {
     const int j = lane + 32 * i;
-    if (j < nv) push4<FX>(ps, d, j, add4(v[i], mul4(e[i], A.gamma_e)), slow, fs, nv, A.eta);
+    if (j < nv) push4<FX>(ps, d, j, add4(v[i], mul4(e[i], A.gamma_e)), slow, fs, nv, A.eta, kFxVal, kFxAda, kFxAdaMax);
   }
   load_row<VPL>(pr, nv, lane, e);
 #pragma unroll
@@ -259,7 +222,7 @@ __device__ __forceinline__ TripleOut triple_body(const Ctx& c, const Args& A, in
     const int j = lane + 32 * i;
     if (j < nv) {
       const float4 gr = sub4(sub4(mul4(ddx<P>(ld4(sx, j), inv_dp), kf), ld4(suo, j)), ld4(sus, j));
-      push4<FX>(pr, d, j, add4(gr, mul4(e[i], A.gamma_r)), slow, fr, nv, A.eta);
+      push4<FX>(pr, d, j, add4(gr, mul4(e[i], A.gamma_r)), slow, fr, nv, A.eta, kFxVal, kFxAda, kFxAdaMax);
     }
   }
 #pragma unroll
@@ -272,7 +235,7 @@ __device__ __forceinline__ TripleOut triple_body(const Ctx& c, const Args& A, in
 #pragma unroll
   for (int i = 0; i < VPL; ++i) {
     const int j = lane + 32 * i;
-    if (j < nv) push4<FX>(po, d, j, add4(v[i], mul4(e[i], A.gamma_e)), slow, fo, nv, A.eta);
+    if (j < nv) push4<FX>(po, d, j, add4(v[i], mul4(e[i], A.gamma_e)), slow, fo, nv, A.eta, kFxVal, kFxAda, kFxAdaMax);
   }
   __syncwarp();
   return out;

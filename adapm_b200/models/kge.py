@@ -1,4 +1,4 @@
-"""Knowledge-graph embeddings (ComplEx, RESCAL, TransE) on the parameter manager.
+"""Knowledge-graph embeddings (ComplEx, RESCAL, TransE, RotatE) on the parameter manager.
 
 Behavioural parity with the reference application ``apps/knowledge_graph_embeddings.cc``:
 
@@ -30,6 +30,15 @@ entity rows are normalised on read, a positive triple and its ``2 * neg_ratio`` 
 numerics oracle is ``ops.transe_reference_step``. Evaluation and prediction rank by distance: ``ops.gather_dist_rank_count``
 and ``ops.gather_dist_topk`` on the GPU, ``torch.cdist`` on the CPU.
 
+RotatE (``algorithm="RotatE"``) rotates the subject by the relation in the complex plane: entity rows hold ``embed_dim / 2``
+complex values interleaved ``(re, im)``, relation rows ``embed_dim / 2`` phases in radians (``relation_len =
+embed_dim``), and ``D = sum_i |s_i e^{i theta_i} - o_i|``. A positive triple and its ``2 * neg_ratio`` negatives train with
+the sigmoid loss and self-adversarial negative weights (``margin`` is gamma, ``adversarial_temperature`` alpha) in one
+fused kernel per batch (``ops.kge_rotate_step``); the CPU route and the numerics oracle is ``ops.rotate_reference_step``.
+Subject and object ranks and predictions use the complex metric of ``ops.gather_dist_rank_count`` /
+``ops.gather_dist_topk`` with ``p="complex"`` (``ops.complex_dist`` on the CPU); the relation side is computed in PyTorch.
+``gamma_relation`` is not used by RotatE (phases get no L2).
+
 ``KGEConfig.deterministic`` selects the deterministic one-GPU variant of the fused kernels (start-of-step reads,
 fixed-point sums, bit-identical runs); the CPU backend accepts it and already follows the start-of-step rule.
 """
@@ -49,7 +58,7 @@ class KGEConfig:
     num_entities: int = 14951
     num_relations: int = 1345
     embed_dim: int = 512            # ComplEx: real half + imaginary half
-    algorithm: str = "ComplEx"      # ComplEx | RESCAL | TransE
+    algorithm: str = "ComplEx"      # ComplEx | RESCAL | TransE | RotatE
     neg_ratio: int = 6
     eta: float = 0.1
     gamma_entity: float = 1e-3
@@ -65,7 +74,8 @@ class KGEConfig:
     model_seed: int = 134827
     deterministic: bool = False      # one GPU: start-of-step reads, bit-identical runs (ops.kge_complex_step)
     p_norm: int = 1                  # TransE only: L1 or L2 distance
-    margin: float = 1.0              # TransE only: margin of the ranking loss
+    margin: float = 1.0              # TransE: margin of the ranking loss; RotatE: gamma of the sigmoid loss
+    adversarial_temperature: float = 1.0   # RotatE only: alpha of the self-adversarial negative weights (0: uniform)
 
     @property
     def entity_len(self) -> int:
@@ -73,6 +83,8 @@ class KGEConfig:
 
     @property
     def relation_len(self) -> int:
+        if self.algorithm == "RotatE":   # [phases (d / 2) | AdaGrad (d / 2)]
+            return self.embed_dim
         return 2 * self.embed_dim * (self.embed_dim if self.algorithm == "RESCAL" else 1)
 
     @property
@@ -97,7 +109,8 @@ class KGEConfig:
 
     @property
     def updates_per_triple(self) -> int:
-        """ComplEx / RESCAL; a TransE triple pushes 3 rows plus one per active negative pair (count them instead)."""
+        """ComplEx / RESCAL; a TransE triple pushes 3 rows plus one per active negative pair (count them instead), a
+        RotatE triple 3 + 2 * neg_ratio rows."""
         return 3 * (1 + 2 * self.neg_ratio)
 
 
@@ -129,6 +142,10 @@ def load_triples(path: str) -> torch.Tensor:
 class KGE:
     def __init__(self, server, worker, cfg: KGEConfig):
         self.server, self.worker, self.cfg = server, worker, cfg
+        if cfg.algorithm == "RotatE":
+            from ..ops import _check_rotate_shape
+
+            _check_rotate_shape(cfg.embed_dim)
         # the fused kernels are float32; float64 rows (the reference's ValT = double, kge.cc:33) train through the
         # Pull / Push API with the same update rule (kge_reference_step) on either backend
         self.cuda = server.backend == "cuda" and server.dtype == torch.float32
@@ -154,7 +171,8 @@ class KGE:
     # ------------------------------------------------------------------ init
     def init_model(self, chunk: int = 8192, init: str = "") -> None:
         """``init``: the reference's ``init_parameters`` syntax - ``normal{mean/std}`` (default ``normal{0/init_std}``),
-        ``uniform{a/b}`` or ``none``; AdaGrad accumulators start at 1e-6."""
+        ``uniform{a/b}`` or ``none``; AdaGrad accumulators start at 1e-6. RotatE: the entity rows follow ``init``, the
+        relation phases are drawn uniform in [-pi, pi) (``none`` skips both)."""
         cfg, world, rank = self.cfg, self.server.num_servers(), self.server.my_rank()
         kind, p1, p2 = "normal", 0.0, cfg.init_std
         if init:
@@ -181,7 +199,10 @@ class KGE:
             for i in range(0, keys.numel(), per):
                 k = keys[i:i + per]
                 rows = torch.empty(k.numel(), ln, dtype=self.dtype)
-                if kind == "normal":
+                if cfg.algorithm == "RotatE" and first == cfg.num_entities:
+                    rows[:, : ln // 2] = ((torch.rand(k.numel(), ln // 2, generator=gen, dtype=torch.float64) * 2 - 1)
+                                          * np.pi).to(self.dtype)
+                elif kind == "normal":
                     rows[:, : ln // 2] = (torch.randn(k.numel(), ln // 2, generator=gen) * p2 + p1).to(self.dtype)
                 else:
                     rows[:, : ln // 2] = (torch.rand(k.numel(), ln // 2, generator=gen) * (p2 - p1) + p1).to(self.dtype)
@@ -221,6 +242,8 @@ class KGE:
         B = triples_host.shape[0]
         if cfg.algorithm == "TransE":
             return self._step_transe(triples_host)
+        if cfg.algorithm == "RotatE":
+            return self._step_rotate(triples_host)
         if self.cuda:
             from ..ops import kge_complex_step, kge_rescal_step
 
@@ -267,6 +290,33 @@ class KGE:
         self.step_no += 1
         return torch.tensor([loss], dtype=torch.float32)
 
+    def _step_rotate(self, triples_host: torch.Tensor) -> torch.Tensor:
+        """RotatE: one fused launch per batch on CUDA (``ops.kge_rotate_step``), else ``ops.rotate_reference_step``;
+        negatives ``[B, 2 * neg_ratio]`` in the layout of ``_expand`` (corrupted objects first)."""
+        from ..ops import kge_rotate_step, rotate_reference_step
+
+        cfg = self.cfg
+        if cfg.dropout_entity > 0 or cfg.dropout_relation > 0:
+            raise ValueError("dropout is not defined for RotatE")
+        B, ne = triples_host.shape[0], cfg.num_entities
+        if self.cuda:
+            tr = triples_host.to(self.server.device, non_blocking=True)
+            local_only = cfg.sampling_scheme == "local" and self.server.num_servers() > 1
+            seed = (cfg.model_seed * 7 + self.server.my_rank() * 7919 + self.step_no) & 0xFFFFFFFFFFFF
+            neg = self.sampler.sample(B * 2 * cfg.neg_ratio, seed, local_only=local_only).view(B, 2 * cfg.neg_ratio)
+            kge_rotate_step(self.server, tr[:, 0].contiguous(), (tr[:, 1] + ne).contiguous(), tr[:, 2].contiguous(), neg,
+                            cfg.embed_dim, cfg.margin, cfg.adversarial_temperature, cfg.eta, cfg.gamma_entity,
+                            self.loss, self.stats, deterministic=cfg.deterministic)
+            self.step_no += 1
+            return self.loss
+        neg = torch.randint(0, ne, (B, 2 * cfg.neg_ratio), generator=self._gen)
+        loss, pushes = rotate_reference_step(self.worker, triples_host[:, 0], triples_host[:, 1] + ne, triples_host[:, 2],
+                                             neg, cfg.embed_dim, cfg.margin, cfg.adversarial_temperature, cfg.eta,
+                                             cfg.gamma_entity)
+        self.pushes += pushes
+        self.step_no += 1
+        return torch.tensor([loss], dtype=torch.float32)
+
     # ------------------------------------------------------------------ full-model pull (eval / checkpoints)
     def pull_embeddings(self, device=None):
         """Returns (E [ne, d], Eg [ne, d], R [nr, rel_dim], Rg) by pulling the whole model through the API."""
@@ -284,6 +334,9 @@ class KGE:
         return tuple(t.to(device) for t in out) if device is not None else out
 
     def save(self, path_prefix: str, epoch: int, write_checkpoint: bool = False) -> None:
+        """``export.epoch.N.{entities,relations}.bin`` (float32 embedding halves) and, with ``write_checkpoint``, the
+        float64 ``checkpoint.epoch.N.*`` files with the AdaGrad halves. RotatE: entity rows are interleaved
+        ``(re_0, im_0, re_1, im_1, ...)`` and relation exports hold the ``embed_dim / 2`` phases in radians."""
         self.worker.wait_sync()
         if self.server.my_rank() != 0:
             return
@@ -309,6 +362,8 @@ class KGE:
         cfg = self.cfg
         if cfg.algorithm == "TransE":
             return self._rank_transe(triples, known, batch)
+        if cfg.algorithm == "RotatE":
+            return self._rank_rotate(triples, known, batch)
         dev = self.server.device if self.cuda else torch.device("cpu")
         E, _, R, _ = self.pull_embeddings(dev)
         triples = triples.to(dev)
@@ -432,6 +487,60 @@ class KGE:
         dev = self.server.device if self.cuda else torch.device("cpu")
         return {k: torch.cat(v) if v else torch.zeros(0, dtype=torch.int64, device=dev) for k, v in out.items()}
 
+    def _rank_rotate(self, triples: torch.Tensor, known: torch.Tensor, batch: int) -> dict:
+        """``rank_triples`` for RotatE: ranks by the complex distance (a candidate is better when strictly closer),
+        subject and object filtered by the known answers. Object side q = s o rho, subject side q = o o conj(rho) (exact,
+        |rho_i| = 1), against the raw entity rows: CUDA ``ops.gather_dist_rank_count(p="complex")`` over the store rows,
+        CPU ``ops.dist_rank_reference`` in float64. Relation side: D(r') = sum_i |s_i rho'_i - o_i| depends on the
+        candidate's phases, so it is computed in PyTorch on the pulled relation rows (fp32 on the GPU, float64 on the CPU,
+        chunked; ``_rotate_relation_ranks``)."""
+        cfg = self.cfg
+        ne, nr, d = cfg.num_entities, cfg.num_relations, cfg.embed_dim
+        out = {k: [] for k in ("rank_s", "rank_r", "rank_o", "rank_s_raw", "rank_o_raw")}
+        if self.cuda:
+            from ..ops import gather_dist_rank_count
+
+            dev, kv = self.server.device, self.worker
+            triples = triples.to(dev)
+            all_ent = torch.arange(ne, dtype=torch.int64, device=dev)
+
+            def pull_rows(keys, ln):
+                buf = torch.empty(keys.numel() * 2 * ln, dtype=torch.float32, device=dev)
+                kv.wait(kv.pull(keys.contiguous(), buf, True))
+                return buf.view(-1, 2 * ln)[:, :ln]
+
+            R = pull_rows(torch.arange(ne, ne + nr, dtype=torch.int64, device=dev), d // 2)   # all phases
+            for i in range(0, triples.shape[0], batch):
+                t = triples[i:i + batch]
+                Es, Eo, th = pull_rows(t[:, 0], d), pull_rows(t[:, 2], d), R[t[:, 1]]
+                for side, q, true_e, given in ((0, rotate_query(Es, th, False), t[:, 2], t[:, 0]),
+                                               (1, rotate_query(Eo, th, True), t[:, 0], t[:, 2])):
+                    excl = self._known_answers(given, t[:, 1], "object" if side == 0 else "subject", known)
+                    raw, filt = gather_dist_rank_count(self.server, q, all_ent, d, "complex", False, true_e.contiguous(),
+                                                       excl)
+                    out["rank_o_raw" if side == 0 else "rank_s_raw"].append(raw + 1)
+                    out["rank_o" if side == 0 else "rank_s"].append(filt + 1)
+                out["rank_r"].append(_rotate_relation_ranks(Es, Eo, R, t[:, 1]) + 1)
+        else:
+            from ..ops import dist_rank_reference
+
+            E, _, R, _ = self.pull_embeddings()
+            E, R = E.double(), R.double()
+            for i in range(0, triples.shape[0], batch):
+                t = triples[i:i + batch]
+                Es, Eo, th = E[t[:, 0]], E[t[:, 2]], R[t[:, 1]]
+                for side, q, true_e, given in ((0, rotate_query(Es, th, False), t[:, 2], t[:, 0]),
+                                               (1, rotate_query(Eo, th, True), t[:, 0], t[:, 2])):
+                    off, cols = self._known_answers(given, t[:, 1], "object" if side == 0 else "subject", known)
+                    excluded = torch.zeros(t.shape[0], ne, dtype=torch.bool)
+                    excluded[torch.repeat_interleave(torch.arange(t.shape[0]), off[1:] - off[:-1]), cols] = True
+                    raw, filt = dist_rank_reference(q, E, "complex", true_e, excluded)
+                    out["rank_o_raw" if side == 0 else "rank_s_raw"].append(raw + 1)
+                    out["rank_o" if side == 0 else "rank_s"].append(filt + 1)
+                out["rank_r"].append(_rotate_relation_ranks(Es, Eo, R, t[:, 1]) + 1)
+        dev = self.server.device if self.cuda else torch.device("cpu")
+        return {k: torch.cat(v) if v else torch.zeros(0, dtype=torch.int64, device=dev) for k, v in out.items()}
+
     @staticmethod
     def _metric_sums(ranks: dict) -> torch.Tensor:
         """The 19 partial sums of the reference (EVAL_METRICS order) as a float64 vector."""
@@ -538,6 +647,8 @@ class KGE:
             raise ValueError("entities and relations must have the same length")
         if cfg.algorithm == "TransE":
             return self._predict_transe(ents, rels, side, k, known)
+        if cfg.algorithm == "RotatE":
+            return self._predict_rotate(ents, rels, side, k, known)
         if self.cuda:
             from ..ops import gather_gemm_topk
 
@@ -604,6 +715,76 @@ class KGE:
             excluded[torch.repeat_interleave(torch.arange(ents.numel()), off[1:] - off[:-1]), cols] = True
         vals, idx = topk_reference(-torch.cdist(q, En, p=float(p)), int(k), excluded)
         return idx, vals
+
+    def _predict_rotate(self, ents, rels, side, k, known):
+        """``predict`` for RotatE: the ``k`` nearest entities by the complex distance to ``s o rho`` (objects) or
+        ``o o conj(rho)`` (subjects); scores are ``-distance``. CUDA: ``ops.gather_dist_topk(p="complex")``; CPU:
+        ``ops.complex_dist`` + ``ops.topk_reference``."""
+        cfg = self.cfg
+        d, ne = cfg.embed_dim, cfg.num_entities
+        conj = side == "subject"
+        if self.cuda:
+            from ..ops import gather_dist_topk
+
+            dev, kv = self.server.device, self.worker
+            ents, rels = ents.to(dev), rels.to(dev)
+
+            def pull_rows(keys, ln):
+                buf = torch.empty(keys.numel() * 2 * ln, dtype=torch.float32, device=dev)
+                kv.wait(kv.pull(keys.contiguous(), buf, True))
+                return buf.view(-1, 2 * ln)[:, :ln]
+
+            q = rotate_query(pull_rows(ents, d), pull_rows(rels + ne, d // 2), conj)
+            excl = self._known_answers(ents, rels, side, known) if known is not None else None
+            vals, idx = gather_dist_topk(self.server, q, torch.arange(ne, dtype=torch.int64, device=dev), d, k,
+                                         "complex", False, exclude=excl)
+            return idx, vals
+        from ..ops import _check_topk, complex_dist, topk_reference
+
+        _check_topk(ents.numel(), ne, k, None, None)
+        E, _, R, _ = self.pull_embeddings()
+        E, R = E.float(), R.float()
+        q = rotate_query(E[ents], R[rels], conj)
+        excluded = None
+        if known is not None:
+            off, cols = self._known_answers(ents, rels, side, known)
+            excluded = torch.zeros(ents.numel(), ne, dtype=torch.bool)
+            excluded[torch.repeat_interleave(torch.arange(ents.numel()), off[1:] - off[:-1]), cols] = True
+        vals, idx = topk_reference(-complex_dist(q, E), int(k), excluded)
+        return idx, vals
+
+
+def rotate_query(e: torch.Tensor, theta: torch.Tensor, conj: bool) -> torch.Tensor:
+    """RotatE query rows, interleaved (re, im): ``e o rho`` (object side) or ``e o conj(rho)`` (subject side, conj=True)
+    with ``rho = e^{i theta}``; the distance to a candidate is ``ops.complex_dist(query, candidate)``."""
+    n, d = e.shape
+    z = e.reshape(n, d // 2, 2)
+    re, im = z[..., 0], z[..., 1]
+    c, s = torch.cos(theta), torch.sin(theta)
+    if conj:
+        s = -s
+    return torch.stack([re * c - im * s, re * s + im * c], -1).reshape(n, d).contiguous()
+
+
+def _rotate_relation_ranks(Es: torch.Tensor, Eo: torch.Tensor, R: torch.Tensor, true_rel: torch.Tensor,
+                           chunk_elems: int = 1 << 24) -> torch.Tensor:
+    """RotatE relation-side raw ranks - 1: ``#{r' != r : D(s, r', o) < D(s, r, o)}`` with ``D = sum_i |s_i rho'_i - o_i|``
+    over every relation's phases ``R`` [nr, d / 2], in the dtype and on the device of the inputs, in relation chunks.
+    The true relation's distance is read from the same matrix, so it cannot disagree with its column by rounding."""
+    B, d = Es.shape
+    nr, m = R.shape
+    s, o = Es.reshape(B, 1, m, 2), Eo.reshape(B, 1, m, 2)
+    D = torch.empty(B, nr, dtype=Es.dtype, device=Es.device)
+    step = max(1, chunk_elems // max(1, B * d))
+    for j in range(0, nr, step):
+        c, sn = torch.cos(R[j:j + step]).unsqueeze(0), torch.sin(R[j:j + step]).unsqueeze(0)
+        xr = s[..., 0] * c - s[..., 1] * sn - o[..., 0]
+        xi = s[..., 0] * sn + s[..., 1] * c - o[..., 1]
+        D[:, j:j + step] = torch.sqrt(xr * xr + xi * xi).sum(-1)
+    dt = D.gather(1, true_rel.view(-1, 1))
+    better = D < dt
+    better.scatter_(1, true_rel.view(-1, 1), False)
+    return better.sum(1)
 
 
 def normalize_rows(e: torch.Tensor) -> torch.Tensor:
@@ -698,7 +879,7 @@ def evaluate_fused(model: "KGE", triples: torch.Tensor, known: torch.Tensor, bat
     of the test triples concurrently."""
     from ..ops import gather_gemm_rank_count
 
-    if model.cfg.algorithm == "TransE":   # distance ranks from the store rows (ops.gather_dist_rank_count)
+    if model.cfg.algorithm in ("TransE", "RotatE"):   # distance ranks from the store rows (ops.gather_dist_rank_count)
         ranks = model.rank_triples(triples, known, batch)
         rf = torch.cat([ranks["rank_o"], ranks["rank_s"]]).double()
         rr = torch.cat([ranks["rank_o_raw"], ranks["rank_s_raw"]]).double()

@@ -344,9 +344,175 @@ def transe_reference_step(kv, subj: torch.Tensor, rel: torch.Tensor, obj: torch.
     return loss, 3 * B + int(sel.sum())
 
 
-def _dist_operands(server, q, keys, dim, p, exclude, stats, M):
+ROTATE_MAX_DIM = 512
+ROTATE_MAX_NEG = 256
+
+
+def _check_rotate_shape(embed_dim: int) -> None:
+    if isinstance(embed_dim, bool) or int(embed_dim) != embed_dim or not (
+            8 <= int(embed_dim) <= ROTATE_MAX_DIM and int(embed_dim) % 8 == 0):
+        raise ValueError(f"embed_dim must be a multiple of 8 in [8, {ROTATE_MAX_DIM}], got {embed_dim}")
+
+
+def _check_rotate_neg(neg: torch.Tensor, B: int) -> None:
+    if neg.dim() != 2 or neg.shape[0] != B or neg.shape[1] % 2 or not 2 <= neg.shape[1] <= ROTATE_MAX_NEG:
+        raise ValueError(f"neg must be [B, 2n] with 2 <= 2n <= {ROTATE_MAX_NEG}, got {tuple(neg.shape)}")
+
+
+def kge_rotate_step(server, subj: torch.Tensor, rel: torch.Tensor, obj: torch.Tensor, neg: torch.Tensor, embed_dim: int,
+                    margin: float, adversarial_temperature: float, eta: float, gamma_entity: float, loss: torch.Tensor,
+                    stats: Optional[torch.Tensor] = None, deterministic: bool = False) -> None:
+    """Fused RotatE training step (csrc/cuda/ops_rotate.cu) on ``server``'s store: one warp per positive triple
+    ``(subj[i], rel[i], obj[i])`` (store keys) with the entity keys ``neg[i]`` ([B, 2n], 2 <= 2n <= 256; the first n
+    replace the object, the last n the subject). Entity rows are ``[z (embed_dim) | AdaGrad (embed_dim)]`` with ``z``
+    interleaved ``(re_0, im_0, re_1, im_1, ...)``; relation rows are ``[phases (embed_dim / 2) | AdaGrad (embed_dim / 2)]``
+    in radians; ``embed_dim % 8 == 0``, ``8 <= embed_dim <= 512``. The rule is :func:`rotate_reference_step`'s: distance
+    ``D = sum_i |(s o rho - o)_i|``, loss ``softplus(D+ - margin) + 1/2 sum_side sum_j w_j softplus(margin - D_j)`` with
+    the self-adversarial weights ``w = softmax(adversarial_temperature (margin - D))`` per side, one AdaGrad push per row
+    of the positive and one per negative. ``loss``: float32[1], accumulated (+=); ``stats``: optional int64[4]
+    accumulated with (local rows, peer rows, slow-path rows, pushes issued = (3 + 2n) per triple).
+
+    ``deterministic=True`` (single-GPU servers only): start-of-step reads, fixed-point sums, bit-identical runs (three
+    launches instead of one)."""
+    _i64(subj, "subj"); _i64(rel, "rel"); _i64(obj, "obj"); _i64(neg, "neg"); _f32(loss, "loss")
+    _check_rotate_shape(embed_dim)
+    B = subj.numel()
+    if not (rel.numel() == B and obj.numel() == B):
+        raise ValueError("subj, rel and obj must have the same length")
+    _check_rotate_neg(neg, B)
+    if stats is not None and not (stats.is_cuda and stats.dtype == torch.int64 and stats.numel() >= 4):
+        raise TypeError("stats must be a CUDA int64 tensor with 4 entries")
+    det = _check_deterministic(server, deterministic)
+    _C.kge_rotate_step(server._impl.backend_handle(), _stream(subj), subj.data_ptr(), rel.data_ptr(), obj.data_ptr(),
+                       neg.data_ptr(), B, int(neg.shape[1]), int(embed_dim), float(margin),
+                       float(adversarial_temperature), float(eta), float(gamma_entity), loss.data_ptr(),
+                       stats.data_ptr() if stats is not None else 0, det)
+
+
+def _as_complex(e: torch.Tensor) -> torch.Tensor:
+    """interleaved (re, im) rows [..., d] -> complex [..., d / 2]"""
+    return torch.view_as_complex(e.reshape(*e.shape[:-1], -1, 2).contiguous())
+
+
+def _as_interleaved(z: torch.Tensor) -> torch.Tensor:
+    return torch.view_as_real(z).reshape(*z.shape[:-1], -1)
+
+
+def rotate_reference_step(kv, subj: torch.Tensor, rel: torch.Tensor, obj: torch.Tensor, neg: torch.Tensor, embed_dim: int,
+                          margin: float, adversarial_temperature: float, eta: float, gamma_entity: float):
+    """The RotatE rule of :func:`kge_rotate_step` in float64 through Pull / Push (CPU servers, float64 rows, and the
+    oracle of the tests). Every row is read at the start of the step. Returns ``(loss, pushes)``.
+
+    Per positive triple, with rho = e^{i theta}, x = a o rho - b, D(x) = sum_i |x_i| and u = x / |x| (0 where |x_i| = 0):
+    the positive x = s o rho - o, object-side negatives x_j = s o rho - o'_j, subject-side x_j = s'_j o rho - o;
+    ``w_j = softmax_j(adversarial_temperature (margin - D_j))`` over the n negatives of a side (no gradient); loss
+    ``softplus(D+ - margin) + 1/2 sum_side sum_j w_j softplus(margin - D_j)``. ``dD/da = conj(rho) o u``, ``dD/db = -u``,
+    ``dD/dtheta_i = -Im(conj(u_i) a_i rho_i)``, scaled by ``sigmoid(D+ - margin)`` for the positive and
+    ``-1/2 w_j sigmoid(margin - D_j)`` for negative j. L2 adds ``gamma_entity * s`` and ``gamma_entity * o`` to the raw
+    entity rows; phases get none. Pushes ``[-eta g / sqrt(acc + g^2) | g^2]`` (0 where g == 0) with the pulled
+    accumulator: s, r and o once per triple, every negative once."""
+    _check_rotate_shape(embed_dim)
+    d = int(embed_dim)
+    m = d // 2
+    subj, rel, obj = (t.reshape(-1).cpu() for t in (subj, rel, obj))
+    neg = neg.cpu()
+    B = subj.numel()
+    _check_rotate_neg(neg, B)
+    nn = neg.shape[1]
+    h = nn // 2
+    f64 = torch.float64
+    alpha = float(adversarial_temperature)
+
+    def pull(keys, ln):
+        v = torch.empty(keys.numel() * 2 * ln, dtype=kv.server.dtype)
+        if keys.numel():
+            kv.wait(kv.pull(keys.contiguous(), v))
+        v = v.view(-1, 2 * ln).to(f64)
+        return v[:, :ln], v[:, ln:]
+
+    def dist(x):
+        return x.abs().sum(-1)
+
+    def unit(x):
+        a = x.abs()
+        return torch.where(a > 0, x / torch.where(a > 0, a, torch.ones_like(a)), torch.zeros_like(x))
+
+    def dtheta(u, p):
+        return -(u.conj() * p).imag
+
+    def softplus(x):
+        return torch.logaddexp(x, torch.zeros_like(x))
+
+    Es, As = pull(subj, d)
+    Th, Ar = pull(rel, m)
+    Eo, Ao = pull(obj, d)
+    En, An = pull(neg.reshape(-1), d)
+    s, o, n = _as_complex(Es), _as_complex(Eo), _as_complex(En).view(B, nn, m)
+    rho = torch.complex(torch.cos(Th), torch.sin(Th))
+    sr = s * rho
+    nsr = n[:, h:] * rho.unsqueeze(1)
+    x = sr - o
+    xo = sr.unsqueeze(1) - n[:, :h]
+    xs = nsr - o.unsqueeze(1)
+    Dp = dist(x)
+    Dn = torch.cat([dist(xo), dist(xs)], 1)
+    z = alpha * (margin - Dn)
+    w = torch.cat([torch.softmax(z[:, :h], 1), torch.softmax(z[:, h:], 1)], 1)
+    loss = float(softplus(Dp - margin).sum() + 0.5 * (w * softplus(margin - Dn)).sum())
+    cp = torch.sigmoid(Dp - margin).unsqueeze(1)
+    cn = (-0.5 * w * torch.sigmoid(margin - Dn)).unsqueeze(2)
+    u, uo, us = unit(x), unit(xo), unit(xs)
+    rc = rho.conj()
+    gs = (cp * u + (cn[:, :h] * uo).sum(1)) * rc
+    go = -cp * u - (cn[:, h:] * us).sum(1)
+    gt = cp * dtheta(u, sr) + (cn[:, :h] * dtheta(uo, sr.unsqueeze(1))).sum(1) + (cn[:, h:] * dtheta(us, nsr)).sum(1)
+    gn = torch.cat([-cn[:, :h] * uo, cn[:, h:] * rc.unsqueeze(1) * us], 1)
+
+    def upd(g, a):
+        ue = torch.where(g != 0, -eta * g / torch.sqrt(a + g * g), torch.zeros_like(g))
+        return torch.cat([ue, g * g], -1).to(kv.server.dtype).contiguous().view(-1)
+
+    kv.wait(kv.push(subj.contiguous(), upd(_as_interleaved(gs) + gamma_entity * Es, As)))
+    kv.wait(kv.push(rel.contiguous(), upd(gt, Ar)))
+    kv.wait(kv.push(obj.contiguous(), upd(_as_interleaved(go) + gamma_entity * Eo, Ao)))
+    kv.wait(kv.push(neg.reshape(-1).contiguous(), upd(_as_interleaved(gn).reshape(-1, d), An)))
+    return loss, B * (3 + nn)
+
+
+DIST_COMPLEX = 3          # the kernels' code of p = "complex"
+
+
+def _dist_p(p, normalize) -> int:
+    """validated metric code: 1, 2, or DIST_COMPLEX for p = "complex" (which never normalises)"""
+    if isinstance(p, str):
+        if p != "complex":
+            raise ValueError(f"p must be 1, 2 or 'complex', got {p!r}")
+        if normalize:
+            raise ValueError("normalize=True is not defined for p='complex' (RotatE scores raw entity rows)")
+        return DIST_COMPLEX
+    if p not in (1, 2) or isinstance(p, bool):
+        raise ValueError(f"p must be 1, 2 or 'complex', got {p}")
+    return int(p)
+
+
+def complex_dist(q: torch.Tensor, e: torch.Tensor, chunk_elems: int = 1 << 24) -> torch.Tensor:
+    """``D[i, j] = sum_k |q_i,k - e_j,k|`` over the complex values of interleaved (re, im) rows ``q`` [M, dim] and ``e``
+    [N, dim], in the dtype of the inputs, computed in column chunks of about ``chunk_elems`` elements."""
+    M, dim = q.shape
+    N = e.shape[0]
+    qc = q.reshape(M, 1, dim // 2, 2)
+    out = torch.empty(M, N, dtype=q.dtype, device=q.device)
+    step = max(1, chunk_elems // max(1, M * dim))
+    for j in range(0, N, step):
+        diff = qc - e[j:j + step].reshape(1, -1, dim // 2, 2)
+        out[:, j:j + step] = torch.linalg.vector_norm(diff, dim=-1).sum(-1)
+    return out
+
+
+def _dist_operands(server, q, keys, dim, p, normalize, exclude, stats, M):
+    p = _dist_p(p, normalize)
     _i64(keys, "keys")
-    _check_transe_shape(dim, p)
+    _check_transe_shape(dim, 1)
     if q.dim() != 2 or q.shape[1] != int(dim):
         raise ValueError(f"q must be a matrix [M, dim = {dim}]")
     if not (q.is_cuda and q.device == keys.device):
@@ -358,7 +524,7 @@ def _dist_operands(server, q, keys, dim, p, exclude, stats, M):
     _, eo, ec = _topk_operands(q.device, exclude, None)
     if q.data_ptr() % 16:              # the kernels read q in 16-byte vectors: a view at an odd offset is copied
         q = q.clone()
-    return q, eo, ec
+    return q, eo, ec, p
 
 
 def _dist_slices(server, M, N):
@@ -373,9 +539,12 @@ def gather_dist_rank_count(server, q: torch.Tensor, keys: torch.Tensor, dim: int
     ``raw[i] = #{j != true_col[i] : D(i, j) < D(i, true_col[i])}`` and ``filtered`` the same without the columns of the
     CSR ``exclude = (offsets int64 [M + 1], cols int64 [nnz])`` (ascending per row, as for :func:`gather_gemm_topk`).
     The true distance comes from the kernel's own distance function, bit-identical to the column's. ``stats``: as for
-    :func:`gather_gemm`; on several ranks the call waits and raises ``RuntimeError`` if a row could not be resolved."""
+    :func:`gather_gemm`; on several ranks the call waits and raises ``RuntimeError`` if a row could not be resolved.
+
+    ``p="complex"`` (RotatE): ``D(i, j) = sum_k |(q_i - e_j)_k|`` over the complex values of interleaved (re, im) rows,
+    each modulus and sum explicitly rounded in a fixed order; ``normalize`` must be False (else ``ValueError``)."""
     M = q.shape[0] if q.dim() == 2 else 0
-    q, eo, ec = _dist_operands(server, q, keys, dim, p, exclude, stats, M)
+    q, eo, ec, p = _dist_operands(server, q, keys, dim, p, normalize, exclude, stats, M)
     _i64(true_col, "true_col")
     if true_col.numel() != M:
         raise ValueError(f"true_col must have M = {M} entries")
@@ -400,11 +569,12 @@ def gather_dist_topk(server, q: torch.Tensor, keys: torch.Tensor, dim: int, k: i
     """The ``k`` columns of smallest distance per query (the distances of :func:`gather_dist_rank_count`): returns
     ``(values = -D fp32 [M, k], indices int64 [M, k])`` with :func:`gather_gemm_topk`'s conventions - smallest distance
     first, ties to the smaller column, NaN never selected, ``(-inf, -1)`` padding, ``1 <= k <= 64``, exclusions as a
-    CSR; indices are positions into ``keys``. Per-slice lists are merged by the top-k merge kernel."""
+    CSR; indices are positions into ``keys``. Per-slice lists are merged by the top-k merge kernel. ``p``: 1, 2 or
+    ``"complex"``, as for :func:`gather_dist_rank_count`."""
     M = q.shape[0] if q.dim() == 2 else 0
     if isinstance(k, bool) or int(k) != k or not 1 <= int(k) <= TOPK_MAX_K:
         raise ValueError(f"k must be an integer in [1, {TOPK_MAX_K}], got {k}")
-    q, eo, ec = _dist_operands(server, q, keys, dim, p, exclude, stats, M)
+    q, eo, ec, p = _dist_operands(server, q, keys, dim, p, normalize, exclude, stats, M)
     k, N = int(k), keys.numel()
     if M == 0 or N == 0:
         return _topk_empty(M, k, q.device)
@@ -420,8 +590,9 @@ def gather_dist_topk(server, q: torch.Tensor, keys: torch.Tensor, dim: int, k: i
 
 def dist_rank_reference(q: torch.Tensor, e: torch.Tensor, p: int, true_col: torch.Tensor, excluded=None):
     """PyTorch ``cdist`` ranking with the rule of :func:`gather_dist_rank_count` on dense candidates ``e`` [N, dim]
-    (already normalised if wanted): ``(raw, filtered)`` int64 [M]; ``excluded``: bool [M, N] or None."""
-    D = torch.cdist(q, e, p=float(p))
+    (already normalised if wanted): ``(raw, filtered)`` int64 [M]; ``excluded``: bool [M, N] or None. ``p="complex"``
+    uses :func:`complex_dist` (chunked; there is no ``cdist`` form of it)."""
+    D = complex_dist(q, e) if isinstance(p, str) and p == "complex" else torch.cdist(q, e, p=float(p))
     dt = D.gather(1, true_col.view(-1, 1))
     better = D < dt
     better.scatter_(1, true_col.view(-1, 1), False)
