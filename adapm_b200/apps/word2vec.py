@@ -15,9 +15,10 @@ import torch
 import adapm_b200 as ad
 from adapm_b200.apps._common import (add_ablation_options, add_system_options, enforce_full_replication, id_permutation,
                                       strip_dashes, system_options, wants_sync_push)
-from adapm_b200.models.word2vec import (SyntheticPairs, Word2Vec, Word2VecConfig, load_checkpoint, syn0_key, syn1_key,
-                                        zipf_counts)
-from adapm_b200.utils.text import NativeCorpus, Vocabulary, pairs_from_sentences, read_sentences
+from adapm_b200.models.word2vec import (SyntheticPairs, SyntheticWindows, Word2Vec, Word2VecConfig, load_checkpoint,
+                                        syn0_key, syn1_key, zipf_counts)
+from adapm_b200.utils.text import (NativeCorpus, Vocabulary, pairs_from_sentences, read_sentences,
+                                   windows_from_sentences)
 
 
 def main(argv=None) -> int:
@@ -45,6 +46,10 @@ def main(argv=None) -> int:
     ap.add_argument("--model_seed", type=int, default=134827)
     ap.add_argument("--max_runtime", type=float, default=float("inf"))
     ap.add_argument("--batch_pairs", type=int, default=32768)
+    ap.add_argument("--cbow", type=int, default=0, choices=[0, 1],
+                    help="1 = continuous bag of words (word2vec.c's -cbow 1): one window per corpus word, the mean of the "
+                         "context rows scored against the centre and the negatives; 0 = skip-gram (window <= 16 for CBOW)")
+    ap.add_argument("--batch_windows", type=int, default=8192, help="CBOW: windows per step")
     ap.add_argument("--synthetic_vocab", type=int, default=0, help="train on a synthetic Zipf corpus of this vocabulary size")
     ap.add_argument("--synthetic_batches", type=int, default=50)
     ap.add_argument("--init_model", default="random",
@@ -62,6 +67,8 @@ def main(argv=None) -> int:
     add_system_options(ap)
     args = ap.parse_args(strip_dashes(argv if argv is not None else sys.argv[1:]))
 
+    if args.cbow and args.shared_negatives > 0:
+        raise ValueError("--shared_negatives is a skip-gram option: it cannot be combined with --cbow 1")
     rng = np.random.default_rng(args.model_seed)
     words = None
     native = None
@@ -95,7 +102,7 @@ def main(argv=None) -> int:
                          starting_alpha=args.starting_alpha, neg_power=args.neg_power, batch_pairs=args.batch_pairs,
                          read_ahead=args.read_sentences_ahead, signal_intent=bool(args.signal_intent),
                          sampling_scheme=getattr(args, "sampling.scheme") or "local", model_seed=args.model_seed,
-                         shared_negatives=args.shared_negatives)
+                         shared_negatives=args.shared_negatives, cbow=bool(args.cbow), batch_windows=args.batch_windows)
     ad.setup(cfg.num_keys, 1)   # one worker per rank: the per-thread loops of the reference are batched kernels here
     server = ad.Server(cfg.row_len, backend=args.backend, options=system_options(args))
     kv = ad.Worker(0, server)
@@ -116,6 +123,18 @@ def main(argv=None) -> int:
         native.encode(args.input_file, rank, world)      # this rank's share of the lines, as word ids
 
     def batches(epoch):
+        if cfg.cbow:
+            if args.input_file and native is not None:
+                yield from native.window_batches(args.window, args.subsample, cfg.batch_windows, args.model_seed + rank,
+                                                 epoch, pin=model.cuda)
+            elif args.input_file:
+                sents = read_sentences(args.input_file, vocab, rank, world, args.subsample, rng)
+                yield from windows_from_sentences(sents, args.window, cfg.batch_windows, rng)
+            else:
+                data = SyntheticWindows(cfg, counts, rank, seed=epoch + 1)
+                for s in range(args.synthetic_batches):
+                    yield data.batch(s)
+            return
         if args.input_file and native is not None:
             yield from native.pair_batches(args.window, args.subsample, cfg.batch_pairs, args.model_seed + rank, epoch,
                                            pin=model.cuda)
@@ -142,25 +161,26 @@ def main(argv=None) -> int:
             cur = window.pop(0)
             if model.cuda:
                 model.loss.zero_()
-            loss = model.step(cur if cur.shape[1] == cfg.batch_pairs or not model.cuda else _pad(cur, cfg.batch_pairs))
+            loss = model.step(_full(cur, cfg, model.cuda))
             if sync_push and model.cuda:
                 torch.cuda.current_stream().synchronize()
             kv.advance_clock()
-            total_pairs += getattr(cur, "valid_pairs", cur.shape[1])
-            epoch_pairs += getattr(cur, "valid_pairs", cur.shape[1])
+            total_pairs += _items(cur, cfg)
+            epoch_pairs += _items(cur, cfg)
             if time.time() - t0 > args.max_runtime or (args.data_words and epoch_pairs >= args.data_words):
                 break
         for cur in window:
             if model.cuda:
                 model.loss.zero_()
-            loss = model.step(cur if cur.shape[1] == cfg.batch_pairs or not model.cuda else _pad(cur, cfg.batch_pairs))
+            loss = model.step(_full(cur, cfg, model.cuda))
             kv.advance_clock()
-            total_pairs += getattr(cur, "valid_pairs", cur.shape[1])
+            total_pairs += _items(cur, cfg)
         model.set_alpha((epoch + 1) / args.num_iterations)
         kv.barrier()
         if rank == 0:
-            print(f"[w2v] epoch {epoch} done: {total_pairs} pairs on rank 0, {time.time() - t0:.1f}s, "
-                  f"last batch loss {float(loss) / max(1, cfg.batch_pairs * (cfg.negative + 1)):.4f}", flush=True)
+            unit, per_step = ("windows", cfg.batch_windows) if cfg.cbow else ("pairs", cfg.batch_pairs)
+            print(f"[w2v] epoch {epoch} done: {total_pairs} {unit} on rank 0, {time.time() - t0:.1f}s, "
+                  f"last batch loss {float(loss) / max(1, per_step * (cfg.negative + 1)):.4f}", flush=True)
         if args.write_results:
             model.write_checkpoint(f"{args.output_file}.epoch.{epoch}", words)
     kv.finalize()
@@ -168,6 +188,20 @@ def main(argv=None) -> int:
         print(server.stats(), flush=True)
     server.shutdown()
     return 0
+
+
+def _items(b: torch.Tensor, cfg) -> int:
+    """real pairs / windows of a batch"""
+    if cfg.cbow:
+        return getattr(b, "valid_windows", b.shape[0])
+    return getattr(b, "valid_pairs", b.shape[1])
+
+
+def _full(b: torch.Tensor, cfg, cuda: bool) -> torch.Tensor:
+    """the batch at the fixed size of the fused kernel (window batches are padded by their loaders)"""
+    if cfg.cbow or not cuda or b.shape[1] == cfg.batch_pairs:
+        return b
+    return _pad(b, cfg.batch_pairs)
 
 
 def _pad(b: torch.Tensor, n: int) -> torch.Tensor:

@@ -144,18 +144,16 @@ void Corpus::encode(const std::string& path, int rank, int world) {
   });
 }
 
-// ------------------------------------------------------------------------------------- pair stream
-PairStream::PairStream(std::shared_ptr<Corpus> corpus, int window, double subsample, int64_t batch_pairs, uint64_t seed,
-                       int queue_depth)
-    : corpus_(std::move(corpus)), window_(window), subsample_(subsample), batch_(batch_pairs), seed_(seed) {
-  ADAPM_CHECK(window_ >= 1 && batch_ >= 1 && queue_depth >= 1, "PairStream: bad window / batch size / queue depth");
+// ------------------------------------------------------------------------------------- batch streams
+KeyBatchStream::KeyBatchStream(std::shared_ptr<Corpus> corpus, int window, double subsample, uint64_t seed,
+                               int64_t batch_keys, int queue_depth)
+    : corpus_(std::move(corpus)), window_(window), subsample_(subsample), seed_(seed), batch_keys_(batch_keys) {
+  ADAPM_CHECK(window_ >= 1 && batch_keys_ >= 1 && queue_depth >= 1, "batch stream: bad window / batch size / queue depth");
   ring_.resize((size_t)queue_depth);
-  for (auto& s : ring_) s.keys.resize((size_t)(2 * batch_));
+  for (auto& sl : ring_) sl.keys.resize((size_t)batch_keys_);
 }
 
-PairStream::~PairStream() { stop(); }
-
-void PairStream::stop() {
+void KeyBatchStream::stop() {
   {
     std::lock_guard<std::mutex> lk(mu_);
     abort_ = true;
@@ -166,7 +164,7 @@ void PairStream::stop() {
   abort_ = false;
 }
 
-void PairStream::start_epoch(uint64_t epoch) {
+void KeyBatchStream::start_epoch(uint64_t epoch) {
   stop();
   {
     std::lock_guard<std::mutex> lk(mu_);
@@ -176,7 +174,8 @@ void PairStream::start_epoch(uint64_t epoch) {
   thread_ = std::thread([this, epoch] { run(epoch); });
 }
 
-void PairStream::run(uint64_t epoch) {
+template <class F>
+bool KeyBatchStream::walk(uint64_t epoch, F&& fn) {
   Rng rng(seed_ * 0x2545F4914F6CDD1Dull + epoch * 0x9E3779B97F4A7C15ull + 1);
   const int32_t* tok = corpus_->tokens();
   const int64_t* off = corpus_->sentence_offsets();
@@ -193,43 +192,8 @@ void PairStream::run(uint64_t epoch) {
       keep[i] = (float)((std::sqrt(fr / subsample_) + 1.0) * subsample_ / fr);
     }
   }
-  std::vector<Key> cur((size_t)(2 * batch_)), uniq;
-  uniq.reserve((size_t)(2 * batch_));
-  int64_t n = 0;
   std::vector<int32_t> s;
-
-  auto publish = [&](int64_t valid) -> bool {
-    if (valid < batch_) {   // pad a short last batch by repeating its pairs (fixed-size batches for the fused kernel)
-      for (int64_t i = valid; i < batch_; ++i) {
-        cur[(size_t)i] = cur[(size_t)(i % valid)];
-        cur[(size_t)(batch_ + i)] = cur[(size_t)(batch_ + i % valid)];
-      }
-    }
-    // distinct keys of the batch (before taking the lock: this is the expensive part)
-    if (seen_.empty()) seen_.assign((size_t)(2 * corpus_->vocab_size()), 0u);
-    if (++seen_epoch_ == 0) { std::fill(seen_.begin(), seen_.end(), 0u); seen_epoch_ = 1; }
-    uniq.clear();
-    for (int64_t i = 0; i < 2 * batch_; ++i) {
-      const Key k = cur[(size_t)i];
-      if (seen_[(size_t)k] != seen_epoch_) { seen_[(size_t)k] = seen_epoch_; uniq.push_back(k); }
-    }
-    std::unique_lock<std::mutex> lk(mu_);
-    cv_put_.wait(lk, [&] { return count_ < ring_.size() || abort_; });
-    if (abort_) return false;
-    Slot& sl = ring_[tail_];
-    sl.keys.swap(cur);
-    sl.uniq.swap(uniq);
-    sl.valid = valid;
-    tail_ = (tail_ + 1) % ring_.size();
-    ++count_;
-    produced_.fetch_add((uint64_t)valid);
-    lk.unlock();
-    cv_get_.notify_one();
-    return true;
-  };
-
-  bool ok = true;
-  for (int64_t si = 0; si < ns && ok; ++si) {
+  for (int64_t si = 0; si < ns; ++si) {
     s.clear();
     for (int64_t t = off[si]; t < off[si + 1]; ++t) {
       const int32_t w = tok[t];
@@ -238,24 +202,41 @@ void PairStream::run(uint64_t epoch) {
     }
     const int64_t L = (int64_t)s.size();
     if (L < 2) continue;
-    for (int64_t pos = 0; pos < L && ok; ++pos) {
+    for (int64_t pos = 0; pos < L; ++pos) {
       const int64_t b = (int64_t)(rng.next() % (uint64_t)window_);   // window shrink in [0, window)
       const int64_t r = window_ - b;
       const int64_t lo = std::max<int64_t>(0, pos - r), hi = std::min<int64_t>(L, pos + r + 1);
-      const Key target = 2 * (Key)s[(size_t)pos] + 1;               // syn1 key of the centre word
-      for (int64_t j = lo; j < hi; ++j) {
-        if (j == pos) continue;
-        cur[(size_t)n] = 2 * (Key)s[(size_t)j];                       // syn0 key of the context word
-        cur[(size_t)(batch_ + n)] = target;
-        if (++n == batch_) {
-          ok = publish(batch_);
-          n = 0;
-          if (!ok) break;
-        }
-      }
+      if (!fn(s, pos, lo, hi)) return false;
     }
   }
-  if (ok && n > 0) publish(n);
+  return true;
+}
+
+bool KeyBatchStream::publish(std::vector<Key>& cur, int64_t valid) {
+  // distinct keys of the batch (before taking the lock: this is the expensive part)
+  if (seen_.empty()) seen_.assign((size_t)(2 * corpus_->vocab_size()), 0u);
+  if (++seen_epoch_ == 0) { std::fill(seen_.begin(), seen_.end(), 0u); seen_epoch_ = 1; }
+  uniq_.clear();
+  for (int64_t i = 0; i < batch_keys_; ++i) {
+    const Key k = cur[(size_t)i];
+    if (k >= 0 && seen_[(size_t)k] != seen_epoch_) { seen_[(size_t)k] = seen_epoch_; uniq_.push_back(k); }
+  }
+  std::unique_lock<std::mutex> lk(mu_);
+  cv_put_.wait(lk, [&] { return count_ < ring_.size() || abort_; });
+  if (abort_) return false;
+  Slot& sl = ring_[tail_];
+  sl.keys.swap(cur);
+  sl.uniq.swap(uniq_);
+  sl.valid = valid;
+  tail_ = (tail_ + 1) % ring_.size();
+  ++count_;
+  produced_.fetch_add((uint64_t)valid);
+  lk.unlock();
+  cv_get_.notify_one();
+  return true;
+}
+
+void KeyBatchStream::finish() {
   {
     std::lock_guard<std::mutex> lk(mu_);
     done_ = true;
@@ -263,16 +244,14 @@ void PairStream::run(uint64_t epoch) {
   cv_get_.notify_all();
 }
 
-int64_t PairStream::next(Key* out) { return next_with_unique(out, nullptr, nullptr); }
-
-int64_t PairStream::next_with_unique(Key* out, Key* uniq, int64_t* n_uniq) {
+int64_t KeyBatchStream::next_with_unique(Key* out, Key* uniq, int64_t* n_uniq) {
   std::unique_lock<std::mutex> lk(mu_);
   cv_get_.wait(lk, [&] { return count_ > 0 || done_ || abort_; });
   if (count_ == 0) return 0;
   Slot& sl = ring_[head_];
   const int64_t valid = sl.valid;
   lk.unlock();
-  memcpy(out, sl.keys.data(), (size_t)(2 * batch_) * sizeof(Key));   // the slot stays reserved while we copy
+  memcpy(out, sl.keys.data(), (size_t)batch_keys_ * sizeof(Key));   // the slot stays reserved while we copy
   if (uniq) {
     memcpy(uniq, sl.uniq.data(), sl.uniq.size() * sizeof(Key));
     *n_uniq = (int64_t)sl.uniq.size();
@@ -283,6 +262,80 @@ int64_t PairStream::next_with_unique(Key* out, Key* uniq, int64_t* n_uniq) {
   lk.unlock();
   cv_put_.notify_one();
   return valid;
+}
+
+// ------------------------------------------------------------------------------------- pair stream
+PairStream::PairStream(std::shared_ptr<Corpus> corpus, int window, double subsample, int64_t batch_pairs, uint64_t seed,
+                       int queue_depth)
+    : KeyBatchStream(std::move(corpus), window, subsample, seed, 2 * batch_pairs, queue_depth), batch_(batch_pairs) {
+  ADAPM_CHECK(batch_ >= 1, "PairStream: bad window / batch size / queue depth");
+}
+
+PairStream::~PairStream() { stop(); }
+
+void PairStream::run(uint64_t epoch) {
+  std::vector<Key> cur((size_t)(2 * batch_));
+  int64_t n = 0;
+  auto publish_pairs = [&](int64_t valid) -> bool {
+    if (valid < batch_) {   // pad a short last batch by repeating its pairs (fixed-size batches for the fused kernel)
+      for (int64_t i = valid; i < batch_; ++i) {
+        cur[(size_t)i] = cur[(size_t)(i % valid)];
+        cur[(size_t)(batch_ + i)] = cur[(size_t)(batch_ + i % valid)];
+      }
+    }
+    return publish(cur, valid);
+  };
+  const bool ok = walk(epoch, [&](const std::vector<int32_t>& s, int64_t pos, int64_t lo, int64_t hi) {
+    const Key target = 2 * (Key)s[(size_t)pos] + 1;               // syn1 key of the centre word
+    for (int64_t j = lo; j < hi; ++j) {
+      if (j == pos) continue;
+      cur[(size_t)n] = 2 * (Key)s[(size_t)j];                       // syn0 key of the context word
+      cur[(size_t)(batch_ + n)] = target;
+      if (++n == batch_) {
+        n = 0;
+        if (!publish_pairs(batch_)) return false;
+      }
+    }
+    return true;
+  });
+  if (ok && n > 0) publish_pairs(n);
+  finish();
+}
+
+int64_t PairStream::next(Key* out) { return next_with_unique(out, nullptr, nullptr); }
+
+// ------------------------------------------------------------------------------------- window stream
+WindowStream::WindowStream(std::shared_ptr<Corpus> corpus, int window, double subsample, int64_t batch_windows,
+                           uint64_t seed, int queue_depth)
+    : KeyBatchStream(std::move(corpus), window, subsample, seed, batch_windows * (1 + 2 * (int64_t)window), queue_depth),
+      batch_(batch_windows) {
+  ADAPM_CHECK(window >= 1 && window <= kMaxWindow, "WindowStream: window must be in [1, 16]");
+}
+
+WindowStream::~WindowStream() { stop(); }
+
+void WindowStream::run(uint64_t epoch) {
+  const int64_t cols = columns();
+  std::vector<Key> cur((size_t)batch_keys_);
+  int64_t n = 0;
+  const bool ok = walk(epoch, [&](const std::vector<int32_t>& s, int64_t pos, int64_t lo, int64_t hi) {
+    Key* r = cur.data() + n * cols;
+    r[0] = 2 * (Key)s[(size_t)pos] + 1;                              // syn1 key of the centre word
+    int64_t k = 1;
+    for (int64_t j = lo; j < hi; ++j)
+      if (j != pos) r[k++] = 2 * (Key)s[(size_t)j];                   // syn0 keys of the context words
+    std::fill(r + k, r + cols, (Key)-1);
+    if (++n == batch_) {
+      n = 0;
+      return publish(cur, batch_);
+    }
+    return true;
+  });
+  if (ok && n > 0) {         // pad a short last batch with windows that train nothing
+    std::fill(cur.begin() + n * cols, cur.end(), (Key)-1);
+    publish(cur, n);
+  }
+  finish();
 }
 
 }  // namespace adapm

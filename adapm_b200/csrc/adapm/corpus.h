@@ -1,5 +1,5 @@
-// Native data loader for the word2vec application: vocabulary building, corpus encoding and a background
-// (center, context) pair generator that fills fixed-size key batches.
+// Native data loader for the word2vec application: vocabulary building, corpus encoding and background generators of
+// fixed-size key batches: (center, context) pairs for skip-gram, windows for CBOW.
 //
 // Capability parity with the corpus handling of the reference application (apps/word2vec.cc:147-364 vocabulary hash /
 // sort / min_count pruning, :563-606 reading sentences ahead, :672-690 window shrinking, frequent-word subsampling),
@@ -48,42 +48,85 @@ class Corpus {
   std::shared_ptr<Index> index_;
 };
 
-// Produces [2, batch_pairs] key batches (row 0: syn0 key of the context word = 2*w, row 1: syn1 key of the centre
-// word = 2*w + 1) for one epoch over the encoded sentences, on a background thread.
-class PairStream {
+// Background producer of fixed-size key batches: a C++ thread fills a bounded ring of slots while the consumer trains
+// on earlier batches. Each slot also carries the batch's distinct keys (what Intent() should be called with: the
+// deduplication happens on the loader thread instead of the sync thread).
+class KeyBatchStream {
  public:
-  PairStream(std::shared_ptr<Corpus> corpus, int window, double subsample, int64_t batch_pairs, uint64_t seed,
-             int queue_depth = 8);
-  ~PairStream();
+  virtual ~KeyBatchStream() = default;
   void start_epoch(uint64_t epoch);
-  // Copies the next batch into out[2 * batch_pairs]; returns the number of valid pairs (a short last batch is padded
-  // by repeating its pairs), 0 at the end of the epoch.
-  int64_t next(Key* out);
-  // Same, and also writes the distinct keys of the batch (what Intent() should be called with: the deduplication
-  // happens here, on the loader thread, instead of on the sync thread) into uniq[0 .. *n_uniq); uniq holds 2*batch.
+  // Copies the next batch into out[batch_keys]; returns its number of valid items (pairs or windows), 0 at the end of
+  // the epoch. With uniq: also writes the batch's distinct keys (>= 0) into uniq[0 .. *n_uniq); uniq holds batch_keys.
   int64_t next_with_unique(Key* out, Key* uniq, int64_t* n_uniq);
-  int64_t batch_pairs() const { return batch_; }
-  uint64_t pairs_produced() const { return produced_.load(); }
 
- private:
-  void run(uint64_t epoch);
-  void stop();
-  struct Slot { std::vector<Key> keys, uniq; int64_t valid = 0; };
-  std::vector<uint32_t> seen_;   // producer thread: round-stamped table for the per-batch deduplication
-  uint32_t seen_epoch_ = 0;
+ protected:
+  KeyBatchStream(std::shared_ptr<Corpus> corpus, int window, double subsample, uint64_t seed, int64_t batch_keys,
+                 int queue_depth);
+  void stop();   // derived classes call it in their destructor: the thread runs their run()
+  virtual void run(uint64_t epoch) = 0;
+  // Walks this rank's sentences for one epoch with word2vec.c's frequent-word subsampling and window shrinking:
+  // fn(s, pos, lo, hi) for every position pos of every subsampled sentence s with at least two words, whose context is
+  // s[lo, hi) without pos. Returns false as soon as fn does.
+  template <class F> bool walk(uint64_t epoch, F&& fn);
+  // Publishes cur[0 .. batch_keys) (swapped out) with `valid` items; false if the stream was stopped.
+  bool publish(std::vector<Key>& cur, int64_t valid);
+  void finish();   // end of the epoch
 
   std::shared_ptr<Corpus> corpus_;
   int window_;
   double subsample_;
-  int64_t batch_;
   uint64_t seed_;
+  int64_t batch_keys_;
+  std::atomic<uint64_t> produced_{0};
+
+ private:
+  struct Slot { std::vector<Key> keys, uniq; int64_t valid = 0; };
+  std::vector<uint32_t> seen_;   // producer thread: round-stamped table for the per-batch deduplication
+  uint32_t seen_epoch_ = 0;
+  std::vector<Key> uniq_;
   std::vector<Slot> ring_;
   size_t head_ = 0, tail_ = 0, count_ = 0;   // ring state (mu_)
   bool done_ = true, abort_ = false;
   std::mutex mu_;
   std::condition_variable cv_put_, cv_get_;
   std::thread thread_;
-  std::atomic<uint64_t> produced_{0};
+};
+
+// Produces [2, batch_pairs] key batches (row 0: syn0 key of the context word = 2*w, row 1: syn1 key of the centre
+// word = 2*w + 1) for one epoch over the encoded sentences, on a background thread.
+class PairStream : public KeyBatchStream {
+ public:
+  PairStream(std::shared_ptr<Corpus> corpus, int window, double subsample, int64_t batch_pairs, uint64_t seed,
+             int queue_depth = 8);
+  ~PairStream() override;
+  // Copies the next batch into out[2 * batch_pairs]; returns the number of valid pairs (a short last batch is padded
+  // by repeating its pairs), 0 at the end of the epoch.
+  int64_t next(Key* out);
+  int64_t batch_pairs() const { return batch_; }
+  uint64_t pairs_produced() const { return produced_.load(); }
+
+ private:
+  void run(uint64_t epoch) override;
+  int64_t batch_;
+};
+
+// Produces CBOW window batches [batch_windows, 1 + 2 * window]: column 0 the syn1 key of the centre word, then the syn0
+// keys of its context words in sentence order, padded with -1. The rng draws (subsampling, window shrink) are
+// PairStream's: for the same seed and epoch, expanding every window into (context, centre) pairs gives exactly the
+// pairs of PairStream. A short last batch is padded with windows whose centre is -1. window <= 16.
+class WindowStream : public KeyBatchStream {
+ public:
+  static constexpr int kMaxWindow = 16;
+  WindowStream(std::shared_ptr<Corpus> corpus, int window, double subsample, int64_t batch_windows, uint64_t seed,
+               int queue_depth = 8);
+  ~WindowStream() override;
+  int64_t batch_windows() const { return batch_; }
+  int64_t columns() const { return 1 + 2 * (int64_t)window_; }
+  uint64_t windows_produced() const { return produced_.load(); }
+
+ private:
+  void run(uint64_t epoch) override;
+  int64_t batch_;
 };
 
 }  // namespace adapm

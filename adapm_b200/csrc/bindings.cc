@@ -255,6 +255,20 @@ PYBIND11_MODULE(_C, m) {
            })
       .def("batch_pairs", &PairStream::batch_pairs)
       .def("pairs_produced", &PairStream::pairs_produced);
+  py::class_<WindowStream, std::shared_ptr<WindowStream>>(m, "WindowStream")
+      .def(py::init<std::shared_ptr<Corpus>, int, double, int64_t, uint64_t, int>(), py::arg("corpus"), py::arg("window"),
+           py::arg("subsample"), py::arg("batch_windows"), py::arg("seed"), py::arg("queue_depth") = 8)
+      .def("start_epoch", &WindowStream::start_epoch, py::call_guard<py::gil_scoped_release>())
+      .def("next_with_unique", [](WindowStream& p, uintptr_t out, uintptr_t uniq) {
+             int64_t n = 0;
+             int64_t valid;
+             { py::gil_scoped_release r; valid = p.next_with_unique(ptr<Key>(out), ptr<Key>(uniq), &n); }
+             return py::make_tuple(valid, n);
+           })
+      .def("batch_windows", &WindowStream::batch_windows)
+      .def("columns", &WindowStream::columns)
+      .def("windows_produced", &WindowStream::windows_produced);
+  m.attr("window_stream_max_window") = WindowStream::kMaxWindow;
 
   // host RPC (legacy SimpleApp capability, rpc.h)
   m.attr("kServerGroup") = (int)kServerGroup;

@@ -17,6 +17,18 @@ void sgns_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const K
 bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, const Key* negatives,
                    int n_pairs, int neg, int d, float alpha, float* loss_out, unsigned long long* stats);
 
+// word2vec CBOW (ops_cbow.cu): one window per centre[i] with contexts[i * nc .. (i + 1) * nc) (syn0 keys, -1 = padding)
+// and negatives[i * neg .. (i + 1) * neg) (syn1 keys); rows [embedding d | AdaGrad d]. d % 4 == 0, 4 <= d <= 336,
+// 1 + neg <= 32, nc <= 32. deterministic (one GPU only): start-of-step reads, updates grouped by key and summed in fixed
+// point (8 launches, the scan counted as two), bit-identical runs; else one kernel that adds the updates in place.
+// stats: (local rows, remote rows, slow-path rows, updates), accumulated.
+constexpr int kCbowMaxDim = 336;
+constexpr int kCbowMaxTargets = 32;
+constexpr int kCbowMaxContexts = 32;
+void cbow_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, const Key* negatives,
+               int n_win, int nc, int neg, int d, float alpha, float* loss_out, unsigned long long* stats,
+               bool deterministic);
+
 // word2vec SGNS with shared negatives on the tensor cores (ops_sgns_shared.cu): three wgmma GEMMs + three elementwise
 // kernels between ONE Pull and ONE Push of the rows [centers | contexts | shared negatives].
 size_t sgns_shared_workspace_bytes(int B, int Nn, int d);

@@ -25,6 +25,16 @@ void bind(py::module_& m) {
     sgns_step(backend_of(be), (cudaStream_t)stream, ptr<const Key>(centers), ptr<const Key>(contexts),
               ptr<const Key>(negatives), n_pairs, neg, d, alpha, ptr<float>(loss), ptr<unsigned long long>(stats), impl);
   });
+  m.attr("cbow_max_dim") = kCbowMaxDim;
+  m.attr("cbow_max_targets") = kCbowMaxTargets;
+  m.attr("cbow_max_contexts") = kCbowMaxContexts;
+  m.def("cbow_step", [](uintptr_t be, uintptr_t stream, uintptr_t centers, uintptr_t contexts, uintptr_t negatives,
+                        int n_win, int nc, int neg, int d, float alpha, uintptr_t loss, uintptr_t stats,
+                        bool deterministic) {
+    cbow_step(backend_of(be), (cudaStream_t)stream, ptr<const Key>(centers), ptr<const Key>(contexts),
+              ptr<const Key>(negatives), n_win, nc, neg, d, alpha, ptr<float>(loss), ptr<unsigned long long>(stats),
+              deterministic);
+  });
   m.def("sample_keys", [](uintptr_t be, uintptr_t stream, int kind, uintptr_t prob, uintptr_t alias, int64_t n_table,
                           Key first, Key stride, uintptr_t out, int64_t n, uint64_t seed, bool local_only, int max_tries,
                           uintptr_t stats) {

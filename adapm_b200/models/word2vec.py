@@ -1,4 +1,4 @@
-"""word2vec skip-gram with negative sampling (SGNS) + AdaGrad on the parameter manager.
+"""word2vec skip-gram (SGNS) or continuous bag of words (CBOW) with negative sampling + AdaGrad on the parameter manager.
 
 Behavioural parity with the reference application ``apps/word2vec.cc``:
 
@@ -16,6 +16,12 @@ Behavioural parity with the reference application ``apps/word2vec.cc``:
 
 GPU-first differences: the per-pair loop of the reference is one batched kernel
 (``ops.sgns_step``) that fuses pull, scoring, AdaGrad and push over local HBM / NVLink peers.
+
+CBOW (``cbow=True``, word2vec.c's ``-cbow 1``, which the reference does not implement) trains one window per corpus word:
+the mean ``h`` of the context rows is scored against the centre's syn1 row and the negatives, each target gets
+``g_t h`` and every context occurrence the unscaled ``neu1e = sum_t g_t t`` (word2vec.c), each through worker-side
+AdaGrad (``cbow_reference_step``; ``ops.cbow_step`` on the GPU). Batches are windows ``[B, 1 + 2 window]`` (centre syn1
+key, context syn0 keys, -1 padding) from ``NativeCorpus.window_batches`` or ``windows_from_sentences``.
 """
 from __future__ import annotations
 
@@ -47,6 +53,8 @@ class Word2VecConfig:
     intent_prepass: bool = False     # experimental: device-side Intent for keys that are already local (ops.IntentPrepass)
     shared_negatives: int = 0        # > 0: ONE set of this many negatives per batch, contractions on the tensor cores
                                      # (ops.SgnsSharedStep); 0: `negative` private negatives per pair (the reference)
+    cbow: bool = False               # continuous bag of words (word2vec.c -cbow 1) instead of skip-gram
+    batch_windows: int = 8192        # CBOW: windows per step
 
     @property
     def row_len(self) -> int:
@@ -55,6 +63,11 @@ class Word2VecConfig:
     @property
     def num_keys(self) -> int:
         return 2 * self.vocab_size
+
+    @property
+    def window_columns(self) -> int:
+        # CBOW batch columns: the centre, then up to 2 * window contexts
+        return 1 + 2 * self.window
 
     @property
     def updates_per_pair(self) -> int:
@@ -101,11 +114,45 @@ class SyntheticPairs:
         return t
 
 
+class SyntheticWindows:
+    """Synthetic CBOW window batches [batch_windows, 1 + 2 window] drawn like the loader's: a stream of Zipf words read
+    as one long sentence, and for each of ``batch_windows`` consecutive positions a window shrunk by b uniform in
+    [0, window). Deterministic per (seed, rank, step)."""
+
+    def __init__(self, cfg: Word2VecConfig, counts: np.ndarray, rank: int, seed: int = 1, pin: bool = False):
+        self.cfg, self.rank, self.seed = cfg, rank, seed
+        p = counts / counts.sum()
+        self.cdf = np.cumsum(p)
+        self.cdf[-1] = 1.0
+        self.pin = pin
+
+    def batch(self, step: int):
+        rng = np.random.default_rng([self.seed, self.rank, step, 1])
+        B, W = self.cfg.batch_windows, self.cfg.window
+        w = np.searchsorted(self.cdf, rng.random(B + 2 * W), side="right").astype(np.int64)
+        np.clip(w, 0, self.cfg.vocab_size - 1, out=w)
+        r = W - rng.integers(0, W, B)                                   # shrunk radius per window
+        off = np.concatenate([np.arange(-W, 0), np.arange(1, W + 1)])  # context offsets in sentence order
+        pos = np.arange(W, W + B)
+        ctx = syn0_key(w[pos[:, None] + off[None, :]])
+        keep = np.abs(off)[None, :] <= r[:, None]
+        out = np.full((B, 1 + 2 * W), -1, dtype=np.int64)
+        out[:, 0] = syn1_key(w[pos])
+        order = np.argsort(~keep, axis=1, kind="stable")                # kept contexts first, in sentence order
+        out[:, 1:] = np.where(np.take_along_axis(keep, order, 1), np.take_along_axis(ctx, order, 1), -1)
+        t = torch.from_numpy(out)
+        if self.pin:
+            t = t.pin_memory()
+        return t
+
+
 class Word2Vec:
     def __init__(self, server, worker, cfg: Word2VecConfig, counts: Optional[np.ndarray] = None):
         self.server, self.worker, self.cfg = server, worker, cfg
         self.counts = counts if counts is not None else zipf_counts(cfg.vocab_size, cfg.zipf_exponent)
         assert len(self.counts) == cfg.vocab_size
+        if cfg.cbow and cfg.shared_negatives > 0:
+            raise ValueError("shared_negatives is a skip-gram option: CBOW draws its own negatives per window")
         self.cuda = server.backend == "cuda"
         self.alpha = cfg.starting_alpha
         self.step_no = 0
@@ -118,13 +165,16 @@ class Word2Vec:
             dev = server.device
             self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
             self.stats = torch.zeros(4, dtype=torch.int64, device=dev)
-            self._neg = torch.empty(cfg.batch_pairs * cfg.negative, dtype=torch.int64, device=dev)
-            self._keys_dev = [torch.empty(2, cfg.batch_pairs, dtype=torch.int64, device=dev)
+            # a step's key batch: [2, batch_pairs] pairs, or CBOW windows [batch_windows, 1 + 2 window]
+            shape = (cfg.batch_windows, cfg.window_columns) if cfg.cbow else (2, cfg.batch_pairs)
+            n_items = cfg.batch_windows if cfg.cbow else cfg.batch_pairs
+            self._neg = torch.empty(n_items * cfg.negative, dtype=torch.int64, device=dev)
+            self._keys_dev = [torch.empty(*shape, dtype=torch.int64, device=dev)
                               for _ in range(max(1, cfg.max_inflight) + 1)]
             self._events = [None] * len(self._keys_dev)
             # data-loader side: the NEXT batch is copied host->device on a copy stream while the current step runs
             self._copy_stream = torch.cuda.Stream(device=dev)
-            self._pf_bufs = [torch.empty(2, cfg.batch_pairs, dtype=torch.int64, device=dev)
+            self._pf_bufs = [torch.empty(*shape, dtype=torch.int64, device=dev)
                              for _ in range(max(1, cfg.max_inflight) + 2)]
             self._pf_no = 0
             self._pf = None
@@ -162,12 +212,15 @@ class Word2Vec:
 
     # ------------------------------------------------------------------ intent
     def signal_intent(self, keys_host: torch.Tensor, clock: int) -> None:
-        """keys_host: [2, B] (syn0 keys, syn1 keys) of a future batch (CPU tensor)."""
+        """keys_host: [2, B] (syn0 keys, syn1 keys) or CBOW windows [B, 1 + 2 window] of a future batch (CPU tensor)."""
         if not self.cfg.signal_intent or self.server.num_servers() == 1:
             return
         # batches of the native loader carry their distinct keys (deduplicated on the loader thread)
         keys = getattr(keys_host, "unique_keys", None)
-        keys = keys if keys is not None else keys_host.view(-1)
+        if keys is None:
+            keys = keys_host.reshape(-1)
+            if self.cfg.cbow:
+                keys = keys[keys >= 0]                 # window padding
         if self.cuda and self._prepass is not None:
             self._prepass.harvest()                    # left-overs of earlier batches -> host path
             self._prepass.submit(keys, clock, clock + 1)
@@ -176,7 +229,8 @@ class Word2Vec:
 
     # ------------------------------------------------------------------ one training step
     def step(self, keys_host: torch.Tensor) -> torch.Tensor:
-        """Runs one batch. ``keys_host``: [2, B] int64 CPU tensor (pinned for the e2e path).
+        """Runs one batch. ``keys_host``: [2, B] int64 CPU tensor (pinned for the e2e path); CBOW: windows
+        [batch_windows, 1 + 2 window] (column 0 the centre's syn1 key, then context syn0 keys, -1 = padding).
         Returns the device tensor that accumulates the summed loss (read it with ``.item()``/copy)."""
         cfg = self.cfg
         if self.cuda:
@@ -191,13 +245,18 @@ class Word2Vec:
                 kd = self._keys_dev[slot]
                 kd.copy_(keys_host, non_blocking=True)               # H2D of this step's inputs
             self.sample_negatives()
-            self._device_step(kd[0], kd[1])
+            self._device_step(*self._operands(kd))
             ev = self._events[slot] or torch.cuda.Event()
             ev.record()
             self._events[slot] = ev
             self.step_no += 1
             return self.loss
         return self._step_cpu(keys_host)
+
+    def _operands(self, kd: torch.Tensor):
+        if self.cfg.cbow:                 # (centres, contexts) of the windows, contiguous for the kernel
+            return kd[:, 0].contiguous(), kd[:, 1:].contiguous()
+        return kd[0], kd[1]
 
     def prefetch(self, keys_host: torch.Tensor) -> None:
         """Start the host->device copy of a future step's key batch (pinned memory) on the copy stream; the
@@ -213,7 +272,7 @@ class Word2Vec:
         self._pf = (keys_host, b, ev)
 
     def sample_negatives(self) -> torch.Tensor:
-        """PrepareSample/PullSample on the device: draws batch_pairs*negative syn1 keys; the ``local``
+        """PrepareSample/PullSample on the device: draws batch_pairs*negative (CBOW: batch_windows*negative) syn1 keys; the ``local``
         scheme rejects keys that are not resident in this GPU's HBM."""
         cfg = self.cfg
         local_only = cfg.sampling_scheme == "local" and self.server.num_servers() > 1
@@ -224,7 +283,12 @@ class Word2Vec:
         from ..ops import SgnsSharedStep, sgns_step
 
         cfg = self.cfg
-        if cfg.shared_negatives > 0:
+        if cfg.cbow:
+            from ..ops import cbow_step
+
+            cbow_step(self.server, centers, contexts, self._neg.view(centers.numel(), cfg.negative), cfg.embed_dim,
+                      self.alpha, self.loss, self.stats)
+        elif cfg.shared_negatives > 0:
             if getattr(self, "_shared", None) is None:
                 self._shared = SgnsSharedStep(self.server, self.worker, cfg.batch_pairs, cfg.shared_negatives, cfg.embed_dim)
             self._shared(centers, contexts, self._neg[:cfg.shared_negatives], self.alpha, self.loss)
@@ -237,7 +301,7 @@ class Word2Vec:
         if self._events[slot] is not None:
             self._events[slot].synchronize()
         self.sample_negatives()
-        self._device_step(keys_dev[0], keys_dev[1])
+        self._device_step(*self._operands(keys_dev))
         ev = self._events[slot] or torch.cuda.Event()
         ev.record()
         self._events[slot] = ev
@@ -255,8 +319,10 @@ class Word2Vec:
         from ``intent_batches`` (default: ``batches``): host tensors that may carry ``unique_keys`` (their distinct keys)."""
         from .. import _C
 
-        assert self.cuda, "run_steps needs the cuda backend"
         cfg = self.cfg
+        if cfg.cbow:
+            raise ValueError("run_steps drives skip-gram steps only: run CBOW steps with step()")
+        assert self.cuda, "run_steps needs the cuda backend"
         if getattr(self, "_loop", None) is None:
             local_only = cfg.sampling_scheme == "local" and self.server.num_servers() > 1
             sp = self.sampler
@@ -288,6 +354,14 @@ class Word2Vec:
     # reference-semantics step through the public Pull/Push API (CPU backend; also the numerics oracle)
     def _step_cpu(self, keys_host: torch.Tensor) -> torch.Tensor:
         cfg, kv, d = self.cfg, self.worker, self.cfg.embed_dim
+        if cfg.cbow:
+            B = keys_host.shape[0]
+            u = torch.rand(B * cfg.negative, generator=self._gen, dtype=torch.float64)
+            negw = torch.searchsorted(self._neg_cdf, u).clamp_(max=cfg.vocab_size - 1)
+            loss = cbow_reference_step(kv, keys_host[:, 0], keys_host[:, 1:], syn1_key(negw).view(B, cfg.negative), d,
+                                       self.alpha)
+            self.step_no += 1
+            return torch.tensor([loss], dtype=torch.float32)
         centers, contexts = keys_host[0], keys_host[1]
         B = centers.numel()
         if cfg.shared_negatives > 0:      # one set of negatives for the batch (the GEMM formulation), through Pull / Push
@@ -492,3 +566,50 @@ def sgns_reference_step(kv, centers: torch.Tensor, contexts: torch.Tensor, negat
     kv.wait(kv.push(centers, torch.cat([u0e, u0a], -1).contiguous().view(-1)))
     z = torch.where(label > 0.5, f, -f).clamp(-6, 6)
     return float((torch.log1p(torch.exp(-z)) * valid).sum())
+
+
+def cbow_reference_step(kv, centers: torch.Tensor, contexts: torch.Tensor, negatives: torch.Tensor, d: int,
+                        alpha: float) -> float:
+    """Plain PyTorch fp32 CBOW step through Pull/Push, the rule of ``ops.cbow_step``. ``centers``: [B] syn1 keys (< 0:
+    the window does nothing), ``contexts``: [B, C] syn0 keys (-1 = padding), ``negatives``: [B, neg] syn1 keys. All
+    windows read the state at the start of the step: ``h`` = mean of the C context embeddings (a repeated word counts
+    every time), targets the centre (label 1) and the negatives (label 0; one equal to the centre is skipped),
+    ``g = label - sigmoid(h . t)`` saturated at |f| > 6, one AdaGrad push of ``g h`` per (window, target) and one of
+    ``neu1e = sum_t g t`` (not divided by C, as word2vec.c) per context occurrence; updates of repeated keys add up.
+    Returns the summed logistic loss."""
+    centers, contexts, negatives = centers.reshape(-1), contexts.reshape(centers.numel(), -1), negatives
+    B, C = contexts.shape
+    neg = negatives.shape[1]
+    xm = (contexts >= 0) & (centers >= 0).view(B, 1)
+    n_ctx = xm.sum(1)
+    active = (centers >= 0) & (n_ctx > 0)
+    xm &= active.view(B, 1)
+    tk = torch.cat([centers.view(B, 1), negatives], 1)              # [B, 1 + neg] target keys
+    tm = active.view(B, 1).repeat(1, 1 + neg)
+    tm[:, 1:] &= negatives != centers.view(B, 1)
+    xkeys, tkeys = contexts[xm], tk[tm]
+    rows = torch.empty((xkeys.numel() + tkeys.numel()) * 2 * d, dtype=torch.float32)
+    kv.wait(kv.pull(torch.cat([xkeys, tkeys]), rows))
+    rows = rows.view(-1, 2 * d)
+    rx, rt = rows[:xkeys.numel()], rows[xkeys.numel():]
+    ex = torch.zeros(B, C, d)
+    ex[xm] = rx[:, :d]
+    h = ex.sum(1) / n_ctx.clamp(min=1).view(B, 1).to(torch.float32)
+    et, at = torch.zeros(B, 1 + neg, d), torch.ones(B, 1 + neg, d)
+    et[tm], at[tm] = rt[:, :d], rt[:, d:]
+    label = torch.zeros(B, 1 + neg)
+    label[:, 0] = 1
+    f = (h.unsqueeze(1) * et).sum(-1)
+    g = label - torch.sigmoid(f)
+    g = torch.where(f > 6, label - 1, g)
+    g = torch.where(f < -6, label, g)
+    g = g * tm
+    neu1e = (g.unsqueeze(-1) * et).sum(1)                           # [B, d]
+    gt = g.unsqueeze(-1) * h.unsqueeze(1)
+    ut = torch.cat([alpha * gt / torch.sqrt(at + gt * gt), gt * gt], -1)[tm]
+    gx = neu1e.unsqueeze(1).expand(B, C, d)[xm]
+    ax = rx[:, d:]
+    ux = torch.cat([alpha * gx / torch.sqrt(ax + gx * gx), gx * gx], -1)
+    kv.wait(kv.push(torch.cat([tkeys, xkeys]), torch.cat([ut, ux]).contiguous().view(-1)))
+    z = torch.where(label > 0.5, f, -f).clamp(-6, 6)
+    return float((torch.log1p(torch.exp(-z)) * tm).sum())

@@ -46,6 +46,43 @@ def sgns_step(server, centers: torch.Tensor, contexts: torch.Tensor, negatives: 
                  stats.data_ptr() if stats is not None else 0, {"auto": 0, "ldg": 1, "tma": 2}[impl])
 
 
+CBOW_MAX_DIM = 336
+CBOW_MAX_TARGETS = 32
+CBOW_MAX_CONTEXTS = 32
+
+
+def cbow_step(server, centers: torch.Tensor, contexts: torch.Tensor, negatives: torch.Tensor, embed_dim: int,
+              alpha: float, loss: torch.Tensor, stats: Optional[torch.Tensor] = None,
+              deterministic: Optional[bool] = None) -> None:
+    """Fused word2vec CBOW step (csrc/cuda/ops_cbow.cu) on ``server``'s store: one window per ``centers[i]`` (syn1 key;
+    < 0: the window does nothing) with the syn0 keys ``contexts[i]`` ([B, C], -1 = padding) and the syn1 keys
+    ``negatives[i]`` ([B, neg]). The rule is :func:`adapm_b200.models.word2vec.cbow_reference_step`'s: ``h`` = mean of
+    the context embeddings, one AdaGrad push per (window, target) of ``g_t h`` and one per context occurrence of
+    ``neu1e = sum_t g_t t``; a negative equal to the centre is skipped. ``loss``: float32[1], accumulated (+=);
+    ``stats``: optional int64[4] accumulated with (local rows, remote rows, slow-path rows, updates).
+    ``4 <= embed_dim <= 336`` and a multiple of 4, ``1 + neg <= 32``, ``C <= 32``.
+
+    ``deterministic``: ``None`` picks the deterministic step on a single-GPU server (start-of-step reads, updates
+    grouped by key and summed in fixed point: bit-identical runs, 8 launches) and the in-place kernel (one launch,
+    Hogwild between windows) on several GPUs; ``False`` forces the in-place kernel; ``True`` on several GPUs raises
+    ``ValueError``."""
+    _i64(centers, "centers"); _i64(contexts, "contexts"); _i64(negatives, "negatives"); _f32(loss, "loss")
+    if isinstance(embed_dim, bool) or int(embed_dim) != embed_dim or not (
+            4 <= int(embed_dim) <= CBOW_MAX_DIM and int(embed_dim) % 4 == 0):
+        raise ValueError(f"embed_dim must be a multiple of 4 in [4, {CBOW_MAX_DIM}], got {embed_dim}")
+    B = centers.numel()
+    if contexts.dim() != 2 or contexts.shape[0] != B or not 1 <= contexts.shape[1] <= CBOW_MAX_CONTEXTS:
+        raise ValueError(f"contexts must be [B, C] with 1 <= C <= {CBOW_MAX_CONTEXTS}, got {tuple(contexts.shape)}")
+    if negatives.dim() != 2 or negatives.shape[0] != B or negatives.shape[1] + 1 > CBOW_MAX_TARGETS:
+        raise ValueError(f"negatives must be [B, neg] with 1 + neg <= {CBOW_MAX_TARGETS}, got {tuple(negatives.shape)}")
+    if stats is not None and not (stats.is_cuda and stats.dtype == torch.int64 and stats.numel() >= 4):
+        raise TypeError("stats must be a CUDA int64 tensor with 4 entries")
+    det = _check_deterministic(server, server.num_servers() == 1 if deterministic is None else deterministic)
+    _C.cbow_step(server._impl.backend_handle(), _stream(centers), centers.data_ptr(), contexts.data_ptr(),
+                 negatives.data_ptr(), B, int(contexts.shape[1]), int(negatives.shape[1]), int(embed_dim), float(alpha),
+                 loss.data_ptr(), stats.data_ptr() if stats is not None else 0, det)
+
+
 class SgnsSharedStep:
     """word2vec SGNS with one set of negatives shared by all pairs of a batch, on the tensor cores
     (csrc/cuda/ops_sgns_shared.cu; SURVEY K7's GEMM formulation, an option next to the reference-faithful fused step).

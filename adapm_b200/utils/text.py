@@ -82,10 +82,45 @@ def pairs_from_sentences(sentences: Iterator[np.ndarray], window: int, batch_pai
         yield torch.from_numpy(np.stack([np.concatenate(buf_c), np.concatenate(buf_t)]))
 
 
+def windows_from_sentences(sentences: Iterator[np.ndarray], window: int, batch_windows: int, rng) -> Iterator[torch.Tensor]:
+    """CBOW window batches [batch_windows, 1 + 2 * window]: column 0 the syn1 key of the centre word, then the syn0 keys
+    of its context words in sentence order, padded with -1. The window shrink is drawn like :func:`pairs_from_sentences`
+    (same rng calls), so expanding the windows into (context, centre) pairs gives its pairs. A short last batch is padded
+    with windows whose centre is -1; ``valid_windows`` of each batch tells how many are real."""
+    if not 1 <= window <= 16:
+        raise ValueError(f"window must be in [1, 16], got {window}")
+    cols = 1 + 2 * window
+    cur = np.full((batch_windows, cols), -1, dtype=np.int64)
+    n = 0
+    for s in sentences:
+        L = s.size
+        for pos in range(L):
+            b = int(rng.integers(0, window))
+            lo, hi = max(0, pos - (window - b)), min(L, pos + (window - b) + 1)
+            ctx = np.concatenate([s[lo:pos], s[pos + 1:hi]])
+            if ctx.size == 0:
+                continue
+            cur[n] = -1
+            cur[n, 0] = 2 * s[pos] + 1                               # syn1 key of the centre word
+            cur[n, 1:1 + ctx.size] = 2 * ctx                         # syn0 keys of the context words
+            n += 1
+            if n == batch_windows:
+                t = torch.from_numpy(cur.copy())
+                t.valid_windows = n
+                yield t
+                n = 0
+    if n:
+        cur[n:] = -1
+        t = torch.from_numpy(cur.copy())
+        t.valid_windows = n
+        yield t
+
+
 # ------------------------------------------------------------------------------------------ native loader
 class NativeCorpus:
     """C++ corpus (csrc/adapm/corpus.{h,cc}): same vocabulary rules as :class:`Vocabulary` (count-descending, ties by
-    first occurrence, ``</s>`` = word 0), plus the encoded sentences of this rank and a background pair generator."""
+    first occurrence, ``</s>`` = word 0), plus the encoded sentences of this rank and background generators of
+    skip-gram pairs and CBOW windows."""
 
     def __init__(self, impl):
         self._impl = impl
@@ -142,4 +177,30 @@ class NativeCorpus:
                 return
             t.valid_pairs = int(valid)
             t.unique_keys = u[:n_u]          # what to call Intent() with (deduplicated on the loader thread)
+            yield t
+
+    def window_batches(self, window: int, subsample: float, batch_windows: int, seed: int, epoch: int = 0,
+                       pin: bool = False, queue_depth: int = 8) -> Iterator[torch.Tensor]:
+        """CBOW window batches [batch_windows, 1 + 2 * window] of one epoch (layout of :func:`windows_from_sentences`),
+        generated by a background C++ thread with the rng draws of :meth:`pair_batches`: for the same seed and epoch,
+        expanding the windows into (context, centre) pairs gives its pairs. ``window <= 16``. A short final batch is
+        padded with windows whose centre is -1; ``valid_windows`` tells how many are real, ``unique_keys`` holds the
+        batch's distinct keys (for Intent)."""
+        from .. import _C
+
+        if not 1 <= window <= _C.window_stream_max_window:
+            raise ValueError(f"window must be in [1, {_C.window_stream_max_window}], got {window}")
+        ws = _C.WindowStream(self._impl, int(window), float(subsample), int(batch_windows), int(seed), int(queue_depth))
+        ws.start_epoch(int(epoch))
+        cols = ws.columns()
+        while True:
+            t = torch.empty(batch_windows, cols, dtype=torch.int64)
+            if pin:
+                t = t.pin_memory()
+            u = torch.empty(batch_windows * cols, dtype=torch.int64)
+            valid, n_u = ws.next_with_unique(t.data_ptr(), u.data_ptr())
+            if valid == 0:
+                return
+            t.valid_windows = int(valid)
+            t.unique_keys = u[:n_u]
             yield t
