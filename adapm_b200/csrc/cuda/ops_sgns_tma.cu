@@ -9,9 +9,10 @@
 //   whole warp  : mbarrier.try_wait, LDS.128 the row from shared memory, dot / sigmoid / AdaGrad,
 //                 the update overwrites the consumed ring slot
 //   lane 0      : cp.reduce.async.bulk (UBLKRED) of that slot into the row's home (local HBM or NVLink peer)
-// The deterministic one-GPU step (sgns_step_det) runs the same body as a score pass that loads only the targets'
-// embedding halves and writes no row, then groups the step's contributions by key and lets one warp per row gather them
-// as fixed-point integer sums.
+// The deterministic one-GPU step (sgns_step_det) runs the same body as a score pass that loads the targets' embedding
+// halves, then groups the step's contributions by key and lets one warp per row gather them as fixed-point integer sums.
+// A key with a single entry in the step (two thirds of the keys at the benchmark's shape) skips the grouping: the score
+// pass loads its whole row and writes the update back itself, with the gather pass's fixed-point arithmetic.
 // The TMA engine reads rows that live on a peer GPU through their NVLink-mapped addresses as well;
 // rows in a transitional protocol state take the generic out-of-line path.
 #include <cuda_runtime.h>
@@ -20,6 +21,7 @@
 #include <cstdlib>
 
 #include <cub/cub.cuh>
+#include <thrust/iterator/transform_iterator.h>
 
 #include "fx_accum.cuh"
 #include "ops.h"
@@ -45,6 +47,8 @@ struct ScoreOut {
   float* snap;                   // [distinct centers x d] start-of-step embedding of each center, by compact id
                                  // (the deterministic step keeps it right after g0 in one buffer)
   int* pcid;                     // [n_pairs] compact id of the pair's center
+  const int* cnt;                // [distinct keys] entries of each key in the step, by compact id: the score pass
+                                 // applies a key with one entry itself
 };
 
 struct WarpSmem {
@@ -61,9 +65,11 @@ struct WarpSmem {
 // slot with [embedding update | AdaGrad update] and lane 0 issues cp.reduce.async.bulk from it; the slot is reloaded one
 // target later, after the reduction has read it (prefetch distance RING - 1).
 // SCORE: score pass of the deterministic one-GPU step (sgns_score_tma_kernel, its own kernel so that the in-place
-// variants keep their register allocation). It reads start-of-step rows only - the embedding half of each target - and
-// writes no store row: per pair the center gradient g0, per target gs, and each center's embedding (ScoreOut). The
-// gather pass forms and applies every row's update from these.
+// variants keep their register allocation). It reads start-of-step rows - the embedding half of each target - and
+// writes per pair the center gradient g0, per target gs, and each center's embedding (ScoreOut). The gather pass forms
+// and applies the rows' updates from these. A key whose only entry in the step is this pair's (ScoreOut::cnt) is the
+// exception: no other warp reads or writes its row during the step, so the warp loads the whole row (target) or its
+// AdaGrad half (center), applies the one term exactly as the gather pass would (fx_apply_one) and stores the row.
 template <int VPL, bool SCORE>
 __device__ __forceinline__ void
 sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
@@ -107,16 +113,26 @@ sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __r
     // version counter (owned row) and the dirty byte (replica), so one pointer + a kind bit hold it (frees registers)
     float* my_row = nullptr;
     void* my_mark = nullptr;
-    int my_bits = 0;                     // bit 1: my_mark is a replica dirty byte,
+    int my_bits = 0;                     // bit 0: the key's only entry in the step is this one (SCORE),
+                                         // bit 1: my_mark is a replica dirty byte,
                                          // bits 2..: the center's compact id (SCORE, lane 0)
     if (lane == 0) my_key = ckey;
     else if (lane - 1 < n_targets) my_key = (lane == 1) ? pos_key : negatives[(size_t)p * neg + (lane - 2)];
     if (my_key >= 0) {
+      int cid = 0, n_entries = 0;
+      if (SCORE) {                       // (a chain of its own, next to resolve_fast's)
+        cid = __ldg(cidx + my_key);
+        n_entries = __ldg(so.cnt + cid);
+      }
       const Target tg = dev::resolve_fast(c, my_key, 0, &n_local, &n_remote);
       my_row = tg.row;
       my_mark = tg.flag ? (void*)tg.flag : (void*)tg.version;
-      my_bits = (tg.flag ? 2 : 0) | (SCORE && lane == 0 ? __ldg(cidx + my_key) << 2 : 0);
+      const bool dup = lane >= 2 && my_key == pos_key;   // a negative equal to the context is no entry
+      my_bits = (tg.flag ? 2 : 0) | (SCORE && lane == 0 ? cid << 2 : 0) | (SCORE && n_entries == 1 && !dup ? 1 : 0);
     }
+    // SCORE: lane l's key has one entry in the step, and it is this pair's: no other warp reads or writes its row during
+    // the step, so this warp loads the whole row and writes its update back (the gather pass does not see the key)
+    const unsigned single = SCORE ? __ballot_sync(0xffffffffu, my_bits & 1) : 0u;
     // target t (0-based) -> lane t+1 (only pairs with <= 31 targets use this kernel)
     auto issue = [&](int t) {
       const int b = issued % RING;
@@ -130,8 +146,9 @@ sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __r
         // local HBM row - or a peer's row: the TMA engine reads NVLink-mapped addresses as well
         if (BULK) bulk_wait_read<1>();   // the reduction that used this slot (issued one target ago) has read it
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // order earlier LDS of this slot before the TMA write
-        mbar_expect_tx(&bars[b], load_bytes);
-        bulk_g2s(buf, row, load_bytes, &bars[b]);
+        const uint32_t bytes = (single >> (t + 1)) & 1u ? row_bytes : load_bytes;
+        mbar_expect_tx(&bars[b], bytes);
+        bulk_g2s(buf, row, bytes, &bars[b]);
       }
       ++issued;
     };
@@ -211,6 +228,7 @@ sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __r
         loss_acc += sgns::slow_target(c, tkey, label, alpha, d, buf, e0s, g0s, &applied);  // ring slot b is free: use it as stage
         if (applied) ++n_upd;
       } else if (!dup) {
+        const bool one = (single >> (t + 1)) & 1u;   // SCORE: the slot holds the whole row, which this warp updates
         float4 e1[VPL];
         float f = 0.f;
 #pragma unroll
@@ -235,6 +253,15 @@ sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __r
           if (j < nvec) {
             if (SCORE) {                  // the gather pass forms the target's update from gs
               g0[v].x += gs * e1[v].x; g0[v].y += gs * e1[v].y; g0[v].z += gs * e1[v].z; g0[v].w += gs * e1[v].w;
+              if (one) {                  // ... unless its key has this one entry: gs * e0 as the gather pass adds it
+                float4 a1 = reinterpret_cast<const float4*>(buf + d)[j];
+                fx_apply_one(e1[v].x, a1.x, gs * e0[v].x, alpha);
+                fx_apply_one(e1[v].y, a1.y, gs * e0[v].y, alpha);
+                fx_apply_one(e1[v].z, a1.z, gs * e0[v].z, alpha);
+                fx_apply_one(e1[v].w, a1.w, gs * e0[v].w, alpha);
+                reinterpret_cast<float4*>(t_row)[j] = e1[v];
+                reinterpret_cast<float4*>(t_row + d)[j] = a1;
+              }
               continue;
             }
             float4 a1 = reinterpret_cast<const float4*>(buf + d)[j];
@@ -306,10 +333,27 @@ sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __r
       }
       if (SCORE && lane == 0) gs_buf[(size_t)p * (neg + 2)] = kNoEntry;
     } else if (SCORE) {                   // the gather pass applies g0 to the center row
+      if (single & 1u) {                  // ... unless this pair is the center's one entry: 1 * g0 as the gather adds it
 #pragma unroll
-      for (int v = 0; v < VPL; ++v) {
-        int j = lane + v * 32;
-        if (j < nvec) reinterpret_cast<float4*>(so.g0 + (size_t)p * d)[j] = g0[v];
+        for (int v = 0; v < VPL; ++v) {
+          int j = lane + v * 32;
+          if (j < nvec) {
+            float4 r = e0[v];
+            float4 a0 = dev::ld_row4(c_row + d + 4 * j);
+            fx_apply_one(r.x, a0.x, g0[v].x, alpha);
+            fx_apply_one(r.y, a0.y, g0[v].y, alpha);
+            fx_apply_one(r.z, a0.z, g0[v].z, alpha);
+            fx_apply_one(r.w, a0.w, g0[v].w, alpha);
+            reinterpret_cast<float4*>(c_row)[j] = r;
+            reinterpret_cast<float4*>(c_row + d)[j] = a0;
+          }
+        }
+      } else {
+#pragma unroll
+        for (int v = 0; v < VPL; ++v) {
+          int j = lane + v * 32;
+          if (j < nvec) reinterpret_cast<float4*>(so.g0 + (size_t)p * d)[j] = g0[v];
+        }
       }
       if (lane == 0) gs_buf[(size_t)p * (neg + 2)] = 0.f;
       if (lane == 0) mark_pushed(my_mark, my_bits);
@@ -421,7 +465,8 @@ __global__ void sgns_det_index_kernel(const __grid_constant__ Ctx c, const Key* 
 }
 
 // SCATTER = false: cnt[id] = entries of key id. SCATTER = true: desc / kid of CSR position off[id] + i, i < cnt[id],
-// describe the entries of key id (from the score pass's gs and pcid); counts cnt back down to zero.
+// describe the entries of key id (from the score pass's gs and pcid); counts cnt back down to zero. A key with one entry
+// has no CSR positions (the score pass applied it): its count is cleared.
 template <bool SCATTER>
 __global__ void sgns_det_group_kernel(const Key* __restrict__ centers, const Key* __restrict__ contexts,
                                       const Key* __restrict__ negatives, int n_pairs, int neg,
@@ -437,7 +482,12 @@ __global__ void sgns_det_group_kernel(const Key* __restrict__ centers, const Key
     if (!SCATTER) {
       atomicAdd(cnt + id, 1);
     } else {
-      const int q = __ldg(off + id) + atomicSub(cnt + id, 1) - 1;
+      const int q0 = __ldg(off + id);
+      if (__ldg(off + id + 1) == q0) {
+        cnt[id] = 0;
+        continue;
+      }
+      const int q = q0 + atomicSub(cnt + id, 1) - 1;
       const float gx = __ldg(gsb + x);
       GatherDesc e;
       if (s == 0) {
@@ -453,7 +503,12 @@ __global__ void sgns_det_group_kernel(const Key* __restrict__ centers, const Key
   }
 }
 
-// The deterministic one-GPU step: index -> score -> count, scan, scatter -> gather -> finish, all on `stream`.
+// CSR positions of a key with c entries: none for a key with one entry (the score pass applies it)
+struct GatheredEntries {
+  __host__ __device__ int operator()(int c) const { return c == 1 ? 0 : c; }
+};
+
+// The deterministic one-GPU step: index -> count, scan -> score -> scatter -> gather -> finish, all on `stream`.
 void sgns_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, const Key* negatives,
                    int n_pairs, int neg, int d, float alpha, float* loss_out, unsigned long long* stats, int vpl,
                    int score_blocks, size_t score_smem) {
@@ -477,8 +532,10 @@ void sgns_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   long long* part = static_cast<long long*>(                                            // zero between steps
       be.step_buffer(kBufPart, ((size_t)n_ranges + 1) * 2 * d * sizeof(long long)));
   float** rowp = static_cast<float**>(be.step_buffer(kBufRowp, (size_t)n_ids * sizeof(float*)));
+  so.cnt = cnt;
+  const auto gathered = thrust::make_transform_iterator(static_cast<const int*>(cnt), GatheredEntries{});
   size_t scan_bytes = 0;
-  ADAPM_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, cnt, off, n_ids + 1, stream));
+  ADAPM_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, gathered, off, n_ids + 1, stream));
   void* scan_tmp = be.step_buffer(kBufScan, scan_bytes);
 
   const int grid_n = be.num_sms() * 8;
@@ -490,6 +547,12 @@ void sgns_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   sgns_det_index_kernel<<<blocks_for((long)n_pairs * (neg + 1)), 256, 0, stream>>>(
       c, centers, contexts, negatives, n_pairs, neg, 1, neg + 1, fx.cidx, fx.keys, rowp, fx.count);
   ADAPM_COUNT_LAUNCH();
+  sgns_det_group_kernel<false><<<blocks_for(n_entries), 256, 0, stream>>>(centers, contexts, negatives, n_pairs, neg,
+                                                                           fx.cidx, cnt, off, kid, gsb, so.pcid, desc);
+  ADAPM_COUNT_LAUNCH();
+  ADAPM_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, gathered, off, n_ids + 1, stream));
+  ADAPM_COUNT_LAUNCH();
+  ADAPM_COUNT_LAUNCH();   // (the scan is two kernels)
 #define ADAPM_LAUNCH_SCORE(V)                                                                                  \
   do {                                                                                                         \
     static bool attr_set = false;                                                                              \
@@ -508,12 +571,6 @@ void sgns_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   }
 #undef ADAPM_LAUNCH_SCORE
   ADAPM_COUNT_LAUNCH();
-  sgns_det_group_kernel<false><<<blocks_for(n_entries), 256, 0, stream>>>(centers, contexts, negatives, n_pairs, neg,
-                                                                           fx.cidx, cnt, off, kid, gsb, so.pcid, desc);
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, cnt, off, n_ids + 1, stream));
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_COUNT_LAUNCH();   // (the scan is two kernels)
   sgns_det_group_kernel<true><<<blocks_for(n_entries), 256, 0, stream>>>(centers, contexts, negatives, n_pairs, neg,
                                                                           fx.cidx, cnt, off, kid, gsb, so.pcid, desc);
   ADAPM_COUNT_LAUNCH();

@@ -1,7 +1,8 @@
 // Shared pieces of the deterministic one-GPU word2vec steps (SGNS: ops_sgns_tma.cu, CBOW: ops_cbow.cu) and of their
 // TMA rings: mbarrier and bulk-copy helpers, the fixed-point scales, and the gather and finish passes that apply a step's
 // contributions grouped by key. A step's score pass describes every contribution to a row as GatherDesc{g, vec}: the
-// row gains AdaGrad(g * vecs[vec]) in fixed point against its start-of-step accumulator.
+// row gains AdaGrad(g * vecs[vec]) in fixed point against its start-of-step accumulator. (The SGNS score pass applies a
+// row with a single contribution itself, with the same arithmetic: fx_apply_one.)
 #pragma once
 #include <cuda_runtime.h>
 
@@ -90,12 +91,25 @@ struct alignas(8) GatherDesc {
 };
 
 // The fixed-point terms of one element of one contribution (gr = gs * e0 of a target, g0 of a center; a = the row's
-// AdaGrad value at the start of the step), with the expressions of the in-place step.
+// AdaGrad value at the start of the step), with the expressions of the in-place step. a + gr * gr is rounded twice (no
+// FMA), so that every caller computes the same terms.
 __device__ __forceinline__ void fx_terms(float gr, float a, float alpha, long long& se, long long& sa) {
-  const float ua = gr * gr;
-  const float ue = alpha * gr * rsqrtf(a + ua);
+  const float ua = __fmul_rn(gr, gr);
+  const float ue = alpha * gr * rsqrtf(__fadd_rn(a, ua));
   se += __float2ll_rn(ue * kFxEmb);
   sa += __float2ll_rn(ua * kFxAda);
+}
+// row element r and its AdaGrad value a += their summed terms; a zero sum leaves the element as it is (a -0.0 stays -0.0)
+__device__ __forceinline__ void fx_apply(float& r, float& a, long long se, long long sa) {
+  if (se) r += (float)((double)se * (1.0 / (double)kFxEmb));
+  if (sa) a += (float)((double)sa * (1.0 / (double)kFxAda));
+}
+// An element of a row with one contribution in the step gets exactly what the gather pass would give it: the score
+// pass applies such rows itself.
+__device__ __forceinline__ void fx_apply_one(float& r, float& a, float gr, float alpha) {
+  long long se = 0, sa = 0;
+  fx_terms(gr, a, alpha, se, sa);
+  fx_apply(r, a, se, sa);
 }
 
 // Gather pass: warp w works on CSR positions [w R, (w + 1) R). A key with at most R entries ("light") belongs wholly to
@@ -277,8 +291,6 @@ sgns_det_gather_kernel(const __grid_constant__ Ctx c, float* const* __restrict__
             }
           }
         } else if (row) {
-          // row += sum / scale; a zero sum leaves the element as it is (a -0.0 stays -0.0)
-          const double ie = 1.0 / (double)kFxEmb, ia = 1.0 / (double)kFxAda;
 #pragma unroll
           for (int v = 0; v < VPL; ++v) {
             const int j = lane + v * 32;
@@ -288,10 +300,7 @@ sgns_det_gather_kernel(const __grid_constant__ Ctx c, float* const* __restrict__
               float* rp = &r.x;
               float* ap = &na.x;
 #pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                if (se[v][q]) rp[q] += (float)((double)se[v][q] * ie);
-                if (sa[v][q]) ap[q] += (float)((double)sa[v][q] * ia);
-              }
+              for (int q = 0; q < 4; ++q) fx_apply(rp[q], ap[q], se[v][q], sa[v][q]);
               reinterpret_cast<float4*>(row)[j] = r;
               reinterpret_cast<float4*>(row + d)[j] = na;
             }

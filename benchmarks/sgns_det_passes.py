@@ -50,23 +50,31 @@ def key_counts(batch, negs, B, neg):
     valid = negs != contexts.view(B, 1)
     targets = torch.cat([contexts, negs[valid]])
     allk = torch.cat([centers, targets])
+    keys, n = torch.unique(allk, return_counts=True)
+    single = keys[n == 1]
     return {"pairs": B, "entries": int(B + targets.numel()), "centers": int(torch.unique(centers).numel()),
-            "targets": int(torch.unique(targets).numel()), "keys": int(torch.unique(allk).numel())}
+            "targets": int(torch.unique(targets).numel()), "keys": int(keys.numel()),
+            # keys with one entry in the step, which the score pass applies; those of them that are centers
+            "singletons": int(single.numel()), "singleton_centers": int(torch.isin(centers, single).sum())}
 
 
 def pass_bytes(kc, d, neg):
     """Least HBM traffic of each pass (bytes), from the step's key counts: each distinct row is read once (written once
     where the pass updates it), per-pair and per-entry buffers once each way."""
     P, E, C, U = kc["pairs"], kc["entries"], kc["centers"], kc["keys"]
+    S, SC = kc.get("singletons", 0), kc.get("singleton_centers", 0)
     half, row, key = 4 * d, 8 * d, 8
     slots = P * (neg + 2)
     return {
         # gather-based step
         "index": slots * key + U * (key + 4),
-        "score": U * half + P * half + C * half + slots * 4,                 # rows' embedding halves; g0, snapshot, gs
+        "score": U * half + S * (half + row) + (P - SC) * half + C * half + slots * 4,   # rows' embedding halves;
+                                                                            # one-entry rows: AdaGrad half read, row
+                                                                            # written; g0, snapshot, gs
         "group": 2 * slots * key + 2 * E * 8 + E * 12 + 3 * U * 4,          # keys twice; descriptors + kid, gs + pcid
                                                                             # read for them; counts and scan
-        "gather": 2 * U * row + P * half + C * half + E * 8,                # rows read + written; g0, snapshot; descriptors
+        "gather": 2 * (U - S) * row + (P - SC) * half + C * half + (E - S) * 8,   # the other rows read + written; g0,
+                                                                                  # snapshot; descriptors
         "finish": U * 12,
         # accumulator-based step
         "step": U * row + P * half + 2 * U * 2 * row,                       # rows; 8-byte accumulators read + written
