@@ -278,6 +278,9 @@ void sgns_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const K
   ADAPM_CHECK(be.ctx().L.val_bytes == 4, "the fused ops need float32 rows (Options::dtype)");
   be.track_stream(stream);
   if ((impl == 0 || impl == 2) && sgns_step_tma(be, stream, centers, contexts, negatives, n_pairs, neg, d, alpha, loss_out, stats)) return;
+  // auto falls back to the register kernel (in place, also on one GPU); an explicit tma request does not
+  ADAPM_CHECK(impl != 2, "sgns_step: impl=\"tma\" takes embed_dim <= 336 and negative <= 30, got embed_dim "
+                             << d << ", negative " << neg << " (impl=\"auto\" runs the in-place register kernel)");
   const int vpl = (d / 4 + 31) / 32;
   const int warps_per_block = kThreads / 32;
   int blocks = std::min((n_pairs + warps_per_block - 1) / warps_per_block, be.num_sms() * 8);

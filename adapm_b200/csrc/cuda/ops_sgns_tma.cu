@@ -581,7 +581,8 @@ void sgns_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, con
 
 }  // namespace
 
-// Returns false if this variant does not support the shape (the caller falls back to the LDG kernel).
+// Returns false if this variant does not support the shape: neg + 1 > 31, or d >= 340, where the ring of 5 row buffers
+// per warp no longer fits two blocks per SM. sgns_step then falls back to the LDG kernel (impl auto) or raises (impl tma).
 bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, const Key* negatives,
                    int n_pairs, int neg, int d, float alpha, float* loss_out, unsigned long long* stats) {
   if (neg + 1 > 31 || d % 4 != 0 || d > 384) return false;

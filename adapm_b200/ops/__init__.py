@@ -33,6 +33,11 @@ def sgns_step(server, centers: torch.Tensor, contexts: torch.Tensor, negatives: 
     ``stats``: optional int64[4] accumulated with (local rows, remote rows, slow-path rows, updates).
     ``impl``: ``tma`` (rows prefetched by the TMA engine into a shared-memory ring), ``ldg`` (register
     variant) or ``auto`` (tma when the shape fits, else ldg).
+
+    On one GPU the tma step is deterministic: every pair reads the rows at the start of the step and two runs from
+    the same inputs give bit-identical rows and loss. It takes ``embed_dim <= 336`` (a multiple of 4) and
+    ``neg <= 30``. Outside that window ``auto`` runs the in-place register kernel, whose runs are not reproducible
+    when keys repeat, and ``tma`` raises ``AdapmError``.
     """
     _i64(centers, "centers"); _i64(contexts, "contexts"); _i64(negatives, "negatives")
     B = centers.numel()

@@ -90,3 +90,16 @@ def run_cluster(fn, world, workers, mode="threads", setup_fn=None, timeout=300, 
     errs = [e for (_, _, es) in res for e in es]
     assert not errs, "\n".join(errs)
     return {rank: results for (rank, results, _) in res}
+
+
+# The fused training steps launch min(ceil(n / 8), num_sms * cap) blocks of 8 warps and loop over the n calls with a
+# grid stride (cap: 16 for MF, 8 for ComplEx, 4 for RESCAL, TransE and RotatE). A test that passes n = WRAP runs
+# wrap_calls(WRAP, cap) calls: 2.5 passes of the resident grid, so every warp runs a second call and some a third.
+WRAP = "wrap"
+
+
+def wrap_calls(n, cap):
+    if n != WRAP:
+        return n
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    return 5 * sms * cap * 8 // 2

@@ -12,6 +12,15 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LOGS = os.path.join(ROOT, "build", "adapm_b200")
 
 
+def kernel_name(name):
+    """a kernel's name as the tests use it, e.g. ``transe_step_kernel<3, 1, true>``: demangled (c++filt) if mangled,
+    without the project's namespaces, cut at the argument list"""
+    if name.startswith("_Z"):
+        name = subprocess.run(["c++filt", name], capture_output=True, text=True).stdout.strip()
+    name = name.replace("(anonymous namespace)::", "").replace("adapm::cudaops::", "").replace("adapm::", "")
+    return re.sub(r"^void ", "", name).split("(")[0]
+
+
 def _kernels():
     logs = glob.glob(os.path.join(LOGS, "*.cu.o.log"))
     if not logs:
@@ -25,10 +34,7 @@ def _kernels():
                      r"ptxas info\s*:\s*Used (\d+) registers")
     for f in logs:
         for name, stack, st, ld, regs in pat.findall(open(f).read()):
-            dem = subprocess.run(["c++filt", name], capture_output=True, text=True).stdout.strip()
-            dem = dem.replace("(anonymous namespace)::", "").replace("adapm::cudaops::", "").replace("adapm::", "")
-            dem = re.sub(r"^void ", "", dem).split("(")[0]
-            out[dem] = {"regs": int(regs), "spill": int(st or 0) + int(ld or 0)}
+            out[kernel_name(name)] = {"regs": int(regs), "spill": int(st or 0) + int(ld or 0)}
     return out
 
 

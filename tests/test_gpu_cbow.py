@@ -80,7 +80,9 @@ def _hot_batch(g, vocab, B, C, neg, step):
     return c, x, n
 
 
-SHAPES = [(4, 5), (64, 1), (100, 25), (128, 31), (300, 25), (336, 5), (300, 1), (300, 5), (300, 31)]
+# float4 per lane (VPL) 1 up to d 128, 2 up to 256, 3 up to 336
+SHAPES = [(4, 5), (64, 1), (100, 25), (128, 31), (300, 25), (336, 5), (300, 1), (300, 5), (300, 31), (132, 5),
+          (200, 25), (256, 31)]
 
 
 @gpu
@@ -178,7 +180,7 @@ def _distinct_batch(g, words, B, C, neg, pad=True):
 
 
 @gpu
-@pytest.mark.parametrize("d,neg", [(64, 5), (300, 25), (336, 30), (4, 1)])
+@pytest.mark.parametrize("d,neg", [(64, 5), (300, 25), (336, 30), (4, 1), (132, 5), (256, 30)])
 def test_inplace_kernel_on_one_gpu_matches_rule(d, neg):
     from adapm_b200 import _C
 

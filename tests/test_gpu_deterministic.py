@@ -10,6 +10,8 @@ import numpy as np
 import pytest
 import torch
 
+from harness import WRAP, wrap_calls
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 gpu = pytest.mark.gpu
 
@@ -49,20 +51,26 @@ def _pull(kv, keys, n_vals, dtype=torch.float32):
 
 # ---------------------------------------------------------------------------------------------- start-of-step numerics
 @gpu
-@pytest.mark.parametrize("algo,d,p_e,p_r", [("ComplEx", 512, 0.0, 0.0), ("ComplEx", 128, 0.25, 0.4),
-                                            ("ComplEx", 20, 0.0, 0.0), ("RESCAL", 32, 0.0, 0.0),
-                                            ("RESCAL", 12, 0.0, 0.0), ("RESCAL", 32, 0.3, 0.2),
-                                            ("RESCAL", 12, 0.2, 0.3)])
-def test_kge_steps_with_repeated_keys_match_start_of_step_reference(cluster1, algo, d, p_e, p_r):
+@pytest.mark.parametrize("algo,d,p_e,p_r,n", [pytest.param(*c, 256, id="-".join(map(str, c))) for c in (
+    ("ComplEx", 512, 0.0, 0.0), ("ComplEx", 128, 0.25, 0.4), ("ComplEx", 20, 0.0, 0.0), ("RESCAL", 32, 0.0, 0.0),
+    ("RESCAL", 12, 0.0, 0.0), ("RESCAL", 32, 0.3, 0.2), ("RESCAL", 12, 0.2, 0.3),
+    # ComplEx: generic path with nh = 2 (mod 4) and above 512, two float4 per lane and half with the second one partly
+    # filled; RESCAL: 1, 5 and 32 lanes per matrix row
+    ("ComplEx", 18, 0.0, 0.0), ("ComplEx", 264, 0.0, 0.0), ("ComplEx", 1064, 0.0, 0.0),
+    ("RESCAL", 4, 0.0, 0.0), ("RESCAL", 20, 0.0, 0.0), ("RESCAL", 128, 0.0, 0.0))]
+                         + [pytest.param("ComplEx", 128, 0.0, 0.0, WRAP, id="ComplEx-128-0.0-0.0-wrap"),
+                            pytest.param("RESCAL", 32, 0.0, 0.0, WRAP, id="RESCAL-32-0.0-0.0-wrap")])
+def test_kge_steps_with_repeated_keys_match_start_of_step_reference(cluster1, algo, d, p_e, p_r, n):
     """12 entities and 3 relations over 256 calls: every row is updated by many calls of each step. Over 3 steps the
     deterministic kernels equal the reference rule (all calls read the start-of-step state) evaluated on a float64 CPU
-    store loaded with the GPU's state (an accumulator that is not cleared, or a row applied twice, shows in step 2)."""
+    store loaded with the GPU's state (an accumulator that is not cleared, or a row applied twice, shows in step 2).
+    The cases that wrap the kernel's grid keep about 20 calls per entity and 80 per relation."""
     from adapm_b200.models.kge import KGEConfig, kge_reference_step
     from adapm_b200.ops import kge_complex_step, kge_dropout_mask, kge_rescal_step
 
-    n = 256
-    cfg = KGEConfig(num_entities=12, num_relations=3, embed_dim=d, neg_ratio=1, algorithm=algo, eta=0.05,
-                    dropout_entity=p_e, dropout_relation=p_r)
+    n = wrap_calls(n, 8 if algo == "ComplEx" else 4)
+    cfg = KGEConfig(num_entities=max(12, n // 20), num_relations=max(3, n // 80), embed_dim=d, neg_ratio=1,
+                    algorithm=algo, eta=0.05, dropout_entity=p_e, dropout_relation=p_r)
     server, kv = cluster1(cfg.value_lengths(), cfg.num_keys)
     dev = server.device
     g = torch.Generator().manual_seed(d + int(100 * p_e) + (1000 if algo == "RESCAL" else 0))
@@ -103,20 +111,24 @@ def test_kge_steps_with_repeated_keys_match_start_of_step_reference(cluster1, al
             torch.testing.assert_close(got_r, ref_r, rtol=2e-4, atol=2e-5)
             torch.testing.assert_close(loss.cpu()[0].double(), torch.tensor(ref_loss, dtype=torch.float64), rtol=1e-4, atol=0)
             s = stats.tolist()
-            assert s[1] == 0 and s[2] == (n if algo == "ComplEx" and d % 8 else 0) and s[3] == 3 * n, s
+            generic = algo == "ComplEx" and (d % 8 or d > 512)
+            assert s[1] == 0 and s[2] == (n if generic else 0) and s[3] == 3 * n, s
     finally:
         ref_kv.finalize(); ref_server.shutdown()
 
 
 @gpu
-@pytest.mark.parametrize("rank", [128, 64, 10])
-def test_mf_steps_with_repeated_keys_match_start_of_step_reference(cluster1, rank):
+@pytest.mark.parametrize("rank,n", [pytest.param(r, 512, id=str(r)) for r in (128, 64, 10, 132, 256, 260, 768)]
+                         + [pytest.param(64, WRAP, id="64-wrap")])
+def test_mf_steps_with_repeated_keys_match_start_of_step_reference(cluster1, rank, n):
     """20 rows and 8 columns over 512 non-zeros, 3 steps, against mf_reference_step on a float64 CPU store loaded with
-    the GPU's state at the start of every step (rank 10 runs the generic scalar path)."""
+    the GPU's state at the start of every step (ranks 10, 260 and 768 run the generic scalar path; 132 and 256 two
+    float4 per lane). The case that wraps the kernel's grid keeps about 25 non-zeros per row and 64 per column."""
     from adapm_b200.models.mf import mf_reference_step
     from adapm_b200.ops import mf_step
 
-    n, nr, nc = 512, 20, 8
+    n = wrap_calls(n, 16)
+    nr, nc = max(20, n // 25), max(8, n // 64)
     nk = nr + nc
     server, kv = cluster1(2 * rank, nk)
     dev = server.device
@@ -145,7 +157,7 @@ def test_mf_steps_with_repeated_keys_match_start_of_step_reference(cluster1, ran
             torch.testing.assert_close(got, ref, rtol=2e-4, atol=2e-5)
             torch.testing.assert_close(loss.cpu()[0].double(), torch.tensor(ref_loss, dtype=torch.float64), rtol=1e-4, atol=0)
             s = stats.tolist()
-            assert s[1] == 0 and s[2] == (n if rank % 4 else 0) and s[3] == 2 * n, s
+            assert s[1] == 0 and s[2] == (n if rank % 4 or rank > 256 else 0) and s[3] == 2 * n, s
     finally:
         ref_kv.finalize(); ref_server.shutdown()
 

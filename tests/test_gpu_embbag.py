@@ -67,7 +67,8 @@ MODES = [("sum", False), ("mean", False), ("sum", True)]
 
 
 @gpu
-@pytest.mark.parametrize("dim", [4, 20, 64, 128, 512])
+# float4 per lane (VPL) 1 to 4; dim 4 and 8 give 1 and 2 lanes per bag
+@pytest.mark.parametrize("dim", [4, 20, 64, 128, 512, 8, 132, 256, 260, 384])
 def test_forward_and_step_match_float64_rule(dim):
     from adapm_b200 import _C
     from adapm_b200.ops import StoreEmbeddingBag, embedding_bag_reference

@@ -3,6 +3,8 @@ import numpy as np
 import pytest
 import torch
 
+from harness import WRAP, wrap_calls
+
 pytestmark = pytest.mark.gpu
 
 
@@ -78,7 +80,8 @@ def test_mixed_value_lengths(cluster1):
 
 
 @pytest.mark.parametrize("d,neg,impl", [(300, 25, "tma"), (300, 25, "ldg"), (128, 5, "tma"), (128, 5, "ldg"),
-                                        (64, 40, "auto"), (512, 3, "auto"), (200, 30, "tma"), (16, 2, "tma")])
+                                        (64, 40, "auto"), (512, 3, "auto"), (200, 30, "tma"), (16, 2, "tma"),
+                                        (132, 5, "ldg"), (256, 5, "ldg")])
 def test_sgns_step_matches_pytorch_reference(cluster1, d, neg, impl):
     """Distinct keys per batch -> every row is touched by exactly one pair-target, so the batched kernel and the
     PyTorch fp32 formula must agree (AdaGrad with the pulled accumulator, |f|>6 saturation, negative==target skip)."""
@@ -141,7 +144,7 @@ def test_sgns_step_matches_pytorch_reference(cluster1, d, neg, impl):
     assert s[1] == 0 and s[2] == 0 and s[3] == int(valid.sum()) + B
 
 
-@pytest.mark.parametrize("d,neg", [(300, 25), (128, 5), (64, 2)])
+@pytest.mark.parametrize("d,neg", [(300, 25), (128, 5), (64, 2), (132, 5), (256, 30), (336, 30)])
 def test_sgns_steps_with_repeated_keys_match_start_of_step_reference(cluster1, d, neg):
     """Few distinct keys, so every row is updated by many pairs of a step, over several steps: on one GPU every pair
     reads the state at the start of the step and the step adds all pairs' updates, which the fp64 formula below
@@ -307,15 +310,17 @@ def test_native_step_driver_matches_python_loop(cluster1):
     assert model.stats.tolist()[3] > 0 and kv.current_clock() == 6
 
 
-@pytest.mark.parametrize("nh", [512, 128, 20])
-def test_kge_complex_step_matches_pytorch_reference(cluster1, nh):
+@pytest.mark.parametrize("nh,n", [pytest.param(nh, 48, id=str(nh)) for nh in (512, 128, 20, 18, 264, 1064)]
+                         + [pytest.param(128, WRAP, id="128-wrap")])
+def test_kge_complex_step_matches_pytorch_reference(cluster1, nh, n):
     """Distinct keys per call -> the fused kernel must equal the reference formula evaluated in PyTorch
-    (nh=20 exercises the generic scalar path: 20/8 is not integral)."""
+    (nh=20 and 18 exercise the generic scalar path: nh/8 is not integral; so does nh=1064, more than two float4 per
+    lane and half; at nh=264 one lane holds a second float4 of each half)."""
     from adapm_b200.models.kge import KGEConfig, kge_reference_step
     from adapm_b200.ops import kge_complex_step
     import adapm_b200 as ad
 
-    n = 48
+    n = wrap_calls(n, 8)
     cfg = KGEConfig(num_entities=2 * n + 5, num_relations=n + 3, embed_dim=nh, neg_ratio=1)
     server, kv = cluster1(cfg.value_lengths(), cfg.num_keys)
     dev = server.device
@@ -351,9 +356,12 @@ def test_kge_complex_step_matches_pytorch_reference(cluster1, nh):
     assert stats.tolist()[3] == 3 * n
 
 
-@pytest.mark.parametrize("algo,d,p_e,p_r", [("RESCAL", 32, 0.0, 0.0), ("RESCAL", 64, 0.0, 0.0), ("RESCAL", 12, 0.0, 0.0),
-                                            ("RESCAL", 32, 0.3, 0.2), ("ComplEx", 128, 0.25, 0.4), ("ComplEx", 20, 0.5, 0.0)])
-def test_kge_rescal_and_dropout_match_pytorch_reference(cluster1, algo, d, p_e, p_r):
+@pytest.mark.parametrize("algo,d,p_e,p_r,n", [pytest.param(*c, 40, id="-".join(map(str, c))) for c in (
+    ("RESCAL", 32, 0.0, 0.0), ("RESCAL", 64, 0.0, 0.0), ("RESCAL", 12, 0.0, 0.0), ("RESCAL", 32, 0.3, 0.2),
+    ("ComplEx", 128, 0.25, 0.4), ("ComplEx", 20, 0.5, 0.0),
+    ("RESCAL", 4, 0.0, 0.0), ("RESCAL", 20, 0.0, 0.0), ("RESCAL", 128, 0.0, 0.0))]   # D/4 lanes per matrix row: 1, 5, 32
+                         + [pytest.param("RESCAL", 32, 0.0, 0.0, WRAP, id="RESCAL-32-0.0-0.0-wrap")])
+def test_kge_rescal_and_dropout_match_pytorch_reference(cluster1, algo, d, p_e, p_r, n):
     """The fused RESCAL kernel (s^T R o, rank-1 relation gradient) and the in-kernel dropout of both KGE kernels
     against the reference formula in PyTorch; the dropout mask is a pure function of (seed, call, row, element) that
     ``ops.kge_dropout_mask`` reproduces on the host, so the comparison is exact up to fp32 rounding."""
@@ -361,7 +369,7 @@ def test_kge_rescal_and_dropout_match_pytorch_reference(cluster1, algo, d, p_e, 
     from adapm_b200.ops import kge_complex_step, kge_rescal_step, kge_dropout_mask
     import adapm_b200 as ad
 
-    n = 40
+    n = wrap_calls(n, 8 if algo == "ComplEx" else 4)
     cfg = KGEConfig(num_entities=2 * n + 5, num_relations=n + 3, embed_dim=d, neg_ratio=1, algorithm=algo,
                     dropout_entity=p_e, dropout_relation=p_r)
     server, kv = cluster1(cfg.value_lengths(), cfg.num_keys)
@@ -406,13 +414,17 @@ def test_kge_rescal_and_dropout_match_pytorch_reference(cluster1, algo, d, p_e, 
     assert stats.tolist()[3] == 3 * n
 
 
-@pytest.mark.parametrize("rank", [128, 64, 10])
-def test_mf_step_matches_pytorch_reference(cluster1, rank):
+@pytest.mark.parametrize("rank,n", [pytest.param(r, 64, id=str(r)) for r in (128, 64, 10, 132, 256, 260, 768)]
+                         + [pytest.param(64, WRAP, id="64-wrap")])
+def test_mf_step_matches_pytorch_reference(cluster1, rank, n):
+    """float4 per lane 1 (rank 64, 128) and 2 (132, 256); the generic scalar path for rank % 4 != 0 (10) and for more
+    than two float4 per lane (260, 768, the largest rank the staging buffer takes)."""
     from adapm_b200.models.mf import mf_reference_step
     from adapm_b200.ops import mf_step
     import adapm_b200 as ad
 
-    n, nk = 64, 300
+    n = wrap_calls(n, 16)
+    nk = max(300, 2 * n + 100)
     server, kv = cluster1(2 * rank, nk)
     dev = server.device
     g = torch.Generator().manual_seed(rank)

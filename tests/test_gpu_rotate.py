@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 import torch
 
-from harness import run_cluster
+from harness import WRAP, run_cluster, wrap_calls
 from test_gpu_fused_multirank import WORLD, _idiom, _mover
 from test_gpu_transe import _check_rank, _check_topk, _dist_inputs
 
@@ -40,7 +40,8 @@ def _init_table(ne, nr, d, g):
 
 
 def _batch(ne, nr, B, nn, g, distinct=False, hot=False):
-    """(subj, rel keys, obj, neg [B, nn]); distinct: no key twice in the step; hot: entity 0 is in every triple"""
+    """(subj, rel keys, obj, neg [B, nn]); distinct: no key twice in the step; hot: entity 0 is in each of the first
+    64 triples"""
     if distinct:
         e = torch.randperm(ne, generator=g)[:B * (2 + nn)]
         subj, obj, neg = e[:B], e[B:2 * B], e[2 * B:].view(B, nn)
@@ -50,7 +51,7 @@ def _batch(ne, nr, B, nn, g, distinct=False, hot=False):
         rel = ne + torch.randint(0, nr, (B,), generator=g)
         neg = torch.randint(0, ne, (B, nn), generator=g)
         if hot:
-            subj[::2] = 0; obj[1::2] = 0
+            subj[:64:2] = 0; obj[1:64:2] = 0
             neg[0, 0] = obj[0]                  # a negative equal to the positive's object
             neg[1, nn - 1] = subj[1]            # a negative equal to the positive's subject
     return subj, rel, obj, neg
@@ -101,15 +102,23 @@ def _fused(table, ne, nr, batches, d, gamma, alpha, eta, ge, deterministic):
         s.shutdown()
 
 
-SHAPES = [(8, 12), (152, 256), (512, 64)]     # (d, 2n)
+# (d, 2n): float4 per lane (VPL) 1, 2, 4, 3, 3; 2n = 2 is the fewest negatives the step takes
+SHAPES = [(8, 12), (152, 256), (512, 64), (264, 2), (384, 64)]
+
+
+def _cases(B):
+    """SHAPES with B triples crossed with alpha, and one case whose triples wrap the kernel's resident grid"""
+    return ([pytest.param(d, nn, a, B, id=f"{d}-{nn}-{a}") for a in (0.0, 1.0) for d, nn in SHAPES]
+            + [pytest.param(8, 12, 1.0, WRAP, id="8-12-1.0-wrap")])
 
 
 @gpu
-@pytest.mark.parametrize("alpha", [0.0, 1.0])
-@pytest.mark.parametrize("d,nn", SHAPES)
-def test_deterministic_step_matches_float64_rule(d, nn, alpha):
-    """Repeated keys in every role, one entity in every triple, negatives equal to the positive's rows; two steps."""
-    ne, nr, B = 300, 20, 64
+@pytest.mark.parametrize("d,nn,alpha,B", _cases(64))
+def test_deterministic_step_matches_float64_rule(d, nn, alpha, B):
+    """Repeated keys in every role, one entity in the first 64 triples, negatives equal to the positive's rows; two
+    steps."""
+    B = wrap_calls(B, 4)
+    ne, nr = max(300, 2 * B), max(20, B // 16)
     g = torch.Generator().manual_seed(d * 7 + nn + int(alpha))
     table = _init_table(ne, nr, d, g)
     batches = [_batch(ne, nr, B, nn, g, hot=True) for _ in range(2)]
@@ -125,11 +134,10 @@ def test_deterministic_step_matches_float64_rule(d, nn, alpha):
 
 
 @gpu
-@pytest.mark.parametrize("alpha", [0.0, 1.0])
-@pytest.mark.parametrize("d,nn", SHAPES)
-def test_inplace_step_matches_rule_on_distinct_keys(d, nn, alpha):
-    nr, B = 200, 60
-    ne = B * (2 + nn) + 100
+@pytest.mark.parametrize("d,nn,alpha,B", _cases(60))
+def test_inplace_step_matches_rule_on_distinct_keys(d, nn, alpha, B):
+    B = wrap_calls(B, 4)
+    nr, ne = max(200, B), B * (2 + nn) + 100
     g = torch.Generator().manual_seed(d * 11 + nn + int(alpha))
     table = _init_table(ne, nr, d, g)
     batches = [_batch(ne, nr, B, nn, g, distinct=True) for _ in range(2)]

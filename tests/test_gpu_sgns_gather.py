@@ -99,7 +99,7 @@ def test_keys_that_are_centers_and_targets_in_one_step(cluster1, d, neg):
 
 
 @gpu
-@pytest.mark.parametrize("d", [300, 16])
+@pytest.mark.parametrize("d", [300, 16, 132, 256])
 def test_one_key_with_more_entries_than_many_ranges(cluster1, d):
     """One negative in almost every slot of 512 pairs (about 12 800 contributions to one row, far more than one warp's
     range), another key as the context of every pair, and a few pairs whose context is that hot key."""

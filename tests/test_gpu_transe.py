@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 import torch
 
-from harness import run_cluster
+from harness import WRAP, run_cluster, wrap_calls
 from test_gpu_fused_multirank import WORLD, _idiom, _mover
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -34,7 +34,8 @@ def _init_table(num_keys, d, g):
 
 
 def _batch(ne, nr, B, nn, g, distinct=False, hot=False):
-    """(subj, rel keys, obj, neg [B, nn]); distinct: no key twice in the step; hot: entity 0 is in every triple"""
+    """(subj, rel keys, obj, neg [B, nn]); distinct: no key twice in the step; hot: entity 0 is in each of the first
+    64 triples"""
     if distinct:
         e = torch.randperm(ne, generator=g)[:B * (2 + nn)]
         subj, obj, neg = e[:B], e[B:2 * B], e[2 * B:].view(B, nn)
@@ -44,7 +45,7 @@ def _batch(ne, nr, B, nn, g, distinct=False, hot=False):
         rel = ne + torch.randint(0, nr, (B,), generator=g)
         neg = torch.randint(0, ne, (B, nn), generator=g)
         if hot:
-            subj[::2] = 0; obj[1::2] = 0
+            subj[:64:2] = 0; obj[1:64:2] = 0
             neg[0, 0] = obj[0]                  # a negative equal to the positive's object
     return subj, rel, obj, neg
 
@@ -96,12 +97,19 @@ def _fused(table, batches, d, p, margin, eta, ge, gr, deterministic):
         s.shutdown()
 
 
+def _cases(B, wrap_d, wrap_p):
+    """d 4, 152, 260, 384 and 512 (4 float4 per lane: VPL 1 to 4) with B triples, crossed with p; and one (wrap_d,
+    wrap_p) case whose triples wrap the kernel's resident grid"""
+    return ([pytest.param(d, p, B, id=f"{d}-{p}") for p in (1, 2) for d in (4, 152, 260, 384, 512)]
+            + [pytest.param(wrap_d, wrap_p, WRAP, id=f"{wrap_d}-{wrap_p}-wrap")])
+
+
 @gpu
-@pytest.mark.parametrize("p", [1, 2])
-@pytest.mark.parametrize("d", [4, 152, 512])
-def test_deterministic_step_matches_float64_rule(d, p):
-    """Repeated keys in every role, one entity in every triple, a negative equal to the positive; two steps."""
-    ne, nr, B, nn = 300, 20, 64, 12
+@pytest.mark.parametrize("d,p,B", _cases(64, 64, 1))
+def test_deterministic_step_matches_float64_rule(d, p, B):
+    """Repeated keys in every role, one entity in the first 64 triples, a negative equal to the positive; two steps."""
+    B = wrap_calls(B, 4)
+    ne, nr, nn = max(300, 2 * B), max(20, B // 16), 12
     g = torch.Generator().manual_seed(d * 7 + p)
     table = _init_table(ne + nr, d, g)
     batches = [_batch(ne, nr, B, nn, g, hot=True) for _ in range(2)]
@@ -118,10 +126,10 @@ def test_deterministic_step_matches_float64_rule(d, p):
 
 
 @gpu
-@pytest.mark.parametrize("p", [1, 2])
-@pytest.mark.parametrize("d", [4, 152, 512])
-def test_inplace_step_matches_rule_on_distinct_keys(d, p):
-    ne, nr, B, nn = 4000, 200, 150, 12
+@pytest.mark.parametrize("d,p,B", _cases(150, 64, 2))
+def test_inplace_step_matches_rule_on_distinct_keys(d, p, B):
+    B, nn = wrap_calls(B, 4), 12
+    ne, nr = max(4000, B * (2 + nn)), max(200, B)
     g = torch.Generator().manual_seed(d * 11 + p)
     table = _init_table(ne + nr, d, g)
     batches = [_batch(ne, nr, B, nn, g, distinct=True) for _ in range(2)]
