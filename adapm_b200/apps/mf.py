@@ -2,6 +2,10 @@
 
     python -m adapm_b200.launch -s 2 -m adapm_b200.apps.mf -- --dataset train.mmc --rank 10 --algorithm dsgd --epochs 10
     python -m adapm_b200.apps.mf --synthetic_nnz 2000000 --num_rows 100000 --num_cols 20000 --rank 128
+    python -m adapm_b200.apps.mf --loss bpr --num_negatives 4 --synthetic_nnz 2000000 --num_rows 50000 --rank 64
+
+``--loss bpr``: implicit feedback (every entry is an interaction, its value is ignored), BPR against sampled negative
+items; each epoch reports the BPR loss and, with a test set, Recall@K and NDCG@K of top-K lists without seen items.
 """
 from __future__ import annotations
 
@@ -52,6 +56,10 @@ def main(argv=None) -> int:
     ap.add_argument("--write_generated_factors", default="", help="path prefix to write the initial factors to")
     ap.add_argument("--deterministic", type=int, default=0, choices=[0, 1],
                     help="one GPU: every non-zero of a batch reads the start-of-batch state, bit-identical runs")
+    ap.add_argument("--loss", default="squared", choices=["squared", "bpr"],
+                    help="squared: explicit ratings; bpr: implicit feedback (every entry is an interaction, values ignored)")
+    ap.add_argument("--num_negatives", type=int, default=1, help="bpr: sampled negative items per interaction")
+    ap.add_argument("--eval_k", type=int, default=10, help="bpr: length of the recommendation lists for recall / ndcg")
     add_ablation_options(ap)
     add_system_options(ap)
     args = ap.parse_args(strip_dashes(argv if argv is not None else sys.argv[1:]))
@@ -59,6 +67,9 @@ def main(argv=None) -> int:
     if args.deterministic and world > 1:
         ap.error("--deterministic 1 needs a single GPU (WORLD_SIZE=1): on several GPUs rows move between ranks during a step")
     rank = int(__import__("os").environ.get("RANK", "0"))
+    bpr = args.loss == "bpr"
+    if bpr and args.num_negatives < 1:
+        ap.error("--num_negatives must be >= 1")
     test = None
     if args.dataset:
         i, j, x, m, n = read_matrix_market_coo(args.dataset)
@@ -71,7 +82,14 @@ def main(argv=None) -> int:
             ti, tj, tx, _, _ = read_matrix_market_coo(tpath)
             if args.enforce_random_keys:
                 ti, tj = fr[ti], fc[tj]
-            test = (ti[rank::world], tj[rank::world], tx[rank::world])
+            # bpr: every rank ranks the items of its own row block, so it keeps the whole test set
+            test = (ti, tj) if bpr else (ti[rank::world], tj[rank::world], tx[rank::world])
+    elif bpr:
+        m, n = args.num_rows, args.num_cols
+        data, test = SparseMatrix.synthetic_implicit(m, n, max(1, (args.synthetic_nnz or 200000) // m), 8, world, rank,
+                                                     seed=args.model_seed)
+        if not args.compute_loss:
+            test = None
     else:
         m, n = args.num_rows, args.num_cols
         data = SparseMatrix.synthetic(m, n, args.synthetic_nnz or 200000, 8, world, rank, seed=args.model_seed)
@@ -79,7 +97,9 @@ def main(argv=None) -> int:
                    batch_nnz=args.batch_nnz, signal_intent_cols=args.signal_intent_cols, bold_driver=bool(args.bold_driver),
                    model_seed=args.model_seed, eps_inc=args.increase_step_factor, eps_dec=args.decrease_step_factor,
                    signal_intent_rows=bool(args.signal_intent_rows), wor_blocks=bool(args.wor_blocks),
-                   wor_points=bool(args.wor_points), early_stop=args.early_stop, deterministic=bool(args.deterministic))
+                   wor_points=bool(args.wor_points), early_stop=args.early_stop, deterministic=bool(args.deterministic),
+                   loss=args.loss, num_negatives=args.num_negatives,
+                   sampling_scheme=getattr(args, "sampling.scheme") or "local")
     ad.setup(cfg.num_keys(world), 1)   # one worker per rank: the per-thread loops of the reference are batched kernels here
     server = ad.Server(cfg.row_len, backend=args.backend, options=system_options(args),
                        dtype={"float": "float32", "double": "float64"}[args.value_type])
@@ -102,7 +122,16 @@ def main(argv=None) -> int:
         kv.barrier()
         model.bold_driver(loss, prev)
         prev = loss
-        if args.compute_loss:
+        if args.compute_loss and bpr:
+            msg = f"[mf] epoch {epoch}: local BPR loss {loss:.6g}, eps {model.eps:.4g}"
+            if test is not None:
+                kv.wait_sync()
+                tr = server.allreduce_sum([float(v) for v in model.evaluate_ranking(*test, k=args.eval_k)])
+                users = max(1.0, float(tr[2]))
+                msg += f", test recall@{args.eval_k} {tr[0] / users:.4f}, ndcg@{args.eval_k} {tr[1] / users:.4f}"
+            if server.my_rank() == 0:
+                print(msg + f" ({time.time() - t0:.1f}s)", flush=True)
+        elif args.compute_loss:
             msg = f"[mf] epoch {epoch}: local squared error {loss:.6g}, eps {model.eps:.4g}"
             if test is not None:
                 kv.wait_sync()

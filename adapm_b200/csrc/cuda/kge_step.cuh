@@ -1,5 +1,6 @@
-// Device helpers of the warp-per-triple KGE steps (ops_transe.cu, ops_rotate.cu): float4 arithmetic, row loads into a
-// lane's float4 registers and the three-mode AdaGrad push (in place, onto a staged copy, into a fixed-point region).
+// Device helpers of the warp-per-triple KGE steps (ops_transe.cu, ops_rotate.cu) and the BPR step of matrix
+// factorisation (ops_bpr.cu): float4 arithmetic, row loads into a lane's float4 registers and the three-mode AdaGrad push
+// (in place, onto a staged copy, into a fixed-point region).
 #pragma once
 #include <cuda_runtime.h>
 

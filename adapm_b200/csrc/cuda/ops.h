@@ -84,6 +84,15 @@ void mf_step(CudaBackend& be, cudaStream_t stream, const Key* row_keys, const Ke
              const int* row_nnz, const int* col_nnz, int n, int rank, float eps, float lambda, float* loss_out,
              unsigned long long* stats, bool deterministic = false);
 
+// implicit-feedback matrix factorisation: fused pull + BPR loss over sampled negatives + L2 + AdaGrad + push
+// (ops_bpr.cu). One positive (users[i], pos[i]) per i with neg[i * n_neg .. (i + 1) * n_neg) item keys; rows
+// [factors (rank) | AdaGrad (rank)], rank % 4 == 0, 4 <= rank <= 512, 1 <= n_neg <= 256. stats[3] counts the pushes
+// issued (2 + n_neg per positive).
+constexpr int kBprMaxRank = 512;
+constexpr int kBprMaxNeg = 256;
+void mf_bpr_step(CudaBackend& be, cudaStream_t stream, const Key* users, const Key* pos, const Key* neg, int B, int n_neg,
+                 int rank, float eps, float lam, float* loss_out, unsigned long long* stats, bool deterministic = false);
+
 // wgmma/TMA GEMM: C[M,N] fp32 = A[M,K] bf16 x B[N,K]^T bf16 (ops_gemm_wgmma.cu)
 void gemm_nt_bf16(cudaStream_t stream, const void* A, const void* B, int M, int N, int K, float* C, int ldc);
 void gemm_nt_e4m3(cudaStream_t stream, const void* A, const void* B, int M, int N, int K, float* C, int ldc, float alpha);

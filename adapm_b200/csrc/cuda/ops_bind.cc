@@ -128,6 +128,13 @@ void bind(py::module_& m) {
                     ptr<const Key>(neg), B, n_neg, d, margin, alpha, eta, gamma_e, ptr<float>(loss),
                     ptr<unsigned long long>(stats), deterministic);
   });
+  m.attr("bpr_max_rank") = kBprMaxRank;
+  m.attr("bpr_max_neg") = kBprMaxNeg;
+  m.def("mf_bpr_step", [](uintptr_t be, uintptr_t stream, uintptr_t users, uintptr_t pos, uintptr_t neg, int B, int n_neg,
+                          int rank, float eps, float lam, uintptr_t loss, uintptr_t stats, bool deterministic) {
+    mf_bpr_step(backend_of(be), (cudaStream_t)stream, ptr<const Key>(users), ptr<const Key>(pos), ptr<const Key>(neg), B,
+                n_neg, rank, eps, lam, ptr<float>(loss), ptr<unsigned long long>(stats), deterministic);
+  });
   m.def("dist_num_slices", [](uintptr_t be, int M, int N, int max_tiles_per_cta) {
     return dist_num_slices(backend_of(be), M, N, max_tiles_per_cta);
   });

@@ -14,6 +14,11 @@ Behavioural parity with the reference application ``apps/matrix_factorization.cc
   (apps/mf/io.h:265-352).
 
 The per-non-zero loop of the reference is one fused kernel over a batch of non-zeros (``ops.mf_step``).
+
+Implicit feedback (``MFConfig.loss = "bpr"``, an addition of this implementation): every entry is an interaction, trained
+with the BPR pairwise loss against sampled negative items in one fused kernel (``ops.mf_bpr_step``) on the same rows and
+schedules; ``recommend`` ranks the items of a user with the seen ones left out, ``evaluate_ranking`` gives Recall@k and
+NDCG@k.
 """
 from __future__ import annotations
 
@@ -47,6 +52,9 @@ class MFConfig:
     early_stop: int = 0              # stop an epoch after N data points (debugging)
     deterministic: bool = False      # one GPU: start-of-step reads, bit-identical runs (ops.mf_step); the CPU backend
                                      # accepts it and already follows the start-of-step rule
+    loss: str = "squared"            # squared (explicit ratings) | bpr (implicit feedback: every entry is an interaction)
+    num_negatives: int = 1           # bpr: sampled negative items per positive
+    sampling_scheme: str = "local"   # bpr on several ranks outside dsgd: "local" draws only resident items
 
     def first_col_key(self, num_workers: int) -> int:
         return ((self.num_rows + num_workers - 1) // num_workers) * num_workers
@@ -86,9 +94,61 @@ class SparseMatrix:
         x = (w[i % w.shape[0]] * h[j % h.shape[0]]).sum(1) / np.sqrt(rank_true) + 0.01 * rng.standard_normal(nnz)
         return SparseMatrix(i, j, x.astype(np.float32), num_rows, num_cols, world, rank)
 
+    @staticmethod
+    def synthetic_implicit(num_rows: int, num_cols: int, per_row: int, rank_true: int, world: int, rank: int,
+                           seed: int = 0, holdout: float = 0.2):
+        """Implicit feedback with planted structure: user u draws ``per_row`` distinct items with probability
+        proportional to ``exp(<p_u, q_i> / tau + b_i)``, p and q standard normal of dimension ``rank_true`` and
+        ``b_i = -0.7 log(1 + pi(i))`` a heavy-tailed popularity over a random item order pi. A ``holdout`` fraction of
+        each user's items (at least one when holdout > 0) goes to the test set. Returns ``(train SparseMatrix, (test_i,
+        test_j))``; the test set holds every user's items, on every rank."""
+        per_row = int(min(per_row, num_cols))
+        rng = np.random.default_rng(seed)
+        tau = 0.5 * np.sqrt(rank_true)
+        P = rng.standard_normal((num_rows, rank_true))
+        Q = rng.standard_normal((num_cols, rank_true))
+        b = -0.7 * np.log1p(rng.permutation(num_cols).astype(np.float64))
+        n_test = 0 if holdout <= 0 else max(1, int(round(per_row * holdout)))
+        n_test = min(n_test, per_row - 1)
+        tr_i, tr_j, te_i, te_j = [], [], [], []
+        for s in range(0, num_rows, 1024):
+            logits = P[s:s + 1024] @ Q.T / tau + b
+            gumbel = -np.log(-np.log(rng.random(logits.shape)))
+            items = np.argpartition(-(logits + gumbel), per_row - 1, axis=1)[:, :per_row]   # a random draw order
+            items = np.take_along_axis(items, rng.random(items.shape).argsort(1), 1)
+            users = np.repeat(np.arange(s, s + items.shape[0]), per_row).reshape(items.shape)
+            tr_i.append(users[:, n_test:].ravel()); tr_j.append(items[:, n_test:].ravel())
+            te_i.append(users[:, :n_test].ravel()); te_j.append(items[:, :n_test].ravel())
+        i, j = np.concatenate(tr_i), np.concatenate(tr_j)
+        train = SparseMatrix(i, j, np.ones(i.shape[0], np.float32), num_rows, num_cols, world, rank)
+        return train, (np.concatenate(te_i), np.concatenate(te_j))
+
     def block(self, b: int):
         s, e = self.block_start[b], self.block_end[b]
         return self.i[s:e], self.j[s:e], self.x[s:e]
+
+    def row_block(self):
+        """[lo, hi): the rows of this rank's block"""
+        lo = self.rank * self.rows_per_block
+        return lo, min(self.num_rows, lo + self.rows_per_block)
+
+    def seen(self, rows):
+        """Training items of ``rows`` (all in this rank's row block, else ``ValueError``) as a CSR ``(offsets int64
+        [n + 1], items int64)`` with each row's items distinct and ascending: the ``exclude`` of a recommendation."""
+        rows = np.asarray(rows, dtype=np.int64).reshape(-1)
+        lo, hi = self.row_block()
+        if rows.size and (rows.min() < lo or rows.max() >= hi):
+            raise ValueError(f"rows must lie in this rank's row block [{lo}, {hi})")
+        if not hasattr(self, "_seen"):
+            pairs = np.unique((self.i.astype(np.int64) - lo) * self.num_cols + self.j)
+            start = np.searchsorted(pairs, np.arange(hi - lo + 1, dtype=np.int64) * self.num_cols)
+            self._seen = (start, pairs % self.num_cols)
+        start, items = self._seen
+        a, e = start[rows - lo], start[rows - lo + 1]
+        off = np.zeros(rows.size + 1, dtype=np.int64)
+        np.cumsum(e - a, out=off[1:])
+        idx = np.repeat(a - off[:-1], e - a) + np.arange(off[-1])
+        return torch.from_numpy(off), torch.from_numpy(items[idx].astype(np.int64))
 
 
 from ..parallel.schedules import column_intent_plan, wor_block_schedule  # noqa: E402,F401  (re-exported: tests, docs)
@@ -106,6 +166,13 @@ class MatrixFactorization:
         self.eps = cfg.eps
         self.step_no = 0
         dev = server.device
+        if cfg.loss not in ("squared", "bpr"):
+            raise ValueError(f"loss must be 'squared' or 'bpr', got {cfg.loss!r}")
+        if cfg.loss == "bpr" and cfg.num_negatives < 1:
+            raise ValueError(f"num_negatives must be >= 1, got {cfg.num_negatives}")
+        self._neg_range = (0, cfg.num_cols)          # bpr: the items negatives are drawn from (set per sub-epoch)
+        self._samplers = {}
+        self._gen = torch.Generator().manual_seed(cfg.model_seed * 3 + server.my_rank())
         if self.cuda:
             self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
             self.stats = torch.zeros(4, dtype=torch.int64, device=dev)
@@ -142,6 +209,8 @@ class MatrixFactorization:
     # one batch of non-zeros (numpy views of this rank's data)
     def step(self, i: np.ndarray, j: np.ndarray, x: np.ndarray) -> torch.Tensor:
         cfg = self.cfg
+        if cfg.loss == "bpr":
+            return self.bpr_step(i, j)
         rn = self.data.row_nnz_all[i]
         cn = self.data.col_nnz_all[j]
         if self.cuda:
@@ -161,6 +230,38 @@ class MatrixFactorization:
         self.step_no += 1
         return torch.tensor([loss], dtype=torch.float32)
 
+    def bpr_step(self, i: np.ndarray, j: np.ndarray) -> torch.Tensor:
+        """One batch of positives (user i[b], item j[b]) with ``num_negatives`` items each, drawn uniformly from the
+        current negative range: the sub-epoch's column block under dsgd, all items otherwise (on several ranks with the
+        ``local`` scheme only items resident on this GPU)."""
+        cfg = self.cfg
+        lo, num = self._neg_range
+        B, n = i.shape[0], cfg.num_negatives
+        if self.cuda:
+            from ..ops import DeviceSampler, mf_bpr_step
+
+            dev = self.server.device
+            smp = self._samplers.get((lo, num))
+            if smp is None:
+                smp = self._samplers[(lo, num)] = DeviceSampler(self.server, distribution="uniform",
+                                                                first_key=self.fck + lo, num_keys=num)
+            local_only = cfg.algorithm != "dsgd" and cfg.sampling_scheme == "local" and self.world > 1
+            seed = (cfg.model_seed * 7 + self.server.my_rank() * 7919 + self.step_no) & 0xFFFFFFFFFFFF
+            neg = smp.sample(B * n, seed, local_only=local_only).view(B, n)
+            uk = torch.from_numpy(np.ascontiguousarray(i, dtype=np.int64)).to(dev, non_blocking=True)
+            ik = (torch.from_numpy(np.ascontiguousarray(j, dtype=np.int64)) + self.fck).to(dev, non_blocking=True)
+            mf_bpr_step(self.server, uk, ik, neg, cfg.rank, self.eps, cfg.lam, self.loss, self.stats,
+                        deterministic=cfg.deterministic)
+            self.step_no += 1
+            return self.loss
+        from ..ops import bpr_reference_step
+
+        neg = torch.randint(lo, lo + num, (B, n), generator=self._gen) + self.fck
+        loss, _ = bpr_reference_step(self.worker, torch.from_numpy(i.astype(np.int64)),
+                                     torch.from_numpy(j.astype(np.int64)) + self.fck, neg, cfg.rank, self.eps, cfg.lam)
+        self.step_no += 1
+        return torch.tensor([loss], dtype=torch.float32)
+
     def run_epoch(self, epoch: int) -> float:
         """One epoch with the configured schedule. Returns this rank's summed squared error."""
         cfg, kv, data, W = self.cfg, self.worker, self.data, self.world
@@ -172,6 +273,8 @@ class MatrixFactorization:
                      else np.array([[(r + se) % W for r in range(W)] for se in range(W)]))
             for se in range(W):
                 b = int(sched[se, self.server.my_rank()])
+                blo = b * data.cols_per_block
+                self._neg_range = (blo, max(0, min(cfg.num_cols, blo + data.cols_per_block) - blo))
                 if cfg.signal_intent_cols != 0 and W > 1:
                     lo = b * data.cols_per_block
                     hi = min(cfg.num_cols, lo + data.cols_per_block)
@@ -190,6 +293,7 @@ class MatrixFactorization:
                 kv.advance_clock()
                 kv.barrier()
         else:
+            self._neg_range = (0, cfg.num_cols)
             n = data.i.shape[0]
             if cfg.algorithm == "columnwise":
                 order = np.argsort(data.j, kind="stable")
@@ -264,6 +368,85 @@ class MatrixFactorization:
             pred = (wv.view(-1, 2 * cfg.rank)[:, :cfg.rank] * hv.view(-1, 2 * cfg.rank)[:, :cfg.rank]).sum(1)
             total += float(((torch.from_numpy(np.ascontiguousarray(x[s:s + (1 << 16)])).to(self.dtype) - pred) ** 2).sum())
         return total
+
+    def recommend(self, rows, k: int = 10, seen=None):
+        """The ``k`` items of highest score ``<w_u, h_i>`` for each user in ``rows``. Returns ``(item ids int64 [n, k],
+        scores float32 [n, k])``, best first; equal scores go to the smaller item id. ``seen``: a CSR ``(offsets int64
+        [n + 1], items int64)`` with each row's items ascending (e.g. ``data.seen(rows)``); those items are left out. A
+        row with fewer than ``k`` items left is padded with ``(-1, -inf)``. ``1 <= k <= 64``.
+
+        CUDA backend (float32 rows): only the users' rows are pulled; the scores against all items are computed from
+        bf16-rounded operands in the fused gather + top-k kernel (``ops.gather_gemm_topk``), which reads the item rows
+        wherever they live; this needs ``rank % 4 == 0`` (``ValueError`` otherwise). CPU route: fp32 PyTorch over the
+        pulled item factors with the same order (``ops.topk_reference``)."""
+        from ..ops import _check_topk, gather_gemm_topk, topk_reference
+
+        cfg, kv = self.cfg, self.worker
+        users = torch.as_tensor(np.asarray(rows), dtype=torch.int64).reshape(-1)
+        n, N = users.numel(), cfg.num_cols
+        if seen is not None:
+            seen = (torch.as_tensor(seen[0], dtype=torch.int64), torch.as_tensor(seen[1], dtype=torch.int64))
+        _check_topk(n, N, k, seen, None)
+        if self.cuda:
+            if cfg.rank % 4:
+                raise ValueError(f"recommend on the GPU needs rank % 4 == 0, got rank {cfg.rank}")
+            dev = self.server.device
+            buf = torch.empty(n * 2 * cfg.rank, dtype=torch.float32, device=dev)
+            if n:
+                kv.wait(kv.pull(self.row_key(users).to(dev), buf, True))
+            if not hasattr(self, "_item_keys"):
+                self._item_keys = torch.arange(N, dtype=torch.int64, device=dev) + self.fck
+            excl = (seen[0].to(dev), seen[1].to(dev)) if seen is not None else None
+            vals, idx = gather_gemm_topk(self.server, buf.view(n, 2 * cfg.rank)[:, :cfg.rank], self._item_keys,
+                                         cfg.rank, k, exclude=excl)
+            return idx, vals
+        wv = torch.empty(n * 2 * cfg.rank, dtype=self.dtype)
+        if n:
+            kv.wait(kv.pull(self.row_key(users), wv))
+        hv = torch.empty(N * 2 * cfg.rank, dtype=self.dtype)
+        kv.wait(kv.pull(torch.arange(N, dtype=torch.int64) + self.fck, hv))
+        q = wv.view(n, 2 * cfg.rank)[:, :cfg.rank].float()
+        E = hv.view(N, 2 * cfg.rank)[:, :cfg.rank].float()
+        excluded = None
+        if seen is not None:
+            off, cols = seen
+            excluded = torch.zeros(n, N, dtype=torch.bool)
+            excluded[torch.repeat_interleave(torch.arange(n), off[1:] - off[:-1]), cols] = True
+        vals, idx = topk_reference(q @ E.t(), int(k), excluded)
+        return idx, vals
+
+    def evaluate_ranking(self, test_i: np.ndarray, test_j: np.ndarray, k: int = 10, batch: int = 2048):
+        """Recall@k and NDCG@k of the top-k lists of this rank's users with held-out items (the test pairs of users in
+        this rank's row block; the rest are ignored). T_u: the held-out items of u that are not training items; L_u: u's
+        top-k list with the training items left out. ``Recall@k = |L_u & T_u| / min(k, |T_u|)``, ``NDCG@k = sum over
+        positions r of L_u with an item in T_u of 1 / log2(r + 2)``, divided by the same sum over ``r < min(k, |T_u|)``.
+        Users with empty T_u are skipped. Returns ``(sum of recall, sum of ndcg, users)``: sums over ranks give the
+        means (``server.allreduce_sum``)."""
+        data = self.data
+        lo, hi = data.row_block()
+        ti, tj = np.asarray(test_i, dtype=np.int64), np.asarray(test_j, dtype=np.int64)
+        mine = (ti >= lo) & (ti < hi)
+        ti, tj = ti[mine], tj[mine]
+        pairs = np.unique(ti * data.num_cols + tj)
+        trained = np.unique((data.i.astype(np.int64)) * data.num_cols + data.j)
+        pairs = pairs[~np.isin(pairs, trained, assume_unique=True)]
+        ti, tj = pairs // data.num_cols, pairs % data.num_cols
+        users, start = np.unique(ti, return_index=True)
+        end = np.append(start[1:], ti.shape[0])
+        disc = 1.0 / np.log2(np.arange(k) + 2.0)
+        idcg = np.cumsum(disc)
+        rec_sum, ndcg_sum = 0.0, 0.0
+        for s in range(0, users.shape[0], batch):
+            u = users[s:s + batch]
+            idx, _ = self.recommend(u, k, seen=data.seen(u))
+            idx = idx.cpu().numpy()
+            for r in range(u.shape[0]):
+                T = tj[start[s + r]:end[s + r]]
+                hit = np.isin(idx[r], T)
+                m = min(k, T.shape[0])
+                rec_sum += hit.sum() / m
+                ndcg_sum += float((disc * hit).sum()) / idcg[m - 1]
+        return rec_sum, ndcg_sum, int(users.shape[0])
 
     def bold_driver(self, loss: float, prev_loss: Optional[float]) -> None:
         if not self.cfg.bold_driver or prev_loss is None:

@@ -686,6 +686,88 @@ def mf_step(server, row_keys: torch.Tensor, col_keys: torch.Tensor, x: torch.Ten
                stats.data_ptr() if stats is not None else 0, det)
 
 
+BPR_MAX_RANK = 512
+BPR_MAX_NEG = 256
+
+
+def _check_bpr_shape(rank: int, neg: torch.Tensor, B: int) -> None:
+    if isinstance(rank, bool) or int(rank) != rank or not (4 <= int(rank) <= BPR_MAX_RANK and int(rank) % 4 == 0):
+        raise ValueError(f"rank must be a multiple of 4 in [4, {BPR_MAX_RANK}], got {rank}")
+    if neg.dim() != 2 or neg.shape[0] != B or not 1 <= neg.shape[1] <= BPR_MAX_NEG:
+        raise ValueError(f"neg must be [B = {B}, n] with 1 <= n <= {BPR_MAX_NEG}, got {tuple(neg.shape)}")
+
+
+def mf_bpr_step(server, users: torch.Tensor, pos: torch.Tensor, neg: torch.Tensor, rank: int, eps: float, lam: float,
+                loss: torch.Tensor, stats: Optional[torch.Tensor] = None, deterministic: bool = False) -> None:
+    """Fused BPR step of implicit-feedback matrix factorisation (csrc/cuda/ops_bpr.cu) on ``server``'s store: one warp
+    per positive ``(users[b], pos[b])`` (store keys of a user row and an item row) with the item keys ``neg[b]``
+    (int64 [B, n], 1 <= n <= 256, used as given: repeats and a negative equal to the positive included). Rows are the
+    squared-loss layout ``[factors (rank) | AdaGrad (rank)]``, ``rank`` a multiple of 4 in [4, 512]. The rule is
+    :func:`bpr_reference_step`'s: loss ``sum_j softplus(-x_j)`` with ``x_j = <w_u, h_i> - <w_u, h_j>``, one AdaGrad push
+    per user, positive item and negative occurrence (``2 + n`` per positive). ``loss``: float32[1], accumulated (+=);
+    ``stats``: optional int64[4] accumulated with (local rows, peer rows, slow-path rows, pushes issued).
+
+    ``deterministic=True`` (single-GPU servers only): start-of-step reads, fixed-point sums, bit-identical runs (three
+    launches instead of one); the AdaGrad increment of one push is clamped to 2^24 there (see ops_bpr.cu)."""
+    _i64(users, "users"); _i64(pos, "pos"); _i64(neg, "neg"); _f32(loss, "loss")
+    B = users.numel()
+    if pos.numel() != B:
+        raise ValueError("users and pos must have the same length")
+    _check_bpr_shape(rank, neg, B)
+    if stats is not None and not (stats.is_cuda and stats.dtype == torch.int64 and stats.numel() >= 4):
+        raise TypeError("stats must be a CUDA int64 tensor with 4 entries")
+    det = _check_deterministic(server, deterministic)
+    _C.mf_bpr_step(server._impl.backend_handle(), _stream(users), users.data_ptr(), pos.data_ptr(), neg.data_ptr(), B,
+                   int(neg.shape[1]), int(rank), float(eps), float(lam), loss.data_ptr(),
+                   stats.data_ptr() if stats is not None else 0, det)
+
+
+def bpr_reference_step(kv, users: torch.Tensor, pos: torch.Tensor, neg: torch.Tensor, rank: int, eps: float, lam: float):
+    """The BPR rule of :func:`mf_bpr_step` in float64 through Pull / Push (CPU servers, float64 rows, and the oracle of
+    the tests). Every row is read at the start of the step. Returns ``(loss, pushes)``.
+
+    Per positive (u, i) with negatives j: ``x_j = <w_u, h_i> - <w_u, h_j>``, ``c_j = sigmoid(-x_j)``, ``C = sum_j c_j``,
+    ``S = sum_j c_j h_j``; gradients ``g_u = S - C h_i + lam w_u``, ``g_i = -C w_u + lam h_i``, ``g_j = c_j w_u +
+    lam h_j``; pushes ``[-eps g / sqrt(acc + g^2) | g^2]`` (0 where g == 0) with the pulled accumulator: u and i once per
+    positive, every negative once per occurrence. The loss is ``sum softplus(-x_j)`` (no L2 term)."""
+    users, pos = users.reshape(-1).cpu(), pos.reshape(-1).cpu()
+    neg = neg.cpu()
+    B = users.numel()
+    if neg.dim() != 2 or neg.shape[0] != B or neg.shape[1] < 1:
+        raise ValueError(f"neg must be [B = {B}, n] with n >= 1, got {tuple(neg.shape)}")
+    n, r = neg.shape[1], int(rank)
+    f64 = torch.float64
+
+    def pull(keys):
+        v = torch.empty(keys.numel() * 2 * r, dtype=kv.server.dtype)
+        if keys.numel():
+            kv.wait(kv.pull(keys.contiguous(), v))
+        v = v.view(-1, 2 * r).to(f64)
+        return v[:, :r], v[:, r:]
+
+    W, Aw = pull(users)
+    H, Ah = pull(pos)
+    Hn, An = pull(neg.reshape(-1))
+    Hn = Hn.view(B, n, r)
+    x = (W * H).sum(-1, keepdim=True) - torch.einsum("br,bnr->bn", W, Hn)
+    loss = float(torch.nn.functional.softplus(-x).sum())
+    c = torch.sigmoid(-x)
+    C = c.sum(1, keepdim=True)
+    gu = torch.einsum("bn,bnr->br", c, Hn) - C * H + lam * W
+    gi = -C * W + lam * H
+    gn = c.unsqueeze(-1) * W.unsqueeze(1) + lam * Hn
+
+    def upd(g, a):
+        ue = torch.where(g != 0, -eps * g / torch.sqrt(a + g * g), torch.zeros_like(g))
+        return torch.cat([ue, g * g], -1).to(kv.server.dtype).contiguous().view(-1)
+
+    if B:
+        kv.wait(kv.push(users.contiguous(), upd(gu, Aw)))
+        kv.wait(kv.push(pos.contiguous(), upd(gi, Ah)))
+        kv.wait(kv.push(neg.reshape(-1).contiguous(), upd(gn.reshape(-1, r), An)))
+    return loss, B * (2 + n)
+
+
 def _bf16_k8(t: torch.Tensor) -> torch.Tensor:
     """contiguous bf16 copy whose K (last dim) is padded to a multiple of 8 (16-byte TMA row pitch)."""
     t = t.to(torch.bfloat16)
