@@ -6,6 +6,12 @@
 
 ``--loss bpr``: implicit feedback (every entry is an interaction, its value is ignored), BPR against sampled negative
 items; each epoch reports the BPR loss and, with a test set, Recall@K and NDCG@K of top-K lists without seen items.
+
+``--algorithm als``: alternating least squares, no step size; each epoch reports the objective (summed over ranks) and,
+with a test set, the test rmse (``--loss squared``) or Recall@K and NDCG@K (``--loss implicit``: the weighted loss of
+Hu, Koren and Volinsky over all pairs, confidence ``1 + alpha x``).
+
+    python -m adapm_b200.apps.mf --algorithm als --loss implicit --alpha 4 --synthetic_nnz 2000000 --num_rows 50000
 """
 from __future__ import annotations
 
@@ -33,7 +39,7 @@ def main(argv=None) -> int:
     ap.add_argument("--rank", "-r", type=int, default=10)
     ap.add_argument("--epochs", type=int, default=10)
     ap.add_argument("--num_threads", "-t", type=int, default=1)
-    ap.add_argument("--algorithm", default="dsgd", choices=["dsgd", "columnwise", "plain"])
+    ap.add_argument("--algorithm", default="dsgd", choices=["dsgd", "columnwise", "plain", "als"])
     ap.add_argument("--eps", type=float, default=0.01)
     ap.add_argument("--lambda", dest="lam", type=float, default=0.05)
     ap.add_argument("--signal_intent_cols", type=int, default=1000)
@@ -56,10 +62,13 @@ def main(argv=None) -> int:
     ap.add_argument("--write_generated_factors", default="", help="path prefix to write the initial factors to")
     ap.add_argument("--deterministic", type=int, default=0, choices=[0, 1],
                     help="one GPU: every non-zero of a batch reads the start-of-batch state, bit-identical runs")
-    ap.add_argument("--loss", default="squared", choices=["squared", "bpr"],
-                    help="squared: explicit ratings; bpr: implicit feedback (every entry is an interaction, values ignored)")
+    ap.add_argument("--loss", default="squared", choices=["squared", "bpr", "implicit"],
+                    help="squared: explicit ratings; bpr: implicit feedback (every entry is an interaction, values ignored); "
+                         "implicit: als on implicit feedback (values are interaction strengths)")
     ap.add_argument("--num_negatives", type=int, default=1, help="bpr: sampled negative items per interaction")
-    ap.add_argument("--eval_k", type=int, default=10, help="bpr: length of the recommendation lists for recall / ndcg")
+    ap.add_argument("--eval_k", type=int, default=10,
+                    help="bpr, implicit: length of the recommendation lists for recall / ndcg")
+    ap.add_argument("--alpha", type=float, default=1.0, help="implicit: confidence 1 + alpha x of an entry with value x")
     add_ablation_options(ap)
     add_system_options(ap)
     args = ap.parse_args(strip_dashes(argv if argv is not None else sys.argv[1:]))
@@ -70,6 +79,12 @@ def main(argv=None) -> int:
     bpr = args.loss == "bpr"
     if bpr and args.num_negatives < 1:
         ap.error("--num_negatives must be >= 1")
+    als = args.algorithm == "als"
+    if als and bpr:
+        ap.error("--algorithm als takes --loss squared or implicit")
+    if args.loss == "implicit" and not als:
+        ap.error("--loss implicit needs --algorithm als")
+    ranking = bpr or args.loss == "implicit"       # implicit feedback: evaluated by recall / ndcg of top-K lists
     test = None
     if args.dataset:
         i, j, x, m, n = read_matrix_market_coo(args.dataset)
@@ -82,9 +97,9 @@ def main(argv=None) -> int:
             ti, tj, tx, _, _ = read_matrix_market_coo(tpath)
             if args.enforce_random_keys:
                 ti, tj = fr[ti], fc[tj]
-            # bpr: every rank ranks the items of its own row block, so it keeps the whole test set
-            test = (ti, tj) if bpr else (ti[rank::world], tj[rank::world], tx[rank::world])
-    elif bpr:
+            # bpr, implicit: every rank ranks the items of its own row block, so it keeps the whole test set
+            test = (ti, tj) if ranking else (ti[rank::world], tj[rank::world], tx[rank::world])
+    elif ranking:
         m, n = args.num_rows, args.num_cols
         data, test = SparseMatrix.synthetic_implicit(m, n, max(1, (args.synthetic_nnz or 200000) // m), 8, world, rank,
                                                      seed=args.model_seed)
@@ -99,7 +114,7 @@ def main(argv=None) -> int:
                    signal_intent_rows=bool(args.signal_intent_rows), wor_blocks=bool(args.wor_blocks),
                    wor_points=bool(args.wor_points), early_stop=args.early_stop, deterministic=bool(args.deterministic),
                    loss=args.loss, num_negatives=args.num_negatives,
-                   sampling_scheme=getattr(args, "sampling.scheme") or "local")
+                   sampling_scheme=getattr(args, "sampling.scheme") or "local", alpha=args.alpha)
     ad.setup(cfg.num_keys(world), 1)   # one worker per rank: the per-thread loops of the reference are batched kernels here
     server = ad.Server(cfg.row_len, backend=args.backend, options=system_options(args),
                        dtype={"float": "float32", "double": "float64"}[args.value_type])
@@ -120,6 +135,24 @@ def main(argv=None) -> int:
     for epoch in range(args.epochs):
         loss = model.run_epoch(epoch)
         kv.barrier()
+        if als:                                    # no step size: the bold driver does not apply
+            objective = server.allreduce_sum([loss])[0]
+            if args.compute_loss:
+                msg = f"[mf] epoch {epoch}: objective {objective:.9g}"
+                if test is not None:
+                    kv.wait_sync()
+                    if ranking:
+                        tr = server.allreduce_sum([float(v) for v in model.evaluate_ranking(*test, k=args.eval_k)])
+                        users = max(1.0, float(tr[2]))
+                        msg += f", test recall@{args.eval_k} {tr[0] / users:.4f}, ndcg@{args.eval_k} {tr[1] / users:.4f}"
+                    else:
+                        tl = server.allreduce_sum([model.evaluate(*test), float(len(test[2]))])
+                        msg += f", test rmse {float((tl[0] / max(1.0, float(tl[1]))) ** 0.5):.4f}"
+                if server.my_rank() == 0:
+                    print(msg + f" ({time.time() - t0:.1f}s)", flush=True)
+            if time.time() - t0 > args.max_runtime:
+                break
+            continue
         model.bold_driver(loss, prev)
         prev = loss
         if args.compute_loss and bpr:

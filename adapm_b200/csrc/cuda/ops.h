@@ -93,6 +93,18 @@ constexpr int kBprMaxNeg = 256;
 void mf_bpr_step(CudaBackend& be, cudaStream_t stream, const Key* users, const Key* pos, const Key* neg, int B, int n_neg,
                  int rank, float eps, float lam, float* loss_out, unsigned long long* stats, bool deterministic = false);
 
+// alternating least squares for matrix factorisation (ops_als.cu). Target targets[t] (distinct) has the entries
+// others[offsets[t] .. offsets[t + 1]) with weights a, b; rows [factors (rank) | AdaGrad (rank)], rank % 4 == 0,
+// 4 <= rank <= 128. One CTA per target, in the given order: A = gram + lam I + sum_e a_e h_e h_e^T, r = sum_e b_e h_e,
+// w <- A^{-1} r pushed as [w_new - w_old | 0]; a pivot <= 0 leaves the target unchanged. gram: [rank, rank] or null.
+// stats: (other rows local, other rows from peers, slow-path rows, rows solved), accumulated. 1 launch.
+constexpr int kAlsMaxRank = 128;
+void als_solve(CudaBackend& be, cudaStream_t stream, const Key* targets, const int64_t* offsets, const Key* others,
+               const float* a, const float* b, int n, int rank, float lam, const float* gram, unsigned long long* stats);
+// G[rank, rank] = sum over keys[0 .. n) of h h^T (factor halves): partials of 1024 keys added in index order,
+// bit-identical from call to call and wherever the rows live. 2 launches.
+void als_gram(CudaBackend& be, cudaStream_t stream, const Key* keys, int64_t n, int rank, float* G);
+
 // wgmma/TMA GEMM: C[M,N] fp32 = A[M,K] bf16 x B[N,K]^T bf16 (ops_gemm_wgmma.cu)
 void gemm_nt_bf16(cudaStream_t stream, const void* A, const void* B, int M, int N, int K, float* C, int ldc);
 void gemm_nt_e4m3(cudaStream_t stream, const void* A, const void* B, int M, int N, int K, float* C, int ldc, float alpha);

@@ -135,6 +135,16 @@ void bind(py::module_& m) {
     mf_bpr_step(backend_of(be), (cudaStream_t)stream, ptr<const Key>(users), ptr<const Key>(pos), ptr<const Key>(neg), B,
                 n_neg, rank, eps, lam, ptr<float>(loss), ptr<unsigned long long>(stats), deterministic);
   });
+  m.attr("als_max_rank") = kAlsMaxRank;
+  m.def("als_solve", [](uintptr_t be, uintptr_t stream, uintptr_t targets, uintptr_t offsets, uintptr_t others,
+                        uintptr_t a, uintptr_t b, int n, int rank, float lam, uintptr_t gram, uintptr_t stats) {
+    als_solve(backend_of(be), (cudaStream_t)stream, ptr<const Key>(targets), ptr<const int64_t>(offsets),
+              ptr<const Key>(others), ptr<const float>(a), ptr<const float>(b), n, rank, lam, ptr<const float>(gram),
+              ptr<unsigned long long>(stats));
+  });
+  m.def("als_gram", [](uintptr_t be, uintptr_t stream, uintptr_t keys, int64_t n, int rank, uintptr_t G) {
+    als_gram(backend_of(be), (cudaStream_t)stream, ptr<const Key>(keys), n, rank, ptr<float>(G));
+  });
   m.def("dist_num_slices", [](uintptr_t be, int M, int N, int max_tiles_per_cta) {
     return dist_num_slices(backend_of(be), M, N, max_tiles_per_cta);
   });

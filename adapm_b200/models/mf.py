@@ -19,6 +19,12 @@ Implicit feedback (``MFConfig.loss = "bpr"``, an addition of this implementation
 with the BPR pairwise loss against sampled negative items in one fused kernel (``ops.mf_bpr_step``) on the same rows and
 schedules; ``recommend`` ranks the items of a user with the seen ones left out, ``evaluate_ranking`` gives Recall@k and
 NDCG@k.
+
+Alternating least squares (``MFConfig.algorithm = "als"``, also an addition): each half-step solves every row of one
+side exactly for the other side held fixed, one fused gather + Cholesky kernel per row (``ops.als_solve``). With
+``loss = "squared"`` it minimises the objective above; with ``loss = "implicit"`` the Hu-Koren-Volinsky objective
+``sum_{u,i} c_ui (p_ui - w_u.h_i)^2 + lambda (|W|^2 + |H|^2)`` over all pairs (``c = 1 + alpha x`` and ``p = 1`` on the
+entries, ``c = 1`` and ``p = 0`` elsewhere) through the Gram matrix of the other side (``ops.als_gram``).
 """
 from __future__ import annotations
 
@@ -36,7 +42,7 @@ class MFConfig:
     num_rows: int = 10_000_000
     num_cols: int = 1_000_000
     rank: int = 128
-    algorithm: str = "dsgd"          # dsgd | columnwise | plain
+    algorithm: str = "dsgd"          # dsgd | columnwise | plain | als
     eps: float = 0.01                # initial step size
     lam: float = 0.05
     batch_nnz: int = 1 << 18
@@ -53,8 +59,10 @@ class MFConfig:
     deterministic: bool = False      # one GPU: start-of-step reads, bit-identical runs (ops.mf_step); the CPU backend
                                      # accepts it and already follows the start-of-step rule
     loss: str = "squared"            # squared (explicit ratings) | bpr (implicit feedback: every entry is an interaction)
+                                     # | implicit (als only: the Hu-Koren-Volinsky weighted loss over all pairs)
     num_negatives: int = 1           # bpr: sampled negative items per positive
     sampling_scheme: str = "local"   # bpr on several ranks outside dsgd: "local" draws only resident items
+    alpha: float = 1.0               # implicit: confidence c = 1 + alpha x of an entry with value x
 
     def first_col_key(self, num_workers: int) -> int:
         return ((self.num_rows + num_workers - 1) // num_workers) * num_workers
@@ -76,6 +84,8 @@ class SparseMatrix:
         self.col_nnz_all = np.bincount(j, minlength=num_cols).astype(np.int32)
         self.rows_per_block = (num_rows + world - 1) // world
         self.cols_per_block = (num_cols + world - 1) // world
+        cb = (j // self.cols_per_block) == rank                          # this rank's column block (als)
+        self._col_entries = (i[cb], j[cb], x[cb].astype(np.float32))
         mine = (i // self.rows_per_block) == rank                       # row partitioning (apps/mf/io.h:163-175)
         self.i, self.j, self.x = i[mine], j[mine], x[mine].astype(np.float32)
         blk = self.j // self.cols_per_block
@@ -132,6 +142,31 @@ class SparseMatrix:
         lo = self.rank * self.rows_per_block
         return lo, min(self.num_rows, lo + self.rows_per_block)
 
+    def col_block(self):
+        """[lo, hi): the columns of this rank's block"""
+        lo = self.rank * self.cols_per_block
+        return lo, min(self.num_cols, lo + self.cols_per_block)
+
+    def als_csr(self, side: str):
+        """The entries of this rank's row block by row (``side = "rows"``) or of its column block by column
+        (``"cols"``), every row / column of the block included, ordered by descending entry count (ties to the smaller
+        index; entries in file order): ``(targets, offsets [n + 1], others, x)``, numpy, with row and column indices."""
+        if side == "rows":
+            lo, hi = self.row_block()
+            t, o, x = self.i.astype(np.int64), self.j.astype(np.int64), self.x
+        else:
+            lo, hi = self.col_block()
+            t, o, x = (self._col_entries[1].astype(np.int64), self._col_entries[0].astype(np.int64),
+                       self._col_entries[2])
+        cnt = np.bincount(t - lo, minlength=hi - lo)
+        targets = np.argsort(-cnt, kind="stable")
+        rank_of = np.empty_like(targets)
+        rank_of[targets] = np.arange(targets.shape[0])
+        order = np.argsort(rank_of[t - lo], kind="stable")
+        offsets = np.zeros(targets.shape[0] + 1, dtype=np.int64)
+        np.cumsum(cnt[targets], out=offsets[1:])
+        return targets + lo, offsets, o[order], x[order]
+
     def seen(self, rows):
         """Training items of ``rows`` (all in this rank's row block, else ``ValueError``) as a CSR ``(offsets int64
         [n + 1], items int64)`` with each row's items distinct and ascending: the ``exclude`` of a recommendation."""
@@ -166,8 +201,16 @@ class MatrixFactorization:
         self.eps = cfg.eps
         self.step_no = 0
         dev = server.device
-        if cfg.loss not in ("squared", "bpr"):
-            raise ValueError(f"loss must be 'squared' or 'bpr', got {cfg.loss!r}")
+        if cfg.loss not in ("squared", "bpr", "implicit"):
+            raise ValueError(f"loss must be 'squared', 'bpr' or 'implicit', got {cfg.loss!r}")
+        if cfg.algorithm == "als" and cfg.loss == "bpr":
+            raise ValueError("algorithm 'als' takes loss 'squared' or 'implicit', not 'bpr'")
+        if cfg.loss == "implicit" and cfg.algorithm != "als":
+            raise ValueError(f"loss 'implicit' needs algorithm 'als', got {cfg.algorithm!r}")
+        if cfg.algorithm == "als" and not (cfg.lam > 0 and cfg.alpha >= 0):
+            raise ValueError(f"als needs lam > 0 and alpha >= 0, got lam {cfg.lam}, alpha {cfg.alpha}")
+        if cfg.loss == "implicit" and ((data.x < 0).any() or (data._col_entries[2] < 0).any()):
+            raise ValueError("loss 'implicit' needs entry values >= 0 (interaction strengths)")
         if cfg.loss == "bpr" and cfg.num_negatives < 1:
             raise ValueError(f"num_negatives must be >= 1, got {cfg.num_negatives}")
         self._neg_range = (0, cfg.num_cols)          # bpr: the items negatives are drawn from (set per sub-epoch)
@@ -205,6 +248,9 @@ class MatrixFactorization:
             lo = rank * self.data.rows_per_block
             hi = min(cfg.num_rows, lo + self.data.rows_per_block)
             self.worker.intent(torch.arange(lo, hi), 0, CLOCK_MAX)
+        if world > 1 and cfg.algorithm == "als":      # the column block is written by this rank in every item half-step
+            lo, hi = self.data.col_block()
+            self.worker.intent(torch.arange(lo, hi) + self.fck, 0, CLOCK_MAX)
 
     # one batch of non-zeros (numpy views of this rank's data)
     def step(self, i: np.ndarray, j: np.ndarray, x: np.ndarray) -> torch.Tensor:
@@ -265,6 +311,8 @@ class MatrixFactorization:
     def run_epoch(self, epoch: int) -> float:
         """One epoch with the configured schedule. Returns this rank's summed squared error."""
         cfg, kv, data, W = self.cfg, self.worker, self.data, self.world
+        if cfg.algorithm == "als":
+            return self.als_epoch()
         total = 0.0
         if self.cuda:
             self.loss.zero_()
@@ -331,6 +379,109 @@ class MatrixFactorization:
                 kv.advance_clock()
         if self.cuda:
             total = float(self.loss.item())
+        return total
+
+    # ------------------------------------------------------------------------------------------ alternating least squares
+    def _als_block(self, side: str):
+        """(target keys, offsets, other keys, a, b) of this rank's row (``"rows"``) or column (``"cols"``) block, longest
+        target first; built once, on the device on CUDA"""
+        cache = self.__dict__.setdefault("_als_blocks", {})
+        if side not in cache:
+            cfg = self.cfg
+            t, off, o, x = self.data.als_csr(side)
+            if side == "rows":
+                t, o = t, o + self.fck
+            else:
+                t, o = t + self.fck, o
+            x = x.astype(np.float64)
+            if cfg.loss == "implicit":
+                a, b = cfg.alpha * x, 1.0 + cfg.alpha * x
+            else:
+                a, b = np.ones_like(x), x
+            blk = [torch.from_numpy(np.ascontiguousarray(v)) for v in (t, off, o)]
+            blk += [torch.from_numpy(a.astype(np.float32)), torch.from_numpy(b.astype(np.float32))]
+            if self.cuda:
+                blk = [v.to(self.server.device) for v in blk]
+            cache[side] = blk
+        return cache[side]
+
+    def _other_keys(self, side: str) -> torch.Tensor:
+        """all keys of the side that the targets of ``side`` read (items for the row block, users for the column block)"""
+        cfg = self.cfg
+        keys = (torch.arange(cfg.num_cols, dtype=torch.int64) + self.fck if side == "rows"
+                else torch.arange(cfg.num_rows, dtype=torch.int64))
+        return keys.to(self.server.device) if self.cuda else keys
+
+    def als_half_step(self, side: str) -> None:
+        """Solve every row of this rank's row block (``side = "rows"``) or column block (``"cols"``) for the other side
+        held fixed; collective (ends with a barrier)."""
+        cfg, kv = self.cfg, self.worker
+        t, off, o, a, b = self._als_block(side)
+        implicit = cfg.loss == "implicit"
+        if self.cuda:
+            from ..ops import als_gram, als_solve
+
+            gram = als_gram(self.server, self._other_keys(side), cfg.rank) if implicit else None
+            als_solve(self.server, t, off, o, a, b, cfg.rank, cfg.lam, gram, self.stats)
+            torch.cuda.current_stream(self.server.device).synchronize()
+        else:
+            from ..ops import als_gram_reference, als_reference_solve
+
+            gram = als_gram_reference(kv, self._other_keys(side), cfg.rank) if implicit else None
+            als_reference_solve(kv, t, off, o, a, b, cfg.rank, cfg.lam, gram)
+        self.step_no += 1
+        kv.advance_clock()
+        kv.barrier()
+
+    def als_epoch(self) -> float:
+        """One ALS epoch: the row block, then the column block. Returns this rank's share of ``als_objective``."""
+        self.als_half_step("rows")
+        self.als_half_step("cols")
+        return self.als_objective()
+
+    def als_objective(self, chunk: int = 1 << 16) -> float:
+        """This rank's share of the ALS objective, in float64 from pulled rows; the shares of all ranks sum to it
+        (``server.allreduce_sum``). Squared: ``sum_e (x_e - w.h)^2`` over this rank's entries; implicit: ``sum_e [c_e
+        (1 - w.h)^2 - (w.h)^2]`` over them (``c_e = 1 + alpha x_e``) plus ``sum_u w_u^T G w_u`` over this rank's users,
+        G the Gram matrix of all items; both plus ``lambda (|W_block|^2 + |H_block|^2)`` of this rank's row and column
+        blocks. Entries that occur twice count twice, as in the solve."""
+        cfg, kv, data, r = self.cfg, self.worker, self.data, self.cfg.rank
+        f64 = torch.float64
+
+        def pull(keys):
+            keys = torch.as_tensor(keys, dtype=torch.int64)
+            v = torch.empty(keys.numel() * 2 * r, dtype=self.dtype,
+                            device=self.server.device if self.cuda else "cpu")
+            if keys.numel():
+                if self.cuda:
+                    kv.wait(kv.pull(keys.to(self.server.device), v, True))
+                    torch.cuda.current_stream(self.server.device).synchronize()
+                else:
+                    kv.wait(kv.pull(keys, v))
+            return v.view(-1, 2 * r)[:, :r].to(f64).cpu()
+
+        total = 0.0
+        for s in range(0, data.i.shape[0], chunk):
+            w = pull(data.i[s:s + chunk].astype(np.int64))
+            h = pull(data.j[s:s + chunk].astype(np.int64) + self.fck)
+            pred = (w * h).sum(1)
+            x = torch.from_numpy(data.x[s:s + chunk].astype(np.float64))
+            if cfg.loss == "implicit":
+                total += float(((1.0 + cfg.alpha * x) * (1.0 - pred) ** 2 - pred ** 2).sum())
+            else:
+                total += float(((x - pred) ** 2).sum())
+        G = None
+        if cfg.loss == "implicit":
+            G = torch.zeros(r, r, dtype=f64)
+            for s in range(0, cfg.num_cols, chunk):
+                h = pull(np.arange(s, min(cfg.num_cols, s + chunk)) + self.fck)
+                G += h.t() @ h
+        for lo, hi, first, gram in ((*data.row_block(), 0, G), (*data.col_block(), self.fck, None)):
+            for s in range(lo, hi, chunk):
+                w = pull(np.arange(s, min(hi, s + chunk)) + first)
+                total += cfg.lam * float((w * w).sum())
+                if gram is not None:
+                    total += float(((w @ gram) * w).sum())
         return total
 
     def load_factors(self, w_path: str, h_path: str, chunk: int = 1 << 16) -> None:

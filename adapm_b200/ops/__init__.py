@@ -768,6 +768,124 @@ def bpr_reference_step(kv, users: torch.Tensor, pos: torch.Tensor, neg: torch.Te
     return loss, B * (2 + n)
 
 
+ALS_MAX_RANK = 128
+
+
+def _check_als_rank(rank: int) -> None:
+    if isinstance(rank, bool) or int(rank) != rank or not (4 <= int(rank) <= ALS_MAX_RANK and int(rank) % 4 == 0):
+        raise ValueError(f"rank must be a multiple of 4 in [4, {ALS_MAX_RANK}], got {rank}")
+
+
+def _check_als_args(targets, offsets, others, a, b, rank, lam, gram) -> None:
+    _check_als_rank(rank)
+    if not lam > 0:
+        raise ValueError(f"lam must be > 0, got {lam}")
+    n, nnz = targets.numel(), others.numel()
+    if offsets.numel() != n + 1 or a.numel() != nnz or b.numel() != nnz:
+        raise ValueError(f"offsets must have len(targets) + 1 = {n + 1} entries and a, b len(others) = {nnz}, got "
+                         f"{offsets.numel()}, {a.numel()}, {b.numel()}")
+    if int(offsets[0]) != 0 or int(offsets[-1]) != nnz or bool((offsets[1:] < offsets[:-1]).any()):
+        raise ValueError("offsets must be monotone from 0 to len(others)")
+    if nnz and not bool((a >= 0).all()):
+        raise ValueError("a must be >= 0")
+    if torch.unique(targets).numel() != n:
+        raise ValueError("targets must be distinct")
+    if gram is not None and not (gram.dtype == torch.float32 and tuple(gram.shape) == (rank, rank)):
+        raise ValueError(f"gram must be float32 [{rank}, {rank}] or None, got {gram.dtype} {tuple(gram.shape)}")
+
+
+def als_solve(server, targets: torch.Tensor, offsets: torch.Tensor, others: torch.Tensor, a: torch.Tensor,
+              b: torch.Tensor, rank: int, lam: float, gram: Optional[torch.Tensor] = None,
+              stats: Optional[torch.Tensor] = None) -> None:
+    """One alternating-least-squares solve per target row (csrc/cuda/ops_als.cu) on ``server``'s store: target
+    ``targets[t]`` (distinct store keys) has the entries ``others[offsets[t] .. offsets[t + 1])`` (store keys of the other
+    side, repeats count as often as they occur) with weights ``a`` (>= 0) and ``b`` (float32). Rows are ``[factors
+    (rank) | AdaGrad (rank)]``, ``rank`` a multiple of 4 in [4, 128]. The rule is :func:`als_reference_solve`'s:
+    ``A = gram + lam I + sum_e a_e h_e h_e^T``, ``r = sum_e b_e h_e``, ``w <- A^{-1} r`` pushed as ``[w_new - w_old | 0]``
+    (the AdaGrad half is untouched); a target without entries becomes ``0``. One CTA per target in the given order (pass
+    the longest first); the result does not depend on the order and is bit-identical from run to run. Factorised by
+    Cholesky in fp32: a pivot <= 0 leaves the target unchanged and uncounted. ``gram``: float32 [rank, rank] or None;
+    ``stats``: optional int64[4] accumulated with (other rows local, other rows from peers, slow-path rows, rows solved).
+    Every half-step must only read rows it does not write: targets and others are keys of different sides."""
+    _i64(targets, "targets"); _i64(offsets, "offsets"); _i64(others, "others"); _f32(a, "a"); _f32(b, "b")
+    if gram is not None:
+        _f32(gram, "gram")
+    _check_als_args(targets, offsets, others, a, b, rank, lam, gram)
+    if stats is not None and not (stats.is_cuda and stats.dtype == torch.int64 and stats.numel() >= 4):
+        raise TypeError("stats must be a CUDA int64 tensor with 4 entries")
+    _C.als_solve(server._impl.backend_handle(), _stream(targets), targets.data_ptr(), offsets.data_ptr(),
+                 others.data_ptr(), a.data_ptr(), b.data_ptr(), targets.numel(), int(rank), float(lam),
+                 gram.data_ptr() if gram is not None else 0, stats.data_ptr() if stats is not None else 0)
+
+
+def als_gram(server, keys: torch.Tensor, rank: int) -> torch.Tensor:
+    """``G = sum_k h_k h_k^T`` (float32 [rank, rank]) over the factor halves of the store rows ``keys`` (CUDA int64), read
+    wherever they live. Each 1 024 keys form a partial in fp32 (fixed order) and the partials are added in index order,
+    so G is bit-identical from call to call and on every rank of a multi-rank store."""
+    _i64(keys, "keys")
+    _check_als_rank(rank)
+    G = torch.empty(int(rank), int(rank), dtype=torch.float32, device=keys.device)
+    _C.als_gram(server._impl.backend_handle(), _stream(keys), keys.data_ptr(), keys.numel(), int(rank), G.data_ptr())
+    return G
+
+
+def als_gram_reference(kv, keys: torch.Tensor, rank: int, chunk: int = 1 << 16) -> torch.Tensor:
+    """:func:`als_gram` in float64 through Pull (CPU servers and the tests)."""
+    keys = keys.reshape(-1).cpu()
+    r = int(rank)
+    G = torch.zeros(r, r, dtype=torch.float64)
+    for s in range(0, keys.numel(), chunk):
+        k = keys[s:s + chunk].contiguous()
+        v = torch.empty(k.numel() * 2 * r, dtype=kv.server.dtype)
+        kv.wait(kv.pull(k, v))
+        H = v.view(-1, 2 * r)[:, :r].to(torch.float64)
+        G += H.t() @ H
+    return G
+
+
+def als_reference_solve(kv, targets: torch.Tensor, offsets: torch.Tensor, others: torch.Tensor, a: torch.Tensor,
+                        b: torch.Tensor, rank: int, lam: float, gram: Optional[torch.Tensor] = None,
+                        chunk: int = 8192) -> int:
+    """The rule of :func:`als_solve` in float64 through Pull / Push (CPU servers, float64 rows, and the oracle of the
+    tests): per target ``A = gram + lam I + sum_e a_e h_e h_e^T``, ``r = sum_e b_e h_e``, ``w <- A^{-1} r`` by Cholesky,
+    pushed as ``[w_new - w_old | 0]``; a target whose A is not positive definite is left unchanged. Every row is read
+    before any is written. Returns the number of targets solved."""
+    targets, offsets, others = targets.reshape(-1).cpu(), offsets.reshape(-1).cpu(), others.reshape(-1).cpu()
+    a, b = a.reshape(-1).cpu().to(torch.float64), b.reshape(-1).cpu().to(torch.float64)
+    if gram is not None:
+        gram = gram.cpu()
+    _check_als_args(targets, offsets, others, a, b, rank, lam, gram if gram is None else gram.float())
+    n, r, f64 = targets.numel(), int(rank), torch.float64
+    if n == 0:
+        return 0
+
+    def pull(keys):
+        v = torch.empty(keys.numel() * 2 * r, dtype=kv.server.dtype)
+        if keys.numel():
+            kv.wait(kv.pull(keys.contiguous(), v))
+        return v.view(-1, 2 * r)[:, :r].to(f64)
+
+    W, H = pull(targets), pull(others)
+    A = torch.zeros(n, r, r, dtype=f64)
+    if gram is not None:
+        A += gram.to(f64)
+    A += lam * torch.eye(r, dtype=f64)
+    owner = torch.repeat_interleave(torch.arange(n), offsets[1:] - offsets[:-1])
+    rhs = torch.zeros(n, r, dtype=f64)
+    rhs.index_add_(0, owner, b.unsqueeze(1) * H)
+    for s in range(0, H.shape[0], chunk):
+        h = H[s:s + chunk]
+        A.index_add_(0, owner[s:s + chunk], a[s:s + chunk, None, None] * h.unsqueeze(2) * h.unsqueeze(1))
+    L, info = torch.linalg.cholesky_ex(A)
+    ok = info == 0
+    x = torch.cholesky_solve(rhs[ok].unsqueeze(2), L[ok]).squeeze(2)
+    upd = torch.zeros(int(ok.sum()), 2 * r, dtype=f64)
+    upd[:, :r] = x - W[ok]
+    if upd.shape[0]:
+        kv.wait(kv.push(targets[ok].contiguous(), upd.to(kv.server.dtype).contiguous().view(-1)))
+    return int(ok.sum())
+
+
 def _bf16_k8(t: torch.Tensor) -> torch.Tensor:
     """contiguous bf16 copy whose K (last dim) is padded to a multiple of 8 (16-byte TMA row pitch)."""
     t = t.to(torch.bfloat16)
