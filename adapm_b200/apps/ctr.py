@@ -1,8 +1,10 @@
-"""CTR DeepFM application (BASELINE config #5) on the bindings-style API.
+"""CTR application (BASELINE config #5) on the bindings-style API: DeepFM, or a field-aware factorisation machine
+(``--model ffm``, libffm's model: one latent vector per field in every feature's row; ``--embed_dim`` is its k).
 
     python -m adapm_b200.launch -s 8 --backend cuda -m adapm_b200.apps.ctr -- --num_features 100000000
     python -m adapm_b200.apps.ctr --backend cpu --num_features 20000 --steps 30 --batch_size 512
     python -m adapm_b200.apps.ctr --backend cpu --num_features 20000 --steps 30 --batch_size 512 --multi_hot 3
+    python -m adapm_b200.apps.ctr --backend cpu --model ffm --num_features 20000 --num_fields 8 --embed_dim 4 --steps 30
 """
 from __future__ import annotations
 
@@ -13,24 +15,34 @@ import time
 import adapm_b200 as ad
 from adapm_b200.apps._common import add_system_options, strip_dashes, system_options
 from adapm_b200.models.deepfm import DeepFM, DeepFMConfig, synthetic_ctr_batch, synthetic_multi_hot_batch
+from adapm_b200.models.ffm import FFM, FFMConfig, synthetic_ffm_batch
 
 
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--model", default="deepfm", choices=["deepfm", "ffm"])
     ap.add_argument("--num_features", type=int, default=1_000_000)
     ap.add_argument("--num_fields", type=int, default=26)
-    ap.add_argument("--embed_dim", type=int, default=16)
+    ap.add_argument("--embed_dim", type=int, default=16, help="DeepFM: embedding size; FFM: k, latent values per field")
     ap.add_argument("--batch_size", type=int, default=8192)
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--read_ahead", type=int, default=4)
-    ap.add_argument("--precision", default="bf16", choices=["fp32", "bf16", "fp8"])
+    ap.add_argument("--precision", default="bf16", choices=["fp32", "bf16", "fp8"], help="DeepFM only: the dense GEMMs")
     ap.add_argument("--table_precision", default="fp32", choices=["fp32", "fp8_block"],
-                    help="fp8_block: train on the values a block-scaled e4m3 embedding table would deliver (fp32 master rows)")
+                    help="DeepFM only. fp8_block: train on the values a block-scaled e4m3 embedding table would deliver "
+                         "(fp32 master rows)")
     ap.add_argument("--multi_hot", type=int, default=0,
                     help="> 0: every field holds a bag of 1..L ids, pooled into one embedding (fused kernels on CUDA)")
     ap.add_argument("--pooling", default="sum", choices=["sum", "mean"], help="pooling of multi-hot bags")
+    ap.add_argument("--eta", type=float, default=0.2, help="FFM: AdaGrad step size")
+    ap.add_argument("--lam", type=float, default=2e-5, help="FFM: L2 regularisation")
+    ap.add_argument("--test_batches", type=int, default=4, help="FFM: held-out batches evaluated after training")
     add_system_options(ap)
     args = ap.parse_args(strip_dashes(argv if argv is not None else sys.argv[1:]))
+    if args.model == "ffm":
+        if args.multi_hot > 0:
+            ap.error("--multi_hot is not supported with --model ffm (one id per field)")
+        return run_ffm(args)
     cfg = DeepFMConfig(num_features=args.num_features, num_fields=args.num_fields, embed_dim=args.embed_dim,
                        batch_size=args.batch_size, read_ahead=args.read_ahead, precision=args.precision,
                        table_precision=args.table_precision, multi_hot=args.multi_hot, pooling=args.pooling)
@@ -72,6 +84,49 @@ def main(argv=None) -> int:
     kv.barrier()
     kv.finalize()
     if rank == 0:
+        print(server.stats(), flush=True)
+    server.shutdown()
+    return 0
+
+
+def run_ffm(args) -> int:
+    cfg = FFMConfig(num_features=args.num_features, num_fields=args.num_fields, k=args.embed_dim, eta=args.eta,
+                    lam=args.lam, batch_size=args.batch_size, read_ahead=args.read_ahead)
+    ad.setup(cfg.num_features, 1)
+    server = ad.Server(cfg.row_len, backend=args.backend, options=system_options(args))
+    kv = ad.Worker(0, server)
+    model = FFM(server, kv, cfg)
+    model.init_model()
+    rank = server.my_rank()
+    from ..parallel.schedules import LookaheadIntents
+
+    batches = {}
+
+    def batch(b):
+        if b not in batches:
+            batches[b] = synthetic_ffm_batch(cfg, b, rank)
+        return batches[b]
+
+    look = LookaheadIntents(kv, args.steps + cfg.read_ahead, cfg.read_ahead, lambda b: batch(b)[0]) if server.num_servers() > 1 else None
+    if look:
+        look.prime()
+    t0, losses = time.time(), []
+    for s in range(args.steps):
+        if look:
+            look.signal(s)
+        ids, y = batch(s)
+        batches.pop(s - 1, None)
+        losses.append(model.step(ids, y))
+        kv.advance_clock()
+        if rank == 0 and (s + 1) % max(1, args.steps // 5) == 0:
+            print(f"[ctr] step {s + 1}: loss {sum(losses[-10:]) / len(losses[-10:]):.4f} "
+                  f"({(s + 1) * cfg.batch_size / (time.time() - t0):.0f} examples/s/rank)", flush=True)
+    kv.barrier()
+    ll, auc = model.evaluate(synthetic_ffm_batch(cfg, b, rank, held_out=True) for b in range(args.test_batches))
+    kv.barrier()
+    kv.finalize()
+    if rank == 0:
+        print(f"[ctr] test logloss {ll:.4f} auc {auc:.4f}", flush=True)
         print(server.stats(), flush=True)
     server.shutdown()
     return 0

@@ -172,6 +172,24 @@ void embedding_bag_backward(CudaBackend& be, cudaStream_t stream, const Key* key
                             float lr, float grad_scale, void* workspace, size_t workspace_bytes,
                             unsigned long long* stats);
 
+// field-aware factorisation machines (ops_ffm.cu) over rows [w, 0, 0, 0 | V_0 .. V_{F-1} (k each) | AdaGrad], E =
+// 4 + F k values: ids [B, F] (the field of ids[b, f] is f), labels [B]; 2 <= F <= 64, k a multiple of 4 in [4, 32],
+// F k <= 512, B F < 2^31. stats: int64[5] accumulated with (local rows, peer rows, slow-path rows, rows updated, rows
+// that could not be resolved).
+// forward (1 launch): logits[b] = phi_b = sum_f w[x_bf] + r sum_{f1<f2} <V[x_bf1][f2], V[x_bf2][f1]>.
+// step (5 launches, the radix sort counted as one): phi from the rows at the start of the step; per distinct key the
+// sum over its occurrences (b, f), in position order, of [kappa_b + lam w | 0 | kappa_b r V[x_b,f2][f] + lam V_f2 for
+// f2 != f], kappa_b = sigmoid(phi_b) - y_b, pushed once as [-eta G / sqrt(acc + G^2) | G^2]; *loss = sum_b
+// softplus(phi_b) - y_b phi_b.
+constexpr int kFfmMaxFields = 64;
+constexpr int kFfmMaxK = 32;
+constexpr int kFfmMaxFk = 512;
+size_t ffm_workspace_bytes(int B, int F, int k);
+void ffm_forward(CudaBackend& be, cudaStream_t stream, const Key* ids, int B, int F, int k, float r, float* logits,
+                 unsigned long long* stats);
+void ffm_step(CudaBackend& be, cudaStream_t stream, const Key* ids, const float* labels, int B, int F, int k, float r,
+              float eta, float lam, void* workspace, size_t workspace_bytes, float* loss, unsigned long long* stats);
+
 // Native step driver of the word2vec SGNS loop (ops_train_loop.cu)
 struct SgnsLoopConfig {
   int batch_pairs = 0, negative = 0, embed_dim = 0, read_ahead = 0, max_inflight = 3, rank = 0;

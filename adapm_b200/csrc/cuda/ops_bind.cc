@@ -179,6 +179,20 @@ void bind(py::module_& m) {
                            ptr<const float>(weights), nnz, nbags, E, mean, ptr<const float>(grad_out), lr, grad_scale,
                            ptr<void>(ws), ws_bytes, ptr<unsigned long long>(stats));
   });
+  m.attr("ffm_max_fields") = kFfmMaxFields;
+  m.attr("ffm_max_k") = kFfmMaxK;
+  m.attr("ffm_max_fk") = kFfmMaxFk;
+  m.def("ffm_workspace_bytes", [](int B, int F, int k) { return ffm_workspace_bytes(B, F, k); });
+  m.def("ffm_forward", [](uintptr_t be, uintptr_t stream, uintptr_t ids, int B, int F, int k, float r, uintptr_t logits,
+                          uintptr_t stats) {
+    ffm_forward(backend_of(be), (cudaStream_t)stream, ptr<const Key>(ids), B, F, k, r, ptr<float>(logits),
+                ptr<unsigned long long>(stats));
+  });
+  m.def("ffm_step", [](uintptr_t be, uintptr_t stream, uintptr_t ids, uintptr_t labels, int B, int F, int k, float r,
+                       float eta, float lam, uintptr_t ws, size_t ws_bytes, uintptr_t loss, uintptr_t stats) {
+    ffm_step(backend_of(be), (cudaStream_t)stream, ptr<const Key>(ids), ptr<const float>(labels), B, F, k, r, eta, lam,
+             ptr<void>(ws), ws_bytes, ptr<float>(loss), ptr<unsigned long long>(stats));
+  });
   py::class_<SgnsLoop>(m, "SgnsLoop")
       .def(py::init([](uintptr_t worker, uintptr_t be, int batch_pairs, int negative, int embed_dim, int read_ahead,
                        int max_inflight, int rank, bool signal_intent, bool local_only, int64_t model_seed, int sampler_kind,

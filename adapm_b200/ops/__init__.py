@@ -1333,6 +1333,194 @@ def embedding_bag_reference(table: torch.Tensor, keys: torch.Tensor, offsets: to
     return out, new
 
 
+FFM_MAX_FIELDS = 64
+FFM_MAX_K = 32
+FFM_MAX_FK = 512
+
+
+def ffm_row_values(num_fields: int, k: int) -> int:
+    """E, the values of an FFM row before its AdaGrad half: ``[w, 0, 0, 0 | V_0 | ... | V_{F-1}]``."""
+    return 4 + int(num_fields) * int(k)
+
+
+def _check_ffm_shape(num_fields, k, row_len) -> None:
+    for v, nm in ((num_fields, "num_fields"), (k, "k")):
+        if isinstance(v, bool) or int(v) != v:
+            raise ValueError(f"{nm} must be an integer, got {v!r}")
+    F, k = int(num_fields), int(k)
+    if not 2 <= F <= FFM_MAX_FIELDS:
+        raise ValueError(f"num_fields must be in [2, {FFM_MAX_FIELDS}], got {F}")
+    if not (4 <= k <= FFM_MAX_K and k % 4 == 0):
+        raise ValueError(f"k must be a multiple of 4 in [4, {FFM_MAX_K}], got {k}")
+    if F * k > FFM_MAX_FK:
+        raise ValueError(f"num_fields * k must be <= {FFM_MAX_FK}, got {F * k}")
+    E = ffm_row_values(F, k)
+    if row_len != 2 * E:
+        raise ValueError(f"rows must be [w, 0, 0, 0 | V (num_fields * k) | AdaGrad]: the server's value length is "
+                         f"{row_len}, expected 2 * (4 + num_fields * k) = {2 * E}")
+
+
+def _check_ffm_rates(eta, lam) -> None:
+    for v, nm in ((eta, "eta"), (lam, "lam")):
+        if not float(v) >= 0.0:
+            raise ValueError(f"{nm} must be >= 0, got {v}")
+
+
+def _check_ffm_ids(ids, num_fields, device) -> int:
+    if not isinstance(ids, torch.Tensor) or ids.dtype != torch.int64 or ids.dim() != 2:
+        raise TypeError("ids must be a 2-D int64 tensor [B, num_fields]")
+    if device is not None and ids.device != device:
+        raise TypeError(f"ids must be on the store's device {device}, got {ids.device}")
+    if ids.shape[1] != num_fields:
+        raise ValueError(f"ids must have one column per field ({num_fields}), got {ids.shape[1]}")
+    if ids.numel() >= _NNZ_LIMIT:
+        raise ValueError(f"batch * num_fields must be < 2^31, got {ids.numel()}")
+    return ids.shape[0]
+
+
+def _check_ffm_labels(labels, B, device) -> None:
+    if not isinstance(labels, torch.Tensor) or labels.dtype != torch.float32:
+        raise TypeError("labels must be a float32 tensor")
+    if device is not None and labels.device != device:
+        raise TypeError(f"labels must be on the store's device {device}, got {labels.device}")
+    if labels.dim() != 1 or labels.numel() != B:
+        raise ValueError(f"labels must be [B = {B}], got {tuple(labels.shape)}")
+
+
+class StoreFFM:
+    """Field-aware factorisation machine (FFM, as in libffm) over the rows of a parameter store, trained by fused
+    sm_90a kernels (csrc/cuda/ops_ffm.cu) on a CUDA server.
+
+    A key's row is ``[w, 0, 0, 0 | V_0 | ... | V_{F-1} | AdaGrad of all E values]``, ``V_f`` its k-vector for field f
+    and ``E = 4 + F k`` (the server's value length must be ``2 E``). ``ids`` int64 ``[B, F]``: the field of
+    ``ids[b, f]`` is f. With ``r = pair_scale`` (``1 / F`` is libffm's instance normalisation of one-hot data)
+
+    * ``phi_b = sum_f w[x_bf] + r sum_{f1<f2} <V[x_bf1][f2], V[x_bf2][f1]>``, ``kappa_b = sigmoid(phi_b) - y_b``, loss
+      ``softplus(phi_b) - y_b phi_b``, all from the rows at the start of the step;
+    * per distinct key, summed over its occurrences ``(b, f)`` in position order ``b F + f``: ``G_w = sum kappa_b +
+      lam w`` and, for every field ``f2 != f``, ``G_(V, f2) = sum kappa_b r V[x_b,f2][f] + lam V_f2``;
+    * one push per distinct key ``[-eta G / sqrt(acc + G^2) | G^2]`` (0 where ``G == 0``, so the own-field block and the
+      padding never change), ``acc`` from the start of the step.
+
+    ``step(ids, labels)`` returns the summed loss as a device tensor; ``forward(ids)`` the logits ``phi`` [B]. Both
+    are sums in fp32 in a fixed order: on one GPU two runs from the same rows give bit-identical rows and loss.
+    :func:`ffm_reference_step` is the same rule in float64 through Pull / Push.
+
+    ``stats``: int64[4] accumulated with (rows read or updated locally, on peers, through the slow path of keys in a
+    transitional state, rows updated: one per distinct key and step). On several ranks a step or forward that could
+    not resolve a row raises ``RuntimeError``. Calls on one object must not overlap (one CUDA stream): the step's
+    scratch is owned by the object and grows on demand."""
+
+    def __init__(self, server, num_fields: int, k: int, eta: float = 0.2, lam: float = 2e-5, pair_scale: float = 1.0):
+        if server.backend != "cuda":
+            raise ValueError("StoreFFM needs a server with backend='cuda' (ffm_reference_step is the CPU route)")
+        if getattr(server, "dtype", torch.float32) != torch.float32:
+            raise ValueError("StoreFFM needs float32 rows")
+        _check_ffm_shape(num_fields, k, getattr(server, "_uniform_len", None))
+        _check_ffm_rates(eta, lam)
+        self.server, self.num_fields, self.k = server, int(num_fields), int(k)
+        self.eta, self.lam, self.pair_scale = float(eta), float(lam), float(pair_scale)
+        self.device = server.device
+        self._stats = torch.zeros(5, dtype=torch.int64, device=self.device)
+        self._ws = None
+
+    @property
+    def stats(self) -> torch.Tensor:
+        return self._stats[:4]
+
+    def _check_resolved(self, op):
+        if self.server.num_servers() > 1 and int(self._stats[4]):   # (waits for the kernel)
+            raise RuntimeError(f"StoreFFM {op}: {int(self._stats[4])} store rows could not be resolved")
+
+    def step(self, ids: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
+        """One training step on ``ids`` [B, F] and ``labels`` float32 [B] in [0, 1]; returns the summed loss (float32
+        [1] on the device)."""
+        B = _check_ffm_ids(ids, self.num_fields, self.device)
+        _check_ffm_labels(labels, B, self.device)
+        _check_ffm_rates(self.eta, self.lam)
+        ids, labels = ids.contiguous(), labels.contiguous()
+        need = _C.ffm_workspace_bytes(B, self.num_fields, self.k)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(max(need, 1), dtype=torch.uint8, device=self.device)
+        loss = torch.empty(1, dtype=torch.float32, device=self.device)
+        _C.ffm_step(self.server._impl.backend_handle(), _stream(ids), ids.data_ptr(), labels.data_ptr(), B,
+                    self.num_fields, self.k, self.pair_scale, self.eta, self.lam, self._ws.data_ptr(), self._ws.numel(),
+                    loss.data_ptr(), self._stats.data_ptr())
+        self._check_resolved("step")
+        return loss
+
+    def forward(self, ids: torch.Tensor) -> torch.Tensor:
+        """The logits ``phi`` (float32 [B]) of ``ids`` [B, F]; the rows are not changed."""
+        B = _check_ffm_ids(ids, self.num_fields, self.device)
+        ids = ids.contiguous()
+        out = torch.empty(B, dtype=torch.float32, device=self.device)
+        _C.ffm_forward(self.server._impl.backend_handle(), _stream(ids), ids.data_ptr(), B, self.num_fields, self.k,
+                       self.pair_scale, out.data_ptr(), self._stats.data_ptr())
+        self._check_resolved("forward")
+        return out
+
+
+def _ffm_pull(kv, ids: torch.Tensor, k: int, pair_scale: float):
+    """(distinct keys, their rows in float64 [U, 2E], position -> distinct key, phi [B], V [B, F, F, k])"""
+    B, F = ids.shape
+    E = ffm_row_values(F, k)
+    uniq, inv = torch.unique(ids.reshape(-1), return_inverse=True)
+    v = torch.empty(uniq.numel() * 2 * E, dtype=kv.server.dtype)
+    if uniq.numel():
+        kv.wait(kv.pull(uniq.contiguous(), v))
+    rows = v.view(-1, 2 * E).to(torch.float64)
+    x = rows[inv].view(B, F, 2 * E)
+    V = x[:, :, 4:E].reshape(B, F, F, k)                  # V[b, f1, f2] = V[x_bf1][f2]
+    P = torch.einsum("bijd,bjid->bij", V, V)              # <V[x_bi][j], V[x_bj][i]>
+    phi = x[:, :, 0].sum(1) + pair_scale * torch.triu(P, diagonal=1).sum((1, 2))
+    return uniq, rows, inv, phi, V
+
+
+def _ffm_ids_cpu(ids):
+    if not isinstance(ids, torch.Tensor) or ids.dim() != 2:
+        raise TypeError("ids must be a 2-D int64 tensor [B, num_fields]")
+    ids = ids.cpu()
+    _check_ffm_ids(ids, ids.shape[1], None)
+    return ids
+
+
+def ffm_reference_forward(kv, ids: torch.Tensor, k: int, pair_scale: float = 1.0) -> torch.Tensor:
+    """The logits of :class:`StoreFFM` in float64 (CPU tensor [B]) from rows read through Pull."""
+    ids = _ffm_ids_cpu(ids)
+    _check_ffm_shape(ids.shape[1], k, getattr(kv.server, "_uniform_len", None))
+    return _ffm_pull(kv, ids, int(k), float(pair_scale))[3]
+
+
+def ffm_reference_step(kv, ids: torch.Tensor, labels: torch.Tensor, k: int, eta: float, lam: float,
+                       pair_scale: float = 1.0) -> float:
+    """The rule of :class:`StoreFFM` in float64 through Pull / Push (CPU servers, and the oracle of the tests): every
+    row is read at the start of the step, each distinct key gets one push. Returns the summed loss."""
+    ids = _ffm_ids_cpu(ids)
+    B, F = ids.shape
+    _check_ffm_labels(labels.cpu(), B, None)
+    _check_ffm_shape(F, k, getattr(kv.server, "_uniform_len", None))
+    _check_ffm_rates(eta, lam)
+    k, r = int(k), float(pair_scale)
+    E = ffm_row_values(F, k)
+    y = labels.cpu().to(torch.float64)
+    uniq, rows, inv, phi, V = _ffm_pull(kv, ids, k, r)
+    loss = float((torch.nn.functional.softplus(phi) - y * phi).sum())
+    if B == 0:
+        return loss
+    kappa = (torch.sigmoid(phi) - y).view(B, 1, 1, 1)
+    w = rows[inv, 0].view(B, F)
+    c = torch.zeros(B, F, E, dtype=torch.float64)
+    c[:, :, 0] = kappa.view(B, 1) + lam * w
+    cv = kappa * r * V.transpose(1, 2) + lam * V          # [b, f, f2]: kappa r V[x_b,f2][f] + lam V[x_bf][f2]
+    cv[:, torch.arange(F), torch.arange(F)] = 0.0          # no term for f2 == f
+    c[:, :, 4:] = cv.reshape(B, F, F * k)
+    G = torch.zeros(uniq.numel(), E, dtype=torch.float64).index_add_(0, inv, c.view(B * F, E))
+    acc = rows[:, E:]
+    upd = torch.where(G != 0, -eta * G / torch.sqrt(acc + G * G), torch.zeros_like(G))
+    kv.wait(kv.push(uniq.contiguous(), torch.cat([upd, G * G], 1).to(kv.server.dtype).contiguous().view(-1)))
+    return loss
+
+
 class IntentPrepass:
     """Device-side pre-pass for ``Worker.intent`` (experimental; ``csrc/cuda/ops_intent.cu``).
 
