@@ -1,5 +1,8 @@
 // WarpGroup: the device-side "group of lanes" for protocol.h (one 32-wide warp per key/slot).
 #pragma once
+#include <sstream>
+
+#include "../adapm/log.h"
 #include "../adapm/protocol.h"
 
 namespace adapm {
@@ -45,5 +48,16 @@ struct LaneGroup {
       throw ::adapm::Error(_os.str());                                                          \
     }                                                                                           \
   } while (0)
+
+// Raises Kernel's dynamic shared memory limit to `bytes` on the first call in the process (a function-local static,
+// initialised once and thread-safely); a failure throws here instead of surfacing as a later launch error.
+template <auto Kernel>
+inline void set_max_dynamic_smem(int bytes) {
+  static const bool done = [bytes] {
+    ADAPM_CUDA_CHECK(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    return true;
+  }();
+  (void)done;
+}
 
 }  // namespace adapm

@@ -1,8 +1,13 @@
-// Device helpers of the warp-per-triple KGE steps (ops_transe.cu, ops_rotate.cu) and the BPR step of matrix
-// factorisation (ops_bpr.cu): float4 arithmetic, row loads into a lane's float4 registers and the three-mode AdaGrad push
-// (in place, onto a staged copy, into a fixed-point region).
+// The warp-per-positive steps with sampled negatives: the TransE and RotatE steps (ops_transe.cu, ops_rotate.cu) and the
+// BPR step of matrix factorisation (ops_bpr.cu). Device helpers (float4 arithmetic, row loads into a lane's float4
+// registers, the three-mode AdaGrad push: in place, onto a staged copy, into a fixed-point region) and the skeleton the
+// three share: the kernel's loop over positives with its fast / generic split (warp_step), the generic path
+// (step_generic) and the host side (launch_step, run_step).
 #pragma once
 #include <cuda_runtime.h>
+
+#include <algorithm>
+#include <type_traits>
 
 #include "fx_accum.cuh"
 #include "pm_kernels.cuh"
@@ -10,6 +15,8 @@
 namespace adapm {
 namespace cudaops {
 namespace kge {
+
+constexpr int kStepThreads = 256;
 
 __device__ __forceinline__ float4 f4(float v) { return make_float4(v, v, v, v); }
 __device__ __forceinline__ float4 add4(float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
@@ -54,6 +61,175 @@ __device__ __forceinline__ void push4(float* row, int d, int j, float4 g, bool s
     dev::red_row4(row + 4 * j, ue);
     dev::red_row4(row + d + 4 * j, ua);
   }
+}
+
+__device__ __forceinline__ float softplus(float x) { return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x))); }
+__device__ __forceinline__ float sigmoid(float x) {
+  const float e = expf(-fabsf(x));
+  return x >= 0.f ? 1.f / (1.f + e) : e / (1.f + e);
+}
+
+// What one positive adds to its warp's loss and counters. pushed: bit q set when negative q was pushed in place (read
+// only by rules whose negatives may push nothing, see Rule::neg_pushed).
+struct StepOut {
+  float loss;
+  unsigned upd, slow;
+  unsigned long long pushed;
+};
+
+// The positive's NP rows: store rows, nullptr (not resolved) or staged copies.
+template <int NP>
+struct Rows {
+  float* p[NP];
+};
+
+// A step has an Args struct (B, n_neg, d, neg = [B, n_neg] keys, scratch, fx_acc, fx_cidx, call_loss and its own) and
+// a Rule type with
+//   kPositives                   NP, the keys of a positive (3: s, r, o; 2: u, i)
+//   kMaxDim, kMaxNeg             the largest d and n_neg it takes
+//   positive(A, t, i)            key i of positive t
+//   state_bytes(d, n_neg)        its own per-warp shared memory; the negatives' targets follow it
+//   warp_bytes(d, n_neg)         the per-warp stride: state_bytes + n_neg targets (rounded up as the rule needs)
+//   neg_pushed(out, q)           whether negative q was pushed (then its mark follows)
+//   body<FX, GEN>(c, A, t, rows, slow, ntg, wsm, stage)
+//     one positive and its negatives on rows (slow: they are staged copies that the generic path pushes afterwards);
+//     ntg: the negatives' targets (row == nullptr: not resolved); GEN: negatives in a transitional state are staged one
+//     at a time at stage + NP * 2 d (only the out-of-line generic path calls slow_pull / slow_push; the kernel's own
+//     loop has no calls, so nothing it holds is spilled around them). It counts its negatives' pushes and stagings.
+
+// Generic path of a positive with a row in a transitional protocol state: the positive's rows are staged through
+// slow_pull into stage ((NP + 1) rows of 2 d per warp) and pushed back through slow_push, negatives one at a time. (Out
+// of line: the calls would otherwise make the kernel spill everything it holds around them.)
+template <class Rule, bool FX, class Args>
+__device__ __noinline__ StepOut step_generic(const Ctx& c, const Args& A, int t, Rows<Rule::kPositives> rows,
+                                             const dev::Target* ntg, float* wsm, float* stage) {
+  constexpr int NP = Rule::kPositives;
+  const int L = 2 * A.d;
+  bool slow = false;
+#pragma unroll
+  for (int i = 0; i < NP; ++i) slow = slow || !rows.p[i];
+  StepOut out = {0.f, 0u, 0u, 0ull};
+  if (slow) {
+    out.slow = 1;
+#pragma unroll
+    for (int i = 0; i < NP; ++i) {
+      if (!dev::slow_pull(c, Rule::positive(A, t, i), stage + i * L)) return out;
+      rows.p[i] = stage + i * L;
+    }
+  }
+  StepOut r = Rule::template body<FX, true>(c, A, t, rows, slow, ntg, wsm, stage);
+  r.slow += out.slow;
+  if (slow && !FX) {
+    bool ok = true;
+#pragma unroll
+    for (int i = 0; i < NP; ++i) ok = dev::slow_push(c, Rule::positive(A, t, i), rows.p[i]) && ok;
+    r.upd += ok ? NP : 0;
+  } else {
+    r.upd += NP;
+  }
+  return r;
+}
+
+// The kernel of a step: one warp per positive. Lanes below NP resolve the positive's keys, lane l the negatives l,
+// l + 32, ... (targets kept per warp in shared memory after the rule's state); a positive whose rows all resolved runs
+// the rule's body in place, any other the generic path. Completed pushes are marked (positives, then the negatives the
+// rule pushed). FX: one loss slot per positive; else the loss is summed into *loss_out. stats: flush_stats.
+template <class Rule, bool FX, class Args>
+__device__ __forceinline__ void warp_step(const Ctx& c, const Args& A, float* loss_out, unsigned long long* stats) {
+  constexpr int NP = Rule::kPositives;
+  dev::cta_enter(c);
+  const int lane = threadIdx.x & 31;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  extern __shared__ float4 step_smem[];
+  unsigned char* const wbase =
+      reinterpret_cast<unsigned char*>(step_smem) + (size_t)(threadIdx.x >> 5) * Rule::warp_bytes(A.d, A.n_neg);
+  float* const wsm = reinterpret_cast<float*>(wbase);
+  dev::Target* const ntg = reinterpret_cast<dev::Target*>(wbase + Rule::state_bytes(A.d, A.n_neg));
+  float loss_acc = 0.f;
+  unsigned n_local = 0, n_remote = 0, n_slow = 0, n_upd = 0;
+
+  for (int t = warp; t < A.B; t += nwarps) {
+    dev::Target tg;
+    tg.row = nullptr; tg.version = nullptr; tg.flag = nullptr;
+    if (lane < NP) {
+      const Key k = Rule::positive(A, t, lane);
+      tg = dev::resolve_fast(c, k, class_of_key(c, k), &n_local, &n_remote);
+    }
+    bool ok = lane >= NP || tg.row;
+    for (int q = lane; q < A.n_neg; q += 32) {
+      const Key k = A.neg[(size_t)t * A.n_neg + q];
+      const dev::Target nt = dev::resolve_fast(c, k, class_of_key(c, k), &n_local, &n_remote);
+      ntg[q] = nt;
+      ok = ok && nt.row;
+    }
+    __syncwarp();
+    Rows<NP> rows;
+#pragma unroll
+    for (int i = 0; i < NP; ++i) rows.p[i] = (float*)__shfl_sync(0xffffffffu, (unsigned long long)tg.row, i);
+    StepOut r;
+    if (__all_sync(0xffffffffu, ok)) {
+      r = Rule::template body<FX, false>(c, A, t, rows, false, ntg, wsm, nullptr);
+      if (lane < NP) dev::mark_pushed(tg);
+      r.upd += NP;
+    } else {
+      r = step_generic<Rule, FX>(c, A, t, rows, ntg, wsm, A.scratch + (size_t)warp * (NP + 1) * 2 * A.d);
+      bool resolved = true;   // the positive's rows were pushed in place
+#pragma unroll
+      for (int i = 0; i < NP; ++i) resolved = resolved && rows.p[i];
+      if (lane < NP && resolved) dev::mark_pushed(tg);
+    }
+    for (int q = lane; q < A.n_neg; q += 32)
+      if (ntg[q].row && Rule::neg_pushed(r, q)) dev::mark_pushed(ntg[q]);
+    __syncwarp();
+    n_upd += r.upd;
+    n_slow += r.slow;
+    if (FX) { if (lane == 0) A.call_loss[t] = r.loss; }
+    else loss_acc += r.loss;
+  }
+
+  __syncwarp();
+  if (!FX && lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
+  dev::flush_stats(stats, n_local, n_remote, n_slow, n_upd);
+  dev::cta_exit(c);
+}
+
+// Launches Kernel, a warp_step over Rule, with the rule's per-warp shared memory (the limit is raised once, to the
+// layout at the rule's largest shape).
+template <class Rule, auto Kernel, class Args>
+void launch_step(cudaStream_t stream, int blocks, const Ctx& c, const Args& A, float* loss_out,
+                 unsigned long long* stats) {
+  set_max_dynamic_smem<Kernel>((int)(kStepThreads / 32 * Rule::warp_bytes(Rule::kMaxDim, Rule::kMaxNeg)));
+  Kernel<<<blocks, kStepThreads, kStepThreads / 32 * Rule::warp_bytes(A.d, A.n_neg), stream>>>(c, A, loss_out, stats);
+}
+
+// Host side of a step with NP keys per positive (A filled but for scratch and the FX fields): float32 rows,
+// min(ceil(B / 8), 4 per SM) CTAs, the generic path's scratch ((NP + 1) rows of 2 d per warp in the backend's last step
+// buffer, which the steps share and never use concurrently on one stream), then launch(fx, blocks, loss_out) with
+// fx = std::false_type (in place) or, deterministic (one GPU, start-of-step reads), std::true_type between fx::begin
+// over src (regions in units of `unit` values) and fx::apply with the rule's scales.
+template <int NP, class Args, class Launch>
+void run_step(CudaBackend& be, cudaStream_t stream, Args& A, bool deterministic, const fx::Source* src, int n_src,
+              int unit, float fx_val, float fx_ada, float* loss_out, Launch&& launch) {
+  ADAPM_CHECK(be.ctx().L.val_bytes == 4, "the fused ops need float32 rows (Options::dtype)");
+  be.track_stream(stream);
+  const int warps_per_block = kStepThreads / 32;
+  const int blocks = std::min((A.B + warps_per_block - 1) / warps_per_block, be.num_sms() * 4);
+  A.scratch = static_cast<float*>(be.step_buffer(
+      CudaBackend::kStepBuffers - 1, (size_t)blocks * warps_per_block * (NP + 1) * 2 * (size_t)A.d * sizeof(float)));
+  A.fx_acc = nullptr; A.fx_cidx = nullptr; A.call_loss = nullptr;
+  if (deterministic) {
+    CudaBackend::FxScratch& fxs = fx::begin(be, stream, src, n_src, unit, A.B);
+    A.fx_acc = fxs.acc; A.fx_cidx = fxs.cidx; A.call_loss = fxs.call_loss;
+    launch(std::true_type{}, blocks, nullptr);
+    ADAPM_COUNT_LAUNCH();
+    ADAPM_CUDA_CHECK(cudaGetLastError());
+    fx::apply(be, stream, unit, fx_val, fx_ada, 0.f, A.B, loss_out);
+    return;
+  }
+  launch(std::false_type{}, blocks, loss_out);
+  ADAPM_COUNT_LAUNCH();
+  ADAPM_CUDA_CHECK(cudaGetLastError());
 }
 
 }  // namespace kge

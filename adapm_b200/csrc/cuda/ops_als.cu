@@ -371,21 +371,14 @@ __global__ void als_gram_reduce_kernel(const float* __restrict__ part, int npart
 }
 
 template <int KP>
-void set_smem(const void* fn) {
-  ADAPM_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Smem<KP>::bytes()));
-}
-
-template <int KP>
 void launch_solve(cudaStream_t stream, int n, const Ctx& c, const SolveArgs& A, unsigned long long* stats) {
-  static bool attr_set = false;
-  if (!attr_set) { set_smem<KP>((const void*)als_solve_kernel<KP>); attr_set = true; }
+  set_max_dynamic_smem<als_solve_kernel<KP>>((int)Smem<KP>::bytes());
   als_solve_kernel<KP><<<n, kThreads, Smem<KP>::bytes(), stream>>>(c, A, stats);
 }
 
 template <int KP>
 void launch_gram(cudaStream_t stream, int blocks, const Ctx& c, const Key* keys, int64_t n, int rank, float* part) {
-  static bool attr_set = false;
-  if (!attr_set) { set_smem<KP>((const void*)als_gram_kernel<KP>); attr_set = true; }
+  set_max_dynamic_smem<als_gram_kernel<KP>>((int)Smem<KP>::bytes());
   als_gram_kernel<KP><<<blocks, kThreads, Smem<KP>::bytes(), stream>>>(c, keys, n, rank, part);
 }
 

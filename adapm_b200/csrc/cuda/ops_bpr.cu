@@ -35,11 +35,6 @@ namespace {
 
 using namespace kge;
 
-constexpr int kThreads = 256;
-// the backend's step buffer that holds the generic path's staged rows (shared with the KGE steps, never concurrently on
-// one stream)
-constexpr int kScratchBuf = CudaBackend::kStepBuffers - 1;
-
 // Fixed-point scales of the deterministic mode. |value update| <= eps per push (AdaGrad normalises it): 2^40 leaves
 // 2^23 / eps pushes per element and step. One push's gradient is bounded by the factors: c_j <= 1, so an element of g_j
 // is at most |w_u| + lam |h_j|, of g_i at most n |w_u| + lam |h_i| and of g_u at most 2 n max|h| + lam |w_u|. The AdaGrad
@@ -49,12 +44,6 @@ constexpr int kScratchBuf = CudaBackend::kStepBuffers - 1;
 constexpr float kFxVal = 1099511627776.f;     // 2^40
 constexpr float kFxAda = 268435456.f;         // 2^28
 constexpr float kFxAdaMax = 16777216.f;       // 2^24
-
-__device__ __forceinline__ float softplus(float x) { return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x))); }
-__device__ __forceinline__ float sigmoid(float x) {
-  const float e = expf(-fabsf(x));
-  return x >= 0.f ? 1.f / (1.f + e) : e / (1.f + e);
-}
 
 template <int VPL>
 __device__ __forceinline__ float dot(const float4 (&a)[VPL], const float4 (&b)[VPL]) {
@@ -68,7 +57,7 @@ struct Args {
   const Key* users;
   const Key* pos;
   const Key* neg;              // [B, n_neg] item keys
-  int B, n_neg, rank;
+  int B, n_neg, d;             // d: the rank
   float eps, lam;
   float* scratch;              // generic path: 3 rows per warp
   long long* fx_acc;           // FX: fixed-point regions, per-positive loss slots
@@ -76,21 +65,31 @@ struct Args {
   float* call_loss;
 };
 
-struct PosOut {
-  float loss;
-  unsigned upd, slow;
+// The step as a warp_step rule (kge_step.cuh): positive (u, i), targets only in shared memory.
+template <int VPL>
+struct Bpr {
+  static constexpr int kPositives = 2, kMaxDim = kBprMaxRank, kMaxNeg = kBprMaxNeg;
+  static __device__ __forceinline__ Key positive(const Args& A, int t, int i) { return i == 0 ? A.users[t] : A.pos[t]; }
+  static __host__ __device__ __forceinline__ size_t state_bytes(int, int) { return 0; }
+  static __host__ __device__ __forceinline__ size_t warp_bytes(int, int n_neg) {
+    return (size_t)n_neg * sizeof(dev::Target);
+  }
+  static __device__ __forceinline__ bool neg_pushed(const StepOut&, int) { return true; }
+  template <bool FX, bool GEN>
+  static __device__ StepOut body(const Ctx& c, const Args& A, int t, const Rows<2>& rows, bool slow,
+                                 const dev::Target* ntg, float* wsm, float* my_scratch);
 };
 
-// One positive and its negatives. pu / pi: the positive's rows, or (slow) their staged copies in global scratch that are
-// pushed through the generic path afterwards. ntg: the negatives' targets (row == nullptr: not resolved). GEN: negatives
-// in a transitional state are staged one at a time (only the out-of-line generic path calls slow_pull / slow_push; the
-// kernel's own loop has no calls, so nothing it holds is spilled around them).
-template <int VPL, bool FX, bool GEN>
-__device__ __forceinline__ PosOut positive_body(const Ctx& c, const Args& A, int t, float* pu, float* pi, bool slow,
-                                                const dev::Target* ntg, float* my_scratch) {
+// One positive and its negatives: pu / pi the positive's rows.
+template <int VPL>
+template <bool FX, bool GEN>
+__device__ __forceinline__ StepOut Bpr<VPL>::body(const Ctx& c, const Args& A, int t, const Rows<2>& rows, bool slow,
+                                                  const dev::Target* ntg, float*, float* my_scratch) {
   const int lane = threadIdx.x & 31;
-  const int rank = A.rank, nv = rank >> 2, n_neg = A.n_neg;
-  PosOut out = {0.f, 0u, 0u};
+  const int rank = A.d, nv = rank >> 2, n_neg = A.n_neg;
+  float* const pu = rows.p[0];
+  float* const pi = rows.p[1];
+  StepOut out = {0.f, 0u, 0u, 0ull};
   float4 w[VPL], h[VPL], s[VPL], e[VPL];
   load_row<VPL>(pu, nv, lane, w);
   load_row<VPL>(pi, nv, lane, h);
@@ -148,119 +147,21 @@ __device__ __forceinline__ PosOut positive_body(const Ctx& c, const Args& A, int
   return out;
 }
 
-// Generic path of a positive with a row in a transitional protocol state: the positive's rows are staged through
-// slow_pull (and pushed back through slow_push), negatives one at a time. (Out of line: the calls would otherwise make
-// the kernel spill everything it holds around them.)
 template <int VPL, bool FX>
-__device__ __noinline__ PosOut positive_generic(const Ctx& c, const Args& A, int t, float* pu, float* pi,
-                                                const dev::Target* ntg, float* my_scratch) {
-  const int L = 2 * A.rank;
-  const bool slow = !pu || !pi;
-  PosOut out = {0.f, 0u, 0u};
-  const Key ku = A.users[t], ki = A.pos[t];
-  if (slow) {
-    out.slow = 1;
-    if (!dev::slow_pull(c, ku, my_scratch) || !dev::slow_pull(c, ki, my_scratch + L)) return out;
-    pu = my_scratch; pi = my_scratch + L;
-  }
-  PosOut r = positive_body<VPL, FX, true>(c, A, t, pu, pi, slow, ntg, my_scratch);
-  r.slow += out.slow;
-  if (slow && !FX) {
-    bool ok = dev::slow_push(c, ku, pu);
-    ok = dev::slow_push(c, ki, pi) && ok;
-    r.upd += ok ? 2 : 0;
-  } else {
-    r.upd += 2;
-  }
-  return r;
-}
-
-template <int VPL, bool FX>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kStepThreads, 1)
 mf_bpr_step_kernel(const __grid_constant__ Ctx c, const __grid_constant__ Args A, float* __restrict__ loss_out,
                    unsigned long long* __restrict__ stats) {
-  dev::cta_enter(c);
-  const int lane = threadIdx.x & 31;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  extern __shared__ float4 bpr_smem[];
-  dev::Target* const ntg = reinterpret_cast<dev::Target*>(bpr_smem) + (size_t)(threadIdx.x >> 5) * A.n_neg;
-  float loss_acc = 0.f;
-  unsigned n_local = 0, n_remote = 0, n_slow = 0, n_upd = 0;
-
-  for (int t = warp; t < A.B; t += nwarps) {
-    // lanes 0 and 1 resolve u and i; lane l resolves negatives l, l + 32, ...
-    dev::Target tg;
-    tg.row = nullptr; tg.version = nullptr; tg.flag = nullptr;
-    if (lane < 2) {
-      const Key k = lane == 0 ? A.users[t] : A.pos[t];
-      tg = dev::resolve_fast(c, k, class_of_key(c, k), &n_local, &n_remote);
-    }
-    bool ok = lane >= 2 || tg.row;
-    for (int q = lane; q < A.n_neg; q += 32) {
-      const Key k = A.neg[(size_t)t * A.n_neg + q];
-      const dev::Target nt = dev::resolve_fast(c, k, class_of_key(c, k), &n_local, &n_remote);
-      ntg[q] = nt;
-      ok = ok && nt.row;
-    }
-    __syncwarp();
-    float* pu = (float*)__shfl_sync(0xffffffffu, (unsigned long long)tg.row, 0);
-    float* pi = (float*)__shfl_sync(0xffffffffu, (unsigned long long)tg.row, 1);
-    PosOut r;
-    if (__all_sync(0xffffffffu, ok)) {
-      r = positive_body<VPL, FX, false>(c, A, t, pu, pi, false, ntg, nullptr);
-      if (lane < 2) dev::mark_pushed(tg);
-      r.upd += 2;
-    } else {
-      r = positive_generic<VPL, FX>(c, A, t, pu, pi, ntg, A.scratch + (size_t)warp * 6 * A.rank);
-      if (lane < 2 && pu && pi) dev::mark_pushed(tg);
-    }
-    for (int q = lane; q < A.n_neg; q += 32)
-      if (ntg[q].row) dev::mark_pushed(ntg[q]);
-    __syncwarp();
-    n_upd += r.upd;
-    n_slow += r.slow;
-    if (FX) { if (lane == 0) A.call_loss[t] = r.loss; }
-    else loss_acc += r.loss;
-  }
-
-  __syncwarp();
-  if (!FX && lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
-  unsigned sl = n_local, sr = n_remote;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    sl += __shfl_xor_sync(0xffffffffu, sl, o);
-    sr += __shfl_xor_sync(0xffffffffu, sr, o);
-  }
-  if (lane == 0 && stats) {
-    if (sl) atomicAdd(stats + 0, (unsigned long long)sl);
-    if (sr) atomicAdd(stats + 1, (unsigned long long)sr);
-    if (n_slow) atomicAdd(stats + 2, (unsigned long long)n_slow);
-    if (n_upd) atomicAdd(stats + 3, (unsigned long long)n_upd);
-  }
-  dev::cta_exit(c);
-}
-
-template <int VPL, bool FX>
-void launch(cudaStream_t stream, int blocks, const Ctx& c, const Args& A, float* loss_out, unsigned long long* stats) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    ADAPM_CUDA_CHECK(cudaFuncSetAttribute(mf_bpr_step_kernel<VPL, FX>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)(kThreads / 32 * kBprMaxNeg * sizeof(dev::Target))));
-    attr_set = true;
-  }
-  mf_bpr_step_kernel<VPL, FX><<<blocks, kThreads, kThreads / 32 * A.n_neg * sizeof(dev::Target), stream>>>(c, A, loss_out,
-                                                                                                          stats);
+  warp_step<Bpr<VPL>, FX>(c, A, loss_out, stats);
 }
 
 template <bool FX>
 void launch_shape(int vpl, cudaStream_t stream, int blocks, const Ctx& c, const Args& A, float* loss_out,
                   unsigned long long* stats) {
   switch (vpl) {
-    case 1: launch<1, FX>(stream, blocks, c, A, loss_out, stats); break;
-    case 2: launch<2, FX>(stream, blocks, c, A, loss_out, stats); break;
-    case 3: launch<3, FX>(stream, blocks, c, A, loss_out, stats); break;
-    default: launch<4, FX>(stream, blocks, c, A, loss_out, stats); break;
+    case 1: launch_step<Bpr<1>, mf_bpr_step_kernel<1, FX>>(stream, blocks, c, A, loss_out, stats); break;
+    case 2: launch_step<Bpr<2>, mf_bpr_step_kernel<2, FX>>(stream, blocks, c, A, loss_out, stats); break;
+    case 3: launch_step<Bpr<3>, mf_bpr_step_kernel<3, FX>>(stream, blocks, c, A, loss_out, stats); break;
+    default: launch_step<Bpr<4>, mf_bpr_step_kernel<4, FX>>(stream, blocks, c, A, loss_out, stats); break;
   }
 }
 
@@ -273,33 +174,15 @@ void mf_bpr_step(CudaBackend& be, cudaStream_t stream, const Key* users, const K
               "mf_bpr_step: rank must be a multiple of 4 in [4, " << kBprMaxRank << "]");
   ADAPM_CHECK(n_neg >= 1 && n_neg <= kBprMaxNeg, "mf_bpr_step: the negatives per positive must be in [1, " << kBprMaxNeg
                                                                                                             << "]");
-  ADAPM_CHECK(be.ctx().L.val_bytes == 4, "the fused ops need float32 rows (Options::dtype)");
-  be.track_stream(stream);
-  const Ctx& c = be.ctx();
-  const int warps_per_block = kThreads / 32;
-  const int blocks = std::min((B + warps_per_block - 1) / warps_per_block, be.num_sms() * 4);
-  // generic-path scratch (rows in a transitional protocol state): three rows of 2 rank per warp
-  float* scratch = static_cast<float*>(
-      be.step_buffer(kScratchBuf, (size_t)blocks * warps_per_block * 6 * (size_t)rank * sizeof(float)));
   const int vpl = (rank / 4 + 31) / 32;
   Args A;
-  A.users = users; A.pos = pos; A.neg = neg; A.B = B; A.n_neg = n_neg; A.rank = rank;
-  A.eps = eps; A.lam = lam; A.scratch = scratch;
-  A.fx_acc = nullptr; A.fx_cidx = nullptr; A.call_loss = nullptr;
-  if (deterministic) {
-    // one GPU, start-of-step reads: every key (user or item, both 2 rank long) gets a [rank | rank] region
-    const fx::Source src[3] = {{users, B, 1}, {pos, B, 1}, {neg, (long)B * n_neg, 1}};
-    CudaBackend::FxScratch& fxs = fx::begin(be, stream, src, 3, 2 * rank, B);
-    A.fx_acc = fxs.acc; A.fx_cidx = fxs.cidx; A.call_loss = fxs.call_loss;
-    launch_shape<true>(vpl, stream, blocks, c, A, nullptr, stats);
-    ADAPM_COUNT_LAUNCH();
-    ADAPM_CUDA_CHECK(cudaGetLastError());
-    fx::apply(be, stream, 2 * rank, kFxVal, kFxAda, 0.f, B, loss_out);
-    return;
-  }
-  launch_shape<false>(vpl, stream, blocks, c, A, loss_out, stats);
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_CUDA_CHECK(cudaGetLastError());
+  A.users = users; A.pos = pos; A.neg = neg; A.B = B; A.n_neg = n_neg; A.d = rank;
+  A.eps = eps; A.lam = lam;
+  // deterministic: every key (user or item, both 2 rank long) gets a [rank | rank] region
+  const fx::Source src[3] = {{users, B, 1}, {pos, B, 1}, {neg, (long)B * n_neg, 1}};
+  run_step<2>(be, stream, A, deterministic, src, 3, 2 * rank, kFxVal, kFxAda, loss_out, [&](auto fx, int blocks, float* lo) {
+    launch_shape<decltype(fx)::value>(vpl, stream, blocks, be.ctx(), A, lo, stats);
+  });
 }
 
 }  // namespace cudaops

@@ -360,18 +360,7 @@ cbow_step_body(const Ctx& c, const Key* __restrict__ centers, const Key* __restr
   __syncwarp();
   if (SCORE && lane == 0) atomicAdd(fx_loss, (unsigned long long)__float2ll_rn(loss_acc * kFxLoss));
   else if (lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
-  unsigned sum_local = n_local, sum_remote = n_remote;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    sum_local += __shfl_xor_sync(0xffffffffu, sum_local, o);
-    sum_remote += __shfl_xor_sync(0xffffffffu, sum_remote, o);
-  }
-  if (lane == 0 && stats) {
-    if (sum_local) atomicAdd(stats + 0, (unsigned long long)sum_local);
-    if (sum_remote) atomicAdd(stats + 1, (unsigned long long)sum_remote);
-    if (n_slow) atomicAdd(stats + 2, (unsigned long long)n_slow);
-    if (n_upd) atomicAdd(stats + 3, (unsigned long long)n_upd);
-  }
+  dev::flush_stats(stats, n_local, n_remote, n_slow, n_upd);
   dev::cta_exit(c);
 }
 
@@ -492,12 +481,7 @@ void cbow_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   ADAPM_COUNT_LAUNCH();
 #define ADAPM_LAUNCH_CBOW_SCORE(V)                                                                          \
   do {                                                                                                      \
-    static bool attr_set = false;                                                                           \
-    if (!attr_set) {                                                                                        \
-      ADAPM_CUDA_CHECK(                                                                                     \
-          cudaFuncSetAttribute(cbow_score_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024)); \
-      attr_set = true;                                                                                      \
-    }                                                                                                       \
+    set_max_dynamic_smem<cbow_score_kernel<V>>(110 * 1024);                                                 \
     cbow_score_kernel<V><<<score_blocks, kThreads, smem, stream>>>(c, centers, contexts, negatives, n_win, nc, neg, \
                                                                    d, stats, fx.loss, so);                  \
   } while (0)
@@ -544,12 +528,7 @@ void cbow_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const K
   }
 #define ADAPM_LAUNCH_CBOW(V)                                                                                \
   do {                                                                                                      \
-    static bool attr_set = false;                                                                           \
-    if (!attr_set) {                                                                                        \
-      ADAPM_CUDA_CHECK(                                                                                     \
-          cudaFuncSetAttribute(cbow_step_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024)); \
-      attr_set = true;                                                                                      \
-    }                                                                                                       \
+    set_max_dynamic_smem<cbow_step_kernel<V>>(110 * 1024);                                                  \
     cbow_step_kernel<V><<<blocks, kThreads, smem, stream>>>(c, centers, contexts, negatives, n_win, nc, neg, d,     \
                                                             alpha, loss_out, stats);                        \
   } while (0)

@@ -462,14 +462,9 @@ void gather_dist_topk(CudaBackend& be, cudaStream_t stream, const float* q, cons
   a.k = k; a.part_v = part_v; a.part_c = part_c;
   be.track_stream(stream);
   const size_t smem = sizeof(DistSmem) + sizeof(TopkLists);
-  static bool attr_set = false;
-  if (!attr_set) {
-    ADAPM_CUDA_CHECK(cudaFuncSetAttribute(dist_topk_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    ADAPM_CUDA_CHECK(cudaFuncSetAttribute(dist_topk_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    ADAPM_CUDA_CHECK(
-        cudaFuncSetAttribute(cdist_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  set_max_dynamic_smem<dist_topk_kernel<1>>((int)smem);
+  set_max_dynamic_smem<dist_topk_kernel<2>>((int)smem);
+  set_max_dynamic_smem<cdist_topk_kernel>((int)smem);
   const dim3 grid((M + DB - 1) / DB, S);
   if (p == 1) dist_topk_kernel<1><<<grid, kDistThreads, smem, stream>>>(be.ctx(), a, stats);
   else if (p == 2) dist_topk_kernel<2><<<grid, kDistThreads, smem, stream>>>(be.ctx(), a, stats);

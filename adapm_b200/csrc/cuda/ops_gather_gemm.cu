@@ -134,11 +134,7 @@ void launch_gather(CudaBackend& be, cudaStream_t stream, const void* Q, const Ke
   be.track_stream(stream);
   CUtensorMap mq = make_map(Q, M, ldq, BM, KIND_BF16);
   const size_t smem = sizeof(SmemLayout) + 1024;
-  static bool attr_set = false;
-  if (!attr_set) {
-    ADAPM_CUDA_CHECK(cudaFuncSetAttribute(gather_gemm_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  set_max_dynamic_smem<gather_gemm_kernel<EPI>>((int)smem);
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
   gather_gemm_kernel<EPI><<<grid, kGemmThreads, smem, stream>>>(mq, be.ctx(), keys, M, N, K, C, ldc, true_score, true_col,
                                                                   rank_out, stats);

@@ -274,18 +274,7 @@ kge_step_body(const Ctx& c, const Key* __restrict__ subj, const Key* __restrict_
 
   __syncwarp();
   if (!FX && lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
-  unsigned sl = n_local, sr = n_remote;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    sl += __shfl_xor_sync(0xffffffffu, sl, o);
-    sr += __shfl_xor_sync(0xffffffffu, sr, o);
-  }
-  if (lane == 0 && stats) {
-    if (sl) atomicAdd(stats + 0, (unsigned long long)sl);
-    if (sr) atomicAdd(stats + 1, (unsigned long long)sr);
-    if (n_slow) atomicAdd(stats + 2, (unsigned long long)n_slow);
-    if (n_upd) atomicAdd(stats + 3, (unsigned long long)n_upd);
-  }
+  dev::flush_stats(stats, n_local, n_remote, n_slow, n_upd);
   dev::cta_exit(c);
 }
 
@@ -497,18 +486,7 @@ kge_rescal_body(const Ctx& c, const Key* __restrict__ subj, const Key* __restric
 
   __syncwarp();
   if (!FX && lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
-  unsigned sl = n_local, sr = n_remote;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    sl += __shfl_xor_sync(0xffffffffu, sl, o);
-    sr += __shfl_xor_sync(0xffffffffu, sr, o);
-  }
-  if (lane == 0 && stats) {
-    if (sl) atomicAdd(stats + 0, (unsigned long long)sl);
-    if (sr) atomicAdd(stats + 1, (unsigned long long)sr);
-    if (n_slow) atomicAdd(stats + 2, (unsigned long long)n_slow);
-    if (n_upd) atomicAdd(stats + 3, (unsigned long long)n_upd);
-  }
+  dev::flush_stats(stats, n_local, n_remote, n_slow, n_upd);
   dev::cta_exit(c);
 }
 
@@ -561,21 +539,13 @@ void kge_complex_step(CudaBackend& be, cudaStream_t stream, const Key* subj, con
   if (vplh > 2) vplh = 0;
 #define ADAPM_LAUNCH_KGE(V)                                                                                    \
   do {                                                                                                         \
-    static bool attr_set = false;                                                                              \
-    if (!attr_set) {                                                                                           \
-      cudaFuncSetAttribute(kge_step_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);       \
-      attr_set = true;                                                                                         \
-    }                                                                                                          \
+    set_max_dynamic_smem<kge_step_kernel<V>>(200 * 1024);                                                      \
     kge_step_kernel<V><<<blocks, kThreads, smem, stream>>>(c, subj, rel, obj, labels, n_calls, nh, eta,        \
                                                            gamma_e, gamma_r, loss_out, stats, de, dr);         \
   } while (0)
 #define ADAPM_LAUNCH_KGE_FX(V)                                                                                 \
   do {                                                                                                         \
-    static bool attr_set = false;                                                                              \
-    if (!attr_set) {                                                                                           \
-      cudaFuncSetAttribute(kge_step_fx_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);    \
-      attr_set = true;                                                                                         \
-    }                                                                                                          \
+    set_max_dynamic_smem<kge_step_fx_kernel<V>>(200 * 1024);                                                   \
     kge_step_fx_kernel<V><<<blocks, kThreads, smem, stream>>>(c, subj, rel, obj, labels, n_calls, nh, eta,     \
                                                               gamma_e, gamma_r, stats, de, dr, fxs->acc,       \
                                                               fxs->cidx, fxs->call_loss);                      \

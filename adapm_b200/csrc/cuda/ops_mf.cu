@@ -157,18 +157,7 @@ mf_step_body(const Ctx& c, const Key* __restrict__ row_keys, const Key* __restri
   }
   __syncwarp();
   if (!FX && lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
-  unsigned sl = n_local, sr = n_remote;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    sl += __shfl_xor_sync(0xffffffffu, sl, o);
-    sr += __shfl_xor_sync(0xffffffffu, sr, o);
-  }
-  if (lane == 0 && stats) {
-    if (sl) atomicAdd(stats + 0, (unsigned long long)sl);
-    if (sr) atomicAdd(stats + 1, (unsigned long long)sr);
-    if (n_slow) atomicAdd(stats + 2, (unsigned long long)n_slow);
-    if (n_upd) atomicAdd(stats + 3, (unsigned long long)n_upd);
-  }
+  dev::flush_stats(stats, n_local, n_remote, n_slow, n_upd);
   dev::cta_exit(c);
 }
 
@@ -208,21 +197,13 @@ void mf_step(CudaBackend& be, cudaStream_t stream, const Key* row_keys, const Ke
   if (vpl > 2) vpl = 0;
 #define ADAPM_LAUNCH_MF(V)                                                                                   \
   do {                                                                                                       \
-    static bool attr_set = false;                                                                            \
-    if (!attr_set) {                                                                                         \
-      cudaFuncSetAttribute(mf_step_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);       \
-      attr_set = true;                                                                                       \
-    }                                                                                                        \
+    set_max_dynamic_smem<mf_step_kernel<V>>(96 * 1024);                                                      \
     mf_step_kernel<V><<<blocks, kThreads, smem, stream>>>(c, row_keys, col_keys, xs, row_nnz, col_nnz, n, rank, eps, \
                                                           lambda, loss_out, stats);                          \
   } while (0)
 #define ADAPM_LAUNCH_MF_FX(V)                                                                                \
   do {                                                                                                       \
-    static bool attr_set = false;                                                                            \
-    if (!attr_set) {                                                                                         \
-      cudaFuncSetAttribute(mf_step_fx_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);    \
-      attr_set = true;                                                                                       \
-    }                                                                                                        \
+    set_max_dynamic_smem<mf_step_fx_kernel<V>>(96 * 1024);                                                   \
     mf_step_fx_kernel<V><<<blocks, kThreads, smem, stream>>>(c, row_keys, col_keys, xs, row_nnz, col_nnz, n, rank, \
                                                              eps, lambda, stats, fxs.acc, fxs.cidx,          \
                                                              fxs.call_loss);                                 \

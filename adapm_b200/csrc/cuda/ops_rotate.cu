@@ -42,11 +42,6 @@ namespace {
 
 using namespace kge;
 
-constexpr int kThreads = 256;
-// the backend's step buffer that holds the generic path's staged rows (shared with the TransE step, never concurrently
-// on one stream)
-constexpr int kScratchBuf = CudaBackend::kStepBuffers - 1;
-
 // Fixed-point scales of the deterministic mode. |value update| <= eta per push (AdaGrad normalises it): 2^40 leaves
 // 2^23 / eta pushes per element and step. One push's gradient is bounded by the model: an entity element gets at most
 // 1 (positive) + 1/2 (the weights of a side sum to 1) from the distance terms plus gamma_e |e|, a phase at most
@@ -87,11 +82,6 @@ __device__ __forceinline__ float cabs2(float4 x, float4& u) {
 // dD/dtheta of the two values for x = p - b, p = a o rho: -Im(conj(u) p) = u_im p_re - u_re p_im
 __device__ __forceinline__ float2 dtheta(float4 u, float4 p) {
   return make_float2(u.y * p.x - u.x * p.y, u.w * p.z - u.z * p.w);
-}
-__device__ __forceinline__ float softplus(float x) { return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x))); }
-__device__ __forceinline__ float sigmoid(float x) {
-  const float e = expf(-fabsf(x));
-  return x >= 0.f ? 1.f / (1.f + e) : e / (1.f + e);
 }
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
@@ -134,28 +124,37 @@ struct Args {
   float* call_loss;
 };
 
-struct TripleOut {
-  float loss;
-  unsigned upd, slow;
+// The step as a warp_step rule (kge_step.cuh): positive (s, r, o). Per-warp shared memory: s o rho | o | (cos, sin) |
+// g_s | g_o (d each) | g_theta (m) | distance / dL/dD of every negative (n_neg) | the negatives' targets.
+template <int VPL>
+struct RotatE {
+  static constexpr int kPositives = 3, kMaxDim = kRotatEMaxDim, kMaxNeg = kRotatEMaxNeg;
+  static __device__ __forceinline__ Key positive(const Args& A, int t, int i) {
+    return i == 0 ? A.subj[t] : (i == 1 ? A.rel[t] : A.obj[t]);
+  }
+  static __host__ __device__ __forceinline__ size_t state_bytes(int d, int n_neg) {
+    return (size_t)((5 * d + d / 2 + n_neg + 3) & ~3) * sizeof(float);
+  }
+  static __host__ __device__ __forceinline__ size_t warp_bytes(int d, int n_neg) {
+    return (state_bytes(d, n_neg) + (size_t)n_neg * sizeof(dev::Target) + 15) & ~(size_t)15;
+  }
+  static __device__ __forceinline__ bool neg_pushed(const StepOut&, int) { return true; }
+  template <bool FX, bool GEN>
+  static __device__ StepOut body(const Ctx& c, const Args& A, int t, const Rows<3>& rows, bool slow,
+                                 const dev::Target* ntg, float* wsm, float* my_scratch);
 };
 
-// per-warp shared memory: s o rho | o | (cos, sin) | g_s | g_o (d each) | g_theta (m) | distance / dL/dD of every
-// negative (n_neg) | the negatives' targets
-__host__ __device__ __forceinline__ int warp_floats(int d, int n_neg) { return (5 * d + d / 2 + n_neg + 3) & ~3; }
-__host__ __device__ __forceinline__ size_t warp_bytes(int d, int n_neg) {
-  return ((size_t)warp_floats(d, n_neg) * sizeof(float) + (size_t)n_neg * sizeof(dev::Target) + 15) & ~(size_t)15;
-}
-
-// One positive triple and its negatives. ps / pr / po: the positive's rows, or (slow) their staged copies in global
-// scratch that are pushed through the generic path afterwards. ntg: the negatives' targets (row == nullptr: not
-// resolved). GEN: negatives in a transitional state are staged one at a time (only the out-of-line generic path calls
-// slow_pull / slow_push; the kernel's own loop has no calls, so nothing it holds is spilled around them).
-template <int VPL, bool FX, bool GEN>
-__device__ __forceinline__ TripleOut triple_body(const Ctx& c, const Args& A, int t, float* ps, float* pr, float* po,
-                                                 bool slow, const dev::Target* ntg, float* wsm, float* my_scratch) {
+// One positive triple and its negatives: ps / pr / po the positive's rows.
+template <int VPL>
+template <bool FX, bool GEN>
+__device__ __forceinline__ StepOut RotatE<VPL>::body(const Ctx& c, const Args& A, int t, const Rows<3>& rows, bool slow,
+                                                     const dev::Target* ntg, float* wsm, float* my_scratch) {
   const int lane = threadIdx.x & 31;
   const int d = A.d, m = d >> 1, nv = d >> 2, L = 2 * d, n_neg = A.n_neg, half = n_neg >> 1;
-  TripleOut out = {0.f, 0u, 0u};
+  float* const ps = rows.p[0];
+  float* const pr = rows.p[1];
+  float* const po = rows.p[2];
+  StepOut out = {0.f, 0u, 0u, 0ull};
   float* const sa = wsm; float* const so = wsm + d; float* const scs = wsm + 2 * d;
   float* const sgs = wsm + 3 * d; float* const sgo = wsm + 4 * d; float* const sgt = wsm + 5 * d;
   float* const swq = sgt + m;
@@ -304,126 +303,21 @@ __device__ __forceinline__ TripleOut triple_body(const Ctx& c, const Args& A, in
   return out;
 }
 
-// Generic path of a triple with a row in a transitional protocol state: the positive's rows are staged through
-// slow_pull (and pushed back through slow_push), negatives one at a time. (Out of line: the calls would otherwise make
-// the kernel spill everything it holds around them.)
 template <int VPL, bool FX>
-__device__ __noinline__ TripleOut triple_generic(const Ctx& c, const Args& A, int t, float* ps, float* pr, float* po,
-                                                 const dev::Target* ntg, float* wsm, float* my_scratch) {
-  const int L = 2 * A.d;
-  const bool slow = !ps || !pr || !po;
-  TripleOut out = {0.f, 0u, 0u};
-  const Key ks = A.subj[t], kr = A.rel[t], ko = A.obj[t];
-  if (slow) {
-    out.slow = 1;
-    if (!dev::slow_pull(c, ks, my_scratch) || !dev::slow_pull(c, kr, my_scratch + L) ||
-        !dev::slow_pull(c, ko, my_scratch + 2 * L))
-      return out;
-    ps = my_scratch; pr = my_scratch + L; po = my_scratch + 2 * L;
-  }
-  TripleOut r = triple_body<VPL, FX, true>(c, A, t, ps, pr, po, slow, ntg, wsm, my_scratch);
-  r.slow += out.slow;
-  if (slow && !FX) {
-    bool ok = dev::slow_push(c, ks, ps);
-    ok = dev::slow_push(c, kr, pr) && ok;
-    ok = dev::slow_push(c, ko, po) && ok;
-    r.upd += ok ? 3 : 0;
-  } else {
-    r.upd += 3;
-  }
-  return r;
-}
-
-template <int VPL, bool FX>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kStepThreads, 1)
 rotate_step_kernel(const __grid_constant__ Ctx c, const __grid_constant__ Args A, float* __restrict__ loss_out,
                    unsigned long long* __restrict__ stats) {
-  dev::cta_enter(c);
-  const int lane = threadIdx.x & 31;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  extern __shared__ float4 rotate_smem[];
-  unsigned char* const wbase =
-      reinterpret_cast<unsigned char*>(rotate_smem) + (size_t)(threadIdx.x >> 5) * warp_bytes(A.d, A.n_neg);
-  float* const wsm = reinterpret_cast<float*>(wbase);
-  dev::Target* const ntg = reinterpret_cast<dev::Target*>(wbase + (size_t)warp_floats(A.d, A.n_neg) * sizeof(float));
-  float loss_acc = 0.f;
-  unsigned n_local = 0, n_remote = 0, n_slow = 0, n_upd = 0;
-
-  for (int t = warp; t < A.B; t += nwarps) {
-    // lanes 0-2 resolve s, r, o; lane l resolves negatives l, l + 32, ...
-    dev::Target tg;
-    tg.row = nullptr; tg.version = nullptr; tg.flag = nullptr;
-    if (lane < 3) {
-      const Key k = lane == 0 ? A.subj[t] : (lane == 1 ? A.rel[t] : A.obj[t]);
-      tg = dev::resolve_fast(c, k, class_of_key(c, k), &n_local, &n_remote);
-    }
-    bool ok = lane >= 3 || tg.row;
-    for (int q = lane; q < A.n_neg; q += 32) {
-      const Key k = A.neg[(size_t)t * A.n_neg + q];
-      const dev::Target nt = dev::resolve_fast(c, k, class_of_key(c, k), &n_local, &n_remote);
-      ntg[q] = nt;
-      ok = ok && nt.row;
-    }
-    __syncwarp();
-    float* ps = (float*)__shfl_sync(0xffffffffu, (unsigned long long)tg.row, 0);
-    float* pr = (float*)__shfl_sync(0xffffffffu, (unsigned long long)tg.row, 1);
-    float* po = (float*)__shfl_sync(0xffffffffu, (unsigned long long)tg.row, 2);
-    TripleOut r;
-    if (__all_sync(0xffffffffu, ok)) {
-      r = triple_body<VPL, FX, false>(c, A, t, ps, pr, po, false, ntg, wsm, nullptr);
-      if (lane < 3) dev::mark_pushed(tg);
-      r.upd += 3;
-    } else {
-      r = triple_generic<VPL, FX>(c, A, t, ps, pr, po, ntg, wsm, A.scratch + (size_t)warp * 8 * A.d);
-      if (lane < 3 && ps && pr && po) dev::mark_pushed(tg);
-    }
-    for (int q = lane; q < A.n_neg; q += 32)
-      if (ntg[q].row) dev::mark_pushed(ntg[q]);
-    __syncwarp();
-    n_upd += r.upd;
-    n_slow += r.slow;
-    if (FX) { if (lane == 0) A.call_loss[t] = r.loss; }
-    else loss_acc += r.loss;
-  }
-
-  __syncwarp();
-  if (!FX && lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
-  unsigned sl = n_local, sr = n_remote;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    sl += __shfl_xor_sync(0xffffffffu, sl, o);
-    sr += __shfl_xor_sync(0xffffffffu, sr, o);
-  }
-  if (lane == 0 && stats) {
-    if (sl) atomicAdd(stats + 0, (unsigned long long)sl);
-    if (sr) atomicAdd(stats + 1, (unsigned long long)sr);
-    if (n_slow) atomicAdd(stats + 2, (unsigned long long)n_slow);
-    if (n_upd) atomicAdd(stats + 3, (unsigned long long)n_upd);
-  }
-  dev::cta_exit(c);
-}
-
-template <int VPL, bool FX>
-void launch(cudaStream_t stream, int blocks, const Ctx& c, const Args& A, float* loss_out, unsigned long long* stats) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    ADAPM_CUDA_CHECK(cudaFuncSetAttribute(rotate_step_kernel<VPL, FX>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)(kThreads / 32 * warp_bytes(kRotatEMaxDim, kRotatEMaxNeg))));
-    attr_set = true;
-  }
-  rotate_step_kernel<VPL, FX><<<blocks, kThreads, kThreads / 32 * warp_bytes(A.d, A.n_neg), stream>>>(c, A, loss_out,
-                                                                                                     stats);
+  warp_step<RotatE<VPL>, FX>(c, A, loss_out, stats);
 }
 
 template <bool FX>
 void launch_shape(int vpl, cudaStream_t stream, int blocks, const Ctx& c, const Args& A, float* loss_out,
                   unsigned long long* stats) {
   switch (vpl) {
-    case 1: launch<1, FX>(stream, blocks, c, A, loss_out, stats); break;
-    case 2: launch<2, FX>(stream, blocks, c, A, loss_out, stats); break;
-    case 3: launch<3, FX>(stream, blocks, c, A, loss_out, stats); break;
-    default: launch<4, FX>(stream, blocks, c, A, loss_out, stats); break;
+    case 1: launch_step<RotatE<1>, rotate_step_kernel<1, FX>>(stream, blocks, c, A, loss_out, stats); break;
+    case 2: launch_step<RotatE<2>, rotate_step_kernel<2, FX>>(stream, blocks, c, A, loss_out, stats); break;
+    case 3: launch_step<RotatE<3>, rotate_step_kernel<3, FX>>(stream, blocks, c, A, loss_out, stats); break;
+    default: launch_step<RotatE<4>, rotate_step_kernel<4, FX>>(stream, blocks, c, A, loss_out, stats); break;
   }
 }
 
@@ -437,33 +331,15 @@ void kge_rotate_step(CudaBackend& be, cudaStream_t stream, const Key* subj, cons
                                                               << kRotatEMaxDim << "]");
   ADAPM_CHECK(n_neg >= 2 && n_neg % 2 == 0 && n_neg <= kRotatEMaxNeg,
               "kge_rotate_step: the negatives per triple must be an even count in [2, " << kRotatEMaxNeg << "]");
-  ADAPM_CHECK(be.ctx().L.val_bytes == 4, "the fused ops need float32 rows (Options::dtype)");
-  be.track_stream(stream);
-  const Ctx& c = be.ctx();
-  const int warps_per_block = kThreads / 32;
-  const int blocks = std::min((B + warps_per_block - 1) / warps_per_block, be.num_sms() * 4);
-  // generic-path scratch (rows in a transitional protocol state): four rows of 2 d per warp
-  float* scratch = static_cast<float*>(
-      be.step_buffer(kScratchBuf, (size_t)blocks * warps_per_block * 8 * (size_t)d * sizeof(float)));
   const int vpl = (d / 4 + 31) / 32;
   Args A;
   A.subj = subj; A.rel = rel; A.obj = obj; A.neg = neg; A.B = B; A.n_neg = n_neg; A.d = d;
-  A.margin = margin; A.alpha = alpha; A.eta = eta; A.gamma_e = gamma_e; A.scratch = scratch;
-  A.fx_acc = nullptr; A.fx_cidx = nullptr; A.call_loss = nullptr;
-  if (deterministic) {
-    // one GPU, start-of-step reads: entity keys get a [d | d] region (2 units), relation keys a [m | m] region (1 unit)
-    const fx::Source src[4] = {{subj, B, 2}, {rel, B, 1}, {obj, B, 2}, {neg, (long)B * n_neg, 2}};
-    CudaBackend::FxScratch& fxs = fx::begin(be, stream, src, 4, d, B);
-    A.fx_acc = fxs.acc; A.fx_cidx = fxs.cidx; A.call_loss = fxs.call_loss;
-    launch_shape<true>(vpl, stream, blocks, c, A, nullptr, stats);
-    ADAPM_COUNT_LAUNCH();
-    ADAPM_CUDA_CHECK(cudaGetLastError());
-    fx::apply(be, stream, d, kFxVal, kFxAda, 0.f, B, loss_out);
-    return;
-  }
-  launch_shape<false>(vpl, stream, blocks, c, A, loss_out, stats);
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_CUDA_CHECK(cudaGetLastError());
+  A.margin = margin; A.alpha = alpha; A.eta = eta; A.gamma_e = gamma_e;
+  // deterministic: entity keys get a [d | d] region (2 units), relation keys a [m | m] region (1 unit)
+  const fx::Source src[4] = {{subj, B, 2}, {rel, B, 1}, {obj, B, 2}, {neg, (long)B * n_neg, 2}};
+  run_step<3>(be, stream, A, deterministic, src, 4, d, kFxVal, kFxAda, loss_out, [&](auto fx, int blocks, float* lo) {
+    launch_shape<decltype(fx)::value>(vpl, stream, blocks, be.ctx(), A, lo, stats);
+  });
 }
 
 }  // namespace cudaops

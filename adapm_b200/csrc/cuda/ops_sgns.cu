@@ -249,18 +249,7 @@ sgns_step_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers,
   // ---- per-warp results
   __syncwarp();
   if (lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
-  unsigned sum_local = n_local, sum_remote = n_remote;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    sum_local += __shfl_xor_sync(0xffffffffu, sum_local, o);
-    sum_remote += __shfl_xor_sync(0xffffffffu, sum_remote, o);
-  }
-  if (lane == 0 && stats) {
-    if (sum_local) atomicAdd(stats + 0, (unsigned long long)sum_local);
-    if (sum_remote) atomicAdd(stats + 1, (unsigned long long)sum_remote);
-    if (n_slow) atomicAdd(stats + 2, (unsigned long long)n_slow);
-    if (n_upd) atomicAdd(stats + 3, (unsigned long long)n_upd);
-  }
+  dev::flush_stats(stats, n_local, n_remote, n_slow, n_upd);
   dev::cta_exit(c);
 }
 
@@ -287,11 +276,7 @@ void sgns_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const K
   size_t smem = (size_t)warps_per_block * 4 * d * sizeof(float);
 #define ADAPM_LAUNCH_SGNS(V)                                                                             \
   do {                                                                                                   \
-    static bool attr_set = false;                                                                        \
-    if (!attr_set) {                                                                                     \
-      cudaFuncSetAttribute(sgns_step_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024); \
-      attr_set = true;                                                                                   \
-    }                                                                                                    \
+    set_max_dynamic_smem<sgns_step_kernel<V>>(96 * 1024);                                                \
     sgns_step_kernel<V><<<blocks, kThreads, smem, stream>>>(c, centers, contexts, negatives, n_pairs, neg, d, \
                                                            alpha, loss_out, stats);                     \
   } while (0)

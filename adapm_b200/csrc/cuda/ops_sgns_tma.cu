@@ -392,18 +392,7 @@ sgns_step_tma_body(const Ctx& c, const Key* __restrict__ centers, const Key* __r
   __syncwarp();
   if (SCORE && lane == 0) atomicAdd(fx_loss, (unsigned long long)__float2ll_rn(loss_acc * kFxLoss));
   else if (lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
-  unsigned sum_local = n_local, sum_remote = n_remote;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    sum_local += __shfl_xor_sync(0xffffffffu, sum_local, o);
-    sum_remote += __shfl_xor_sync(0xffffffffu, sum_remote, o);
-  }
-  if (lane == 0 && stats) {
-    if (sum_local) atomicAdd(stats + 0, (unsigned long long)sum_local);
-    if (sum_remote) atomicAdd(stats + 1, (unsigned long long)sum_remote);
-    if (n_slow) atomicAdd(stats + 2, (unsigned long long)n_slow);
-    if (n_upd) atomicAdd(stats + 3, (unsigned long long)n_upd);
-  }
+  dev::flush_stats(stats, n_local, n_remote, n_slow, n_upd);
   dev::cta_exit(c);
 }
 
@@ -555,11 +544,7 @@ void sgns_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   ADAPM_COUNT_LAUNCH();   // (the scan is two kernels)
 #define ADAPM_LAUNCH_SCORE(V)                                                                                  \
   do {                                                                                                         \
-    static bool attr_set = false;                                                                              \
-    if (!attr_set) {                                                                                           \
-      cudaFuncSetAttribute(sgns_score_tma_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024); \
-      attr_set = true;                                                                                         \
-    }                                                                                                          \
+    set_max_dynamic_smem<sgns_score_tma_kernel<V>>(110 * 1024);                                                \
     sgns_score_tma_kernel<V><<<score_blocks, kThreads, score_smem, stream>>>(c, centers, contexts, negatives,  \
                                                                              n_pairs, neg, d, alpha, stats, fx.cidx, \
                                                                              gsb, fx.loss, so);                  \
@@ -614,11 +599,7 @@ bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   }
 #define ADAPM_LAUNCH_TMA2(V, R)                                                                                 \
   do {                                                                                                          \
-    static bool attr_set = false;                                                                               \
-    if (!attr_set) {                                                                                            \
-      cudaFuncSetAttribute(sgns_step_tma_kernel<V, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);  \
-      attr_set = true;                                                                                          \
-    }                                                                                                           \
+    set_max_dynamic_smem<sgns_step_tma_kernel<V, R>>(110 * 1024);                                               \
     sgns_step_tma_kernel<V, R><<<blocks, threads, smem, stream>>>(c, centers, contexts, negatives, n_pairs, neg, d, \
                                                                   alpha, loss_out, stats);                      \
   } while (0)

@@ -467,11 +467,7 @@ void gemm_nt_topk(cudaStream_t stream, const void* A, const void* B, int M, int 
   ADAPM_CHECK((((uintptr_t)A) & 15u) == 0 && (((uintptr_t)B) & 15u) == 0, "gemm_nt_topk: operands must be 16-byte aligned");
   CUtensorMap ma = make_map(A, M, K, BM, KIND_BF16);
   CUtensorMap mb = make_map(B, N, K, BN, KIND_BF16);
-  static bool attr_set = false;
-  if (!attr_set) {
-    ADAPM_CUDA_CHECK(cudaFuncSetAttribute(gemm_nt_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)topk_smem()));
-    attr_set = true;
-  }
+  set_max_dynamic_smem<gemm_nt_topk_kernel>((int)topk_smem());
   dim3 grid((M + BM - 1) / BM, S);
   gemm_nt_topk_kernel<<<grid, kGemmThreads, topk_smem(), stream>>>(ma, mb, a);
   ADAPM_COUNT_LAUNCH();
@@ -497,12 +493,7 @@ void gather_gemm_topk(CudaBackend& be, cudaStream_t stream, const void* Q, const
   ADAPM_CHECK(be.ctx().L.val_bytes == 4, "the fused ops need float32 rows (Options::dtype)");
   be.track_stream(stream);
   CUtensorMap mq = make_map(Q, M, ldq, BM, KIND_BF16);
-  static bool attr_set = false;
-  if (!attr_set) {
-    ADAPM_CUDA_CHECK(cudaFuncSetAttribute(gather_gemm_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)topk_smem()));
-    attr_set = true;
-  }
+  set_max_dynamic_smem<gather_gemm_topk_kernel>((int)topk_smem());
   dim3 grid((M + BM - 1) / BM, S);
   gather_gemm_topk_kernel<<<grid, kGemmThreads, topk_smem(), stream>>>(mq, be.ctx(), keys, a, stats);
   ADAPM_COUNT_LAUNCH();

@@ -35,10 +35,7 @@ namespace cudaops {
 
 namespace {
 
-constexpr int kThreads = 256;
 constexpr float kNormEps = 1e-12f;
-// the backend's step buffer that holds the generic path's staged rows (the deterministic SGNS step uses buffers 0 - 9)
-constexpr int kScratchBuf = CudaBackend::kStepBuffers - 1;
 
 // Fixed-point scales of the deterministic mode. |value update| <= eta per push (AdaGrad normalises it): 2^40 leaves
 // 2^23 / eta pushes per element and step. The gradient has no bound as |e| -> 0 (the 1/|e| factor), so the AdaGrad
@@ -102,23 +99,37 @@ struct Args {
   float* call_loss;
 };
 
-struct TripleOut {
-  float loss;
-  unsigned upd, slow;
+// The step as a warp_step rule (kge_step.cuh): positive (s, r, o). Per-warp shared memory: a = s^ + r | b = r - o^ |
+// x | U_o | U_s (d each; each lane touches only its own float4s) | the negatives' targets.
+template <int VPL, int P>
+struct TransE {
+  static constexpr int kPositives = 3, kMaxDim = kTransEMaxDim, kMaxNeg = kTransEMaxNeg;
+  static __device__ __forceinline__ Key positive(const Args& A, int t, int i) {
+    return i == 0 ? A.subj[t] : (i == 1 ? A.rel[t] : A.obj[t]);
+  }
+  static __host__ __device__ __forceinline__ size_t state_bytes(int d, int) { return (size_t)5 * d * sizeof(float); }
+  static __host__ __device__ __forceinline__ size_t warp_bytes(int d, int n_neg) {
+    return state_bytes(d, n_neg) + (size_t)n_neg * sizeof(dev::Target);
+  }
+  // an inactive pair pushes nothing (n_neg <= 64: one bit per negative)
+  static __device__ __forceinline__ bool neg_pushed(const StepOut& r, int q) { return r.pushed >> q & 1ull; }
+  template <bool FX, bool GEN>
+  static __device__ StepOut body(const Ctx& c, const Args& A, int t, const Rows<3>& rows, bool slow,
+                                 const dev::Target* ntg, float* wsm, float* my_scratch);
 };
 
-// One positive triple and its negatives. ps / pr / po: the positive's rows, or (slow) their staged copies in global
-// scratch that are pushed through the generic path afterwards. nt0 / nt1: this lane's negatives lane and lane + 32.
-// GEN: negatives in a transitional state are staged one at a time (only the out-of-line generic path calls
-// slow_pull / slow_push; the kernel's own loop has no calls, so nothing it holds is spilled around them).
-template <int VPL, int P, bool FX, bool GEN>
-__device__ __forceinline__ TripleOut triple_body(const Ctx& c, const Args& A, int t, float* ps, float* pr, float* po,
-                                                 bool slow, const dev::Target& nt0, const dev::Target& nt1, float* wsm,
-                                                 float* my_scratch) {
+// One positive triple and its negatives: ps / pr / po the positive's rows.
+template <int VPL, int P>
+template <bool FX, bool GEN>
+__device__ __forceinline__ StepOut TransE<VPL, P>::body(const Ctx& c, const Args& A, int t, const Rows<3>& rows,
+                                                        bool slow, const dev::Target* ntg, float* wsm,
+                                                        float* my_scratch) {
   const int lane = threadIdx.x & 31;
   const int d = A.d, nv = d >> 2, L = 2 * d, n_neg = A.n_neg, half = n_neg >> 1;
-  TripleOut out = {0.f, 0u, 0u};
-  // per-warp state in shared memory (each lane touches only its own float4s): a = s^ + r | b = r - o^ | x | U_o | U_s
+  float* const ps = rows.p[0];
+  float* const pr = rows.p[1];
+  float* const po = rows.p[2];
+  StepOut out = {0.f, 0u, 0u, 0ull};
   float* const sa = wsm; float* const sb = wsm + d; float* const sx = wsm + 2 * d;
   float* const suo = wsm + 3 * d; float* const sus = wsm + 4 * d;
   float4 e[VPL], v[VPL];
@@ -142,12 +153,11 @@ __device__ __forceinline__ TripleOut triple_body(const Ctx& c, const Args& A, in
   }
   const float Dp = dist<P, VPL>(e);
   int k_act = 0;
-  unsigned long long pushed = 0ull;
 
   // ---- the 2n negatives, one row at a time
   for (int q = 0; q < n_neg; ++q) {
     const Key kn = A.neg[(size_t)t * n_neg + q];
-    float* pn = (float*)__shfl_sync(0xffffffffu, (unsigned long long)(q < 32 ? nt0.row : nt1.row), q & 31);
+    float* pn = ntg[q].row;
     const bool nslow = !pn;
     if (GEN && nslow) {
       ++out.slow;
@@ -188,12 +198,10 @@ __device__ __forceinline__ TripleOut triple_body(const Ctx& c, const Args& A, in
     if (GEN && nslow && !FX) {
       if (dev::slow_push(c, kn, pn)) ++out.upd;
     } else {
-      if (!nslow) pushed |= 1ull << q;
+      if (!nslow) out.pushed |= 1ull << q;
       ++out.upd;
     }
   }
-  if (pushed >> lane & 1ull) dev::mark_pushed(nt0);
-  if (pushed >> (lane + 32) & 1ull) dev::mark_pushed(nt1);
 
   // ---- the positive's rows: summed gradients, L2 on the raw rows, one push each
   const float inv_dp = Dp > 0.f ? 1.f / Dp : 0.f;
@@ -241,128 +249,28 @@ __device__ __forceinline__ TripleOut triple_body(const Ctx& c, const Args& A, in
   return out;
 }
 
-// Generic path of a triple with a row in a transitional protocol state: the positive's rows are staged through
-// slow_pull (and pushed back through slow_push), negatives one at a time. (Out of line: the calls would otherwise make
-// the kernel spill everything it holds around them.)
 template <int VPL, int P, bool FX>
-__device__ __noinline__ TripleOut triple_generic(const Ctx& c, const Args& A, int t, float* ps, float* pr, float* po,
-                                                 const dev::Target nt0, const dev::Target nt1, float* wsm, float* my_scratch) {
-  const int L = 2 * A.d;
-  const bool slow = !ps || !pr || !po;
-  TripleOut out = {0.f, 0u, 0u};
-  const Key ks = A.subj[t], kr = A.rel[t], ko = A.obj[t];
-  if (slow) {
-    out.slow = 1;
-    if (!dev::slow_pull(c, ks, my_scratch) || !dev::slow_pull(c, kr, my_scratch + L) ||
-        !dev::slow_pull(c, ko, my_scratch + 2 * L))
-      return out;
-    ps = my_scratch; pr = my_scratch + L; po = my_scratch + 2 * L;
-  }
-  TripleOut r = triple_body<VPL, P, FX, true>(c, A, t, ps, pr, po, slow, nt0, nt1, wsm, my_scratch);
-  r.slow += out.slow;
-  if (slow && !FX) {
-    bool ok = dev::slow_push(c, ks, ps);
-    ok = dev::slow_push(c, kr, pr) && ok;
-    ok = dev::slow_push(c, ko, po) && ok;
-    r.upd += ok ? 3 : 0;
-  } else {
-    r.upd += 3;
-  }
-  return r;
-}
-
-template <int VPL, int P, bool FX>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kStepThreads, 1)
 transe_step_kernel(const __grid_constant__ Ctx c, const __grid_constant__ Args A, float* __restrict__ loss_out,
                    unsigned long long* __restrict__ stats) {
-  dev::cta_enter(c);
-  const int lane = threadIdx.x & 31;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  extern __shared__ float4 transe_smem[];
-  float* const wsm = reinterpret_cast<float*>(transe_smem) + (size_t)(threadIdx.x >> 5) * 5 * A.d;
-  float loss_acc = 0.f;
-  unsigned n_local = 0, n_remote = 0, n_slow = 0, n_upd = 0;
-
-  for (int t = warp; t < A.B; t += nwarps) {
-    // lanes 0-2 resolve s, r, o; lane l resolves negatives l and l + 32
-    dev::Target tg, nt0, nt1;
-    tg.row = nullptr; tg.version = nullptr; tg.flag = nullptr;
-    nt0 = tg; nt1 = tg;
-    if (lane < 3) {
-      const Key k = lane == 0 ? A.subj[t] : (lane == 1 ? A.rel[t] : A.obj[t]);
-      tg = dev::resolve_fast(c, k, class_of_key(c, k), &n_local, &n_remote);
-    }
-    bool ok = lane >= 3 || tg.row;
-    if (lane < A.n_neg) {
-      const Key k = A.neg[(size_t)t * A.n_neg + lane];
-      nt0 = dev::resolve_fast(c, k, class_of_key(c, k), &n_local, &n_remote);
-      ok = ok && nt0.row;
-    }
-    if (lane + 32 < A.n_neg) {
-      const Key k = A.neg[(size_t)t * A.n_neg + lane + 32];
-      nt1 = dev::resolve_fast(c, k, class_of_key(c, k), &n_local, &n_remote);
-      ok = ok && nt1.row;
-    }
-    float* ps = (float*)__shfl_sync(0xffffffffu, (unsigned long long)tg.row, 0);
-    float* pr = (float*)__shfl_sync(0xffffffffu, (unsigned long long)tg.row, 1);
-    float* po = (float*)__shfl_sync(0xffffffffu, (unsigned long long)tg.row, 2);
-    TripleOut r;
-    if (__all_sync(0xffffffffu, ok)) {
-      r = triple_body<VPL, P, FX, false>(c, A, t, ps, pr, po, false, nt0, nt1, wsm, nullptr);
-      if (lane < 3) dev::mark_pushed(tg);
-      r.upd += 3;
-    } else {
-      r = triple_generic<VPL, P, FX>(c, A, t, ps, pr, po, nt0, nt1, wsm, A.scratch + (size_t)warp * 8 * A.d);
-      if (lane < 3 && ps && pr && po) dev::mark_pushed(tg);
-    }
-    n_upd += r.upd;
-    n_slow += r.slow;
-    if (FX) { if (lane == 0) A.call_loss[t] = r.loss; }
-    else loss_acc += r.loss;
-  }
-
-  __syncwarp();
-  if (!FX && lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
-  unsigned sl = n_local, sr = n_remote;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    sl += __shfl_xor_sync(0xffffffffu, sl, o);
-    sr += __shfl_xor_sync(0xffffffffu, sr, o);
-  }
-  if (lane == 0 && stats) {
-    if (sl) atomicAdd(stats + 0, (unsigned long long)sl);
-    if (sr) atomicAdd(stats + 1, (unsigned long long)sr);
-    if (n_slow) atomicAdd(stats + 2, (unsigned long long)n_slow);
-    if (n_upd) atomicAdd(stats + 3, (unsigned long long)n_upd);
-  }
-  dev::cta_exit(c);
+  warp_step<TransE<VPL, P>, FX>(c, A, loss_out, stats);
 }
 
-template <int VPL, int P, bool FX>
-void launch(cudaStream_t stream, int blocks, const Ctx& c, const Args& A, float* loss_out, unsigned long long* stats) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    ADAPM_CUDA_CHECK(cudaFuncSetAttribute(transe_step_kernel<VPL, P, FX>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          kThreads / 32 * 5 * kTransEMaxDim * (int)sizeof(float)));
-    attr_set = true;
-  }
-  transe_step_kernel<VPL, P, FX><<<blocks, kThreads, kThreads / 32 * 5 * A.d * sizeof(float), stream>>>(c, A, loss_out,
-                                                                                                         stats);
+template <int VPL, bool FX>
+void launch_p(int p, cudaStream_t stream, int blocks, const Ctx& c, const Args& A, float* loss_out,
+              unsigned long long* stats) {
+  if (p == 1) launch_step<TransE<VPL, 1>, transe_step_kernel<VPL, 1, FX>>(stream, blocks, c, A, loss_out, stats);
+  else launch_step<TransE<VPL, 2>, transe_step_kernel<VPL, 2, FX>>(stream, blocks, c, A, loss_out, stats);
 }
 
 template <bool FX>
 void launch_shape(int vpl, int p, cudaStream_t stream, int blocks, const Ctx& c, const Args& A, float* loss_out,
                   unsigned long long* stats) {
-  switch (vpl * 2 + p - 1) {
-    case 2: launch<1, 1, FX>(stream, blocks, c, A, loss_out, stats); break;
-    case 3: launch<1, 2, FX>(stream, blocks, c, A, loss_out, stats); break;
-    case 4: launch<2, 1, FX>(stream, blocks, c, A, loss_out, stats); break;
-    case 5: launch<2, 2, FX>(stream, blocks, c, A, loss_out, stats); break;
-    case 6: launch<3, 1, FX>(stream, blocks, c, A, loss_out, stats); break;
-    case 7: launch<3, 2, FX>(stream, blocks, c, A, loss_out, stats); break;
-    case 8: launch<4, 1, FX>(stream, blocks, c, A, loss_out, stats); break;
-    default: launch<4, 2, FX>(stream, blocks, c, A, loss_out, stats); break;
+  switch (vpl) {
+    case 1: launch_p<1, FX>(p, stream, blocks, c, A, loss_out, stats); break;
+    case 2: launch_p<2, FX>(p, stream, blocks, c, A, loss_out, stats); break;
+    case 3: launch_p<3, FX>(p, stream, blocks, c, A, loss_out, stats); break;
+    default: launch_p<4, FX>(p, stream, blocks, c, A, loss_out, stats); break;
   }
 }
 
@@ -377,33 +285,15 @@ void kge_transe_step(CudaBackend& be, cudaStream_t stream, const Key* subj, cons
   ADAPM_CHECK(p == 1 || p == 2, "kge_transe_step: p must be 1 or 2");
   ADAPM_CHECK(n_neg >= 0 && n_neg % 2 == 0 && n_neg <= kTransEMaxNeg,
               "kge_transe_step: the negatives per triple must be an even count <= " << kTransEMaxNeg);
-  ADAPM_CHECK(be.ctx().L.val_bytes == 4, "the fused ops need float32 rows (Options::dtype)");
-  be.track_stream(stream);
-  const Ctx& c = be.ctx();
-  const int warps_per_block = kThreads / 32;
-  const int blocks = std::min((B + warps_per_block - 1) / warps_per_block, be.num_sms() * 4);
-  // generic-path scratch (rows in a transitional protocol state): four rows per warp, one of the backend's step buffers
-  float* scratch = static_cast<float*>(
-      be.step_buffer(kScratchBuf, (size_t)blocks * warps_per_block * 8 * (size_t)d * sizeof(float)));
   const int vpl = (d / 4 + 31) / 32;
   Args A;
   A.subj = subj; A.rel = rel; A.obj = obj; A.neg = neg; A.B = B; A.n_neg = n_neg; A.d = d;
-  A.margin = margin; A.eta = eta; A.gamma_e = gamma_e; A.gamma_r = gamma_r; A.scratch = scratch;
-  A.fx_acc = nullptr; A.fx_cidx = nullptr; A.call_loss = nullptr;
-  if (deterministic) {
-    // one GPU, start-of-step reads: every key (entity or relation, both 2 d long) gets a [d | d] region
-    const fx::Source src[4] = {{subj, B, 1}, {rel, B, 1}, {obj, B, 1}, {neg, (long)B * n_neg, 1}};
-    CudaBackend::FxScratch& fxs = fx::begin(be, stream, src, 4, 2 * d, B);
-    A.fx_acc = fxs.acc; A.fx_cidx = fxs.cidx; A.call_loss = fxs.call_loss;
-    launch_shape<true>(vpl, p, stream, blocks, c, A, nullptr, stats);
-    ADAPM_COUNT_LAUNCH();
-    ADAPM_CUDA_CHECK(cudaGetLastError());
-    fx::apply(be, stream, 2 * d, kFxVal, kFxAda, 0.f, B, loss_out);
-    return;
-  }
-  launch_shape<false>(vpl, p, stream, blocks, c, A, loss_out, stats);
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_CUDA_CHECK(cudaGetLastError());
+  A.margin = margin; A.eta = eta; A.gamma_e = gamma_e; A.gamma_r = gamma_r;
+  // deterministic: every key (entity or relation, both 2 d long) gets a [d | d] region
+  const fx::Source src[4] = {{subj, B, 1}, {rel, B, 1}, {obj, B, 1}, {neg, (long)B * n_neg, 1}};
+  run_step<3>(be, stream, A, deterministic, src, 4, 2 * d, kFxVal, kFxAda, loss_out, [&](auto fx, int blocks, float* lo) {
+    launch_shape<decltype(fx)::value>(vpl, p, stream, blocks, be.ctx(), A, lo, stats);
+  });
 }
 
 }  // namespace cudaops

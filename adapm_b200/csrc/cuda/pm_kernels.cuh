@@ -210,6 +210,23 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// End of a fused step's kernel, all lanes of the warp: stats[0..3] += (local rows, peer rows, slow-path rows, pushes).
+// The resolve counts are per lane and summed over the warp; n_slow and n_upd are warp-uniform and lane 0's are added.
+__device__ __forceinline__ void flush_stats(unsigned long long* stats, unsigned n_local, unsigned n_remote,
+                                            unsigned n_slow, unsigned n_upd) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    n_local += __shfl_xor_sync(0xffffffffu, n_local, o);
+    n_remote += __shfl_xor_sync(0xffffffffu, n_remote, o);
+  }
+  if ((threadIdx.x & 31) == 0 && stats) {
+    if (n_local) atomicAdd(stats + 0, (unsigned long long)n_local);
+    if (n_remote) atomicAdd(stats + 1, (unsigned long long)n_remote);
+    if (n_slow) atomicAdd(stats + 2, (unsigned long long)n_slow);
+    if (n_upd) atomicAdd(stats + 3, (unsigned long long)n_upd);
+  }
+}
+
 // generic out-of-line fallbacks (warp-cooperative)
 static __device__ __noinline__ bool slow_pull(const Ctx& c, Key key, float* stage) {
   WarpGroup g;
