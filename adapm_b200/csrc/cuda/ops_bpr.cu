@@ -68,12 +68,15 @@ struct Args {
 // The step as a warp_step rule (kge_step.cuh): positive (u, i), targets only in shared memory.
 template <int VPL>
 struct Bpr {
-  static constexpr int kPositives = 2, kMaxDim = kBprMaxRank, kMaxNeg = kBprMaxNeg;
+  static constexpr int kPositives = 2, kMaxDim = kBprMaxRank, kMaxNeg = kBprMaxNeg, kBlocksPerSM = 4;
+  static constexpr bool kInPlace = true, kStageInSmem = false;
   static __device__ __forceinline__ Key positive(const Args& A, int t, int i) { return i == 0 ? A.users[t] : A.pos[t]; }
   static __host__ __device__ __forceinline__ size_t state_bytes(int, int) { return 0; }
   static __host__ __device__ __forceinline__ size_t warp_bytes(int, int n_neg) {
     return (size_t)n_neg * sizeof(dev::Target);
   }
+  static __host__ __device__ __forceinline__ int scratch_rows(int) { return kPositives + 1; }
+  static __device__ __forceinline__ int stage_row(int, int i) { return i; }
   static __device__ __forceinline__ bool neg_pushed(const StepOut&, int) { return true; }
   template <bool FX, bool GEN>
   static __device__ StepOut body(const Ctx& c, const Args& A, int t, const Rows<2>& rows, bool slow,
@@ -155,13 +158,13 @@ mf_bpr_step_kernel(const __grid_constant__ Ctx c, const __grid_constant__ Args A
 }
 
 template <bool FX>
-void launch_shape(int vpl, cudaStream_t stream, int blocks, const Ctx& c, const Args& A, float* loss_out,
+void launch_shape(int vpl, CudaBackend& be, cudaStream_t stream, const Args& A, float* loss_out,
                   unsigned long long* stats) {
   switch (vpl) {
-    case 1: launch_step<Bpr<1>, mf_bpr_step_kernel<1, FX>>(stream, blocks, c, A, loss_out, stats); break;
-    case 2: launch_step<Bpr<2>, mf_bpr_step_kernel<2, FX>>(stream, blocks, c, A, loss_out, stats); break;
-    case 3: launch_step<Bpr<3>, mf_bpr_step_kernel<3, FX>>(stream, blocks, c, A, loss_out, stats); break;
-    default: launch_step<Bpr<4>, mf_bpr_step_kernel<4, FX>>(stream, blocks, c, A, loss_out, stats); break;
+    case 1: launch_step<Bpr<1>, mf_bpr_step_kernel<1, FX>>(be, stream, A, loss_out, stats); break;
+    case 2: launch_step<Bpr<2>, mf_bpr_step_kernel<2, FX>>(be, stream, A, loss_out, stats); break;
+    case 3: launch_step<Bpr<3>, mf_bpr_step_kernel<3, FX>>(be, stream, A, loss_out, stats); break;
+    default: launch_step<Bpr<4>, mf_bpr_step_kernel<4, FX>>(be, stream, A, loss_out, stats); break;
   }
 }
 
@@ -180,8 +183,8 @@ void mf_bpr_step(CudaBackend& be, cudaStream_t stream, const Key* users, const K
   A.eps = eps; A.lam = lam;
   // deterministic: every key (user or item, both 2 rank long) gets a [rank | rank] region
   const fx::Source src[3] = {{users, B, 1}, {pos, B, 1}, {neg, (long)B * n_neg, 1}};
-  run_step<2>(be, stream, A, deterministic, src, 3, 2 * rank, kFxVal, kFxAda, loss_out, [&](auto fx, int blocks, float* lo) {
-    launch_shape<decltype(fx)::value>(vpl, stream, blocks, be.ctx(), A, lo, stats);
+  run_step(be, stream, A, deterministic, src, 3, 2 * rank, kFxVal, kFxAda, loss_out, [&](auto fx, float* lo) {
+    launch_shape<decltype(fx)::value>(vpl, be, stream, A, lo, stats);
   });
 }
 

@@ -1,4 +1,4 @@
-// Fused knowledge-graph-embedding training step (ComplEx) for sm_90a: Pull(s, r, o) + score +
+// Fused knowledge-graph-embedding training steps (ComplEx, RESCAL) for sm_90a: Pull(s, r, o) + score +
 // BCE gradient + L2 + AdaGrad + Push(s, r, o) in one kernel over local HBM / NVLink peers
 // (SURVEY K1 + K8 + K9 + K2 + K14).
 //
@@ -9,17 +9,16 @@
 //   d_x   = dl * dscore/dx  (+ gamma * x for positives)
 //   push(x, [-eta * d_x / sqrt(acc_x + d_x^2) | d_x^2])        for x in {s, r, o}
 // Row layout [embedding(nh) | AdaGrad(nh)], embedding = [real(nh/2) | imag(nh/2)].
-// One warp per training call; the three directory lookups are issued by three lanes at once.
+// Both steps are warp_step rules without negatives (kge_step.cuh): one warp per training call; the three directory
+// lookups are issued by three lanes at once.
 //
 // Deterministic one-GPU variants (kge_step_fx_kernel, kge_rescal_fx_kernel): every call reads the state at the start of
 // the step and adds its updates as fixed-point integers into per-key accumulator regions (fx_accum.cuh), which one
 // apply pass adds to the rows; each call's loss goes to its own slot and is summed in a fixed order.
 #include <cuda_runtime.h>
 
-#include <map>
-#include <mutex>
-
 #include "fx_accum.cuh"
+#include "kge_step.cuh"
 #include "ops.h"
 #include "pm_kernels.cuh"
 
@@ -28,14 +27,7 @@ namespace cudaops {
 
 namespace {
 
-constexpr int kThreads = 256;
-
-__device__ __forceinline__ float4 f4_mul(float4 a, float4 b) { return make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w); }
-__device__ __forceinline__ float4 f4_fma(float4 a, float4 b, float4 c) {
-  return make_float4(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y), fmaf(a.z, b.z, c.z), fmaf(a.w, b.w, c.w));
-}
-__device__ __forceinline__ float4 f4_sub(float4 a, float4 b) { return make_float4(a.x - b.x, a.y - b.y, a.z - b.z, a.w - b.w); }
-__device__ __forceinline__ float f4_hsum(float4 a) { return a.x + a.y + a.z + a.w; }
+using namespace kge;
 
 // Dropout on the pulled copies (reference kge.cc:405-413,478-484: Bernoulli(p) zero, others scaled by 1/(1-p); score,
 // gradients and L2 all see the masked copy; the AdaGrad half of a row is untouched). The mask is a pure function of
@@ -61,241 +53,192 @@ struct Dropout {
 
 // Fixed-point scales of the deterministic mode. |value update| <= eta per call (AdaGrad normalises it): 2^40 leaves
 // 2^23 / eta calls per element and step. AdaGrad increments are g^2 with g = dl * (sum of products of two embedding
-// values) + gamma * x and |dl| < 1: 2^36 leaves 2^27 of summed g^2 per element and step (resolution 1.5e-11).
+// values) + gamma * x and |dl| < 1: 2^36 leaves 2^27 of summed g^2 per element and step (resolution 1.5e-11). The
+// increments are not clamped (kFxAdaMax = +inf).
 constexpr float kFxVal = 1099511627776.f;     // 2^40
 constexpr float kFxAda = 68719476736.f;       // 2^36
+constexpr float kFxAdaMax = INFINITY;
+// the largest nh whose three staged rows per warp fit 200 KB of shared memory per CTA
+constexpr int kComplexMaxDim = 200 * 1024 / (kStepThreads / 32 * 6 * (int)sizeof(float));
+constexpr int kRescalMaxDim = 128;
 
-// g = dl * d + (reg ? gamma * x : 0); returns AdaGrad update pair and issues the reductions.
-__device__ __forceinline__ void adagrad_push4(float* emb_ptr, float* acc_ptr, float4 d, float4 x, float dl, float gamma,
-                                              float eta) {
-  float4 g = make_float4(fmaf(gamma, x.x, dl * d.x), fmaf(gamma, x.y, dl * d.y), fmaf(gamma, x.z, dl * d.z),
-                         fmaf(gamma, x.w, dl * d.w));
-  float4 a = dev::ld_row4(acc_ptr);
-  float4 ua = f4_mul(g, g);
-  float4 ue = make_float4(-eta * g.x * rsqrtf(a.x + ua.x), -eta * g.y * rsqrtf(a.y + ua.y),
-                          -eta * g.z * rsqrtf(a.z + ua.z), -eta * g.w * rsqrtf(a.w + ua.w));
-  dev::red_row4(emb_ptr, ue);
-  dev::red_row4(acc_ptr, ua);
-}
-// deterministic mode: the same update, added to float4 jj of the key's accumulator region (halves of h values)
-__device__ __forceinline__ void adagrad_fx4(const float* acc_ptr, long long* region, int jj, int h, float4 d, float4 x,
-                                            float dl, float gamma, float eta) {
-  float4 g = make_float4(fmaf(gamma, x.x, dl * d.x), fmaf(gamma, x.y, dl * d.y), fmaf(gamma, x.z, dl * d.z),
-                         fmaf(gamma, x.w, dl * d.w));
-  float4 a = dev::ld_row4(acc_ptr);
-  float4 ua = f4_mul(g, g);
-  float4 ue = make_float4(-eta * g.x * rsqrtf(a.x + ua.x), -eta * g.y * rsqrtf(a.y + ua.y),
-                          -eta * g.z * rsqrtf(a.z + ua.z), -eta * g.w * rsqrtf(a.w + ua.w));
-  fx::add4(region, jj, h >> 2, ue, kFxVal);
-  fx::add4(region + h, jj, h >> 2, ua, kFxAda);
-}
-// deterministic mode: adds a staged row of updates [value update (h) | AdaGrad update (h)] to the key's region
-__device__ __forceinline__ void fx_add_staged(long long* region, const float* stage, int h) {
-  for (int i = threadIdx.x & 31; i < 2 * h; i += 32) {
-    const int hf = i >= h;
-    fx::add1(region + hf * h, i - hf * h, h, stage[i], hf ? kFxAda : kFxVal);
-  }
-}
+struct Args {
+  const Key* subj;
+  const Key* rel;
+  const Key* obj;
+  const float* labels;
+  int B, n_neg, d;             // n_neg = 0; d: nh (ComplEx) or D (RESCAL)
+  float eta, gamma_e, gamma_r;
+  Dropout de, dr;
+  float* scratch;              // RESCAL's generic path: a relation row and two entity rows per warp
+  long long* fx_acc;           // FX: fixed-point regions, per-call loss slots
+  const int* fx_cidx;
+  float* call_loss;
+};
 
-// scalar generic path (any nh; also used when a row is in a transitional state): rows staged in smem
-template <bool FX>
-__device__ __noinline__ float kge_call_generic(const Ctx& c, Key ks, Key kr, Key ko, float label, int nh, float eta,
-                                               float gamma_e, float gamma_r, float* stage, bool* applied, uint32_t call,
-                                               Dropout de, Dropout dr, long long* fx_acc, const int* fx_cidx) {
-  const int lane = threadIdx.x & 31;
-  float* S = stage; float* R = stage + 2 * nh; float* O = stage + 4 * nh;
-  *applied = false;
-  if (!dev::slow_pull(c, ks, S) || !dev::slow_pull(c, kr, R) || !dev::slow_pull(c, ko, O)) return 0.f;
-  if (de.p > 0.f || dr.p > 0.f) {
-    for (int i = lane; i < nh; i += 32) {
-      if (de.p > 0.f) { S[i] *= de.keep(call, 0, (uint32_t)i); O[i] *= de.keep(call, 2, (uint32_t)i); }
-      if (dr.p > 0.f) R[i] *= dr.keep(call, 1, (uint32_t)i);
-    }
-    __syncwarp();
+// What ComplEx and RESCAL share as warp_step rules: positive (s, r, o), no negatives.
+struct TripleRule {
+  static constexpr int kPositives = 3, kMaxNeg = 0;
+  static __device__ __forceinline__ Key positive(const Args& A, int t, int i) {
+    return i == 0 ? A.subj[t] : (i == 1 ? A.rel[t] : A.obj[t]);
   }
-  const int H = nh / 2;
-  float sc = 0.f;
-  for (int i = lane; i < H; i += 32)
-    sc += R[i] * S[i] * O[i] + R[i] * S[H + i] * O[H + i] + R[H + i] * S[i] * O[H + i] - R[H + i] * S[H + i] * O[i];
-  sc = dev::warp_sum(sc);
-  const float dl = 1.f / (1.f + __expf(-sc)) - label;
-  const float ge = label > 0.5f ? gamma_e : 0.f, gr = label > 0.5f ? gamma_r : 0.f;
-  for (int i = lane; i < H; i += 32) {
-    float sre = S[i], sim = S[H + i], rre = R[i], rim = R[H + i], ore = O[i], oim = O[H + i];
-    float d[6] = {rre * ore + rim * oim, rre * oim - rim * ore, sre * ore + sim * oim,
-                  sre * oim - sim * ore, rre * sre - rim * sim, rre * sim + rim * sre};
-    float x[6] = {sre, sim, rre, rim, ore, oim};
-    float gm[6] = {ge, ge, gr, gr, ge, ge};
-    float* rows[6] = {S, S, R, R, O, O};
-    int off[6] = {i, H + i, i, H + i, i, H + i};
-#pragma unroll
-    for (int q = 0; q < 6; ++q) {
-      float g = dl * d[q] + gm[q] * x[q];
-      float a = rows[q][nh + off[q]];
-      float ua = g * g;
-      rows[q][off[q]] = -eta * g * rsqrtf(a + ua);
-      rows[q][nh + off[q]] = ua;
-    }
-  }
-  __syncwarp();
-  if (FX) {
-    fx_add_staged(fx::region(fx_acc, fx_cidx, ks, 2 * nh), S, nh);
-    fx_add_staged(fx::region(fx_acc, fx_cidx, kr, 2 * nh), R, nh);
-    fx_add_staged(fx::region(fx_acc, fx_cidx, ko, 2 * nh), O, nh);
-    *applied = true;
-  } else {
-    bool ok = dev::slow_push(c, ks, S);
-    ok = dev::slow_push(c, kr, R) && ok;
-    ok = dev::slow_push(c, ko, O) && ok;
-    *applied = ok;
-  }
-  float z = label > 0.5f ? sc : -sc;
+};
+
+// g = dl * d + gamma * x
+__device__ __forceinline__ float4 grad4(float4 d, float4 x, float dl, float gamma) {
+  return make_float4(fmaf(gamma, x.x, dl * d.x), fmaf(gamma, x.y, dl * d.y), fmaf(gamma, x.z, dl * d.z),
+                     fmaf(gamma, x.w, dl * d.w));
+}
+// BCE loss of a call with score sc
+__device__ __forceinline__ float bce_loss(float sc, bool pos) {
+  const float z = pos ? sc : -sc;
   return __logf(1.f + __expf(-fminf(fmaxf(z, -30.f), 30.f)));
 }
 
-// VPLH = float4 vectors per lane per half-embedding (nh/8 float4 per half); VPLH = 0 -> generic only
-// The kernels run 2 blocks of 256 threads per SM at 128 registers, which use the whole register file.
-// FX: deterministic mode (kge_step_fx_kernel): start-of-step reads, fixed-point sums into fx_acc, call losses.
-template <int VPLH, bool FX>
-__device__ __forceinline__ void
-kge_step_body(const Ctx& c, const Key* __restrict__ subj, const Key* __restrict__ rel, const Key* __restrict__ obj,
-              const float* __restrict__ labels, int n_calls, int nh, float eta, float gamma_e, float gamma_r,
-              float* __restrict__ loss_out, unsigned long long* __restrict__ stats, Dropout de, Dropout dr,
-              long long* __restrict__ fx_acc, const int* __restrict__ fx_cidx, float* __restrict__ call_loss) {
-  extern __shared__ float smem_f[];  // generic path: per warp 6*nh floats
-  dev::cta_enter(c);
-  const int lane = threadIdx.x & 31;
-  const int warp_in_block = threadIdx.x >> 5;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  float* stage = smem_f + (size_t)warp_in_block * 6 * nh;
-  const int H = nh >> 1;
-  const int nvh = H >> 2;
-  float loss_acc = 0.f;
-  unsigned n_local = 0, n_remote = 0, n_slow = 0, n_upd = 0;
+// ComplEx. VPLH = float4 vectors per lane per half-embedding (nh/8 float4 per half); VPLH = 0: no float4 body (nh % 8
+// != 0 or nh > 512), every call takes the generic path. The generic path stages the three rows in the warp's
+// shared memory (6 nh floats per warp, the rule's whole state). The kernels run 2 blocks of 256 threads per SM at 128
+// registers, which use the whole register file.
+template <int VPLH>
+struct ComplEx : TripleRule {
+  static constexpr int kMaxDim = kComplexMaxDim, kBlocksPerSM = 8;
+  static constexpr bool kInPlace = VPLH > 0, kStageInSmem = true;
+  static __host__ __device__ __forceinline__ size_t state_bytes(int nh, int) { return (size_t)6 * nh * sizeof(float); }
+  static __host__ __device__ __forceinline__ size_t warp_bytes(int nh, int n_neg) { return state_bytes(nh, n_neg); }
+  static __host__ __device__ __forceinline__ int scratch_rows(int) { return 0; }
+  static __device__ __forceinline__ int stage_row(int, int i) { return i; }
+  template <bool FX, bool GEN>
+  static __device__ StepOut body(const Ctx& c, const Args& A, int t, const Rows<3>& rows, bool slow,
+                                 const dev::Target* ntg, float* wsm, float* stage);
+};
 
-  for (int p = warp; p < n_calls; p += nwarps) {
-    const Key ks = subj[p], kr = rel[p], ko = obj[p];
-    const float label = labels[p];
-    dev::Target t;
-    t.row = nullptr; t.version = nullptr; t.flag = nullptr;
-    if (VPLH > 0 && lane < 3) {
-      Key k = lane == 0 ? ks : (lane == 1 ? kr : ko);
-      t = dev::resolve_fast(c, k, class_of_key(c, k), &n_local, &n_remote);
+// One call. The generic path (GEN: the three rows are staged in shared memory) runs the scalar body at every VPLH.
+template <int VPLH>
+template <bool FX, bool GEN>
+__device__ __forceinline__ StepOut ComplEx<VPLH>::body(const Ctx&, const Args& A, int t, const Rows<3>& rows, bool,
+                                                       const dev::Target*, float*, float*) {
+  constexpr int V = VPLH > 0 ? VPLH : 1;
+  const int lane = threadIdx.x & 31;
+  const int nh = A.d, H = nh >> 1, nvh = H >> 2;
+  const uint32_t call = (uint32_t)t;
+  float* const ps = rows.p[0];
+  float* const pr = rows.p[1];
+  float* const po = rows.p[2];
+  float4 sre[V], sim[V], rre[V], rim[V], ore[V], oim[V];
+  float sc = 0.f;
+  if constexpr (VPLH == 0 || GEN) {   // scalar, any nh: dropout on the staged rows themselves
+    if (A.de.p > 0.f || A.dr.p > 0.f) {
+      for (int i = lane; i < nh; i += 32) {
+        if (A.de.p > 0.f) { ps[i] *= A.de.keep(call, 0, (uint32_t)i); po[i] *= A.de.keep(call, 2, (uint32_t)i); }
+        if (A.dr.p > 0.f) pr[i] *= A.dr.keep(call, 1, (uint32_t)i);
+      }
+      __syncwarp();
     }
-    float* ps = (float*)__shfl_sync(0xffffffffu, (unsigned long long)t.row, 0);
-    float* pr = (float*)__shfl_sync(0xffffffffu, (unsigned long long)t.row, 1);
-    float* po = (float*)__shfl_sync(0xffffffffu, (unsigned long long)t.row, 2);
-    if (VPLH == 0 || !ps || !pr || !po) {
-      ++n_slow;
-      bool applied;
-      const float l = kge_call_generic<FX>(c, ks, kr, ko, label, nh, eta, gamma_e, gamma_r, stage, &applied,
-                                           (uint32_t)p, de, dr, fx_acc, fx_cidx);
-      if (FX) { if (lane == 0) call_loss[p] = l; }
-      else loss_acc += l;
-      if (applied) n_upd += 3;
-      continue;
-    }
-    constexpr int V = VPLH > 0 ? VPLH : 1;
-    float4 sre[V], sim[V], rre[V], rim[V], ore[V], oim[V];
-    float sc = 0.f;
+    for (int i = lane; i < H; i += 32)
+      sc += pr[i] * ps[i] * po[i] + pr[i] * ps[H + i] * po[H + i] + pr[H + i] * ps[i] * po[H + i] -
+            pr[H + i] * ps[H + i] * po[i];
+  } else {
 #pragma unroll
-    for (int v = 0; v < V; ++v) {
+    for (int v = 0; v < VPLH; ++v) {
       const int j = lane + 32 * v;
       const bool in = j < nvh;
-      const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-      sre[v] = in ? dev::ld_row4(ps + 4 * j) : z; sim[v] = in ? dev::ld_row4(ps + H + 4 * j) : z;
-      rre[v] = in ? dev::ld_row4(pr + 4 * j) : z; rim[v] = in ? dev::ld_row4(pr + H + 4 * j) : z;
-      ore[v] = in ? dev::ld_row4(po + 4 * j) : z; oim[v] = in ? dev::ld_row4(po + H + 4 * j) : z;
-      if (in && (de.p > 0.f || dr.p > 0.f)) {   // dropout on the pulled copies (uniform branch: kernel arguments)
-        const uint32_t e = 4u * (uint32_t)j, cp = (uint32_t)p;
-        sre[v] = de.apply4(sre[v], cp, 0, e); sim[v] = de.apply4(sim[v], cp, 0, (uint32_t)H + e);
-        rre[v] = dr.apply4(rre[v], cp, 1, e); rim[v] = dr.apply4(rim[v], cp, 1, (uint32_t)H + e);
-        ore[v] = de.apply4(ore[v], cp, 2, e); oim[v] = de.apply4(oim[v], cp, 2, (uint32_t)H + e);
+      sre[v] = in ? dev::ld_row4(ps + 4 * j) : f4(0.f); sim[v] = in ? dev::ld_row4(ps + H + 4 * j) : f4(0.f);
+      rre[v] = in ? dev::ld_row4(pr + 4 * j) : f4(0.f); rim[v] = in ? dev::ld_row4(pr + H + 4 * j) : f4(0.f);
+      ore[v] = in ? dev::ld_row4(po + 4 * j) : f4(0.f); oim[v] = in ? dev::ld_row4(po + H + 4 * j) : f4(0.f);
+      if (in && (A.de.p > 0.f || A.dr.p > 0.f)) {   // dropout on the pulled copies (uniform branch: kernel arguments)
+        const uint32_t e = 4u * (uint32_t)j;
+        sre[v] = A.de.apply4(sre[v], call, 0, e); sim[v] = A.de.apply4(sim[v], call, 0, (uint32_t)H + e);
+        rre[v] = A.dr.apply4(rre[v], call, 1, e); rim[v] = A.dr.apply4(rim[v], call, 1, (uint32_t)H + e);
+        ore[v] = A.de.apply4(ore[v], call, 2, e); oim[v] = A.de.apply4(oim[v], call, 2, (uint32_t)H + e);
       }
     }
 #pragma unroll
-    for (int v = 0; v < V; ++v) {
-      float4 a = f4_fma(sre[v], ore[v], f4_mul(sim[v], oim[v]));   // s_re o_re + s_im o_im
-      float4 b = f4_sub(f4_mul(sre[v], oim[v]), f4_mul(sim[v], ore[v]));  // s_re o_im - s_im o_re
-      sc += f4_hsum(f4_fma(rre[v], a, f4_mul(rim[v], b)));
+    for (int v = 0; v < VPLH; ++v) {
+      const float4 a = fma4(sre[v], ore[v], mul4(sim[v], oim[v]));       // s_re o_re + s_im o_im
+      const float4 b = sub4(mul4(sre[v], oim[v]), mul4(sim[v], ore[v]));  // s_re o_im - s_im o_re
+      const float4 u = fma4(rre[v], a, mul4(rim[v], b));
+      sc += u.x + u.y + u.z + u.w;
     }
-    sc = dev::warp_sum(sc);
-    const float dl = 1.f / (1.f + __expf(-sc)) - label;
-    const bool pos = label > 0.5f;
-    const float ge = pos ? gamma_e : 0.f, gr = pos ? gamma_r : 0.f;
-    {
-      float z = pos ? sc : -sc;
-      const float l = __logf(1.f + __expf(-fminf(fmaxf(z, -30.f), 30.f)));
-      if (FX) { if (lane == 0) call_loss[p] = l; }
-      else loss_acc += l;
-    }
-    long long *fs = nullptr, *fr = nullptr, *fo = nullptr;
-    if (FX) {
-      fs = fx::region(fx_acc, fx_cidx, ks, 2 * nh); fr = fx::region(fx_acc, fx_cidx, kr, 2 * nh);
-      fo = fx::region(fx_acc, fx_cidx, ko, 2 * nh);
-    }
-#pragma unroll
-    for (int v = 0; v < V; ++v) {
-      const int j = lane + 32 * v;
-      if (FX && j < nvh) {
-        float4 ds_re = f4_fma(rre[v], ore[v], f4_mul(rim[v], oim[v]));
-        float4 ds_im = f4_sub(f4_mul(rre[v], oim[v]), f4_mul(rim[v], ore[v]));
-        float4 dr_re = f4_fma(sre[v], ore[v], f4_mul(sim[v], oim[v]));
-        float4 dr_im = f4_sub(f4_mul(sre[v], oim[v]), f4_mul(sim[v], ore[v]));
-        float4 do_re = f4_sub(f4_mul(rre[v], sre[v]), f4_mul(rim[v], sim[v]));
-        float4 do_im = f4_fma(rre[v], sim[v], f4_mul(rim[v], sre[v]));
-        // float4 j of the real half, float4 nvh + j of the imaginary half
-        adagrad_fx4(ps + nh + 4 * j, fs, j, nh, ds_re, sre[v], dl, ge, eta);
-        adagrad_fx4(ps + nh + H + 4 * j, fs, nvh + j, nh, ds_im, sim[v], dl, ge, eta);
-        adagrad_fx4(pr + nh + 4 * j, fr, j, nh, dr_re, rre[v], dl, gr, eta);
-        adagrad_fx4(pr + nh + H + 4 * j, fr, nvh + j, nh, dr_im, rim[v], dl, gr, eta);
-        adagrad_fx4(po + nh + 4 * j, fo, j, nh, do_re, ore[v], dl, ge, eta);
-        adagrad_fx4(po + nh + H + 4 * j, fo, nvh + j, nh, do_im, oim[v], dl, ge, eta);
-      } else if (j < nvh) {
-        // gradients of the trilinear score (reference score_grad)
-        float4 ds_re = f4_fma(rre[v], ore[v], f4_mul(rim[v], oim[v]));
-        float4 ds_im = f4_sub(f4_mul(rre[v], oim[v]), f4_mul(rim[v], ore[v]));
-        float4 dr_re = f4_fma(sre[v], ore[v], f4_mul(sim[v], oim[v]));
-        float4 dr_im = f4_sub(f4_mul(sre[v], oim[v]), f4_mul(sim[v], ore[v]));
-        float4 do_re = f4_sub(f4_mul(rre[v], sre[v]), f4_mul(rim[v], sim[v]));
-        float4 do_im = f4_fma(rre[v], sim[v], f4_mul(rim[v], sre[v]));
-        adagrad_push4(ps + 4 * j, ps + nh + 4 * j, ds_re, sre[v], dl, ge, eta);
-        adagrad_push4(ps + H + 4 * j, ps + nh + H + 4 * j, ds_im, sim[v], dl, ge, eta);
-        adagrad_push4(pr + 4 * j, pr + nh + 4 * j, dr_re, rre[v], dl, gr, eta);
-        adagrad_push4(pr + H + 4 * j, pr + nh + H + 4 * j, dr_im, rim[v], dl, gr, eta);
-        adagrad_push4(po + 4 * j, po + nh + 4 * j, do_re, ore[v], dl, ge, eta);
-        adagrad_push4(po + H + 4 * j, po + nh + H + 4 * j, do_im, oim[v], dl, ge, eta);
-      }
-    }
-    if (lane < 3) dev::mark_pushed(t);
-    n_upd += 3;
   }
-
-  __syncwarp();
-  if (!FX && lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
-  dev::flush_stats(stats, n_local, n_remote, n_slow, n_upd);
-  dev::cta_exit(c);
+  sc = dev::warp_sum(sc);
+  const float label = A.labels[t];
+  const float dl = 1.f / (1.f + __expf(-sc)) - label;
+  const bool pos = label > 0.5f;
+  const float ge = pos ? A.gamma_e : 0.f, gr = pos ? A.gamma_r : 0.f;
+  long long *fs = nullptr, *fr = nullptr, *fo = nullptr;
+  if (FX) {
+    fs = fx::region(A.fx_acc, A.fx_cidx, A.subj[t], 2 * nh); fr = fx::region(A.fx_acc, A.fx_cidx, A.rel[t], 2 * nh);
+    fo = fx::region(A.fx_acc, A.fx_cidx, A.obj[t], 2 * nh);
+  }
+  if constexpr (VPLH == 0 || GEN) {
+    for (int i = lane; i < H; i += 32) {
+      float sre = ps[i], sim = ps[H + i], rre = pr[i], rim = pr[H + i], ore = po[i], oim = po[H + i];
+      float d[6] = {rre * ore + rim * oim, rre * oim - rim * ore, sre * ore + sim * oim,
+                    sre * oim - sim * ore, rre * sre - rim * sim, rre * sim + rim * sre};
+      float x[6] = {sre, sim, rre, rim, ore, oim};
+      float gm[6] = {ge, ge, gr, gr, ge, ge};
+      float* rw[6] = {ps, ps, pr, pr, po, po};
+      long long* rg[6] = {fs, fs, fr, fr, fo, fo};
+      int off[6] = {i, H + i, i, H + i, i, H + i};
+#pragma unroll
+      for (int q = 0; q < 6; ++q) {
+        float g = dl * d[q] + gm[q] * x[q];
+        float a = rw[q][nh + off[q]];
+        float ua = g * g;
+        const float ue = -A.eta * g * rsqrtf(a + ua);
+        if (FX) {
+          fx::add1(rg[q], off[q], nh, ue, kFxVal);
+          fx::add1(rg[q] + nh, off[q], nh, ua, kFxAda);
+        } else {
+          rw[q][off[q]] = ue;
+          rw[q][nh + off[q]] = ua;
+        }
+      }
+    }
+  } else {
+    const int nv = nh >> 2;
+#pragma unroll
+    for (int v = 0; v < VPLH; ++v) {
+      const int j = lane + 32 * v;
+      if (j < nvh) {
+        // gradients of the trilinear score (reference score_grad)
+        const float4 ds_re = fma4(rre[v], ore[v], mul4(rim[v], oim[v]));
+        const float4 ds_im = sub4(mul4(rre[v], oim[v]), mul4(rim[v], ore[v]));
+        const float4 dr_re = fma4(sre[v], ore[v], mul4(sim[v], oim[v]));
+        const float4 dr_im = sub4(mul4(sre[v], oim[v]), mul4(sim[v], ore[v]));
+        const float4 do_re = sub4(mul4(rre[v], sre[v]), mul4(rim[v], sim[v]));
+        const float4 do_im = fma4(rre[v], sim[v], mul4(rim[v], sre[v]));
+        // float4 j of the real half, float4 nvh + j of the imaginary half
+        push4<FX>(ps, nh, j, grad4(ds_re, sre[v], dl, ge), false, fs, nv, A.eta, kFxVal, kFxAda, kFxAdaMax);
+        push4<FX>(ps, nh, nvh + j, grad4(ds_im, sim[v], dl, ge), false, fs, nv, A.eta, kFxVal, kFxAda, kFxAdaMax);
+        push4<FX>(pr, nh, j, grad4(dr_re, rre[v], dl, gr), false, fr, nv, A.eta, kFxVal, kFxAda, kFxAdaMax);
+        push4<FX>(pr, nh, nvh + j, grad4(dr_im, rim[v], dl, gr), false, fr, nv, A.eta, kFxVal, kFxAda, kFxAdaMax);
+        push4<FX>(po, nh, j, grad4(do_re, ore[v], dl, ge), false, fo, nv, A.eta, kFxVal, kFxAda, kFxAdaMax);
+        push4<FX>(po, nh, nvh + j, grad4(do_im, oim[v], dl, ge), false, fo, nv, A.eta, kFxVal, kFxAda, kFxAdaMax);
+      }
+    }
+  }
+  return {bce_loss(sc, pos), 0u, 0u, 0ull};
 }
 
 template <int VPLH>
 __global__ void __maxnreg__(128)
-kge_step_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, const Key* __restrict__ rel,
-                const Key* __restrict__ obj, const float* __restrict__ labels, int n_calls, int nh, float eta,
-                float gamma_e, float gamma_r, float* __restrict__ loss_out, unsigned long long* __restrict__ stats,
-                Dropout de, Dropout dr) {
-  kge_step_body<VPLH, false>(c, subj, rel, obj, labels, n_calls, nh, eta, gamma_e, gamma_r, loss_out, stats, de, dr,
-                             nullptr, nullptr, nullptr);
+kge_step_kernel(const __grid_constant__ Ctx c, const __grid_constant__ Args A, float* __restrict__ loss_out,
+                unsigned long long* __restrict__ stats) {
+  warp_step<ComplEx<VPLH>, false>(c, A, loss_out, stats);
 }
 
 template <int VPLH>
 __global__ void __maxnreg__(128)
-kge_step_fx_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, const Key* __restrict__ rel,
-                   const Key* __restrict__ obj, const float* __restrict__ labels, int n_calls, int nh, float eta,
-                   float gamma_e, float gamma_r, unsigned long long* __restrict__ stats, Dropout de, Dropout dr,
-                   long long* __restrict__ fx_acc, const int* __restrict__ fx_cidx, float* __restrict__ call_loss) {
-  kge_step_body<VPLH, true>(c, subj, rel, obj, labels, n_calls, nh, eta, gamma_e, gamma_r, nullptr, stats, de, dr,
-                            fx_acc, fx_cidx, call_loss);
+kge_step_fx_kernel(const __grid_constant__ Ctx c, const __grid_constant__ Args A, float* __restrict__ loss_out,
+                   unsigned long long* __restrict__ stats) {
+  warp_step<ComplEx<VPLH>, true>(c, A, loss_out, stats);
+}
+
+template <bool FX, int VPLH>
+void launch_complex(CudaBackend& be, cudaStream_t stream, const Args& A, float* loss_out, unsigned long long* stats) {
+  if constexpr (FX) launch_step<ComplEx<VPLH>, kge_step_fx_kernel<VPLH>>(be, stream, A, loss_out, stats);
+  else launch_step<ComplEx<VPLH>, kge_step_kernel<VPLH>>(be, stream, A, loss_out, stats);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -303,14 +246,11 @@ kge_step_fx_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, 
 // 2 D^2 floats), gradients d_s = R o, d_o = R^T s, d_R = s o^T (rank 1). One warp per training call:
 //   pass 1  stream R once (16-byte loads, local HBM or NVLink): per float4 a row-dot into ds[i] and four axpy terms
 //           into do[j..j+3] (shared-memory accumulators of the warp) -> score = s . ds
-//   entity rows: AdaGrad + 16-byte reductions for s and o
+//   entity rows: AdaGrad + scalar reductions for s and o
 //   pass 2  stream R's values + accumulators again (L2 hits), form dl * s_i * o_j (+ gamma R_ij), AdaGrad, 16-byte
 //           reductions into both halves of the relation row
-// Rows in a transitional protocol state go through the generic Pull/Push path with a global scratch buffer.
-__device__ __noinline__ bool rescal_slow_rows(const Ctx& c, Key ks, Key kr, Key ko, float* gs, float* gr, float* go) {
-  return dev::slow_pull(c, ks, gs) && dev::slow_pull(c, kr, gr) && dev::slow_pull(c, ko, go);
-}
-
+// The generic path stages the relation row and the two entity rows of a call in global scratch.
+//
 // Deterministic mode (FX, kge_rescal_fx_kernel): pass 1 forms ds and do in a fixed order instead of with shared-memory
 // atomics - the G = D/4 float4 of a matrix row are read by G consecutive lanes, 32/G rows per round; ds[i] is the sum of
 // its G partial dots (shuffle tree for G a power of two, else lane-ordered), each lane keeps its four do partial sums in
@@ -318,195 +258,143 @@ __device__ __noinline__ bool rescal_slow_rows(const Ctx& c, Key ks, Key kr, Key 
 // (relation region [D^2 | D^2], entity regions [D | D]) and each call's loss to its own slot.
 constexpr int kRescalFxSmem = 32 + 128;   // extra floats per warp: ds partials [32] | do partials [32/G][D]
 
-template <bool FX>
-__device__ __forceinline__ void
-kge_rescal_body(const Ctx& c, const Key* __restrict__ subj, const Key* __restrict__ rel, const Key* __restrict__ obj,
-                const float* __restrict__ labels, int n_calls, int D, float eta, float gamma_e, float gamma_r,
-                float* __restrict__ loss_out, unsigned long long* __restrict__ stats, Dropout de, Dropout dr,
-                float* __restrict__ scratch, long long* __restrict__ fx_acc, const int* __restrict__ fx_cidx,
-                float* __restrict__ call_loss) {
-  extern __shared__ float smem_f[];   // per warp: s[D] | o[D] | ds[D] | do[D] (| FX partials)
-  dev::cta_enter(c);
-  const int lane = threadIdx.x & 31;
-  const int wib = threadIdx.x >> 5;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  float* sv = smem_f + (size_t)wib * (FX ? 4 * D + kRescalFxSmem : 4 * D);
-  float* ov = sv + D; float* dsv = ov + D; float* dov = dsv + D;
-  const int DD = D * D;
-  const int nv = DD >> 2;          // float4 of the relation matrix
-  float* my_scratch = scratch + (size_t)warp * (size_t)(2 * DD + 4 * D);   // generic path: rel row | s row | o row
-  float loss_acc = 0.f;
-  unsigned n_local = 0, n_remote = 0, n_slow = 0, n_upd = 0;
+// Per-warp shared memory: s[D] | o[D] | ds[D] | do[D] (| FX partials); DET: the kernel's mode.
+template <bool DET>
+struct Rescal : TripleRule {
+  static constexpr int kMaxDim = kRescalMaxDim, kBlocksPerSM = 4;
+  static constexpr bool kInPlace = true, kStageInSmem = false;
+  static __host__ __device__ __forceinline__ size_t state_bytes(int D, int) {
+    return (size_t)(DET ? 4 * D + kRescalFxSmem : 4 * D) * sizeof(float);
+  }
+  static __host__ __device__ __forceinline__ size_t warp_bytes(int D, int n_neg) { return state_bytes(D, n_neg); }
+  // relation row (D rows of 2 D) | s row | o row
+  static __host__ __device__ __forceinline__ int scratch_rows(int D) { return D + 2; }
+  static __device__ __forceinline__ int stage_row(int D, int i) { return i == 1 ? 0 : D + i / 2; }
+  template <bool FX, bool GEN>
+  static __device__ StepOut body(const Ctx& c, const Args& A, int t, const Rows<3>& rows, bool slow,
+                                 const dev::Target* ntg, float* wsm, float* stage);
+};
 
-  for (int p = warp; p < n_calls; p += nwarps) {
-    const Key ks = subj[p], kr = rel[p], ko = obj[p];
-    const float label = labels[p];
-    dev::Target t;
-    t.row = nullptr; t.version = nullptr; t.flag = nullptr;
-    if (lane < 3) {
-      Key k = lane == 0 ? ks : (lane == 1 ? kr : ko);
-      t = dev::resolve_fast(c, k, class_of_key(c, k), &n_local, &n_remote);
-    }
-    float* ps = (float*)__shfl_sync(0xffffffffu, (unsigned long long)t.row, 0);
-    float* pr = (float*)__shfl_sync(0xffffffffu, (unsigned long long)t.row, 1);
-    float* po = (float*)__shfl_sync(0xffffffffu, (unsigned long long)t.row, 2);
-    const bool slow = !ps || !pr || !po;
-    if (slow) {   // stage the three rows in global scratch and run the same math on the copies
-      ++n_slow;
-      float* gr_ = my_scratch; float* gs_ = my_scratch + 2 * DD; float* go_ = gs_ + 2 * D;
-      if (!rescal_slow_rows(c, ks, kr, ko, gs_, gr_, go_)) {
-        if (FX && lane == 0) call_loss[p] = 0.f;
-        continue;
-      }
-      ps = gs_; pr = gr_; po = go_;
-    }
-    const uint32_t cp = (uint32_t)p;
-    for (int i = lane; i < D; i += 32) {
-      float a = reinterpret_cast<const volatile float*>(ps)[i];
-      float b = reinterpret_cast<const volatile float*>(po)[i];
-      if (de.p > 0.f) { a *= de.keep(cp, 0, (uint32_t)i); b *= de.keep(cp, 2, (uint32_t)i); }
-      sv[i] = a; ov[i] = b; dsv[i] = 0.f; dov[i] = 0.f;
-    }
-    __syncwarp();
-    // ---- pass 1: ds = R o, do = R^T s
-    if (FX) {
-      const int G = D >> 2, rpr = 32 / G;           // float4 per matrix row, rows per round
-      const int rg = lane / G, j = 4 * (lane - rg * G);
-      const bool pow2 = (G & (G - 1)) == 0;
-      float* dsp = dov + D;                         // [32] partial dots
-      float* dop = dsp + 32;                        // [rpr][D] partial do sums
-      float4 dacc = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int i0 = 0; i0 < D; i0 += rpr) {
-        const int i = i0 + rg;
-        float part = 0.f;
-        if (rg < rpr && i < D) {
-          const int e = i * D + j;
-          float4 r4 = dev::ld_row4(pr + e);
-          if (dr.p > 0.f) r4 = dr.apply4(r4, cp, 1, (uint32_t)e);
-          part = r4.x * ov[j] + r4.y * ov[j + 1] + r4.z * ov[j + 2] + r4.w * ov[j + 3];
-          const float si = sv[i];
-          dacc.x += si * r4.x; dacc.y += si * r4.y; dacc.z += si * r4.z; dacc.w += si * r4.w;
-        }
-        if (pow2) {                                 // G | 32: fixed shuffle tree inside each group of G lanes
-          for (int o = G >> 1; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-          if (lane - rg * G == 0 && i < D) dsv[i] = part;
-        } else {
-          dsp[lane] = part;
-          __syncwarp();
-          if (lane < rpr && i0 + lane < D) {
-            float t = 0.f;
-            for (int q = 0; q < G; ++q) t += dsp[lane * G + q];
-            dsv[i0 + lane] = t;
-          }
-          __syncwarp();
-        }
-      }
-      if (rg < rpr) {
-        float* d4 = dop + rg * D + j;
-        d4[0] = dacc.x; d4[1] = dacc.y; d4[2] = dacc.z; d4[3] = dacc.w;
-      }
-      __syncwarp();
-      for (int jj = lane; jj < D; jj += 32) {
-        float t = 0.f;
-        for (int r = 0; r < rpr; ++r) t += dop[r * D + jj];
-        dov[jj] = t;
-      }
-    } else {
-      for (int q = lane; q < nv; q += 32) {
-        const int e = 4 * q, i = e / D, j = e - i * D;
+template <bool DET>
+template <bool FX, bool GEN>
+__device__ __forceinline__ StepOut Rescal<DET>::body(const Ctx&, const Args& A, int t, const Rows<3>& rows, bool slow,
+                                                     const dev::Target*, float* wsm, float*) {
+  static_assert(FX == DET, "the shared-memory layout follows the mode");
+  const int lane = threadIdx.x & 31;
+  const int D = A.d, DD = D * D;
+  const int nv = DD >> 2;          // float4 of the relation matrix
+  float* const ps = rows.p[0];
+  float* const pr = rows.p[1];
+  float* const po = rows.p[2];
+  float* const sv = wsm; float* const ov = sv + D; float* const dsv = ov + D; float* const dov = dsv + D;
+  const float label = A.labels[t];
+  const uint32_t cp = (uint32_t)t;
+  for (int i = lane; i < D; i += 32) {
+    float a = reinterpret_cast<const volatile float*>(ps)[i];
+    float b = reinterpret_cast<const volatile float*>(po)[i];
+    if (A.de.p > 0.f) { a *= A.de.keep(cp, 0, (uint32_t)i); b *= A.de.keep(cp, 2, (uint32_t)i); }
+    sv[i] = a; ov[i] = b; dsv[i] = 0.f; dov[i] = 0.f;
+  }
+  __syncwarp();
+  // ---- pass 1: ds = R o, do = R^T s
+  if (FX) {
+    const int G = D >> 2, rpr = 32 / G;           // float4 per matrix row, rows per round
+    const int rg = lane / G, j = 4 * (lane - rg * G);
+    const bool pow2 = (G & (G - 1)) == 0;
+    float* dsp = dov + D;                         // [32] partial dots
+    float* dop = dsp + 32;                        // [rpr][D] partial do sums
+    float4 dacc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int i0 = 0; i0 < D; i0 += rpr) {
+      const int i = i0 + rg;
+      float part = 0.f;
+      if (rg < rpr && i < D) {
+        const int e = i * D + j;
         float4 r4 = dev::ld_row4(pr + e);
-        if (dr.p > 0.f) r4 = dr.apply4(r4, cp, 1, (uint32_t)e);
+        if (A.dr.p > 0.f) r4 = A.dr.apply4(r4, cp, 1, (uint32_t)e);
+        part = r4.x * ov[j] + r4.y * ov[j + 1] + r4.z * ov[j + 2] + r4.w * ov[j + 3];
         const float si = sv[i];
-        atomicAdd(dsv + i, r4.x * ov[j] + r4.y * ov[j + 1] + r4.z * ov[j + 2] + r4.w * ov[j + 3]);
-        atomicAdd(dov + j, si * r4.x); atomicAdd(dov + j + 1, si * r4.y);
-        atomicAdd(dov + j + 2, si * r4.z); atomicAdd(dov + j + 3, si * r4.w);
+        dacc.x += si * r4.x; dacc.y += si * r4.y; dacc.z += si * r4.z; dacc.w += si * r4.w;
+      }
+      if (pow2) {                                 // G | 32: fixed shuffle tree inside each group of G lanes
+        for (int o = G >> 1; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+        if (lane - rg * G == 0 && i < D) dsv[i] = part;
+      } else {
+        dsp[lane] = part;
+        __syncwarp();
+        if (lane < rpr && i0 + lane < D) {
+          float acc = 0.f;
+          for (int q = 0; q < G; ++q) acc += dsp[lane * G + q];
+          dsv[i0 + lane] = acc;
+        }
+        __syncwarp();
       }
     }
+    if (rg < rpr) {
+      float* d4 = dop + rg * D + j;
+      d4[0] = dacc.x; d4[1] = dacc.y; d4[2] = dacc.z; d4[3] = dacc.w;
+    }
     __syncwarp();
-    float sc = 0.f;
-    for (int i = lane; i < D; i += 32) sc += sv[i] * dsv[i];
-    sc = dev::warp_sum(sc);
-    const float dl = 1.f / (1.f + __expf(-sc)) - label;
-    const bool pos = label > 0.5f;
-    const float ge = pos ? gamma_e : 0.f, grr = pos ? gamma_r : 0.f;
-    {
-      float z = pos ? sc : -sc;
-      const float l = __logf(1.f + __expf(-fminf(fmaxf(z, -30.f), 30.f)));
-      if (FX) { if (lane == 0) call_loss[p] = l; }
-      else loss_acc += l;
+    for (int jj = lane; jj < D; jj += 32) {
+      float acc = 0.f;
+      for (int r = 0; r < rpr; ++r) acc += dop[r * D + jj];
+      dov[jj] = acc;
     }
-    long long *fs = nullptr, *fr = nullptr, *fo = nullptr;
-    if (FX) {   // regions in units of an entity row (2 D): relation regions are D units
-      fs = fx::region(fx_acc, fx_cidx, ks, 2 * D); fr = fx::region(fx_acc, fx_cidx, kr, 2 * D);
-      fo = fx::region(fx_acc, fx_cidx, ko, 2 * D);
-    }
-    // ---- entity rows
-    for (int i = lane; i < D; i += 32) {
-      const float g_s = fmaf(ge, sv[i], dl * dsv[i]), g_o = fmaf(ge, ov[i], dl * dov[i]);
-      const float a_s = reinterpret_cast<const volatile float*>(ps)[D + i], a_o = reinterpret_cast<const volatile float*>(po)[D + i];
-      const float us = -eta * g_s * rsqrtf(a_s + g_s * g_s), uo = -eta * g_o * rsqrtf(a_o + g_o * g_o);
-      if (FX) {
-        fx::add1(fs, i, D, us, kFxVal); fx::add1(fs + D, i, D, g_s * g_s, kFxAda);
-        fx::add1(fo, i, D, uo, kFxVal); fx::add1(fo + D, i, D, g_o * g_o, kFxAda);
-      } else if (slow) { ps[i] = us; ps[D + i] = g_s * g_s; po[i] = uo; po[D + i] = g_o * g_o; }
-      else { mem::red_add(ps + i, us); mem::red_add(ps + D + i, g_s * g_s); mem::red_add(po + i, uo); mem::red_add(po + D + i, g_o * g_o); }
-    }
-    // ---- pass 2: relation matrix update (rank-1 gradient)
+  } else {
     for (int q = lane; q < nv; q += 32) {
       const int e = 4 * q, i = e / D, j = e - i * D;
       float4 r4 = dev::ld_row4(pr + e);
-      if (dr.p > 0.f) r4 = dr.apply4(r4, cp, 1, (uint32_t)e);
-      const float4 a4 = dev::ld_row4(pr + DD + e);
-      const float w = dl * sv[i];
-      const float4 g = make_float4(fmaf(grr, r4.x, w * ov[j]), fmaf(grr, r4.y, w * ov[j + 1]), fmaf(grr, r4.z, w * ov[j + 2]),
-                                   fmaf(grr, r4.w, w * ov[j + 3]));
-      const float4 ua = f4_mul(g, g);
-      const float4 ue = make_float4(-eta * g.x * rsqrtf(a4.x + ua.x), -eta * g.y * rsqrtf(a4.y + ua.y),
-                                    -eta * g.z * rsqrtf(a4.z + ua.z), -eta * g.w * rsqrtf(a4.w + ua.w));
-      if (FX) { fx::add4(fr, q, nv, ue, kFxVal); fx::add4(fr + DD, q, nv, ua, kFxAda); }
-      else if (slow) { *reinterpret_cast<float4*>(pr + e) = ue; *reinterpret_cast<float4*>(pr + DD + e) = ua; }
-      else { dev::red_row4(pr + e, ue); dev::red_row4(pr + DD + e, ua); }
+      if (A.dr.p > 0.f) r4 = A.dr.apply4(r4, cp, 1, (uint32_t)e);
+      const float si = sv[i];
+      atomicAdd(dsv + i, r4.x * ov[j] + r4.y * ov[j + 1] + r4.z * ov[j + 2] + r4.w * ov[j + 3]);
+      atomicAdd(dov + j, si * r4.x); atomicAdd(dov + j + 1, si * r4.y);
+      atomicAdd(dov + j + 2, si * r4.z); atomicAdd(dov + j + 3, si * r4.w);
     }
-    if (FX) {
-      if (lane < 3 && !slow) dev::mark_pushed(t);
-      n_upd += 3;
-    } else if (slow) {
-      __syncwarp();
-      bool ok = dev::slow_push(c, ks, ps);
-      ok = dev::slow_push(c, kr, pr) && ok;
-      ok = dev::slow_push(c, ko, po) && ok;
-      if (ok) n_upd += 3;
-    } else {
-      if (lane < 3) dev::mark_pushed(t);
-      n_upd += 3;
-    }
-    __syncwarp();
   }
-
   __syncwarp();
-  if (!FX && lane == 0 && loss_out) atomicAdd(loss_out, loss_acc);
-  dev::flush_stats(stats, n_local, n_remote, n_slow, n_upd);
-  dev::cta_exit(c);
+  float sc = 0.f;
+  for (int i = lane; i < D; i += 32) sc += sv[i] * dsv[i];
+  sc = dev::warp_sum(sc);
+  const float dl = 1.f / (1.f + __expf(-sc)) - label;
+  const bool pos = label > 0.5f;
+  const float ge = pos ? A.gamma_e : 0.f, grr = pos ? A.gamma_r : 0.f;
+  long long *fs = nullptr, *fr = nullptr, *fo = nullptr;
+  if (FX) {   // regions in units of an entity row (2 D): relation regions are D units
+    fs = fx::region(A.fx_acc, A.fx_cidx, A.subj[t], 2 * D); fr = fx::region(A.fx_acc, A.fx_cidx, A.rel[t], 2 * D);
+    fo = fx::region(A.fx_acc, A.fx_cidx, A.obj[t], 2 * D);
+  }
+  // ---- entity rows
+  for (int i = lane; i < D; i += 32) {
+    const float g_s = fmaf(ge, sv[i], dl * dsv[i]), g_o = fmaf(ge, ov[i], dl * dov[i]);
+    const float a_s = reinterpret_cast<const volatile float*>(ps)[D + i], a_o = reinterpret_cast<const volatile float*>(po)[D + i];
+    const float us = -A.eta * g_s * rsqrtf(a_s + g_s * g_s), uo = -A.eta * g_o * rsqrtf(a_o + g_o * g_o);
+    if (FX) {
+      fx::add1(fs, i, D, us, kFxVal); fx::add1(fs + D, i, D, g_s * g_s, kFxAda);
+      fx::add1(fo, i, D, uo, kFxVal); fx::add1(fo + D, i, D, g_o * g_o, kFxAda);
+    } else if (slow) { ps[i] = us; ps[D + i] = g_s * g_s; po[i] = uo; po[D + i] = g_o * g_o; }
+    else { mem::red_add(ps + i, us); mem::red_add(ps + D + i, g_s * g_s); mem::red_add(po + i, uo); mem::red_add(po + D + i, g_o * g_o); }
+  }
+  // ---- pass 2: relation matrix update (rank-1 gradient)
+  for (int q = lane; q < nv; q += 32) {
+    const int e = 4 * q, i = e / D, j = e - i * D;
+    float4 r4 = dev::ld_row4(pr + e);
+    if (A.dr.p > 0.f) r4 = A.dr.apply4(r4, cp, 1, (uint32_t)e);
+    const float4 a4 = dev::ld_row4(pr + DD + e);
+    const float4 g = grad4(make_float4(ov[j], ov[j + 1], ov[j + 2], ov[j + 3]), r4, dl * sv[i], grr);
+    push4<FX>(pr, DD, q, g, a4, slow, fr, nv, A.eta, kFxVal, kFxAda, kFxAdaMax);
+  }
+  return {bce_loss(sc, pos), 0u, 0u, 0ull};
 }
 
-__global__ void __launch_bounds__(kThreads)
-kge_rescal_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, const Key* __restrict__ rel,
-                  const Key* __restrict__ obj, const float* __restrict__ labels, int n_calls, int D, float eta,
-                  float gamma_e, float gamma_r, float* __restrict__ loss_out, unsigned long long* __restrict__ stats,
-                  Dropout de, Dropout dr, float* __restrict__ scratch) {
-  kge_rescal_body<false>(c, subj, rel, obj, labels, n_calls, D, eta, gamma_e, gamma_r, loss_out, stats, de, dr, scratch,
-                         nullptr, nullptr, nullptr);
+__global__ void __launch_bounds__(kStepThreads)
+kge_rescal_kernel(const __grid_constant__ Ctx c, const __grid_constant__ Args A, float* __restrict__ loss_out,
+                  unsigned long long* __restrict__ stats) {
+  warp_step<Rescal<false>, false>(c, A, loss_out, stats);
 }
 
-__global__ void __launch_bounds__(kThreads)
-kge_rescal_fx_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ subj, const Key* __restrict__ rel,
-                     const Key* __restrict__ obj, const float* __restrict__ labels, int n_calls, int D, float eta,
-                     float gamma_e, float gamma_r, unsigned long long* __restrict__ stats, Dropout de, Dropout dr,
-                     float* __restrict__ scratch, long long* __restrict__ fx_acc, const int* __restrict__ fx_cidx,
-                     float* __restrict__ call_loss) {
-  kge_rescal_body<true>(c, subj, rel, obj, labels, n_calls, D, eta, gamma_e, gamma_r, nullptr, stats, de, dr, scratch,
-                        fx_acc, fx_cidx, call_loss);
+__global__ void __launch_bounds__(kStepThreads)
+kge_rescal_fx_kernel(const __grid_constant__ Ctx c, const __grid_constant__ Args A, float* __restrict__ loss_out,
+                     unsigned long long* __restrict__ stats) {
+  warp_step<Rescal<true>, true>(c, A, loss_out, stats);
 }
 
 }  // namespace
@@ -525,52 +413,25 @@ void kge_complex_step(CudaBackend& be, cudaStream_t stream, const Key* subj, con
                       const float* labels, int n_calls, int nh, float eta, float gamma_e, float gamma_r, float* loss_out,
                       unsigned long long* stats, float dropout_e, float dropout_r, uint64_t seed, bool deterministic) {
   if (n_calls == 0) return;
-  const Dropout de = make_dropout(dropout_e, seed, 0x11u), dr = make_dropout(dropout_r, seed, 0x22u);
+  Args A;
+  A.de = make_dropout(dropout_e, seed, 0x11u); A.dr = make_dropout(dropout_r, seed, 0x22u);
   ADAPM_CHECK(nh % 2 == 0, "ComplEx needs an even embedding size");
-  ADAPM_CHECK(be.ctx().L.val_bytes == 4, "the fused ops need float32 rows (Options::dtype)");
-  be.track_stream(stream);
-  const Ctx& c = be.ctx();
-  const int warps_per_block = kThreads / 32;
-  int blocks = std::min((n_calls + warps_per_block - 1) / warps_per_block, be.num_sms() * 8);
-  size_t smem = (size_t)warps_per_block * 6 * nh * sizeof(float);
-  ADAPM_CHECK(smem <= 200 * 1024, "kge_complex_step: embedding size too large for the staging buffer");
-  const int nvh = nh / 8;
-  int vplh = (nh % 8 == 0) ? (nvh + 31) / 32 : 0;
+  ADAPM_CHECK(kStepThreads / 32 * ComplEx<0>::warp_bytes(nh, 0) <= 200 * 1024,
+              "kge_complex_step: embedding size too large for the staging buffer");
+  int vplh = (nh % 8 == 0) ? (nh / 8 + 31) / 32 : 0;
   if (vplh > 2) vplh = 0;
-#define ADAPM_LAUNCH_KGE(V)                                                                                    \
-  do {                                                                                                         \
-    set_max_dynamic_smem<kge_step_kernel<V>>(200 * 1024);                                                      \
-    kge_step_kernel<V><<<blocks, kThreads, smem, stream>>>(c, subj, rel, obj, labels, n_calls, nh, eta,        \
-                                                           gamma_e, gamma_r, loss_out, stats, de, dr);         \
-  } while (0)
-#define ADAPM_LAUNCH_KGE_FX(V)                                                                                 \
-  do {                                                                                                         \
-    set_max_dynamic_smem<kge_step_fx_kernel<V>>(200 * 1024);                                                   \
-    kge_step_fx_kernel<V><<<blocks, kThreads, smem, stream>>>(c, subj, rel, obj, labels, n_calls, nh, eta,     \
-                                                              gamma_e, gamma_r, stats, de, dr, fxs->acc,       \
-                                                              fxs->cidx, fxs->call_loss);                      \
-  } while (0)
-  if (deterministic) {
-    // one GPU, start-of-step reads: every key gets a [nh | nh] accumulator region (entity and relation rows alike)
-    const fx::Source src[3] = {{subj, n_calls, 1}, {rel, n_calls, 1}, {obj, n_calls, 1}};
-    CudaBackend::FxScratch* fxs = &fx::begin(be, stream, src, 3, 2 * nh, n_calls);
+  A.subj = subj; A.rel = rel; A.obj = obj; A.labels = labels; A.B = n_calls; A.n_neg = 0; A.d = nh;
+  A.eta = eta; A.gamma_e = gamma_e; A.gamma_r = gamma_r;
+  // deterministic: every key gets a [nh | nh] accumulator region (entity and relation rows alike)
+  const fx::Source src[3] = {{subj, n_calls, 1}, {rel, n_calls, 1}, {obj, n_calls, 1}};
+  run_step(be, stream, A, deterministic, src, 3, 2 * nh, kFxVal, kFxAda, loss_out, [&](auto fx, float* lo) {
+    constexpr bool FX = decltype(fx)::value;
     switch (vplh) {
-      case 1: ADAPM_LAUNCH_KGE_FX(1); break;
-      case 2: ADAPM_LAUNCH_KGE_FX(2); break;
-      default: ADAPM_LAUNCH_KGE_FX(0); break;
+      case 1: launch_complex<FX, 1>(be, stream, A, lo, stats); break;
+      case 2: launch_complex<FX, 2>(be, stream, A, lo, stats); break;
+      default: launch_complex<FX, 0>(be, stream, A, lo, stats); break;
     }
-    ADAPM_COUNT_LAUNCH();
-    ADAPM_CUDA_CHECK(cudaGetLastError());
-    fx::apply(be, stream, 2 * nh, kFxVal, kFxAda, 0.f, n_calls, loss_out);
-    return;
-  }
-  switch (vplh) {
-    case 1: ADAPM_LAUNCH_KGE(1); break;
-    case 2: ADAPM_LAUNCH_KGE(2); break;
-    default: ADAPM_LAUNCH_KGE(0); break;
-  }
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_CUDA_CHECK(cudaGetLastError());
+  });
 }
 
 // RESCAL training calls: entity rows 2*D floats, relation rows 2*D*D floats (D % 4 == 0, D <= 128).
@@ -578,45 +439,18 @@ void kge_rescal_step(CudaBackend& be, cudaStream_t stream, const Key* subj, cons
                      const float* labels, int n_calls, int D, float eta, float gamma_e, float gamma_r, float* loss_out,
                      unsigned long long* stats, float dropout_e, float dropout_r, uint64_t seed, bool deterministic) {
   if (n_calls == 0) return;
-  ADAPM_CHECK(D % 4 == 0 && D >= 4 && D <= 128, "kge_rescal_step: embedding size must be a multiple of 4 in [4, 128]");
-  ADAPM_CHECK(be.ctx().L.val_bytes == 4, "the fused ops need float32 rows (Options::dtype)");
-  be.track_stream(stream);
-  const Ctx& c = be.ctx();
-  const Dropout de = make_dropout(dropout_e, seed, 0x11u), dr = make_dropout(dropout_r, seed, 0x22u);
-  const int warps_per_block = kThreads / 32;
-  const int blocks = std::min((n_calls + warps_per_block - 1) / warps_per_block, be.num_sms() * 4);
-  const size_t smem = (size_t)warps_per_block * (deterministic ? 4 * D + kRescalFxSmem : 4 * D) * sizeof(float);
-  // generic-path scratch (rows in a transitional protocol state): one relation row + two entity rows per warp
-  static std::mutex mu;
-  static std::map<int, std::pair<float*, size_t>> scratch_by_dev;
-  float* scratch = nullptr;
-  {
-    std::lock_guard<std::mutex> lk(mu);
-    const size_t need = (size_t)blocks * warps_per_block * (size_t)(2 * D * D + 4 * D) * sizeof(float);
-    auto& e = scratch_by_dev[be.device()];
-    if (e.second < need) {
-      if (e.first) cudaFree(e.first);
-      ADAPM_CUDA_CHECK(cudaMalloc((void**)&e.first, need));
-      e.second = need;
-    }
-    scratch = e.first;
-  }
-  if (deterministic) {
-    // one GPU, start-of-step reads: entity regions [D | D] (one unit), relation regions [D^2 | D^2] (D units)
-    const fx::Source src[3] = {{subj, n_calls, 1}, {obj, n_calls, 1}, {rel, n_calls, D}};
-    CudaBackend::FxScratch& fxs = fx::begin(be, stream, src, 3, 2 * D, n_calls);
-    kge_rescal_fx_kernel<<<blocks, kThreads, smem, stream>>>(c, subj, rel, obj, labels, n_calls, D, eta, gamma_e,
-                                                             gamma_r, stats, de, dr, scratch, fxs.acc, fxs.cidx,
-                                                             fxs.call_loss);
-    ADAPM_COUNT_LAUNCH();
-    ADAPM_CUDA_CHECK(cudaGetLastError());
-    fx::apply(be, stream, 2 * D, kFxVal, kFxAda, 0.f, n_calls, loss_out);
-    return;
-  }
-  kge_rescal_kernel<<<blocks, kThreads, smem, stream>>>(c, subj, rel, obj, labels, n_calls, D, eta, gamma_e, gamma_r,
-                                                        loss_out, stats, de, dr, scratch);
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_CUDA_CHECK(cudaGetLastError());
+  ADAPM_CHECK(D % 4 == 0 && D >= 4 && D <= kRescalMaxDim,
+              "kge_rescal_step: embedding size must be a multiple of 4 in [4, 128]");
+  Args A;
+  A.de = make_dropout(dropout_e, seed, 0x11u); A.dr = make_dropout(dropout_r, seed, 0x22u);
+  A.subj = subj; A.rel = rel; A.obj = obj; A.labels = labels; A.B = n_calls; A.n_neg = 0; A.d = D;
+  A.eta = eta; A.gamma_e = gamma_e; A.gamma_r = gamma_r;
+  // deterministic: entity regions [D | D] (one unit), relation regions [D^2 | D^2] (D units)
+  const fx::Source src[3] = {{subj, n_calls, 1}, {obj, n_calls, 1}, {rel, n_calls, D}};
+  run_step(be, stream, A, deterministic, src, 3, 2 * D, kFxVal, kFxAda, loss_out, [&](auto fx, float* lo) {
+    if constexpr (decltype(fx)::value) launch_step<Rescal<true>, kge_rescal_fx_kernel>(be, stream, A, lo, stats);
+    else launch_step<Rescal<false>, kge_rescal_kernel>(be, stream, A, lo, stats);
+  });
 }
 
 }  // namespace cudaops

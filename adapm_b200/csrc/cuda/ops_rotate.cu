@@ -128,7 +128,8 @@ struct Args {
 // g_s | g_o (d each) | g_theta (m) | distance / dL/dD of every negative (n_neg) | the negatives' targets.
 template <int VPL>
 struct RotatE {
-  static constexpr int kPositives = 3, kMaxDim = kRotatEMaxDim, kMaxNeg = kRotatEMaxNeg;
+  static constexpr int kPositives = 3, kMaxDim = kRotatEMaxDim, kMaxNeg = kRotatEMaxNeg, kBlocksPerSM = 4;
+  static constexpr bool kInPlace = true, kStageInSmem = false;
   static __device__ __forceinline__ Key positive(const Args& A, int t, int i) {
     return i == 0 ? A.subj[t] : (i == 1 ? A.rel[t] : A.obj[t]);
   }
@@ -138,6 +139,8 @@ struct RotatE {
   static __host__ __device__ __forceinline__ size_t warp_bytes(int d, int n_neg) {
     return (state_bytes(d, n_neg) + (size_t)n_neg * sizeof(dev::Target) + 15) & ~(size_t)15;
   }
+  static __host__ __device__ __forceinline__ int scratch_rows(int) { return kPositives + 1; }
+  static __device__ __forceinline__ int stage_row(int, int i) { return i; }
   static __device__ __forceinline__ bool neg_pushed(const StepOut&, int) { return true; }
   template <bool FX, bool GEN>
   static __device__ StepOut body(const Ctx& c, const Args& A, int t, const Rows<3>& rows, bool slow,
@@ -311,13 +314,13 @@ rotate_step_kernel(const __grid_constant__ Ctx c, const __grid_constant__ Args A
 }
 
 template <bool FX>
-void launch_shape(int vpl, cudaStream_t stream, int blocks, const Ctx& c, const Args& A, float* loss_out,
+void launch_shape(int vpl, CudaBackend& be, cudaStream_t stream, const Args& A, float* loss_out,
                   unsigned long long* stats) {
   switch (vpl) {
-    case 1: launch_step<RotatE<1>, rotate_step_kernel<1, FX>>(stream, blocks, c, A, loss_out, stats); break;
-    case 2: launch_step<RotatE<2>, rotate_step_kernel<2, FX>>(stream, blocks, c, A, loss_out, stats); break;
-    case 3: launch_step<RotatE<3>, rotate_step_kernel<3, FX>>(stream, blocks, c, A, loss_out, stats); break;
-    default: launch_step<RotatE<4>, rotate_step_kernel<4, FX>>(stream, blocks, c, A, loss_out, stats); break;
+    case 1: launch_step<RotatE<1>, rotate_step_kernel<1, FX>>(be, stream, A, loss_out, stats); break;
+    case 2: launch_step<RotatE<2>, rotate_step_kernel<2, FX>>(be, stream, A, loss_out, stats); break;
+    case 3: launch_step<RotatE<3>, rotate_step_kernel<3, FX>>(be, stream, A, loss_out, stats); break;
+    default: launch_step<RotatE<4>, rotate_step_kernel<4, FX>>(be, stream, A, loss_out, stats); break;
   }
 }
 
@@ -337,8 +340,8 @@ void kge_rotate_step(CudaBackend& be, cudaStream_t stream, const Key* subj, cons
   A.margin = margin; A.alpha = alpha; A.eta = eta; A.gamma_e = gamma_e;
   // deterministic: entity keys get a [d | d] region (2 units), relation keys a [m | m] region (1 unit)
   const fx::Source src[4] = {{subj, B, 2}, {rel, B, 1}, {obj, B, 2}, {neg, (long)B * n_neg, 2}};
-  run_step<3>(be, stream, A, deterministic, src, 4, d, kFxVal, kFxAda, loss_out, [&](auto fx, int blocks, float* lo) {
-    launch_shape<decltype(fx)::value>(vpl, stream, blocks, be.ctx(), A, lo, stats);
+  run_step(be, stream, A, deterministic, src, 4, d, kFxVal, kFxAda, loss_out, [&](auto fx, float* lo) {
+    launch_shape<decltype(fx)::value>(vpl, be, stream, A, lo, stats);
   });
 }
 

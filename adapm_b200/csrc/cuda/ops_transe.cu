@@ -103,7 +103,8 @@ struct Args {
 // x | U_o | U_s (d each; each lane touches only its own float4s) | the negatives' targets.
 template <int VPL, int P>
 struct TransE {
-  static constexpr int kPositives = 3, kMaxDim = kTransEMaxDim, kMaxNeg = kTransEMaxNeg;
+  static constexpr int kPositives = 3, kMaxDim = kTransEMaxDim, kMaxNeg = kTransEMaxNeg, kBlocksPerSM = 4;
+  static constexpr bool kInPlace = true, kStageInSmem = false;
   static __device__ __forceinline__ Key positive(const Args& A, int t, int i) {
     return i == 0 ? A.subj[t] : (i == 1 ? A.rel[t] : A.obj[t]);
   }
@@ -111,6 +112,8 @@ struct TransE {
   static __host__ __device__ __forceinline__ size_t warp_bytes(int d, int n_neg) {
     return state_bytes(d, n_neg) + (size_t)n_neg * sizeof(dev::Target);
   }
+  static __host__ __device__ __forceinline__ int scratch_rows(int) { return kPositives + 1; }
+  static __device__ __forceinline__ int stage_row(int, int i) { return i; }
   // an inactive pair pushes nothing (n_neg <= 64: one bit per negative)
   static __device__ __forceinline__ bool neg_pushed(const StepOut& r, int q) { return r.pushed >> q & 1ull; }
   template <bool FX, bool GEN>
@@ -257,20 +260,19 @@ transe_step_kernel(const __grid_constant__ Ctx c, const __grid_constant__ Args A
 }
 
 template <int VPL, bool FX>
-void launch_p(int p, cudaStream_t stream, int blocks, const Ctx& c, const Args& A, float* loss_out,
-              unsigned long long* stats) {
-  if (p == 1) launch_step<TransE<VPL, 1>, transe_step_kernel<VPL, 1, FX>>(stream, blocks, c, A, loss_out, stats);
-  else launch_step<TransE<VPL, 2>, transe_step_kernel<VPL, 2, FX>>(stream, blocks, c, A, loss_out, stats);
+void launch_p(int p, CudaBackend& be, cudaStream_t stream, const Args& A, float* loss_out, unsigned long long* stats) {
+  if (p == 1) launch_step<TransE<VPL, 1>, transe_step_kernel<VPL, 1, FX>>(be, stream, A, loss_out, stats);
+  else launch_step<TransE<VPL, 2>, transe_step_kernel<VPL, 2, FX>>(be, stream, A, loss_out, stats);
 }
 
 template <bool FX>
-void launch_shape(int vpl, int p, cudaStream_t stream, int blocks, const Ctx& c, const Args& A, float* loss_out,
+void launch_shape(int vpl, int p, CudaBackend& be, cudaStream_t stream, const Args& A, float* loss_out,
                   unsigned long long* stats) {
   switch (vpl) {
-    case 1: launch_p<1, FX>(p, stream, blocks, c, A, loss_out, stats); break;
-    case 2: launch_p<2, FX>(p, stream, blocks, c, A, loss_out, stats); break;
-    case 3: launch_p<3, FX>(p, stream, blocks, c, A, loss_out, stats); break;
-    default: launch_p<4, FX>(p, stream, blocks, c, A, loss_out, stats); break;
+    case 1: launch_p<1, FX>(p, be, stream, A, loss_out, stats); break;
+    case 2: launch_p<2, FX>(p, be, stream, A, loss_out, stats); break;
+    case 3: launch_p<3, FX>(p, be, stream, A, loss_out, stats); break;
+    default: launch_p<4, FX>(p, be, stream, A, loss_out, stats); break;
   }
 }
 
@@ -291,8 +293,8 @@ void kge_transe_step(CudaBackend& be, cudaStream_t stream, const Key* subj, cons
   A.margin = margin; A.eta = eta; A.gamma_e = gamma_e; A.gamma_r = gamma_r;
   // deterministic: every key (entity or relation, both 2 d long) gets a [d | d] region
   const fx::Source src[4] = {{subj, B, 1}, {rel, B, 1}, {obj, B, 1}, {neg, (long)B * n_neg, 1}};
-  run_step<3>(be, stream, A, deterministic, src, 4, 2 * d, kFxVal, kFxAda, loss_out, [&](auto fx, int blocks, float* lo) {
-    launch_shape<decltype(fx)::value>(vpl, p, stream, blocks, be.ctx(), A, lo, stats);
+  run_step(be, stream, A, deterministic, src, 4, 2 * d, kFxVal, kFxAda, loss_out, [&](auto fx, float* lo) {
+    launch_shape<decltype(fx)::value>(vpl, p, be, stream, A, lo, stats);
   });
 }
 
