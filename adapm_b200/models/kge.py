@@ -151,7 +151,7 @@ class KGE:
         self.cuda = server.backend == "cuda" and server.dtype == torch.float32
         self.dtype = server.dtype
         self.step_no = 0
-        self.pushes = 0                 # TransE on the CPU route: rows pushed so far (3 per triple + active negatives)
+        self.pushes = 0                 # TransE / RotatE on the CPU route: rows pushed so far
         dev = server.device
         self._gen = torch.Generator().manual_seed(cfg.model_seed + 31 * server.my_rank())
         if self.cuda:
@@ -236,86 +236,51 @@ class KGE:
         L[:, 0] = 1
         return S.reshape(-1), R.reshape(-1).contiguous(), O.reshape(-1), L.reshape(-1)
 
+    def _negatives(self, B: int):
+        """The step's seed and its ``[B, 2 * neg_ratio]`` uniform negative entities, in the layout of ``_expand``
+        (corrupted objects first): the device sampler on CUDA (local keys only under the local scheme on several ranks),
+        else the rank's generator."""
+        cfg = self.cfg
+        seed = (cfg.model_seed * 7 + self.server.my_rank() * 7919 + self.step_no) & 0xFFFFFFFFFFFF
+        if self.cuda:
+            local_only = cfg.sampling_scheme == "local" and self.server.num_servers() > 1
+            return seed, self.sampler.sample(B * 2 * cfg.neg_ratio, seed, local_only=local_only).view(B, 2 * cfg.neg_ratio)
+        return seed, torch.randint(0, cfg.num_entities, (B, 2 * cfg.neg_ratio), generator=self._gen)
+
     def step(self, triples_host: torch.Tensor) -> torch.Tensor:
-        """One batch of positive triples ([B,3] int64 CPU tensor, pinned for the e2e path)."""
-        cfg = self.cfg
-        B = triples_host.shape[0]
-        if cfg.algorithm == "TransE":
-            return self._step_transe(triples_host)
-        if cfg.algorithm == "RotatE":
-            return self._step_rotate(triples_host)
-        if self.cuda:
-            from ..ops import kge_complex_step, kge_rescal_step
+        """One batch of positive triples ([B,3] int64 CPU tensor, pinned for the e2e path): one fused launch on CUDA,
+        else the float64-capable reference rule through Pull/Push. ComplEx and RESCAL train the calls of ``_expand`` with
+        dropout; TransE and RotatE train each positive against its ``2 * neg_ratio`` negatives and have no dropout."""
+        from .. import ops
 
-            tr = triples_host.to(self.server.device, non_blocking=True)
-            local_only = cfg.sampling_scheme == "local" and self.server.num_servers() > 1
-            seed = (cfg.model_seed * 7 + self.server.my_rank() * 7919 + self.step_no) & 0xFFFFFFFFFFFF
-            neg = self.sampler.sample(B * 2 * cfg.neg_ratio, seed, local_only=local_only).view(B, 2 * cfg.neg_ratio)
+        cfg, ne = self.cfg, self.cfg.num_entities
+        if cfg.algorithm in ("TransE", "RotatE") and (cfg.dropout_entity > 0 or cfg.dropout_relation > 0):
+            raise ValueError(f"dropout is not defined for {cfg.algorithm}")
+        tr = triples_host.to(self.server.device, non_blocking=True) if self.cuda else triples_host
+        seed, neg = self._negatives(tr.shape[0])
+        if cfg.algorithm in ("ComplEx", "RESCAL"):
             S, R, O, L = self._expand(tr, neg)
-            fused = kge_complex_step if cfg.algorithm == "ComplEx" else kge_rescal_step
-            fused(self.server, S, R, O, L, cfg.embed_dim, cfg.eta, cfg.gamma_entity, cfg.gamma_relation, self.loss,
-                  self.stats, cfg.dropout_entity, cfg.dropout_relation, seed, deterministic=cfg.deterministic)
-            self.step_no += 1
-            return self.loss
-        neg = torch.randint(0, cfg.num_entities, (B, 2 * cfg.neg_ratio), generator=self._gen)
-        S, R, O, L = self._expand(triples_host, neg)
-        loss = kge_reference_step(self.worker, S, R, O, L, cfg)
+            if self.cuda:
+                fused = ops.kge_complex_step if cfg.algorithm == "ComplEx" else ops.kge_rescal_step
+                fused(self.server, S, R, O, L, cfg.embed_dim, cfg.eta, cfg.gamma_entity, cfg.gamma_relation, self.loss,
+                      self.stats, cfg.dropout_entity, cfg.dropout_relation, seed, deterministic=cfg.deterministic)
+            else:
+                loss = kge_reference_step(self.worker, S, R, O, L, cfg)
+        else:
+            if cfg.algorithm == "TransE":
+                fused, reference = ops.kge_transe_step, ops.transe_reference_step
+                args = (cfg.embed_dim, cfg.p_norm, cfg.margin, cfg.eta, cfg.gamma_entity, cfg.gamma_relation)
+            else:
+                fused, reference = ops.kge_rotate_step, ops.rotate_reference_step
+                args = (cfg.embed_dim, cfg.margin, cfg.adversarial_temperature, cfg.eta, cfg.gamma_entity)
+            s, r, o = tr[:, 0].contiguous(), (tr[:, 1] + ne).contiguous(), tr[:, 2].contiguous()
+            if self.cuda:
+                fused(self.server, s, r, o, neg, *args, self.loss, self.stats, deterministic=cfg.deterministic)
+            else:
+                loss, pushes = reference(self.worker, s, r, o, neg, *args)
+                self.pushes += pushes
         self.step_no += 1
-        return torch.tensor([loss], dtype=torch.float32)
-
-    def _step_transe(self, triples_host: torch.Tensor) -> torch.Tensor:
-        """TransE: one fused launch per batch on CUDA (``ops.kge_transe_step``), else ``ops.transe_reference_step``;
-        negatives ``[B, 2 * neg_ratio]`` in the layout of ``_expand`` (corrupted objects first)."""
-        from ..ops import kge_transe_step, transe_reference_step
-
-        cfg = self.cfg
-        if cfg.dropout_entity > 0 or cfg.dropout_relation > 0:
-            raise ValueError("dropout is not defined for TransE")
-        B, ne = triples_host.shape[0], cfg.num_entities
-        if self.cuda:
-            tr = triples_host.to(self.server.device, non_blocking=True)
-            local_only = cfg.sampling_scheme == "local" and self.server.num_servers() > 1
-            seed = (cfg.model_seed * 7 + self.server.my_rank() * 7919 + self.step_no) & 0xFFFFFFFFFFFF
-            neg = self.sampler.sample(B * 2 * cfg.neg_ratio, seed, local_only=local_only).view(B, 2 * cfg.neg_ratio)
-            kge_transe_step(self.server, tr[:, 0].contiguous(), (tr[:, 1] + ne).contiguous(), tr[:, 2].contiguous(), neg,
-                            cfg.embed_dim, cfg.p_norm, cfg.margin, cfg.eta, cfg.gamma_entity, cfg.gamma_relation,
-                            self.loss, self.stats, deterministic=cfg.deterministic)
-            self.step_no += 1
-            return self.loss
-        neg = torch.randint(0, ne, (B, 2 * cfg.neg_ratio), generator=self._gen)
-        loss, pushes = transe_reference_step(self.worker, triples_host[:, 0], triples_host[:, 1] + ne, triples_host[:, 2],
-                                             neg, cfg.embed_dim, cfg.p_norm, cfg.margin, cfg.eta, cfg.gamma_entity,
-                                             cfg.gamma_relation)
-        self.pushes += pushes
-        self.step_no += 1
-        return torch.tensor([loss], dtype=torch.float32)
-
-    def _step_rotate(self, triples_host: torch.Tensor) -> torch.Tensor:
-        """RotatE: one fused launch per batch on CUDA (``ops.kge_rotate_step``), else ``ops.rotate_reference_step``;
-        negatives ``[B, 2 * neg_ratio]`` in the layout of ``_expand`` (corrupted objects first)."""
-        from ..ops import kge_rotate_step, rotate_reference_step
-
-        cfg = self.cfg
-        if cfg.dropout_entity > 0 or cfg.dropout_relation > 0:
-            raise ValueError("dropout is not defined for RotatE")
-        B, ne = triples_host.shape[0], cfg.num_entities
-        if self.cuda:
-            tr = triples_host.to(self.server.device, non_blocking=True)
-            local_only = cfg.sampling_scheme == "local" and self.server.num_servers() > 1
-            seed = (cfg.model_seed * 7 + self.server.my_rank() * 7919 + self.step_no) & 0xFFFFFFFFFFFF
-            neg = self.sampler.sample(B * 2 * cfg.neg_ratio, seed, local_only=local_only).view(B, 2 * cfg.neg_ratio)
-            kge_rotate_step(self.server, tr[:, 0].contiguous(), (tr[:, 1] + ne).contiguous(), tr[:, 2].contiguous(), neg,
-                            cfg.embed_dim, cfg.margin, cfg.adversarial_temperature, cfg.eta, cfg.gamma_entity,
-                            self.loss, self.stats, deterministic=cfg.deterministic)
-            self.step_no += 1
-            return self.loss
-        neg = torch.randint(0, ne, (B, 2 * cfg.neg_ratio), generator=self._gen)
-        loss, pushes = rotate_reference_step(self.worker, triples_host[:, 0], triples_host[:, 1] + ne, triples_host[:, 2],
-                                             neg, cfg.embed_dim, cfg.margin, cfg.adversarial_temperature, cfg.eta,
-                                             cfg.gamma_entity)
-        self.pushes += pushes
-        self.step_no += 1
-        return torch.tensor([loss], dtype=torch.float32)
+        return self.loss if self.cuda else torch.tensor([loss], dtype=torch.float32)
 
     # ------------------------------------------------------------------ full-model pull (eval / checkpoints)
     def pull_embeddings(self, device=None):
@@ -354,191 +319,90 @@ class KGE:
                     "hits01_s", "hits01_r", "hits01_o", "hits03_s", "hits03_r", "hits03_o", "hits10_s", "hits10_r",
                     "hits10_o")   # slots 0..18 of the eval_key row (reference kge.cc:94-112)
 
+    def _metric(self):
+        """How entity candidates are compared: ``"dot"`` (ComplEx, RESCAL; a higher score is better), else the
+        ``(p, normalize)`` of ``ops.gather_dist_*`` / ``ops.dist_rank_reference`` (a smaller distance is better): TransE's
+        ``p_norm`` against normalised entity rows, RotatE's ``"complex"`` distance against raw rows."""
+        if self.cfg.algorithm in ("ComplEx", "RESCAL"):
+            return "dot"
+        return (self.cfg.p_norm, True) if self.cfg.algorithm == "TransE" else ("complex", False)
+
+    def _pull_rows(self, keys: torch.Tensor, ln: int) -> torch.Tensor:
+        """Device pull of the store rows of ``keys`` (row length ``ln``): their embedding halves, a [n, ln / 2] view."""
+        buf = torch.empty(keys.numel() * ln, dtype=torch.float32, device=self.server.device)
+        self.worker.wait(self.worker.pull(keys.contiguous(), buf, True))
+        return buf.view(-1, ln)[:, : ln // 2]
+
     def rank_triples(self, triples: torch.Tensor, known: torch.Tensor, batch: int = 2048, use_tensor_cores: bool = True):
         """Ranks of the true subject / relation / object of every triple among all candidates (reference
         ``rank()``, kge.cc:716-774): subject and object ranks raw and filtered (other known-true answers do not count),
         the relation rank unfiltered like in the reference. Returns a dict of int64 tensors
-        ``rank_s, rank_r, rank_o, rank_s_raw, rank_o_raw``. ``known``: all true triples (train+valid+test)."""
-        cfg = self.cfg
-        if cfg.algorithm == "TransE":
-            return self._rank_transe(triples, known, batch)
-        if cfg.algorithm == "RotatE":
-            return self._rank_rotate(triples, known, batch)
+        ``rank_s, rank_r, rank_o, rank_s_raw, rank_o_raw``. ``known``: all true triples (train+valid+test).
+
+        A candidate counts when it is strictly better than the true answer (``_metric``). CUDA: the dot metric scores
+        the whole pulled model with ``ops.gemm_nt_rank_count`` (or an fp32 matmul without ``use_tensor_cores``), the
+        distance metrics pull only each batch's entity rows and ``ops.gather_dist_rank_count`` reads the candidates from
+        the store. CPU: ``pull_embeddings()``, with ``ops.dist_rank_reference`` for the distance metrics. RotatE's
+        relation side depends on the candidate's phases and is computed by ``_rotate_relation_ranks``."""
+        from .. import ops
+
+        cfg, d, ne, nr = self.cfg, self.cfg.embed_dim, self.cfg.num_entities, self.cfg.num_relations
+        metric = self._metric()
         dev = self.server.device if self.cuda else torch.device("cpu")
-        E, _, R, _ = self.pull_embeddings(dev)
         triples = triples.to(dev)
-        known = torch.unique(known.to(dev), dim=0)   # duplicates must not be filtered twice
-        d = cfg.embed_dim
-        tc = self.cuda and use_tensor_cores
-        if tc:
-            from ..ops import gemm_nt_rank_count
-
-            bf = lambda x: x.to(torch.bfloat16).float()   # score with the operands the tensor cores see
+        answers = {side: self._answer_keys(known, side, dev) for side in ("object", "subject")}
+        # Compute dtypes. CUDA ranks in fp32; on the tensor cores from bf16-rounded operands, so the true score is the
+        # one the wgmma kernel sees. The CPU scores the dot metric in the store's dtype (float64 rows rank in float64,
+        # like the reference's ValT = double) and the distance metrics always in float64, where a sum of |differences|
+        # over d terms loses the least to rounding.
+        tc = metric == "dot" and self.cuda and use_tensor_cores
+        bf = (lambda x: x.to(torch.bfloat16).float()) if tc else (lambda x: x)
+        normalize = metric != "dot" and metric[1]   # entity candidates only; relation candidates are raw rows
+        if self.cuda and metric != "dot":
+            R = self._pull_rows(torch.arange(ne, ne + nr, dtype=torch.int64, device=dev), cfg.relation_len)
+            ent_rows = lambda keys: self._pull_rows(keys, cfg.entity_len)
+            cand_e = torch.arange(ne, dtype=torch.int64, device=dev)
+            cand_r = torch.arange(ne, ne + nr, dtype=torch.int64, device=dev)
         else:
-            bf = lambda x: x
-        E_s, R_s = bf(E), bf(R)
-        sr_key = known[:, 0] * cfg.num_relations + known[:, 1]
-        or_key = known[:, 2] * cfg.num_relations + known[:, 1]
-        order = torch.argsort(sr_key)
-        sr_sorted, sr_ent = sr_key[order], known[order, 2]
-        order = torch.argsort(or_key)
-        or_sorted, or_ent = or_key[order], known[order, 0]
-        out = {k: [] for k in ("rank_s", "rank_r", "rank_o", "rank_s_raw", "rank_o_raw")}
+            E, _, R, _ = self.pull_embeddings(dev)
+            if metric != "dot":
+                E, R = E.double(), R.double()
+            ent_rows = lambda keys: E[keys]
+            cand_e = normalize_rows(E) if normalize else bf(E)
+            cand_r = bf(R)
 
-        def count_better(q, cand, true_score, true_idx):
+        def count(q, cand, true, excl=None, norm=False):
+            """(raw, filtered) counts of the candidates other than ``true`` that are strictly better; filtered leaves out
+            the columns of the CSR ``excl``."""
+            if metric != "dot":
+                if self.cuda:
+                    return ops.gather_dist_rank_count(self.server, q, cand, d, metric[0], norm, true.contiguous(), excl)
+                return ops.dist_rank_reference(q, cand, metric[0], true,
+                                               ops.exclusion_mask(excl, cand.shape[0]) if excl is not None else None)
+            q = bf(q)
+            true_score = (q * cand[true]).sum(1)
             if tc:   # wgmma GEMM with the rank-count epilogue: the [B, candidates] scores never reach HBM
-                return gemm_nt_rank_count(q, cand, true_score, true_idx).long() + 1
-            scores = q @ cand.t()
-            scores.scatter_(1, true_idx.view(-1, 1), float("-inf"))
-            return (scores > true_score.view(-1, 1)).sum(1) + 1
+                raw = ops.gemm_nt_rank_count(q, cand, true_score, true).long()
+            else:
+                scores = q @ cand.t()
+                scores.scatter_(1, true.view(-1, 1), float("-inf"))
+                raw = (scores > true_score.view(-1, 1)).sum(1)
+            return raw, (_filter_dot(raw, q, true_score, true, excl, lambda cols: cand[cols]) if excl is not None else raw)
 
+        out = {k: [] for k in ("rank_s", "rank_r", "rank_o", "rank_s_raw", "rank_o_raw")}
         for i in range(0, triples.shape[0], batch):
             t = triples[i:i + batch]
-            Es, Eo, Rr = E[t[:, 0]], E[t[:, 2]], R[t[:, 1]]
-            for side in (0, 1):  # 0: predict object, 1: predict subject
-                if cfg.algorithm == "ComplEx":
-                    q = complex_query(Es if side == 0 else Eo, Rr, conj=(side == 1))
-                else:
-                    Rm = Rr.view(-1, d, d)
-                    q = torch.einsum("bi,bij->bj", Es, Rm) if side == 0 else torch.einsum("bij,bj->bi", Rm, Eo)
-                q = bf(q)
-                true_e = t[:, 2] if side == 0 else t[:, 0]
-                true_score = (q * E_s[true_e]).sum(1)
-                raw = count_better(q, E_s, true_score, true_e)
-                # filtering: other known answers of the same query do not count
-                qkey = (t[:, 0] if side == 0 else t[:, 2]) * cfg.num_relations + t[:, 1]
-                kks, kes = (sr_sorted, sr_ent) if side == 0 else (or_sorted, or_ent)
-                lo = torch.searchsorted(kks, qkey)
-                hi = torch.searchsorted(kks, qkey, right=True)
-                cnt = hi - lo
-                rows = torch.repeat_interleave(torch.arange(t.shape[0], device=dev), cnt)
-                offs = torch.arange(rows.numel(), device=dev) - torch.repeat_interleave(torch.cumsum(cnt, 0) - cnt, cnt)
-                ents = kes[lo[rows] + offs]
-                ks = (q[rows] * E_s[ents]).sum(1)
-                better = (ks > true_score[rows]) & (ents != true_e[rows])
-                filt = raw - torch.zeros_like(raw).index_add_(0, rows, better.to(raw.dtype))
-                out["rank_o_raw" if side == 0 else "rank_s_raw"].append(raw)
-                out["rank_o" if side == 0 else "rank_s"].append(filt)
-            # relation side: score(s, r', o) = <q_r, R[r']> for all relations r'
-            if cfg.algorithm == "ComplEx":
-                h = d // 2
-                sre, sim, ore, oim = Es[:, :h], Es[:, h:], Eo[:, :h], Eo[:, h:]
-                qr = torch.cat([sre * ore + sim * oim, sre * oim - sim * ore], 1)
+            Es, Eo, Rr = ent_rows(t[:, 0]), ent_rows(t[:, 2]), R[t[:, 1]]
+            for side, given, true in (("object", t[:, 0], t[:, 2]), ("subject", t[:, 2], t[:, 0])):
+                q = self._query(Es if side == "object" else Eo, Rr, side)
+                excl = self._known_answers(given, t[:, 1], side, known, answers[side])
+                raw, filt = count(q, cand_e, true, excl, normalize)
+                out[f"rank_{side[0]}_raw"].append(raw + 1)
+                out[f"rank_{side[0]}"].append(filt + 1)
+            if cfg.algorithm == "RotatE":
+                out["rank_r"].append(_rotate_relation_ranks(Es, Eo, R, t[:, 1]) + 1)
             else:
-                qr = torch.einsum("bi,bj->bij", Es, Eo).reshape(t.shape[0], d * d)
-            qr = bf(qr)
-            true_score = (qr * R_s[t[:, 1]]).sum(1)
-            out["rank_r"].append(count_better(qr, R_s, true_score, t[:, 1]))
-        return {k: torch.cat(v) if v else torch.zeros(0, dtype=torch.int64, device=dev) for k, v in out.items()}
-
-    def _transe_queries(self, Es, Rr, Eo):
-        """TransE queries from raw rows: (object side q = s^ + r, subject side q = o^ - r, relation side q = o^ - s^);
-        D(candidate) = |q - candidate|_p against normalised entities, or raw relations for the relation side."""
-        sh, oh = normalize_rows(Es), normalize_rows(Eo)
-        return (sh + Rr).contiguous(), (oh - Rr).contiguous(), (oh - sh).contiguous()
-
-    def _rank_transe(self, triples: torch.Tensor, known: torch.Tensor, batch: int) -> dict:
-        """``rank_triples`` for TransE: ranks by distance (a candidate is better when strictly closer), filtered by the
-        known answers. CUDA: ``ops.gather_dist_rank_count`` over the store rows with the exclusion CSR of
-        ``_known_answers``; CPU: ``torch.cdist`` over the pulled rows with the same rule."""
-        cfg = self.cfg
-        ne, nr, p = cfg.num_entities, cfg.num_relations, cfg.p_norm
-        out = {k: [] for k in ("rank_s", "rank_r", "rank_o", "rank_s_raw", "rank_o_raw")}
-        if self.cuda:
-            from ..ops import gather_dist_rank_count
-
-            dev, kv, d = self.server.device, self.worker, cfg.embed_dim
-            triples = triples.to(dev)
-            all_ent = torch.arange(ne, dtype=torch.int64, device=dev)
-            all_rel = torch.arange(ne, ne + nr, dtype=torch.int64, device=dev)
-
-            def pull_rows(keys):
-                buf = torch.empty(keys.numel() * 2 * d, dtype=torch.float32, device=dev)
-                kv.wait(kv.pull(keys.contiguous(), buf, True))
-                return buf.view(-1, 2 * d)[:, :d]
-
-            for i in range(0, triples.shape[0], batch):
-                t = triples[i:i + batch]
-                qo, qs, qr = self._transe_queries(pull_rows(t[:, 0]), pull_rows(t[:, 1] + ne), pull_rows(t[:, 2]))
-                for side, q, true_e, given in ((0, qo, t[:, 2], t[:, 0]), (1, qs, t[:, 0], t[:, 2])):
-                    excl = self._known_answers(given, t[:, 1], "object" if side == 0 else "subject", known)
-                    raw, filt = gather_dist_rank_count(self.server, q, all_ent, d, p, True, true_e.contiguous(), excl)
-                    out["rank_o_raw" if side == 0 else "rank_s_raw"].append(raw + 1)
-                    out["rank_o" if side == 0 else "rank_s"].append(filt + 1)
-                raw, _ = gather_dist_rank_count(self.server, qr, all_rel, d, p, False, t[:, 1].contiguous())
-                out["rank_r"].append(raw + 1)
-        else:
-            from ..ops import dist_rank_reference
-
-            E, _, R, _ = self.pull_embeddings()
-            E, R = E.double(), R.double()
-            En = normalize_rows(E)
-            for i in range(0, triples.shape[0], batch):
-                t = triples[i:i + batch]
-                qo, qs, qr = self._transe_queries(E[t[:, 0]], R[t[:, 1]], E[t[:, 2]])
-                for side, q, true_e, given in ((0, qo, t[:, 2], t[:, 0]), (1, qs, t[:, 0], t[:, 2])):
-                    off, cols = self._known_answers(given, t[:, 1], "object" if side == 0 else "subject", known)
-                    excluded = torch.zeros(t.shape[0], ne, dtype=torch.bool)
-                    excluded[torch.repeat_interleave(torch.arange(t.shape[0]), off[1:] - off[:-1]), cols] = True
-                    raw, filt = dist_rank_reference(q, En, p, true_e, excluded)
-                    out["rank_o_raw" if side == 0 else "rank_s_raw"].append(raw + 1)
-                    out["rank_o" if side == 0 else "rank_s"].append(filt + 1)
-                out["rank_r"].append(dist_rank_reference(qr, R, p, t[:, 1])[0] + 1)
-        dev = self.server.device if self.cuda else torch.device("cpu")
-        return {k: torch.cat(v) if v else torch.zeros(0, dtype=torch.int64, device=dev) for k, v in out.items()}
-
-    def _rank_rotate(self, triples: torch.Tensor, known: torch.Tensor, batch: int) -> dict:
-        """``rank_triples`` for RotatE: ranks by the complex distance (a candidate is better when strictly closer),
-        subject and object filtered by the known answers. Object side q = s o rho, subject side q = o o conj(rho) (exact,
-        |rho_i| = 1), against the raw entity rows: CUDA ``ops.gather_dist_rank_count(p="complex")`` over the store rows,
-        CPU ``ops.dist_rank_reference`` in float64. Relation side: D(r') = sum_i |s_i rho'_i - o_i| depends on the
-        candidate's phases, so it is computed in PyTorch on the pulled relation rows (fp32 on the GPU, float64 on the CPU,
-        chunked; ``_rotate_relation_ranks``)."""
-        cfg = self.cfg
-        ne, nr, d = cfg.num_entities, cfg.num_relations, cfg.embed_dim
-        out = {k: [] for k in ("rank_s", "rank_r", "rank_o", "rank_s_raw", "rank_o_raw")}
-        if self.cuda:
-            from ..ops import gather_dist_rank_count
-
-            dev, kv = self.server.device, self.worker
-            triples = triples.to(dev)
-            all_ent = torch.arange(ne, dtype=torch.int64, device=dev)
-
-            def pull_rows(keys, ln):
-                buf = torch.empty(keys.numel() * 2 * ln, dtype=torch.float32, device=dev)
-                kv.wait(kv.pull(keys.contiguous(), buf, True))
-                return buf.view(-1, 2 * ln)[:, :ln]
-
-            R = pull_rows(torch.arange(ne, ne + nr, dtype=torch.int64, device=dev), d // 2)   # all phases
-            for i in range(0, triples.shape[0], batch):
-                t = triples[i:i + batch]
-                Es, Eo, th = pull_rows(t[:, 0], d), pull_rows(t[:, 2], d), R[t[:, 1]]
-                for side, q, true_e, given in ((0, rotate_query(Es, th, False), t[:, 2], t[:, 0]),
-                                               (1, rotate_query(Eo, th, True), t[:, 0], t[:, 2])):
-                    excl = self._known_answers(given, t[:, 1], "object" if side == 0 else "subject", known)
-                    raw, filt = gather_dist_rank_count(self.server, q, all_ent, d, "complex", False, true_e.contiguous(),
-                                                       excl)
-                    out["rank_o_raw" if side == 0 else "rank_s_raw"].append(raw + 1)
-                    out["rank_o" if side == 0 else "rank_s"].append(filt + 1)
-                out["rank_r"].append(_rotate_relation_ranks(Es, Eo, R, t[:, 1]) + 1)
-        else:
-            from ..ops import dist_rank_reference
-
-            E, _, R, _ = self.pull_embeddings()
-            E, R = E.double(), R.double()
-            for i in range(0, triples.shape[0], batch):
-                t = triples[i:i + batch]
-                Es, Eo, th = E[t[:, 0]], E[t[:, 2]], R[t[:, 1]]
-                for side, q, true_e, given in ((0, rotate_query(Es, th, False), t[:, 2], t[:, 0]),
-                                               (1, rotate_query(Eo, th, True), t[:, 0], t[:, 2])):
-                    off, cols = self._known_answers(given, t[:, 1], "object" if side == 0 else "subject", known)
-                    excluded = torch.zeros(t.shape[0], ne, dtype=torch.bool)
-                    excluded[torch.repeat_interleave(torch.arange(t.shape[0]), off[1:] - off[:-1]), cols] = True
-                    raw, filt = dist_rank_reference(q, E, "complex", true_e, excluded)
-                    out["rank_o_raw" if side == 0 else "rank_s_raw"].append(raw + 1)
-                    out["rank_o" if side == 0 else "rank_s"].append(filt + 1)
-                out["rank_r"].append(_rotate_relation_ranks(Es, Eo, R, t[:, 1]) + 1)
-        dev = self.server.device if self.cuda else torch.device("cpu")
+                out["rank_r"].append(count(self._relation_query(Es, Eo), cand_r, t[:, 1])[0] + 1)
         return {k: torch.cat(v) if v else torch.zeros(0, dtype=torch.int64, device=dev) for k, v in out.items()}
 
     @staticmethod
@@ -598,23 +462,50 @@ class KGE:
         kv.barrier()
         return self._finish_metrics(row[:19].double(), N)
 
-    # ------------------------------------------------------------------ link prediction
+    # ------------------------------------------------------------------ queries and link prediction
     def _query(self, ent_rows: torch.Tensor, rel_rows: torch.Tensor, side: str) -> torch.Tensor:
-        """The query vector of ``rank_triples``: score(candidate) = <q, E[candidate]>."""
-        if self.cfg.algorithm == "ComplEx":
+        """The entity-side query of ``rank_triples`` and ``predict``, compared with the candidates by ``_metric``:
+        ComplEx and RESCAL score ``<q, E[candidate]>``; TransE ``q = s^ + r`` (objects) or ``o^ - r`` (subjects) against
+        normalised entities; RotatE ``q = s o rho`` or ``o o conj(rho)`` against raw entities (exact, ``|rho_i| = 1``)."""
+        cfg = self.cfg
+        if cfg.algorithm == "ComplEx":
             return complex_query(ent_rows, rel_rows, conj=(side == "subject"))
-        Rm = rel_rows.reshape(-1, self.cfg.embed_dim, self.cfg.embed_dim)
+        if cfg.algorithm == "TransE":
+            e = normalize_rows(ent_rows)
+            return (e + rel_rows if side == "object" else e - rel_rows).contiguous()
+        if cfg.algorithm == "RotatE":
+            return rotate_query(ent_rows, rel_rows, side == "subject")
+        Rm = rel_rows.reshape(-1, cfg.embed_dim, cfg.embed_dim)
         if side == "object":
             return torch.einsum("bi,bij->bj", ent_rows, Rm)
         return torch.einsum("bij,bj->bi", Rm, ent_rows)
 
-    def _known_answers(self, ents: torch.Tensor, rels: torch.Tensor, side: str, known: torch.Tensor):
-        """CSR ``(offsets [n + 1], cols)`` of the known answers of each query, ascending per row."""
+    def _relation_query(self, Es: torch.Tensor, Eo: torch.Tensor) -> torch.Tensor:
+        """The relation-side query of ``rank_triples`` (not RotatE): ComplEx and RESCAL score ``<q, R[candidate]>``,
+        TransE ``q = o^ - s^`` at the distance of ``_metric`` from the raw relation rows."""
+        cfg = self.cfg
+        if cfg.algorithm == "ComplEx":
+            h = cfg.embed_dim // 2
+            sre, sim, ore, oim = Es[:, :h], Es[:, h:], Eo[:, :h], Eo[:, h:]
+            return torch.cat([sre * ore + sim * oim, sre * oim - sim * ore], 1)
+        if cfg.algorithm == "TransE":
+            return (normalize_rows(Eo) - normalize_rows(Es)).contiguous()
+        return torch.einsum("bi,bj->bij", Es, Eo).reshape(Es.shape[0], cfg.embed_dim * cfg.embed_dim)
+
+    def _answer_keys(self, known: torch.Tensor, side: str, dev) -> torch.Tensor:
+        """The known triples as sorted, distinct keys ``(given * nr + relation) * ne + answer`` for ``side``'s queries:
+        the known answers of one query are one run of them."""
         ne, nr = self.cfg.num_entities, self.cfg.num_relations
-        dev = ents.device
         known = torch.as_tensor(known, dtype=torch.int64).to(dev).view(-1, 3)
         given, ans = (known[:, 0], known[:, 2]) if side == "object" else (known[:, 2], known[:, 0])
-        comp = torch.unique((given * nr + known[:, 1]) * ne + ans)        # sorted (query, answer) pairs, no duplicates
+        return torch.unique((given * nr + known[:, 1]) * ne + ans)
+
+    def _known_answers(self, ents: torch.Tensor, rels: torch.Tensor, side: str, known: torch.Tensor, keys=None):
+        """CSR ``(offsets [n + 1], cols)`` of the known answers of each query, ascending per row, each answer once.
+        ``keys``: ``_answer_keys(known, side)`` when the caller has built them already."""
+        ne, nr = self.cfg.num_entities, self.cfg.num_relations
+        dev = ents.device
+        comp = self._answer_keys(known, side, dev) if keys is None else keys
         qkey = (ents * nr + rels) * ne
         lo = torch.searchsorted(comp, qkey)
         cnt = torch.searchsorted(comp, qkey + ne) - lo
@@ -631,12 +522,15 @@ class KGE:
         Returns ``(entity ids int64 [n, k], scores float32 [n, k])``, best first; equal scores go to the smaller entity
         id. ``known``: triples [m, 3] (e.g. train + valid + test); every known answer of a query is left out (the
         filtered setting). A query with fewer than ``k`` candidates left is padded with ``(-1, -inf)``.
-        ``1 <= k <= 64``. The query vector is the one of ``rank_triples``.
+        ``1 <= k <= 64``. The query and the metric are the ones of ``rank_triples``; for TransE and RotatE the score is
+        ``-distance``.
 
-        CUDA backend (float32 rows): only the rows of the queries are pulled; the scores against all entities are
-        computed from bf16-rounded operands in the fused gather + top-k kernel (``ops.gather_gemm_topk``), which reads
-        the entity rows wherever they live, on any number of GPUs. CPU backend: fp32 PyTorch over ``pull_embeddings()``
-        with the same order (``ops.topk_reference``)."""
+        CUDA backend (float32 rows): only the rows of the queries are pulled, and a fused gather + top-k kernel reads the
+        entity rows wherever they live, on any number of GPUs: ``ops.gather_gemm_topk`` scores bf16-rounded operands for
+        ComplEx and RESCAL, ``ops.gather_dist_topk`` computes fp32 distances for TransE and RotatE. CPU backend: fp32
+        PyTorch over ``pull_embeddings()`` with the same order (``ops.topk_reference``)."""
+        from .. import ops
+
         if side not in ("object", "subject"):
             raise ValueError(f"side must be 'object' or 'subject', got {side!r}")
         cfg = self.cfg
@@ -645,112 +539,30 @@ class KGE:
         rels = torch.as_tensor(relations, dtype=torch.int64).reshape(-1)
         if ents.numel() != rels.numel():
             raise ValueError("entities and relations must have the same length")
-        if cfg.algorithm == "TransE":
-            return self._predict_transe(ents, rels, side, k, known)
-        if cfg.algorithm == "RotatE":
-            return self._predict_rotate(ents, rels, side, k, known)
+        metric = self._metric()
         if self.cuda:
-            from ..ops import gather_gemm_topk
-
-            dev, kv = self.server.device, self.worker
+            dev = self.server.device
             ents, rels = ents.to(dev), rels.to(dev)
-
-            def pull_rows(keys, ln):
-                buf = torch.empty(keys.numel() * ln, dtype=torch.float32, device=dev)
-                kv.wait(kv.pull(keys.contiguous(), buf, True))
-                return buf.view(-1, ln)[:, : ln // 2]
-
-            q = self._query(pull_rows(ents, cfg.entity_len), pull_rows(rels + ne, cfg.relation_len), side)
+            q = self._query(self._pull_rows(ents, cfg.entity_len), self._pull_rows(rels + ne, cfg.relation_len), side)
             excl = self._known_answers(ents, rels, side, known) if known is not None else None
-            vals, idx = gather_gemm_topk(self.server, q, torch.arange(ne, dtype=torch.int64, device=dev), d, k,
-                                         exclude=excl)
+            keys = torch.arange(ne, dtype=torch.int64, device=dev)
+            if metric == "dot":
+                vals, idx = ops.gather_gemm_topk(self.server, q, keys, d, k, exclude=excl)
+            else:
+                vals, idx = ops.gather_dist_topk(self.server, q, keys, d, k, *metric, exclude=excl)
             return idx, vals
-        from ..ops import _check_topk, topk_reference
-
-        _check_topk(ents.numel(), ne, k, None, None)
+        ops._check_topk(ents.numel(), ne, k, None, None)
         E, _, R, _ = self.pull_embeddings()
-        E, R = E.float(), R.float()
+        E, R = E.float(), R.float()   # fp32 scores, the dtype the CUDA route returns, whatever the store's dtype
         q = self._query(E[ents], R[rels], side)
-        excluded = None
-        if known is not None:
-            off, cols = self._known_answers(ents, rels, side, known)
-            excluded = torch.zeros(ents.numel(), ne, dtype=torch.bool)
-            excluded[torch.repeat_interleave(torch.arange(ents.numel()), off[1:] - off[:-1]), cols] = True
-        vals, idx = topk_reference(q @ E.t(), int(k), excluded)
-        return idx, vals
-
-    def _predict_transe(self, ents, rels, side, k, known):
-        """``predict`` for TransE: the ``k`` nearest entities to ``s^ + r`` (objects) or ``o^ - r`` (subjects);
-        scores are ``-distance``. CUDA: ``ops.gather_dist_topk``; CPU: ``torch.cdist`` + ``ops.topk_reference``."""
-        cfg = self.cfg
-        d, ne, p = cfg.embed_dim, cfg.num_entities, cfg.p_norm
-        if self.cuda:
-            from ..ops import gather_dist_topk
-
-            dev, kv = self.server.device, self.worker
-            ents, rels = ents.to(dev), rels.to(dev)
-
-            def pull_rows(keys):
-                buf = torch.empty(keys.numel() * 2 * d, dtype=torch.float32, device=dev)
-                kv.wait(kv.pull(keys.contiguous(), buf, True))
-                return buf.view(-1, 2 * d)[:, :d]
-
-            e, r = pull_rows(ents), pull_rows(rels + ne)
-            q = (normalize_rows(e) + r) if side == "object" else (normalize_rows(e) - r)
-            excl = self._known_answers(ents, rels, side, known) if known is not None else None
-            vals, idx = gather_dist_topk(self.server, q.contiguous(), torch.arange(ne, dtype=torch.int64, device=dev), d,
-                                         k, p, True, exclude=excl)
-            return idx, vals
-        from ..ops import _check_topk, topk_reference
-
-        _check_topk(ents.numel(), ne, k, None, None)
-        E, _, R, _ = self.pull_embeddings()
-        E, R = E.float(), R.float()
-        En = normalize_rows(E)
-        q = (En[ents] + R[rels]) if side == "object" else (En[ents] - R[rels])
-        excluded = None
-        if known is not None:
-            off, cols = self._known_answers(ents, rels, side, known)
-            excluded = torch.zeros(ents.numel(), ne, dtype=torch.bool)
-            excluded[torch.repeat_interleave(torch.arange(ents.numel()), off[1:] - off[:-1]), cols] = True
-        vals, idx = topk_reference(-torch.cdist(q, En, p=float(p)), int(k), excluded)
-        return idx, vals
-
-    def _predict_rotate(self, ents, rels, side, k, known):
-        """``predict`` for RotatE: the ``k`` nearest entities by the complex distance to ``s o rho`` (objects) or
-        ``o o conj(rho)`` (subjects); scores are ``-distance``. CUDA: ``ops.gather_dist_topk(p="complex")``; CPU:
-        ``ops.complex_dist`` + ``ops.topk_reference``."""
-        cfg = self.cfg
-        d, ne = cfg.embed_dim, cfg.num_entities
-        conj = side == "subject"
-        if self.cuda:
-            from ..ops import gather_dist_topk
-
-            dev, kv = self.server.device, self.worker
-            ents, rels = ents.to(dev), rels.to(dev)
-
-            def pull_rows(keys, ln):
-                buf = torch.empty(keys.numel() * 2 * ln, dtype=torch.float32, device=dev)
-                kv.wait(kv.pull(keys.contiguous(), buf, True))
-                return buf.view(-1, 2 * ln)[:, :ln]
-
-            q = rotate_query(pull_rows(ents, d), pull_rows(rels + ne, d // 2), conj)
-            excl = self._known_answers(ents, rels, side, known) if known is not None else None
-            vals, idx = gather_dist_topk(self.server, q, torch.arange(ne, dtype=torch.int64, device=dev), d, k,
-                                         "complex", False, exclude=excl)
-            return idx, vals
-        from ..ops import _check_topk, complex_dist, topk_reference
-
-        _check_topk(ents.numel(), ne, k, None, None)
-        E, _, R, _ = self.pull_embeddings()
-        E, R = E.float(), R.float()
-        q = rotate_query(E[ents], R[rels], conj)
-        excluded = None
-        if known is not None:
-            off, cols = self._known_answers(ents, rels, side, known)
-            excluded = torch.zeros(ents.numel(), ne, dtype=torch.bool)
-            excluded[torch.repeat_interleave(torch.arange(ents.numel()), off[1:] - off[:-1]), cols] = True
-        vals, idx = topk_reference(-complex_dist(q, E), int(k), excluded)
+        excluded = ops.exclusion_mask(self._known_answers(ents, rels, side, known), ne) if known is not None else None
+        if metric == "dot":
+            scores = q @ E.t()
+        elif metric[0] == "complex":
+            scores = -ops.complex_dist(q, E)
+        else:
+            scores = -torch.cdist(q, normalize_rows(E), p=float(metric[0]))
+        vals, idx = ops.topk_reference(scores, int(k), excluded)
         return idx, vals
 
 
@@ -871,6 +683,23 @@ def kge_reference_step(kv, S, R, O, L, cfg: KGEConfig, masks=None) -> float:
     return float(torch.log1p(torch.exp(-y)).sum())
 
 
+def _filter_dot(raw: torch.Tensor, q: torch.Tensor, true_score: torch.Tensor, true: torch.Tensor, excl, answer_rows):
+    """Filtered dot-metric counts: ``raw`` minus, per query, its known answers (CSR ``excl``) other than the true one that
+    score strictly higher. ``answer_rows(cols)``: the candidate rows of the answers, as the raw count scored them."""
+    off, cols = excl
+    rows = torch.repeat_interleave(torch.arange(q.shape[0], device=q.device), off[1:] - off[:-1])
+    better = ((q[rows] * answer_rows(cols)).sum(1) > true_score[rows]) & (cols != true[rows])
+    return raw - torch.zeros_like(raw).index_add_(0, rows, better.to(raw.dtype))
+
+
+def _ranking_summary(rf: torch.Tensor, rr: torch.Tensor) -> dict:
+    """MRR and Hits@k of the filtered entity ranks ``rf`` and the raw MRR of ``rr`` (subject and object sides)."""
+    rf, rr = rf.double(), rr.double()
+    return {"mrr": float((1 / rf).mean()), "mrr_raw": float((1 / rr).mean()),
+            "hits@1": float((rf <= 1).double().mean()), "hits@3": float((rf <= 3).double().mean()),
+            "hits@10": float((rf <= 10).double().mean()), "n": int(rf.numel() // 2)}
+
+
 def evaluate_fused(model: "KGE", triples: torch.Tensor, known: torch.Tensor, batch: int = 2048) -> dict:
     """Filtered ranking without ever pulling the model: per batch only the rows of the queries, of the true
     answers and of the known answers are pulled (device Pull); the 1-vs-all scoring against ALL entities runs in
@@ -881,56 +710,30 @@ def evaluate_fused(model: "KGE", triples: torch.Tensor, known: torch.Tensor, bat
 
     if model.cfg.algorithm in ("TransE", "RotatE"):   # distance ranks from the store rows (ops.gather_dist_rank_count)
         ranks = model.rank_triples(triples, known, batch)
-        rf = torch.cat([ranks["rank_o"], ranks["rank_s"]]).double()
-        rr = torch.cat([ranks["rank_o_raw"], ranks["rank_s_raw"]]).double()
-        return {"mrr": float((1 / rf).mean()), "mrr_raw": float((1 / rr).mean()),
-                "hits@1": float((rf <= 1).double().mean()), "hits@3": float((rf <= 3).double().mean()),
-                "hits@10": float((rf <= 10).double().mean()), "n": int(rf.numel() // 2)}
-    cfg, kv, dev = model.cfg, model.worker, model.server.device
-    d, ne = cfg.embed_dim, cfg.num_entities
+        return _ranking_summary(torch.cat([ranks["rank_o"], ranks["rank_s"]]),
+                                torch.cat([ranks["rank_o_raw"], ranks["rank_s_raw"]]))
+    cfg, dev = model.cfg, model.server.device
+    d, ne, ln = cfg.embed_dim, cfg.num_entities, cfg.entity_len
     triples = triples.to(dev)
-    known = torch.unique(known.to(dev), dim=0)
+    answers = {side: model._answer_keys(known, side, dev) for side in ("object", "subject")}
     all_ent = torch.arange(ne, dtype=torch.int64, device=dev)
-    sr_key = known[:, 0] * cfg.num_relations + known[:, 1]
-    or_key = known[:, 2] * cfg.num_relations + known[:, 1]
-    order = torch.argsort(sr_key); sr_sorted, sr_ent = sr_key[order], known[order, 2]
-    order = torch.argsort(or_key); or_sorted, or_ent = or_key[order], known[order, 0]
     stats = torch.zeros(2, dtype=torch.int64, device=dev)
+    bf = lambda x: x.to(torch.bfloat16).float()   # the operands the tensor cores see
 
-    def pull_emb(keys):
-        keys = keys.contiguous()
-        buf = torch.empty(keys.numel() * cfg.entity_len, dtype=torch.float32, device=dev)
-        kv.wait(kv.pull(keys, buf, True))
-        return buf.view(-1, cfg.entity_len)[:, :d]
+    def answer_rows(cols):
+        return bf(model._pull_rows(cols, ln)) if cols.numel() else torch.empty(0, d, device=dev)
 
     ranks_f, ranks_r = [], []
     for i in range(0, triples.shape[0], batch):
         t = triples[i:i + batch]
-        Es, Eo = pull_emb(t[:, 0]), pull_emb(t[:, 2])
-        Rr = pull_emb(t[:, 1] + ne)
-        for side in (0, 1):
-            q = complex_query(Es if side == 0 else Eo, Rr, conj=(side == 1)).to(torch.bfloat16).float()
-            true_e = t[:, 2] if side == 0 else t[:, 0]
-            Et = (Eo if side == 0 else Es).to(torch.bfloat16).float()
-            true_score = (q * Et).sum(1)
-            raw = gather_gemm_rank_count(model.server, q, all_ent, d, true_score, true_e, stats).long() + 1
-            qkey = (t[:, 0] if side == 0 else t[:, 2]) * cfg.num_relations + t[:, 1]
-            kks, kes = (sr_sorted, sr_ent) if side == 0 else (or_sorted, or_ent)
-            lo = torch.searchsorted(kks, qkey)
-            hi = torch.searchsorted(kks, qkey, right=True)
-            cnt = hi - lo
-            rows = torch.repeat_interleave(torch.arange(t.shape[0], device=dev), cnt)
-            offs = torch.arange(rows.numel(), device=dev) - torch.repeat_interleave(torch.cumsum(cnt, 0) - cnt, cnt)
-            ents = kes[lo[rows] + offs]
-            Ek = pull_emb(ents).to(torch.bfloat16).float() if ents.numel() else torch.empty(0, d, device=dev)
-            better = ((q[rows] * Ek).sum(1) > true_score[rows]) & (ents != true_e[rows])
-            filt = raw - torch.zeros_like(raw).index_add_(0, rows, better.to(raw.dtype))
+        Es, Eo, Rr = model._pull_rows(t[:, 0], ln), model._pull_rows(t[:, 2], ln), model._pull_rows(t[:, 1] + ne, ln)
+        for side, given, true in (("object", t[:, 0], t[:, 2]), ("subject", t[:, 2], t[:, 0])):
+            q = bf(complex_query(Es if side == "object" else Eo, Rr, conj=(side == "subject")))
+            true_score = (q * bf(Eo if side == "object" else Es)).sum(1)
+            raw = gather_gemm_rank_count(model.server, q, all_ent, d, true_score, true, stats).long() + 1
+            excl = model._known_answers(given, t[:, 1], side, known, answers[side])
             ranks_r.append(raw)
-            ranks_f.append(filt)
-    rf = torch.cat(ranks_f).double()
-    rr = torch.cat(ranks_r).double()
+            ranks_f.append(_filter_dot(raw, q, true_score, true, excl, answer_rows))
     s = stats.tolist()
-    return {"mrr": float((1 / rf).mean()), "mrr_raw": float((1 / rr).mean()),
-            "hits@1": float((rf <= 1).double().mean()), "hits@3": float((rf <= 3).double().mean()),
-            "hits@10": float((rf <= 10).double().mean()), "n": int(rf.numel() // 2),
+    return {**_ranking_summary(torch.cat(ranks_f), torch.cat(ranks_r)),
             "gathered_rows_local": s[0], "gathered_rows_remote": s[1]}

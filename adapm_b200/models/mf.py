@@ -530,7 +530,7 @@ class MatrixFactorization:
         bf16-rounded operands in the fused gather + top-k kernel (``ops.gather_gemm_topk``), which reads the item rows
         wherever they live; this needs ``rank % 4 == 0`` (``ValueError`` otherwise). CPU route: fp32 PyTorch over the
         pulled item factors with the same order (``ops.topk_reference``)."""
-        from ..ops import _check_topk, gather_gemm_topk, topk_reference
+        from ..ops import _check_topk, exclusion_mask, gather_gemm_topk, topk_reference
 
         cfg, kv = self.cfg, self.worker
         users = torch.as_tensor(np.asarray(rows), dtype=torch.int64).reshape(-1)
@@ -558,11 +558,7 @@ class MatrixFactorization:
         kv.wait(kv.pull(torch.arange(N, dtype=torch.int64) + self.fck, hv))
         q = wv.view(n, 2 * cfg.rank)[:, :cfg.rank].float()
         E = hv.view(N, 2 * cfg.rank)[:, :cfg.rank].float()
-        excluded = None
-        if seen is not None:
-            off, cols = seen
-            excluded = torch.zeros(n, N, dtype=torch.bool)
-            excluded[torch.repeat_interleave(torch.arange(n), off[1:] - off[:-1]), cols] = True
+        excluded = exclusion_mask(seen, N) if seen is not None else None
         vals, idx = topk_reference(q @ E.t(), int(k), excluded)
         return idx, vals
 

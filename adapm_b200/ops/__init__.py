@@ -1131,6 +1131,16 @@ def topk_reference(scores: torch.Tensor, k: int, excluded: Optional[torch.Tensor
     return vals, idx
 
 
+def exclusion_mask(exclude, n_cols: int) -> torch.Tensor:
+    """The dense form of an exclusion CSR ``exclude = (offsets int64 [M + 1], cols int64 [nnz])``, as the top-k and
+    rank-count ops take it: bool [M, n_cols], True at ``[i, cols[offsets[i]:offsets[i + 1]]]``. For
+    :func:`topk_reference` and :func:`dist_rank_reference`."""
+    off, cols = exclude
+    mask = torch.zeros(off.numel() - 1, n_cols, dtype=torch.bool, device=off.device)
+    mask[torch.repeat_interleave(torch.arange(off.numel() - 1, device=off.device), off[1:] - off[:-1]), cols] = True
+    return mask
+
+
 EMBEDDING_BAG_MAX_DIM = 512
 _NNZ_LIMIT = 1 << 31
 

@@ -27,21 +27,33 @@ def _brute_topk(scores: np.ndarray, k: int, excluded=None):
     return np.array(out_i, dtype=np.int64), np.array(out_v)
 
 
-@pytest.mark.parametrize("algo", ["ComplEx", "RESCAL"])
+@pytest.mark.parametrize("algo", ["ComplEx", "RESCAL", "TransE", "RotatE"])
 @pytest.mark.parametrize("side", ["object", "subject"])
 def test_kge_predict_cpu_matches_float64_bruteforce(algo, side):
-    """Embeddings with quarter-integer entries make every score exact in float32, so ties are exact: duplicated entity
-    rows must come out in ascending id order, and filtering must remove exactly the known answers."""
+    """Embeddings with quarter-integer entries (TransE: entity rows with one entry of +-1 or +-2, so normalising is exact)
+    make every score exact in float32, so ties are exact: duplicated entity rows must come out in ascending id order,
+    and filtering must remove exactly the known answers. RotatE's scores round, so its rows are drawn at random and the
+    order may differ only between scores within float32 rounding of each other."""
     from adapm_b200.models.kge import KGE, KGEConfig
 
-    cfg = KGEConfig(num_entities=40, num_relations=3, embed_dim=4, algorithm=algo)
+    cfg = KGEConfig(num_entities=40, num_relations=3, embed_dim=8 if algo == "RotatE" else 4, algorithm=algo)
     server, kv = _server(cfg.value_lengths(), cfg.num_keys)
     model = KGE(server, kv, cfg)
     g = torch.Generator().manual_seed(5)
     d, ne, nr = cfg.embed_dim, cfg.num_entities, cfg.num_relations
-    E = torch.randint(-3, 4, (ne, d), generator=g).double() / 4
+    if algo == "TransE":
+        E = torch.zeros(ne, d, dtype=torch.float64)
+        E[torch.arange(ne), torch.randint(0, d, (ne,), generator=g)] = (
+            torch.tensor([-2.0, -1.0, 1.0, 2.0], dtype=torch.float64)[torch.randint(0, 4, (ne,), generator=g)])
+    elif algo == "RotatE":
+        E = torch.randn(ne, d, generator=g, dtype=torch.float64).float().double()
+    else:
+        E = torch.randint(-3, 4, (ne, d), generator=g).double() / 4
     E[7] = E[3]; E[20] = E[3]; E[11] = E[30]               # exact ties
-    R = torch.randint(-2, 3, (nr, cfg.relation_len // 2), generator=g).double() / 4
+    if algo == "RotatE":
+        R = ((torch.rand(nr, d // 2, generator=g, dtype=torch.float64) * 2 - 1) * np.pi).float().double()
+    else:
+        R = torch.randint(-2, 3, (nr, cfg.relation_len // 2), generator=g).double() / 4
     ent_rows = torch.cat([E, torch.full((ne, d), 1e-6, dtype=torch.float64)], 1).float()
     rel_rows = torch.cat([R, torch.full_like(R, 1e-6)], 1).float()
     kv.set(torch.arange(ne), ent_rows.reshape(-1))
@@ -63,9 +75,22 @@ def test_kge_predict_cpu_matches_float64_bruteforce(algo, side):
                 q = torch.cat([rre * are - rim * aim, rre * aim + rim * are], 1)
             else:
                 q = torch.cat([rre * are + rim * aim, rre * aim - rim * are], 1)
-        else:
+            scores = q @ E.t()
+        elif algo == "RESCAL":
             Rm = R[rels].view(-1, d, d)
             q = torch.einsum("bi,bij->bj", E[ents], Rm) if side == "object" else torch.einsum("bij,bj->bi", Rm, E[ents])
+            scores = q @ E.t()
+        elif algo == "TransE":                             # -|s^ + r - o^|_1, candidates o (object) or s (subject)
+            En = E / E.norm(dim=1, keepdim=True)
+            q = En[ents] + R[rels] if side == "object" else En[ents] - R[rels]
+            scores = -(q.unsqueeze(1) - En.unsqueeze(0)).abs().sum(-1)
+        else:                                              # -sum_i |s_i e^{i theta_i} - o_i|
+            Z = torch.view_as_complex(E.view(ne, d // 2, 2).contiguous())
+            rho = torch.exp(1j * R[rels]).unsqueeze(1)
+            if side == "object":
+                scores = -(Z[ents].unsqueeze(1) * rho - Z.unsqueeze(0)).abs().sum(-1)
+            else:
+                scores = -(Z.unsqueeze(0) * rho - Z[ents].unsqueeze(1)).abs().sum(-1)
         excl = None
         if kn is not None:
             excl = [set() for _ in range(5)]
@@ -75,9 +100,21 @@ def test_kge_predict_cpu_matches_float64_bruteforce(algo, side):
                         excl[i].add(o)
                     if side == "subject" and (o, r) == (int(ents[i]), int(rels[i])):
                         excl[i].add(s)
-        ref_i, ref_v = _brute_topk((q @ E.t()).numpy(), k, excl)
-        assert np.array_equal(ids.numpy(), ref_i), (k, ids, ref_i)
-        assert np.array_equal(vals.double().numpy(), ref_v), (k, vals, ref_v)
+        ref_i, ref_v = _brute_topk(scores.numpy(), k, excl)
+        if algo == "RotatE":
+            got_i, n_ok = ids.numpy(), min(k, ne)
+            np.testing.assert_allclose(vals.double().numpy()[:, :n_ok], ref_v[:, :n_ok], rtol=1e-6, atol=1e-5)
+            assert np.array_equal(np.isneginf(vals.numpy()), np.isneginf(ref_v))
+            for i in range(5):
+                for a, b, va in zip(got_i[i], ref_i[i], ref_v[i]):
+                    if a != b:    # only a near-tie may swap
+                        assert a >= 0 and abs(float(scores[i, a]) - va) < 1e-5, (i, a, b)
+                for tied in ((3, 7, 20), (11, 30)):        # exact ties keep ascending ids
+                    got = [j for j in got_i[i].tolist() if j in tied]
+                    assert got == sorted(got), (i, got)
+        else:
+            assert np.array_equal(ids.numpy(), ref_i), (k, ids, ref_i)
+            assert np.array_equal(vals.double().numpy(), ref_v), (k, vals, ref_v)
         if kn is not None:
             for i in range(5):
                 assert not (set(ids[i].tolist()) & excl[i])
