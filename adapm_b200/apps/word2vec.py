@@ -50,6 +50,9 @@ def main(argv=None) -> int:
                     help="1 = continuous bag of words (word2vec.c's -cbow 1): one window per corpus word, the mean of the "
                          "context rows scored against the centre and the negatives; 0 = skip-gram (window <= 16 for CBOW)")
     ap.add_argument("--batch_windows", type=int, default=8192, help="CBOW: windows per step")
+    ap.add_argument("--hs", type=int, default=0, choices=[0, 1],
+                    help="1 = hierarchical softmax (word2vec.c's -hs 1): each item is scored against the inner nodes on "
+                         "the Huffman path of its word instead of negatives; needs --negative 0")
     ap.add_argument("--synthetic_vocab", type=int, default=0, help="train on a synthetic Zipf corpus of this vocabulary size")
     ap.add_argument("--synthetic_batches", type=int, default=50)
     ap.add_argument("--init_model", default="random",
@@ -69,6 +72,9 @@ def main(argv=None) -> int:
 
     if args.cbow and args.shared_negatives > 0:
         raise ValueError("--shared_negatives is a skip-gram option: it cannot be combined with --cbow 1")
+    if args.hs and (args.negative > 0 or args.shared_negatives > 0):
+        raise ValueError("--hs 1 with negative sampling is not supported: run hierarchical softmax with --negative 0 "
+                         "and without --shared_negatives")
     rng = np.random.default_rng(args.model_seed)
     words = None
     native = None
@@ -102,7 +108,8 @@ def main(argv=None) -> int:
                          starting_alpha=args.starting_alpha, neg_power=args.neg_power, batch_pairs=args.batch_pairs,
                          read_ahead=args.read_sentences_ahead, signal_intent=bool(args.signal_intent),
                          sampling_scheme=getattr(args, "sampling.scheme") or "local", model_seed=args.model_seed,
-                         shared_negatives=args.shared_negatives, cbow=bool(args.cbow), batch_windows=args.batch_windows)
+                         shared_negatives=args.shared_negatives, cbow=bool(args.cbow), batch_windows=args.batch_windows,
+                         hs=bool(args.hs))
     ad.setup(cfg.num_keys, 1)   # one worker per rank: the per-thread loops of the reference are batched kernels here
     server = ad.Server(cfg.row_len, backend=args.backend, options=system_options(args))
     kv = ad.Worker(0, server)
@@ -161,7 +168,8 @@ def main(argv=None) -> int:
             cur = window.pop(0)
             if model.cuda:
                 model.loss.zero_()
-            loss = model.step(_full(cur, cfg, model.cuda))
+            last = _full(cur, cfg, model.cuda)
+            loss = model.step(last)
             if sync_push and model.cuda:
                 torch.cuda.current_stream().synchronize()
             kv.advance_clock()
@@ -172,15 +180,18 @@ def main(argv=None) -> int:
         for cur in window:
             if model.cuda:
                 model.loss.zero_()
-            loss = model.step(_full(cur, cfg, model.cuda))
+            last = _full(cur, cfg, model.cuda)
+            loss = model.step(last)
             kv.advance_clock()
             total_pairs += _items(cur, cfg)
         model.set_alpha((epoch + 1) / args.num_iterations)
         kv.barrier()
         if rank == 0:
             unit, per_step = ("windows", cfg.batch_windows) if cfg.cbow else ("pairs", cfg.batch_pairs)
+            # (hierarchical softmax: per path node of the last batch's items)
+            terms = model.loss_terms(last) if cfg.hs else per_step * (cfg.negative + 1)
             print(f"[w2v] epoch {epoch} done: {total_pairs} {unit} on rank 0, {time.time() - t0:.1f}s, "
-                  f"last batch loss {float(loss) / max(1, per_step * (cfg.negative + 1)):.4f}", flush=True)
+                  f"last batch loss {float(loss) / max(1, terms):.4f}", flush=True)
         if args.write_results:
             model.write_checkpoint(f"{args.output_file}.epoch.{epoch}", words)
     kv.finalize()

@@ -4,6 +4,8 @@
 #include <cmath>
 #include <cstring>
 #include <fstream>
+#include <limits>
+#include <stdexcept>
 #include <string_view>
 #include <unordered_map>
 
@@ -336,6 +338,56 @@ void WindowStream::run(uint64_t epoch) {
     publish(cur, n);
   }
   finish();
+}
+
+HuffmanTree huffman_tree(const double* counts, int64_t n) {
+  if (n < 2) throw std::invalid_argument("huffman_tree: needs at least 2 words, got " + std::to_string(n));
+  if (n > INT32_MAX / 2) throw std::invalid_argument("huffman_tree: too many words");
+  for (int64_t w = 0; w < n; ++w)
+    if (!(counts[w] > 0) || !std::isfinite(counts[w]))
+      throw std::invalid_argument("huffman_tree: count of word " + std::to_string(w) + " is not a positive number");
+  // leaf p < n is the word order[p] (count descending, ties by id); node n + a is the a-th merge (inner node a)
+  std::vector<int32_t> order(n);
+  for (int64_t w = 0; w < n; ++w) order[w] = (int32_t)w;
+  std::stable_sort(order.begin(), order.end(), [&](int32_t a, int32_t b) { return counts[a] > counts[b]; });
+  std::vector<double> cnt(2 * n, std::numeric_limits<double>::infinity());
+  for (int64_t p = 0; p < n; ++p) cnt[p] = counts[order[p]];
+  std::vector<int32_t> parent(2 * n - 1, -1);
+  std::vector<uint8_t> bit(2 * n - 1, 0);
+  int64_t pos1 = n - 1, pos2 = n;     // the smallest unmerged leaf, the oldest unmerged inner node
+  auto take = [&]() {
+    if (pos1 >= 0 && cnt[pos1] < cnt[pos2]) return pos1--;
+    return pos2++;
+  };
+  for (int64_t a = 0; a < n - 1; ++a) {
+    const int64_t m1 = take(), m2 = take();
+    cnt[n + a] = cnt[m1] + cnt[m2];
+    parent[m1] = parent[m2] = (int32_t)(n + a);
+    bit[m2] = 1;
+  }
+  // depths top-down: a parent is always created after its children
+  std::vector<int32_t> depth(2 * n - 1, 0);
+  for (int64_t v = 2 * n - 3; v >= 0; --v) depth[v] = depth[parent[v]] + 1;
+  HuffmanTree t;
+  t.offsets.assign(n + 1, 0);
+  for (int64_t p = 0; p < n; ++p) t.max_len = std::max(t.max_len, depth[p]);
+  if (t.max_len > kMaxHuffmanDepth)
+    throw std::invalid_argument("huffman_tree: the tree is " + std::to_string(t.max_len) + " levels deep, more than " +
+                                std::to_string(kMaxHuffmanDepth));
+  for (int64_t p = 0; p < n; ++p) t.offsets[order[p] + 1] = depth[p];
+  for (int64_t w = 0; w < n; ++w) t.offsets[w + 1] += t.offsets[w];
+  t.nodes.resize(t.offsets[n]);
+  t.codes.assign(n, 0u);
+  for (int64_t p = 0; p < n; ++p) {
+    const int32_t w = order[p];
+    int64_t v = p;
+    for (int j = depth[p] - 1; j >= 0; --j) {     // walk up: the node at depth j is v's parent
+      t.nodes[t.offsets[w] + j] = (int32_t)(parent[v] - n);
+      t.codes[w] |= (uint32_t)bit[v] << j;
+      v = parent[v];
+    }
+  }
+  return t;
 }
 
 }  // namespace adapm

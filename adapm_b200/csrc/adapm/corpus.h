@@ -18,6 +18,20 @@
 
 namespace adapm {
 
+// Huffman coding of a vocabulary for hierarchical softmax, built like word2vec.c's CreateBinaryTree so that trees match
+// word2vec.c and gensim for the same counts: words ordered by count (descending, ties by word id), the two-queue O(V)
+// merge, inner nodes numbered 0 .. V-2 in creation order (the root is V-2), code bit 1 for the second-smallest child of
+// each merge. Word w's path is nodes[offsets[w] .. offsets[w + 1]), root first, and bit j of codes[w] is its code bit
+// at depth j. Throws std::invalid_argument for V < 2, a count that is not > 0, or a path longer than kMaxHuffmanDepth.
+constexpr int kMaxHuffmanDepth = 32;
+struct HuffmanTree {
+  std::vector<int64_t> offsets;    // [V + 1]
+  std::vector<int32_t> nodes;      // [sum of the path lengths]
+  std::vector<uint32_t> codes;     // [V]
+  int max_len = 0;
+};
+HuffmanTree huffman_tree(const double* counts, int64_t n);
+
 class Corpus {
  public:
   // Pass 1: whitespace-tokenise `path`, count words, keep those with count >= min_count, order by count

@@ -226,6 +226,24 @@ PYBIND11_MODULE(_C, m) {
     return py::make_tuple(i, j, x, c.rows, c.cols);
   });
 
+  m.attr("max_huffman_depth") = kMaxHuffmanDepth;
+  m.def("huffman_tree", [](py::array_t<double, py::array::c_style | py::array::forcecast> counts) {
+    HuffmanTree t;
+    {
+      const double* c = counts.data();
+      const int64_t n = (int64_t)counts.size();
+      py::gil_scoped_release r;
+      t = huffman_tree(c, n);
+    }
+    py::array_t<int64_t> off((py::ssize_t)t.offsets.size());
+    py::array_t<int32_t> nodes((py::ssize_t)t.nodes.size());
+    py::array_t<uint32_t> codes((py::ssize_t)t.codes.size());
+    memcpy(off.mutable_data(), t.offsets.data(), t.offsets.size() * sizeof(int64_t));
+    if (!t.nodes.empty()) memcpy(nodes.mutable_data(), t.nodes.data(), t.nodes.size() * sizeof(int32_t));
+    memcpy(codes.mutable_data(), t.codes.data(), t.codes.size() * sizeof(uint32_t));
+    return py::make_tuple(off, nodes, codes, t.max_len);
+  });
+
   // native data loader (corpus.h)
   py::class_<Corpus, std::shared_ptr<Corpus>>(m, "Corpus")
       .def_static("build", &Corpus::build, py::arg("path"), py::arg("min_count") = 5,

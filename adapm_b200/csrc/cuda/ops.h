@@ -28,6 +28,13 @@ constexpr int kCbowMaxContexts = 32;
 void cbow_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, const Key* negatives,
                int n_win, int nc, int neg, int d, float alpha, float* loss_out, unsigned long long* stats,
                bool deterministic);
+// word2vec hierarchical softmax (ops_cbow.cu, the CBOW body with Huffman-path targets): item i has the syn1 key
+// centers[i] = 2w + 1 (< 0: nothing) and the syn0 contexts[i * nc .. (i + 1) * nc) (-1 = padding); its targets are the
+// inner nodes nodes[offsets[w] .. offsets[w + 1]) of word w's path (rows 2 node + 1), labelled 1 - bit j of codes[w];
+// a node with |f| >= 6 is skipped. Shapes, stats and the two paths as for cbow_step; max_len (the longest path) <= 32.
+void hs_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, int n_items, int nc,
+             const int64_t* offsets, const int32_t* nodes, const uint32_t* codes, int n_words, int max_len, int d,
+             float alpha, float* loss_out, unsigned long long* stats, bool deterministic);
 
 // word2vec SGNS with shared negatives on the tensor cores (ops_sgns_shared.cu): three wgmma GEMMs + three elementwise
 // kernels between ONE Pull and ONE Push of the rows [centers | contexts | shared negatives].

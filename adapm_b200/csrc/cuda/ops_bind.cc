@@ -35,6 +35,13 @@ void bind(py::module_& m) {
               ptr<const Key>(negatives), n_win, nc, neg, d, alpha, ptr<float>(loss), ptr<unsigned long long>(stats),
               deterministic);
   });
+  m.def("hs_step", [](uintptr_t be, uintptr_t stream, uintptr_t centers, uintptr_t contexts, int n_items, int nc,
+                      uintptr_t offsets, uintptr_t nodes, uintptr_t codes, int n_words, int max_len, int d, float alpha,
+                      uintptr_t loss, uintptr_t stats, bool deterministic) {
+    hs_step(backend_of(be), (cudaStream_t)stream, ptr<const Key>(centers), ptr<const Key>(contexts), n_items, nc,
+            ptr<const int64_t>(offsets), ptr<const int32_t>(nodes), ptr<const uint32_t>(codes), n_words, max_len, d,
+            alpha, ptr<float>(loss), ptr<unsigned long long>(stats), deterministic);
+  });
   m.def("sample_keys", [](uintptr_t be, uintptr_t stream, int kind, uintptr_t prob, uintptr_t alias, int64_t n_table,
                           Key first, Key stride, uintptr_t out, int64_t n, uint64_t seed, bool local_only, int max_tries,
                           uintptr_t stats) {

@@ -9,6 +9,14 @@
 //   syn0[c] += [alpha neu1e / sqrt(a_c + neu1e^2) | neu1e^2]          one push per context occurrence
 // A window with centre < 0 or no context does nothing.
 //
+// Hierarchical softmax (word2vec.c's -hs 1) is the same body with another target source. The centre's syn1 key 2w + 1
+// names the word w whose Huffman path supplies the targets: lane j gets inner node nodes[offsets[w] + j] (row
+// syn1_key(node) = 2 node + 1) with label 1 - bit j of codes[w], for j < len(w) <= 32. A node with |f| >= 6 gets no
+// update and adds nothing to neu1e (word2vec.c and gensim skip it); its loss term is counted. The skip-gram form is an
+// item with one context. The root is on every path, so in the deterministic step it takes one contribution per item:
+// its AdaGrad half gains sum over the step's items of (g h)^2 per element, which must stay below 2^27 (|g h| < 1 per
+// item keeps it there for B < 2^27 items; h is a mean of embeddings, |h| < 1 in practice).
+//
 // Two paths, selected by the world size:
 //  * in place (several GPUs; on one GPU on request): cbow_step_kernel, one warp per window. The lanes resolve the
 //    contexts and the targets through the directory at once. The window's rows stream through a per-warp shared-memory
@@ -51,15 +59,81 @@ using dev::warp_sum;
 // What the score pass writes besides the loss.
 struct CbowScoreOut {
   float* vecs;                   // [2 B x d]: h of window w at row w, neu1e at row B + w
-  float* gs;                     // [B x (1 + neg)]: g of target t of window w, kNoEntry if the target adds nothing
+  float* gs;                     // [B x n_t]: g of target t of window w, kNoEntry if the target adds nothing
 };
 
-// Lane-resolved window: lane l holds context occurrence l and target l (0: the centre, 1 + j: negative j).
+// Where a window's targets come from. n_t(): target slots per window. target(): lane l's target key (-1: none) of a
+// window with centre ckey >= 0, filling the window's Item. label(): target s's label. slow_key(): target s's key again,
+// for the generic path. entry_key() / entry_counts(): entry s < n_t() of the deterministic step's index and group
+// kernels (entry_key also gives the contexts' entries), which skip entries for which entry_counts() is false.
+//
+// Negative sampling: the centre (label 1) and the negatives (label 0; one equal to the centre is skipped); the gradient
+// saturates at |f| > 6.
+struct NegTargets {
+  const Key* __restrict__ negatives;
+  int neg;
+  static constexpr bool kSkipSaturated = false;
+  struct Item {};
+  __host__ __device__ __forceinline__ int n_t() const { return neg + 1; }
+  __device__ __forceinline__ Key target(Item&, Key ckey, int w, int lane, int n_t) const {
+    Key tk = lane == 0 ? ckey : (lane < n_t ? negatives[(size_t)w * neg + lane - 1] : -1);
+    if (lane > 0 && tk == ckey) tk = -1;
+    return tk;
+  }
+  __device__ __forceinline__ float label(const Item&, int s) const { return s == 0 ? 1.f : 0.f; }
+  __device__ __forceinline__ Key slow_key(Key ckey, int w, int s) const {
+    return s == 0 ? ckey : negatives[(size_t)w * neg + s - 1];
+  }
+  __device__ __forceinline__ Key entry_key(const Key* centers, const Key* contexts, int nc, int w, int s) const {
+    const int n_t = neg + 1;
+    return s == 0 ? centers[w] : (s < n_t ? negatives[(size_t)w * neg + s - 1] : contexts[(size_t)w * nc + s - n_t]);
+  }
+  // what adds nothing: a key < 0, every entry of a window whose centre is < 0, a negative equal to the centre
+  __device__ __forceinline__ bool entry_counts(const Key* centers, int w, int s, Key k) const {
+    const Key ck = centers[w];
+    return k >= 0 && ck >= 0 && !(s >= 1 && s <= neg && k == ck);
+  }
+};
+
+// Hierarchical softmax: the Huffman path of the centre's word (offsets [n_words + 1], nodes, codes [n_words]: the CSR of
+// the tree, root first). A centre whose word is not in the tree has no targets.
+struct PathTargets {
+  const int64_t* __restrict__ offsets;
+  const int32_t* __restrict__ nodes;
+  const uint32_t* __restrict__ codes;
+  int n_words;
+  int max_len;
+  static constexpr bool kSkipSaturated = true;
+  struct Item { uint32_t code; };
+  __host__ __device__ __forceinline__ int n_t() const { return max_len; }
+  __device__ __forceinline__ Key node_key(Key ckey, int s) const {   // -1 past the end of the path
+    const Key word = ckey >> 1;
+    if (word >= n_words) return -1;
+    const int64_t o = offsets[word];
+    return s < offsets[word + 1] - o ? 2 * (Key)nodes[o + s] + 1 : -1;
+  }
+  __device__ __forceinline__ Key target(Item& it, Key ckey, int, int lane, int) const {
+    it.code = (ckey >> 1) < n_words ? codes[ckey >> 1] : 0u;
+    return node_key(ckey, lane);
+  }
+  __device__ __forceinline__ float label(const Item& it, int s) const { return (it.code >> s) & 1u ? 0.f : 1.f; }
+  __device__ __forceinline__ Key slow_key(Key ckey, int, int s) const { return node_key(ckey, s); }
+  __device__ __forceinline__ Key entry_key(const Key* centers, const Key* contexts, int nc, int w, int s) const {
+    if (s >= max_len) return contexts[(size_t)w * nc + s - max_len];
+    const Key ck = centers[w];
+    return ck >= 0 ? node_key(ck, s) : -1;
+  }
+  __device__ __forceinline__ bool entry_counts(const Key* centers, int w, int, Key k) const {
+    return k >= 0 && centers[w] >= 0;
+  }
+};
+
+// Lane-resolved window: lane l holds context occurrence l and target l (ts.target(.., l, ..)).
 // bits: 1 context present, 2 its mark is a replica dirty byte, 4 target present, 8 its mark is a dirty byte.
-template <int VPL, bool SCORE>
+template <int VPL, bool SCORE, class Src>
 __device__ __forceinline__ void
-cbow_step_body(const Ctx& c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
-               const Key* __restrict__ negatives, int n_win, int nc, int neg, int d, float alpha,
+cbow_step_body(const Ctx& c, const Key* __restrict__ centers, const Key* __restrict__ contexts, const Src& ts,
+               int n_win, int nc, int d, float alpha,
                float* __restrict__ loss_out, unsigned long long* __restrict__ stats,
                unsigned long long* __restrict__ fx_loss, const CbowScoreOut& so) {
   constexpr bool BULK = !SCORE;
@@ -71,7 +145,7 @@ cbow_step_body(const Ctx& c, const Key* __restrict__ centers, const Key* __restr
   const int warp = blockIdx.x * kWarps + wib;
   const int nwarps = gridDim.x * kWarps;
   const int nvec = d >> 2;
-  const int n_t = neg + 1;
+  const int n_t = ts.n_t();
   const uint32_t half_bytes = (uint32_t)(d * sizeof(float));
   const uint32_t row_bytes = 2 * half_bytes;
   const size_t buf_floats = ((size_t)2 * d + 31) & ~(size_t)31;  // keep every ring slot 128-byte aligned
@@ -96,10 +170,10 @@ cbow_step_body(const Ctx& c, const Key* __restrict__ centers, const Key* __restr
     float* t_row = nullptr;
     void* t_mark = nullptr;
     int bits = 0;
+    typename Src::Item it{};
     if (ckey >= 0) {
       const Key xk = lane < nc ? contexts[(size_t)w * nc + lane] : -1;
-      Key tk = lane == 0 ? ckey : (lane < n_t ? negatives[(size_t)w * neg + lane - 1] : -1);
-      if (lane > 0 && tk == ckey) tk = -1;        // a negative equal to the centre is skipped
+      const Key tk = ts.target(it, ckey, w, lane, n_t);
       if (xk >= 0) {
         const Target tg = dev::resolve_fast(c, xk, 0, &n_local, &n_remote);
         x_row = tg.row;
@@ -214,14 +288,15 @@ cbow_step_body(const Ctx& c, const Key* __restrict__ centers, const Key* __restr
       } else if (i < n_x + n_tt) {
         // ---- target: score against h, g, neu1e, the target's update
         const float* tr = (const float*)__shfl_sync(0xffffffffu, (unsigned long long)t_row, src);
-        const float label = src == 0 ? 1.f : 0.f;
+        const float label = ts.label(it, src);
         if (BULK && tr == nullptr) {
           ++n_slow;
           slot_free();
           have_slow = true;
-          const Key tk = src == 0 ? ckey : negatives[(size_t)w * neg + src - 1];
+          const Key tk = ts.slow_key(ckey, w, src);
           bool applied;
-          loss_acc += sgns::slow_target(c, tk, label, alpha, d, buf, scratch, scratch + d, &applied);
+          loss_acc += sgns::slow_target<Src::kSkipSaturated>(c, tk, label, alpha, d, buf, scratch, scratch + d,
+                                                             &applied);
           if (applied) ++n_upd;
         } else {
           float f = 0.f;
@@ -236,7 +311,11 @@ cbow_step_body(const Ctx& c, const Key* __restrict__ centers, const Key* __restr
           }
           f = warp_sum(f);
           float gs;
-          if (f > kMaxExp) gs = label - 1.f;
+          bool skip = false;                       // hierarchical softmax: |f| >= 6 adds nothing
+          if constexpr (Src::kSkipSaturated) {
+            skip = fabsf(f) >= kMaxExp;
+            gs = label - 1.f / (1.f + __expf(-f));
+          } else if (f > kMaxExp) gs = label - 1.f;
           else if (f < -kMaxExp) gs = label;
           else gs = label - 1.f / (1.f + __expf(-f));
           {
@@ -244,36 +323,39 @@ cbow_step_body(const Ctx& c, const Key* __restrict__ centers, const Key* __restr
             z = fminf(fmaxf(z, -kMaxExp), kMaxExp);
             loss_acc += __logf(1.f + __expf(-z));
           }
+          if (!skip) {
 #pragma unroll
-          for (int v = 0; v < VPL; ++v) {
-            const int j = lane + v * 32;
-            if (j < nvec) {
-              const float4 e = reinterpret_cast<const float4*>(buf)[j];
-              nu[v].x += gs * e.x; nu[v].y += gs * e.y; nu[v].z += gs * e.z; nu[v].w += gs * e.w;
-              if (BULK) {
-                const float4 a = reinterpret_cast<const float4*>(buf + d)[j];
-                const float4 h = reinterpret_cast<const float4*>(scratch)[j];
-                const float4 gr = make_float4(gs * h.x, gs * h.y, gs * h.z, gs * h.w);
-                const float4 ua = make_float4(gr.x * gr.x, gr.y * gr.y, gr.z * gr.z, gr.w * gr.w);
-                float4 ue;
-                ue.x = alpha * gr.x * rsqrtf(a.x + ua.x);
-                ue.y = alpha * gr.y * rsqrtf(a.y + ua.y);
-                ue.z = alpha * gr.z * rsqrtf(a.z + ua.z);
-                ue.w = alpha * gr.w * rsqrtf(a.w + ua.w);
-                reinterpret_cast<float4*>(buf)[j] = ue;      // stage the update in place of the consumed row
-                reinterpret_cast<float4*>(buf + d)[j] = ua;
+            for (int v = 0; v < VPL; ++v) {
+              const int j = lane + v * 32;
+              if (j < nvec) {
+                const float4 e = reinterpret_cast<const float4*>(buf)[j];
+                nu[v].x += gs * e.x; nu[v].y += gs * e.y; nu[v].z += gs * e.z; nu[v].w += gs * e.w;
+                if (BULK) {
+                  const float4 a = reinterpret_cast<const float4*>(buf + d)[j];
+                  const float4 h = reinterpret_cast<const float4*>(scratch)[j];
+                  const float4 gr = make_float4(gs * h.x, gs * h.y, gs * h.z, gs * h.w);
+                  const float4 ua = make_float4(gr.x * gr.x, gr.y * gr.y, gr.z * gr.z, gr.w * gr.w);
+                  float4 ue;
+                  ue.x = alpha * gr.x * rsqrtf(a.x + ua.x);
+                  ue.y = alpha * gr.y * rsqrtf(a.y + ua.y);
+                  ue.z = alpha * gr.z * rsqrtf(a.z + ua.z);
+                  ue.w = alpha * gr.w * rsqrtf(a.w + ua.w);
+                  reinterpret_cast<float4*>(buf)[j] = ue;      // stage the update in place of the consumed row
+                  reinterpret_cast<float4*>(buf + d)[j] = ua;
+                }
               }
             }
-          }
-          if (BULK) {
-            __syncwarp();
-            if (lane == 0) {
-              asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the staged update is visible to the TMA engine
-              bulk_red_s2g(const_cast<float*>(tr), buf, row_bytes);
+            if (BULK) {
+              __syncwarp();
+              if (lane == 0) {
+                // the staged update is visible to the TMA engine
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                bulk_red_s2g(const_cast<float*>(tr), buf, row_bytes);
+              }
             }
+            if (lane == src) { mark_pushed(t_mark, bits >> 2); my_gs = gs; }
+            ++n_upd;
           }
-          if (lane == src) { mark_pushed(t_mark, bits >> 2); my_gs = gs; }
-          ++n_upd;
         }
         if (i == n_x + n_tt - 1) {
           if (have_slow) {                 // neu1e of the targets that took the generic path
@@ -370,8 +452,8 @@ __global__ void __maxnreg__(104)
 cbow_step_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
                  const Key* __restrict__ negatives, int n_win, int nc, int neg, int d, float alpha,
                  float* __restrict__ loss_out, unsigned long long* __restrict__ stats) {
-  cbow_step_body<VPL, false>(c, centers, contexts, negatives, n_win, nc, neg, d, alpha, loss_out, stats, nullptr,
-                             CbowScoreOut{});
+  cbow_step_body<VPL, false>(c, centers, contexts, NegTargets{negatives, neg}, n_win, nc, d, alpha, loss_out, stats,
+                             nullptr, CbowScoreOut{});
 }
 
 template <int VPL>
@@ -380,32 +462,41 @@ cbow_score_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers
                   const Key* __restrict__ negatives, int n_win, int nc, int neg, int d,
                   unsigned long long* __restrict__ stats, unsigned long long* __restrict__ fx_loss,
                   const __grid_constant__ CbowScoreOut so) {
-  cbow_step_body<VPL, true>(c, centers, contexts, negatives, n_win, nc, neg, d, 0.f, nullptr, stats, fx_loss, so);
+  cbow_step_body<VPL, true>(c, centers, contexts, NegTargets{negatives, neg}, n_win, nc, d, 0.f, nullptr, stats, fx_loss,
+                            so);
+}
+
+template <int VPL>
+__global__ void __maxnreg__(104)
+hs_step_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
+               const __grid_constant__ PathTargets ts, int n_win, int nc, int d, float alpha,
+               float* __restrict__ loss_out, unsigned long long* __restrict__ stats) {
+  cbow_step_body<VPL, false>(c, centers, contexts, ts, n_win, nc, d, alpha, loss_out, stats, nullptr, CbowScoreOut{});
+}
+
+template <int VPL>
+__global__ void __maxnreg__(128)
+hs_score_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
+                const __grid_constant__ PathTargets ts, int n_win, int nc, int d, unsigned long long* __restrict__ stats,
+                unsigned long long* __restrict__ fx_loss, const __grid_constant__ CbowScoreOut so) {
+  cbow_step_body<VPL, true>(c, centers, contexts, ts, n_win, nc, d, 0.f, nullptr, stats, fx_loss, so);
 }
 
 // ---- deterministic one-GPU step: index, score, group by key, gather (sgns_det.cuh)
-// Entry x = w * (n_t + nc) + s of a step: s < n_t target s of window w (0: the centre), else context occurrence s - n_t.
-__device__ __forceinline__ Key cbow_entry_key(const Key* centers, const Key* contexts, const Key* negatives, int nc,
-                                              int neg, int w, int s) {
-  const int n_t = neg + 1;
-  return s == 0 ? centers[w] : (s < n_t ? negatives[(size_t)w * neg + s - 1] : contexts[(size_t)w * nc + s - n_t]);
-}
-// what adds nothing: a key < 0, every entry of a window whose centre is < 0, a negative equal to the centre
-__device__ __forceinline__ bool cbow_entry_counts(const Key* centers, int neg, int w, int s, Key k) {
-  const Key ck = centers[w];
-  return k >= 0 && ck >= 0 && !(s >= 1 && s <= neg && k == ck);
-}
+// Entry x = w * (n_t + nc) + s of a step: s < n_t target s of window w, else context occurrence s - n_t
+// (Src::entry_key, Src::entry_counts).
 
 // Gives every key of the step's entries a compact id (cidx[key], keys[id]) and looks its row up once (rowp[id]).
-__global__ void cbow_det_index_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers,
-                                      const Key* __restrict__ contexts, const Key* __restrict__ negatives, int n_win,
-                                      int nc, int neg, int* __restrict__ cidx, Key* __restrict__ keys,
-                                      float** __restrict__ rowp, unsigned int* __restrict__ count) {
-  const int per = neg + 1 + nc;
+template <class Src>
+__device__ __forceinline__ void det_index_body(const Ctx& c, const Key* __restrict__ centers,
+                                               const Key* __restrict__ contexts, const Src& ts, int n_win, int nc,
+                                               int* __restrict__ cidx, Key* __restrict__ keys,
+                                               float** __restrict__ rowp, unsigned int* __restrict__ count) {
+  const int per = ts.n_t() + nc;
   const long n = (long)n_win * per;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
     const int w = (int)(i / per), s = (int)(i % per);
-    const Key k = cbow_entry_key(centers, contexts, negatives, nc, neg, w, s);
+    const Key k = ts.entry_key(centers, contexts, nc, w, s);
     // (the plain load skips the atomic for keys that are already claimed: frequent words appear thousands of times)
     if (k >= 0 && cidx[k] == -1 && atomicCAS(cidx + k, -1, -2) == -1) {
       const unsigned r = atomicAdd(count, 1u);
@@ -419,18 +510,18 @@ __global__ void cbow_det_index_kernel(const __grid_constant__ Ctx c, const Key* 
 // SCATTER = false: cnt[id] = entries of key id. SCATTER = true: desc / kid of CSR position off[id] + i, i < cnt[id],
 // describe the entries of key id; counts cnt back down to zero. A target adds g_t times the window's h (vector row w),
 // a context occurrence 1 times the window's neu1e (vector row n_win + w).
-template <bool SCATTER>
-__global__ void cbow_det_group_kernel(const Key* __restrict__ centers, const Key* __restrict__ contexts,
-                                      const Key* __restrict__ negatives, int n_win, int nc, int neg,
-                                      const int* __restrict__ cidx, int* __restrict__ cnt, const int* __restrict__ off,
-                                      int* __restrict__ kid, const float* __restrict__ gsb,
-                                      GatherDesc* __restrict__ desc) {
-  const int n_t = neg + 1, per = n_t + nc;
+template <bool SCATTER, class Src>
+__device__ __forceinline__ void det_group_body(const Key* __restrict__ centers, const Key* __restrict__ contexts,
+                                               const Src& ts, int n_win, int nc, const int* __restrict__ cidx,
+                                               int* __restrict__ cnt, const int* __restrict__ off,
+                                               int* __restrict__ kid, const float* __restrict__ gsb,
+                                               GatherDesc* __restrict__ desc) {
+  const int n_t = ts.n_t(), per = n_t + nc;
   const long n = (long)n_win * per;
   for (long x = (long)blockIdx.x * blockDim.x + threadIdx.x; x < n; x += (long)gridDim.x * blockDim.x) {
     const int w = (int)(x / per), s = (int)(x - (long)w * per);
-    const Key k = cbow_entry_key(centers, contexts, negatives, nc, neg, w, s);
-    if (!cbow_entry_counts(centers, neg, w, s, k)) continue;
+    const Key k = ts.entry_key(centers, contexts, nc, w, s);
+    if (!ts.entry_counts(centers, w, s, k)) continue;
     const int id = __ldg(cidx + k);
     if (!SCATTER) {
       atomicAdd(cnt + id, 1);
@@ -450,11 +541,97 @@ __global__ void cbow_det_group_kernel(const Key* __restrict__ centers, const Key
   }
 }
 
-void cbow_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, const Key* negatives,
-                   int n_win, int nc, int neg, int d, float alpha, float* loss_out, unsigned long long* stats, int vpl,
+__global__ void cbow_det_index_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers,
+                                      const Key* __restrict__ contexts, const Key* __restrict__ negatives, int n_win,
+                                      int nc, int neg, int* __restrict__ cidx, Key* __restrict__ keys,
+                                      float** __restrict__ rowp, unsigned int* __restrict__ count) {
+  det_index_body(c, centers, contexts, NegTargets{negatives, neg}, n_win, nc, cidx, keys, rowp, count);
+}
+__global__ void hs_det_index_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers,
+                                    const Key* __restrict__ contexts, const __grid_constant__ PathTargets ts, int n_win,
+                                    int nc, int* __restrict__ cidx, Key* __restrict__ keys, float** __restrict__ rowp,
+                                    unsigned int* __restrict__ count) {
+  det_index_body(c, centers, contexts, ts, n_win, nc, cidx, keys, rowp, count);
+}
+
+template <bool SCATTER>
+__global__ void cbow_det_group_kernel(const Key* __restrict__ centers, const Key* __restrict__ contexts,
+                                      const Key* __restrict__ negatives, int n_win, int nc, int neg,
+                                      const int* __restrict__ cidx, int* __restrict__ cnt, const int* __restrict__ off,
+                                      int* __restrict__ kid, const float* __restrict__ gsb,
+                                      GatherDesc* __restrict__ desc) {
+  det_group_body<SCATTER>(centers, contexts, NegTargets{negatives, neg}, n_win, nc, cidx, cnt, off, kid, gsb, desc);
+}
+template <bool SCATTER>
+__global__ void hs_det_group_kernel(const Key* __restrict__ centers, const Key* __restrict__ contexts,
+                                    const __grid_constant__ PathTargets ts, int n_win, int nc,
+                                    const int* __restrict__ cidx, int* __restrict__ cnt, const int* __restrict__ off,
+                                    int* __restrict__ kid, const float* __restrict__ gsb,
+                                    GatherDesc* __restrict__ desc) {
+  det_group_body<SCATTER>(centers, contexts, ts, n_win, nc, cidx, cnt, off, kid, gsb, desc);
+}
+
+// The kernels of one target source.
+template <class Src> struct StepKernels;
+template <> struct StepKernels<NegTargets> {
+  template <int V> static void step(int blocks, size_t smem, cudaStream_t st, const Ctx& c, const Key* centers,
+                                    const Key* contexts, const NegTargets& ts, int n_win, int nc, int d, float alpha,
+                                    float* loss_out, unsigned long long* stats) {
+    set_max_dynamic_smem<cbow_step_kernel<V>>(110 * 1024);
+    cbow_step_kernel<V><<<blocks, kThreads, smem, st>>>(c, centers, contexts, ts.negatives, n_win, nc, ts.neg, d, alpha,
+                                                        loss_out, stats);
+  }
+  template <int V> static void score(int blocks, size_t smem, cudaStream_t st, const Ctx& c, const Key* centers,
+                                     const Key* contexts, const NegTargets& ts, int n_win, int nc, int d,
+                                     unsigned long long* stats, unsigned long long* fx_loss, const CbowScoreOut& so) {
+    set_max_dynamic_smem<cbow_score_kernel<V>>(110 * 1024);
+    cbow_score_kernel<V><<<blocks, kThreads, smem, st>>>(c, centers, contexts, ts.negatives, n_win, nc, ts.neg, d, stats,
+                                                         fx_loss, so);
+  }
+  static void index(int blocks, cudaStream_t st, const Ctx& c, const Key* centers, const Key* contexts,
+                    const NegTargets& ts, int n_win, int nc, int* cidx, Key* keys, float** rowp, unsigned int* count) {
+    cbow_det_index_kernel<<<blocks, 256, 0, st>>>(c, centers, contexts, ts.negatives, n_win, nc, ts.neg, cidx, keys,
+                                                  rowp, count);
+  }
+  template <bool SCATTER> static void group(int blocks, cudaStream_t st, const Key* centers, const Key* contexts,
+                                            const NegTargets& ts, int n_win, int nc, const int* cidx, int* cnt,
+                                            const int* off, int* kid, const float* gsb, GatherDesc* desc) {
+    cbow_det_group_kernel<SCATTER><<<blocks, 256, 0, st>>>(centers, contexts, ts.negatives, n_win, nc, ts.neg, cidx, cnt,
+                                                           off, kid, gsb, desc);
+  }
+};
+template <> struct StepKernels<PathTargets> {
+  template <int V> static void step(int blocks, size_t smem, cudaStream_t st, const Ctx& c, const Key* centers,
+                                    const Key* contexts, const PathTargets& ts, int n_win, int nc, int d, float alpha,
+                                    float* loss_out, unsigned long long* stats) {
+    set_max_dynamic_smem<hs_step_kernel<V>>(110 * 1024);
+    hs_step_kernel<V><<<blocks, kThreads, smem, st>>>(c, centers, contexts, ts, n_win, nc, d, alpha, loss_out, stats);
+  }
+  template <int V> static void score(int blocks, size_t smem, cudaStream_t st, const Ctx& c, const Key* centers,
+                                     const Key* contexts, const PathTargets& ts, int n_win, int nc, int d,
+                                     unsigned long long* stats, unsigned long long* fx_loss, const CbowScoreOut& so) {
+    set_max_dynamic_smem<hs_score_kernel<V>>(110 * 1024);
+    hs_score_kernel<V><<<blocks, kThreads, smem, st>>>(c, centers, contexts, ts, n_win, nc, d, stats, fx_loss, so);
+  }
+  static void index(int blocks, cudaStream_t st, const Ctx& c, const Key* centers, const Key* contexts,
+                    const PathTargets& ts, int n_win, int nc, int* cidx, Key* keys, float** rowp, unsigned int* count) {
+    hs_det_index_kernel<<<blocks, 256, 0, st>>>(c, centers, contexts, ts, n_win, nc, cidx, keys, rowp, count);
+  }
+  template <bool SCATTER> static void group(int blocks, cudaStream_t st, const Key* centers, const Key* contexts,
+                                            const PathTargets& ts, int n_win, int nc, const int* cidx, int* cnt,
+                                            const int* off, int* kid, const float* gsb, GatherDesc* desc) {
+    hs_det_group_kernel<SCATTER><<<blocks, 256, 0, st>>>(centers, contexts, ts, n_win, nc, cidx, cnt, off, kid, gsb,
+                                                         desc);
+  }
+};
+
+template <class Src>
+void cbow_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, const Src& ts,
+                   int n_win, int nc, int d, float alpha, float* loss_out, unsigned long long* stats, int vpl,
                    int score_blocks, size_t smem) {
+  using K = StepKernels<Src>;
   const Ctx& c = be.ctx();
-  const int n_t = neg + 1;
+  const int n_t = ts.n_t();
   const int n_entries = n_win * (n_t + nc);
   const int n_ids = (int)std::min<size_t>((size_t)n_entries, (size_t)c.L.num_keys);   // bound on the distinct keys
   const int n_ranges = (n_entries + kGatherRange - 1) / kGatherRange;
@@ -476,33 +653,48 @@ void cbow_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   const int grid_n = be.num_sms() * 8;
   auto blocks_for = [&](long n) { return (int)std::max<long>(1, std::min<long>((n + 255) / 256, grid_n)); };
   ADAPM_CUDA_CHECK(cudaMemsetAsync(fx.count, 0, 2 * sizeof(unsigned int), stream));
-  cbow_det_index_kernel<<<blocks_for(n_entries), 256, 0, stream>>>(c, centers, contexts, negatives, n_win, nc, neg,
-                                                                    fx.cidx, fx.keys, rowp, fx.count);
+  K::index(blocks_for(n_entries), stream, c, centers, contexts, ts, n_win, nc, fx.cidx, fx.keys, rowp, fx.count);
   ADAPM_COUNT_LAUNCH();
-#define ADAPM_LAUNCH_CBOW_SCORE(V)                                                                          \
-  do {                                                                                                      \
-    set_max_dynamic_smem<cbow_score_kernel<V>>(110 * 1024);                                                 \
-    cbow_score_kernel<V><<<score_blocks, kThreads, smem, stream>>>(c, centers, contexts, negatives, n_win, nc, neg, \
-                                                                   d, stats, fx.loss, so);                  \
-  } while (0)
   switch (vpl) {
-    case 1: ADAPM_LAUNCH_CBOW_SCORE(1); break;
-    case 2: ADAPM_LAUNCH_CBOW_SCORE(2); break;
-    default: ADAPM_LAUNCH_CBOW_SCORE(3); break;
+    case 1: K::template score<1>(score_blocks, smem, stream, c, centers, contexts, ts, n_win, nc, d, stats, fx.loss, so); break;
+    case 2: K::template score<2>(score_blocks, smem, stream, c, centers, contexts, ts, n_win, nc, d, stats, fx.loss, so); break;
+    default: K::template score<3>(score_blocks, smem, stream, c, centers, contexts, ts, n_win, nc, d, stats, fx.loss, so); break;
   }
-#undef ADAPM_LAUNCH_CBOW_SCORE
   ADAPM_COUNT_LAUNCH();
-  cbow_det_group_kernel<false><<<blocks_for(n_entries), 256, 0, stream>>>(centers, contexts, negatives, n_win, nc, neg,
-                                                                           fx.cidx, cnt, off, kid, so.gs, desc);
+  K::template group<false>(blocks_for(n_entries), stream, centers, contexts, ts, n_win, nc, fx.cidx, cnt, off, kid, so.gs,
+                           desc);
   ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, cnt, off, n_ids + 1, stream));
   ADAPM_COUNT_LAUNCH();
   ADAPM_COUNT_LAUNCH();   // (the scan is two kernels)
-  cbow_det_group_kernel<true><<<blocks_for(n_entries), 256, 0, stream>>>(centers, contexts, negatives, n_win, nc, neg,
-                                                                          fx.cidx, cnt, off, kid, so.gs, desc);
+  K::template group<true>(blocks_for(n_entries), stream, centers, contexts, ts, n_win, nc, fx.cidx, cnt, off, kid, so.gs,
+                          desc);
   ADAPM_COUNT_LAUNCH();
   det_gather_finish(be, stream, vpl, rowp, off, n_ids, kid, desc, so.vecs, d, alpha, part, n_ranges,
                     blocks_for(n_entries), fx, loss_out);
+  ADAPM_CUDA_CHECK(cudaGetLastError());
+}
+
+// One step of either target source: the deterministic step or one in-place launch. The caller checks the arguments.
+template <class Src>
+void run_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, const Src& ts, int n_win,
+              int nc, int d, float alpha, float* loss_out, unsigned long long* stats, bool deterministic) {
+  const int vpl = (d / 4 + 31) / 32;
+  const size_t buf_floats = ((size_t)2 * d + 31) & ~(size_t)31;
+  const size_t smem = (size_t)kWarps * (RING + 1) * buf_floats * sizeof(float) + 128;   // <= 110 KB: 2 blocks per SM
+  const int blocks = std::min((n_win + kWarps - 1) / kWarps, be.num_sms() * 12);
+  if (deterministic) {
+    cbow_step_det(be, stream, centers, contexts, ts, n_win, nc, d, alpha, loss_out, stats, vpl, blocks, smem);
+    return;
+  }
+  using K = StepKernels<Src>;
+  const Ctx& c = be.ctx();
+  switch (vpl) {
+    case 1: K::template step<1>(blocks, smem, stream, c, centers, contexts, ts, n_win, nc, d, alpha, loss_out, stats); break;
+    case 2: K::template step<2>(blocks, smem, stream, c, centers, contexts, ts, n_win, nc, d, alpha, loss_out, stats); break;
+    default: K::template step<3>(blocks, smem, stream, c, centers, contexts, ts, n_win, nc, d, alpha, loss_out, stats); break;
+  }
+  ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cudaGetLastError());
 }
 
@@ -514,32 +706,25 @@ void cbow_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const K
   ADAPM_CHECK(d % 4 == 0 && d >= 4 && d <= kCbowMaxDim, "cbow_step: embed_dim must be a multiple of 4 in [4, 336]");
   ADAPM_CHECK(neg >= 0 && neg + 1 <= kCbowMaxTargets, "cbow_step: 1 + negative must be at most 32");
   ADAPM_CHECK(nc >= 1 && nc <= kCbowMaxContexts, "cbow_step: 1 to 32 context columns");
-  const Ctx& c = be.ctx();
-  ADAPM_CHECK(!deterministic || c.L.world == 1, "cbow_step: the deterministic step needs a single-GPU store");
+  ADAPM_CHECK(!deterministic || be.ctx().L.world == 1, "cbow_step: the deterministic step needs a single-GPU store");
   if (n_win <= 0) return;
   ADAPM_CHECK((long)n_win * (neg + 1 + nc) < (1L << 30), "cbow_step: too many keys in one step");
-  const int vpl = (d / 4 + 31) / 32;
-  const size_t buf_floats = ((size_t)2 * d + 31) & ~(size_t)31;
-  const size_t smem = (size_t)kWarps * (RING + 1) * buf_floats * sizeof(float) + 128;   // <= 110 KB: 2 blocks per SM
-  const int blocks = std::min((n_win + kWarps - 1) / kWarps, be.num_sms() * 12);
-  if (deterministic) {
-    cbow_step_det(be, stream, centers, contexts, negatives, n_win, nc, neg, d, alpha, loss_out, stats, vpl, blocks, smem);
-    return;
-  }
-#define ADAPM_LAUNCH_CBOW(V)                                                                                \
-  do {                                                                                                      \
-    set_max_dynamic_smem<cbow_step_kernel<V>>(110 * 1024);                                                  \
-    cbow_step_kernel<V><<<blocks, kThreads, smem, stream>>>(c, centers, contexts, negatives, n_win, nc, neg, d,     \
-                                                            alpha, loss_out, stats);                        \
-  } while (0)
-  switch (vpl) {
-    case 1: ADAPM_LAUNCH_CBOW(1); break;
-    case 2: ADAPM_LAUNCH_CBOW(2); break;
-    default: ADAPM_LAUNCH_CBOW(3); break;
-  }
-#undef ADAPM_LAUNCH_CBOW
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_CUDA_CHECK(cudaGetLastError());
+  run_step(be, stream, centers, contexts, NegTargets{negatives, neg}, n_win, nc, d, alpha, loss_out, stats,
+           deterministic);
+}
+
+void hs_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, int n_items, int nc,
+             const int64_t* offsets, const int32_t* nodes, const uint32_t* codes, int n_words, int max_len, int d,
+             float alpha, float* loss_out, unsigned long long* stats, bool deterministic) {
+  ADAPM_CHECK(d % 4 == 0 && d >= 4 && d <= kCbowMaxDim, "hs_step: embed_dim must be a multiple of 4 in [4, 336]");
+  ADAPM_CHECK(max_len >= 1 && max_len <= kCbowMaxTargets, "hs_step: the tree's paths must be 1 to 32 nodes long");
+  ADAPM_CHECK(n_words >= 2, "hs_step: the tree needs at least 2 words");
+  ADAPM_CHECK(nc >= 1 && nc <= kCbowMaxContexts, "hs_step: 1 to 32 context columns");
+  ADAPM_CHECK(!deterministic || be.ctx().L.world == 1, "hs_step: the deterministic step needs a single-GPU store");
+  if (n_items <= 0) return;
+  ADAPM_CHECK((long)n_items * (max_len + nc) < (1L << 30), "hs_step: too many keys in one step");
+  run_step(be, stream, centers, contexts, PathTargets{offsets, nodes, codes, n_words, max_len}, n_items, nc, d, alpha,
+           loss_out, stats, deterministic);
 }
 
 }  // namespace cudaops

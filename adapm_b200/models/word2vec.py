@@ -22,6 +22,13 @@ the mean ``h`` of the context rows is scored against the centre's syn1 row and t
 ``g_t h`` and every context occurrence the unscaled ``neu1e = sum_t g_t t`` (word2vec.c), each through worker-side
 AdaGrad (``cbow_reference_step``; ``ops.cbow_step`` on the GPU). Batches are windows ``[B, 1 + 2 window]`` (centre syn1
 key, context syn0 keys, -1 padding) from ``NativeCorpus.window_batches`` or ``windows_from_sentences``.
+
+Hierarchical softmax (``hs=True``, word2vec.c's ``-hs 1``, with ``negative=0``) replaces the negatives by the inner nodes
+on the Huffman path of the syn1-side word (``utils.text.huffman_tree`` over the model's counts, word2vec.c's tree):
+node ``n`` is the row ``syn1_key(n)``, its label is ``1 - code bit``, and a node with ``|f| >= 6`` is skipped
+(``hs_reference_step``; ``ops.hs_step`` on the GPU). Skip-gram trains ``syn0[context]`` on the centre word's path
+(word2vec.c's pairing: the pair batch's syn1 word supplies the path, its syn0 word is the one context); CBOW trains the
+window's mean on the centre's path. No negatives are drawn.
 """
 from __future__ import annotations
 
@@ -55,6 +62,7 @@ class Word2VecConfig:
                                      # (ops.SgnsSharedStep); 0: `negative` private negatives per pair (the reference)
     cbow: bool = False               # continuous bag of words (word2vec.c -cbow 1) instead of skip-gram
     batch_windows: int = 8192        # CBOW: windows per step
+    hs: bool = False                 # hierarchical softmax (word2vec.c -hs 1) instead of negative sampling (negative = 0)
 
     @property
     def row_len(self) -> int:
@@ -153,10 +161,21 @@ class Word2Vec:
         assert len(self.counts) == cfg.vocab_size
         if cfg.cbow and cfg.shared_negatives > 0:
             raise ValueError("shared_negatives is a skip-gram option: CBOW draws its own negatives per window")
+        if cfg.hs and (cfg.negative > 0 or cfg.shared_negatives > 0):
+            raise ValueError("hierarchical softmax together with negative sampling is not supported: set negative=0 "
+                             "and shared_negatives=0 with hs=True")
         self.cuda = server.backend == "cuda"
         self.alpha = cfg.starting_alpha
         self.step_no = 0
         weights = np.power(self.counts, cfg.neg_power)
+        self.tree = None
+        if cfg.hs:
+            from ..utils.text import huffman_tree
+
+            host = huffman_tree(self.counts)
+            self._tree_host = (host.offsets.numpy(), host.nodes.numpy())
+            self._seen = np.zeros(cfg.vocab_size, dtype=np.int32)   # intent_keys_hs's marker array (words, nodes)
+            self.tree = host.to(server.device) if self.cuda else host
         if self.cuda:
             from ..ops import DeviceSampler
 
@@ -221,11 +240,44 @@ class Word2Vec:
             keys = keys_host.reshape(-1)
             if self.cfg.cbow:
                 keys = keys[keys >= 0]                 # window padding
+        if self.cfg.hs:
+            keys = self.intent_keys_hs(keys)
         if self.cuda and self._prepass is not None:
             self._prepass.harvest()                    # left-overs of earlier batches -> host path
             self._prepass.submit(keys, clock, clock + 1)
             return
         self.worker.intent(keys, clock, clock + 1)
+
+    def intent_keys_hs(self, keys: torch.Tensor) -> torch.Tensor:
+        """Hierarchical softmax: the rows a batch with these keys touches, i.e. its syn0 keys and the syn1 keys of the
+        inner nodes on the paths of its syn1 words, each once. Paths share their top levels, so the nodes are
+        deduplicated with a marker array (the position that last wrote each node) rather than by sorting."""
+        k = keys.numpy() if isinstance(keys, torch.Tensor) else np.asarray(keys)
+        off, nodes = self._tree_host
+        seen = self._seen
+
+        def once(v):                      # each value of v once: the position that wrote it last keeps it
+            pos = np.arange(v.size)
+            seen[v] = pos
+            return v[seen[v] == pos]
+
+        words = once(k[(k & 1) == 1] >> 1)
+        start, lens = off[words], off[words + 1] - off[words]
+        n = int(lens.sum())
+        idx = np.repeat(start - np.cumsum(lens) + lens, lens) + np.arange(n)   # positions of every path entry
+        path = once(nodes[idx])
+        return torch.from_numpy(np.concatenate([k[(k & 1) == 0], 2 * path.astype(np.int64) + 1]))
+
+    def loss_terms(self, keys_host: torch.Tensor) -> int:
+        """Terms of a batch's summed loss: hierarchical softmax, the path nodes of its items; else ``negative + 1`` per
+        item."""
+        cfg = self.cfg
+        centres = keys_host[:, 0] if cfg.cbow else keys_host[1]
+        if not cfg.hs:
+            return int(centres.numel()) * (cfg.negative + 1)
+        off = self._tree_host[0]
+        w = centres[centres >= 0].numpy() >> 1
+        return int((off[w + 1] - off[w]).sum())
 
     # ------------------------------------------------------------------ one training step
     def step(self, keys_host: torch.Tensor) -> torch.Tensor:
@@ -244,7 +296,8 @@ class Word2Vec:
             else:
                 kd = self._keys_dev[slot]
                 kd.copy_(keys_host, non_blocking=True)               # H2D of this step's inputs
-            self.sample_negatives()
+            if not cfg.hs:
+                self.sample_negatives()
             self._device_step(*self._operands(kd))
             ev = self._events[slot] or torch.cuda.Event()
             ev.record()
@@ -283,7 +336,15 @@ class Word2Vec:
         from ..ops import SgnsSharedStep, sgns_step
 
         cfg = self.cfg
-        if cfg.cbow:
+        if cfg.hs:
+            from ..ops import hs_step
+
+            if cfg.cbow:
+                hs_step(self.server, centers, contexts, self.tree, cfg.embed_dim, self.alpha, self.loss, self.stats)
+            else:                         # the pair's syn1 word supplies the path, its syn0 word is the one context
+                hs_step(self.server, contexts, centers.view(-1, 1), self.tree, cfg.embed_dim, self.alpha, self.loss,
+                        self.stats)
+        elif cfg.cbow:
             from ..ops import cbow_step
 
             cbow_step(self.server, centers, contexts, self._neg.view(centers.numel(), cfg.negative), cfg.embed_dim,
@@ -300,7 +361,8 @@ class Word2Vec:
         slot = self.step_no % len(self._events)
         if self._events[slot] is not None:
             self._events[slot].synchronize()
-        self.sample_negatives()
+        if not self.cfg.hs:
+            self.sample_negatives()
         self._device_step(*self._operands(keys_dev))
         ev = self._events[slot] or torch.cuda.Event()
         ev.record()
@@ -320,8 +382,9 @@ class Word2Vec:
         from .. import _C
 
         cfg = self.cfg
-        if cfg.cbow:
-            raise ValueError("run_steps drives skip-gram steps only: run CBOW steps with step()")
+        if cfg.cbow or cfg.hs:
+            raise ValueError("run_steps drives negative-sampling skip-gram steps only: run CBOW and hierarchical-softmax "
+                             "steps with step()")
         assert self.cuda, "run_steps needs the cuda backend"
         if getattr(self, "_loop", None) is None:
             local_only = cfg.sampling_scheme == "local" and self.server.num_servers() > 1
@@ -354,6 +417,13 @@ class Word2Vec:
     # reference-semantics step through the public Pull/Push API (CPU backend; also the numerics oracle)
     def _step_cpu(self, keys_host: torch.Tensor) -> torch.Tensor:
         cfg, kv, d = self.cfg, self.worker, self.cfg.embed_dim
+        if cfg.hs:
+            if cfg.cbow:
+                loss = hs_reference_step(kv, keys_host[:, 0], keys_host[:, 1:], self.tree, d, self.alpha)
+            else:
+                loss = hs_reference_step(kv, keys_host[1], keys_host[0].view(-1, 1), self.tree, d, self.alpha)
+            self.step_no += 1
+            return torch.tensor([loss], dtype=torch.float32)
         if cfg.cbow:
             B = keys_host.shape[0]
             u = torch.rand(B * cfg.negative, generator=self._gen, dtype=torch.float64)
@@ -611,5 +681,55 @@ def cbow_reference_step(kv, centers: torch.Tensor, contexts: torch.Tensor, negat
     ax = rx[:, d:]
     ux = torch.cat([alpha * gx / torch.sqrt(ax + gx * gx), gx * gx], -1)
     kv.wait(kv.push(torch.cat([tkeys, xkeys]), torch.cat([ut, ux]).contiguous().view(-1)))
+    z = torch.where(label > 0.5, f, -f).clamp(-6, 6)
+    return float((torch.log1p(torch.exp(-z)) * tm).sum())
+
+
+def hs_reference_step(kv, centers: torch.Tensor, contexts: torch.Tensor, tree, d: int, alpha: float) -> float:
+    """Plain PyTorch fp32 hierarchical-softmax step through Pull/Push, the rule of ``ops.hs_step``. ``centers``: [B]
+    syn1 keys ``2 w + 1`` (< 0: the item does nothing), ``contexts``: [B, C] syn0 keys (-1 = padding; C = 1 for
+    skip-gram), ``tree``: a :class:`adapm_b200.utils.text.HuffmanTree`. All items read the state at the start of the
+    step: ``h`` = mean of the C context embeddings (a repeated word counts every time); node j of word w's path
+    (row ``2 node + 1``) has label ``1 - bit j of codes[w]`` and score ``f_j = h . node``; a node with ``|f_j| >= 6``
+    gets no update and adds nothing to ``neu1e`` (word2vec.c), else ``g_j = label - sigmoid(f_j)``, one AdaGrad push of
+    ``g_j h`` per (item, node) and one of ``neu1e = sum_j g_j node_j`` per context occurrence; updates of repeated keys
+    add up. An item without a context does nothing. Returns the summed logistic loss over every path node, skipped or
+    not."""
+    centers = centers.reshape(-1)
+    B = centers.numel()
+    contexts = contexts.reshape(B, -1)
+    C = contexts.shape[1]
+    off, nodes, codes = tree.offsets.cpu(), tree.nodes.cpu(), tree.codes.cpu()
+    L = int(tree.max_len)
+    xm = (contexts >= 0) & (centers >= 0).view(B, 1)
+    n_ctx = xm.sum(1)
+    active = (centers >= 0) & (n_ctx > 0)
+    xm &= active.view(B, 1)
+    w = torch.where(active, centers // 2, torch.zeros_like(centers))
+    start, lens = off[w], off[w + 1] - off[w]
+    j = torch.arange(L)
+    tm = active.view(B, 1) & (j.view(1, L) < lens.view(B, 1))          # [B, L] path nodes
+    node = nodes[torch.where(tm, start.view(B, 1) + j.view(1, L), torch.zeros_like(tm, dtype=torch.int64))].long()
+    label = (1 - ((codes[w].view(B, 1) >> j.view(1, L).to(torch.int32)) & 1)).to(torch.float32)
+    xkeys, tkeys = contexts[xm], (2 * node + 1)[tm]
+    rows = torch.empty((xkeys.numel() + tkeys.numel()) * 2 * d, dtype=torch.float32)
+    kv.wait(kv.pull(torch.cat([xkeys, tkeys]), rows))
+    rows = rows.view(-1, 2 * d)
+    rx, rt = rows[:xkeys.numel()], rows[xkeys.numel():]
+    ex = torch.zeros(B, C, d)
+    ex[xm] = rx[:, :d]
+    h = ex.sum(1) / n_ctx.clamp(min=1).view(B, 1).to(torch.float32)
+    et, at = torch.zeros(B, L, d), torch.ones(B, L, d)
+    et[tm], at[tm] = rt[:, :d], rt[:, d:]
+    f = (h.unsqueeze(1) * et).sum(-1)
+    um = tm & (f.abs() < 6)                                           # nodes that get an update
+    g = (label - torch.sigmoid(f)) * um
+    neu1e = (g.unsqueeze(-1) * et).sum(1)
+    gt = g.unsqueeze(-1) * h.unsqueeze(1)
+    ut = torch.cat([alpha * gt / torch.sqrt(at + gt * gt), gt * gt], -1)[um]
+    gx = neu1e.unsqueeze(1).expand(B, C, d)[xm]
+    ax = rx[:, d:]
+    ux = torch.cat([alpha * gx / torch.sqrt(ax + gx * gx), gx * gx], -1)
+    kv.wait(kv.push(torch.cat([(2 * node + 1)[um], xkeys]), torch.cat([ut, ux]).contiguous().view(-1)))
     z = torch.where(label > 0.5, f, -f).clamp(-6, 6)
     return float((torch.log1p(torch.exp(-z)) * tm).sum())

@@ -88,6 +88,45 @@ def cbow_step(server, centers: torch.Tensor, contexts: torch.Tensor, negatives: 
                  loss.data_ptr(), stats.data_ptr() if stats is not None else 0, det)
 
 
+def hs_step(server, centers: torch.Tensor, contexts: torch.Tensor, tree, embed_dim: int, alpha: float,
+            loss: torch.Tensor, stats: Optional[torch.Tensor] = None, deterministic: Optional[bool] = None) -> None:
+    """Fused word2vec hierarchical-softmax step (csrc/cuda/ops_cbow.cu, the CBOW body with Huffman-path targets) on
+    ``server``'s store. Item ``i`` has the syn1 key ``centers[i] = 2 w + 1`` (< 0: the item does nothing) and the syn0
+    keys ``contexts[i]`` ([B, C], -1 = padding; skip-gram passes C = 1). Its targets are the inner nodes on word
+    ``w``'s path in ``tree`` (a :class:`adapm_b200.utils.text.HuffmanTree` on the device; node ``n`` is the row
+    ``2 n + 1``), labelled ``1 - code bit``. The rule is
+    :func:`adapm_b200.models.word2vec.hs_reference_step`'s: ``h`` = mean of the context embeddings, a node with
+    ``|h . node| >= 6`` is skipped (but counted in the loss), one AdaGrad push per (item, node) of ``g h`` and one per
+    context occurrence of ``neu1e = sum_j g_j node_j``. ``loss``: float32[1], accumulated (+=); ``stats``: optional
+    int64[4] accumulated with (local rows, remote rows, slow-path rows, updates). ``4 <= embed_dim <= 336`` and a
+    multiple of 4, ``C <= 32``, ``tree.max_len <= 32``. Centres must be syn1 keys of words in the tree.
+
+    ``deterministic`` as for :func:`cbow_step`: ``None`` picks the deterministic step (8 launches, bit-identical runs)
+    on a single-GPU server and the in-place kernel (one launch) on several GPUs; ``True`` on several GPUs raises."""
+    _i64(centers, "centers"); _i64(contexts, "contexts"); _f32(loss, "loss")
+    if isinstance(embed_dim, bool) or int(embed_dim) != embed_dim or not (
+            4 <= int(embed_dim) <= CBOW_MAX_DIM and int(embed_dim) % 4 == 0):
+        raise ValueError(f"embed_dim must be a multiple of 4 in [4, {CBOW_MAX_DIM}], got {embed_dim}")
+    B = centers.numel()
+    if contexts.dim() != 2 or contexts.shape[0] != B or not 1 <= contexts.shape[1] <= CBOW_MAX_CONTEXTS:
+        raise ValueError(f"contexts must be [B, C] with 1 <= C <= {CBOW_MAX_CONTEXTS}, got {tuple(contexts.shape)}")
+    if not 1 <= int(tree.max_len) <= CBOW_MAX_TARGETS:
+        raise ValueError(f"the tree's paths must be 1 to {CBOW_MAX_TARGETS} nodes long, got max_len {tree.max_len}")
+    V = tree.codes.numel()
+    for t, name, dt, n in ((tree.offsets, "tree.offsets", torch.int64, V + 1), (tree.nodes, "tree.nodes", torch.int32, None),
+                           (tree.codes, "tree.codes", torch.int32, V)):
+        if not (t.device == centers.device and t.dtype == dt and t.is_contiguous() and (n is None or t.numel() == n)):
+            raise TypeError(f"{name} must be a contiguous {dt} tensor on {centers.device}"
+                            + (f" with {n} entries" if n is not None else ""))
+    if stats is not None and not (stats.is_cuda and stats.dtype == torch.int64 and stats.numel() >= 4):
+        raise TypeError("stats must be a CUDA int64 tensor with 4 entries")
+    det = _check_deterministic(server, server.num_servers() == 1 if deterministic is None else deterministic)
+    _C.hs_step(server._impl.backend_handle(), _stream(centers), centers.data_ptr(), contexts.data_ptr(), B,
+               int(contexts.shape[1]), tree.offsets.data_ptr(), tree.nodes.data_ptr(), tree.codes.data_ptr(), V,
+               int(tree.max_len), int(embed_dim), float(alpha), loss.data_ptr(),
+               stats.data_ptr() if stats is not None else 0, det)
+
+
 class SgnsSharedStep:
     """word2vec SGNS with one set of negatives shared by all pairs of a batch, on the tensor cores
     (csrc/cuda/ops_sgns_shared.cu; SURVEY K7's GEMM formulation, an option next to the reference-faithful fused step).

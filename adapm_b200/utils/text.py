@@ -3,6 +3,7 @@ count, min_count pruning, frequent-word subsampling, per-worker file partitionin
 from __future__ import annotations
 
 from collections import Counter
+from dataclasses import dataclass
 from typing import Iterator, List
 
 import numpy as np
@@ -39,6 +40,41 @@ class Vocabulary:
                 w, n = line.rsplit(" ", 1)
                 words.append(w); counts.append(int(n))
         return Vocabulary(words, np.array(counts, dtype=np.int64))
+
+
+@dataclass
+class HuffmanTree:
+    """Huffman coding of a vocabulary for hierarchical softmax (:func:`huffman_tree`), as a CSR: word ``w``'s path is
+    the inner nodes ``nodes[offsets[w]:offsets[w + 1]]`` (int32, root first; node ``n`` is the syn1 row
+    ``2 n + 1``), and bit ``j`` of ``codes[w]`` (int32 holding the uint32 bit pattern) is its code bit at depth ``j``.
+    ``max_len`` is the longest path."""
+    offsets: torch.Tensor
+    nodes: torch.Tensor
+    codes: torch.Tensor
+    max_len: int
+
+    @property
+    def num_words(self) -> int:
+        return self.codes.numel()
+
+    def to(self, device) -> "HuffmanTree":
+        return HuffmanTree(self.offsets.to(device), self.nodes.to(device), self.codes.to(device), self.max_len)
+
+
+def huffman_tree(counts) -> HuffmanTree:
+    """Builds the Huffman tree of word2vec.c's ``CreateBinaryTree`` over ``counts`` (one positive count per word id, in
+    any order), so that paths and codes match word2vec.c and gensim: words ordered by count (descending, ties by word
+    id), the two-queue O(V) merge, inner nodes numbered ``0 .. V-2`` in creation order (the root is ``V-2``), code bit 1
+    for the second-smallest child of each merge. Native (C++); raises ``ValueError`` for fewer than 2 words, a count
+    that is not > 0, or a tree deeper than 32 levels."""
+    from .. import _C
+
+    c = np.asarray(counts, dtype=np.float64)
+    if c.ndim != 1:
+        raise ValueError(f"counts must be one-dimensional, got shape {c.shape}")
+    off, nodes, codes, max_len = _C.huffman_tree(np.ascontiguousarray(c))
+    return HuffmanTree(torch.from_numpy(off), torch.from_numpy(nodes), torch.from_numpy(codes.view(np.int32)),
+                       int(max_len))
 
 
 def read_sentences(path: str, vocab: Vocabulary, rank: int, world: int, subsample: float, rng) -> Iterator[np.ndarray]:
