@@ -36,6 +36,7 @@ CUDA_SOURCES = [
     "cuda/device_mem.cu",
     "cuda/cuda_backend.cu",
     "cuda/fx_accum.cu",
+    "cuda/grouped_push.cu",
 ]
 
 

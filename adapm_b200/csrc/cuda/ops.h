@@ -170,7 +170,7 @@ void gather_dist_topk(CudaBackend& be, cudaStream_t stream, const float* q, cons
 // backward (4 launches, the radix sort counted as one): G_k = grad_scale * sum over the occurrences of k of
 // c_i * grad_out[bag(i)] in position order, then push [-lr G / sqrt(acc + G^2) | G^2] once per distinct key.
 constexpr int kEmbBagMaxDim = 512;
-size_t embedding_bag_workspace_bytes(int64_t nnz, int64_t nbags, int E);
+size_t embedding_bag_workspace_bytes(int64_t nnz, int E);
 void embedding_bag_forward(CudaBackend& be, cudaStream_t stream, const Key* keys, const int64_t* offsets,
                            const float* weights, int64_t nnz, int nbags, int E, bool mean, float* out,
                            unsigned long long* stats);

@@ -171,8 +171,8 @@ void bind(py::module_& m) {
                      ptr<int>(part_c), ptr<float>(out_v), ptr<int64_t>(out_i), ptr<unsigned long long>(stats));
   });
   m.attr("embedding_bag_max_dim") = kEmbBagMaxDim;
-  m.def("embedding_bag_workspace_bytes", [](int64_t nnz, int64_t nbags, int E) {
-    return embedding_bag_workspace_bytes(nnz, nbags, E);
+  m.def("embedding_bag_workspace_bytes", [](int64_t nnz, int E) {
+    return embedding_bag_workspace_bytes(nnz, E);
   });
   m.def("embedding_bag_forward", [](uintptr_t be, uintptr_t stream, uintptr_t keys, uintptr_t offsets, uintptr_t weights,
                                     int64_t nnz, int nbags, int E, bool mean, uintptr_t out, uintptr_t stats) {

@@ -10,18 +10,12 @@
 //   c_(b,f) = [kappa_b + lam w[x_bf], 0, 0, 0 | for f2 != f: kappa_b r V[x_b,f2][f] + lam V[x_bf][f2]; 0 for f2 == f]
 // to the workspace. Every read of another key's row (the partner blocks V[x_b,f2][f]) happens here, before any push
 // of the step: the later launches read only the workspace and each key's own accumulator.
-// Backward (three launches, the radix sort counted as one), the skeleton of ops_embbag.cu's:
-//   1. sort:   cub radix sort of (key, position b * F + f); stable, so every key's occurrences stay in position order
-//   2. tile:   the sorted occurrences are cut into tiles of kTile; one lane group per tile sums each key's run of
-//              contributions in fp32 in position order. A run inside the tile is pushed right away; a run that crosses
-//              a tile boundary leaves one partial sum per tile it touches
-//   3. finish: one warp per run that crosses a boundary adds its partials in tile order and pushes.
+// Backward (three launches, the radix sort counted as one): the sort, tile and finish passes of grouped_push.cuh, which
+// the embedding-bag backward shares, over FfmSource: each key's contributions are added in fp32 in position order.
 // Every distinct key gets one push [-eta G / sqrt(acc + G^2) | G^2] (0 where G == 0: the key's own-field block and the
 // padding) with one fixed sum, so on one GPU two runs of the same step give bit-identical rows and loss. A last
 // one-CTA launch adds the per-example losses in index order.
 #include <cuda_runtime.h>
-
-#include <cub/cub.cuh>
 
 #include "grouped_push.cuh"
 #include "ops.h"
@@ -35,8 +29,6 @@ namespace {
 using namespace grouped;
 
 constexpr int kFwdThreads = 128;
-constexpr int kThreads = 256;
-constexpr int kTile = 32;     // sorted occurrences per lane group in the tile pass
 
 // ------------------------------------------------------------------------------------------------ forward
 // One CTA per example (grid-stride). srow[f * E4 + j]: float4 j of the values of the row of ids[b, f]. Thread f < F
@@ -137,118 +129,39 @@ ffm_fwd_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ ids, const
 }
 
 // ------------------------------------------------------------------------------------------------ backward
-// 2. one group per tile of kTile sorted occurrences. part[t][0]: the partial of the run that was open at the tile's
-// start (it began in an earlier tile); part[t][1]: the partial of a run that begins in the tile and crosses its end.
+// the passes of grouped_push.cuh over FfmSource, which adds row b * F + f of the forward's contributions for the
+// occurrence at position b * F + f, with a plain add, and nothing to a key's sum before the push
+struct FfmSource {
+  const float* contrib;
+  struct Item { int pos; };
+  __device__ __forceinline__ Item load(int pos) const { return {pos}; }
+  __device__ __forceinline__ Item share(const Item& it, unsigned mask, int src, int G) const {
+    return {__shfl_sync(mask, it.pos, src, G)};
+  }
+  __device__ __forceinline__ const float4* row(const Item& it, int E) const {
+    return reinterpret_cast<const float4*>(contrib + (size_t)it.pos * E);
+  }
+  __device__ __forceinline__ void add(float4& a, const float4& x, const Item&) const {
+    a.x += x.x; a.y += x.y; a.z += x.z; a.w += x.w;
+  }
+  template <int VPL>
+  __device__ __forceinline__ void before_push(float4 (&)[VPL]) const {}
+};
+
 template <int VPL>
 __global__ void __launch_bounds__(kThreads, 2)
 ffm_grad_tile_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ sk, const int* __restrict__ spos,
-                     const float* __restrict__ contrib, int nnz, int E, int log_g, float eta, float* __restrict__ part,
-                     unsigned long long* __restrict__ stats) {
-  dev::cta_enter(c);
-  const int lane = threadIdx.x & 31;
-  const int G = 1 << log_g;
-  const int sub = lane & (G - 1);
-  const unsigned mask = group_mask(lane, log_g);
-  const int E4 = E >> 2;
-  const int n_tiles = (nnz + kTile - 1) / kTile;
-  const int groups_per_warp = 32 >> log_g;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  Counts n;
-  for (int wt = warp * groups_per_warp; wt < n_tiles; wt += nwarps * groups_per_warp) {
-    const int t = wt + (lane >> log_g);
-    if (t >= n_tiles) continue;          // (group-uniform; the shuffles below only involve the group)
-    const int lo = t * kTile, hi = min(nnz, lo + kTile);
-    Key cur = sk[lo];
-    bool open_before = lo > 0 && sk[lo - 1] == cur;
-    float4 acc[VPL];
-#pragma unroll
-    for (int v = 0; v < VPL; ++v) acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int p0 = lo; p0 <= hi; p0 += G) {
-      // lane `sub` loads occurrence p0 + sub; position hi is the end of the last run
-      Key kk = -1;
-      int pp = 0;
-      if (p0 + sub < hi) { kk = sk[p0 + sub]; pp = spos[p0 + sub]; }
-      const int cnt = min(G, hi + 1 - p0);
-      for (int u = 0; u < cnt; ++u) {
-        const Key k = (Key)__shfl_sync(mask, (long long)kk, u, G);
-        const int pu = __shfl_sync(mask, pp, u, G);
-        if (k != cur) {                  // the run of `cur` ends here (k == -1: at the tile's end)
-          const bool crosses = k == -1 && hi < nnz && sk[hi] == cur;
-          if (open_before || crosses) {
-            float* dst = part + ((size_t)t * 2 + (open_before ? 0 : 1)) * E;
-#pragma unroll
-            for (int v = 0; v < VPL; ++v) {
-              const int j = sub + G * v;
-              if (j < E4) reinterpret_cast<float4*>(dst)[j] = acc[v];
-            }
-          } else {
-            push_update<VPL>(c, cur, acc, E, sub, G, mask, eta, n, stats);
-          }
-          if (k == -1) break;
-          cur = k;
-          open_before = false;
-#pragma unroll
-          for (int v = 0; v < VPL; ++v) acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-        const float4* cr = reinterpret_cast<const float4*>(contrib + (size_t)pu * E);
-#pragma unroll
-        for (int v = 0; v < VPL; ++v) {
-          const int j = sub + G * v;
-          if (j < E4) {
-            const float4 x = __ldg(cr + j);
-            acc[v].x += x.x; acc[v].y += x.y; acc[v].z += x.z; acc[v].w += x.w;
-          }
-        }
-      }
-    }
-  }
-  __syncwarp();
-  flush_counts(n, stats);
-  dev::cta_exit(c);
+                     const FfmSource src, int nnz, int E, int log_g, float eta,
+                     float* __restrict__ part, unsigned long long* __restrict__ stats) {
+  tile_pass<VPL>(c, sk, spos, src, nnz, E, log_g, eta, part, stats);
 }
 
-// 3. one warp per tile boundary q = i * kTile: if a run crosses q and does not cross q - kTile, the warp owns it: its
-// partials part[i - 1][1], part[i][0], part[i + 1][0], ... are added in tile order, and the key is pushed.
 template <int VPL>
 __global__ void __launch_bounds__(kThreads, 2)
 ffm_grad_finish_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ sk, int nnz, int E, float eta,
-                       const float* __restrict__ part, unsigned long long* __restrict__ stats) {
-  dev::cta_enter(c);
-  const int lane = threadIdx.x & 31;
-  const int E4 = E >> 2;
-  const int n_tiles = (nnz + kTile - 1) / kTile;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  Counts n;
-  for (int i = 1 + warp; i < n_tiles; i += nwarps) {
-    const int q = i * kTile;
-    const Key k = sk[q];
-    if (sk[q - 1] != k || (q - kTile - 1 >= 0 && sk[q - kTile - 1] == k)) continue;   // (warp-uniform)
-    float4 acc[VPL];
-    const float* p0 = part + ((size_t)(i - 1) * 2 + 1) * E;
-#pragma unroll
-    for (int v = 0; v < VPL; ++v) {
-      const int j = lane + 32 * v;
-      acc[v] = j < E4 ? reinterpret_cast<const float4*>(p0)[j] : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    for (int t = i;; ++t) {
-      const float* pt = part + (size_t)t * 2 * E;
-#pragma unroll
-      for (int v = 0; v < VPL; ++v) {
-        const int j = lane + 32 * v;
-        if (j < E4) {
-          const float4 x = reinterpret_cast<const float4*>(pt)[j];
-          acc[v].x += x.x; acc[v].y += x.y; acc[v].z += x.z; acc[v].w += x.w;
-        }
-      }
-      const int e = (t + 1) * kTile;
-      if (e >= nnz || sk[e] != k) break;
-    }
-    push_update<VPL>(c, k, acc, E, lane, 32, 0xffffffffu, eta, n, stats);
-  }
-  flush_counts(n, stats);
-  dev::cta_exit(c);
+                       const float* __restrict__ part, unsigned long long* __restrict__ stats,
+                       const FfmSource src) {
+  finish_pass<VPL>(c, sk, nnz, E, eta, part, stats, src);
 }
 
 // the step's loss: sum_b loss_ex[b] in a fixed order (one CTA; thread t adds b = t, t + 256, ..., then a fixed tree)
@@ -269,33 +182,19 @@ ffm_loss_sum_kernel(const float* __restrict__ loss_ex, int B, float* __restrict_
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-// workspace layout: sorted keys | positions (in, out) | contributions | tile partials | per-example losses | sort scratch
+// workspace layout: the sort's and the passes' arrays (grouped::carve_push) | contributions | per-example losses
 struct Workspace {
-  Key* sk; int* pos_in; int* pos_out; float* contrib; float* part; float* loss_ex; void* sort_tmp; size_t sort_bytes;
-  size_t total;
+  PushWorkspace g; float* contrib; float* loss_ex; size_t total;
 };
 
 Workspace carve(void* base, int B, int F, int k) {
-  Workspace w{};
   const int64_t nnz = (int64_t)B * F;
-  const int E = 4 + F * k;
-  size_t sort_bytes = 0;
-  ADAPM_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned long long*)nullptr,
-                                                   (unsigned long long*)nullptr, (const int*)nullptr, (int*)nullptr,
-                                                   (int)nnz, 0, 64));
-  const size_t n_tiles = (size_t)(nnz + kTile - 1) / kTile;
-  char* p = static_cast<char*>(base);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char* q = p ? p + off : nullptr; off += align_up(bytes); return q; };
-  w.sk = reinterpret_cast<Key*>(take((size_t)nnz * sizeof(Key)));
-  w.pos_in = reinterpret_cast<int*>(take((size_t)nnz * sizeof(int)));
-  w.pos_out = reinterpret_cast<int*>(take((size_t)nnz * sizeof(int)));
-  w.contrib = reinterpret_cast<float*>(take((size_t)nnz * E * sizeof(float)));
-  w.part = reinterpret_cast<float*>(take(n_tiles * 2 * E * sizeof(float)));
-  w.loss_ex = reinterpret_cast<float*>(take((size_t)B * sizeof(float)));
-  w.sort_tmp = take(sort_bytes);
-  w.sort_bytes = sort_bytes;
-  w.total = off;
+  Carve a{static_cast<char*>(base)};
+  Workspace w{};
+  w.g = carve_push(a, nnz, 4 + F * k);
+  w.contrib = a.take<float>((size_t)nnz * (4 + F * k));
+  w.loss_ex = a.take<float>(B);
+  w.total = a.off;
   return w;
 }
 
@@ -345,31 +244,16 @@ void ffm_step(CudaBackend& be, cudaStream_t stream, const Key* ids, const float*
     return;
   }
   be.track_stream(stream);
-  const Ctx& c = be.ctx();
   Workspace w = carve(workspace, B, F, k);
   ADAPM_CHECK(workspace && workspace_bytes >= w.total, "ffm: workspace too small");
   const int n = B * F, E = 4 + F * k;
-  launch_forward(be, stream, ids, labels, B, F, k, r, lam, nullptr, w.loss_ex, w.contrib, w.pos_in, stats);
-  size_t sort_bytes = w.sort_bytes;
-  ADAPM_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(w.sort_tmp, sort_bytes, reinterpret_cast<const unsigned long long*>(ids),
-                                                   reinterpret_cast<unsigned long long*>(w.sk), w.pos_in, w.pos_out, n, 0,
-                                                   key_bits(c.L.num_keys), stream));
-  ADAPM_COUNT_LAUNCH();   // (the sort counts as one launch; cub runs one or more kernels, depending on nnz and the bits)
+  launch_forward(be, stream, ids, labels, B, F, k, r, lam, nullptr, w.loss_ex, w.contrib, w.g.pos_in, stats);
   int log_g, vpl;
   lane_shape(E, &log_g, &vpl);
-  const int n_tiles = (n + kTile - 1) / kTile;
-  const int tiles_per_block = (kThreads / 32) << (5 - log_g);
-  const int tile_blocks = std::max(1, std::min((n_tiles + tiles_per_block - 1) / tiles_per_block, be.num_sms() * 16));
-  const int fin_blocks = std::max(1, std::min((n_tiles + kThreads / 32 - 1) / (kThreads / 32), be.num_sms() * 8));
+  const FfmSource src{w.contrib};
   switch (vpl) {
-#define ADAPM_FFM_BWD(V)                                                                                             \
-  case V:                                                                                                            \
-    ffm_grad_tile_kernel<V><<<tile_blocks, kThreads, 0, stream>>>(c, w.sk, w.pos_out, w.contrib, n, E, log_g, eta,   \
-                                                                  w.part, stats);                                    \
-    ADAPM_COUNT_LAUNCH();                                                                                            \
-    ffm_grad_finish_kernel<V><<<fin_blocks, kThreads, 0, stream>>>(c, w.sk, n, E, eta, w.part, stats);               \
-    ADAPM_COUNT_LAUNCH();                                                                                            \
-    break
+#define ADAPM_FFM_BWD(V) \
+  case V: sort_and_push<ffm_grad_tile_kernel<V>, ffm_grad_finish_kernel<V>>(be, stream, ids, w.g, src, n, E, log_g, eta, stats); break
     ADAPM_FFM_BWD(1); ADAPM_FFM_BWD(2); ADAPM_FFM_BWD(3); ADAPM_FFM_BWD(4); ADAPM_FFM_BWD(5);
 #undef ADAPM_FFM_BWD
     default: ADAPM_CHECK(false, "ffm: bad row length " << E);

@@ -1321,7 +1321,7 @@ class StoreEmbeddingBag:
         keys, offsets, weights = state
         nnz, nbags = keys.numel(), offsets.numel() - 1
         g = grad.to(torch.float32).contiguous()
-        need = _C.embedding_bag_workspace_bytes(nnz, nbags, self.dim)
+        need = _C.embedding_bag_workspace_bytes(nnz, self.dim)
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(max(need, 1), dtype=torch.uint8, device=self.device)
         _C.embedding_bag_backward(self.server._impl.backend_handle(), _stream(g), keys.data_ptr(), offsets.data_ptr(),
