@@ -28,16 +28,14 @@
 //    pushes of a context repeated within one window.
 //  * deterministic (one GPU): cbow_score_kernel, the same body as a score pass that loads only embedding halves and
 //    writes per window h and neu1e ([h rows | neu1e rows]), per (window, target) g_t, and the loss. Each target
-//    contribution is then GatherDesc{g_t, h row} and each context occurrence GatherDesc{1, neu1e row}: grouped by key,
-//    they go through the gather and finish passes of the deterministic SGNS step (sgns_det.cuh), which sum them in
-//    fixed point. Runs give bit-identical rows and loss. The scales are the SGNS step's: 2^23 of summed embedding update
-//    and 2^27 of summed AdaGrad increment per element and step. A word that is a context in n windows of a step adds
-//    n neu1e^2 terms to its AdaGrad half, so n |neu1e|^2 must stay below 2^27 (n = 10 000: |neu1e| < 115).
+//    contribution is then GatherDesc{g_t, h row} and each context occurrence GatherDesc{1, neu1e row}: the SGNS step's
+//    driver det_step (sgns_det.cuh) with the entry source WindowEntries indexes, groups and gathers them and sums them
+//    in fixed point. Runs give bit-identical rows and loss. The scales are the SGNS step's: 2^23 of summed embedding
+//    update and 2^27 of summed AdaGrad increment per element and step. A word that is a context in n windows of a step
+//    adds n neu1e^2 terms to its AdaGrad half, so n |neu1e|^2 must stay below 2^27 (n = 10 000: |neu1e| < 115).
 #include <cuda_runtime.h>
 
 #include <algorithm>
-
-#include <cub/cub.cuh>
 
 #include "fx_accum.cuh"
 #include "ops.h"
@@ -64,8 +62,8 @@ struct CbowScoreOut {
 
 // Where a window's targets come from. n_t(): target slots per window. target(): lane l's target key (-1: none) of a
 // window with centre ckey >= 0, filling the window's Item. label(): target s's label. slow_key(): target s's key again,
-// for the generic path. entry_key() / entry_counts(): entry s < n_t() of the deterministic step's index and group
-// kernels (entry_key also gives the contexts' entries), which skip entries for which entry_counts() is false.
+// for the generic path. entry_key() / entry_counts(): the key of entry s of a window in the deterministic step (the
+// contexts' entries too) and whether it adds anything (WindowEntries).
 //
 // Negative sampling: the centre (label 1) and the negatives (label 0; one equal to the centre is skipped); the gradient
 // saturates at |f| > 6.
@@ -450,20 +448,18 @@ cbow_step_body(const Ctx& c, const Key* __restrict__ centers, const Key* __restr
 template <int VPL>
 __global__ void __maxnreg__(104)
 cbow_step_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
-                 const Key* __restrict__ negatives, int n_win, int nc, int neg, int d, float alpha,
+                 const __grid_constant__ NegTargets ts, int n_win, int nc, int d, float alpha,
                  float* __restrict__ loss_out, unsigned long long* __restrict__ stats) {
-  cbow_step_body<VPL, false>(c, centers, contexts, NegTargets{negatives, neg}, n_win, nc, d, alpha, loss_out, stats,
-                             nullptr, CbowScoreOut{});
+  cbow_step_body<VPL, false>(c, centers, contexts, ts, n_win, nc, d, alpha, loss_out, stats, nullptr, CbowScoreOut{});
 }
 
 template <int VPL>
 __global__ void __maxnreg__(128)
 cbow_score_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers, const Key* __restrict__ contexts,
-                  const Key* __restrict__ negatives, int n_win, int nc, int neg, int d,
+                  const __grid_constant__ NegTargets ts, int n_win, int nc, int d,
                   unsigned long long* __restrict__ stats, unsigned long long* __restrict__ fx_loss,
                   const __grid_constant__ CbowScoreOut so) {
-  cbow_step_body<VPL, true>(c, centers, contexts, NegTargets{negatives, neg}, n_win, nc, d, 0.f, nullptr, stats, fx_loss,
-                            so);
+  cbow_step_body<VPL, true>(c, centers, contexts, ts, n_win, nc, d, 0.f, nullptr, stats, fx_loss, so);
 }
 
 template <int VPL>
@@ -482,218 +478,101 @@ hs_score_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers, 
   cbow_step_body<VPL, true>(c, centers, contexts, ts, n_win, nc, d, 0.f, nullptr, stats, fx_loss, so);
 }
 
-// ---- deterministic one-GPU step: index, score, group by key, gather (sgns_det.cuh)
-// Entry x = w * (n_t + nc) + s of a step: s < n_t target s of window w, else context occurrence s - n_t
-// (Src::entry_key, Src::entry_counts).
-
-// Gives every key of the step's entries a compact id (cidx[key], keys[id]) and looks its row up once (rowp[id]).
-template <class Src>
-__device__ __forceinline__ void det_index_body(const Ctx& c, const Key* __restrict__ centers,
-                                               const Key* __restrict__ contexts, const Src& ts, int n_win, int nc,
-                                               int* __restrict__ cidx, Key* __restrict__ keys,
-                                               float** __restrict__ rowp, unsigned int* __restrict__ count) {
-  const int per = ts.n_t() + nc;
-  const long n = (long)n_win * per;
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
-    const int w = (int)(i / per), s = (int)(i % per);
-    const Key k = ts.entry_key(centers, contexts, nc, w, s);
-    // (the plain load skips the atomic for keys that are already claimed: frequent words appear thousands of times)
-    if (k >= 0 && cidx[k] == -1 && atomicCAS(cidx + k, -1, -2) == -1) {
-      const unsigned r = atomicAdd(count, 1u);
-      keys[r] = k;
-      rowp[r] = home_row(c, k);
-      cidx[k] = (int)r;
-    }
+// ---- the deterministic one-GPU step (det_step, sgns_det.cuh)
+// Entry x = w * (n_t + nc) + s: s < n_t target s of window w (Targets::entry_key, Targets::entry_counts), else context
+// occurrence s - n_t. A target adds g_t * the window's h (vector row w), a context occurrence 1 * the window's neu1e
+// (vector row n_win + w).
+template <class Targets>
+struct WindowEntries {
+  const Key* __restrict__ centers;
+  const Key* __restrict__ contexts;
+  Targets ts;
+  int n_win, nc;
+  float* gs;                     // [n_win x n_t] CbowScoreOut::gs
+  static constexpr int kFirstSlots = 0;
+  static constexpr bool kSinglesInScore = false;
+  __host__ __device__ int items() const { return n_win; }
+  __host__ __device__ int per() const { return ts.n_t() + nc; }
+  __device__ __forceinline__ Key key(int w, int s) const { return ts.entry_key(centers, contexts, nc, w, s); }
+  __device__ __forceinline__ bool counts(int w, int s, Key k) const { return ts.entry_counts(centers, w, s, k); }
+  __device__ __forceinline__ GatherDesc desc(int w, int s, int) const {
+    const int n_t = ts.n_t();
+    if (s >= n_t) return {1.f, n_win + w};
+    const float g = __ldg(gs + (size_t)w * n_t + s);
+    return {g, g == kNoEntry ? 0 : w};
   }
-}
+};
 
-// SCATTER = false: cnt[id] = entries of key id. SCATTER = true: desc / kid of CSR position off[id] + i, i < cnt[id],
-// describe the entries of key id; counts cnt back down to zero. A target adds g_t times the window's h (vector row w),
-// a context occurrence 1 times the window's neu1e (vector row n_win + w).
-template <bool SCATTER, class Src>
-__device__ __forceinline__ void det_group_body(const Key* __restrict__ centers, const Key* __restrict__ contexts,
-                                               const Src& ts, int n_win, int nc, const int* __restrict__ cidx,
-                                               int* __restrict__ cnt, const int* __restrict__ off,
-                                               int* __restrict__ kid, const float* __restrict__ gsb,
-                                               GatherDesc* __restrict__ desc) {
-  const int n_t = ts.n_t(), per = n_t + nc;
-  const long n = (long)n_win * per;
-  for (long x = (long)blockIdx.x * blockDim.x + threadIdx.x; x < n; x += (long)gridDim.x * blockDim.x) {
-    const int w = (int)(x / per), s = (int)(x - (long)w * per);
-    const Key k = ts.entry_key(centers, contexts, nc, w, s);
-    if (!ts.entry_counts(centers, w, s, k)) continue;
-    const int id = __ldg(cidx + k);
-    if (!SCATTER) {
-      atomicAdd(cnt + id, 1);
-    } else {
-      const int q = __ldg(off + id) + atomicSub(cnt + id, 1) - 1;
-      GatherDesc e;
-      if (s < n_t) {
-        e.g = __ldg(gsb + (size_t)w * n_t + s);
-        e.vec = e.g == kNoEntry ? 0 : w;
-      } else {
-        e.g = 1.f;
-        e.vec = n_win + w;
-      }
-      desc[q] = e;
-      kid[q] = id;
-    }
-  }
+__global__ void cbow_det_index_kernel(const __grid_constant__ Ctx c,
+                                      const __grid_constant__ WindowEntries<NegTargets> src, int first_slot, int n_slots,
+                                      int* __restrict__ cidx, Key* __restrict__ keys, float** __restrict__ rowp,
+                                      unsigned int* __restrict__ count) {
+  det_index(c, src, first_slot, n_slots, cidx, keys, rowp, count);
 }
-
-__global__ void cbow_det_index_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers,
-                                      const Key* __restrict__ contexts, const Key* __restrict__ negatives, int n_win,
-                                      int nc, int neg, int* __restrict__ cidx, Key* __restrict__ keys,
-                                      float** __restrict__ rowp, unsigned int* __restrict__ count) {
-  det_index_body(c, centers, contexts, NegTargets{negatives, neg}, n_win, nc, cidx, keys, rowp, count);
-}
-__global__ void hs_det_index_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers,
-                                    const Key* __restrict__ contexts, const __grid_constant__ PathTargets ts, int n_win,
-                                    int nc, int* __restrict__ cidx, Key* __restrict__ keys, float** __restrict__ rowp,
+__global__ void hs_det_index_kernel(const __grid_constant__ Ctx c,
+                                    const __grid_constant__ WindowEntries<PathTargets> src, int first_slot, int n_slots,
+                                    int* __restrict__ cidx, Key* __restrict__ keys, float** __restrict__ rowp,
                                     unsigned int* __restrict__ count) {
-  det_index_body(c, centers, contexts, ts, n_win, nc, cidx, keys, rowp, count);
+  det_index(c, src, first_slot, n_slots, cidx, keys, rowp, count);
 }
 
 template <bool SCATTER>
-__global__ void cbow_det_group_kernel(const Key* __restrict__ centers, const Key* __restrict__ contexts,
-                                      const Key* __restrict__ negatives, int n_win, int nc, int neg,
+__global__ void cbow_det_group_kernel(const __grid_constant__ WindowEntries<NegTargets> src,
                                       const int* __restrict__ cidx, int* __restrict__ cnt, const int* __restrict__ off,
-                                      int* __restrict__ kid, const float* __restrict__ gsb,
-                                      GatherDesc* __restrict__ desc) {
-  det_group_body<SCATTER>(centers, contexts, NegTargets{negatives, neg}, n_win, nc, cidx, cnt, off, kid, gsb, desc);
+                                      int* __restrict__ kid, GatherDesc* __restrict__ desc) {
+  det_group<SCATTER>(src, cidx, cnt, off, kid, desc);
 }
 template <bool SCATTER>
-__global__ void hs_det_group_kernel(const Key* __restrict__ centers, const Key* __restrict__ contexts,
-                                    const __grid_constant__ PathTargets ts, int n_win, int nc,
+__global__ void hs_det_group_kernel(const __grid_constant__ WindowEntries<PathTargets> src,
                                     const int* __restrict__ cidx, int* __restrict__ cnt, const int* __restrict__ off,
-                                    int* __restrict__ kid, const float* __restrict__ gsb,
-                                    GatherDesc* __restrict__ desc) {
-  det_group_body<SCATTER>(centers, contexts, ts, n_win, nc, cidx, cnt, off, kid, gsb, desc);
+                                    int* __restrict__ kid, GatherDesc* __restrict__ desc) {
+  det_group<SCATTER>(src, cidx, cnt, off, kid, desc);
 }
 
-// The kernels of one target source.
-template <class Src> struct StepKernels;
-template <> struct StepKernels<NegTargets> {
-  template <int V> static void step(int blocks, size_t smem, cudaStream_t st, const Ctx& c, const Key* centers,
-                                    const Key* contexts, const NegTargets& ts, int n_win, int nc, int d, float alpha,
-                                    float* loss_out, unsigned long long* stats) {
-    set_max_dynamic_smem<cbow_step_kernel<V>>(110 * 1024);
-    cbow_step_kernel<V><<<blocks, kThreads, smem, st>>>(c, centers, contexts, ts.negatives, n_win, nc, ts.neg, d, alpha,
-                                                        loss_out, stats);
-  }
-  template <int V> static void score(int blocks, size_t smem, cudaStream_t st, const Ctx& c, const Key* centers,
-                                     const Key* contexts, const NegTargets& ts, int n_win, int nc, int d,
-                                     unsigned long long* stats, unsigned long long* fx_loss, const CbowScoreOut& so) {
-    set_max_dynamic_smem<cbow_score_kernel<V>>(110 * 1024);
-    cbow_score_kernel<V><<<blocks, kThreads, smem, st>>>(c, centers, contexts, ts.negatives, n_win, nc, ts.neg, d, stats,
-                                                         fx_loss, so);
-  }
-  static void index(int blocks, cudaStream_t st, const Ctx& c, const Key* centers, const Key* contexts,
-                    const NegTargets& ts, int n_win, int nc, int* cidx, Key* keys, float** rowp, unsigned int* count) {
-    cbow_det_index_kernel<<<blocks, 256, 0, st>>>(c, centers, contexts, ts.negatives, n_win, nc, ts.neg, cidx, keys,
-                                                  rowp, count);
-  }
-  template <bool SCATTER> static void group(int blocks, cudaStream_t st, const Key* centers, const Key* contexts,
-                                            const NegTargets& ts, int n_win, int nc, const int* cidx, int* cnt,
-                                            const int* off, int* kid, const float* gsb, GatherDesc* desc) {
-    cbow_det_group_kernel<SCATTER><<<blocks, 256, 0, st>>>(centers, contexts, ts.negatives, n_win, nc, ts.neg, cidx, cnt,
-                                                           off, kid, gsb, desc);
-  }
+// The kernels of a target source.
+template <class Targets> struct Kernels;
+template <> struct Kernels<NegTargets> {
+  template <int V> static constexpr auto step = cbow_step_kernel<V>;
+  template <int V> static constexpr auto score = cbow_score_kernel<V>;
+  static constexpr auto index = cbow_det_index_kernel;
+  template <bool SCATTER> static constexpr auto group = cbow_det_group_kernel<SCATTER>;
 };
-template <> struct StepKernels<PathTargets> {
-  template <int V> static void step(int blocks, size_t smem, cudaStream_t st, const Ctx& c, const Key* centers,
-                                    const Key* contexts, const PathTargets& ts, int n_win, int nc, int d, float alpha,
-                                    float* loss_out, unsigned long long* stats) {
-    set_max_dynamic_smem<hs_step_kernel<V>>(110 * 1024);
-    hs_step_kernel<V><<<blocks, kThreads, smem, st>>>(c, centers, contexts, ts, n_win, nc, d, alpha, loss_out, stats);
-  }
-  template <int V> static void score(int blocks, size_t smem, cudaStream_t st, const Ctx& c, const Key* centers,
-                                     const Key* contexts, const PathTargets& ts, int n_win, int nc, int d,
-                                     unsigned long long* stats, unsigned long long* fx_loss, const CbowScoreOut& so) {
-    set_max_dynamic_smem<hs_score_kernel<V>>(110 * 1024);
-    hs_score_kernel<V><<<blocks, kThreads, smem, st>>>(c, centers, contexts, ts, n_win, nc, d, stats, fx_loss, so);
-  }
-  static void index(int blocks, cudaStream_t st, const Ctx& c, const Key* centers, const Key* contexts,
-                    const PathTargets& ts, int n_win, int nc, int* cidx, Key* keys, float** rowp, unsigned int* count) {
-    hs_det_index_kernel<<<blocks, 256, 0, st>>>(c, centers, contexts, ts, n_win, nc, cidx, keys, rowp, count);
-  }
-  template <bool SCATTER> static void group(int blocks, cudaStream_t st, const Key* centers, const Key* contexts,
-                                            const PathTargets& ts, int n_win, int nc, const int* cidx, int* cnt,
-                                            const int* off, int* kid, const float* gsb, GatherDesc* desc) {
-    hs_det_group_kernel<SCATTER><<<blocks, 256, 0, st>>>(centers, contexts, ts, n_win, nc, cidx, cnt, off, kid, gsb,
-                                                         desc);
-  }
+template <> struct Kernels<PathTargets> {
+  template <int V> static constexpr auto step = hs_step_kernel<V>;
+  template <int V> static constexpr auto score = hs_score_kernel<V>;
+  static constexpr auto index = hs_det_index_kernel;
+  template <bool SCATTER> static constexpr auto group = hs_det_group_kernel<SCATTER>;
 };
-
-template <class Src>
-void cbow_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, const Src& ts,
-                   int n_win, int nc, int d, float alpha, float* loss_out, unsigned long long* stats, int vpl,
-                   int score_blocks, size_t smem) {
-  using K = StepKernels<Src>;
-  const Ctx& c = be.ctx();
-  const int n_t = ts.n_t();
-  const int n_entries = n_win * (n_t + nc);
-  const int n_ids = (int)std::min<size_t>((size_t)n_entries, (size_t)c.L.num_keys);   // bound on the distinct keys
-  const int n_ranges = (n_entries + kGatherRange - 1) / kGatherRange;
-  CudaBackend::FxScratch& fx = be.fx_scratch(0, (size_t)n_ids, 0);
-  CbowScoreOut so;
-  so.gs = static_cast<float*>(be.step_buffer(kBufGs, (size_t)n_win * n_t * sizeof(float)));
-  so.vecs = static_cast<float*>(be.step_buffer(kBufVec, (size_t)2 * n_win * d * sizeof(float)));
-  int* cnt = static_cast<int*>(be.step_buffer(kBufCnt, ((size_t)n_ids + 1) * sizeof(int)));    // zero between steps
-  int* off = static_cast<int*>(be.step_buffer(kBufOff, ((size_t)n_ids + 1) * sizeof(int)));
-  GatherDesc* desc = static_cast<GatherDesc*>(be.step_buffer(kBufDesc, (size_t)n_entries * sizeof(GatherDesc)));
-  int* kid = static_cast<int*>(be.step_buffer(kBufKid, (size_t)n_entries * sizeof(int)));
-  long long* part = static_cast<long long*>(                                            // zero between steps
-      be.step_buffer(kBufPart, ((size_t)n_ranges + 1) * 2 * d * sizeof(long long)));
-  float** rowp = static_cast<float**>(be.step_buffer(kBufRowp, (size_t)n_ids * sizeof(float*)));
-  size_t scan_bytes = 0;
-  ADAPM_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, cnt, off, n_ids + 1, stream));
-  void* scan_tmp = be.step_buffer(kBufScan, scan_bytes);
-
-  const int grid_n = be.num_sms() * 8;
-  auto blocks_for = [&](long n) { return (int)std::max<long>(1, std::min<long>((n + 255) / 256, grid_n)); };
-  ADAPM_CUDA_CHECK(cudaMemsetAsync(fx.count, 0, 2 * sizeof(unsigned int), stream));
-  K::index(blocks_for(n_entries), stream, c, centers, contexts, ts, n_win, nc, fx.cidx, fx.keys, rowp, fx.count);
-  ADAPM_COUNT_LAUNCH();
-  switch (vpl) {
-    case 1: K::template score<1>(score_blocks, smem, stream, c, centers, contexts, ts, n_win, nc, d, stats, fx.loss, so); break;
-    case 2: K::template score<2>(score_blocks, smem, stream, c, centers, contexts, ts, n_win, nc, d, stats, fx.loss, so); break;
-    default: K::template score<3>(score_blocks, smem, stream, c, centers, contexts, ts, n_win, nc, d, stats, fx.loss, so); break;
-  }
-  ADAPM_COUNT_LAUNCH();
-  K::template group<false>(blocks_for(n_entries), stream, centers, contexts, ts, n_win, nc, fx.cidx, cnt, off, kid, so.gs,
-                           desc);
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, cnt, off, n_ids + 1, stream));
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_COUNT_LAUNCH();   // (the scan is two kernels)
-  K::template group<true>(blocks_for(n_entries), stream, centers, contexts, ts, n_win, nc, fx.cidx, cnt, off, kid, so.gs,
-                          desc);
-  ADAPM_COUNT_LAUNCH();
-  det_gather_finish(be, stream, vpl, rowp, off, n_ids, kid, desc, so.vecs, d, alpha, part, n_ranges,
-                    blocks_for(n_entries), fx, loss_out);
-  ADAPM_CUDA_CHECK(cudaGetLastError());
-}
 
 // One step of either target source: the deterministic step or one in-place launch. The caller checks the arguments.
-template <class Src>
-void run_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, const Src& ts, int n_win,
-              int nc, int d, float alpha, float* loss_out, unsigned long long* stats, bool deterministic) {
+template <class Targets>
+void run_step(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, const Targets& ts,
+              int n_win, int nc, int d, float alpha, float* loss_out, unsigned long long* stats, bool deterministic) {
+  using K = Kernels<Targets>;
+  const Ctx& c = be.ctx();
   const int vpl = (d / 4 + 31) / 32;
   const size_t buf_floats = ((size_t)2 * d + 31) & ~(size_t)31;
   const size_t smem = (size_t)kWarps * (RING + 1) * buf_floats * sizeof(float) + 128;   // <= 110 KB: 2 blocks per SM
   const int blocks = std::min((n_win + kWarps - 1) / kWarps, be.num_sms() * 12);
   if (deterministic) {
-    cbow_step_det(be, stream, centers, contexts, ts, n_win, nc, d, alpha, loss_out, stats, vpl, blocks, smem);
+    const WindowEntries<Targets> src{centers, contexts, ts, n_win, nc, nullptr};
+    det_step<K::index, K::template group<false>, K::template group<true>>(
+        be, stream, src, (size_t)2 * n_win, d, alpha, vpl, loss_out,
+        [&](float* gs, float* vecs, const int*, CudaBackend::FxScratch& fx) {
+          by_vpl(vpl, [&](auto v) {
+            constexpr auto score = K::template score<decltype(v)::value>;
+            set_max_dynamic_smem<score>(110 * 1024);
+            score<<<blocks, kThreads, smem, stream>>>(c, centers, contexts, ts, n_win, nc, d, stats, fx.loss,
+                                                      CbowScoreOut{vecs, gs});
+          });
+        });
     return;
   }
-  using K = StepKernels<Src>;
-  const Ctx& c = be.ctx();
-  switch (vpl) {
-    case 1: K::template step<1>(blocks, smem, stream, c, centers, contexts, ts, n_win, nc, d, alpha, loss_out, stats); break;
-    case 2: K::template step<2>(blocks, smem, stream, c, centers, contexts, ts, n_win, nc, d, alpha, loss_out, stats); break;
-    default: K::template step<3>(blocks, smem, stream, c, centers, contexts, ts, n_win, nc, d, alpha, loss_out, stats); break;
-  }
+  by_vpl(vpl, [&](auto v) {
+    constexpr auto step = K::template step<decltype(v)::value>;
+    set_max_dynamic_smem<step>(110 * 1024);
+    step<<<blocks, kThreads, smem, stream>>>(c, centers, contexts, ts, n_win, nc, d, alpha, loss_out, stats);
+  });
   ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cudaGetLastError());
 }

@@ -9,8 +9,9 @@
 //   whole warp  : mbarrier.try_wait, LDS.128 the row from shared memory, dot / sigmoid / AdaGrad,
 //                 the update overwrites the consumed ring slot
 //   lane 0      : cp.reduce.async.bulk (UBLKRED) of that slot into the row's home (local HBM or NVLink peer)
-// The deterministic one-GPU step (sgns_step_det) runs the same body as a score pass that loads the targets' embedding
-// halves, then groups the step's contributions by key and lets one warp per row gather them as fixed-point integer sums.
+// The deterministic one-GPU step (det_step in sgns_det.cuh, with the entry source SgnsEntries) runs the same body as a
+// score pass that loads the targets' embedding halves, then groups the step's contributions by key and lets one warp
+// per row gather them as fixed-point integer sums.
 // A key with a single entry in the step (two thirds of the keys at the benchmark's shape) skips the grouping: the score
 // pass loads its whole row and writes the update back itself, with the gather pass's fixed-point arithmetic.
 // The TMA engine reads rows that live on a peer GPU through their NVLink-mapped addresses as well;
@@ -418,150 +419,44 @@ sgns_score_tma_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ cen
                                 fx_loss, so);
 }
 
-// ---- deterministic one-GPU step: index, score, group by key, gather
-// The contributions of a step are grouped by key (CSR: off / list / kid), so that each row is updated by the one warp
-// that owns it and no accumulator per key and element is needed. Integer sums do not depend on the order of their
-// terms, so the grouping may differ from run to run and the rows and loss do not.
-
-__device__ __forceinline__ Key entry_key(const Key* centers, const Key* contexts, const Key* negatives, int neg, int p,
-                                         int s) {
-  return s == 0 ? centers[p] : (s == 1 ? contexts[p] : negatives[(size_t)p * neg + (s - 2)]);
-}
-// a negative equal to the pair's context adds nothing (the step skips it); neither does a negative key
-__device__ __forceinline__ bool entry_counts(const Key* contexts, int p, int s, Key k) {
-  return k >= 0 && !(s >= 2 && k == contexts[p]);
-}
-
-// Gives every key of slots [first_slot, first_slot + n_slots) of each pair a compact id (cidx[key], keys[id]) and
-// looks its row up once (rowp[id]). Run over the centers first, so that the centers' ids are 0 .. distinct centers - 1.
-__global__ void sgns_det_index_kernel(const __grid_constant__ Ctx c, const Key* __restrict__ centers,
-                                      const Key* __restrict__ contexts, const Key* __restrict__ negatives, int n_pairs,
-                                      int neg, int first_slot, int n_slots, int* __restrict__ cidx,
-                                      Key* __restrict__ keys, float** __restrict__ rowp,
-                                      unsigned int* __restrict__ count) {
-  const long n = (long)n_pairs * n_slots;
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
-    const int p = (int)(i / n_slots), s = first_slot + (int)(i % n_slots);
-    const Key k = entry_key(centers, contexts, negatives, neg, p, s);
-    // (the plain load skips the atomic for keys that are already claimed: hot keys appear thousands of times)
-    if (k >= 0 && cidx[k] == -1 && atomicCAS(cidx + k, -1, -2) == -1) {
-      const unsigned r = atomicAdd(count, 1u);
-      keys[r] = k;
-      rowp[r] = home_row(c, k);
-      cidx[k] = (int)r;
-    }
+// ---- the deterministic one-GPU step (det_step, sgns_det.cuh)
+// Entry x = p * (neg + 2) + s: s = 0 the center of pair p, s = 1 its context, s >= 2 negative s - 2. The center adds
+// 1 * the pair's center gradient g0 (vector row p); a target adds gs * the center's start-of-step embedding (vector row
+// n_pairs + the center's compact id).
+struct SgnsEntries {
+  const Key* __restrict__ centers;
+  const Key* __restrict__ contexts;
+  const Key* __restrict__ negatives;
+  int n_pairs, neg;
+  const int* __restrict__ pcid;  // [n_pairs] the compact id of the pair's center (ScoreOut::pcid)
+  float* gs;                     // [n_pairs x (neg + 2)] gs of each target; 0 or kNoEntry: whether the center adds g0
+  static constexpr int kFirstSlots = 1;          // the centers first: their compact ids are the rows of ScoreOut::snap
+  static constexpr bool kSinglesInScore = true;
+  __host__ __device__ int items() const { return n_pairs; }
+  __host__ __device__ int per() const { return neg + 2; }
+  __device__ __forceinline__ Key key(int p, int s) const {
+    return s == 0 ? centers[p] : (s == 1 ? contexts[p] : negatives[(size_t)p * neg + (s - 2)]);
   }
-}
-
-// SCATTER = false: cnt[id] = entries of key id. SCATTER = true: desc / kid of CSR position off[id] + i, i < cnt[id],
-// describe the entries of key id (from the score pass's gs and pcid); counts cnt back down to zero. A key with one entry
-// has no CSR positions (the score pass applied it): its count is cleared.
-template <bool SCATTER>
-__global__ void sgns_det_group_kernel(const Key* __restrict__ centers, const Key* __restrict__ contexts,
-                                      const Key* __restrict__ negatives, int n_pairs, int neg,
-                                      const int* __restrict__ cidx, int* __restrict__ cnt, const int* __restrict__ off,
-                                      int* __restrict__ kid, const float* __restrict__ gsb,
-                                      const int* __restrict__ pcid, GatherDesc* __restrict__ desc) {
-  const int n = n_pairs * (neg + 2);
-  for (int x = blockIdx.x * blockDim.x + threadIdx.x; x < n; x += gridDim.x * blockDim.x) {
-    const int p = x / (neg + 2), s = x - p * (neg + 2);
-    const Key k = entry_key(centers, contexts, negatives, neg, p, s);
-    if (!entry_counts(contexts, p, s, k)) continue;
-    const int id = __ldg(cidx + k);
-    if (!SCATTER) {
-      atomicAdd(cnt + id, 1);
-    } else {
-      const int q0 = __ldg(off + id);
-      if (__ldg(off + id + 1) == q0) {
-        cnt[id] = 0;
-        continue;
-      }
-      const int q = q0 + atomicSub(cnt + id, 1) - 1;
-      const float gx = __ldg(gsb + x);
-      GatherDesc e;
-      if (s == 0) {
-        e.g = gx == kNoEntry ? kNoEntry : 1.f;
-        e.vec = p;
-      } else {
-        e.g = gx;
-        e.vec = gx == kNoEntry ? 0 : n_pairs + __ldg(pcid + p);
-      }
-      desc[q] = e;
-      kid[q] = id;
-    }
+  // a negative equal to the pair's context adds nothing (the step skips it); neither does a negative key
+  __device__ __forceinline__ bool counts(int p, int s, Key k) const { return k >= 0 && !(s >= 2 && k == contexts[p]); }
+  __device__ __forceinline__ GatherDesc desc(int p, int s, int x) const {
+    const float g = __ldg(gs + x);
+    if (s == 0) return {g == kNoEntry ? kNoEntry : 1.f, p};
+    return {g, g == kNoEntry ? 0 : n_pairs + __ldg(pcid + p)};
   }
-}
-
-// CSR positions of a key with c entries: none for a key with one entry (the score pass applies it)
-struct GatheredEntries {
-  __host__ __device__ int operator()(int c) const { return c == 1 ? 0 : c; }
 };
 
-// The deterministic one-GPU step: index -> count, scan -> score -> scatter -> gather -> finish, all on `stream`.
-void sgns_step_det(CudaBackend& be, cudaStream_t stream, const Key* centers, const Key* contexts, const Key* negatives,
-                   int n_pairs, int neg, int d, float alpha, float* loss_out, unsigned long long* stats, int vpl,
-                   int score_blocks, size_t score_smem) {
-  const Ctx& c = be.ctx();
-  const int n_entries = n_pairs * (neg + 2);
-  const size_t num_keys = (size_t)c.L.num_keys;
-  const int n_ids = (int)std::min<size_t>((size_t)n_entries, num_keys);          // bound on the step's distinct keys
-  const size_t n_centers = std::min<size_t>((size_t)n_pairs, num_keys);
-  const int n_ranges = (n_entries + kGatherRange - 1) / kGatherRange;
-  CudaBackend::FxScratch& fx = be.fx_scratch(0, (size_t)n_ids, 0);
-  float* gsb = static_cast<float*>(be.step_buffer(kBufGs, (size_t)n_entries * sizeof(float)));
-  ScoreOut so;
-  // one vector buffer: g0 of every pair, then the centers' snapshots (GatherDesc::vec is a row of it)
-  so.g0 = static_cast<float*>(be.step_buffer(kBufVec, ((size_t)n_pairs + n_centers) * d * sizeof(float)));
-  so.snap = so.g0 + (size_t)n_pairs * d;
-  so.pcid = static_cast<int*>(be.step_buffer(kBufPcid, (size_t)n_pairs * sizeof(int)));
-  int* cnt = static_cast<int*>(be.step_buffer(kBufCnt, ((size_t)n_ids + 1) * sizeof(int)));    // zero between steps
-  int* off = static_cast<int*>(be.step_buffer(kBufOff, ((size_t)n_ids + 1) * sizeof(int)));
-  GatherDesc* desc = static_cast<GatherDesc*>(be.step_buffer(kBufDesc, (size_t)n_entries * sizeof(GatherDesc)));
-  int* kid = static_cast<int*>(be.step_buffer(kBufKid, (size_t)n_entries * sizeof(int)));
-  long long* part = static_cast<long long*>(                                            // zero between steps
-      be.step_buffer(kBufPart, ((size_t)n_ranges + 1) * 2 * d * sizeof(long long)));
-  float** rowp = static_cast<float**>(be.step_buffer(kBufRowp, (size_t)n_ids * sizeof(float*)));
-  so.cnt = cnt;
-  const auto gathered = thrust::make_transform_iterator(static_cast<const int*>(cnt), GatheredEntries{});
-  size_t scan_bytes = 0;
-  ADAPM_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, gathered, off, n_ids + 1, stream));
-  void* scan_tmp = be.step_buffer(kBufScan, scan_bytes);
+__global__ void sgns_det_index_kernel(const __grid_constant__ Ctx c, const __grid_constant__ SgnsEntries src,
+                                      int first_slot, int n_slots, int* __restrict__ cidx, Key* __restrict__ keys,
+                                      float** __restrict__ rowp, unsigned int* __restrict__ count) {
+  det_index(c, src, first_slot, n_slots, cidx, keys, rowp, count);
+}
 
-  const int grid_n = be.num_sms() * 8;
-  auto blocks_for = [&](long n) { return (int)std::max<long>(1, std::min<long>((n + 255) / 256, grid_n)); };
-  ADAPM_CUDA_CHECK(cudaMemsetAsync(fx.count, 0, 2 * sizeof(unsigned int), stream));
-  sgns_det_index_kernel<<<blocks_for(n_pairs), 256, 0, stream>>>(c, centers, contexts, negatives, n_pairs, neg, 0, 1,
-                                                                  fx.cidx, fx.keys, rowp, fx.count);
-  ADAPM_COUNT_LAUNCH();
-  sgns_det_index_kernel<<<blocks_for((long)n_pairs * (neg + 1)), 256, 0, stream>>>(
-      c, centers, contexts, negatives, n_pairs, neg, 1, neg + 1, fx.cidx, fx.keys, rowp, fx.count);
-  ADAPM_COUNT_LAUNCH();
-  sgns_det_group_kernel<false><<<blocks_for(n_entries), 256, 0, stream>>>(centers, contexts, negatives, n_pairs, neg,
-                                                                           fx.cidx, cnt, off, kid, gsb, so.pcid, desc);
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, gathered, off, n_ids + 1, stream));
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_COUNT_LAUNCH();   // (the scan is two kernels)
-#define ADAPM_LAUNCH_SCORE(V)                                                                                  \
-  do {                                                                                                         \
-    set_max_dynamic_smem<sgns_score_tma_kernel<V>>(110 * 1024);                                                \
-    sgns_score_tma_kernel<V><<<score_blocks, kThreads, score_smem, stream>>>(c, centers, contexts, negatives,  \
-                                                                             n_pairs, neg, d, alpha, stats, fx.cidx, \
-                                                                             gsb, fx.loss, so);                  \
-  } while (0)
-  switch (vpl) {
-    case 1: ADAPM_LAUNCH_SCORE(1); break;
-    case 2: ADAPM_LAUNCH_SCORE(2); break;
-    default: ADAPM_LAUNCH_SCORE(3); break;
-  }
-#undef ADAPM_LAUNCH_SCORE
-  ADAPM_COUNT_LAUNCH();
-  sgns_det_group_kernel<true><<<blocks_for(n_entries), 256, 0, stream>>>(centers, contexts, negatives, n_pairs, neg,
-                                                                          fx.cidx, cnt, off, kid, gsb, so.pcid, desc);
-  ADAPM_COUNT_LAUNCH();
-  det_gather_finish(be, stream, vpl, rowp, off, n_ids, kid, desc, so.g0, d, alpha, part, n_ranges, blocks_for(n_entries),
-                    fx, loss_out);
-  ADAPM_CUDA_CHECK(cudaGetLastError());
+template <bool SCATTER>
+__global__ void sgns_det_group_kernel(const __grid_constant__ SgnsEntries src, const int* __restrict__ cidx,
+                                      int* __restrict__ cnt, const int* __restrict__ off, int* __restrict__ kid,
+                                      GatherDesc* __restrict__ desc) {
+  det_group<SCATTER>(src, cidx, cnt, off, kid, desc);
 }
 
 }  // namespace
@@ -587,14 +482,28 @@ bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   // warp's LSU slots stay free for the sync round's kernels. (A software-pipelined target loop - score of target t+1
   // during the update of target t - was measured too: no gain at 128 registers, -5 % at 104: the kernel is not bound by
   // the per-warp dependency chain.)
-  // One GPU: deterministic step (score pass + updates grouped by key, see sgns_step_det), so that the same inputs give
+  // One GPU: deterministic step (score pass + updates grouped by key, det_step), so that the same inputs give
   // the same rows and loss in every run; ADAPM_SGNS_DETERMINISTIC=0 selects in-place (Hogwild) updates. Several GPUs:
   // rows move between ranks during the step and are updated in place.
   static const bool det_env = [] { const char* e = getenv("ADAPM_SGNS_DETERMINISTIC"); return !e || atoi(e) != 0; }();
   const long n_src = (long)n_pairs * (neg + 2);
   ADAPM_CHECK(n_src < (1L << 29), "sgns_step: too many keys in one step");   // (entry or key id << 2 fits an int)
   if (det_env && c.L.world == 1) {
-    sgns_step_det(be, stream, centers, contexts, negatives, n_pairs, neg, d, alpha, loss_out, stats, vpl, blocks, smem);
+    int* pcid = static_cast<int*>(be.step_buffer(kBufPcid, (size_t)n_pairs * sizeof(int)));
+    const SgnsEntries src{centers, contexts, negatives, n_pairs, neg, pcid, nullptr};
+    // vector buffer: g0 of every pair, then the snapshots of the distinct centers
+    const size_t n_centers = std::min<size_t>((size_t)n_pairs, (size_t)c.L.num_keys);
+    det_step<sgns_det_index_kernel, sgns_det_group_kernel<false>, sgns_det_group_kernel<true>>(
+        be, stream, src, n_pairs + n_centers, d, alpha, vpl, loss_out,
+        [&](float* gs, float* vecs, const int* cnt, CudaBackend::FxScratch& fx) {
+          const ScoreOut so{vecs, vecs + (size_t)n_pairs * d, pcid, cnt};
+          by_vpl(vpl, [&](auto v) {
+            constexpr auto score = sgns_score_tma_kernel<decltype(v)::value>;
+            set_max_dynamic_smem<score>(110 * 1024);
+            score<<<blocks, kThreads, smem, stream>>>(c, centers, contexts, negatives, n_pairs, neg, d, alpha, stats,
+                                                      fx.cidx, gs, fx.loss, so);
+          });
+        });
     return true;
   }
 #define ADAPM_LAUNCH_TMA2(V, R)                                                                                 \
@@ -616,6 +525,19 @@ bool sgns_step_tma(CudaBackend& be, cudaStream_t stream, const Key* centers, con
   ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cudaGetLastError());
   return true;
+}
+
+namespace {
+// CSR positions of a key with c entries
+struct GatheredEntries {
+  bool singles_in_score;
+  __host__ __device__ int operator()(int c) const { return singles_in_score && c == 1 ? 0 : c; }
+};
+}  // namespace
+
+void det_scan(void* tmp, size_t& bytes, const int* cnt, int* off, int n, bool singles_in_score, cudaStream_t stream) {
+  const auto gathered = thrust::make_transform_iterator(cnt, GatheredEntries{singles_in_score});
+  ADAPM_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(tmp, bytes, gathered, off, n, stream));
 }
 
 }  // namespace cudaops

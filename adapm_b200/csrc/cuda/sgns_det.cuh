@@ -1,10 +1,16 @@
-// Shared pieces of the deterministic one-GPU word2vec steps (SGNS: ops_sgns_tma.cu, CBOW: ops_cbow.cu) and of their
-// TMA rings: mbarrier and bulk-copy helpers, the fixed-point scales, and the gather and finish passes that apply a step's
-// contributions grouped by key. A step's score pass describes every contribution to a row as GatherDesc{g, vec}: the
-// row gains AdaGrad(g * vecs[vec]) in fixed point against its start-of-step accumulator. (The SGNS score pass applies a
-// row with a single contribution itself, with the same arithmetic: fx_apply_one.)
+// The deterministic one-GPU word2vec steps (SGNS: ops_sgns_tma.cu; CBOW and hierarchical softmax: ops_cbow.cu) and the
+// TMA rings of their kernels: mbarrier and bulk-copy helpers, the fixed-point scales, and one implementation of every
+// pass but the score pass. det_step runs a step: det_index gives each key a compact id, the op's score pass reads
+// start-of-step rows, det_group counts each key's entries and (after a scan) scatters them into a CSR grouped by key,
+// and the gather and finish passes apply them. The passes are generic over an entry source, which says what each entry
+// of the step is. The score pass describes every contribution to a row as GatherDesc{g, vec}: the row gains
+// AdaGrad(g * vecs[vec]) in fixed point against its start-of-step accumulator. (The SGNS score pass applies a row with
+// a single contribution itself, with the same arithmetic: fx_apply_one.)
 #pragma once
 #include <cuda_runtime.h>
+
+#include <algorithm>
+#include <type_traits>
 
 #include "cuda_backend.h"
 #include "fx_accum.cuh"
@@ -12,6 +18,11 @@
 
 namespace adapm {
 namespace cudaops {
+
+// off[0 .. n) = exclusive sum of the CSR positions of keys with cnt[0 .. n) entries (none for a key with one entry if
+// singles_in_score); tmp null: sets bytes. Defined in ops_sgns_tma.cu, so that the extension carries one copy of cub's
+// scan for all the steps.
+void det_scan(void* tmp, size_t& bytes, const int* cnt, int* off, int n, bool singles_in_score, cudaStream_t stream);
 
 namespace {
 
@@ -71,9 +82,8 @@ __device__ __forceinline__ void mark_pushed(void* mark, int bits) {
 constexpr float kFxEmb = 1099511627776.f;     // 2^40
 constexpr float kFxAda = 68719476736.f;       // 2^36
 constexpr float kFxLoss = 4294967296.f;       // 2^32
-// Entry x = p * (neg + 2) + s of a step: s = 0 the center of pair p, s = 1 its context, s >= 2 negative s - 2.
-// gs[x] of an entry that adds nothing (negative == context, generic-path target or center, skipped pair). A real gs is
-// in [-1, 1] or NaN; 0 is a real gs (and a center entry's "valid" mark), so it cannot be the marker.
+// The g a score pass writes for an entry that adds nothing (a skipped target, a generic-path row, a skipped item). A
+// real g is in [-1, 1] or NaN; 0 is a real g (and an SGNS center entry's "valid" mark), so it cannot be the marker.
 constexpr float kNoEntry = __builtin_huge_valf();
 
 // the key's row in this GPU's store (one GPU: rows do not move during a step)
@@ -82,9 +92,8 @@ __device__ __forceinline__ float* home_row(const Ctx& c, Key k) {
   return slot >= 0 ? row_ptr<float>(c, c.rank, class_of_key(c, k), (uint32_t)slot) : nullptr;
 }
 
-// What one contribution (CSR position) adds to its key's row: g times vector vec of the step's vector buffer, which holds
-// the pairs' center gradients g0 (rows 0 .. n_pairs - 1) followed by the centers' start-of-step embeddings (rows
-// n_pairs + compact id). g is 1 for a center (its gradient is g0 itself), gs for a target, kNoEntry for nothing.
+// What one contribution (CSR position) adds to its key's row: g times row vec of the step's vector buffer, which the
+// score pass fills (the entry source's desc() says which row); g = kNoEntry: nothing.
 struct alignas(8) GatherDesc {
   float g;
   int vec;
@@ -378,6 +387,140 @@ inline void det_gather_finish(CudaBackend& be, cudaStream_t stream, int vpl, flo
   sgns_det_finish_kernel<<<finish_blocks, 256, 0, stream>>>(c, fx.keys, rowp, off, n_ids, kid, d, part, fx.cidx,
                                                             fx.count, fx.loss, loss_out);
   ADAPM_COUNT_LAUNCH();
+}
+
+// ---- Before the gather: the step's entries are grouped by key (CSR: off / kid / desc), so that one warp owns each row
+// and no accumulator per key and element is needed. Integer sums do not depend on the order of their terms, so the
+// grouping may differ from run to run and the rows and loss do not. An entry source (a struct passed by value to the
+// index and group kernels) says what entry x = i * per() + s of item i of the step is:
+//   int items() const, int per() const        items of the step, entries per item
+//   Key key(int i, int s) const                the entry's key (< 0: none)
+//   bool counts(int i, int s, Key k) const     whether the entry adds anything to row k
+//   GatherDesc desc(int i, int s, int x) const what it adds, from what the score pass wrote
+//   float* gs                                  the score pass's g of each entry (det_step carves it, at most one per
+//                                              entry; the layout is the source's)
+//   static constexpr int kFirstSlots           slots [0, kFirstSlots) of every item are indexed first, so that their
+//                                              keys get the compact ids 0 .. distinct - 1
+//   static constexpr bool kSinglesInScore      the score pass applies a key with one entry itself: the key gets no CSR
+//                                              position
+
+// Gives every key of slots [first, first + n_slots) of each item a compact id (cidx[key], keys[id]) and looks its row
+// up once (rowp[id]). cidx[key] goes -1 (no id) -> -2 (being claimed) -> id; the plain load skips the atomic for keys
+// that are already claimed (frequent words appear thousands of times in a step).
+template <class Src>
+__device__ __forceinline__ void det_index(const Ctx& c, const Src& src, int first, int n_slots, int* __restrict__ cidx,
+                                          Key* __restrict__ keys, float** __restrict__ rowp,
+                                          unsigned int* __restrict__ count) {
+  const int n = src.items() * n_slots;
+  for (int x = blockIdx.x * blockDim.x + threadIdx.x; x < n; x += gridDim.x * blockDim.x) {
+    const int i = x / n_slots;
+    const Key k = src.key(i, first + (x - i * n_slots));
+    if (k >= 0 && cidx[k] == -1 && atomicCAS(cidx + k, -1, -2) == -1) {
+      const unsigned r = atomicAdd(count, 1u);
+      keys[r] = k;
+      rowp[r] = home_row(c, k);
+      cidx[k] = (int)r;
+    }
+  }
+}
+
+// SCATTER = false: cnt[id] = entries of key id. SCATTER = true: desc / kid of CSR positions off[id] + j, j < cnt[id],
+// describe the entries of key id, and cnt counts back down to zero for the next step; a key without CSR positions
+// (kSinglesInScore) has its count cleared.
+template <bool SCATTER, class Src>
+__device__ __forceinline__ void det_group(const Src& src, const int* __restrict__ cidx, int* __restrict__ cnt,
+                                          const int* __restrict__ off, int* __restrict__ kid,
+                                          GatherDesc* __restrict__ desc) {
+  const int per = src.per();
+  const int n = src.items() * per;
+  for (int x = blockIdx.x * blockDim.x + threadIdx.x; x < n; x += gridDim.x * blockDim.x) {
+    const int i = x / per, s = x - i * per;
+    const Key k = src.key(i, s);
+    if (!src.counts(i, s, k)) continue;
+    const int id = __ldg(cidx + k);
+    if (!SCATTER) {
+      atomicAdd(cnt + id, 1);
+      continue;
+    }
+    const int q0 = __ldg(off + id);
+    if (Src::kSinglesInScore && __ldg(off + id + 1) == q0) {
+      cnt[id] = 0;
+      continue;
+    }
+    const int q = q0 + atomicSub(cnt + id, 1) - 1;
+    desc[q] = src.desc(i, s, x);
+    kid[q] = id;
+  }
+}
+
+// f(std::integral_constant<int, VPL>) for the float4-per-lane count of a row (1, 2 or 3)
+template <class F>
+void by_vpl(int vpl, F&& f) {
+  switch (vpl) {
+    case 1: f(std::integral_constant<int, 1>{}); break;
+    case 2: f(std::integral_constant<int, 2>{}); break;
+    default: f(std::integral_constant<int, 3>{}); break;
+  }
+}
+
+// The deterministic one-GPU step of entry source src on `stream`: index (kFirstSlots first), score, count, scan,
+// scatter, gather, finish - 9 launches with kFirstSlots, else 8. Index, Count and Scatter are the source's det_index,
+// det_group<false> and det_group<true> kernels. score(gs, vecs, cnt, fx) launches the op's score pass (one kernel) with
+// the buffers carved here: the entries' g, the vector buffer (vec_rows rows of d floats) that the descriptors point
+// into, and each key's entry count by compact id. A kSinglesInScore pass reads the counts, so it runs after the scan;
+// any other runs right after the index, and the host enqueues the short count and scan passes while the GPU runs it.
+// The caller checks that the step's entries fit an int.
+template <auto Index, auto Count, auto Scatter, class Src, class Score>
+void det_step(CudaBackend& be, cudaStream_t stream, Src src, size_t vec_rows, int d, float alpha, int vpl,
+              float* loss_out, Score&& score) {
+  const Ctx& c = be.ctx();
+  const int n_entries = src.items() * src.per();
+  const int n_ids = (int)std::min<size_t>((size_t)n_entries, (size_t)c.L.num_keys);   // bound on the distinct keys
+  const int n_ranges = (n_entries + kGatherRange - 1) / kGatherRange;
+  CudaBackend::FxScratch& fx = be.fx_scratch(0, (size_t)n_ids, 0);
+  src.gs = static_cast<float*>(be.step_buffer(kBufGs, (size_t)n_entries * sizeof(float)));
+  float* vecs = static_cast<float*>(be.step_buffer(kBufVec, vec_rows * d * sizeof(float)));
+  int* cnt = static_cast<int*>(be.step_buffer(kBufCnt, ((size_t)n_ids + 1) * sizeof(int)));    // zero between steps
+  int* off = static_cast<int*>(be.step_buffer(kBufOff, ((size_t)n_ids + 1) * sizeof(int)));
+  GatherDesc* desc = static_cast<GatherDesc*>(be.step_buffer(kBufDesc, (size_t)n_entries * sizeof(GatherDesc)));
+  int* kid = static_cast<int*>(be.step_buffer(kBufKid, (size_t)n_entries * sizeof(int)));
+  long long* part = static_cast<long long*>(                                            // zero between steps
+      be.step_buffer(kBufPart, ((size_t)n_ranges + 1) * 2 * d * sizeof(long long)));
+  float** rowp = static_cast<float**>(be.step_buffer(kBufRowp, (size_t)n_ids * sizeof(float*)));
+  size_t scan_bytes = 0;
+  det_scan(nullptr, scan_bytes, cnt, off, n_ids + 1, Src::kSinglesInScore, stream);
+  void* scan_tmp = be.step_buffer(kBufScan, scan_bytes);
+
+  const int grid_n = be.num_sms() * 8;
+  auto blocks_for = [&](long n) { return (int)std::max<long>(1, std::min<long>((n + 255) / 256, grid_n)); };
+  ADAPM_CUDA_CHECK(cudaMemsetAsync(fx.count, 0, 2 * sizeof(unsigned int), stream));
+  constexpr int first = Src::kFirstSlots;
+  if (first > 0) {
+    Index<<<blocks_for((long)src.items() * first), 256, 0, stream>>>(c, src, 0, first, fx.cidx, fx.keys, rowp,
+                                                                     fx.count);
+    ADAPM_COUNT_LAUNCH();
+  }
+  Index<<<blocks_for((long)src.items() * (src.per() - first)), 256, 0, stream>>>(c, src, first, src.per() - first,
+                                                                                 fx.cidx, fx.keys, rowp, fx.count);
+  ADAPM_COUNT_LAUNCH();
+  if constexpr (!Src::kSinglesInScore) {
+    score(src.gs, vecs, static_cast<const int*>(cnt), fx);
+    ADAPM_COUNT_LAUNCH();
+  }
+  Count<<<blocks_for(n_entries), 256, 0, stream>>>(src, fx.cidx, cnt, off, kid, desc);
+  ADAPM_COUNT_LAUNCH();
+  det_scan(scan_tmp, scan_bytes, cnt, off, n_ids + 1, Src::kSinglesInScore, stream);
+  ADAPM_COUNT_LAUNCH();
+  ADAPM_COUNT_LAUNCH();   // (the scan is two kernels)
+  if constexpr (Src::kSinglesInScore) {
+    score(src.gs, vecs, static_cast<const int*>(cnt), fx);
+    ADAPM_COUNT_LAUNCH();
+  }
+  Scatter<<<blocks_for(n_entries), 256, 0, stream>>>(src, fx.cidx, cnt, off, kid, desc);
+  ADAPM_COUNT_LAUNCH();
+  det_gather_finish(be, stream, vpl, rowp, off, n_ids, kid, desc, vecs, d, alpha, part, n_ranges, blocks_for(n_entries),
+                    fx, loss_out);
+  ADAPM_CUDA_CHECK(cudaGetLastError());
 }
 
 }  // namespace
