@@ -3,28 +3,17 @@ solve, element-wise error of the Gram matrix), bit-identical runs and target ord
 replicas and in flight on three logical ranks of one GPU, a full ALS epoch on three ranks, and the model's quality and
 monotone objective on planted data."""
 import functools
-import threading
-import time
 
-import numpy as np
 import pytest
 import torch
 
 from harness import run_cluster
+from multirank import WORLD, Case, on_peer_rows, on_replicas, one_rank_store, while_keys_move
 from test_als_cpu import ALS_QUALITY_MIN_RATIO, train_als_quality
-from test_gpu_fused_multirank import WORLD, _idiom, _mover
 
 gpu = pytest.mark.gpu
 U = 2.0 ** -24
 LAM = 0.1
-
-
-def _store(row_len, num_keys, job):
-    import adapm_b200 as ad
-
-    s = ad.Server(row_len, num_keys=num_keys, num_threads=1, rank=0, world=1, backend="cuda", fabric="inproc",
-                  job=f"{job}_{np.random.randint(1 << 30)}", dtype="float32", device=0)
-    return s, ad.Worker(0, s)
 
 
 def _problem(rank, counts, no, g, implicit):
@@ -53,8 +42,7 @@ def _fused(table, rank, targets, offsets, others, a, b, implicit, order=None, gr
     from adapm_b200.ops import als_gram, als_solve
 
     n = table.shape[0]
-    s, kv = _store(2 * rank, n, "als")
-    try:
+    with one_rank_store(2 * rank, n, "cuda", "float32") as (s, kv):
         dev = s.device
         kv.wait(kv.set(torch.arange(n), table.contiguous().view(-1)))
         G = als_gram(s, gram_keys.to(dev), rank) if implicit else None
@@ -71,9 +59,6 @@ def _fused(table, rank, targets, offsets, others, a, b, implicit, order=None, gr
         rows = torch.empty(n * 2 * rank)
         kv.wait(kv.pull(torch.arange(n), rows))
         return rows.view(n, 2 * rank), (G.cpu() if G is not None else None), stats.tolist()
-    finally:
-        kv.finalize()
-        s.shutdown()
 
 
 def _normal_equations(table, rank, t, offsets, others, a, b, G):
@@ -137,14 +122,10 @@ def test_gram_is_bit_identical_and_matches_float64_over_many_partials():
     rank, n = 36, 5000                                        # 5 partials of 1 024 keys, the last one partial
     g = torch.Generator().manual_seed(4)
     table = torch.randn(n, 2 * rank, generator=g)
-    s, kv = _store(2 * rank, n, "als_gram")
-    try:
+    with one_rank_store(2 * rank, n, "cuda", "float32") as (s, kv):
         kv.wait(kv.set(torch.arange(n), table.contiguous().view(-1)))
         keys = torch.randperm(n, generator=g).to(s.device)
         G1, G2 = als_gram(s, keys, rank), als_gram(s, keys, rank)
-    finally:
-        kv.finalize()
-        s.shutdown()
     assert torch.equal(G1, G2)
     H = table[:, :rank].double()
     assert bool(((G1.cpu().double() - H.t() @ H).abs() <= 2 * n * U * (H.abs().t() @ H.abs())).all())
@@ -154,8 +135,7 @@ def test_gram_is_bit_identical_and_matches_float64_over_many_partials():
 def test_solve_arguments_are_checked():
     from adapm_b200.ops import als_solve
 
-    s, kv = _store(16, 64, "als_args")
-    try:
+    with one_rank_store(16, 64, "cuda", "float32") as (s, kv):
         d = s.device
         t = torch.tensor([0, 1], device=d)
         off = torch.tensor([0, 1, 2], device=d)
@@ -171,30 +151,20 @@ def test_solve_arguments_are_checked():
                           args["gram"])
         with pytest.raises(TypeError):
             als_solve(s, t.int(), off, o, one, one, 8, 0.1)
-    finally:
-        kv.finalize()
-        s.shutdown()
 
 
 # ---------------------------------------------------------------------------------------------- three ranks, one GPU
 def _reference(table, rank, targets, offsets, others, a, b, G):
     """the float64 rule on a CPU store holding the fp32 rows"""
-    import adapm_b200 as ad
     from adapm_b200.ops import als_reference_solve
 
     n = table.shape[0]
-    s = ad.Server(2 * rank, num_keys=n, num_threads=1, rank=0, world=1, backend="cpu", fabric="inproc",
-                  job=f"als_ref_{np.random.randint(1 << 30)}", dtype="float64")
-    kv = ad.Worker(0, s)
-    try:
+    with one_rank_store(2 * rank, n, "cpu", "float64") as (_, kv):
         kv.wait(kv.set(torch.arange(n), table.double().contiguous().view(-1)))
         als_reference_solve(kv, targets, offsets, others, a, b, rank, LAM, G)
         rows = torch.empty(n * 2 * rank, dtype=torch.float64)
         kv.wait(kv.pull(torch.arange(n), rows))
         return rows.view(n, 2 * rank)
-    finally:
-        kv.finalize()
-        s.shutdown()
 
 
 def _check_rows(rows, ref, rank, nt):
@@ -210,127 +180,53 @@ def _multi_problem(seed, rank=64, nt=60, no=900):
     return _problem(rank, counts, no, g, implicit=False)
 
 
-def _load_on_rank0(kv, server, table):
-    if server.my_rank() == 0:
-        kv.wait(kv.set(torch.arange(table.shape[0]), table.contiguous().view(-1)))
-    kv.waitall(); kv.barrier()
+def _case(table, rank):
+    """a batch is a problem (table, targets, offsets, others, a, b): one als_solve without Gram matrix"""
+    def open_solver(server, kv):
+        from adapm_b200.ops import als_solve
 
+        dev = server.device
+        stats = torch.zeros(4, dtype=torch.int64, device=dev)
 
-def _solve_on(server, prob, rank):
-    from adapm_b200.ops import als_solve
+        def step(prob):
+            als_solve(server, *(v.to(dev).contiguous() for v in prob[1:]), rank, LAM, None, stats)
 
-    table, t, off, o, a, b = prob
-    dev = server.device
-    stats = torch.zeros(4, dtype=torch.int64, device=dev)
-    stream = torch.cuda.Stream(dev)
-    with torch.cuda.stream(stream):
-        als_solve(server, *(v.to(dev).contiguous() for v in (t, off, o, a, b)), rank, LAM, None, stats)
-    stream.synchronize()
-    return stats.tolist()
+        step.totals = lambda: (None, stats.tolist())
+        return step
 
-
-def _peer_worker(kv, server, wid, prob, rank):
-    _load_on_rank0(kv, server, prob[0])
-    out = {}
-    if server.my_rank() == 1:                  # key k lives on rank k % 3: two thirds of the rows are peer rows
-        out["stats"] = _solve_on(server, prob, rank)
-    _idiom(kv)
-    if server.my_rank() == 0:
-        n = prob[0].shape[0]
-        rows = torch.empty(n * 2 * rank)
-        kv.wait(kv.pull(torch.arange(n), rows))
-        out["rows"] = rows.view(n, 2 * rank)
-    kv.barrier()
-    kv.finalize()
-    return out
+    n = table.shape[0]
+    return Case(2 * rank, n, [(torch.arange(n), table)], lambda prob: torch.unique(torch.cat([prob[1], prob[3]])),
+                open_solver)
 
 
 @gpu
 def test_solve_reads_other_side_rows_on_peers():
     rank = 64
     prob = _multi_problem(5, rank)
-    table = prob[0]
-    res = run_cluster(functools.partial(_peer_worker, prob=prob, rank=rank), world=WORLD, workers=1, mode="threads",
-                      value_lengths=2 * rank, num_keys=table.shape[0], dtype="float32", backend="cuda")
-    stats = res[1][0]["stats"]
+    # only rank 1 solves; key k lives on rank k % 3: two thirds of the rows are peer rows
+    res = on_peer_rows(_case(prob[0], rank), [None, prob, None], in_turns=True)
+    stats = res[1]["stats"]
     nt = prob[1].numel()
     assert stats[1] > 0 and stats[0] + stats[1] + stats[2] == int(prob[2][-1]) and stats[3] == nt, stats
-    _check_rows(res[0][0]["rows"], _reference(*prob[:1], rank, *prob[1:], None), rank, nt)
-
-
-def _replica_worker(kv, server, wid, prob, rank):
-    _load_on_rank0(kv, server, prob[0])
-    table, t, off, o = prob[:4]
-    rk = server.my_rank()
-    mine = torch.unique(torch.cat([t, o]))
-    c = kv.current_clock()
-    kv.intent(mine, c, c + 1_000_000)          # every rank wants every row: most become replicas
-    for _ in range(50):
-        kv.advance_clock()
-        _idiom(kv)
-        missing = sum(not server.is_local(int(k)) for k in mine)
-        if server.allreduce_sum([float(missing)])[0] == 0:
-            break
-    out = {"local": all(server.is_local(int(k)) for k in mine), "replicas": sum(server.owner_of(int(k)) != rk
-                                                                                for k in mine)}
-    if rk == 2:
-        out["stats"] = _solve_on(server, prob, rank)
-    for _ in range(4):
-        kv.advance_clock()
-        _idiom(kv)
-    n = table.shape[0]
-    rows = torch.empty(n * 2 * rank)
-    kv.wait(kv.pull(torch.arange(n), rows))
-    out["rows"] = rows.view(n, 2 * rank)
-    kv.barrier()
-    kv.finalize()
-    return out
+    _check_rows(res[0]["rows"][0], _reference(*prob[:1], rank, *prob[1:], None), rank, nt)
 
 
 @gpu
 def test_solve_on_replicated_rows():
     rank = 64
     prob = _multi_problem(7, rank)
-    res = run_cluster(functools.partial(_replica_worker, prob=prob, rank=rank), world=WORLD, workers=1, mode="threads",
-                      value_lengths=2 * rank, num_keys=prob[0].shape[0], dtype="float32", backend="cuda",
-                      options={"sys.techniques": "replication_only"})
-    assert sum(x["counters"]["replica_setups"] for x in res.values()) > 0
-    assert all(x["counters"]["protocol_errors"] == 0 for x in res.values())
-    out = res[2][0]
+    case = _case(prob[0], rank)
+    # every rank wants every row, so most become replicas; only rank 2 solves
+    res = on_replicas(case, [None, None, prob], intent_keys=case.keys_of(prob))
+    assert sum(x["counters"]["replica_setups"] for x in res) > 0
+    assert all(x["counters"]["protocol_errors"] == 0 for x in res)
+    out = res[2]
     assert out["local"] and out["replicas"] > 0
     s = out["stats"]
     assert s[0] == int(prob[2][-1]) and s[1] == 0 and s[2] == 0 and s[3] == prob[1].numel(), s
     ref = _reference(*prob[:1], rank, *prob[1:], None)
     for k in range(WORLD):
-        _check_rows(res[k][0]["rows"], ref, rank, prob[1].numel())
-
-
-def _inflight_worker(kv, server, wid, probs, rank, done):
-    _load_on_rank0(kv, server, probs[0][0])
-    out = {}
-    n = probs[0][0].shape[0]
-    if server.my_rank() < 2:
-        out["iters"] = _mover(kv, server.my_rank(), torch.arange(n), done)
-    else:
-        tot = [0, 0, 0, 0]
-        try:
-            for p in probs:
-                tot = [x + y for x, y in zip(tot, _solve_on(server, p, rank))]
-                time.sleep(0.03)
-        finally:
-            done.set()
-        out["stats"] = tot
-    kv.barrier()
-    for _ in range(8):
-        kv.advance_clock()
-    _idiom(kv)
-    if server.my_rank() == 2:
-        rows = torch.empty(n * 2 * rank)
-        kv.wait(kv.pull(torch.arange(n), rows))
-        out["rows"] = rows.view(n, 2 * rank)
-    kv.barrier()
-    kv.finalize()
-    return out
+        _check_rows(res[k]["rows"][0], ref, rank, prob[1].numel())
 
 
 @gpu
@@ -356,33 +252,23 @@ def test_solve_loses_no_update_while_keys_move(technique):
 
     halves = [side(ii, jj, 0, nu, nu), side(jj, ii, nu, 0, ni)] * 6
     probs = [(table,) + h[1:] for h in halves]
-    done = threading.Event()
-    res = run_cluster(functools.partial(_inflight_worker, probs=probs, rank=rank, done=done), world=WORLD, workers=1,
-                      mode="threads", value_lengths=2 * rank, num_keys=nu + ni, dtype="float32", backend="cuda",
-                      options={"sys.techniques": technique})
-    out = res[2][0]
-    relocations = sum(x["counters"]["relocations"] for x in res.values())
+    res = while_keys_move(_case(table, rank), probs, technique)
+    out = res[2]
+    relocations = sum(x["counters"]["relocations"] for x in res)
     info = f"{technique}: stats {out['stats']}, relocations {relocations}"
     print(info)
-    assert relocations > 0 and all(x["counters"]["protocol_errors"] == 0 for x in res.values()), info
+    assert relocations > 0 and all(x["counters"]["protocol_errors"] == 0 for x in res), info
     assert out["stats"][3] == 6 * (nu + ni), info
     # the float64 rule, half-step by half-step, from the same start
-    import adapm_b200 as ad
     from adapm_b200.ops import als_reference_solve
 
-    s = ad.Server(2 * rank, num_keys=nu + ni, num_threads=1, rank=0, world=1, backend="cpu", fabric="inproc",
-                  job=f"als_inflight_ref_{np.random.randint(1 << 30)}", dtype="float64")
-    kv = ad.Worker(0, s)
-    try:
+    with one_rank_store(2 * rank, nu + ni, "cpu", "float64") as (_, kv):
         kv.wait(kv.set(torch.arange(nu + ni), table.double().contiguous().view(-1)))
         for h in halves:
             als_reference_solve(kv, *h[1:], rank, LAM)
         ref = torch.empty((nu + ni) * 2 * rank, dtype=torch.float64)
         kv.wait(kv.pull(torch.arange(nu + ni), ref))
-    finally:
-        kv.finalize()
-        s.shutdown()
-    torch.testing.assert_close(out["rows"].double(), ref.view(nu + ni, 2 * rank), rtol=2e-3, atol=2e-4)
+    torch.testing.assert_close(out["rows"][0].double(), ref.view(nu + ni, 2 * rank), rtol=2e-3, atol=2e-4)
 
 
 # ---------------------------------------------------------------------------------------------- the model

@@ -2,28 +2,19 @@
 ``bpr_reference_step`` on one GPU and on three logical ranks of one GPU (peer rows, replicas, keys in flight),
 ``MatrixFactorization.recommend`` against ``topk_reference``, and the model's quality on planted data."""
 import functools
-import threading
-import time
 
 import numpy as np
 import pytest
 import torch
 
 from harness import WRAP, run_cluster, wrap_calls
+from multirank import (WORLD, Case, Fused, on_peer_rows, on_replicas, one_rank_store, reads_while_keys_move,
+                       rejected_on_ranks, while_keys_move)
 from test_bpr_cpu import QUALITY_MIN_RATIO, train_quality
-from test_gpu_fused_multirank import WORLD, _idiom, _mover
 
 gpu = pytest.mark.gpu
 RTOL, ATOL = 2e-4, 2e-5
 EPS, LAM = 0.05, 0.02
-
-
-def _store(row_len, num_keys, backend, dtype, job):
-    import adapm_b200 as ad
-
-    s = ad.Server(row_len, num_keys=num_keys, num_threads=1, rank=0, world=1, backend=backend, fabric="inproc",
-                  job=f"{job}_{np.random.randint(1 << 30)}", dtype=dtype, **({"device": 0} if backend == "cuda" else {}))
-    return s, ad.Worker(0, s)
 
 
 def _init_table(num_keys, r, g):
@@ -57,8 +48,7 @@ def _rule(table, batches, r):
     from adapm_b200.ops import bpr_reference_step
 
     n = table.shape[0]
-    s, kv = _store(2 * r, n, "cpu", "float64", "bpr_rule")
-    try:
+    with one_rank_store(2 * r, n, "cpu", "float64") as (s, kv):
         kv.wait(kv.set(torch.arange(n), table.contiguous().view(-1)))
         loss, pushes = 0.0, 0
         for b in batches:
@@ -67,9 +57,6 @@ def _rule(table, batches, r):
         rows = torch.empty(n * 2 * r, dtype=torch.float64)
         kv.wait(kv.pull(torch.arange(n), rows))
         return rows.view(n, 2 * r), loss, pushes
-    finally:
-        kv.finalize()
-        s.shutdown()
 
 
 def _fused(table, batches, r, deterministic):
@@ -77,8 +64,7 @@ def _fused(table, batches, r, deterministic):
     from adapm_b200.ops import mf_bpr_step
 
     n = table.shape[0]
-    s, kv = _store(2 * r, n, "cuda", "float32", "bpr_fused")
-    try:
+    with one_rank_store(2 * r, n, "cuda", "float32") as (s, kv):
         kv.wait(kv.set(torch.arange(n), table.float().contiguous().view(-1)))
         dev = s.device
         loss = torch.zeros(1, device=dev)
@@ -92,9 +78,6 @@ def _fused(table, batches, r, deterministic):
         rows = torch.empty(n * 2 * r, dtype=torch.float32)
         kv.wait(kv.pull(torch.arange(n), rows))
         return rows.view(n, 2 * r).double(), float(loss.item()), stats.tolist(), launches
-    finally:
-        kv.finalize()
-        s.shutdown()
 
 
 RANKS = (4, 128, 132, 256, 260, 384, 512)       # VPL 1, 1, 2, 2, 3, 3, 4; 132 and 260 end in a partial float4 row
@@ -146,8 +129,7 @@ def test_inplace_step_matches_rule_on_distinct_keys(rank, n, B):
 def test_step_arguments_are_checked():
     from adapm_b200.ops import mf_bpr_step
 
-    s, kv = _store(16, 64, "cuda", "float32", "bpr_args")
-    try:
+    with one_rank_store(16, 64, "cuda", "float32") as (s, kv):
         dev = s.device
         k = torch.zeros(2, dtype=torch.int64, device=dev)
         loss = torch.zeros(1, device=dev)
@@ -157,62 +139,32 @@ def test_step_arguments_are_checked():
                 mf_bpr_step(s, k, k + 1, neg.long().to(dev), rank, 0.1, 0.0, loss)
         with pytest.raises(TypeError):
             mf_bpr_step(s, k.int(), k + 1, torch.zeros(2, 1, dtype=torch.int64, device=dev), 8, 0.1, 0.0, loss)
-    finally:
-        kv.finalize()
-        s.shutdown()
-
-
-def _reject_worker(kv, server, wid):
-    from adapm_b200.ops import mf_bpr_step
-
-    dev = server.device
-    k = torch.zeros(2, dtype=torch.int64, device=dev)
-    out = {}
-    try:
-        mf_bpr_step(server, k, k + 1, torch.ones(2, 3, dtype=torch.int64, device=dev), 8, 0.1, 0.0,
-                    torch.zeros(1, device=dev), deterministic=True)
-        out["raised"] = False
-    except ValueError:
-        out["raised"] = True
-    kv.barrier()
-    kv.finalize()
-    return out
 
 
 @gpu
 def test_deterministic_step_rejected_on_several_ranks():
-    res = run_cluster(_reject_worker, world=2, workers=1, mode="threads", value_lengths=16, num_keys=64,
-                      dtype="float32", backend="cuda")
-    assert all(r[0]["raised"] for r in res.values())
+    from adapm_b200.ops import mf_bpr_step
+
+    def call(server):
+        dev = server.device
+        k = torch.zeros(2, dtype=torch.int64, device=dev)
+        mf_bpr_step(server, k, k + 1, torch.ones(2, 3, dtype=torch.int64, device=dev), 8, 0.1, 0.0,
+                    torch.zeros(1, device=dev), deterministic=True)
+
+    assert rejected_on_ranks(call)
 
 
 # ---------------------------------------------------------------------------------------------- three ranks, one GPU
-def _peer_worker(kv, server, wid, table, batches, r):
+def _case(table, r):
     from adapm_b200.ops import mf_bpr_step
 
-    rank = server.my_rank()
+    def step(server, b, loss, stats):
+        dev = server.device
+        mf_bpr_step(server, *(t.to(dev).contiguous() for t in b), r, EPS, LAM, loss, stats)
+
     n = table.shape[0]
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(n), table.float().contiguous().view(-1)))
-    kv.waitall(); kv.barrier()
-    dev = server.device
-    loss = torch.zeros(1, device=dev)
-    stats = torch.zeros(4, dtype=torch.int64, device=dev)
-    stream = torch.cuda.Stream(dev)
-    for turn in range(WORLD):                         # one rank at a time, in rank order
-        if turn == rank:
-            with torch.cuda.stream(stream):
-                mf_bpr_step(server, *(t.to(dev).contiguous() for t in batches[rank]), r, EPS, LAM, loss, stats)
-                stream.synchronize()
-        _idiom(kv)
-    out = {"loss": float(loss.item()), "stats": stats.tolist()}
-    if rank == 0:
-        rows = torch.empty(n * 2 * r)
-        kv.wait(kv.pull(torch.arange(n), rows))
-        out["rows"] = rows.view(n, 2 * r).double()
-    kv.barrier()
-    kv.finalize()
-    return out
+    return Case(2 * r, n, [(torch.arange(n), table)], lambda b: torch.unique(torch.cat([t.reshape(-1) for t in b])),
+                lambda server, kv: Fused(server, step))
 
 
 @gpu
@@ -223,50 +175,12 @@ def test_step_on_peer_rows():
     g = torch.Generator().manual_seed(5)
     table = _init_table(nu + ni, r, g)
     batches = [_batch(nu, ni, B, n, g, distinct=True) for _ in range(WORLD)]
-    res = run_cluster(functools.partial(_peer_worker, table=table, batches=batches, r=r), world=WORLD, workers=1,
-                      mode="threads", value_lengths=2 * r, num_keys=nu + ni, dtype="float32", backend="cuda")
+    res = on_peer_rows(_case(table, r), batches, in_turns=True)
     ref, ref_loss, ref_pushes = _rule(table, batches, r)
-    assert sum(x[0]["stats"][3] for x in res.values()) == ref_pushes
-    assert sum(x[0]["stats"][1] for x in res.values()) > 0       # peer rows were read
-    torch.testing.assert_close(res[0][0]["rows"], ref, rtol=RTOL, atol=ATOL)
-    torch.testing.assert_close(sum(x[0]["loss"] for x in res.values()), ref_loss, rtol=1e-4, atol=1e-3)
-
-
-def _replica_worker(kv, server, wid, table, batches, r):
-    from adapm_b200.ops import mf_bpr_step
-
-    rank = server.my_rank()
-    n = table.shape[0]
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(n), table.float().contiguous().view(-1)))
-    kv.waitall(); kv.barrier()
-    mine = torch.unique(torch.cat([t.reshape(-1) for t in batches[rank]]))
-    c = kv.current_clock()
-    kv.intent(mine, c, c + 1_000_000)
-    for _ in range(50):
-        kv.advance_clock()
-        _idiom(kv)
-        missing = sum(not server.is_local(int(k)) for k in mine)
-        if server.allreduce_sum([float(missing)])[0] == 0:
-            break
-    local = all(server.is_local(int(k)) for k in mine)
-    replicas = sum(server.owner_of(int(k)) != rank for k in mine)
-    dev = server.device
-    loss = torch.zeros(1, device=dev)
-    stats = torch.zeros(4, dtype=torch.int64, device=dev)
-    stream = torch.cuda.Stream(dev)
-    for turn in range(WORLD):
-        if turn == rank:
-            with torch.cuda.stream(stream):
-                mf_bpr_step(server, *(t.to(dev).contiguous() for t in batches[rank]), r, EPS, LAM, loss, stats)
-            stream.synchronize()
-        _idiom(kv)
-    rows = torch.empty(n * 2 * r)
-    kv.wait(kv.pull(torch.arange(n), rows))
-    kv.barrier()
-    kv.finalize()
-    return {"loss": float(loss.item()), "stats": stats.tolist(), "rows": rows.view(n, 2 * r).double(), "local": local,
-            "replicas": replicas}
+    assert sum(x["stats"][3] for x in res) == ref_pushes
+    assert sum(x["stats"][1] for x in res) > 0       # peer rows were read
+    torch.testing.assert_close(res[0]["rows"][0].double(), ref, rtol=RTOL, atol=ATOL)
+    torch.testing.assert_close(sum(x["loss"] for x in res), ref_loss, rtol=1e-4, atol=1e-3)
 
 
 @gpu
@@ -279,56 +193,17 @@ def test_step_on_replicas():
     g = torch.Generator().manual_seed(21)
     table = _init_table(nu + ni, r, g)
     batches = [_batch(nu, ni, B, n, g, distinct=True) for _ in range(WORLD)]
-    res = run_cluster(functools.partial(_replica_worker, table=table, batches=batches, r=r), world=WORLD, workers=1,
-                      mode="threads", value_lengths=2 * r, num_keys=nu + ni, dtype="float32", backend="cuda",
-                      options={"sys.techniques": "replication_only"})
-    assert sum(x["counters"]["replica_setups"] for x in res.values()) > 0
-    assert all(x["counters"]["protocol_errors"] == 0 for x in res.values())
+    res = on_replicas(_case(table, r), batches)
+    assert sum(x["counters"]["replica_setups"] for x in res) > 0
+    assert all(x["counters"]["protocol_errors"] == 0 for x in res)
     ref, _, _ = _rule(table, batches, r)
     for k in range(WORLD):
-        out = res[k][0]
+        out = res[k]
         assert out["local"] and out["replicas"] > 0, f"rank {k}: batch keys not local after the intents"
-        torch.testing.assert_close(out["rows"], ref, rtol=RTOL, atol=ATOL, msg=lambda m: f"rows read on rank {k}: {m}")
+        torch.testing.assert_close(out["rows"][0].double(), ref, rtol=RTOL, atol=ATOL,
+                                   msg=lambda m: f"rows read on rank {k}: {m}")
         s = out["stats"]
         assert s[0] == B * (2 + n) and s[1] == 0 and s[2] == 0 and s[3] == B * (2 + n), (k, s)
-
-
-def _inflight_step_worker(kv, server, wid, table, batches, r, done):
-    from adapm_b200.ops import mf_bpr_step
-
-    rank = server.my_rank()
-    n = table.shape[0]
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(n), table.float().contiguous().view(-1)))
-    kv.waitall(); kv.barrier()
-    out = {}
-    if rank < 2:
-        out["iters"] = _mover(kv, rank, torch.arange(n), done)
-    else:
-        dev = server.device
-        loss = torch.zeros(1, device=dev)
-        stats = torch.zeros(4, dtype=torch.int64, device=dev)
-        stream = torch.cuda.Stream(dev)
-        try:
-            with torch.cuda.stream(stream):
-                for b in batches:
-                    mf_bpr_step(server, *(t.to(dev).contiguous() for t in b), r, EPS, LAM, loss, stats)
-                    stream.synchronize()
-                    time.sleep(0.03)
-        finally:
-            done.set()
-        out["loss"], out["stats"] = float(loss.item()), stats.tolist()
-    kv.barrier()
-    for _ in range(8):
-        kv.advance_clock()
-    _idiom(kv)
-    if rank == 2:
-        rows = torch.empty(n * 2 * r)
-        kv.wait(kv.pull(torch.arange(n), rows))
-        out["rows"] = rows.view(n, 2 * r).double()
-    kv.barrier()
-    kv.finalize()
-    return out
 
 
 @gpu
@@ -340,18 +215,15 @@ def test_step_loses_no_update_while_keys_move(technique):
     g = torch.Generator().manual_seed(9)
     table = _init_table(nu + ni, r, g)
     batches = [_batch(nu, ni, B, n, g, distinct=True) for _ in range(32)]
-    done = threading.Event()
-    res = run_cluster(functools.partial(_inflight_step_worker, table=table, batches=batches, r=r, done=done),
-                      world=WORLD, workers=1, mode="threads", value_lengths=2 * r, num_keys=nu + ni, dtype="float32",
-                      backend="cuda", options={"sys.techniques": technique})
-    out = res[2][0]
-    relocations = sum(x["counters"]["relocations"] for x in res.values())
+    res = while_keys_move(_case(table, r), batches, technique)
+    out = res[2]
+    relocations = sum(x["counters"]["relocations"] for x in res)
     info = f"{technique}: stats {out['stats']}, relocations {relocations}"
     print(info)
-    assert relocations > 0 and all(x["counters"]["protocol_errors"] == 0 for x in res.values()), info
+    assert relocations > 0 and all(x["counters"]["protocol_errors"] == 0 for x in res), info
     ref, ref_loss, ref_pushes = _rule(table, batches, r)
     assert out["stats"][3] == ref_pushes == 32 * B * (2 + n), info
-    torch.testing.assert_close(out["rows"], ref, rtol=RTOL, atol=ATOL)
+    torch.testing.assert_close(out["rows"][0].double(), ref, rtol=RTOL, atol=ATOL)
     torch.testing.assert_close(out["loss"], ref_loss, rtol=1e-4, atol=1e-3)
 
 
@@ -379,11 +251,16 @@ def _rec_inputs(g, m=300, n=1000, r=64):
     return W, H, data
 
 
-def _load_factors(kv, model, W, H, dev):
+def _factor_rows(W, H, fck):
+    """(keys, rows [m + n, 2 r]) of the factors, items from key ``fck`` on"""
     m, r = W.shape
     rows = torch.zeros(m + H.shape[0], 2 * r)
     rows[:m, :r], rows[m:, :r] = W, H
-    keys = torch.cat([torch.arange(m), torch.arange(H.shape[0]) + model.fck])
+    return torch.cat([torch.arange(m), torch.arange(H.shape[0]) + fck]), rows
+
+
+def _load_factors(kv, model, W, H, dev):
+    keys, rows = _factor_rows(W, H, model.fck)
     kv.wait(kv.set(keys.to(dev), rows.view(-1).to(dev)))
     kv.waitall()
 
@@ -396,8 +273,7 @@ def test_recommend_matches_topk_reference(k):
     g = torch.Generator().manual_seed(k)
     W, H, data = _rec_inputs(g)
     m, n = W.shape[0], H.shape[0]
-    s, kv = _store(2 * W.shape[1], m + n, "cuda", "float32", "bpr_rec")
-    try:
+    with one_rank_store(2 * W.shape[1], m + n, "cuda", "float32") as (s, kv):
         model = _rec_model(s, kv, W, H, data)
         _load_factors(kv, model, W, H, s.device)
         users = np.arange(m)
@@ -405,9 +281,6 @@ def test_recommend_matches_topk_reference(k):
         idx, vals = model.recommend(users, k, seen=seen)
         idx2, vals2 = model.recommend(users, k, seen=seen)
         plain_idx, plain_vals = model.recommend(users[:50], k)
-    finally:
-        kv.finalize()
-        s.shutdown()
     assert torch.equal(idx, idx2) and torch.equal(vals, vals2)
     excluded = torch.zeros(m, n, dtype=torch.bool)
     excluded[torch.repeat_interleave(torch.arange(m), seen[0][1:] - seen[0][:-1]), seen[1]] = True
@@ -420,58 +293,34 @@ def test_recommend_matches_topk_reference(k):
         assert int((idx[0] == -1).sum()) == k - 5
 
 
-def _rec_inflight_worker(kv, server, wid, W, H, data, exp, done):
-    rank = server.my_rank()
-    model = _rec_model(server, kv, W, H, data)
-    if rank == 0:
-        _load_factors(kv, model, W, H, server.device)
-    kv.waitall(); kv.barrier()
-    out = {}
-    n = W.shape[0] + H.shape[0]
-    if rank < 2:
-        out["iters"] = _mover(kv, rank, torch.arange(0, n, 4), done)
-    else:
-        users = np.arange(W.shape[0])
-        seen = data.seen(users)
-        mism, reps = 0, 0
-        try:
-            t0 = time.time()
-            while (reps < 8 or time.time() - t0 < 3.0) and reps < 200:
-                idx, vals = model.recommend(users, 10, seen=seen)
-                mism += not (torch.equal(idx.cpu(), exp[0]) and torch.equal(vals.cpu(), exp[1]))
-                reps += 1
-        finally:
-            done.set()
-        out.update(mism=mism, reps=reps)
-    kv.barrier()
-    _idiom(kv)
-    kv.finalize()
-    return out
-
-
 @gpu
 def test_recommend_bit_identical_while_keys_move():
+    from adapm_b200.models.mf import MFConfig
+
     g = torch.Generator().manual_seed(31)
     W, H, data = _rec_inputs(g, m=201, n=3000)           # 201 users: the first item key is 201 on 1 and on 3 ranks
-    s, kv = _store(2 * W.shape[1], W.shape[0] + H.shape[0], "cuda", "float32", "bpr_rec1")
-    try:
+    users = np.arange(W.shape[0])
+    seen = data.seen(users)
+    with one_rank_store(2 * W.shape[1], W.shape[0] + H.shape[0], "cuda", "float32") as (s, kv):
         model = _rec_model(s, kv, W, H, data)
         _load_factors(kv, model, W, H, s.device)
-        exp = tuple(t.cpu() for t in model.recommend(np.arange(W.shape[0]), 10, seen=data.seen(np.arange(W.shape[0]))))
-    finally:
-        kv.finalize()
-        s.shutdown()
+        exp = tuple(t.cpu() for t in model.recommend(users, 10, seen=seen))
+
     # the data keeps the one-rank partitioning: all users are in rank 2's row block
-    done = threading.Event()
-    res = run_cluster(functools.partial(_rec_inflight_worker, W=W, H=H, data=data, exp=exp, done=done), world=WORLD,
-                      workers=1, mode="threads", value_lengths=2 * W.shape[1], num_keys=W.shape[0] + H.shape[0],
-                      dtype="float32", backend="cuda", options={"sys.techniques": "relocation_only"})
-    out = res[2][0]
-    relocations = sum(x["counters"]["relocations"] for x in res.values())
+    def read(server, kv, stats):
+        model = _rec_model(server, kv, W, H, data)
+        return lambda: {"top10": model.recommend(users, 10, seen=seen)}
+
+    n = W.shape[0] + H.shape[0]
+    fck = MFConfig(num_rows=W.shape[0], num_cols=H.shape[0], rank=W.shape[1]).first_col_key(WORLD)
+    case = Case(2 * W.shape[1], n, [_factor_rows(W, H, fck)])
+    res = reads_while_keys_move(case, read, {"top10": exp}, torch.arange(0, n, 4), "relocation_only")
+    out = res[2]
+    relocations = sum(x["counters"]["relocations"] for x in res)
     info = f"{out['reps']} repetitions, relocations {relocations}"
     print(info)
     assert relocations > 0, info
-    assert out["mism"] == 0, info
+    assert not out["mism"], info
 
 
 # ---------------------------------------------------------------------------------------------- quality and DSGD

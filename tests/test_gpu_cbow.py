@@ -1,40 +1,27 @@
 """The fused CBOW step (csrc/cuda/ops_cbow.cu) through ``ops.cbow_step`` on an H100: the deterministic one-GPU step
 against the float64 rule over consecutive steps (with a hot word that takes the heavy-key path of the gather) and bit
 for bit against itself, the in-place kernel on one GPU, the in-place kernel on multi-rank stores (three logical ranks on
-one GPU, as in test_gpu_fused_multirank.py: peer rows, replicas, keys in flight), training end to end, and the build
+one GPU, run by multirank.py: peer rows, replicas, keys in flight), training end to end, and the build
 budget of the kernels."""
-import functools
 import glob
 import os
 import re
 import subprocess
 import sys
-import threading
-import time
 
-import numpy as np
 import pytest
 import torch
 
-from harness import run_cluster
+from multirank import (WORLD, Case, Fused, load_rows, on_peer_rows, on_replicas, one_rank_store, rejected_on_ranks,
+                       while_keys_move)
 from test_cbow_cpu import TOPIC_PRECISION, corner_batch, torch_rule64, train_planted
-from test_gpu_fused_multirank import _idiom, _load, _mover
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 gpu = pytest.mark.gpu
-WORLD = 3
 RTOL, ATOL = 2e-4, 2e-5
 # (the hot word moves by up to ALPHA per context occurrence, 10 000 times per step; at 0.05 its neu1e^2 terms summed over
 # three steps leave the deterministic step's fixed-point AdaGrad range of 2^27 per element and step, see ops_cbow.cu)
 ALPHA = 0.01
-
-
-def _cuda_server(row_len, num_keys, job):
-    import adapm_b200 as ad
-
-    s = ad.Server(row_len, num_keys=num_keys, num_threads=1, rank=0, world=1, backend="cuda", fabric="inproc",
-                  job=f"{job}_{np.random.randint(1 << 30)}", device=0)
-    return s, ad.Worker(0, s)
 
 
 def _table(g, n_keys, d):
@@ -93,9 +80,8 @@ def test_deterministic_step_matches_float64_rule(d, neg):
     vocab = 3000
     g = torch.Generator().manual_seed(d * 100 + neg)
     table = _table(g, 2 * vocab, d)
-    server, kv = _cuda_server(2 * d, 2 * vocab, f"cbowdet{d}")
-    try:
-        _load(kv, [(torch.arange(2 * vocab), table)])
+    with one_rank_store(2 * d, 2 * vocab, "cuda", "float32") as (server, kv):
+        load_rows(kv, [(torch.arange(2 * vocab), table)])
         kv.waitall()
         dev = server.device
         ref = table.double()
@@ -116,25 +102,18 @@ def test_deterministic_step_matches_float64_rule(d, neg):
             assert float(loss) == pytest.approx(ref_loss, rel=1e-4), what
             s = stats.tolist()
             assert s[3] == _updates(b) and s[2] == 0 and s[1] == 0, (what, s)
-    finally:
-        kv.finalize()
-        server.shutdown()
 
 
 def _bits_run(d, neg, steps):
-    server, kv = _cuda_server(2 * d, 2 * 3000, "cbowbits")
-    try:
+    with one_rank_store(2 * d, 2 * 3000, "cuda", "float32") as (server, kv):
         g = torch.Generator().manual_seed(1)
-        _load(kv, [(torch.arange(6000), _table(g, 6000, d))])
+        load_rows(kv, [(torch.arange(6000), _table(g, 6000, d))])
         kv.waitall()
         loss = torch.zeros(1, device=server.device)
         for b in steps:
             _step(server, b, d, loss, None)
         torch.cuda.synchronize()
         return _rows(kv, 6000, d), loss.cpu()
-    finally:
-        kv.finalize()
-        server.shutdown()
 
 
 @gpu
@@ -150,10 +129,9 @@ def test_two_runs_on_fresh_stores_are_bit_identical():
 def test_launch_counts():
     from adapm_b200 import _C
 
-    server, kv = _cuda_server(2 * 64, 2000, "cbowlaunch")
-    try:
+    with one_rank_store(2 * 64, 2000, "cuda", "float32") as (server, kv):
         g = torch.Generator().manual_seed(3)
-        _load(kv, [(torch.arange(2000), _table(g, 2000, 64))])
+        load_rows(kv, [(torch.arange(2000), _table(g, 2000, 64))])
         b = corner_batch(g, 1000, 300, 8, 5)
         loss = torch.zeros(1, device=server.device)
         torch.cuda.synchronize()
@@ -163,9 +141,6 @@ def test_launch_counts():
         _step(server, b, 64, loss, None, deterministic=False)
         assert _C.kernel_launches() - n0 == 9          # the in-place kernel
         torch.cuda.synchronize()
-    finally:
-        kv.finalize()
-        server.shutdown()
 
 
 def _distinct_batch(g, words, B, C, neg, pad=True):
@@ -185,11 +160,10 @@ def test_inplace_kernel_on_one_gpu_matches_rule(d, neg):
     from adapm_b200 import _C
 
     vocab = 4000
-    server, kv = _cuda_server(2 * d, 2 * vocab, f"cbowip{d}")
-    try:
+    with one_rank_store(2 * d, 2 * vocab, "cuda", "float32") as (server, kv):
         g = torch.Generator().manual_seed(d + neg)
         table = _table(g, 2 * vocab, d)
-        _load(kv, [(torch.arange(2 * vocab), table)])
+        load_rows(kv, [(torch.arange(2 * vocab), table)])
         kv.waitall()
         ref = table.double()
         dev = server.device
@@ -207,30 +181,18 @@ def test_inplace_kernel_on_one_gpu_matches_rule(d, neg):
             assert float(loss) == pytest.approx(ref_loss, rel=1e-4)
             s = stats.tolist()
             assert s[3] == _updates(b) and s[2] == 0, s
-    finally:
-        kv.finalize()
-        server.shutdown()
 
 
 @gpu
 def test_deterministic_true_is_rejected_on_several_ranks():
-    def worker(kv, server, wid):
-        from adapm_b200.ops import cbow_step
+    from adapm_b200.ops import cbow_step
 
+    def call(server):
         dev = server.device
         z = torch.zeros(4, dtype=torch.int64, device=dev)
-        try:
-            cbow_step(server, z, z.view(4, 1), z.view(4, 1), 8, 0.1, torch.zeros(1, device=dev), deterministic=True)
-            raised = False
-        except ValueError:
-            raised = True
-        kv.barrier()
-        kv.finalize()
-        return raised
+        cbow_step(server, z, z.view(4, 1), z.view(4, 1), 8, 0.1, torch.zeros(1, device=dev), deterministic=True)
 
-    res = run_cluster(worker, world=2, workers=1, mode="threads", value_lengths=16, num_keys=100, dtype="float32",
-                      backend="cuda")
-    assert all(r[0] for r in res.values())
+    assert rejected_on_ranks(call, value_lengths=16, num_keys=100)
 
 
 # ---------------------------------------------------------------------------------------------- several ranks
@@ -249,27 +211,16 @@ def _apply(table, batches):
     return table, loss
 
 
-def _fused(server, b, loss, stats, stream):
-    with torch.cuda.stream(stream):
-        _step(server, b, DIM, loss, stats)
-    stream.synchronize()
+def _keys_of(b):
+    c, x, n = b
+    k = torch.cat([c, x.reshape(-1), n.reshape(-1)])
+    return torch.unique(k[k >= 0])
 
 
-def _peer_worker(kv, server, wid, table, batches):
-    rank = server.my_rank()
+def _case(table):
     n = table.shape[0]
-    if rank == 0:
-        _load(kv, [(torch.arange(n), table)])
-    kv.waitall(); kv.barrier()
-    dev = server.device
-    loss = torch.zeros(1, device=dev)
-    stats = torch.zeros(4, dtype=torch.int64, device=dev)
-    _fused(server, batches[rank], loss, stats, torch.cuda.Stream(dev))
-    kv.barrier()
-    rows = _rows(kv, n, DIM) if rank == 0 else None
-    kv.barrier()
-    kv.finalize()
-    return {"loss": float(loss.item()), "stats": stats.tolist(), "rows": rows}
+    return Case(2 * DIM, n, [(torch.arange(n), table)], _keys_of,
+                lambda server, kv: Fused(server, lambda s, b, loss, stats: _step(s, b, DIM, loss, stats)))
 
 
 @gpu
@@ -279,52 +230,15 @@ def test_peer_rows_match_float64_rule():
     g = torch.Generator().manual_seed(21)
     table = _table(g, 2 * WORLD * m, DIM)
     batches = [_distinct_batch(g, _ranks_words(r, m), 48, CTX, NEG) for r in range(WORLD)]
-    res = run_cluster(functools.partial(_peer_worker, table=table, batches=batches), world=WORLD, workers=1,
-                      mode="threads", value_lengths=2 * DIM, num_keys=table.shape[0], dtype="float32", backend="cuda")
+    res = on_peer_rows(_case(table), batches, in_turns=False)
     ref, _ = _apply(table.double(), batches)
-    torch.testing.assert_close(res[0][0]["rows"].double(), ref, rtol=RTOL, atol=ATOL)
+    torch.testing.assert_close(res[0]["rows"][0].double(), ref, rtol=RTOL, atol=ATOL)
     for r in range(WORLD):
-        out = res[r][0]
+        out = res[r]
         _, (ref_l,) = _apply(table.double(), [batches[r]])
         assert out["loss"] == pytest.approx(ref_l, rel=1e-4)
         s = out["stats"]
         assert s[3] == _updates(batches[r]) and s[1] > 0 and s[2] == 0, (r, s)
-
-
-def _keys_of(b):
-    c, x, n = b
-    k = torch.cat([c, x.reshape(-1), n.reshape(-1)])
-    return torch.unique(k[k >= 0])
-
-
-def _replica_worker(kv, server, wid, table, batches):
-    rank = server.my_rank()
-    n = table.shape[0]
-    if rank == 0:
-        _load(kv, [(torch.arange(n), table)])
-    kv.waitall(); kv.barrier()
-    mine = _keys_of(batches[rank])
-    c = kv.current_clock()
-    kv.intent(mine, c, c + 1_000_000)
-    for _ in range(50):
-        kv.advance_clock()
-        _idiom(kv)
-        missing = sum(not server.is_local(int(k)) for k in mine)
-        if server.allreduce_sum([float(missing)])[0] == 0:
-            break
-    local = all(server.is_local(int(k)) for k in mine)
-    dev = server.device
-    loss = torch.zeros(1, device=dev)
-    stats = torch.zeros(4, dtype=torch.int64, device=dev)
-    stream = torch.cuda.Stream(dev)
-    for turn in range(WORLD):
-        if turn == rank:
-            _fused(server, batches[rank], loss, stats, stream)
-        _idiom(kv)
-    rows = _rows(kv, n, DIM)
-    kv.barrier()
-    kv.finalize()
-    return {"loss": float(loss.item()), "stats": stats.tolist(), "rows": rows, "local": local}
 
 
 @gpu
@@ -335,54 +249,20 @@ def test_replicas_match_float64_rule_in_turn_order():
     g = torch.Generator().manual_seed(22)
     table = _table(g, 2 * vocab, DIM)
     batches = [_distinct_batch(g, torch.arange(vocab), 40, CTX, NEG) for _ in range(WORLD)]
-    res = run_cluster(functools.partial(_replica_worker, table=table, batches=batches), world=WORLD, workers=1,
-                      mode="threads", value_lengths=2 * DIM, num_keys=2 * vocab, dtype="float32", backend="cuda",
-                      options={"sys.techniques": "replication_only"})
-    assert sum(r["counters"]["replica_setups"] for r in res.values()) > 0
-    assert all(r["counters"]["protocol_errors"] == 0 for r in res.values())
+    res = on_replicas(_case(table), batches)
+    assert sum(r["counters"]["replica_setups"] for r in res) > 0
+    assert all(r["counters"]["protocol_errors"] == 0 for r in res)
     ref, losses = _apply(table.double(), batches)
     for r in range(WORLD):
-        out = res[r][0]
+        out = res[r]
         assert out["local"], f"rank {r}: batch keys not local after the intents"
-        torch.testing.assert_close(out["rows"].double(), ref, rtol=RTOL, atol=ATOL, msg=lambda m: f"rank {r}: {m}")
+        torch.testing.assert_close(out["rows"][0].double(), ref, rtol=RTOL, atol=ATOL, msg=lambda m: f"rank {r}: {m}")
         assert out["loss"] == pytest.approx(losses[r], rel=1e-4)
         s = out["stats"]
         assert s[1] == 0 and s[2] == 0 and s[3] == _updates(batches[r]), (r, s)
 
 
 INFLIGHT_STEPS = 32
-
-
-def _inflight_worker(kv, server, wid, table, steps, done):
-    rank = server.my_rank()
-    n = table.shape[0]
-    if rank == 0:
-        _load(kv, [(torch.arange(n), table)])
-    kv.waitall(); kv.barrier()
-    out = {}
-    if rank < 2:
-        out["iters"] = _mover(kv, rank, torch.arange(n), done)
-    else:
-        dev = server.device
-        loss = torch.zeros(1, device=dev)
-        stats = torch.zeros(4, dtype=torch.int64, device=dev)
-        stream = torch.cuda.Stream(dev)
-        try:
-            for b in steps:
-                _fused(server, b, loss, stats, stream)
-                time.sleep(0.03)          # spread the steps over many sync rounds
-        finally:
-            done.set()
-        out["loss"], out["stats"] = float(loss.item()), stats.tolist()
-    kv.barrier()
-    for _ in range(8):
-        kv.advance_clock()
-    _idiom(kv)
-    if rank == 2:
-        out["rows"] = _rows(kv, n, DIM)
-    kv.barrier()
-    kv.finalize()
-    return out
 
 
 @gpu
@@ -393,20 +273,17 @@ def test_steps_lose_no_update_while_keys_move(technique):
     g = torch.Generator().manual_seed(23)
     table = _table(g, 2 * vocab, DIM)
     steps = [_distinct_batch(g, torch.arange(vocab), 16, CTX, NEG) for _ in range(INFLIGHT_STEPS)]
-    done = threading.Event()
-    res = run_cluster(functools.partial(_inflight_worker, table=table, steps=steps, done=done), world=WORLD, workers=1,
-                      mode="threads", value_lengths=2 * DIM, num_keys=2 * vocab, dtype="float32", backend="cuda",
-                      options={"sys.techniques": technique})
-    out = res[2][0]
+    res = while_keys_move(_case(table), steps, technique)
+    out = res[2]
     s = out["stats"]
-    relocations = sum(r["counters"]["relocations"] for r in res.values())
+    relocations = sum(r["counters"]["relocations"] for r in res)
     info = f"{technique}: stats {s}, relocations {relocations}"
     print(info)
     assert relocations > 0, info
-    assert all(r["counters"]["protocol_errors"] == 0 for r in res.values()), info
+    assert all(r["counters"]["protocol_errors"] == 0 for r in res), info
     assert s[3] == sum(_updates(b) for b in steps), info
     ref, losses = _apply(table.double(), steps)
-    torch.testing.assert_close(out["rows"].double(), ref, rtol=RTOL, atol=ATOL, msg=lambda m: f"{info}: {m}")
+    torch.testing.assert_close(out["rows"][0].double(), ref, rtol=RTOL, atol=ATOL, msg=lambda m: f"{info}: {m}")
     assert out["loss"] == pytest.approx(sum(losses), rel=1e-3), info
 
 

@@ -249,35 +249,24 @@ def test_default_steps_are_one_in_place_launch(cluster1):
     torch.cuda.synchronize()
 
 
-def _reject_on_two_ranks(kv, server, wid):
-    from adapm_b200.ops import kge_complex_step, mf_step
-
-    dev = server.device
-    k = torch.zeros(4, dtype=torch.int64, device=dev)
-    f = torch.zeros(4, device=dev)
-    loss = torch.zeros(1, device=dev)
-    out = []
-    try:
-        kge_complex_step(server, k, k, k, f, 4, 0.1, 0.0, 0.0, loss, deterministic=True)
-    except ValueError as e:
-        out.append(str(e))
-    try:
-        mf_step(server, k, k, f, k.int(), k.int(), 2, 0.1, 0.0, loss, deterministic=True)
-    except ValueError as e:
-        out.append(str(e))
-    kv.barrier()
-    return out
-
-
 @gpu
 def test_deterministic_steps_are_rejected_on_several_ranks():
-    from harness import run_cluster
+    from adapm_b200.ops import kge_complex_step, mf_step
+    from multirank import rejected_on_ranks
 
-    res = run_cluster(_reject_on_two_ranks, world=2, workers=1, mode="threads", value_lengths=4, num_keys=16,
-                      dtype="float32", backend="cuda")
-    for rank in (0, 1):
-        msgs = res[rank][0]
-        assert len(msgs) == 2 and all("single-GPU" in m for m in msgs), msgs
+    def args(server):
+        dev = server.device
+        return torch.zeros(4, dtype=torch.int64, device=dev), torch.zeros(4, device=dev), torch.zeros(1, device=dev)
+
+    def complex_step(server):
+        k, f, loss = args(server)
+        kge_complex_step(server, k, k, k, f, 4, 0.1, 0.0, 0.0, loss, deterministic=True)
+
+    def mf(server):
+        k, f, loss = args(server)
+        mf_step(server, k, k, f, k.int(), k.int(), 2, 0.1, 0.0, loss, deterministic=True)
+
+    assert rejected_on_ranks(complex_step, mf, value_lengths=4, num_keys=16, match="single-GPU")
 
 
 # ---------------------------------------------------------------------------------------------- apps

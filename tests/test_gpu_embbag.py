@@ -1,29 +1,15 @@
 """The fused embedding-bag kernels (csrc/cuda/ops_embbag.cu) through ``ops.StoreEmbeddingBag`` on an H100: against
 the float64 rule ``embedding_bag_reference``, bit for bit against themselves, against the torch route, in multi-hot
-DeepFM, and on multi-rank stores (three logical ranks on one GPU, as in test_gpu_fused_multirank.py): rows owned by a
-peer, local replicas and keys whose relocation is in flight."""
-import functools
-import threading
-import time
-
+DeepFM, and on multi-rank stores (three logical ranks on one GPU, run by multirank.py): rows owned by a peer,
+local replicas and keys whose relocation is in flight."""
 import numpy as np
 import pytest
 import torch
 
-from harness import run_cluster
-from test_gpu_fused_multirank import _idiom, _load, _mover
+from multirank import WORLD, Case, load_rows, on_peer_rows, on_replicas, one_rank_store, spread_keys, while_keys_move
 
 gpu = pytest.mark.gpu
-WORLD = 3
 RTOL, ATOL = 2e-4, 2e-5
-
-
-def _cuda_server(dim, num_keys, job):
-    import adapm_b200 as ad
-
-    s = ad.Server(2 * dim, num_keys=num_keys, num_threads=1, rank=0, world=1, backend="cuda", fabric="inproc",
-                  job=f"{job}_{np.random.randint(1 << 30)}", device=0)
-    return s, ad.Worker(0, s)
 
 
 def _table(num_keys, dim, g):
@@ -74,15 +60,14 @@ def test_forward_and_step_match_float64_rule(dim):
     from adapm_b200.ops import StoreEmbeddingBag, embedding_bag_reference
 
     num_keys = 20_000
-    server, kv = _cuda_server(dim, num_keys, f"bag{dim}")
-    try:
+    with one_rank_store(2 * dim, num_keys, "cuda", "float32") as (server, kv):
         for mode, weighted in MODES:
             g = torch.Generator().manual_seed(dim + 3 * weighted + 5 * (mode == "mean"))
             table = _table(num_keys, dim, g)
             keys, offsets = _hard_bags(g, num_keys)
             w = torch.rand(keys.numel(), generator=g) * 2 - 0.5 if weighted else None
             grad = torch.randn(offsets.numel() - 1, dim, generator=g) * 1e-3
-            _load(kv, [(torch.arange(num_keys), table)])
+            load_rows(kv, [(torch.arange(num_keys), table)])
             kv.waitall()
             bag = StoreEmbeddingBag(server, kv, dim, mode=mode, lr=0.05, grad_scale=7.0)
             n0 = _C.kernel_launches()
@@ -100,9 +85,6 @@ def test_forward_and_step_match_float64_rule(dim):
             torch.testing.assert_close(rows.double(), ref_table, rtol=RTOL, atol=ATOL, msg=lambda m: f"{what}: {m}")
             s = bag.stats.tolist()
             assert s[3] == torch.unique(keys).numel() and s[2] == 0 and s[1] == 0, (what, s)
-    finally:
-        kv.finalize()
-        server.shutdown()
 
 
 @gpu
@@ -110,8 +92,7 @@ def test_launch_counts():
     from adapm_b200 import _C
     from adapm_b200.ops import StoreEmbeddingBag
 
-    server, kv = _cuda_server(20, 1000, "baglaunch")
-    try:
+    with one_rank_store(2 * 20, 1000, "cuda", "float32") as (server, kv):
         bag = StoreEmbeddingBag(server, kv, 20)
         dev = server.device
         keys = torch.randint(0, 1000, (500,), device=dev)
@@ -123,9 +104,6 @@ def test_launch_counts():
         out.sum().backward()
         assert _C.kernel_launches() - n0 == 5
         torch.cuda.synchronize()
-    finally:
-        kv.finalize()
-        server.shutdown()
 
 
 def _deepfm_batch(g, B=8192, F=26, L=8, num_keys=1_000_000):
@@ -150,16 +128,12 @@ def test_two_runs_on_fresh_stores_are_bit_identical():
     table = _table(num_keys, dim, g)
     res = []
     for run in range(2):
-        server, kv = _cuda_server(dim, num_keys, f"bagdet{run}")
-        try:
-            _load(kv, [(torch.arange(num_keys), table)])
+        with one_rank_store(2 * dim, num_keys, "cuda", "float32") as (server, kv):
+            load_rows(kv, [(torch.arange(num_keys), table)])
             kv.waitall()
             bag = StoreEmbeddingBag(server, kv, dim, lr=0.05, grad_scale=8192.0)
             out = _run(kv, bag, keys, offsets, w, grad)
             res.append((out, _rows(kv, num_keys, dim)))
-        finally:
-            kv.finalize()
-            server.shutdown()
     assert torch.equal(res[0][0], res[1][0])
     assert torch.equal(res[0][1], res[1][1])
     assert not torch.equal(res[0][1], table)
@@ -177,17 +151,13 @@ def test_fused_route_matches_torch_route_at_deepfm_shape(mode):
     table = _table(num_keys, dim, g)
     res = {}
     for impl in ("fused", "torch"):
-        server, kv = _cuda_server(dim, num_keys, f"bagroute{impl}")
-        try:
-            _load(kv, [(torch.arange(num_keys), table)])
+        with one_rank_store(2 * dim, num_keys, "cuda", "float32") as (server, kv):
+            load_rows(kv, [(torch.arange(num_keys), table)])
             kv.waitall()
             bag = StoreEmbeddingBag(server, kv, dim, mode=mode, lr=0.05, grad_scale=8192.0, impl=impl)
             out = _run(kv, bag, keys, offsets, None, grad)
             kv.waitall()
             res[impl] = (out, _rows(kv, num_keys, dim))
-        finally:
-            kv.finalize()
-            server.shutdown()
     torch.testing.assert_close(res["fused"][0], res["torch"][0], rtol=1e-5, atol=1e-6)
     torch.testing.assert_close(res["fused"][1], res["torch"][1], rtol=1e-4, atol=1e-6)
 
@@ -206,8 +176,7 @@ def test_multi_hot_of_length_one_matches_single_hot_deepfm():
     out = {}
     for mh in (0, 1):
         cfg = _deepfm_cfg(mh)
-        server, kv = _cuda_server(cfg.emb_len, cfg.num_features, f"fm{mh}")
-        try:
+        with one_rank_store(2 * cfg.emb_len, cfg.num_features, "cuda", "float32") as (server, kv):
             model = DeepFM(server, kv, cfg)
             model.init_model()
             losses, first = [], None
@@ -225,9 +194,6 @@ def test_multi_hot_of_length_one_matches_single_hot_deepfm():
             kv.waitall()
             torch.cuda.synchronize()
             out[mh] = (losses, _rows(kv, cfg.num_features, cfg.emb_len), model.rows_pushed, first)
-        finally:
-            kv.finalize()
-            server.shutdown()
     np.testing.assert_allclose(out[1][0], out[0][0], rtol=1e-4)
     # after one step the rows differ by the order of the gradient sums only (amplified up to lr / sqrt(acc) = 50 x for
     # the fresh accumulators of 1e-6); later steps also see the MLPs drift apart (Adam amplifies the last-bit
@@ -242,8 +208,7 @@ def test_multi_hot_deepfm_trains_on_gpu():
     from adapm_b200.models.deepfm import DeepFM, synthetic_multi_hot_batch
 
     cfg = _deepfm_cfg(8)
-    server, kv = _cuda_server(cfg.emb_len, cfg.num_features, "fmtrain")
-    try:
+    with one_rank_store(2 * cfg.emb_len, cfg.num_features, "cuda", "float32") as (server, kv):
         model = DeepFM(server, kv, cfg)
         model.init_model()
         losses = []
@@ -254,20 +219,10 @@ def test_multi_hot_deepfm_trains_on_gpu():
         assert all(np.isfinite(losses)), losses
         assert np.mean(losses[-5:]) < np.mean(losses[:5]) - 0.02, losses
         assert model.bag.stats[3].item() == model.rows_pushed > 0
-    finally:
-        kv.finalize()
-        server.shutdown()
 
 
 # ---------------------------------------------------------------------------------------------- several ranks
 DIM = 20
-
-
-def _spread(rank, m, g):
-    """m distinct keys for ``rank``, disjoint from the other ranks' keys, 3 in 4 homed on another rank"""
-    j = torch.arange(m)
-    home = torch.where(j % 4 == 0, torch.full_like(j, rank), (rank + 1 + (j // 4) % 2) % WORLD)
-    return WORLD * (rank * m + j) + home
 
 
 def _bag_batch(pool, g, nbags=96, L=6, w=False):
@@ -277,16 +232,6 @@ def _bag_batch(pool, g, nbags=96, L=6, w=False):
     weights = torch.rand(keys.numel(), generator=g) if w else None
     grad = torch.randn(nbags, DIM, generator=g) * 1e-2
     return keys, offsets, weights, grad
-
-
-def _fused_step(server, kv, bag, b, stream):
-    keys, offsets, w, grad = b
-    dev = server.device
-    with torch.cuda.stream(stream):
-        out = bag(keys.to(dev), offsets.to(dev), w.to(dev) if w is not None else None)
-        out.backward(grad.to(dev))
-    stream.synchronize()
-    return out.detach().cpu()
 
 
 def _apply_rule(table, batches):
@@ -299,21 +244,25 @@ def _apply_rule(table, batches):
     return table, outs
 
 
-def _peer_worker(kv, server, wid, table, batches):
-    from adapm_b200.ops import StoreEmbeddingBag
+def _case(table):
+    """one forward and backward per batch through a StoreEmbeddingBag of this rank; a step returns the forward output"""
+    def open_bag(server, kv):
+        from adapm_b200.ops import StoreEmbeddingBag
 
-    rank = server.my_rank()
+        bag = StoreEmbeddingBag(server, kv, DIM, lr=0.05, grad_scale=3.0)
+        dev = server.device
+
+        def step(b):
+            keys, offsets, w, grad = b
+            out = bag(keys.to(dev), offsets.to(dev), w.to(dev) if w is not None else None)
+            out.backward(grad.to(dev))
+            return out.detach().cpu()
+
+        step.totals = lambda: (None, bag.stats.tolist())
+        return step
+
     n = table.shape[0]
-    if rank == 0:
-        _load(kv, [(torch.arange(n), table)])
-    kv.waitall(); kv.barrier()
-    bag = StoreEmbeddingBag(server, kv, DIM, lr=0.05, grad_scale=3.0)
-    out = _fused_step(server, kv, bag, batches[rank], torch.cuda.Stream(server.device))
-    kv.barrier()
-    rows = _rows(kv, n, DIM) if rank == 0 else None
-    kv.barrier()
-    kv.finalize()
-    return {"out": out, "rows": rows, "stats": bag.stats.tolist()}
+    return Case(2 * DIM, n, [(torch.arange(n), table)], lambda b: torch.unique(b[0]), open_bag)
 
 
 @gpu
@@ -323,48 +272,16 @@ def test_peer_rows_match_float64_rule():
     n = WORLD * WORLD * m
     g = torch.Generator().manual_seed(21)
     table = _table(n, DIM, g)
-    batches = [_bag_batch(_spread(r, m, g), g, w=r == 1) for r in range(WORLD)]
-    res = run_cluster(functools.partial(_peer_worker, table=table, batches=batches), world=WORLD, workers=1,
-                      mode="threads", value_lengths=2 * DIM, num_keys=n, dtype="float32", backend="cuda")
+    batches = [_bag_batch(spread_keys(r, m, g), g, w=r == 1) for r in range(WORLD)]
+    res = on_peer_rows(_case(table), batches, in_turns=False)
     ref_table, _ = _apply_rule(table, batches)
-    torch.testing.assert_close(res[0][0]["rows"].double(), ref_table, rtol=RTOL, atol=ATOL)
+    torch.testing.assert_close(res[0]["rows"][0].double(), ref_table, rtol=RTOL, atol=ATOL)
     for r in range(WORLD):
         _, (ref_out,) = _apply_rule(table, [batches[r]])
-        torch.testing.assert_close(res[r][0]["out"].double(), ref_out, rtol=RTOL, atol=ATOL)
-        s = res[r][0]["stats"]
+        torch.testing.assert_close(res[r]["outs"][0].double(), ref_out, rtol=RTOL, atol=ATOL)
+        s = res[r]["stats"]
         keys = batches[r][0]
         assert s[3] == torch.unique(keys).numel() and s[1] > 0 and s[2] == 0, (r, s)
-
-
-def _replica_worker(kv, server, wid, table, batches):
-    from adapm_b200.ops import StoreEmbeddingBag
-
-    rank = server.my_rank()
-    n = table.shape[0]
-    if rank == 0:
-        _load(kv, [(torch.arange(n), table)])
-    kv.waitall(); kv.barrier()
-    mine = torch.unique(batches[rank][0])
-    c = kv.current_clock()
-    kv.intent(mine, c, c + 1_000_000)
-    for _ in range(50):
-        kv.advance_clock()
-        _idiom(kv)
-        missing = sum(not server.is_local(int(k)) for k in mine)
-        if server.allreduce_sum([float(missing)])[0] == 0:
-            break
-    local = all(server.is_local(int(k)) for k in mine)
-    bag = StoreEmbeddingBag(server, kv, DIM, lr=0.05, grad_scale=3.0)
-    stream = torch.cuda.Stream(server.device)
-    out = None
-    for turn in range(WORLD):
-        if turn == rank:
-            out = _fused_step(server, kv, bag, batches[rank], stream)
-        _idiom(kv)
-    rows = _rows(kv, n, DIM)
-    kv.barrier()
-    kv.finalize()
-    return {"out": out, "rows": rows, "stats": bag.stats.tolist(), "local": local}
 
 
 @gpu
@@ -376,55 +293,21 @@ def test_replicas_match_float64_rule_in_turn_order():
     table = _table(n, DIM, g)
     pool = torch.arange(n)
     batches = [_bag_batch(pool[torch.randperm(n, generator=g)[:200]], g) for _ in range(WORLD)]
-    res = run_cluster(functools.partial(_replica_worker, table=table, batches=batches), world=WORLD, workers=1,
-                      mode="threads", value_lengths=2 * DIM, num_keys=n, dtype="float32", backend="cuda",
-                      options={"sys.techniques": "replication_only"})
-    assert sum(r["counters"]["replica_setups"] for r in res.values()) > 0
-    assert all(r["counters"]["protocol_errors"] == 0 for r in res.values())
+    res = on_replicas(_case(table), batches)
+    assert sum(r["counters"]["replica_setups"] for r in res) > 0
+    assert all(r["counters"]["protocol_errors"] == 0 for r in res)
     ref_table, ref_outs = _apply_rule(table, batches)
     for r in range(WORLD):
-        out = res[r][0]
+        out = res[r]
         assert out["local"], f"rank {r}: batch keys not local after the intents"
-        torch.testing.assert_close(out["rows"].double(), ref_table, rtol=RTOL, atol=ATOL, msg=lambda m: f"rank {r}: {m}")
-        torch.testing.assert_close(out["out"].double(), ref_outs[r], rtol=RTOL, atol=ATOL)
+        torch.testing.assert_close(out["rows"][0].double(), ref_table, rtol=RTOL, atol=ATOL,
+                                   msg=lambda m: f"rank {r}: {m}")
+        torch.testing.assert_close(out["outs"][0].double(), ref_outs[r], rtol=RTOL, atol=ATOL)
         s = out["stats"]
         assert s[1] == 0 and s[2] == 0 and s[3] == torch.unique(batches[r][0]).numel(), (r, s)
 
 
 INFLIGHT_STEPS = 32
-
-
-def _inflight_worker(kv, server, wid, table, steps, done):
-    from adapm_b200.ops import StoreEmbeddingBag
-
-    rank = server.my_rank()
-    n = table.shape[0]
-    if rank == 0:
-        _load(kv, [(torch.arange(n), table)])
-    kv.waitall(); kv.barrier()
-    out = {}
-    if rank < 2:
-        out["iters"] = _mover(kv, rank, torch.arange(n), done)
-    else:
-        bag = StoreEmbeddingBag(server, kv, DIM, lr=0.05, grad_scale=3.0)
-        stream = torch.cuda.Stream(server.device)
-        outs = []
-        try:
-            for b in steps:
-                outs.append(_fused_step(server, kv, bag, b, stream))
-                time.sleep(0.03)          # spread the steps over many sync rounds
-        finally:
-            done.set()
-        out["outs"], out["stats"] = outs, bag.stats.tolist()
-    kv.barrier()
-    for _ in range(8):
-        kv.advance_clock()
-    _idiom(kv)
-    if rank == 2:
-        out["rows"] = _rows(kv, n, DIM)
-    kv.barrier()
-    kv.finalize()
-    return out
 
 
 @gpu
@@ -435,19 +318,16 @@ def test_steps_lose_no_update_while_keys_move(technique):
     g = torch.Generator().manual_seed(23)
     table = _table(n, DIM, g)
     steps = [_bag_batch(torch.arange(n), g, nbags=64, w=i % 2 == 1) for i in range(INFLIGHT_STEPS)]
-    done = threading.Event()
-    res = run_cluster(functools.partial(_inflight_worker, table=table, steps=steps, done=done), world=WORLD, workers=1,
-                      mode="threads", value_lengths=2 * DIM, num_keys=n, dtype="float32", backend="cuda",
-                      options={"sys.techniques": technique})
-    out = res[2][0]
+    res = while_keys_move(_case(table), steps, technique)
+    out = res[2]
     s = out["stats"]
-    relocations = sum(r["counters"]["relocations"] for r in res.values())
+    relocations = sum(r["counters"]["relocations"] for r in res)
     info = f"{technique}: stats {s}, relocations {relocations}"
     print(info)
     assert relocations > 0, info
-    assert all(r["counters"]["protocol_errors"] == 0 for r in res.values()), info
+    assert all(r["counters"]["protocol_errors"] == 0 for r in res), info
     assert s[3] == sum(torch.unique(b[0]).numel() for b in steps), info
     ref_table, ref_outs = _apply_rule(table, steps)
-    torch.testing.assert_close(out["rows"].double(), ref_table, rtol=RTOL, atol=ATOL, msg=lambda m: f"{info}: {m}")
+    torch.testing.assert_close(out["rows"][0].double(), ref_table, rtol=RTOL, atol=ATOL, msg=lambda m: f"{info}: {m}")
     for i, (o, r) in enumerate(zip(out["outs"], ref_outs)):
         torch.testing.assert_close(o.double(), r, rtol=RTOL, atol=ATOL, msg=lambda m: f"{info}, step {i}: {m}")

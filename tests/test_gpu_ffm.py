@@ -2,17 +2,11 @@
 ``ffm_reference_forward`` (float64): at every backward instantiation, at the edges of the envelope and with a batch that
 wraps the forward's grid; bit-identical runs; one push per distinct key; on three logical ranks of one GPU (peer rows,
 replicas, keys in flight); quality on the planted data of the CPU test."""
-import functools
-import threading
-import time
-
-import numpy as np
 import pytest
 import torch
 
-from harness import run_cluster
+from multirank import WORLD, Case, on_peer_rows, on_replicas, one_rank_store, while_keys_move
 from test_ffm_cpu import QUALITY_MIN_AUC_GAIN, QUALITY_MIN_LOGLOSS_GAIN, base_rate_logloss, train_ffm_quality
-from test_gpu_fused_multirank import WORLD, _idiom, _mover
 
 gpu = pytest.mark.gpu
 ETA, LAM = 0.2, 1e-3
@@ -36,38 +30,18 @@ def _batch(F, per_field, B, g):
     return ids, (torch.rand(B, generator=g) < 0.5).float()
 
 
-def _cpu_store(row_len, n):
-    import adapm_b200 as ad
-
-    s = ad.Server(row_len, num_keys=n, num_threads=1, rank=0, world=1, backend="cpu", fabric="inproc",
-                  job=f"ffm_ref_{np.random.randint(1 << 30)}", dtype="float64")
-    return s, ad.Worker(0, s)
-
-
 def _rule(table, batches, k, r):
     """the batches applied in order by the float64 rule; returns (rows, losses, logits of the first batch)"""
     from adapm_b200.ops import ffm_reference_forward, ffm_reference_step
 
     n, L = table.shape
-    s, kv = _cpu_store(L, n)
-    try:
+    with one_rank_store(L, n, "cpu", "float64") as (s, kv):
         kv.wait(kv.set(torch.arange(n), table.contiguous().view(-1)))
         logits = ffm_reference_forward(kv, batches[0][0], k, r)
         losses = [ffm_reference_step(kv, ids, y, k, ETA, LAM, r) for ids, y in batches]
         rows = torch.empty(n * L, dtype=torch.float64)
         kv.wait(kv.pull(torch.arange(n), rows))
         return rows.view(n, L), losses, logits
-    finally:
-        kv.finalize()
-        s.shutdown()
-
-
-def _gpu_store(row_len, n):
-    import adapm_b200 as ad
-
-    s = ad.Server(row_len, num_keys=n, num_threads=1, rank=0, world=1, backend="cuda", fabric="inproc",
-                  job=f"ffm_gpu_{np.random.randint(1 << 30)}", device=0)
-    return s, ad.Worker(0, s)
 
 
 def _fused(table, batches, F, k, r):
@@ -75,8 +49,7 @@ def _fused(table, batches, F, k, r):
     from adapm_b200.ops import StoreFFM
 
     n, L = table.shape
-    s, kv = _gpu_store(L, n)
-    try:
+    with one_rank_store(L, n, "cuda", "float32") as (s, kv):
         kv.wait(kv.set(torch.arange(n), table.float().contiguous().view(-1)))
         kv.waitall()
         torch.cuda.synchronize()
@@ -88,9 +61,6 @@ def _fused(table, batches, F, k, r):
         rows = torch.empty(n * L)
         kv.wait(kv.pull(torch.arange(n), rows))
         return rows.view(n, L).double(), [float(x) for x in losses], logits, op.stats.tolist()
-    finally:
-        kv.finalize()
-        s.shutdown()
 
 
 def _tolerances(F, k, batches):
@@ -155,8 +125,7 @@ def test_step_arguments_are_checked():
     from adapm_b200.ops import StoreFFM
 
     F, k = 4, 4
-    s, kv = _gpu_store(2 * (4 + F * k), 64)
-    try:
+    with one_rank_store(2 * (4 + F * k), 64, "cuda", "float32") as (s, kv):
         dev = s.device
         op = StoreFFM(s, F, k)
         ids, y = torch.zeros(8, F, dtype=torch.int64, device=dev), torch.zeros(8, device=dev)
@@ -169,9 +138,6 @@ def test_step_arguments_are_checked():
         for kw in (dict(k=8), dict(num_fields=3), dict(eta=-1.0), dict(lam=-1.0)):
             with pytest.raises(ValueError):
                 StoreFFM(s, **(dict(num_fields=F, k=k) | kw))
-    finally:
-        kv.finalize()
-        s.shutdown()
 
 
 @gpu
@@ -187,38 +153,23 @@ def test_quality_on_planted_data_passes_the_cpu_threshold():
 F3, K3, PF3 = 8, 8, 40
 
 
-def _run_steps(server, batches, stream):
-    from adapm_b200.ops import StoreFFM
+def _case(table):
+    """one StoreFFM step per batch; a step returns its loss"""
+    def open_ffm(server, kv):
+        from adapm_b200.ops import StoreFFM
 
-    op = StoreFFM(server, F3, K3, ETA, LAM, 1.0 / F3)
-    dev = server.device
-    losses = []
-    with torch.cuda.stream(stream):
-        for ids, y in batches:
-            losses.append(float(op.step(ids.to(dev), y.to(dev))))
-            stream.synchronize()
-    return losses, op.stats.tolist()
+        op = StoreFFM(server, F3, K3, ETA, LAM, 1.0 / F3)
+        dev = server.device
 
+        def step(b):
+            ids, y = b
+            return float(op.step(ids.to(dev), y.to(dev)))
 
-def _peer_worker(kv, server, wid, table, batches):
-    rank = server.my_rank()
+        step.totals = lambda: (None, op.stats.tolist())
+        return step
+
     n = table.shape[0]
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(n), table.float().contiguous().view(-1)))
-    kv.waitall(); kv.barrier()
-    stream = torch.cuda.Stream(server.device)
-    out = {}
-    for turn in range(WORLD):                         # one rank at a time, in rank order
-        if turn == rank:
-            out["losses"], out["stats"] = _run_steps(server, [batches[rank]], stream)
-        _idiom(kv)
-    if rank == 0:
-        rows = torch.empty(n * table.shape[1])
-        kv.wait(kv.pull(torch.arange(n), rows))
-        out["rows"] = rows.view(n, -1).double()
-    kv.barrier()
-    kv.finalize()
-    return out
+    return Case(table.shape[1], n, [(torch.arange(n), table)], lambda b: torch.unique(b[0]), open_ffm)
 
 
 @gpu
@@ -227,47 +178,16 @@ def test_step_on_peer_rows():
     g = torch.Generator().manual_seed(5)
     table = _table(F3 * PF3, F3, K3, g)
     batches = [_batch(F3, PF3, 256, g) for _ in range(WORLD)]
-    res = run_cluster(functools.partial(_peer_worker, table=table, batches=batches), world=WORLD, workers=1,
-                      mode="threads", value_lengths=table.shape[1], num_keys=table.shape[0], dtype="float32",
-                      backend="cuda")
+    res = on_peer_rows(_case(table), batches, in_turns=True)
     ref, ref_losses, _ = _rule(table, batches, K3, 1.0 / F3)
     tol_v, tol_a, _ = _tolerances(F3, K3, batches)
     E = 4 + F3 * K3
-    assert sum(x[0]["stats"][3] for x in res.values()) == sum(int(torch.unique(i).numel()) for i, _ in batches)
-    assert sum(x[0]["stats"][1] for x in res.values()) > 0
-    torch.testing.assert_close(res[0][0]["rows"][:, :E], ref[:, :E], rtol=0, atol=tol_v)
-    torch.testing.assert_close(res[0][0]["rows"][:, E:], ref[:, E:], rtol=tol_a, atol=0)
-    torch.testing.assert_close(sum(x[0]["losses"][0] for x in res.values()), sum(ref_losses), rtol=1e-4, atol=1e-3)
-
-
-def _replica_worker(kv, server, wid, table, batches):
-    rank = server.my_rank()
-    n = table.shape[0]
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(n), table.float().contiguous().view(-1)))
-    kv.waitall(); kv.barrier()
-    mine = torch.unique(batches[rank][0])
-    c = kv.current_clock()
-    kv.intent(mine, c, c + 1_000_000)
-    for _ in range(50):
-        kv.advance_clock()
-        _idiom(kv)
-        missing = sum(not server.is_local(int(k)) for k in mine)
-        if server.allreduce_sum([float(missing)])[0] == 0:
-            break
-    out = {"local": all(server.is_local(int(k)) for k in mine),
-           "replicas": sum(server.owner_of(int(k)) != rank for k in mine)}
-    stream = torch.cuda.Stream(server.device)
-    for turn in range(WORLD):
-        if turn == rank:
-            out["losses"], out["stats"] = _run_steps(server, [batches[rank]], stream)
-        _idiom(kv)
-    rows = torch.empty(n * table.shape[1])
-    kv.wait(kv.pull(torch.arange(n), rows))
-    out["rows"] = rows.view(n, -1).double()
-    kv.barrier()
-    kv.finalize()
-    return out
+    rows = res[0]["rows"][0].double()
+    assert sum(x["stats"][3] for x in res) == sum(int(torch.unique(i).numel()) for i, _ in batches)
+    assert sum(x["stats"][1] for x in res) > 0
+    torch.testing.assert_close(rows[:, :E], ref[:, :E], rtol=0, atol=tol_v)
+    torch.testing.assert_close(rows[:, E:], ref[:, E:], rtol=tol_a, atol=0)
+    torch.testing.assert_close(sum(x["outs"][0] for x in res), sum(ref_losses), rtol=1e-4, atol=1e-3)
 
 
 @gpu
@@ -277,58 +197,19 @@ def test_step_on_replicas():
     g = torch.Generator().manual_seed(21)
     table = _table(F3 * PF3, F3, K3, g)
     batches = [_batch(F3, PF3, 128, g) for _ in range(WORLD)]
-    res = run_cluster(functools.partial(_replica_worker, table=table, batches=batches), world=WORLD, workers=1,
-                      mode="threads", value_lengths=table.shape[1], num_keys=table.shape[0], dtype="float32",
-                      backend="cuda", options={"sys.techniques": "replication_only"})
-    assert sum(x["counters"]["replica_setups"] for x in res.values()) > 0
-    assert all(x["counters"]["protocol_errors"] == 0 for x in res.values())
+    res = on_replicas(_case(table), batches)
+    assert sum(x["counters"]["replica_setups"] for x in res) > 0
+    assert all(x["counters"]["protocol_errors"] == 0 for x in res)
     ref, _, _ = _rule(table, batches, K3, 1.0 / F3)
     tol_v, tol_a, _ = _tolerances(F3, K3, batches)
     E = 4 + F3 * K3
     for k in range(WORLD):
-        out = res[k][0]
+        out = res[k]
+        rows = out["rows"][0].double()
         assert out["local"] and out["replicas"] > 0, f"rank {k}: batch keys not local after the intents"
-        torch.testing.assert_close(out["rows"][:, :E], ref[:, :E], rtol=0, atol=tol_v)
-        torch.testing.assert_close(out["rows"][:, E:], ref[:, E:], rtol=tol_a, atol=0)
+        torch.testing.assert_close(rows[:, :E], ref[:, :E], rtol=0, atol=tol_v)
+        torch.testing.assert_close(rows[:, E:], ref[:, E:], rtol=tol_a, atol=0)
         assert out["stats"][1] == 0 and out["stats"][2] == 0, (k, out["stats"])
-
-
-def _inflight_worker(kv, server, wid, table, batches, done):
-    rank = server.my_rank()
-    n = table.shape[0]
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(n), table.float().contiguous().view(-1)))
-    kv.waitall(); kv.barrier()
-    out = {}
-    if rank < 2:
-        out["iters"] = _mover(kv, rank, torch.arange(n), done)
-    else:
-        stream = torch.cuda.Stream(server.device)
-        try:
-            out["losses"], out["stats"] = [], None
-            from adapm_b200.ops import StoreFFM
-
-            op = StoreFFM(server, F3, K3, ETA, LAM, 1.0 / F3)
-            dev = server.device
-            with torch.cuda.stream(stream):
-                for ids, y in batches:
-                    out["losses"].append(float(op.step(ids.to(dev), y.to(dev))))
-                    stream.synchronize()
-                    time.sleep(0.03)
-            out["stats"] = op.stats.tolist()
-        finally:
-            done.set()
-    kv.barrier()
-    for _ in range(8):
-        kv.advance_clock()
-    _idiom(kv)
-    if rank == 2:
-        rows = torch.empty(n * table.shape[1])
-        kv.wait(kv.pull(torch.arange(n), rows))
-        out["rows"] = rows.view(n, -1).double()
-    kv.barrier()
-    kv.finalize()
-    return out
 
 
 @gpu
@@ -338,19 +219,17 @@ def test_step_loses_no_update_while_keys_move(technique):
     g = torch.Generator().manual_seed(9)
     table = _table(F3 * PF3, F3, K3, g)
     batches = [_batch(F3, PF3, 64, g) for _ in range(24)]
-    done = threading.Event()
-    res = run_cluster(functools.partial(_inflight_worker, table=table, batches=batches, done=done), world=WORLD,
-                      workers=1, mode="threads", value_lengths=table.shape[1], num_keys=table.shape[0],
-                      dtype="float32", backend="cuda", options={"sys.techniques": technique})
-    out = res[2][0]
-    relocations = sum(x["counters"]["relocations"] for x in res.values())
+    res = while_keys_move(_case(table), batches, technique)
+    out = res[2]
+    relocations = sum(x["counters"]["relocations"] for x in res)
     info = f"{technique}: stats {out['stats']}, relocations {relocations}"
     print(info)
-    assert relocations > 0 and all(x["counters"]["protocol_errors"] == 0 for x in res.values()), info
+    assert relocations > 0 and all(x["counters"]["protocol_errors"] == 0 for x in res), info
     ref, ref_losses, _ = _rule(table, batches, K3, 1.0 / F3)
     tol_v, tol_a, _ = _tolerances(F3, K3, batches)
     E = 4 + F3 * K3
+    rows = out["rows"][0].double()
     assert out["stats"][3] == sum(int(torch.unique(i).numel()) for i, _ in batches), info
-    torch.testing.assert_close(out["rows"][:, :E], ref[:, :E], rtol=0, atol=tol_v)
-    torch.testing.assert_close(out["rows"][:, E:], ref[:, E:], rtol=tol_a, atol=0)
-    torch.testing.assert_close(sum(out["losses"]), sum(ref_losses), rtol=1e-4, atol=1e-3)
+    torch.testing.assert_close(rows[:, :E], ref[:, :E], rtol=0, atol=tol_v)
+    torch.testing.assert_close(rows[:, E:], ref[:, E:], rtol=tol_a, atol=0)
+    torch.testing.assert_close(sum(out["outs"]), sum(ref_losses), rtol=1e-4, atol=1e-3)

@@ -4,12 +4,7 @@ flight, and the in-place word2vec step of one GPU.
 Every fused op resolves each row to one of four outcomes (``dev::resolve_fast`` in ``pm_kernels.cuh``): a local owned
 row, a local replica (the update also sets the dirty byte), a peer's owned row (the update bumps the owner's version) or
 none, for a key in a transitional state, which takes the generic out-of-line path. On several GPUs these branches are
-the hot path. All of this runs here on ONE device: ``run_cluster(mode="threads")`` runs three logical ranks in this
-process, with the inproc fabric and peer pointers into the same HBM; the initial owner of key ``k`` is ``k % world``,
-so remote keys are chosen on purpose.
-
-Every rank runs its fused ops on a CUDA stream of its own, so that one rank's kernels do not queue behind another
-rank's on the legacy default stream (which synchronises with every other blocking stream of the device).
+the hot path. The scenarios (three logical ranks on one GPU) are the runners of ``multirank.py``; ``Op`` is their case.
 
 Training steps are compared with the float64 rule (``kge_reference_step``, ``mf_reference_step`` and
 ``sgns_reference_step`` below, applied through a float64 CPU store), gathers bit for bit with the same op on a
@@ -19,18 +14,17 @@ import functools
 import os
 import subprocess
 import sys
-import threading
-import time
 
 import numpy as np
 import pytest
 import torch
 
 from harness import run_cluster
+from multirank import (WORLD, Case, Fused, load_rows, make_local, on_peer_rows, on_replicas, one_rank_store, pull_rows,
+                       reads_while_keys_move, spread_keys, while_keys_move)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 gpu = pytest.mark.gpu
-WORLD = 3
 RTOL, ATOL = 2e-4, 2e-5
 
 
@@ -69,7 +63,8 @@ def sgns_reference_step(kv, centers, contexts, negatives, d, alpha):
 
 
 class Op:
-    """One fused training op at one shape: store layout, batches of distinct keys, the fused call and its reference.
+    """One fused training op at one shape: store layout, batches of distinct keys, the fused call and its reference; with
+    ``init`` set, a case of the ``multirank`` runners.
 
     ``kind``: ``sgns`` (d, neg, impl, B), ``complex`` / ``rescal`` (d = embed_dim, p_e, p_r, n calls) or ``mf`` (d = rank,
     n non-zeros). Entity keys (all keys for sgns / mf) are ``[0, ne)``, relation keys ``[ne, ne + nr)``."""
@@ -77,6 +72,7 @@ class Op:
     def __init__(self, kind, d, neg=0, impl="auto", n=32, p_e=0.0, p_r=0.0, ne=0, nr=0, lr=None):
         self.kind, self.d, self.neg, self.impl, self.n, self.p_e, self.p_r = kind, d, neg, impl, n, p_e, p_r
         self.ne, self.nr = ne, nr
+        self.init = None
         self.lr = lr if lr is not None else {"sgns": 0.05, "complex": 0.1, "rescal": 0.1, "mf": 0.05}[kind]
 
     def __repr__(self):
@@ -107,6 +103,7 @@ class Op:
     def rel_len(self):
         return self.cfg.relation_len if self.kge else 2 * self.d
 
+    @property
     def value_lengths(self):
         return self.cfg.value_lengths() if self.kge else 2 * self.d
 
@@ -175,6 +172,9 @@ class Op:
         return 0
 
     # ---- the fused op and its rule
+    def open(self, server, kv):
+        return Fused(server, self.fused)
+
     def fused(self, server, b, loss, stats):
         from adapm_b200.ops import kge_complex_step, kge_rescal_step, mf_step, sgns_step
 
@@ -213,36 +213,13 @@ class Op:
         return mf_reference_step(kv, b["rk"], b["ck"], b["x"], ones, ones, self.d, self.lr, 0.02)
 
 
-def _load(kv, groups):
-    for keys, rows in groups:
-        kv.wait(kv.set(keys, rows.to(kv.server.dtype).contiguous().view(-1)))
-
-
-def _pull_groups(kv, groups, dtype=torch.float32):
-    out = []
-    for keys, rows in groups:
-        v = torch.empty(rows.numel(), dtype=dtype)
-        kv.wait(kv.pull(keys, v))
-        out.append(v.view(rows.shape))
-    return out
-
-
-def _cpu_f64(op, job):
-    import adapm_b200 as ad
-
-    s = ad.Server(op.value_lengths(), num_keys=op.num_keys, num_threads=1, rank=0, world=1, backend="cpu",
-                  fabric="inproc", job=f"{job}_{np.random.randint(1 << 30)}", dtype="float64")
-    return s, ad.Worker(0, s)
-
-
 def reference_run(op, init, steps, drop=None, stale=None):
     """Applies ``steps`` (batches) one after another by the float64 rule, from the rows ``init``. Returns (rows per key
     group, summed loss). Negative controls: ``drop = (step, call)`` leaves one call out; ``stale = (step, key)`` lets
     step ``step`` read row ``key`` as it was before step ``step - 1`` (the update of ``step - 1`` to that row itself is
     kept)."""
-    server, kv = _cpu_f64(op, "ref")
-    try:
-        _load(kv, init)
+    with one_rank_store(op.value_lengths, op.num_keys, "cpu", "float64") as (_, kv):
+        load_rows(kv, init)
         loss, snap = 0.0, None
         for i, b in enumerate(steps):
             if drop is not None and drop[0] == i:
@@ -261,10 +238,7 @@ def reference_run(op, init, steps, drop=None, stale=None):
                 kv.wait(kv.set(k, cur + (new - snap)))
             else:
                 loss += op.reference(kv, b)
-        return _pull_groups(kv, init, torch.float64), loss
-    finally:
-        kv.finalize()
-        server.shutdown()
+        return pull_rows(kv, init, torch.float64), loss
 
 
 def _assert_rows(got, ref, what):
@@ -272,40 +246,7 @@ def _assert_rows(got, ref, what):
         torch.testing.assert_close(a.double(), b, rtol=RTOL, atol=ATOL, msg=lambda m: f"{what}, key group {i}: {m}")
 
 
-def _idiom(kv):
-    kv.waitall(); kv.wait_sync(); kv.barrier(); kv.wait_sync(); kv.barrier()
-
-
-def _spread_keys(rank, m, g):
-    """m distinct keys for ``rank``, disjoint from the other ranks' keys, 3 in 4 of them homed on another rank (the
-    initial owner of key k is k % world): keys < world * world * m."""
-    j = torch.arange(m)
-    home = torch.where(j % 4 == 0, torch.full_like(j, rank), (rank + 1 + (j // 4) % 2) % WORLD)
-    keys = WORLD * (rank * m + j) + home
-    return keys[torch.randperm(m, generator=g)]
-
-
 # ---------------------------------------------------------------------------------------------- 1. peer rows
-def _peer_worker(kv, server, wid, op, init, batches):
-    rank = server.my_rank()
-    remote = sum(server.owner_of(int(k)) != rank for k in op.keys_of(batches[rank]))
-    if rank == 0:
-        _load(kv, init)
-    kv.waitall(); kv.barrier()
-    dev = server.device
-    loss = torch.zeros(1, device=dev)
-    stats = torch.zeros(4, dtype=torch.int64, device=dev)
-    stream = torch.cuda.Stream(dev)
-    with torch.cuda.stream(stream):
-        op.fused(server, batches[rank], loss, stats)
-    stream.synchronize()
-    kv.barrier()
-    rows = _pull_groups(kv, init) if rank == 0 else None
-    kv.barrier()
-    kv.finalize()
-    return {"loss": float(loss.item()), "stats": stats.tolist(), "rows": rows, "remote": remote}
-
-
 PEER_OPS = [Op("sgns", 64, 5, "tma", n=64), Op("sgns", 200, 30, "tma", n=64), Op("sgns", 300, 25, "tma", n=64),
             Op("sgns", 336, 3, "tma", n=64), Op("sgns", 128, 5, "ldg", n=64), Op("sgns", 512, 3, "ldg", n=64),
             Op("sgns", 64, 40, "auto", n=64),
@@ -322,18 +263,16 @@ def test_fused_steps_on_peer_rows_match_float64_rule(op):
     ne_need, nr_need = op.need()
     op = op.sized(WORLD * WORLD * ne_need, WORLD * WORLD * nr_need)
     g = torch.Generator().manual_seed(op.d * 7 + op.neg + int(100 * op.p_e))
-    init = op.init_rows(g)
-    batches = [op.batch(_spread_keys(r, ne_need, g), op.ne + _spread_keys(r, nr_need, g) if nr_need else None, g,
+    op.init = op.init_rows(g)
+    batches = [op.batch(spread_keys(r, ne_need, g), op.ne + spread_keys(r, nr_need, g) if nr_need else None, g,
                         seed=0x5EED + r) for r in range(WORLD)]
-    res = run_cluster(functools.partial(_peer_worker, op=op, init=init, batches=batches), world=WORLD, workers=1,
-                      mode="threads", value_lengths=op.value_lengths(), num_keys=op.num_keys, dtype="float32",
-                      backend="cuda")
-    ref_rows, ref_loss = reference_run(op, init, batches)
-    _assert_rows(res[0][0]["rows"], ref_rows, repr(op))
+    res = on_peer_rows(op, batches, in_turns=False)
+    ref_rows, ref_loss = reference_run(op, op.init, batches)
+    _assert_rows(res[0]["rows"], ref_rows, repr(op))
     for r in range(WORLD):
-        out = res[r][0]
+        out = res[r]
         b = batches[r]
-        ref_l = reference_run(op, init, [b])[1]
+        ref_l = reference_run(op, op.init, [b])[1]
         torch.testing.assert_close(out["loss"], ref_l, rtol=1e-3 if op.kind == "sgns" else 1e-4, atol=1e-3)
         s = out["stats"]
         assert 3 * out["remote"] >= 2 * op.updates(b), out["remote"]
@@ -342,37 +281,6 @@ def test_fused_steps_on_peer_rows_match_float64_rule(op):
 
 
 # ---------------------------------------------------------------------------------------------- 2. replica rows
-def _replica_worker(kv, server, wid, op, init, batches):
-    rank = server.my_rank()
-    if rank == 0:
-        _load(kv, init)
-    kv.waitall(); kv.barrier()
-    mine = op.keys_of(batches[rank])
-    c = kv.current_clock()
-    kv.intent(mine, c, c + 1_000_000)
-    for _ in range(50):
-        kv.advance_clock()
-        _idiom(kv)
-        missing = sum(not server.is_local(int(k)) for k in mine)
-        if server.allreduce_sum([float(missing)])[0] == 0:
-            break
-    local = all(server.is_local(int(k)) for k in mine)
-    dev = server.device
-    loss = torch.zeros(1, device=dev)
-    stats = torch.zeros(4, dtype=torch.int64, device=dev)
-    stream = torch.cuda.Stream(dev)
-    for turn in range(WORLD):
-        if turn == rank:
-            with torch.cuda.stream(stream):
-                op.fused(server, batches[rank], loss, stats)
-            stream.synchronize()
-        _idiom(kv)
-    rows = _pull_groups(kv, init)
-    kv.barrier()
-    kv.finalize()
-    return {"loss": float(loss.item()), "stats": stats.tolist(), "rows": rows, "local": local}
-
-
 REPLICA_OPS = [Op("sgns", 300, 25, "tma", n=32), Op("complex", 128), Op("rescal", 32), Op("mf", 64)]
 
 
@@ -386,18 +294,16 @@ def test_fused_steps_on_replicas_match_float64_rule(op):
     ne_need, nr_need = op.need()
     op = op.sized(2 * ne_need, 2 * nr_need)
     g = torch.Generator().manual_seed(op.d + 11)
-    init = op.init_rows(g)
+    op.init = op.init_rows(g)
     batches = [op.batch(torch.randperm(op.ne, generator=g)[:ne_need],
                         op.ne + torch.randperm(op.nr, generator=g)[:nr_need] if nr_need else None, g, seed=0x7E + r)
                for r in range(WORLD)]
-    res = run_cluster(functools.partial(_replica_worker, op=op, init=init, batches=batches), world=WORLD, workers=1,
-                      mode="threads", value_lengths=op.value_lengths(), num_keys=op.num_keys, dtype="float32",
-                      backend="cuda", options={"sys.techniques": "replication_only"})
-    assert sum(r["counters"]["replica_setups"] for r in res.values()) > 0
-    assert all(r["counters"]["protocol_errors"] == 0 for r in res.values())
-    ref_rows, _ = reference_run(op, init, batches)
+    res = on_replicas(op, batches)
+    assert sum(r["counters"]["replica_setups"] for r in res) > 0
+    assert all(r["counters"]["protocol_errors"] == 0 for r in res)
+    ref_rows, _ = reference_run(op, op.init, batches)
     for r in range(WORLD):
-        out = res[r][0]
+        out = res[r]
         assert out["local"], f"rank {r}: batch keys not local after the intents"
         _assert_rows(out["rows"], ref_rows, f"{op}, rows read on rank {r}")
         s = out["stats"]
@@ -405,67 +311,13 @@ def test_fused_steps_on_replicas_match_float64_rule(op):
         assert s[0] == n_rows and s[1] == 0 and s[2] == op.slow_calls() and s[3] == n_rows, (r, s)
     # each rank's loss: its step on the state left by the ranks before it
     for r in range(WORLD):
-        _, before = reference_run(op, init, batches[:r])
-        _, upto = reference_run(op, init, batches[:r + 1])
-        torch.testing.assert_close(res[r][0]["loss"], upto - before, rtol=1e-3 if op.kind == "sgns" else 1e-4, atol=1e-3)
+        _, before = reference_run(op, op.init, batches[:r])
+        _, upto = reference_run(op, op.init, batches[:r + 1])
+        torch.testing.assert_close(res[r]["loss"], upto - before, rtol=1e-3 if op.kind == "sgns" else 1e-4, atol=1e-3)
 
 
 # ---------------------------------------------------------------------------------------------- 3. keys in flight
 INFLIGHT_STEPS = 32
-MOVER_MIN_ITERS = 60
-
-
-def _mover(kv, rank, block, done, max_iters=3000):
-    """Ranks 0 and 1 pass ``block`` back and forth with intents (read-only: they never write a row) until ``done``."""
-    probe = block[:4]
-    buf = torch.zeros(kv.server.total_len(probe), dtype=kv.server.dtype)
-    it = 0
-    while (it < MOVER_MIN_ITERS or not done.is_set()) and it < max_iters:
-        if it % 2 == rank:
-            kv.intent(block, kv.current_clock(), kv.current_clock() + 3)
-            if it % 16 < 2:
-                kv.wait_sync()
-        for _ in range(3):
-            kv.advance_clock()
-        kv.wait(kv.pull(probe, buf))
-        it += 1
-    return it
-
-
-def _inflight_train_worker(kv, server, wid, op, init, steps, done):
-    rank = server.my_rank()
-    if rank == 0:
-        _load(kv, init)
-    kv.waitall(); kv.barrier()
-    block = torch.cat([k for k, _ in init])
-    out = {}
-    if rank < 2:
-        out["iters"] = _mover(kv, rank, block, done)
-    else:
-        dev = server.device
-        loss = torch.zeros(1, device=dev)
-        stats = torch.zeros(4, dtype=torch.int64, device=dev)
-        stream = torch.cuda.Stream(dev)
-        try:
-            with torch.cuda.stream(stream):
-                for b in steps:
-                    op.fused(server, b, loss, stats)
-                    stream.synchronize()
-                    time.sleep(0.03)         # spread the steps over many sync rounds
-        finally:
-            done.set()
-        out["loss"], out["stats"] = float(loss.item()), stats.tolist()
-    kv.barrier()
-    for _ in range(8):
-        kv.advance_clock()
-    _idiom(kv)
-    if rank == 2:
-        out["rows"] = _pull_groups(kv, init)
-    kv.barrier()
-    kv.finalize()
-    return out
-
-
 INFLIGHT_OPS = {"sgns": lambda: Op("sgns", 64, 5, "tma", n=32, ne=448),
                 "ldg": lambda: Op("sgns", 128, 5, "ldg", n=32, ne=448),
                 "complex": lambda: Op("complex", 128, n=32, ne=96, nr=48),
@@ -523,20 +375,17 @@ def test_fused_steps_lose_no_update_while_keys_move(name, technique):
     keys distinct within a step). Whatever state a row is in when a step meets it (peer owner, relocation source,
     relocation target being filled), the result is rank 2's steps applied one after another."""
     op = INFLIGHT_OPS[name]()
-    init, steps = _inflight_steps(op)
-    done = threading.Event()
-    res = run_cluster(functools.partial(_inflight_train_worker, op=op, init=init, steps=steps, done=done), world=WORLD,
-                      workers=1, mode="threads", value_lengths=op.value_lengths(), num_keys=op.num_keys,
-                      dtype="float32", backend="cuda", options={"sys.techniques": technique})
-    out = res[2][0]
+    op.init, steps = _inflight_steps(op)
+    res = while_keys_move(op, steps, technique)
+    out = res[2]
     s = out["stats"]
-    relocations = sum(r["counters"]["relocations"] for r in res.values())
+    relocations = sum(r["counters"]["relocations"] for r in res)
     info = f"{op} {technique}: stats {s} (remote rows {s[1]}, slow-path calls {s[2]}), relocations {relocations}"
     print(info)
     assert relocations > 0, info
-    assert all(r["counters"]["protocol_errors"] == 0 for r in res.values()), info
+    assert all(r["counters"]["protocol_errors"] == 0 for r in res), info
     assert s[3] == sum(op.updates(b) for b in steps), info
-    ref_rows, ref_loss = reference_run(op, init, steps)
+    ref_rows, ref_loss = reference_run(op, op.init, steps)
     _assert_rows(out["rows"], ref_rows, info)
     torch.testing.assert_close(out["loss"], ref_loss, rtol=1e-3 if op.kind == "sgns" else 1e-4, atol=1e-3)
 
@@ -573,65 +422,13 @@ def _gather_all(server, q, keys, true_col, exclude, scale, stats=None):
 
 
 def _one_rank_expectation():
-    import adapm_b200 as ad
-
     rows, q, keys, true_col, (off, cols), scale = _gather_inputs()
-    s = ad.Server(GATHER_DIM, num_keys=GATHER_KEYS, num_threads=1, rank=0, world=1, backend="cuda", fabric="inproc",
-                  job=f"gx1_{np.random.randint(1 << 30)}", device=0)
-    w = ad.Worker(0, s)
-    try:
+    with one_rank_store(GATHER_DIM, GATHER_KEYS, "cuda", "float32") as (s, w):
         w.wait(w.set(torch.arange(GATHER_KEYS), rows.view(-1)))
         dev = s.device
         exp = _gather_all(s, q.to(dev), keys.to(dev), true_col.to(dev), (off.to(dev), cols.to(dev)), scale.to(dev))
         torch.cuda.synchronize()
         return {k: (tuple(t.cpu() for t in v) if isinstance(v, tuple) else v.cpu()) for k, v in exp.items()}
-    finally:
-        w.finalize()
-        s.shutdown()
-
-
-def _inflight_gather_worker(kv, server, wid, exp, done):
-    rank = server.my_rank()
-    rows, q, keys, true_col, (off, cols), scale = _gather_inputs()
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(GATHER_KEYS), rows.view(-1)))
-    kv.waitall(); kv.barrier()
-    block = torch.arange(0, GATHER_KEYS, 8)       # 8192 keys move between ranks 0 and 1, spread over all tiles
-    out = {}
-    if rank < 2:
-        out["iters"] = _mover(kv, rank, block, done)
-    else:
-        dev = server.device
-        stream = torch.cuda.Stream(dev)
-        stats = torch.zeros(4, dtype=torch.int64, device=dev)
-        mism, reps = {}, 0
-        try:
-            with torch.cuda.stream(stream):
-                args = (q.to(dev), keys.to(dev), true_col.to(dev), (off.to(dev), cols.to(dev)), scale.to(dev))
-                e = {k: (tuple(t.to(dev) for t in v) if isinstance(v, tuple) else v.to(dev)) for k, v in exp.items()}
-                t0 = time.time()     # at least GATHER_REPS repetitions over at least 3 s of relocation rounds
-                while (reps < GATHER_REPS or time.time() - t0 < 3.0) and reps < 50 * GATHER_REPS:
-                    got = _gather_all(server, *args, stats=stats)
-                    for k, v in got.items():
-                        if isinstance(v, tuple):
-                            bad = ~((v[0] == e[k][0]) & (v[1] == e[k][1])).all(1)
-                            where = bad.nonzero().view(-1)
-                        elif k == "scores":
-                            badc = (v != e[k]).any(0)
-                            where = keys[badc.nonzero().view(-1).cpu()]        # store keys of the wrong columns
-                        else:
-                            where = (v != e[k]).nonzero().view(-1)
-                        if where.numel():
-                            mism.setdefault(k, []).append(where[:8].tolist())
-                    reps += 1
-                stream.synchronize()
-        finally:
-            done.set()
-        out.update(mism=mism, reps=reps, stats=stats.tolist())
-    kv.barrier()
-    _idiom(kv)
-    kv.finalize()
-    return out
 
 
 @gpu
@@ -642,17 +439,23 @@ def test_gathers_of_rows_in_flight_are_exact(technique):
     result equals, bit for bit, the same op on a one-rank store loaded with the same rows: a row read as zeros, or
     half-way through its transfer, shows as a wrong score."""
     exp = _one_rank_expectation()
-    done = threading.Event()
-    res = run_cluster(functools.partial(_inflight_gather_worker, exp=exp, done=done), world=WORLD, workers=1,
-                      mode="threads", value_lengths=GATHER_DIM, num_keys=GATHER_KEYS, dtype="float32", backend="cuda",
-                      options={"sys.techniques": technique})
-    out = res[2][0]
-    relocations = sum(r["counters"]["relocations"] for r in res.values())
+    rows, q, keys, true_col, (off, cols), scale = _gather_inputs()
+
+    def read(server, kv, stats):
+        dev = server.device
+        args = (q.to(dev), keys.to(dev), true_col.to(dev), (off.to(dev), cols.to(dev)), scale.to(dev))
+        return lambda: _gather_all(server, *args, stats=stats)
+
+    block = torch.arange(0, GATHER_KEYS, 8)       # 8192 keys move between ranks 0 and 1, spread over all tiles
+    res = reads_while_keys_move(Case(GATHER_DIM, GATHER_KEYS, [(torch.arange(GATHER_KEYS), rows)]), read, exp, block,
+                                technique, min_reps=GATHER_REPS, max_reps=50 * GATHER_REPS)
+    out = res[2]
+    relocations = sum(r["counters"]["relocations"] for r in res)
     info = f"{technique}: {out['reps']} repetitions, stats {out['stats']}, relocations {relocations}"
     print(info)
     assert relocations > 0, info
-    assert all(r["counters"]["protocol_errors"] == 0 for r in res.values()), info
-    assert not out["mism"], f"{info}; mismatches (first rows / keys of each repetition): {out['mism']}"
+    assert all(r["counters"]["protocol_errors"] == 0 for r in res), info
+    assert not out["mism"], f"{info}; mismatches (repetition, result): {out['mism']}"
     assert out["stats"][2] == 0, info
 
 
@@ -660,7 +463,6 @@ def test_gathers_of_rows_in_flight_are_exact(technique):
 def inplace_sgns_check(d, neg):
     """The distinct-key comparison of the one-GPU SGNS step (test_gpu_ops.py) for impl="tma", run in a process with
     ADAPM_SGNS_DETERMINISTIC=0: the in-place kernel sgns_step_tma_kernel<VPL, 128>, one launch."""
-    import adapm_b200 as ad
     from adapm_b200 import _C
 
     assert os.environ.get("ADAPM_SGNS_DETERMINISTIC") == "0"
@@ -670,11 +472,8 @@ def inplace_sgns_check(d, neg):
     init = op.init_rows(g)
     b = op.batch(torch.randperm(op.ne, generator=g)[:op.need()[0]], None, g)
     b["negatives"][0, 0] = b["contexts"][0]          # a negative equal to the context is skipped
-    s = ad.Server(2 * d, num_keys=op.ne, num_threads=1, rank=0, world=1, backend="cuda", fabric="inproc",
-                  job=f"inplace{d}_{np.random.randint(1 << 30)}", device=0)
-    kv = ad.Worker(0, s)
-    try:
-        _load(kv, init)
+    with one_rank_store(2 * d, op.ne, "cuda", "float32") as (s, kv):
+        load_rows(kv, init)
         dev = s.device
         loss = torch.zeros(1, device=dev)
         stats = torch.zeros(4, dtype=torch.int64, device=dev)
@@ -686,10 +485,7 @@ def inplace_sgns_check(d, neg):
         sgns_step(s, b_dev["centers"], b_dev["contexts"], b_dev["negatives"].contiguous(), d, op.lr, loss, stats, impl="tma")
         launches = _C.kernel_launches() - n0
         torch.cuda.synchronize()
-        got = _pull_groups(kv, init)
-    finally:
-        kv.finalize()
-        s.shutdown()
+        got = pull_rows(kv, init)
     ref_rows, ref_loss = reference_run(op, init, [b])
     _assert_rows(got, ref_rows, f"in-place sgns d={d} neg={neg}")
     torch.testing.assert_close(float(loss.item()), ref_loss, rtol=1e-3, atol=1e-3)
@@ -719,14 +515,7 @@ def _local_sampler_worker(kv, server, wid, weights):
     rank = server.my_rank()
     kv.barrier()
     mine = torch.arange(rank * 60, rank * 60 + 120) % SAMPLER_KEYS     # overlapping sets: relocations and replicas
-    c = kv.current_clock()
-    kv.intent(mine, c, c + 1_000_000)
-    for _ in range(50):
-        kv.advance_clock()
-        _idiom(kv)
-        missing = sum(not server.is_local(int(k)) for k in mine)
-        if server.allreduce_sum([float(missing)])[0] == 0:
-            break
+    make_local(kv, server, mine)
     local0 = torch.tensor([server.is_local(k) for k in range(SAMPLER_KEYS)])
     sampler = DeviceSampler(server, weights=weights)
     n = 1 << 21
@@ -766,20 +555,13 @@ def test_local_only_sampling_draws_local_keys_by_weight():
 
 @gpu
 def test_log_uniform_sampling_matches_its_distribution():
-    import adapm_b200 as ad
     from adapm_b200.ops import DeviceSampler
 
     n, first = 1000, 17
-    s = ad.Server(4, num_keys=first + n + 5, num_threads=1, rank=0, world=1, backend="cuda", fabric="inproc",
-                  job=f"logu_{np.random.randint(1 << 30)}", device=0)
-    w = ad.Worker(0, s)
-    try:
+    with one_rank_store(4, first + n + 5, "cuda", "float32") as (s, _):
         sampler = DeviceSampler(s, distribution="log-uniform", num_keys=n, first_key=first)
         draws = 1 << 22
         keys = sampler.sample(draws, seed=42).cpu()
-    finally:
-        w.finalize()
-        s.shutdown()
     assert int(keys.min()) == first and int(keys.max()) == first + n - 1, (int(keys.min()), int(keys.max()))
     hist = torch.bincount(keys - first, minlength=n).double() / draws
     j = torch.arange(n, dtype=torch.float64)

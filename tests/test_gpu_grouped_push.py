@@ -16,11 +16,11 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from test_ffm_cpu import FFM_VPL_SHAPE  # noqa: E402
-from test_gpu_embbag import MODES, _cuda_server, _hard_bags, _rows, _run  # noqa: E402
+from multirank import load_rows, one_rank_store  # noqa: E402
+from test_gpu_embbag import MODES, _hard_bags, _rows, _run  # noqa: E402
 from test_gpu_embbag import _table as _bag_table  # noqa: E402
 from test_gpu_ffm import _batch, _fused  # noqa: E402
 from test_gpu_ffm import _table as _ffm_table  # noqa: E402
-from test_gpu_fused_multirank import _load  # noqa: E402
 
 gpu = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "grouped_push", "golden.json")
@@ -39,24 +39,20 @@ def _bag_run(dim):
     from adapm_b200.ops import StoreEmbeddingBag
 
     num_keys = 20_000
-    server, kv = _cuda_server(dim, num_keys, f"bag_golden{dim}")
     out = {}
-    try:
+    with one_rank_store(2 * dim, num_keys, "cuda", "float32") as (server, kv):
         for mode, weighted in MODES:
             g = torch.Generator().manual_seed(dim + 3 * weighted + 5 * (mode == "mean"))
             table = _bag_table(num_keys, dim, g)
             keys, offsets = _hard_bags(g, num_keys)
             w = torch.rand(keys.numel(), generator=g) * 2 - 0.5 if weighted else None
             grad = torch.randn(offsets.numel() - 1, dim, generator=g) * 1e-3
-            _load(kv, [(torch.arange(num_keys), table)])
+            load_rows(kv, [(torch.arange(num_keys), table)])
             kv.waitall()
             bag = StoreEmbeddingBag(server, kv, dim, mode=mode, lr=0.05, grad_scale=7.0)
             pooled = _run(kv, bag, keys, offsets, w, grad)
             out[f"{dim}-{mode}{'-weighted' if weighted else ''}"] = {
                 "out_sha256": _sha(pooled), "rows_sha256": _sha(_rows(kv, num_keys, dim)), "stats": bag.stats.tolist()}
-    finally:
-        kv.finalize()
-        server.shutdown()
     return out
 
 

@@ -2,37 +2,23 @@
 with trees whose longest path is 1, a middle length, 31 and 32 nodes, bit-identical runs, launch counts, the in-place
 kernel on one GPU and on multi-rank stores (peer rows, replicas, keys in flight), training end to end, and the build
 budget of the new kernels."""
-import functools
 import glob
 import os
 import re
 import subprocess
 import sys
-import threading
-import time
 
-import numpy as np
 import pytest
 import torch
 
-from harness import run_cluster
+from multirank import WORLD, Case, Fused, load_rows, on_peer_rows, on_replicas, one_rank_store, while_keys_move
 from test_cbow_cpu import TOPIC_PRECISION
-from test_gpu_fused_multirank import _idiom, _load, _mover
 from test_hs_cpu import torch_hs_rule64, train_planted_hs
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 gpu = pytest.mark.gpu
-WORLD = 3
 RTOL, ATOL = 2e-4, 2e-5
 ALPHA = 0.01
-
-
-def _cuda_server(row_len, num_keys, job):
-    import adapm_b200 as ad
-
-    s = ad.Server(row_len, num_keys=num_keys, num_threads=1, rank=0, world=1, backend="cuda", fabric="inproc",
-                  job=f"{job}_{np.random.randint(1 << 30)}", device=0)
-    return s, ad.Worker(0, s)
 
 
 def _tree(kind):
@@ -113,9 +99,8 @@ def test_deterministic_step_matches_float64_rule(d, C, kind):
     g = torch.Generator().manual_seed(d * 100 + C)
     tree = _tree(kind)
     table = _table(g, 2 * vocab, d, tree)
-    server, kv = _cuda_server(2 * d, 2 * vocab, f"hsdet{d}")
-    try:
-        _load(kv, [(torch.arange(2 * vocab), table)])
+    with one_rank_store(2 * d, 2 * vocab, "cuda", "float32") as (server, kv):
+        load_rows(kv, [(torch.arange(2 * vocab), table)])
         kv.waitall()
         dev = server.device
         tdev = tree.to(dev)
@@ -139,16 +124,12 @@ def test_deterministic_step_matches_float64_rule(d, C, kind):
             assert s[3] == _updates(b, tree, skipped) and s[2] == 0 and s[1] == 0, (what, s)
             if kind != "l1":
                 assert skipped > 0, what
-    finally:
-        kv.finalize()
-        server.shutdown()
 
 
 def _bits_run(d, steps, tree):
-    server, kv = _cuda_server(2 * d, 2 * 3000, "hsbits")
-    try:
+    with one_rank_store(2 * d, 2 * 3000, "cuda", "float32") as (server, kv):
         g = torch.Generator().manual_seed(1)
-        _load(kv, [(torch.arange(6000), _table(g, 6000, d, tree))])
+        load_rows(kv, [(torch.arange(6000), _table(g, 6000, d, tree))])
         kv.waitall()
         loss = torch.zeros(1, device=server.device)
         tdev = tree.to(server.device)
@@ -156,9 +137,6 @@ def _bits_run(d, steps, tree):
             _step(server, b, tdev, d, loss, None)
         torch.cuda.synchronize()
         return _rows(kv, 6000, d), loss.cpu()
-    finally:
-        kv.finalize()
-        server.shutdown()
 
 
 @gpu
@@ -175,10 +153,9 @@ def test_two_runs_on_fresh_stores_are_bit_identical():
 def test_launch_counts():
     from adapm_b200 import _C
 
-    server, kv = _cuda_server(2 * 64, 2000, "hslaunch")
-    try:
+    with one_rank_store(2 * 64, 2000, "cuda", "float32") as (server, kv):
         g = torch.Generator().manual_seed(3)
-        _load(kv, [(torch.arange(2000), _table(g, 2000, 64))])
+        load_rows(kv, [(torch.arange(2000), _table(g, 2000, 64))])
         b = _batch(g, 1000, _tree("l31"), 300, 8)
         tdev = _tree("l31").to(server.device)
         loss = torch.zeros(1, device=server.device)
@@ -189,17 +166,13 @@ def test_launch_counts():
         _step(server, b, tdev, 64, loss, None, deterministic=False)
         assert _C.kernel_launches() - n0 == 9          # the in-place kernel
         torch.cuda.synchronize()
-    finally:
-        kv.finalize()
-        server.shutdown()
 
 
 @gpu
 def test_argument_checks():
     from adapm_b200.ops import hs_step
 
-    server, kv = _cuda_server(2 * 64, 2000, "hschk")
-    try:
+    with one_rank_store(2 * 64, 2000, "cuda", "float32") as (server, kv):
         dev = server.device
         tree = _tree("mid").to(dev)
         c = torch.ones(4, dtype=torch.int64, device=dev)
@@ -215,9 +188,6 @@ def test_argument_checks():
             hs_step(server, c, x, type(tree)(tree.offsets, tree.nodes, tree.codes, 33), 64, 0.1, loss)
         with pytest.raises(TypeError):
             hs_step(server, c, x, _tree("mid"), 64, 0.1, loss)           # the tree on the host
-    finally:
-        kv.finalize()
-        server.shutdown()
 
 
 def _single_items(g, words, tree, n, C):
@@ -240,12 +210,11 @@ def test_inplace_kernel_on_one_gpu_matches_rule(d, C, kind):
     from adapm_b200 import _C
 
     vocab = 4000
-    server, kv = _cuda_server(2 * d, 2 * vocab, f"hsip{d}")
-    try:
+    with one_rank_store(2 * d, 2 * vocab, "cuda", "float32") as (server, kv):
         g = torch.Generator().manual_seed(d + C)
         tree = _tree(kind)
         table = _table(g, 2 * vocab, d, tree)
-        _load(kv, [(torch.arange(2 * vocab), table)])
+        load_rows(kv, [(torch.arange(2 * vocab), table)])
         kv.waitall()
         ref, ref_loss, n_upd = table.double(), 0.0, 0
         dev = server.device
@@ -265,9 +234,6 @@ def test_inplace_kernel_on_one_gpu_matches_rule(d, C, kind):
         assert float(loss) == pytest.approx(ref_loss, rel=1e-4)
         s = stats.tolist()
         assert s[3] == n_upd and s[2] == 0, s
-    finally:
-        kv.finalize()
-        server.shutdown()
 
 
 # ---------------------------------------------------------------------------------------------- several ranks
@@ -282,61 +248,8 @@ def _apply(table, steps, tree):
     return table, loss
 
 
-def _fused(server, steps, tree, loss, stats, stream):
-    with torch.cuda.stream(stream):
-        for b in steps:
-            _step(server, b, tree, DIM, loss, stats)
-    stream.synchronize()
-
-
-def _peer_worker(kv, server, wid, table, steps, tree):
-    rank = server.my_rank()
-    n = table.shape[0]
-    if rank == 0:
-        _load(kv, [(torch.arange(n), table)])
-    kv.waitall(); kv.barrier()
-    dev = server.device
-    loss = torch.zeros(1, device=dev)
-    stats = torch.zeros(4, dtype=torch.int64, device=dev)
-    tdev = tree.to(dev)
-    stream = torch.cuda.Stream(dev)
-    for turn in range(WORLD):
-        if turn == rank:
-            _fused(server, steps[rank], tdev, loss, stats, stream)
-        kv.barrier()
-    rows = _rows(kv, n, DIM) if rank == 0 else None
-    kv.barrier()
-    kv.finalize()
-    return {"loss": float(loss.item()), "stats": stats.tolist(), "rows": rows}
-
-
 def _rank_steps(g, tree, n_words, n):
     return [_single_items(g, torch.arange(n_words), tree, n, CTX) for _ in range(WORLD)]
-
-
-@gpu
-def test_peer_rows_match_float64_rule():
-    """three ranks, no intents (2 in 3 keys owned by a peer), the ranks' steps in turn"""
-    vocab = 900
-    g = torch.Generator().manual_seed(21)
-    tree = _tree("mid")
-    table = _table(g, 2 * max(vocab, tree.num_words), DIM, tree)
-    steps = _rank_steps(g, tree, vocab, 12)
-    res = run_cluster(functools.partial(_peer_worker, table=table, steps=steps, tree=tree), world=WORLD, workers=1,
-                      mode="threads", value_lengths=2 * DIM, num_keys=table.shape[0], dtype="float32", backend="cuda")
-    ref = table.double()
-    for r in range(WORLD):
-        before = ref
-        ref, ref_l = _apply(ref, steps[r], tree)
-        out = res[r][0]
-        assert out["loss"] == pytest.approx(ref_l, rel=1e-4)
-        n_upd = 0
-        for b in steps[r]:
-            before, _, sk = torch_hs_rule64(before, *b, tree, DIM, ALPHA)
-            n_upd += _updates(b, tree, sk)
-        s = out["stats"]
-        assert s[3] == n_upd and s[1] > 0 and s[2] == 0, (r, s)
-    torch.testing.assert_close(res[0][0]["rows"].double(), ref, rtol=RTOL, atol=ATOL)
 
 
 def _keys_of(steps, tree):
@@ -349,35 +262,43 @@ def _keys_of(steps, tree):
     return torch.unique(torch.cat(ks))
 
 
-def _replica_worker(kv, server, wid, table, steps, tree):
-    rank = server.my_rank()
+def _case(table, tree):
+    """a batch is a list of steps, run one after another"""
+    def open_steps(server, kv):
+        tdev = tree.to(server.device)
+
+        def run(server, steps, loss, stats):
+            for b in steps:
+                _step(server, b, tdev, DIM, loss, stats)
+
+        return Fused(server, run)
+
     n = table.shape[0]
-    if rank == 0:
-        _load(kv, [(torch.arange(n), table)])
-    kv.waitall(); kv.barrier()
-    mine = _keys_of(steps[rank], tree)
-    c = kv.current_clock()
-    kv.intent(mine, c, c + 1_000_000)
-    for _ in range(50):
-        kv.advance_clock()
-        _idiom(kv)
-        missing = sum(not server.is_local(int(k)) for k in mine)
-        if server.allreduce_sum([float(missing)])[0] == 0:
-            break
-    local = all(server.is_local(int(k)) for k in mine)
-    dev = server.device
-    loss = torch.zeros(1, device=dev)
-    stats = torch.zeros(4, dtype=torch.int64, device=dev)
-    stream = torch.cuda.Stream(dev)
-    tdev = tree.to(dev)
-    for turn in range(WORLD):
-        if turn == rank:
-            _fused(server, steps[rank], tdev, loss, stats, stream)
-        _idiom(kv)
-    rows = _rows(kv, n, DIM)
-    kv.barrier()
-    kv.finalize()
-    return {"loss": float(loss.item()), "stats": stats.tolist(), "rows": rows, "local": local}
+    return Case(2 * DIM, n, [(torch.arange(n), table)], lambda steps: _keys_of(steps, tree), open_steps)
+
+
+@gpu
+def test_peer_rows_match_float64_rule():
+    """three ranks, no intents (2 in 3 keys owned by a peer), the ranks' steps in turn"""
+    vocab = 900
+    g = torch.Generator().manual_seed(21)
+    tree = _tree("mid")
+    table = _table(g, 2 * max(vocab, tree.num_words), DIM, tree)
+    steps = _rank_steps(g, tree, vocab, 12)
+    res = on_peer_rows(_case(table, tree), steps, in_turns=True)
+    ref = table.double()
+    for r in range(WORLD):
+        before = ref
+        ref, ref_l = _apply(ref, steps[r], tree)
+        out = res[r]
+        assert out["loss"] == pytest.approx(ref_l, rel=1e-4)
+        n_upd = 0
+        for b in steps[r]:
+            before, _, sk = torch_hs_rule64(before, *b, tree, DIM, ALPHA)
+            n_upd += _updates(b, tree, sk)
+        s = out["stats"]
+        assert s[3] == n_upd and s[1] > 0 and s[2] == 0, (r, s)
+    torch.testing.assert_close(res[0]["rows"][0].double(), ref, rtol=RTOL, atol=ATOL)
 
 
 @gpu
@@ -389,58 +310,23 @@ def test_replicas_match_float64_rule_in_turn_order():
     tree = _tree("mid")
     table = _table(g, 2 * max(vocab, tree.num_words), DIM, tree)
     steps = _rank_steps(g, tree, vocab, 8)
-    res = run_cluster(functools.partial(_replica_worker, table=table, steps=steps, tree=tree), world=WORLD, workers=1,
-                      mode="threads", value_lengths=2 * DIM, num_keys=table.shape[0], dtype="float32", backend="cuda",
-                      options={"sys.techniques": "replication_only"})
-    assert sum(r["counters"]["replica_setups"] for r in res.values()) > 0
-    assert all(r["counters"]["protocol_errors"] == 0 for r in res.values())
+    res = on_replicas(_case(table, tree), steps)
+    assert sum(r["counters"]["replica_setups"] for r in res) > 0
+    assert all(r["counters"]["protocol_errors"] == 0 for r in res)
     ref = table.double()
     losses = []
     for r in range(WORLD):
         ref, l = _apply(ref, steps[r], tree)
         losses.append(l)
     for r in range(WORLD):
-        out = res[r][0]
+        out = res[r]
         assert out["local"], f"rank {r}: batch keys not local after the intents"
-        torch.testing.assert_close(out["rows"].double(), ref, rtol=RTOL, atol=ATOL, msg=lambda m: f"rank {r}: {m}")
+        torch.testing.assert_close(out["rows"][0].double(), ref, rtol=RTOL, atol=ATOL, msg=lambda m: f"rank {r}: {m}")
         assert out["loss"] == pytest.approx(losses[r], rel=1e-4)
         assert out["stats"][1] == 0 and out["stats"][2] == 0, (r, out["stats"])
 
 
 INFLIGHT_STEPS = 32
-
-
-def _inflight_worker(kv, server, wid, table, steps, tree, done):
-    rank = server.my_rank()
-    n = table.shape[0]
-    if rank == 0:
-        _load(kv, [(torch.arange(n), table)])
-    kv.waitall(); kv.barrier()
-    out = {}
-    if rank < 2:
-        out["iters"] = _mover(kv, rank, torch.arange(n), done)
-    else:
-        dev = server.device
-        loss = torch.zeros(1, device=dev)
-        stats = torch.zeros(4, dtype=torch.int64, device=dev)
-        stream = torch.cuda.Stream(dev)
-        tdev = tree.to(dev)
-        try:
-            for b in steps:
-                _fused(server, [b], tdev, loss, stats, stream)
-                time.sleep(0.03)          # spread the steps over many sync rounds
-        finally:
-            done.set()
-        out["loss"], out["stats"] = float(loss.item()), stats.tolist()
-    kv.barrier()
-    for _ in range(8):
-        kv.advance_clock()
-    _idiom(kv)
-    if rank == 2:
-        out["rows"] = _rows(kv, n, DIM)
-    kv.barrier()
-    kv.finalize()
-    return out
 
 
 @gpu
@@ -452,24 +338,21 @@ def test_steps_lose_no_update_while_keys_move(technique):
     tree = _tree("l31")
     table = _table(g, 2 * vocab, DIM, tree)
     steps = _single_items(g, torch.arange(vocab), tree, INFLIGHT_STEPS, CTX)
-    done = threading.Event()
-    res = run_cluster(functools.partial(_inflight_worker, table=table, steps=steps, tree=tree, done=done), world=WORLD,
-                      workers=1, mode="threads", value_lengths=2 * DIM, num_keys=2 * vocab, dtype="float32",
-                      backend="cuda", options={"sys.techniques": technique})
-    out = res[2][0]
+    res = while_keys_move(_case(table, tree), [[b] for b in steps], technique)
+    out = res[2]
     s = out["stats"]
-    relocations = sum(r["counters"]["relocations"] for r in res.values())
+    relocations = sum(r["counters"]["relocations"] for r in res)
     info = f"{technique}: stats {s}, relocations {relocations}"
     print(info)
     assert relocations > 0, info
-    assert all(r["counters"]["protocol_errors"] == 0 for r in res.values()), info
+    assert all(r["counters"]["protocol_errors"] == 0 for r in res), info
     ref, n_upd, ref_loss = table.double(), 0, 0.0
     for b in steps:
         ref, l, sk = torch_hs_rule64(ref, *b, tree, DIM, ALPHA)
         n_upd += _updates(b, tree, sk)
         ref_loss += l
     assert s[3] == n_upd, info
-    torch.testing.assert_close(out["rows"].double(), ref, rtol=RTOL, atol=ATOL, msg=lambda m: f"{info}: {m}")
+    torch.testing.assert_close(out["rows"][0].double(), ref, rtol=RTOL, atol=ATOL, msg=lambda m: f"{info}: {m}")
     assert out["loss"] == pytest.approx(ref_loss, rel=1e-3), info
 
 

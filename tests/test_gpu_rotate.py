@@ -2,16 +2,13 @@
 complex-metric distance kernels (``ops.gather_dist_rank_count`` / ``gather_dist_topk`` with ``p="complex"``) against a
 float64 oracle, both on three logical ranks of one GPU (peer rows, replicas, keys in flight), and the model's quality on
 the FB15k-237 toy set."""
-import functools
-import threading
-import time
-
 import numpy as np
 import pytest
 import torch
 
-from harness import WRAP, run_cluster, wrap_calls
-from test_gpu_fused_multirank import WORLD, _idiom, _mover
+from harness import WRAP, wrap_calls
+from multirank import (WORLD, Case, Fused, on_peer_rows, on_replicas, one_rank_store, reads_while_keys_move,
+                       rejected_on_ranks, while_keys_move)
 from test_gpu_transe import _check_rank, _check_topk, _dist_inputs
 
 gpu = pytest.mark.gpu
@@ -20,14 +17,6 @@ RTOL, ATOL = 2e-4, 2e-5
 
 def _lens(ne, nr, d):
     return torch.tensor([2 * d] * ne + [d] * nr, dtype=torch.int64)
-
-
-def _store(ne, nr, d, backend, dtype, job):
-    import adapm_b200 as ad
-
-    s = ad.Server(_lens(ne, nr, d), num_keys=ne + nr, num_threads=1, rank=0, world=1, backend=backend, fabric="inproc",
-                  job=f"{job}_{np.random.randint(1 << 30)}", dtype=dtype, **({"device": 0} if backend == "cuda" else {}))
-    return s, ad.Worker(0, s)
 
 
 def _init_table(ne, nr, d, g):
@@ -61,8 +50,7 @@ def _rule(table, ne, nr, batches, d, gamma, alpha, eta, ge):
     """batches applied one after another by the float64 rule on a float64 CPU store; returns (rows, loss, pushes)"""
     from adapm_b200.ops import rotate_reference_step
 
-    s, kv = _store(ne, nr, d, "cpu", "float64", "rotate_rule")
-    try:
+    with one_rank_store(_lens(ne, nr, d), ne + nr, "cpu", "float64") as (s, kv):
         kv.wait(kv.set(torch.arange(ne + nr), table.contiguous()))
         loss, pushes = 0.0, 0
         for b in batches:
@@ -71,9 +59,6 @@ def _rule(table, ne, nr, batches, d, gamma, alpha, eta, ge):
         rows = torch.empty(table.numel(), dtype=torch.float64)
         kv.wait(kv.pull(torch.arange(ne + nr), rows))
         return rows, loss, pushes
-    finally:
-        kv.finalize()
-        s.shutdown()
 
 
 def _fused(table, ne, nr, batches, d, gamma, alpha, eta, ge, deterministic):
@@ -81,8 +66,7 @@ def _fused(table, ne, nr, batches, d, gamma, alpha, eta, ge, deterministic):
     from adapm_b200 import _C
     from adapm_b200.ops import kge_rotate_step
 
-    s, kv = _store(ne, nr, d, "cuda", "float32", "rotate_fused")
-    try:
+    with one_rank_store(_lens(ne, nr, d), ne + nr, "cuda", "float32") as (s, kv):
         kv.wait(kv.set(torch.arange(ne + nr), table.float().contiguous()))
         dev = s.device
         loss = torch.zeros(1, device=dev)
@@ -97,9 +81,6 @@ def _fused(table, ne, nr, batches, d, gamma, alpha, eta, ge, deterministic):
         rows = torch.empty(table.numel(), dtype=torch.float32)
         kv.wait(kv.pull(torch.arange(ne + nr), rows))
         return rows.double(), float(loss.item()), stats.tolist(), launches
-    finally:
-        kv.finalize()
-        s.shutdown()
 
 
 # (d, 2n): float4 per lane (VPL) 1, 2, 4, 3, 3; 2n = 2 is the fewest negatives the step takes
@@ -150,28 +131,17 @@ def test_inplace_step_matches_rule_on_distinct_keys(d, nn, alpha, B):
     assert abs(loss - ref_loss) <= 1e-4 * max(1.0, ref_loss)
 
 
-def _reject_worker(kv, server, wid):
-    from adapm_b200.ops import kge_rotate_step
-
-    dev = server.device
-    k = torch.zeros(2, dtype=torch.int64, device=dev)
-    out = {}
-    try:
-        kge_rotate_step(server, k, k + 10, k, torch.zeros(2, 4, dtype=torch.int64, device=dev), 8, 2.0, 1.0, 0.1, 0.0,
-                        torch.zeros(1, device=dev), deterministic=True)
-        out["raised"] = False
-    except ValueError:
-        out["raised"] = True
-    kv.barrier()
-    kv.finalize()
-    return out
-
-
 @gpu
 def test_deterministic_step_rejected_on_several_ranks():
-    res = run_cluster(_reject_worker, world=2, workers=1, mode="threads", value_lengths=16, num_keys=64,
-                      dtype="float32", backend="cuda")
-    assert all(r[0]["raised"] for r in res.values())
+    from adapm_b200.ops import kge_rotate_step
+
+    def call(server):
+        dev = server.device
+        k = torch.zeros(2, dtype=torch.int64, device=dev)
+        kge_rotate_step(server, k, k + 10, k, torch.zeros(2, 4, dtype=torch.int64, device=dev), 8, 2.0, 1.0, 0.1, 0.0,
+                        torch.zeros(1, device=dev), deterministic=True)
+
+    assert rejected_on_ranks(call)
 
 
 # ---------------------------------------------------------------------------------------------- distance kernels
@@ -189,8 +159,7 @@ def test_complex_distance_kernels_match_float64_oracle():
     M, N, d = 70, 1000, 152                          # N is not a multiple of the 64-column tile
     g = torch.Generator().manual_seed(31)
     rows, q, keys, true_col, (off, cols), excluded = _dist_inputs(M, N, d, g)
-    s, kv = _store(N + 3, 0, d // 2, "cuda", "float32", "cdist")
-    try:
+    with one_rank_store(_lens(N + 3, 0, d // 2), N + 3, "cuda", "float32") as (s, kv):
         kv.wait(kv.set(torch.arange(N + 3), rows.contiguous().view(-1)))
         dev = s.device
         qd, kd, td, ex = q.to(dev), keys.to(dev), true_col.to(dev), (off.to(dev), cols.to(dev))
@@ -214,40 +183,19 @@ def test_complex_distance_kernels_match_float64_oracle():
         vals, idx = gather_dist_topk(s, qd, kd[:20], d, 64, "complex", False)     # fewer columns than k: padding
         assert bool((idx[:, 19:] == -1).all()) and bool((vals[:, 19:] == float("-inf")).all())
         assert not bool((idx[:, :19] == 0).any())                                   # column 0 is the NaN row
-    finally:
-        kv.finalize()
-        s.shutdown()
 
 
 # ---------------------------------------------------------------------------------------------- three ranks, one GPU
-def _peer_worker(kv, server, wid, table, ne, batches, d):
+def _case(table, ne, nr, d, ge):
+    """RotatE steps at gamma 6, alpha 1 and eta 0.05 with L2 weight ``ge``"""
     from adapm_b200.ops import kge_rotate_step
 
-    rank = server.my_rank()
-    n = server.num_keys()
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(n), table.float().contiguous()))
-    kv.waitall(); kv.barrier()
-    out = {}
-    dev = server.device
-    loss = torch.zeros(1, device=dev)
-    stats = torch.zeros(4, dtype=torch.int64, device=dev)
-    stream = torch.cuda.Stream(dev)
-    for turn in range(WORLD):                         # one rank at a time, in rank order
-        if turn == rank:
-            with torch.cuda.stream(stream):
-                kge_rotate_step(server, *(t.to(dev).contiguous() for t in batches[rank]), d, 6.0, 1.0, 0.05, 0.0,
-                                loss, stats)
-                stream.synchronize()
-        _idiom(kv)
-    out["loss"], out["stats"] = float(loss.item()), stats.tolist()
-    if rank == 0:
-        rows = torch.empty(table.numel())
-        kv.wait(kv.pull(torch.arange(n), rows))
-        out["rows"] = rows.double()
-    kv.barrier()
-    kv.finalize()
-    return out
+    def step(server, b, loss, stats):
+        dev = server.device
+        kge_rotate_step(server, *(t.to(dev).contiguous() for t in b), d, 6.0, 1.0, 0.05, ge, loss, stats)
+
+    return Case(_lens(ne, nr, d), ne + nr, [(torch.arange(ne + nr), table)],
+                lambda b: torch.unique(torch.cat([t.reshape(-1) for t in b])), lambda server, kv: Fused(server, step))
 
 
 @gpu
@@ -258,51 +206,12 @@ def test_step_on_peer_rows():
     g = torch.Generator().manual_seed(5)
     table = _init_table(ne, nr, d, g)
     batches = [_batch(ne, nr, B, nn, g, distinct=True) for _ in range(WORLD)]
-    res = run_cluster(functools.partial(_peer_worker, table=table, ne=ne, batches=batches, d=d), world=WORLD, workers=1,
-                      mode="threads", value_lengths=_lens(ne, nr, d), num_keys=ne + nr, dtype="float32", backend="cuda")
+    res = on_peer_rows(_case(table, ne, nr, d, 0.0), batches, in_turns=True)
     ref, ref_loss, ref_pushes = _rule(table, ne, nr, batches, d, 6.0, 1.0, 0.05, 0.0)
-    assert sum(r[0]["stats"][3] for r in res.values()) == ref_pushes
-    assert sum(r[0]["stats"][1] for r in res.values()) > 0       # peer rows were read
-    torch.testing.assert_close(res[0][0]["rows"], ref, rtol=RTOL, atol=ATOL)
-    torch.testing.assert_close(sum(r[0]["loss"] for r in res.values()), ref_loss, rtol=1e-4, atol=1e-3)
-
-
-def _replica_worker(kv, server, wid, table, batches, d):
-    from adapm_b200.ops import kge_rotate_step
-
-    rank = server.my_rank()
-    n = server.num_keys()
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(n), table.float().contiguous()))
-    kv.waitall(); kv.barrier()
-    mine = torch.unique(torch.cat([t.reshape(-1) for t in batches[rank]]))
-    c = kv.current_clock()
-    kv.intent(mine, c, c + 1_000_000)
-    for _ in range(50):
-        kv.advance_clock()
-        _idiom(kv)
-        missing = sum(not server.is_local(int(k)) for k in mine)
-        if server.allreduce_sum([float(missing)])[0] == 0:
-            break
-    local = all(server.is_local(int(k)) for k in mine)
-    replicas = sum(server.owner_of(int(k)) != rank for k in mine)
-    dev = server.device
-    loss = torch.zeros(1, device=dev)
-    stats = torch.zeros(4, dtype=torch.int64, device=dev)
-    stream = torch.cuda.Stream(dev)
-    for turn in range(WORLD):                         # one rank at a time, in rank order
-        if turn == rank:
-            with torch.cuda.stream(stream):
-                kge_rotate_step(server, *(t.to(dev).contiguous() for t in batches[rank]), d, 6.0, 1.0, 0.05, 0.01,
-                                loss, stats)
-            stream.synchronize()
-        _idiom(kv)
-    rows = torch.empty(table.numel())
-    kv.wait(kv.pull(torch.arange(n), rows))
-    kv.barrier()
-    kv.finalize()
-    return {"loss": float(loss.item()), "stats": stats.tolist(), "rows": rows.double(), "local": local,
-            "replicas": replicas}
+    assert sum(r["stats"][3] for r in res) == ref_pushes
+    assert sum(r["stats"][1] for r in res) > 0       # peer rows were read
+    torch.testing.assert_close(res[0]["rows"][0].double(), ref, rtol=RTOL, atol=ATOL)
+    torch.testing.assert_close(sum(r["loss"] for r in res), ref_loss, rtol=1e-4, atol=1e-3)
 
 
 @gpu
@@ -315,60 +224,20 @@ def test_step_on_replicas():
     g = torch.Generator().manual_seed(23)
     table = _init_table(ne, nr, d, g)
     batches = [_batch(ne, nr, B, nn, g, distinct=True) for _ in range(WORLD)]
-    res = run_cluster(functools.partial(_replica_worker, table=table, batches=batches, d=d), world=WORLD, workers=1,
-                      mode="threads", value_lengths=_lens(ne, nr, d), num_keys=ne + nr, dtype="float32",
-                      backend="cuda", options={"sys.techniques": "replication_only"})
-    assert sum(r["counters"]["replica_setups"] for r in res.values()) > 0
-    assert all(r["counters"]["protocol_errors"] == 0 for r in res.values())
+    res = on_replicas(_case(table, ne, nr, d, 0.01), batches)
+    assert sum(r["counters"]["replica_setups"] for r in res) > 0
+    assert all(r["counters"]["protocol_errors"] == 0 for r in res)
     args = (d, 6.0, 1.0, 0.05, 0.01)
     ref, _, _ = _rule(table, ne, nr, batches, *args)
     for r in range(WORLD):
-        out = res[r][0]
+        out = res[r]
         assert out["local"] and out["replicas"] > 0, f"rank {r}: batch keys not local after the intents"
-        torch.testing.assert_close(out["rows"], ref, rtol=RTOL, atol=ATOL, msg=lambda m: f"rows read on rank {r}: {m}")
+        torch.testing.assert_close(out["rows"][0].double(), ref, rtol=RTOL, atol=ATOL, msg=lambda m: f"rows read on rank {r}: {m}")
         _, before_loss, before_pushes = _rule(table, ne, nr, batches[:r], *args) if r else (None, 0.0, 0)
         _, upto_loss, upto_pushes = _rule(table, ne, nr, batches[:r + 1], *args)
         s = out["stats"]
         assert s[0] == B * (3 + nn) and s[1] == 0 and s[2] == 0 and s[3] == upto_pushes - before_pushes, (r, s)
         torch.testing.assert_close(out["loss"], upto_loss - before_loss, rtol=1e-4, atol=1e-3)
-
-
-def _inflight_step_worker(kv, server, wid, table, batches, d, done):
-    from adapm_b200.ops import kge_rotate_step
-
-    rank = server.my_rank()
-    n = server.num_keys()
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(n), table.float().contiguous()))
-    kv.waitall(); kv.barrier()
-    out = {}
-    if rank < 2:
-        out["iters"] = _mover(kv, rank, torch.arange(n), done)
-    else:
-        dev = server.device
-        loss = torch.zeros(1, device=dev)
-        stats = torch.zeros(4, dtype=torch.int64, device=dev)
-        stream = torch.cuda.Stream(dev)
-        try:
-            with torch.cuda.stream(stream):
-                for b in batches:
-                    kge_rotate_step(server, *(t.to(dev).contiguous() for t in b), d, 6.0, 1.0, 0.05, 0.0, loss, stats)
-                    stream.synchronize()
-                    time.sleep(0.03)
-        finally:
-            done.set()
-        out["loss"], out["stats"] = float(loss.item()), stats.tolist()
-    kv.barrier()
-    for _ in range(8):
-        kv.advance_clock()
-    _idiom(kv)
-    if rank == 2:
-        rows = torch.empty(table.numel())
-        kv.wait(kv.pull(torch.arange(n), rows))
-        out["rows"] = rows.double()
-    kv.barrier()
-    kv.finalize()
-    return out
 
 
 @gpu
@@ -380,18 +249,15 @@ def test_step_loses_no_update_while_keys_move(technique):
     g = torch.Generator().manual_seed(9)
     table = _init_table(ne, nr, d, g)
     batches = [_batch(ne, nr, B, nn, g, distinct=True) for _ in range(32)]
-    done = threading.Event()
-    res = run_cluster(functools.partial(_inflight_step_worker, table=table, batches=batches, d=d, done=done),
-                      world=WORLD, workers=1, mode="threads", value_lengths=_lens(ne, nr, d), num_keys=ne + nr,
-                      dtype="float32", backend="cuda", options={"sys.techniques": technique})
-    out = res[2][0]
-    relocations = sum(r["counters"]["relocations"] for r in res.values())
+    res = while_keys_move(_case(table, ne, nr, d, 0.0), batches, technique)
+    out = res[2]
+    relocations = sum(r["counters"]["relocations"] for r in res)
     info = f"{technique}: stats {out['stats']}, relocations {relocations}"
     print(info)
-    assert relocations > 0 and all(r["counters"]["protocol_errors"] == 0 for r in res.values()), info
+    assert relocations > 0 and all(r["counters"]["protocol_errors"] == 0 for r in res), info
     ref, ref_loss, ref_pushes = _rule(table, ne, nr, batches, d, 6.0, 1.0, 0.05, 0.0)
     assert out["stats"][3] == ref_pushes, info
-    torch.testing.assert_close(out["rows"], ref, rtol=RTOL, atol=ATOL)
+    torch.testing.assert_close(out["rows"][0].double(), ref, rtol=RTOL, atol=ATOL)
     torch.testing.assert_close(out["loss"], ref_loss, rtol=1e-4, atol=1e-3)
 
 
@@ -413,66 +279,28 @@ def _dist_mr_inputs():
     return rows, q, keys, true_col, ex
 
 
-def _inflight_dist_worker(kv, server, wid, exp, done):
-    rank = server.my_rank()
-    rows, q, keys, true_col, (off, cols) = _dist_mr_inputs()
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(DK), rows.contiguous().view(-1)))
-    kv.waitall(); kv.barrier()
-    out = {}
-    if rank < 2:
-        out["iters"] = _mover(kv, rank, torch.arange(0, DK, 8), done)
-    else:
-        dev = server.device
-        stream = torch.cuda.Stream(dev)
-        stats = torch.zeros(3, dtype=torch.int64, device=dev)
-        mism, reps = [], 0
-        try:
-            with torch.cuda.stream(stream):
-                args = (q.to(dev), keys.to(dev), true_col.to(dev), (off.to(dev), cols.to(dev)))
-                t0 = time.time()
-                while (reps < 8 or time.time() - t0 < 3.0) and reps < 200:
-                    got = _dist_all(server, *args, stats=stats)
-                    for k, v in got.items():
-                        if not all(torch.equal(a.cpu(), b) for a, b in zip(v, exp[k])):
-                            mism.append(k)
-                    reps += 1
-                stream.synchronize()
-        finally:
-            done.set()
-        out.update(mism=mism, reps=reps, stats=stats.tolist())
-    kv.barrier()
-    _idiom(kv)
-    kv.finalize()
-    return out
-
-
 @gpu
 def test_complex_distance_kernels_bit_identical_while_keys_move():
-    import adapm_b200 as ad
-
     rows, q, keys, true_col, (off, cols) = _dist_mr_inputs()
-    s = ad.Server(DD, num_keys=DK, num_threads=1, rank=0, world=1, backend="cuda", fabric="inproc",
-                  job=f"cdist1_{np.random.randint(1 << 30)}", dtype="float32", device=0)
-    kv = ad.Worker(0, s)
-    try:
+    with one_rank_store(DD, DK, "cuda", "float32") as (s, kv):
         kv.wait(kv.set(torch.arange(DK), rows.contiguous().view(-1)))
         dev = s.device
         exp = _dist_all(s, q.to(dev), keys.to(dev), true_col.to(dev), (off.to(dev), cols.to(dev)))
         exp = {k: tuple(t.cpu() for t in v) for k, v in exp.items()}
-    finally:
-        kv.finalize()
-        s.shutdown()
-    done = threading.Event()
-    res = run_cluster(functools.partial(_inflight_dist_worker, exp=exp, done=done), world=WORLD, workers=1,
-                      mode="threads", value_lengths=DD, num_keys=DK, dtype="float32", backend="cuda",
-                      options={"sys.techniques": "relocation_only"})
-    out = res[2][0]
-    relocations = sum(r["counters"]["relocations"] for r in res.values())
+
+    def read(server, kv, stats):
+        dev = server.device
+        args = (q.to(dev), keys.to(dev), true_col.to(dev), (off.to(dev), cols.to(dev)))
+        return lambda: _dist_all(server, *args, stats=stats)
+
+    res = reads_while_keys_move(Case(DD, DK, [(torch.arange(DK), rows)]), read, exp, torch.arange(0, DK, 8),
+                                "relocation_only")
+    out = res[2]
+    relocations = sum(r["counters"]["relocations"] for r in res)
     info = f"{out['reps']} repetitions, stats {out['stats']}, relocations {relocations}"
     print(info)
     assert relocations > 0, info
-    assert not out["mism"], f"{info}; mismatches: {sorted(set(out['mism']))}"
+    assert not out["mism"], f"{info}; mismatches: {sorted({k for _, k in out['mism']})}"
     assert out["stats"][2] == 0, info
 
 

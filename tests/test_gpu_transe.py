@@ -1,30 +1,19 @@
 """TransE on the H100: the fused step (``ops.kge_transe_step``) against the float64 rule ``transe_reference_step``, the
 distance kernels (``ops.gather_dist_rank_count`` / ``gather_dist_topk``) against a float64 ``cdist`` oracle, both on
 three logical ranks of one GPU (peer rows, replicas, keys in flight), and the model's quality on the FB15k-237 toy set."""
-import functools
 import os
-import threading
-import time
 
-import numpy as np
 import pytest
 import torch
 
-from harness import WRAP, run_cluster, wrap_calls
-from test_gpu_fused_multirank import WORLD, _idiom, _mover
+from harness import WRAP, wrap_calls
+from multirank import (WORLD, Case, Fused, on_peer_rows, on_replicas, one_rank_store, reads_while_keys_move,
+                       rejected_on_ranks, while_keys_move)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "kge_fb15k237_toy")
 gpu = pytest.mark.gpu
 RTOL, ATOL = 2e-4, 2e-5
-
-
-def _store(row_len, num_keys, backend, dtype, job):
-    import adapm_b200 as ad
-
-    s = ad.Server(row_len, num_keys=num_keys, num_threads=1, rank=0, world=1, backend=backend, fabric="inproc",
-                  job=f"{job}_{np.random.randint(1 << 30)}", dtype=dtype, **({"device": 0} if backend == "cuda" else {}))
-    return s, ad.Worker(0, s)
 
 
 def _init_table(num_keys, d, g):
@@ -55,8 +44,7 @@ def _rule(table, batches, d, p, margin, eta, ge, gr):
     from adapm_b200.ops import transe_reference_step
 
     n = table.shape[0]
-    s, kv = _store(2 * d, n, "cpu", "float64", "transe_rule")
-    try:
+    with one_rank_store(2 * d, n, "cpu", "float64") as (s, kv):
         kv.wait(kv.set(torch.arange(n), table.contiguous().view(-1)))
         loss, pushes = 0.0, 0
         for b in batches:
@@ -65,9 +53,6 @@ def _rule(table, batches, d, p, margin, eta, ge, gr):
         rows = torch.empty(n * 2 * d, dtype=torch.float64)
         kv.wait(kv.pull(torch.arange(n), rows))
         return rows.view(n, 2 * d), loss, pushes
-    finally:
-        kv.finalize()
-        s.shutdown()
 
 
 def _fused(table, batches, d, p, margin, eta, ge, gr, deterministic):
@@ -76,8 +61,7 @@ def _fused(table, batches, d, p, margin, eta, ge, gr, deterministic):
     from adapm_b200.ops import kge_transe_step
 
     n = table.shape[0]
-    s, kv = _store(2 * d, n, "cuda", "float32", "transe_fused")
-    try:
+    with one_rank_store(2 * d, n, "cuda", "float32") as (s, kv):
         kv.wait(kv.set(torch.arange(n), table.float().contiguous().view(-1)))
         dev = s.device
         loss = torch.zeros(1, device=dev)
@@ -92,9 +76,6 @@ def _fused(table, batches, d, p, margin, eta, ge, gr, deterministic):
         rows = torch.empty(n * 2 * d, dtype=torch.float32)
         kv.wait(kv.pull(torch.arange(n), rows))
         return rows.view(n, 2 * d).double(), float(loss.item()), stats.tolist(), launches
-    finally:
-        kv.finalize()
-        s.shutdown()
 
 
 def _cases(B, wrap_d, wrap_p):
@@ -142,28 +123,17 @@ def test_inplace_step_matches_rule_on_distinct_keys(d, p, B):
     assert abs(loss - ref_loss) <= 1e-4 * max(1.0, ref_loss)
 
 
-def _reject_worker(kv, server, wid):
-    from adapm_b200.ops import kge_transe_step
-
-    dev = server.device
-    k = torch.zeros(2, dtype=torch.int64, device=dev)
-    out = {}
-    try:
-        kge_transe_step(server, k, k + 10, k, torch.zeros(2, 4, dtype=torch.int64, device=dev), 8, 1, 1.0, 0.1, 0.0,
-                        0.0, torch.zeros(1, device=dev), deterministic=True)
-        out["raised"] = False
-    except ValueError:
-        out["raised"] = True
-    kv.barrier()
-    kv.finalize()
-    return out
-
-
 @gpu
 def test_deterministic_step_rejected_on_several_ranks():
-    res = run_cluster(_reject_worker, world=2, workers=1, mode="threads", value_lengths=16, num_keys=64,
-                      dtype="float32", backend="cuda")
-    assert all(r[0]["raised"] for r in res.values())
+    from adapm_b200.ops import kge_transe_step
+
+    def call(server):
+        dev = server.device
+        k = torch.zeros(2, dtype=torch.int64, device=dev)
+        kge_transe_step(server, k, k + 10, k, torch.zeros(2, 4, dtype=torch.int64, device=dev), 8, 1, 1.0, 0.1, 0.0,
+                        0.0, torch.zeros(1, device=dev), deterministic=True)
+
+    assert rejected_on_ranks(call)
 
 
 # ---------------------------------------------------------------------------------------------- distance kernels
@@ -241,8 +211,7 @@ def test_distance_kernels_match_float64_cdist(p, normalize):
     M, N, d = 70, 1000, 152                          # N is not a multiple of the 64-column tile
     g = torch.Generator().manual_seed(p * 2 + normalize)
     rows, q, keys, true_col, (off, cols), excluded = _dist_inputs(M, N, d, g)
-    s, kv = _store(d, N + 3, "cuda", "float32", "dist")
-    try:
+    with one_rank_store(d, N + 3, "cuda", "float32") as (s, kv):
         kv.wait(kv.set(torch.arange(N + 3), rows.contiguous().view(-1)))
         dev = s.device
         qd, kd, td, ex = q.to(dev), keys.to(dev), true_col.to(dev), (off.to(dev), cols.to(dev))
@@ -266,40 +235,20 @@ def test_distance_kernels_match_float64_cdist(p, normalize):
                                                      gather_dist_topk(s, qd, kd, d, 10, p, normalize, exclude=ex)))
         vals, idx = gather_dist_topk(s, qd, kd[:20], d, 64, p, normalize)         # fewer columns than k: padding
         assert bool((idx[:, 19:] == -1).all()) and bool((vals[:, 19:] == float("-inf")).all())
-    finally:
-        kv.finalize()
-        s.shutdown()
 
 
 # ---------------------------------------------------------------------------------------------- three ranks, one GPU
-def _peer_worker(kv, server, wid, table, batches, d, p):
+def _case(table, d, p, ge, gr):
+    """TransE steps at margin 1 and eta 0.05 with L2 weights ``ge``, ``gr``"""
     from adapm_b200.ops import kge_transe_step
 
-    rank = server.my_rank()
+    def step(server, b, loss, stats):
+        dev = server.device
+        kge_transe_step(server, *(t.to(dev).contiguous() for t in b), d, p, 1.0, 0.05, ge, gr, loss, stats)
+
     n = table.shape[0]
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(n), table.float().contiguous().view(-1)))
-    kv.waitall(); kv.barrier()
-    out = {}
-    dev = server.device
-    loss = torch.zeros(1, device=dev)
-    stats = torch.zeros(4, dtype=torch.int64, device=dev)
-    stream = torch.cuda.Stream(dev)
-    for turn in range(WORLD):                         # one rank at a time, in rank order
-        if turn == rank:
-            with torch.cuda.stream(stream):
-                kge_transe_step(server, *(t.to(dev).contiguous() for t in batches[rank]), d, p, 1.0, 0.05, 0.0, 0.0,
-                                loss, stats)
-                stream.synchronize()
-        _idiom(kv)
-    out["loss"], out["stats"] = float(loss.item()), stats.tolist()
-    if rank == 0:
-        rows = torch.empty(n * 2 * d)
-        kv.wait(kv.pull(torch.arange(n), rows))
-        out["rows"] = rows.view(n, 2 * d).double()
-    kv.barrier()
-    kv.finalize()
-    return out
+    return Case(2 * d, n, [(torch.arange(n), table)], lambda b: torch.unique(torch.cat([t.reshape(-1) for t in b])),
+                lambda server, kv: Fused(server, step))
 
 
 @gpu
@@ -310,89 +259,12 @@ def test_step_on_peer_rows():
     g = torch.Generator().manual_seed(5)
     table = _init_table(ne + nr, d, g)
     batches = [_batch(ne, nr, B, nn, g, distinct=True) for _ in range(WORLD)]
-    res = run_cluster(functools.partial(_peer_worker, table=table, batches=batches, d=d, p=p), world=WORLD, workers=1,
-                      mode="threads", value_lengths=2 * d, num_keys=ne + nr, dtype="float32", backend="cuda")
+    res = on_peer_rows(_case(table, d, p, 0.0, 0.0), batches, in_turns=True)
     ref, ref_loss, ref_pushes = _rule(table, batches, d, p, 1.0, 0.05, 0.0, 0.0)
-    assert sum(r[0]["stats"][3] for r in res.values()) == ref_pushes
-    assert sum(r[0]["stats"][1] for r in res.values()) > 0       # peer rows were read
-    torch.testing.assert_close(res[0][0]["rows"], ref, rtol=RTOL, atol=ATOL)
-    torch.testing.assert_close(sum(r[0]["loss"] for r in res.values()), ref_loss, rtol=1e-4, atol=1e-3)
-
-
-def _inflight_step_worker(kv, server, wid, table, batches, d, p, done):
-    from adapm_b200.ops import kge_transe_step
-
-    rank = server.my_rank()
-    n = table.shape[0]
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(n), table.float().contiguous().view(-1)))
-    kv.waitall(); kv.barrier()
-    out = {}
-    if rank < 2:
-        out["iters"] = _mover(kv, rank, torch.arange(n), done)
-    else:
-        dev = server.device
-        loss = torch.zeros(1, device=dev)
-        stats = torch.zeros(4, dtype=torch.int64, device=dev)
-        stream = torch.cuda.Stream(dev)
-        try:
-            with torch.cuda.stream(stream):
-                for b in batches:
-                    kge_transe_step(server, *(t.to(dev).contiguous() for t in b), d, p, 1.0, 0.05, 0.0, 0.0, loss, stats)
-                    stream.synchronize()
-                    time.sleep(0.03)
-        finally:
-            done.set()
-        out["loss"], out["stats"] = float(loss.item()), stats.tolist()
-    kv.barrier()
-    for _ in range(8):
-        kv.advance_clock()
-    _idiom(kv)
-    if rank == 2:
-        rows = torch.empty(n * 2 * d)
-        kv.wait(kv.pull(torch.arange(n), rows))
-        out["rows"] = rows.view(n, 2 * d).double()
-    kv.barrier()
-    kv.finalize()
-    return out
-
-
-def _replica_worker(kv, server, wid, table, batches, d, p):
-    from adapm_b200.ops import kge_transe_step
-
-    rank = server.my_rank()
-    n = table.shape[0]
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(n), table.float().contiguous().view(-1)))
-    kv.waitall(); kv.barrier()
-    mine = torch.unique(torch.cat([t.reshape(-1) for t in batches[rank]]))
-    c = kv.current_clock()
-    kv.intent(mine, c, c + 1_000_000)
-    for _ in range(50):
-        kv.advance_clock()
-        _idiom(kv)
-        missing = sum(not server.is_local(int(k)) for k in mine)
-        if server.allreduce_sum([float(missing)])[0] == 0:
-            break
-    local = all(server.is_local(int(k)) for k in mine)
-    replicas = sum(server.owner_of(int(k)) != rank for k in mine)
-    dev = server.device
-    loss = torch.zeros(1, device=dev)
-    stats = torch.zeros(4, dtype=torch.int64, device=dev)
-    stream = torch.cuda.Stream(dev)
-    for turn in range(WORLD):                         # one rank at a time, in rank order
-        if turn == rank:
-            with torch.cuda.stream(stream):
-                kge_transe_step(server, *(t.to(dev).contiguous() for t in batches[rank]), d, p, 1.0, 0.05, 0.01, 0.02,
-                                loss, stats)
-            stream.synchronize()
-        _idiom(kv)
-    rows = torch.empty(n * 2 * d)
-    kv.wait(kv.pull(torch.arange(n), rows))
-    kv.barrier()
-    kv.finalize()
-    return {"loss": float(loss.item()), "stats": stats.tolist(), "rows": rows.view(n, 2 * d).double(), "local": local,
-            "replicas": replicas}
+    assert sum(r["stats"][3] for r in res) == ref_pushes
+    assert sum(r["stats"][1] for r in res) > 0       # peer rows were read
+    torch.testing.assert_close(res[0]["rows"][0].double(), ref, rtol=RTOL, atol=ATOL)
+    torch.testing.assert_close(sum(r["loss"] for r in res), ref_loss, rtol=1e-4, atol=1e-3)
 
 
 @gpu
@@ -407,17 +279,15 @@ def test_step_on_replicas(p):
     g = torch.Generator().manual_seed(21 + p)
     table = _init_table(ne + nr, d, g)
     batches = [_batch(ne, nr, B, nn, g, distinct=True) for _ in range(WORLD)]
-    res = run_cluster(functools.partial(_replica_worker, table=table, batches=batches, d=d, p=p), world=WORLD, workers=1,
-                      mode="threads", value_lengths=2 * d, num_keys=ne + nr, dtype="float32", backend="cuda",
-                      options={"sys.techniques": "replication_only"})
-    assert sum(r["counters"]["replica_setups"] for r in res.values()) > 0
-    assert all(r["counters"]["protocol_errors"] == 0 for r in res.values())
+    res = on_replicas(_case(table, d, p, 0.01, 0.02), batches)
+    assert sum(r["counters"]["replica_setups"] for r in res) > 0
+    assert all(r["counters"]["protocol_errors"] == 0 for r in res)
     args = (d, p, 1.0, 0.05, 0.01, 0.02)
     ref, _, _ = _rule(table, batches, *args)
     for r in range(WORLD):
-        out = res[r][0]
+        out = res[r]
         assert out["local"] and out["replicas"] > 0, f"rank {r}: batch keys not local after the intents"
-        torch.testing.assert_close(out["rows"], ref, rtol=RTOL, atol=ATOL, msg=lambda m: f"rows read on rank {r}: {m}")
+        torch.testing.assert_close(out["rows"][0].double(), ref, rtol=RTOL, atol=ATOL, msg=lambda m: f"rows read on rank {r}: {m}")
         _, before_loss, before_pushes = _rule(table, batches[:r], *args) if r else (None, 0.0, 0)
         _, upto_loss, upto_pushes = _rule(table, batches[:r + 1], *args)
         s = out["stats"]
@@ -434,18 +304,15 @@ def test_step_loses_no_update_while_keys_move(technique):
     g = torch.Generator().manual_seed(9)
     table = _init_table(ne + nr, d, g)
     batches = [_batch(ne, nr, B, nn, g, distinct=True) for _ in range(32)]
-    done = threading.Event()
-    res = run_cluster(functools.partial(_inflight_step_worker, table=table, batches=batches, d=d, p=p, done=done),
-                      world=WORLD, workers=1, mode="threads", value_lengths=2 * d, num_keys=ne + nr, dtype="float32",
-                      backend="cuda", options={"sys.techniques": technique})
-    out = res[2][0]
-    relocations = sum(r["counters"]["relocations"] for r in res.values())
+    res = while_keys_move(_case(table, d, p, 0.0, 0.0), batches, technique)
+    out = res[2]
+    relocations = sum(r["counters"]["relocations"] for r in res)
     info = f"{technique}: stats {out['stats']}, relocations {relocations}"
     print(info)
-    assert relocations > 0 and all(r["counters"]["protocol_errors"] == 0 for r in res.values()), info
+    assert relocations > 0 and all(r["counters"]["protocol_errors"] == 0 for r in res), info
     ref, ref_loss, ref_pushes = _rule(table, batches, d, p, 1.0, 0.05, 0.0, 0.0)
     assert out["stats"][3] == ref_pushes, info
-    torch.testing.assert_close(out["rows"], ref, rtol=RTOL, atol=ATOL)
+    torch.testing.assert_close(out["rows"][0].double(), ref, rtol=RTOL, atol=ATOL)
     torch.testing.assert_close(out["loss"], ref_loss, rtol=1e-4, atol=1e-3)
 
 
@@ -469,62 +336,28 @@ def _dist_mr_inputs():
     return rows, q, keys, true_col, ex
 
 
-def _inflight_dist_worker(kv, server, wid, exp, done):
-    rank = server.my_rank()
-    rows, q, keys, true_col, (off, cols) = _dist_mr_inputs()
-    if rank == 0:
-        kv.wait(kv.set(torch.arange(DK), rows.contiguous().view(-1)))
-    kv.waitall(); kv.barrier()
-    out = {}
-    if rank < 2:
-        out["iters"] = _mover(kv, rank, torch.arange(0, DK, 8), done)
-    else:
-        dev = server.device
-        stream = torch.cuda.Stream(dev)
-        stats = torch.zeros(3, dtype=torch.int64, device=dev)
-        mism, reps = [], 0
-        try:
-            with torch.cuda.stream(stream):
-                args = (q.to(dev), keys.to(dev), true_col.to(dev), (off.to(dev), cols.to(dev)))
-                t0 = time.time()
-                while (reps < 8 or time.time() - t0 < 3.0) and reps < 200:
-                    got = _dist_all(server, *args, stats=stats)
-                    for k, v in got.items():
-                        if not all(torch.equal(a.cpu(), b) for a, b in zip(v, exp[k])):
-                            mism.append(k)
-                    reps += 1
-                stream.synchronize()
-        finally:
-            done.set()
-        out.update(mism=mism, reps=reps, stats=stats.tolist())
-    kv.barrier()
-    _idiom(kv)
-    kv.finalize()
-    return out
-
-
 @gpu
 def test_distance_kernels_bit_identical_while_keys_move():
     rows, q, keys, true_col, (off, cols) = _dist_mr_inputs()
-    s, kv = _store(DD, DK, "cuda", "float32", "dist1")
-    try:
+    with one_rank_store(DD, DK, "cuda", "float32") as (s, kv):
         kv.wait(kv.set(torch.arange(DK), rows.contiguous().view(-1)))
         dev = s.device
         exp = _dist_all(s, q.to(dev), keys.to(dev), true_col.to(dev), (off.to(dev), cols.to(dev)))
         exp = {k: tuple(t.cpu() for t in v) for k, v in exp.items()}
-    finally:
-        kv.finalize()
-        s.shutdown()
-    done = threading.Event()
-    res = run_cluster(functools.partial(_inflight_dist_worker, exp=exp, done=done), world=WORLD, workers=1,
-                      mode="threads", value_lengths=DD, num_keys=DK, dtype="float32", backend="cuda",
-                      options={"sys.techniques": "relocation_only"})
-    out = res[2][0]
-    relocations = sum(r["counters"]["relocations"] for r in res.values())
+
+    def read(server, kv, stats):
+        dev = server.device
+        args = (q.to(dev), keys.to(dev), true_col.to(dev), (off.to(dev), cols.to(dev)))
+        return lambda: _dist_all(server, *args, stats=stats)
+
+    res = reads_while_keys_move(Case(DD, DK, [(torch.arange(DK), rows)]), read, exp, torch.arange(0, DK, 8),
+                                "relocation_only")
+    out = res[2]
+    relocations = sum(r["counters"]["relocations"] for r in res)
     info = f"{out['reps']} repetitions, stats {out['stats']}, relocations {relocations}"
     print(info)
     assert relocations > 0, info
-    assert not out["mism"], f"{info}; mismatches: {sorted(set(out['mism']))}"
+    assert not out["mism"], f"{info}; mismatches: {sorted({k for _, k in out['mism']})}"
     assert out["stats"][2] == 0, info
 
 
@@ -533,16 +366,12 @@ def test_distance_kernels_bit_identical_while_keys_move():
 def test_fused_transe_quality_on_fb15k237_toy():
     """The fused step and the fused distance evaluation reach the CPU test's thresholds (published: MRR 0.60,
     Hits@10 84.86 %) with TransE L1, d = 152, eta 0.1, margin 3, neg_ratio 6, gamma 0, 12 epochs of 70 triples."""
-    import adapm_b200 as ad
     from adapm_b200.models.kge import KGE, KGEConfig, evaluate_fused, load_triples
 
     tr, va, te = (load_triples(os.path.join(GOLDEN, f"{n}.del")) for n in ("train", "valid", "test"))
     cfg = KGEConfig(num_entities=280, num_relations=112, embed_dim=152, algorithm="TransE", p_norm=1, margin=3.0,
                     eta=0.1, neg_ratio=6, gamma_entity=0.0, gamma_relation=0.0, batch_triples=70, deterministic=True)
-    server = ad.Server(cfg.value_lengths(), num_keys=cfg.num_keys, num_threads=1, rank=0, world=1, backend="cuda",
-                       fabric="inproc", job=f"transe_gq_{np.random.randint(1 << 30)}", device=0)
-    kv = ad.Worker(0, server)
-    try:
+    with one_rank_store(cfg.value_lengths(), cfg.num_keys, "cuda", "float32") as (server, kv):
         model = KGE(server, kv, cfg)
         model.init_model()
         for epoch in range(1, 13):
@@ -555,9 +384,6 @@ def test_fused_transe_quality_on_fb15k237_toy():
         ev = evaluate_fused(model, te, known)
         full = model.evaluate(te, known)
         idx, vals = model.predict(te[:8, 0], te[:8, 1], "object", k=10, known=known)
-    finally:
-        kv.finalize()
-        server.shutdown()
     print("TransE toy test (GPU):", ev)
     assert ev["mrr"] >= 0.50 and ev["hits@10"] >= 0.80, ev
     assert abs(full["mrr"] - ev["mrr"]) < 1e-9
