@@ -100,6 +100,38 @@ constexpr int kBprMaxNeg = 256;
 void mf_bpr_step(CudaBackend& be, cudaStream_t stream, const Key* users, const Key* pos, const Key* neg, int B, int n_neg,
                  int rank, float eps, float lam, float* loss_out, unsigned long long* stats, bool deterministic = false);
 
+// GloVe: fused pull + weighted least squares + AdaGrad + push (ops_glove.cu). One non-zero (words[i], ctxs[i], xs[i])
+// per i: the keys of a word row and a context row, X > 0. Rows [vector (d) | bias, 0, 0, 0 | AdaGrad (d + 4)],
+// d % 4 == 0, 4 <= d <= 508. stats[3] counts the pushes issued (2 per non-zero).
+constexpr int kGloveMaxDim = 508;
+void glove_step(CudaBackend& be, cudaStream_t stream, const Key* words, const Key* ctxs, const float* xs, int n, int d,
+                float eta, float x_max, float alpha, float* loss_out, unsigned long long* stats,
+                bool deterministic = false);
+
+// GloVe co-occurrence counts of an encoded corpus on the device (ops_cooc.cu): tokens[0 .. n_tokens) int32 word ids in
+// [0, V), sentence s = tokens[offsets[s] .. offsets[s + 1]). For every pair of positions of one sentence where word a
+// comes k <= window positions before word b, X[a][b] += 1 / k (1 without distance weighting), and with symmetric also
+// X[b][a]; only rows a with a % world == rank are kept. Sums are exact: integer numerators over lcm(1..window) in 64
+// bits, divided once at the end. Processed in token chunks so that the device memory of the call stays within
+// max_bytes; run() returns the number of non-zeros, write() stores them sorted by (row, col).
+constexpr int kCoocMaxWindow = 16;
+class Cooccurrence {
+ public:
+  Cooccurrence(cudaStream_t stream, const int32_t* tokens, int64_t n_tokens, const int64_t* offsets, int64_t n_sentences,
+               int64_t V, int window, bool symmetric, bool distance_weighting, int rank, int world, int64_t max_bytes);
+  ~Cooccurrence();
+  int64_t run();
+  void write(int32_t* rows, int32_t* cols, float* x) const;
+  int chunks() const { return chunks_; }
+  int64_t denominator() const { return lw_; }
+
+ private:
+  struct Impl;
+  Impl* impl_;
+  int chunks_ = 0;
+  int64_t lw_ = 1;
+};
+
 // alternating least squares for matrix factorisation (ops_als.cu). Target targets[t] (distinct) has the entries
 // others[offsets[t] .. offsets[t + 1]) with weights a, b; rows [factors (rank) | AdaGrad (rank)], rank % 4 == 0,
 // 4 <= rank <= 128. One CTA per target, in the given order: A = gram + lam I + sum_e a_e h_e h_e^T, r = sum_e b_e h_e,

@@ -142,6 +142,29 @@ void bind(py::module_& m) {
     mf_bpr_step(backend_of(be), (cudaStream_t)stream, ptr<const Key>(users), ptr<const Key>(pos), ptr<const Key>(neg), B,
                 n_neg, rank, eps, lam, ptr<float>(loss), ptr<unsigned long long>(stats), deterministic);
   });
+  m.attr("glove_max_dim") = kGloveMaxDim;
+  m.def("glove_step", [](uintptr_t be, uintptr_t stream, uintptr_t words, uintptr_t ctxs, uintptr_t xs, int n, int d,
+                         float eta, float x_max, float alpha, uintptr_t loss, uintptr_t stats, bool deterministic) {
+    glove_step(backend_of(be), (cudaStream_t)stream, ptr<const Key>(words), ptr<const Key>(ctxs), ptr<const float>(xs), n,
+               d, eta, x_max, alpha, ptr<float>(loss), ptr<unsigned long long>(stats), deterministic);
+  });
+  m.attr("cooc_max_window") = kCoocMaxWindow;
+  py::class_<Cooccurrence>(m, "Cooccurrence")
+      .def(py::init([](uintptr_t stream, uintptr_t tokens, int64_t n_tokens, uintptr_t offsets, int64_t n_sentences,
+                       int64_t V, int window, bool symmetric, bool distance_weighting, int rank, int world,
+                       int64_t max_bytes) {
+        return new Cooccurrence((cudaStream_t)stream, ptr<const int32_t>(tokens), n_tokens, ptr<const int64_t>(offsets),
+                                n_sentences, V, window, symmetric, distance_weighting, rank, world, max_bytes);
+      }))
+      .def("run", [](Cooccurrence& c) {
+        py::gil_scoped_release rel;
+        return c.run();
+      })
+      .def("write", [](const Cooccurrence& c, uintptr_t rows, uintptr_t cols, uintptr_t x) {
+        c.write(ptr<int32_t>(rows), ptr<int32_t>(cols), ptr<float>(x));
+      })
+      .def("chunks", &Cooccurrence::chunks)
+      .def("denominator", &Cooccurrence::denominator);
   m.attr("als_max_rank") = kAlsMaxRank;
   m.def("als_solve", [](uintptr_t be, uintptr_t stream, uintptr_t targets, uintptr_t offsets, uintptr_t others,
                         uintptr_t a, uintptr_t b, int n, int rank, float lam, uintptr_t gram, uintptr_t stats) {

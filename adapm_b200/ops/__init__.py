@@ -807,6 +807,150 @@ def bpr_reference_step(kv, users: torch.Tensor, pos: torch.Tensor, neg: torch.Te
     return loss, B * (2 + n)
 
 
+GLOVE_MAX_DIM = 508
+GLOVE_MAX_WINDOW = 16
+# default device-memory budget of glove_cooccurrence: leaves most of an 80 GB card to the training tables
+GLOVE_COOC_MAX_BYTES = 8 << 30
+
+
+def glove_cooccurrence(tokens: torch.Tensor, offsets: torch.Tensor, vocab_size: int, window: int,
+                       symmetric: bool = True, distance_weighting: bool = True, rank: int = 0, world: int = 1,
+                       max_bytes: int = GLOVE_COOC_MAX_BYTES, info: Optional[dict] = None):
+    """GloVe's co-occurrence matrix (glove.c's ``cooccur.c``) of an encoded corpus, counted on the device
+    (csrc/cuda/ops_cooc.cu). ``tokens``: int32 word ids in ``[0, vocab_size)``; ``offsets``: int64 ``[n_sentences + 1]``,
+    sentence ``s`` is ``tokens[offsets[s]:offsets[s + 1]]`` (both contiguous CUDA tensors, e.g. from
+    ``NativeCorpus.arrays()``). For every pair of positions of one sentence where word ``a`` comes ``k <= window``
+    positions before word ``b``, ``X[a][b] += 1 / k`` (``1`` with ``distance_weighting=False``), and with ``symmetric``
+    also ``X[b][a]``. Windows never cross a sentence. ``1 <= window <= 16``.
+
+    Only rows ``a`` with ``a % world == rank`` are kept: ranks that each count the whole corpus get disjoint partitions
+    that together make the full matrix. The sums are exact (integer numerators over ``lcm(1..window)`` in 64 bits,
+    divided once and rounded to float32), so the result is bit-identical to :func:`utils.text.cooccurrence_reference`
+    and independent of ``max_bytes``, which bounds the device memory of the call (the corpus is processed in token
+    chunks whose sorted counts are merged; the working set is allocated with ``cudaMalloc``, outside PyTorch's caching
+    allocator); a budget too small for the result raises ``RuntimeError``.
+
+    Returns ``(rows int32, cols int32, x float32)`` on the device of ``tokens``, sorted by ``(row, col)``. ``info``: a
+    dict that receives ``chunks`` (token chunks processed) and ``denominator`` (``lcm(1..window)`` or 1)."""
+    if not (tokens.is_cuda and tokens.dtype == torch.int32 and tokens.is_contiguous() and tokens.dim() == 1):
+        raise TypeError("tokens must be a contiguous 1-D CUDA int32 tensor")
+    if not (offsets.is_cuda and offsets.dtype == torch.int64 and offsets.is_contiguous() and offsets.dim() == 1
+            and offsets.device == tokens.device):
+        raise TypeError("offsets must be a contiguous 1-D CUDA int64 tensor on the device of tokens")
+    if offsets.numel() < 1 or int(offsets[0]) != 0 or int(offsets[-1]) != tokens.numel():
+        raise ValueError("offsets must start at 0 and end at the number of tokens")
+    if isinstance(window, bool) or int(window) != window or not 1 <= int(window) <= GLOVE_MAX_WINDOW:
+        raise ValueError(f"window must be an integer in [1, {GLOVE_MAX_WINDOW}], got {window}")
+    if not 1 <= int(world) or not 0 <= int(rank) < int(world):
+        raise ValueError(f"rank must be in [0, world), got rank {rank}, world {world}")
+    if int(vocab_size) < 1 or int(max_bytes) < 1:
+        raise ValueError("vocab_size and max_bytes must be positive")
+    dev = tokens.device
+    with torch.cuda.device(dev):
+        c = _C.Cooccurrence(_stream(tokens), tokens.data_ptr(), tokens.numel(), offsets.data_ptr(), offsets.numel() - 1,
+                            int(vocab_size), int(window), bool(symmetric), bool(distance_weighting), int(rank),
+                            int(world), int(max_bytes))
+        n = c.run()
+        rows = torch.empty(n, dtype=torch.int32, device=dev)
+        cols = torch.empty(n, dtype=torch.int32, device=dev)
+        x = torch.empty(n, dtype=torch.float32, device=dev)
+        c.write(rows.data_ptr(), cols.data_ptr(), x.data_ptr())
+        if info is not None:
+            info["chunks"], info["denominator"] = c.chunks(), c.denominator()
+        torch.cuda.current_stream(dev).synchronize()
+        del c
+    return rows, cols, x
+
+
+def _check_glove_dim(embed_dim: int) -> None:
+    if isinstance(embed_dim, bool) or int(embed_dim) != embed_dim or not (
+            4 <= int(embed_dim) <= GLOVE_MAX_DIM and int(embed_dim) % 4 == 0):
+        raise ValueError(f"embed_dim must be a multiple of 4 in [4, {GLOVE_MAX_DIM}], got {embed_dim}")
+
+
+def _check_glove_rates(x_max: float, alpha: float) -> None:
+    if not float(x_max) > 0 or not float(alpha) >= 0:
+        raise ValueError(f"x_max must be > 0 and alpha >= 0, got x_max {x_max}, alpha {alpha}")
+
+
+def glove_step(server, words: torch.Tensor, ctxs: torch.Tensor, x: torch.Tensor, embed_dim: int, eta: float,
+               x_max: float, alpha: float, loss: torch.Tensor, stats: Optional[torch.Tensor] = None,
+               deterministic: bool = False) -> None:
+    """Fused GloVe step (csrc/cuda/ops_glove.cu) on ``server``'s store: one warp per non-zero ``(words[b], ctxs[b],
+    x[b])``, where ``words`` holds the keys of word rows (``2 i``), ``ctxs`` those of context rows (``2 j + 1``) and
+    ``x > 0`` the co-occurrence values. Rows are ``[vector (d) | bias, 0, 0, 0 | AdaGrad (d + 4)]``, ``d = embed_dim``
+    a multiple of 4 in [4, 508]. The rule is :func:`glove_reference_step`'s: ``diff = <w, c> + b + b~ - ln X``, weight
+    ``f = min(1, (X / x_max)^alpha)``, loss ``f diff^2 / 2``, one AdaGrad push per row and non-zero (``2`` per
+    non-zero). ``loss``: float32[1], accumulated (+=); ``stats``: optional int64[4] accumulated with (local rows, peer
+    rows, slow-path rows, pushes issued).
+
+    The AdaGrad form is the project's (as for KGE and BPR): ``-eta g / sqrt(acc + g^2)`` with the accumulator as read,
+    which bounds every update by ``eta``. glove.c instead divides by the old accumulator and clips gradients at 100;
+    with the accumulators initialised to 1 (as ``GloVe.init_model`` does, glove.c's initial ``gradsq``) early steps
+    behave alike.
+
+    ``deterministic=True`` (single-GPU servers only): start-of-step reads, fixed-point sums, bit-identical runs (three
+    launches instead of one); the AdaGrad increment of one push is clamped to 2^24 there (see ops_glove.cu)."""
+    _i64(words, "words"); _i64(ctxs, "ctxs"); _f32(x, "x"); _f32(loss, "loss")
+    B = words.numel()
+    if ctxs.numel() != B or x.numel() != B:
+        raise ValueError("words, ctxs and x must have the same length")
+    _check_glove_dim(embed_dim)
+    _check_glove_rates(x_max, alpha)
+    if stats is not None and not (stats.is_cuda and stats.dtype == torch.int64 and stats.numel() >= 4):
+        raise TypeError("stats must be a CUDA int64 tensor with 4 entries")
+    det = _check_deterministic(server, deterministic)
+    _C.glove_step(server._impl.backend_handle(), _stream(words), words.data_ptr(), ctxs.data_ptr(), x.data_ptr(), B,
+                  int(embed_dim), float(eta), float(x_max), float(alpha), loss.data_ptr(),
+                  stats.data_ptr() if stats is not None else 0, det)
+
+
+def glove_reference_step(kv, words: torch.Tensor, ctxs: torch.Tensor, x: torch.Tensor, embed_dim: int, eta: float,
+                         x_max: float, alpha: float):
+    """The GloVe rule of :func:`glove_step` in float64 through Pull / Push (CPU servers, float64 rows, and the oracle of
+    the tests). Every row is read at the start of the step. Returns ``(loss, pushes)``.
+
+    Per non-zero with word row ``(w, b)`` and context row ``(c, b~)``: ``diff = <w, c> + b + b~ - ln X``, ``f =
+    (X / x_max)^alpha`` if ``X < x_max`` else 1, loss ``f diff^2 / 2``; gradients ``g_w = f diff c``, ``g_c = f diff
+    w``, ``g_b = g_b~ = f diff``; pushes ``[-eta g / sqrt(acc + g^2) | g^2]`` (0 where g == 0, so the padding stays 0)
+    with the pulled accumulator, each row once per non-zero."""
+    _check_glove_dim(embed_dim)
+    _check_glove_rates(x_max, alpha)
+    words, ctxs = words.reshape(-1).cpu(), ctxs.reshape(-1).cpu()
+    x = x.reshape(-1).cpu().to(torch.float64)
+    B, d = words.numel(), int(embed_dim)
+    if ctxs.numel() != B or x.numel() != B:
+        raise ValueError("words, ctxs and x must have the same length")
+    D = d + 4
+    f64 = torch.float64
+
+    def pull(keys):
+        v = torch.empty(keys.numel() * 2 * D, dtype=kv.server.dtype)
+        if keys.numel():
+            kv.wait(kv.pull(keys.contiguous(), v))
+        v = v.view(-1, 2 * D).to(f64)
+        return v[:, :D], v[:, D:]
+
+    W, Aw = pull(words)
+    C, Ac = pull(ctxs)
+    diff = (W[:, :d] * C[:, :d]).sum(-1) + W[:, d] + C[:, d] - torch.log(x)
+    f = torch.where(x < x_max, (x / x_max) ** alpha, torch.ones_like(x))
+    loss = float((0.5 * f * diff * diff).sum())
+    fd = (f * diff).unsqueeze(-1)
+    gw, gc = torch.zeros(B, D, dtype=f64), torch.zeros(B, D, dtype=f64)
+    gw[:, :d], gc[:, :d] = fd * C[:, :d], fd * W[:, :d]
+    gw[:, d], gc[:, d] = fd[:, 0], fd[:, 0]
+
+    def upd(g, a):
+        ue = torch.where(g != 0, -eta * g / torch.sqrt(a + g * g), torch.zeros_like(g))
+        return torch.cat([ue, g * g], -1).to(kv.server.dtype).contiguous().view(-1)
+
+    if B:
+        kv.wait(kv.push(words.contiguous(), upd(gw, Aw)))
+        kv.wait(kv.push(ctxs.contiguous(), upd(gc, Ac)))
+    return loss, 2 * B
+
+
 ALS_MAX_RANK = 128
 
 

@@ -152,6 +152,42 @@ def windows_from_sentences(sentences: Iterator[np.ndarray], window: int, batch_w
         yield t
 
 
+def cooccurrence_reference(sentences, vocab_size: int, window: int, symmetric: bool = True,
+                           distance_weighting: bool = True, rank: int = 0, world: int = 1):
+    """GloVe's co-occurrence matrix in numpy (the rule of ``ops.glove_cooccurrence``, its tests' oracle and the CPU
+    backend's counter). ``sentences``: arrays of word ids in ``[0, vocab_size)``; windows never cross a sentence. For
+    every pair of positions where word ``a`` comes ``k <= window`` positions before word ``b``, ``X[a][b] += 1 / k`` (1
+    without ``distance_weighting``), with ``symmetric`` also ``X[b][a]``; only rows ``a % world == rank`` are kept.
+    Numerators over ``lcm(1..window)`` are summed as int64 by packed key ``a * V + b`` and divided once (float64, then
+    rounded to float32). Returns ``(rows int32, cols int32, x float32)`` sorted by ``(row, col)``."""
+    if not 1 <= int(window) <= 16:
+        raise ValueError(f"window must be in [1, 16], got {window}")
+    V, window = int(vocab_size), int(window)
+    lw = int(np.lcm.reduce(np.arange(1, window + 1))) if distance_weighting else 1
+    sents = [np.asarray(s, dtype=np.int64) for s in sentences if len(s)]
+    if not sents:
+        e = np.zeros(0, np.int32)
+        return e, e.copy(), np.zeros(0, np.float32)
+    tok = np.concatenate(sents)
+    sid = np.repeat(np.arange(len(sents)), [s.size for s in sents])
+    keys, nums = [np.zeros(0, np.int64)], [np.zeros(0, np.int64)]
+    for k in range(1, min(window, tok.size - 1) + 1):
+        same = sid[k:] == sid[:-k]
+        a, b = tok[:-k][same], tok[k:][same]
+        num = lw // k if distance_weighting else 1
+        for r, c in ((a, b), (b, a)) if symmetric else ((a, b),):
+            m = r % world == rank
+            keys.append(r[m] * V + c[m])
+            nums.append(np.full(int(m.sum()), num, dtype=np.int64))
+    keys, nums = np.concatenate(keys), np.concatenate(nums)
+    uniq, inv = np.unique(keys, return_inverse=True)
+    sums = np.zeros(uniq.size, dtype=np.int64)
+    if keys.size:
+        order = np.argsort(inv, kind="stable")
+        sums = np.add.reduceat(nums[order], np.searchsorted(inv[order], np.arange(uniq.size)))
+    return (uniq // V).astype(np.int32), (uniq % V).astype(np.int32), (sums / lw).astype(np.float32)
+
+
 # ------------------------------------------------------------------------------------------ native loader
 class NativeCorpus:
     """C++ corpus (csrc/adapm/corpus.{h,cc}): same vocabulary rules as :class:`Vocabulary` (count-descending, ties by
@@ -194,6 +230,16 @@ class NativeCorpus:
         tok = np.ctypeslib.as_array((ctypes.c_int32 * max(n, 1)).from_address(self._impl.tokens_ptr()))[:n].copy()
         off = np.ctypeslib.as_array((ctypes.c_int64 * (ns + 1)).from_address(self._impl.sentence_offsets_ptr())).copy()
         return [tok[off[i]:off[i + 1]] for i in range(ns)]
+
+    def arrays(self):
+        """The encoded sentences as ``(tokens int32 [n_tokens], offsets int64 [n_sentences + 1])`` numpy copies: sentence
+        ``s`` is ``tokens[offsets[s]:offsets[s + 1]]`` (the input of ``ops.glove_cooccurrence``)."""
+        import ctypes
+
+        n, ns = self.num_tokens(), self.num_sentences()
+        tok = np.ctypeslib.as_array((ctypes.c_int32 * max(n, 1)).from_address(self._impl.tokens_ptr()))[:n].copy()
+        off = np.ctypeslib.as_array((ctypes.c_int64 * (ns + 1)).from_address(self._impl.sentence_offsets_ptr())).copy()
+        return tok, off
 
     def pair_batches(self, window: int, subsample: float, batch_pairs: int, seed: int, epoch: int = 0,
                      pin: bool = False, queue_depth: int = 8) -> Iterator[torch.Tensor]:
