@@ -225,6 +225,24 @@ PYBIND11_MODULE(_C, m) {
     }
     return py::make_tuple(i, j, x, c.rows, c.cols);
   });
+  m.def("read_edge_list", [](const std::string& path) {
+    EdgeList g;
+    { py::gil_scoped_release r; g = read_edge_list_file(path); }
+    const py::ssize_t n = (py::ssize_t)g.src.size();
+    py::array_t<int64_t> src(n), dst(n), ids((py::ssize_t)g.ids.size());
+    if (n) {
+      memcpy(src.mutable_data(), g.src.data(), (size_t)n * 8);
+      memcpy(dst.mutable_data(), g.dst.data(), (size_t)n * 8);
+    }
+    if (!g.ids.empty()) memcpy(ids.mutable_data(), g.ids.data(), g.ids.size() * 8);
+    py::object w = py::none();
+    if (!g.weight.empty()) {
+      py::array_t<double> wa(n);
+      memcpy(wa.mutable_data(), g.weight.data(), (size_t)n * 8);
+      w = wa;
+    }
+    return py::make_tuple(src, dst, w, ids);
+  });
 
   m.attr("max_huffman_depth") = kMaxHuffmanDepth;
   m.def("huffman_tree", [](py::array_t<double, py::array::c_style | py::array::forcecast> counts) {

@@ -132,6 +132,23 @@ class Cooccurrence {
   int64_t lw_ = 1;
 };
 
+// node2vec / DeepWalk random walks on a CSR graph (ops_walk.cu; the rule is in its header): walk w starts at
+// starts[w] and is numbered walk_nos[w]; out [n_walks, L] int64, -1 after a node without out-edges. cumw: the inclusive
+// prefix sums of the quantised weights per node (null: unweighted). second_order: rejection sampling with the 24-bit
+// acceptance thresholds of alpha = 1 / p (return), 1 (x in N(t)) and 1 / q (outward); else first order. 1 launch.
+void node2vec_walks(cudaStream_t stream, const int64_t* offsets, const int32_t* nbrs, const int64_t* cumw,
+                    const int64_t* starts, const int64_t* walk_nos, int64_t n_walks, int L, uint64_t seed,
+                    uint64_t epoch, uint32_t thr_return, uint32_t thr_in, uint32_t thr_out, bool second_order,
+                    int64_t* out);
+// skip-gram pairs of walks [n_walks, L] (ops_walk.cu): walk_pair_ends writes each position's pair count to counts
+// and their inclusive scan to ends (cub, temp of walk_pair_scan_bytes(n_walks * L) bytes; 2 launches);
+// walk_pairs_write then stores the ends[last] pairs as out [2, n_pairs] (1 launch).
+size_t walk_pair_scan_bytes(int64_t n_items);
+void walk_pair_ends(cudaStream_t stream, const int64_t* walks, int64_t n_walks, int L, int window, uint64_t seed,
+                    int64_t* counts, int64_t* ends, void* temp, size_t temp_bytes);
+void walk_pairs_write(cudaStream_t stream, const int64_t* walks, int64_t n_walks, int L, int window, uint64_t seed,
+                      const int64_t* ends, int64_t n_pairs, Key* out);
+
 // alternating least squares for matrix factorisation (ops_als.cu). Target targets[t] (distinct) has the entries
 // others[offsets[t] .. offsets[t + 1]) with weights a, b; rows [factors (rank) | AdaGrad (rank)], rank % 4 == 0,
 // 4 <= rank <= 128. One CTA per target, in the given order: A = gram + lam I + sum_e a_e h_e h_e^T, r = sum_e b_e h_e,

@@ -165,6 +165,24 @@ void bind(py::module_& m) {
       })
       .def("chunks", &Cooccurrence::chunks)
       .def("denominator", &Cooccurrence::denominator);
+  m.def("node2vec_walks", [](uintptr_t stream, uintptr_t offsets, uintptr_t nbrs, uintptr_t cumw, uintptr_t starts,
+                             uintptr_t walk_nos, int64_t n_walks, int L, uint64_t seed, uint64_t epoch,
+                             uint32_t thr_return, uint32_t thr_in, uint32_t thr_out, bool second_order, uintptr_t out) {
+    node2vec_walks((cudaStream_t)stream, ptr<const int64_t>(offsets), ptr<const int32_t>(nbrs), ptr<const int64_t>(cumw),
+                   ptr<const int64_t>(starts), ptr<const int64_t>(walk_nos), n_walks, L, seed, epoch, thr_return, thr_in,
+                   thr_out, second_order, ptr<int64_t>(out));
+  });
+  m.def("walk_pair_scan_bytes", [](int64_t n_items) { return walk_pair_scan_bytes(n_items); });
+  m.def("walk_pair_ends", [](uintptr_t stream, uintptr_t walks, int64_t n_walks, int L, int window, uint64_t seed,
+                             uintptr_t counts, uintptr_t ends, uintptr_t temp, size_t temp_bytes) {
+    walk_pair_ends((cudaStream_t)stream, ptr<const int64_t>(walks), n_walks, L, window, seed, ptr<int64_t>(counts),
+                   ptr<int64_t>(ends), ptr<void>(temp), temp_bytes);
+  });
+  m.def("walk_pairs_write", [](uintptr_t stream, uintptr_t walks, int64_t n_walks, int L, int window, uint64_t seed,
+                               uintptr_t ends, int64_t n_pairs, uintptr_t out) {
+    walk_pairs_write((cudaStream_t)stream, ptr<const int64_t>(walks), n_walks, L, window, seed, ptr<const int64_t>(ends),
+                     n_pairs, ptr<Key>(out));
+  });
   m.attr("als_max_rank") = kAlsMaxRank;
   m.def("als_solve", [](uintptr_t be, uintptr_t stream, uintptr_t targets, uintptr_t offsets, uintptr_t others,
                         uintptr_t a, uintptr_t b, int n, int rank, float lam, uintptr_t gram, uintptr_t stats) {

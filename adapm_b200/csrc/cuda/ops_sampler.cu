@@ -4,6 +4,7 @@
 // key is resident on this node; never communicates; does not preserve the distribution).
 #include <cuda_runtime.h>
 
+#include "hash.cuh"
 #include "ops.h"
 #include "pm_kernels.cuh"
 
@@ -11,13 +12,6 @@ namespace adapm {
 namespace cudaops {
 
 namespace {
-
-__device__ __forceinline__ uint64_t mix64(uint64_t x) {
-  x ^= x >> 33; x *= 0xff51afd7ed558ccdULL;
-  x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ULL;
-  x ^= x >> 33;
-  return x;
-}
 
 // kind: 0 = alias table, 1 = uniform over [first, first+n), 2 = log-uniform over [first, first+n)
 __device__ __forceinline__ Key draw_key(int kind, const float* __restrict__ prob, const int32_t* __restrict__ alias,

@@ -7,8 +7,10 @@ fallback on a GPU box.
 """
 from __future__ import annotations
 
+import math
 from typing import Optional
 
+import numpy as np
 import torch
 
 from .. import _C
@@ -1779,3 +1781,209 @@ class IntentPrepass:
         """Hands the left-over keys of completed submissions to the host path (all submissions when ``block``)."""
         for s in self._slots:
             self._finish(s, block)
+
+
+# ---------------------------------------------------------------------------------------------- node2vec walks
+_U64 = (1 << 64) - 1
+_M1, _M2 = np.uint64(0xff51afd7ed558ccd), np.uint64(0xc4ceb9fe1a85ec53)
+
+
+def _mix64_np(x: np.ndarray) -> np.ndarray:
+    """``mix64`` of csrc/cuda/hash.cuh on a uint64 array (integer arrays wrap on overflow)"""
+    s = np.uint64(33)
+    x = x ^ (x >> s)
+    x = x * _M1
+    x = x ^ (x >> s)
+    x = x * _M2
+    return x ^ (x >> s)
+
+
+def _mix64_int(x: int) -> int:
+    return int(_mix64_np(np.array([int(x) & _U64], dtype=np.uint64))[0])
+
+
+def _umulhi_np(a: np.ndarray, b: np.ndarray) -> np.ndarray:
+    """the high 64 bits of a * b for uint64 arrays (``__umul64hi``)"""
+    m, s = np.uint64(0xFFFFFFFF), np.uint64(32)
+    al, ah, bl, bh = a & m, a >> s, b & m, b >> s
+    ll, hl, lh = al * bl, ah * bl, al * bh
+    cross = (ll >> s) + (hl & m) + lh
+    return ah * bh + (hl >> s) + (cross >> s)
+
+
+def walk_thresholds(p: float, q: float):
+    """The 24-bit acceptance thresholds of node2vec's rejection rule, ``max(1, round(alpha / alpha_max * 2^24))`` for
+    alpha = 1 / p (return to the previous node), 1 (a neighbour of the previous node) and 1 / q (outward), and whether
+    the walk is second order (not ``p == q == 1``)."""
+    p, q = float(p), float(q)
+    if not (math.isfinite(p) and math.isfinite(q) and p > 0 and q > 0):
+        raise ValueError(f"p and q must be positive and finite, got p {p}, q {q}")
+    a = (1.0 / p, 1.0, 1.0 / q)
+    top = max(a)
+    thr = tuple(max(1, int(round(x / top * (1 << 24)))) for x in a)
+    return thr, not (p == 1.0 and q == 1.0)
+
+
+def _check_walk_length(walk_length) -> int:
+    if isinstance(walk_length, bool) or int(walk_length) != walk_length or int(walk_length) < 2:
+        raise ValueError(f"walk_length must be an integer >= 2, got {walk_length}")
+    return int(walk_length)
+
+
+def _check_window(window) -> int:
+    if isinstance(window, bool) or int(window) != window or int(window) < 1:
+        raise ValueError(f"window must be an integer >= 1, got {window}")
+    return int(window)
+
+
+def _walk_starts(graph, starts, walk_numbers):
+    """(starts, walk numbers) as int64 numpy arrays of one shape, checked against the graph"""
+    s = (starts.cpu().numpy() if isinstance(starts, torch.Tensor) else np.asarray(starts)).reshape(-1)
+    if s.size and not np.issubdtype(s.dtype, np.integer):
+        raise ValueError(f"starts must be integer node ids, got dtype {s.dtype}")
+    s = s.astype(np.int64)
+    if isinstance(walk_numbers, torch.Tensor):
+        walk_numbers = walk_numbers.cpu().numpy()
+    wn = np.broadcast_to(np.asarray(walk_numbers, dtype=np.int64).reshape(-1) if np.ndim(walk_numbers) else
+                         np.int64(walk_numbers), s.shape).astype(np.int64)
+    if s.size and (int(s.min()) < 0 or int(s.max()) >= graph.num_nodes):
+        raise ValueError(f"start ids must be in [0, {graph.num_nodes})")
+    if wn.size and int(wn.min()) < 0:
+        raise ValueError("walk numbers must be non-negative")
+    return s, wn
+
+
+def random_walks(graph, starts, walk_numbers, walk_length: int, p: float = 1.0, q: float = 1.0, seed: int = 0,
+                 epoch: int = 0) -> torch.Tensor:
+    """node2vec walks on the device (csrc/cuda/ops_walk.cu): walk ``w`` starts at ``starts[w]`` and is the
+    ``walk_numbers[w]``-th walk from it (an int applies to every walk). Returns int64 ``[n, walk_length]`` on the graph's
+    device; position 0 is the start, and the positions after a node without out-edges are -1. First order (DeepWalk)
+    when ``p == q == 1``, else node2vec's second-order walk by rejection sampling; weighted graphs draw by their quantised
+    weights. Every draw is a counter hash of ``(seed, epoch, start, walk number, step, trial)``, so a walk does not
+    depend on which call, chunk or rank makes it, and :func:`random_walks_reference` gives the same walks bit for bit.
+
+    ``starts`` and ``walk_numbers`` are checked on the host: pass CPU tensors or arrays to keep the call free of device
+    synchronisation. ``ValueError`` on ``p, q <= 0``, ``walk_length < 2``, start ids out of range, or a graph that is
+    not on a CUDA device."""
+    if not graph.offsets.is_cuda:
+        raise ValueError("random_walks needs a graph on a CUDA device (Graph.to('cuda')); use random_walks_reference "
+                         "on the CPU")
+    L = _check_walk_length(walk_length)
+    (t_ret, t_in, t_out), second = walk_thresholds(p, q)
+    s, wn = _walk_starts(graph, starts, walk_numbers)
+    dev = graph.device
+    out = torch.empty(s.size, L, dtype=torch.int64, device=dev)
+    if s.size == 0:
+        return out
+    sd = torch.from_numpy(s).to(dev, non_blocking=True)
+    wd = torch.from_numpy(np.ascontiguousarray(wn)).to(dev, non_blocking=True)
+    with torch.cuda.device(dev):
+        _C.node2vec_walks(_stream(out), graph.offsets.data_ptr(), graph.neighbors.data_ptr(),
+                          graph.cum_weights.data_ptr() if graph.weighted else 0, sd.data_ptr(), wd.data_ptr(), s.size,
+                          L, int(seed) & _U64, int(epoch) & _U64, t_ret, t_in, t_out, second, out.data_ptr())
+    return out
+
+
+def walk_pairs(walks: torch.Tensor, window: int, seed: int = 0) -> torch.Tensor:
+    """Skip-gram pairs of walks ``[n, L]`` (int64 CUDA, -1 padding after a walk's end) in the layout ``sgns_step``
+    takes: int64 ``[2, n_pairs]``, row 0 the syn0 keys ``2 walk[j]``, row 1 the syn1 keys ``2 walk[i] + 1``. Position
+    ``i`` of walk row ``r`` draws a window shrink ``b`` in ``[0, window)`` by a counter hash of ``(seed, r, i)`` and pairs
+    with every position ``j != i`` of its walk within ``window - b``: walk-major, then ``i``, then ascending ``j``, the
+    order of ``utils.text.pairs_from_sentences``. Count kernel, cub scan, write kernel; reading the pair count is the
+    call's one host synchronisation. :func:`walk_pairs_reference` is the same rule in numpy."""
+    if not (walks.is_cuda and walks.dtype == torch.int64 and walks.dim() == 2 and walks.is_contiguous()):
+        raise TypeError("walks must be a contiguous 2-D CUDA int64 tensor")
+    W = _check_window(window)
+    n, L = walks.shape
+    dev = walks.device
+    if n * L == 0:
+        return torch.empty(2, 0, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        counts = torch.empty(n * L, dtype=torch.int64, device=dev)
+        ends = torch.empty(n * L, dtype=torch.int64, device=dev)
+        temp = torch.empty(max(1, _C.walk_pair_scan_bytes(n * L)), dtype=torch.uint8, device=dev)
+        s = int(seed) & _U64
+        _C.walk_pair_ends(_stream(walks), walks.data_ptr(), n, L, W, s, counts.data_ptr(), ends.data_ptr(),
+                          temp.data_ptr(), temp.numel())
+        P = int(ends[-1])
+        out = torch.empty(2, P, dtype=torch.int64, device=dev)
+        _C.walk_pairs_write(_stream(walks), walks.data_ptr(), n, L, W, s, ends.data_ptr(), P, out.data_ptr())
+    return out
+
+
+def random_walks_reference(graph, starts, walk_numbers, walk_length: int, p: float = 1.0, q: float = 1.0,
+                           seed: int = 0, epoch: int = 0) -> np.ndarray:
+    """The walks of :func:`random_walks` in numpy (int64 ``[n, walk_length]``), with the same integer rule; the CPU
+    backend's walk generator and the device kernels' oracle. The graph may be on any device."""
+    L = _check_walk_length(walk_length)
+    (t_ret, t_in, t_out), second = walk_thresholds(p, q)
+    s, wn = _walk_starts(graph, starts, walk_numbers)
+    off = graph.offsets.cpu().numpy()
+    nbr = graph.neighbors.cpu().numpy().astype(np.int64)
+    n = graph.num_nodes
+    deg = np.diff(off)
+    src = np.repeat(np.arange(n, dtype=np.int64), deg)
+    edge_key = src * n + nbr                                            # sorted: the CSR is sorted by (node, neighbour)
+    if graph.weighted:
+        cw = graph.cum_weights.cpu().numpy()
+        total = np.zeros(n + 1, dtype=np.int64)
+        last = off[1:] - 1
+        total[1:] = np.cumsum(np.where(deg > 0, cw[np.maximum(last, 0)], 0))
+        glob = (cw + np.repeat(total[:-1], deg)).astype(np.uint64)      # strictly increasing over all edges
+    s0 = _mix64_int(_mix64_int(seed) ^ (int(epoch) & _U64))
+    out = np.full((s.size, L), -1, dtype=np.int64)
+    out[:, 0] = s
+    base = _mix64_np(_mix64_np(np.uint64(s0) ^ s.astype(np.uint64)) ^ wn.astype(np.uint64))
+    v, t = s.copy(), np.full(s.size, -1, dtype=np.int64)
+    alive = np.arange(s.size)
+    for k in range(1, L):
+        alive = alive[deg[v[alive]] > 0]
+        if alive.size == 0:
+            break
+        x_new = np.empty(alive.size, dtype=np.int64)
+        pend = np.arange(alive.size)
+        j = 0
+        while pend.size:
+            w = alive[pend]
+            h = _mix64_np(base[w] ^ np.uint64((k << 32) | j))
+            vv = v[w]
+            if graph.weighted:
+                r = _umulhi_np(h, cw[off[vv + 1] - 1].astype(np.uint64))
+                e = np.searchsorted(glob, total[vv].astype(np.uint64) + r, side="right")
+            else:
+                e = off[vv] + ((h >> np.uint64(32)) * deg[vv].astype(np.uint64) >> np.uint64(32)).astype(np.int64)
+            x = nbr[e]
+            acc = np.ones(pend.size, dtype=bool)
+            if second and k >= 2:
+                u = (_mix64_np(h) >> np.uint64(40)).astype(np.int64)
+                tt = t[w]
+                key = tt * n + x
+                pos = np.minimum(np.searchsorted(edge_key, key), max(edge_key.size - 1, 0))
+                inn = (edge_key[pos] == key) if edge_key.size else np.zeros(pend.size, dtype=bool)
+                thr = np.where(x == tt, t_ret, np.where(inn, t_in, t_out))
+                acc = u < thr
+            x_new[pend[acc]] = x[acc]
+            pend = pend[~acc]
+            j += 1
+        out[alive, k] = x_new
+        t[alive] = v[alive]
+        v[alive] = x_new
+    return out
+
+
+def walk_pairs_reference(walks, window: int, seed: int = 0) -> np.ndarray:
+    """The pairs of :func:`walk_pairs` in numpy: int64 ``[2, n_pairs]``."""
+    W = _check_window(window)
+    w = walks.cpu().numpy() if isinstance(walks, torch.Tensor) else np.asarray(walks, dtype=np.int64)
+    n, L = w.shape
+    r = np.arange(n, dtype=np.uint64).reshape(n, 1)
+    i = np.arange(L, dtype=np.uint64).reshape(1, L)
+    h = _mix64_np(np.uint64(_mix64_int(seed)) ^ ((r << np.uint64(32)) | i))
+    rad = W - ((h >> np.uint64(32)) * np.uint64(W) >> np.uint64(32)).astype(np.int64)     # [n, L]
+    delta = np.concatenate([np.arange(-W, 0), np.arange(1, W + 1)])                       # ascending j = i + delta
+    jj = np.arange(L).reshape(1, L, 1) + delta.reshape(1, 1, -1)
+    inside = (jj >= 0) & (jj < L)
+    ctx = w[np.arange(n).reshape(n, 1, 1), np.clip(jj, 0, L - 1)]                           # [n, L, 2 W]
+    keep = inside & (np.abs(delta).reshape(1, 1, -1) <= rad[:, :, None]) & (w[:, :, None] >= 0) & (ctx >= 0)
+    centre = np.broadcast_to(w[:, :, None], keep.shape)
+    return np.stack([2 * ctx[keep], 2 * centre[keep] + 1]).astype(np.int64)
