@@ -8,6 +8,9 @@
 //   local   nothing at PrepareSample; PullSample rejects draws until a key is resident
 //           locally (or, for a declared contiguous key range, walks upward to the next
 //           resident key). Never communicates; does not preserve the distribution.
+#include <cmath>
+#include <cstdint>
+
 #include "node.h"
 
 namespace adapm {
@@ -74,8 +77,16 @@ class CallbackDist : public KeyDistribution {
 }  // namespace
 
 void build_alias_table(const double* w, int64_t n, float* prob, int32_t* alias) {
+  ADAPM_CHECK(n >= 1, "alias table: needs at least one weight");
+  ADAPM_CHECK(n <= INT32_MAX, "alias table: " << n << " weights, at most " << INT32_MAX << " fit the int32 alias");
   double sum = 0;
-  for (int64_t i = 0; i < n; ++i) sum += w[i];
+  for (int64_t i = 0; i < n; ++i) {
+    // a negative weight yields prob < 0 and an infinite one prob = 0 for every other key: both draw garbage silently
+    ADAPM_CHECK(std::isfinite(w[i]) && w[i] >= 0, "alias table: weight " << i << " is " << w[i]
+                                                                          << ", weights must be finite and >= 0");
+    sum += w[i];
+  }
+  ADAPM_CHECK(std::isfinite(sum), "alias table: the weights' sum overflows a double");
   ADAPM_CHECK(sum > 0, "alias table: weights sum to zero");
   std::vector<double> p(n);
   std::vector<int64_t> small, large;

@@ -4,6 +4,8 @@
 // key is resident on this node; never communicates; does not preserve the distribution).
 #include <cuda_runtime.h>
 
+#include <cmath>
+
 #include "hash.cuh"
 #include "ops.h"
 #include "pm_kernels.cuh"
@@ -13,9 +15,10 @@ namespace cudaops {
 
 namespace {
 
-// kind: 0 = alias table, 1 = uniform over [first, first+n), 2 = log-uniform over [first, first+n)
+// kind: 0 = alias table, 1 = uniform over [first, first+n), 2 = log-uniform over [first, first+n); lg = ln(n + 1)
+// (log-uniform only). The rules are replayed bit for bit by ops.sample_keys_reference.
 __device__ __forceinline__ Key draw_key(int kind, const float* __restrict__ prob, const int32_t* __restrict__ alias,
-                                        int64_t n, Key first, Key stride, uint64_t h) {
+                                        int64_t n, double lg, Key first, Key stride, uint64_t h) {
   uint32_t hi = (uint32_t)(h >> 32), lo = (uint32_t)h;
   if (kind == 0) {
     int64_t i = (int64_t)(((uint64_t)hi * (uint64_t)n) >> 32);
@@ -24,9 +27,10 @@ __device__ __forceinline__ Key draw_key(int kind, const float* __restrict__ prob
     return first + j * stride;
   }
   if (kind == 1) return first + (Key)(((uint64_t)hi * (uint64_t)n) >> 32) * stride;
-  // log-uniform: floor(exp(u * ln(n + 1))) - 1   (reference bindings.cc:72-76)
-  float u = (float)hi * 2.3283064365386963e-10f;
-  int64_t j = (int64_t)(__expf(u * __logf((float)(n + 1)))) - 1;
+  // log-uniform: floor(exp(u * ln(n + 1))) - 1   (reference bindings.cc:72-76), u = hi / 2^32. In double: float32 u
+  // and the fast intrinsics err by about 1e-6 relative, which moves whole keys once n reaches 10^5 to 10^6.
+  double u = (double)hi * 0x1p-32;
+  int64_t j = (int64_t)exp(u * lg) - 1;
   j = j < 0 ? 0 : (j >= n ? n - 1 : j);
   return first + j * stride;
 }
@@ -41,7 +45,7 @@ __device__ __forceinline__ bool resident_weak(const Ctx& c, Key k) {
 }
 
 __global__ void sample_kernel(const __grid_constant__ Ctx c, int kind, const float* __restrict__ prob,
-                              const int32_t* __restrict__ alias, int64_t n_table, Key first, Key stride,
+                              const int32_t* __restrict__ alias, int64_t n_table, double lg, Key first, Key stride,
                               Key* __restrict__ out, int64_t n, uint64_t seed, int local_only, int max_tries,
                               unsigned long long* __restrict__ stats) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -51,7 +55,7 @@ __global__ void sample_kernel(const __grid_constant__ Ctx c, int kind, const flo
     int t = 0;
     for (;;) {
       uint64_t h = mix64(seed ^ ((uint64_t)i * 0x9E3779B97F4A7C15ULL + (uint64_t)t * 0xD1B54A32D192ED03ULL));
-      k = draw_key(kind, prob, alias, n_table, first, stride, h);
+      k = draw_key(kind, prob, alias, n_table, lg, first, stride, h);
       if (!local_only) break;
       ++checks;
       if (resident_weak(c, k)) break;
@@ -77,11 +81,14 @@ __global__ void sample_kernel(const __grid_constant__ Ctx c, int kind, const flo
 void sample_keys(CudaBackend& be, cudaStream_t stream, int kind, const float* prob, const int32_t* alias,
                  int64_t n_table, Key first, Key stride, Key* out, int64_t n, uint64_t seed, bool local_only,
                  int max_tries, unsigned long long* stats) {
+  // the bucket is (hi * n_table) >> 32 in 64 bits, and an alias index is an int32
+  ADAPM_CHECK(n_table >= 1 && n_table < (kind == 0 ? ((int64_t)1 << 31) : ((int64_t)1 << 32)),
+              "sample_keys: " << n_table << " keys, need 1 <= keys < " << (kind == 0 ? "2^31" : "2^32"));
   if (n == 0) return;
   be.track_stream(stream);
   int blocks = (int)((n + 255) / 256);
-  sample_kernel<<<blocks, 256, 0, stream>>>(be.ctx(), kind, prob, alias, n_table, first, stride, out, n, seed,
-                                            local_only ? 1 : 0, max_tries, stats);
+  sample_kernel<<<blocks, 256, 0, stream>>>(be.ctx(), kind, prob, alias, n_table, std::log((double)(n_table + 1)),
+                                            first, stride, out, n, seed, local_only ? 1 : 0, max_tries, stats);
   ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cudaGetLastError());
 }

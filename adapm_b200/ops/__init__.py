@@ -213,6 +213,11 @@ class DeviceSampler:
 
     ``local_only=True`` implements the reference's *local* sampling scheme (sampling.h:361-446):
     draws are rejected until the key is resident in this GPU's HBM (owned or usable replica).
+
+    Draw ``i`` of a call is a pure function of ``(seed, i)`` and the table; :func:`sample_keys_reference` replays it bit
+    for bit and :func:`alias_draw_probabilities` gives the exact distribution a table draws. ``ValueError`` on weights
+    that are negative, NaN or infinite, none or all zero, or more than 2^31 - 1 of them, and on ``num_keys`` outside
+    ``[1, 2^32)``.
     """
 
     def __init__(self, server, *, weights: Optional[torch.Tensor] = None, distribution: str = "alias",
@@ -221,17 +226,27 @@ class DeviceSampler:
         self.first_key, self.key_stride = int(first_key), int(key_stride)
         dev = server.device
         if weights is not None:
-            w = torch.as_tensor(weights, dtype=torch.float64).contiguous().cpu()
+            w = torch.as_tensor(weights, dtype=torch.float64)
             n = w.numel()
+            if n > (1 << 31) - 1:                    # before the weights are copied: the int32 alias cannot index them
+                raise ValueError(f"{n} weights, at most 2^31 - 1 fit the alias table")
+            w = w.contiguous().cpu()
             prob = torch.empty(n, dtype=torch.float32)
             alias = torch.empty(n, dtype=torch.int32)
-            _C.build_alias_table(w.data_ptr(), n, prob.data_ptr(), alias.data_ptr())
+            try:
+                _C.build_alias_table(w.data_ptr(), n, prob.data_ptr(), alias.data_ptr())
+            except _C.AdapmError as e:
+                raise ValueError(str(e)) from None
             self.kind, self.n = 0, n
             self.prob, self.alias = prob.to(dev), alias.to(dev)
         else:
             if num_keys is None:
                 raise ValueError("num_keys is required for uniform / log-uniform sampling")
-            self.kind = {"uniform": 1, "log-uniform": 2}[distribution]
+            if distribution not in ("uniform", "log-uniform"):
+                raise ValueError(f"distribution must be 'uniform' or 'log-uniform' without weights, got {distribution!r}")
+            if not 1 <= int(num_keys) < 1 << 32:     # the bucket is (hi * num_keys) >> 32 in 64 bits
+                raise ValueError(f"num_keys must be in [1, 2^32), got {num_keys}")
+            self.kind = _SAMPLER_KINDS[distribution]
             self.n = int(num_keys)
             self.prob = torch.zeros(1, dtype=torch.float32, device=dev)
             self.alias = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -1987,3 +2002,102 @@ def walk_pairs_reference(walks, window: int, seed: int = 0) -> np.ndarray:
     keep = inside & (np.abs(delta).reshape(1, 1, -1) <= rad[:, :, None]) & (w[:, :, None] >= 0) & (ctx >= 0)
     centre = np.broadcast_to(w[:, :, None], keep.shape)
     return np.stack([2 * ctx[keep], 2 * centre[keep] + 1]).astype(np.int64)
+
+
+# ---------------------------------------------------------------------------------------------- device key sampler
+_SAMPLER_KINDS = {"alias": 0, "uniform": 1, "log-uniform": 2}
+
+
+def _sampler_hash(seed: int, i: np.ndarray, t: int) -> np.ndarray:
+    """the 64-bit hash of try ``t`` of draws ``i`` (uint64 array): ``mix64(seed ^ (i * C1 + t * C2))``"""
+    ti = np.uint64((int(t) * 0xD1B54A32D192ED03) & _U64)
+    return _mix64_np(np.uint64(int(seed) & _U64) ^ (i * np.uint64(0x9E3779B97F4A7C15) + ti))
+
+
+def _sampler_draw(kind: int, h: np.ndarray, prob, alias, n_table: int, first: int, stride: int) -> np.ndarray:
+    hi, lo = h >> np.uint64(32), (h & np.uint64(0xFFFFFFFF)).astype(np.uint32)
+    if kind == 2:
+        x = np.exp(hi.astype(np.float64) * 2.0 ** -32 * math.log(n_table + 1))
+        j = np.clip(np.floor(x).astype(np.int64) - 1, 0, n_table - 1)
+    else:
+        j = ((hi * np.uint64(n_table)) >> np.uint64(32)).astype(np.int64)
+        if kind == 0:
+            u = lo.astype(np.float32) * np.float32(2.0 ** -32)     # the device's round-to-nearest cast, exact scaling
+            j = np.where(u < prob[j], j, alias[j].astype(np.int64))
+    return first + j * stride
+
+
+def sample_keys_reference(n: int, seed: int, *, distribution: str = "alias", prob=None, alias=None,
+                          num_keys: Optional[int] = None, first_key: int = 0, key_stride: int = 1, resident=None,
+                          max_tries: int = 64, chunk: int = 1 << 22):
+    """The ``n`` keys of :meth:`DeviceSampler.sample` (csrc/cuda/ops_sampler.cu) in numpy, bit for bit; the device
+    kernel's oracle. Draw ``i``, try ``t`` hashes ``h = mix64(seed ^ (i * 0x9E3779B97F4A7C15 + t * 0xD1B54A32D192ED03))``
+    and splits it into ``hi = h >> 32`` and ``lo = h mod 2^32``:
+
+    - ``alias`` (``prob`` float32 and ``alias`` int32 of the table): bucket ``b = (hi * n) >> 32``, ``u = float32(lo) *
+      2^-32`` (round to nearest, as the device casts), index ``b if u < prob[b] else alias[b]``;
+    - ``uniform`` over ``num_keys``: index ``(hi * num_keys) >> 32``;
+    - ``log-uniform`` over ``num_keys``: index ``floor(exp(hi * 2^-32 * ln(num_keys + 1))) - 1`` in float64, clamped
+      to ``[0, num_keys)``. The device takes ``exp`` in double too, so the two agree except where the value lies within
+      a few ulps of an integer.
+
+    The key is ``first_key + index * key_stride``. With ``resident`` (a bool array over keys: the residency the
+    ``local_only`` kernel probes), a draw that is not resident is redrawn with ``t + 1`` until one is or ``max_tries``
+    draws were made (then the last draw is kept: a give-up); returns ``(keys, checks, misses)``, the draws made and the
+    give-ups, as the kernel counts them into ``stats``. Otherwise returns the keys (int64 numpy array)."""
+    kind = _SAMPLER_KINDS[distribution]
+    if kind == 0:
+        prob = np.asarray(prob.cpu() if isinstance(prob, torch.Tensor) else prob, dtype=np.float32)
+        alias = np.asarray(alias.cpu() if isinstance(alias, torch.Tensor) else alias, dtype=np.int64)
+        n_table = prob.size
+    else:
+        n_table = int(num_keys)
+    if isinstance(resident, torch.Tensor):
+        resident = resident.cpu().numpy()
+    keys = np.empty(int(n), dtype=np.int64)
+    checks = misses = 0
+    tries = max(1, int(max_tries))
+    for s in range(0, int(n), chunk):
+        idx = np.arange(s, min(int(n), s + chunk), dtype=np.uint64)
+        k = _sampler_draw(kind, _sampler_hash(seed, idx, 0), prob, alias, n_table, first_key, key_stride)
+        if resident is not None:
+            checks += idx.size
+            pend = np.flatnonzero(~resident[k])
+            for t in range(1, tries):
+                if pend.size == 0:
+                    break
+                k[pend] = _sampler_draw(kind, _sampler_hash(seed, idx[pend], t), prob, alias, n_table, first_key,
+                                        key_stride)
+                checks += pend.size
+                pend = pend[~resident[k[pend]]]
+            misses += pend.size
+        keys[s:s + idx.size] = k
+    return keys if resident is None else (keys, checks, misses)
+
+
+def alias_draw_probabilities(prob, alias) -> np.ndarray:
+    """The probability (float64 ``[n]``) with which the device draws each index from the alias table ``(prob, alias)``
+    under the rule of :func:`sample_keys_reference`. Bucket ``i`` takes ``c_i = ceil((i+1) 2^32 / n) - ceil(i 2^32 / n)``
+    of the ``hi`` values; of those, the ``L_i`` values of ``lo`` with ``float32(lo) 2^-32 < prob[i]`` (a binary search
+    over ``lo``: the cast is monotone) draw ``i`` and the rest draw ``alias[i]``. ``P_j = sum c_i L_i / 2^64`` over
+    the buckets that draw ``j``, summed in integers, so the only rounding is the final one to float64. Compare it with
+    ``w / sum(w)``: it is the distribution of table and draw rule together, without sampling noise."""
+    prob = np.asarray(prob.cpu() if isinstance(prob, torch.Tensor) else prob, dtype=np.float32)
+    alias = np.asarray(alias.cpu() if isinstance(alias, torch.Tensor) else alias, dtype=np.int64)
+    n = prob.size
+    i = np.arange(n + 1, dtype=np.uint64)
+    c = np.diff(((i << np.uint64(32)) + np.uint64(n - 1)) // np.uint64(n)).astype(np.int64)
+    lo, hi = np.zeros(n, dtype=np.int64), np.full(n, 1 << 32, dtype=np.int64)   # L_i in [lo, hi]
+    while True:
+        active = lo < hi
+        if not active.any():
+            break
+        mid = (lo + hi) >> 1
+        at_or_above = mid.astype(np.float32) * np.float32(2.0 ** -32) >= prob
+        hi = np.where(active & at_or_above, mid, hi)
+        lo = np.where(active & ~at_or_above, mid + 1, lo)
+    A, B = np.zeros(n, dtype=np.int64), np.zeros(n, dtype=np.int64)   # P = (A 2^16 + B) / 2^64; A, B <= 2^48
+    for to, cnt in ((np.arange(n), lo), (alias, (1 << 32) - lo)):
+        np.add.at(A, to, c * (cnt >> 16))
+        np.add.at(B, to, c * (cnt & 0xFFFF))
+    return A * 2.0 ** -48 + B * 2.0 ** -64
