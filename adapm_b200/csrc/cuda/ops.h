@@ -86,6 +86,21 @@ void kge_rotate_step(CudaBackend& be, cudaStream_t stream, const Key* subj, cons
                      const Key* neg, int B, int n_neg, int d, float margin, float alpha, float eta, float gamma_e,
                      float* loss_out, unsigned long long* stats, bool deterministic = false);
 
+// KGE 1vsAll training for ComplEx (model 0) and RESCAL (model 1) on pulled rows (ops_kge_1vsall.cu): every query
+// (s, r, ?) and (?, r, o) of the B triples against all N entities with a softmax cross-entropy loss. R: the pulled rows
+// [N entity rows (2 d) | nrel relation rows (2 d or 2 d d)]; s, o: entity ids, rel: the triple's relation as an index
+// into the pulled relations; ent_off [N + 1] / ent_pos: per entity, the positions p (2 i: subject of triple i, 2 i + 1:
+// object) in ascending order; rel_off [nrel + 1] / rel_pos: per pulled relation, its triples in ascending order.
+// U: the additive updates [-eta g / sqrt(a + g^2) | g^2] of every pulled row, for one Push. Queries run in chunks of
+// `chunk` (a multiple of 128) rows; the workspace holds kge_1vsall_workspace_bytes(...). No floating-point atomics: on
+// one GPU the same inputs give bit-identical updates and loss. *loss += sum of the 2 B cross-entropies.
+constexpr int kKge1vsAllMaxDim = 1024;
+size_t kge_1vsall_workspace_bytes(int N, int B, int d, int chunk);
+void kge_1vsall_core(cudaStream_t stream, int model, const float* R, const Key* s, const Key* o, const int32_t* rel,
+                     const int64_t* ent_off, const int32_t* ent_pos, const int64_t* rel_off, const int32_t* rel_pos,
+                     int N, int nrel, int B, int d, int chunk, float eta, float gamma_e, float gamma_r, void* workspace,
+                     float* U, float* loss);
+
 // matrix factorisation: fused pull + error + L2 + AdaGrad + push (ops_mf.cu)
 void mf_step(CudaBackend& be, cudaStream_t stream, const Key* row_keys, const Key* col_keys, const float* xs,
              const int* row_nnz, const int* col_nnz, int n, int rank, float eps, float lambda, float* loss_out,

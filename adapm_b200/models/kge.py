@@ -39,6 +39,12 @@ Subject and object ranks and predictions use the complex metric of ``ops.gather_
 ``ops.gather_dist_topk`` with ``p="complex"`` (``ops.complex_dist`` on the CPU); the relation side is computed in PyTorch.
 ``gamma_relation`` is not used by RotatE (phases get no L2).
 
+``KGEConfig.train_type = "1vsAll"`` (ComplEx and RESCAL) trains LibKGE's 1vsAll type instead of negative sampling: each
+query ``(s, r, ?)`` and ``(?, r, o)`` of a batch is scored against every entity with a softmax cross-entropy loss, and every
+entity row gets one AdaGrad update per step (``ops.kge_1vsall_step`` on the tensor cores, deterministic on one GPU;
+``ops.kge_1vsall_reference_step`` on the CPU backend and for float64 stores). ``neg_ratio`` is not used. Since every step
+reads every entity, several ranks signal one intent for all entity keys over ``[0, CLOCK_MAX)`` at initialisation.
+
 ``KGEConfig.deterministic`` selects the deterministic one-GPU variant of the fused kernels (start-of-step reads,
 fixed-point sums, bit-identical runs); the CPU backend accepts it and already follows the start-of-step rule.
 """
@@ -76,6 +82,8 @@ class KGEConfig:
     p_norm: int = 1                  # TransE only: L1 or L2 distance
     margin: float = 1.0              # TransE: margin of the ranking loss; RotatE: gamma of the sigmoid loss
     adversarial_temperature: float = 1.0   # RotatE only: alpha of the self-adversarial negative weights (0: uniform)
+    train_type: str = "negative_sampling"  # or "1vsAll" (ComplEx, RESCAL): cross-entropy over every entity
+    max_bytes: int = 1 << 30         # 1vsAll: device memory for one chunk of scores and G (ops.kge_1vsall_step)
 
     @property
     def entity_len(self) -> int:
@@ -142,6 +150,13 @@ def load_triples(path: str) -> torch.Tensor:
 class KGE:
     def __init__(self, server, worker, cfg: KGEConfig):
         self.server, self.worker, self.cfg = server, worker, cfg
+        if cfg.train_type not in ("negative_sampling", "1vsAll"):
+            raise ValueError(f"train_type must be 'negative_sampling' or '1vsAll', got {cfg.train_type!r}")
+        if cfg.train_type == "1vsAll":
+            if cfg.algorithm not in ("ComplEx", "RESCAL"):
+                raise ValueError(f"1vsAll training is defined for ComplEx and RESCAL, not {cfg.algorithm}")
+            if cfg.dropout_entity > 0 or cfg.dropout_relation > 0:
+                raise ValueError("dropout is not defined for 1vsAll training")
         if cfg.algorithm == "RotatE":
             from ..ops import _check_rotate_shape
 
@@ -187,8 +202,7 @@ class KGE:
             elif kind == "uniform":
                 p1, p2 = -cfg.init_std, cfg.init_std
         if kind == "none":
-            if cfg.signal_initial_relations_intent and world > 1:
-                self.worker.intent(torch.arange(cfg.num_entities, cfg.num_entities + cfg.num_relations), 0, CLOCK_MAX)
+            self._long_term_intents()
             return
         gen = torch.Generator().manual_seed(cfg.model_seed + rank)
         self.worker.begin_setup()
@@ -210,14 +224,26 @@ class KGE:
                 self.worker.set(k, rows.view(-1))
         self.worker.waitall()
         self.worker.end_setup()
-        if cfg.signal_initial_relations_intent and world > 1:
+        self._long_term_intents()
+
+    def _long_term_intents(self) -> None:
+        """The intents over ``[0, CLOCK_MAX)`` on several ranks: the relations on request, and every entity under 1vsAll,
+        whose steps read all of them."""
+        cfg = self.cfg
+        if self.server.num_servers() == 1:
+            return
+        if cfg.signal_initial_relations_intent:
             self.worker.intent(torch.arange(cfg.num_entities, cfg.num_entities + cfg.num_relations), 0, CLOCK_MAX)
+        if cfg.train_type == "1vsAll":
+            self.worker.intent(torch.arange(cfg.num_entities), 0, CLOCK_MAX)
 
     # ------------------------------------------------------------------ intent
     def signal_intent(self, triples: torch.Tensor, clock: int) -> None:
         if not self.cfg.signal_intent or self.server.num_servers() == 1:
             return
-        keys = torch.cat([triples[:, 0], triples[:, 2], triples[:, 1] + self.cfg.num_entities])
+        rels = triples[:, 1] + self.cfg.num_entities
+        # under 1vsAll the entities are covered by the long-term intent of init_model
+        keys = rels if self.cfg.train_type == "1vsAll" else torch.cat([triples[:, 0], triples[:, 2], rels])
         self.worker.intent(keys, clock, clock + 1)
 
     # ------------------------------------------------------------------ training calls of one batch
@@ -257,6 +283,15 @@ class KGE:
         if cfg.algorithm in ("TransE", "RotatE") and (cfg.dropout_entity > 0 or cfg.dropout_relation > 0):
             raise ValueError(f"dropout is not defined for {cfg.algorithm}")
         tr = triples_host.to(self.server.device, non_blocking=True) if self.cuda else triples_host
+        if cfg.train_type == "1vsAll":
+            if self.cuda:
+                ops.kge_1vsall_step(self.worker, tr[:, 0].contiguous(), (tr[:, 1] + ne).contiguous(),
+                                    tr[:, 2].contiguous(), ne, cfg.algorithm, cfg.embed_dim, cfg.eta, cfg.gamma_entity,
+                                    cfg.gamma_relation, self.loss, cfg.max_bytes)
+            else:
+                loss = ops.kge_1vsall_reference_step(self.worker, triples_host, cfg)
+            self.step_no += 1
+            return self.loss if self.cuda else torch.tensor([loss], dtype=torch.float32)
         seed, neg = self._negatives(tr.shape[0])
         if cfg.algorithm in ("ComplEx", "RESCAL"):
             S, R, O, L = self._expand(tr, neg)

@@ -321,6 +321,177 @@ def kge_rescal_step(server, subj: torch.Tensor, rel: torch.Tensor, obj: torch.Te
                        float(dropout_relation), int(seed) & 0xFFFFFFFFFFFFFFFF, det)
 
 
+KGE_1VSALL_MAX_DIM = 1024
+_KGE_1VSALL_MODELS = {"ComplEx": 0, "RESCAL": 1}
+
+
+def _kge_1vsall_chunk(num_entities: int, queries: int, max_bytes: int) -> int:
+    """Query rows per chunk: a multiple of 128 (the GEMM's row tile) whose fp32 scores and bf16 G and G^T fit
+    ``max_bytes``; at most the batch's queries rounded up to 128."""
+    n, npad = int(num_entities), (int(num_entities) + 7) // 8 * 8
+    chunk = int(max_bytes) // (4 * n + 2 * npad + 2 * n) // 128 * 128
+    if chunk < 128:
+        raise ValueError(f"max_bytes={max_bytes} is too small for one tile of 128 queries against {n} entities "
+                         f"(needs {128 * (4 * n + 2 * npad + 2 * n)} bytes)")
+    return min(chunk, (int(queries) + 127) // 128 * 128)
+
+
+def _check_kge_1vsall_shape(algorithm: str, embed_dim: int) -> None:
+    if algorithm not in _KGE_1VSALL_MODELS:
+        raise ValueError(f"1vsAll training is defined for ComplEx and RESCAL, got {algorithm!r}")
+    if isinstance(embed_dim, bool) or int(embed_dim) != embed_dim or not 1 <= int(embed_dim) <= KGE_1VSALL_MAX_DIM:
+        raise ValueError(f"embed_dim must be an integer in [1, {KGE_1VSALL_MAX_DIM}], got {embed_dim}")
+    if algorithm == "ComplEx" and int(embed_dim) % 2:
+        raise ValueError(f"ComplEx needs an even embed_dim (real half + imaginary half), got {embed_dim}")
+
+
+def kge_1vsall_step(kv, subj: torch.Tensor, rel: torch.Tensor, obj: torch.Tensor, num_entities: int, algorithm: str,
+                    embed_dim: int, eta: float, gamma_entity: float, gamma_relation: float, loss: torch.Tensor,
+                    max_bytes: int = 1 << 30) -> None:
+    """1vsAll training step of ComplEx or RESCAL (csrc/cuda/ops_kge_1vsall.cu) on the store of the worker ``kv``.
+
+    Each triple ``(subj[i], rel[i], obj[i])`` (entity keys in ``[0, num_entities)``, relation keys after them; CUDA int64)
+    gives the queries ``(s, r, ?)`` and ``(?, r, o)`` with the query vectors of ``KGE._query``. Each is scored against
+    every entity, ``z = <q, e_x>``, with the loss ``logsumexp(z) - z_answer``; ``loss`` (CUDA float32[1]) is accumulated
+    (+=) with the sum over the ``2 B`` queries. The gradients, all from the rows at the start of the step, are
+    ``softmax - onehot`` through the scores to every entity (``G^T Q``) and to the queries (``G E``), carried back to the
+    given entity and the relation; L2 (``gamma_entity`` on s and o, ``gamma_relation`` on r) is added once per triple.
+    Every entity row and every distinct relation row then gets one AdaGrad update ``[-eta g / sqrt(a + g^2) | g^2]``.
+
+    One Pull of all entity rows and the batch's relation rows and one Push of their updates go through ``kv``, so the
+    step works in every protocol state (local, replica, peer, in flight). The three contractions use bf16 operands and
+    fp32 accumulation on the tensor cores; ``kge_1vsall_reference_step(..., emulate_bf16=True)`` is the same rule in
+    float64. No floating-point atomics: on one GPU two runs with the same arguments give bit-identical rows and loss.
+
+    ``embed_dim`` is any integer up to ``KGE_1VSALL_MAX_DIM`` (1024), even for ComplEx; the op pads it to a multiple of 8
+    for the GEMMs. Queries are processed in chunks of a multiple of 128 so that the ``[chunk, N]`` fp32 scores and bf16
+    G and G^T stay within ``max_bytes``. ``ValueError`` on another algorithm, a bad ``embed_dim``, ``max_bytes`` too
+    small for one chunk of 128 queries, tensors of the wrong device, dtype or length, row lengths that do not match the
+    model, or keys out of range."""
+    _check_kge_1vsall_shape(algorithm, embed_dim)
+    d, N = int(embed_dim), int(num_entities)
+    server = kv.server
+    if not 1 <= N < server.num_keys():
+        raise ValueError(f"num_entities must be in [1, {server.num_keys()}), got {num_entities}")
+    B = subj.numel()
+    chunk = _kge_1vsall_chunk(N, 2 * B, max_bytes)
+    for t, name in ((subj, "subj"), (rel, "rel"), (obj, "obj")):
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.int64 and t.is_contiguous()):
+            raise ValueError(f"{name} must be a contiguous CUDA int64 tensor")
+    if not (rel.numel() == B and obj.numel() == B and B > 0):
+        raise ValueError("subj, rel and obj must have the same, non-zero length")
+    if not (isinstance(loss, torch.Tensor) and loss.is_cuda and loss.dtype == torch.float32 and loss.numel() >= 1):
+        raise ValueError("loss must be a CUDA float32 tensor")
+    if server.backend != "cuda" or server.dtype != torch.float32:
+        raise ValueError("kge_1vsall_step needs a float32 CUDA store (kge_1vsall_reference_step is the other route)")
+    lo_e, hi_e, lo_r, hi_r = torch.stack([torch.minimum(subj.min(), obj.min()), torch.maximum(subj.max(), obj.max()),
+                                          rel.min(), rel.max()]).tolist()
+    if lo_e < 0 or hi_e >= N:
+        raise ValueError(f"entity keys must be in [0, {N}), got [{lo_e}, {hi_e}]")
+    if lo_r < N or hi_r >= server.num_keys():
+        raise ValueError(f"relation keys must be in [{N}, {server.num_keys()}), got [{lo_r}, {hi_r}]")
+    rl = 2 * d * (d if algorithm == "RESCAL" else 1)
+    uniq, inv = torch.unique(rel, return_inverse=True)
+    lens = server._lens_t[uniq.cpu()] if server._uniform_len is None else torch.full((1,), server._uniform_len)
+    if server.get_len(0) != 2 * d or N > 1 and server.get_len(N - 1) != 2 * d or bool((lens != rl).any()):
+        raise ValueError(f"{algorithm} at embed_dim {d} needs entity rows of {2 * d} and relation rows of {rl} values")
+    dev = subj.device
+    nrel = uniq.numel()
+    rel_pos = torch.argsort(inv, stable=True).to(torch.int32)
+    rel_off = torch.zeros(nrel + 1, dtype=torch.int64, device=dev)
+    rel_off[1:] = torch.cumsum(torch.bincount(inv, minlength=nrel), 0)
+    ents = torch.stack([subj, obj], 1).view(-1)          # position 2 i: subject of triple i, 2 i + 1: its object
+    ent_pos = torch.argsort(ents, stable=True).to(torch.int32)
+    ent_off = torch.zeros(N + 1, dtype=torch.int64, device=dev)
+    ent_off[1:] = torch.cumsum(torch.bincount(ents, minlength=N), 0)
+    keys = torch.cat([torch.arange(N, dtype=torch.int64, device=dev), uniq])
+    R = torch.empty(N * 2 * d + nrel * rl, dtype=torch.float32, device=dev)
+    kv.wait(kv.pull(keys, R, True))
+    U = torch.empty_like(R)
+    ws = torch.empty(_C.kge_1vsall_workspace_bytes(N, B, d, chunk), dtype=torch.uint8, device=dev)
+    inv32 = inv.to(torch.int32)
+    _C.kge_1vsall_core(_stream(subj), _KGE_1VSALL_MODELS[algorithm], R.data_ptr(), subj.data_ptr(), obj.data_ptr(),
+                       inv32.data_ptr(), ent_off.data_ptr(), ent_pos.data_ptr(), rel_off.data_ptr(), rel_pos.data_ptr(),
+                       N, nrel, B, d, chunk, float(eta), float(gamma_entity), float(gamma_relation), ws.data_ptr(),
+                       U.data_ptr(), loss.data_ptr())
+    kv.wait(kv.push(keys, U, True))
+
+
+def kge_1vsall_reference_step(kv, triples: torch.Tensor, cfg, emulate_bf16: bool = False) -> float:
+    """The rule of :func:`kge_1vsall_step` in float64 through Pull / Push on either backend: the CPU route of the model
+    (and of float64 stores) and the test oracle. ``triples``: [B, 3] (subject, relation id, object); ``cfg``: a
+    ``KGEConfig`` (``algorithm`` ComplEx or RESCAL, ``num_entities``, ``embed_dim``, ``eta``, ``gamma_entity``,
+    ``gamma_relation``). ``emulate_bf16`` rounds the operands of the three contractions (queries, entities, G) to bf16
+    as the tensor-core path does. Returns the summed loss of the ``2 B`` queries."""
+    from ..models.kge import complex_query
+
+    _check_kge_1vsall_shape(cfg.algorithm, cfg.embed_dim)
+    d, N = cfg.embed_dim, cfg.num_entities
+    dt = kv.server.dtype
+    tr = torch.as_tensor(triples, dtype=torch.int64).view(-1, 3).cpu()
+    s, r, o = tr[:, 0], tr[:, 1], tr[:, 2]
+    if tr.numel() == 0 or int(torch.minimum(s, o).min()) < 0 or int(torch.maximum(s, o).max()) >= N:
+        raise ValueError(f"triples must be non-empty with entity ids in [0, {N})")
+    if int(r.min()) < 0 or int(r.max()) >= cfg.num_relations:
+        raise ValueError(f"relation ids must be in [0, {cfg.num_relations})")
+    uniq, inv = torch.unique(r, return_inverse=True)
+    el, rl = 2 * d, cfg.relation_len
+
+    def pull(keys, ln):
+        v = torch.empty(keys.numel() * ln, dtype=dt)
+        kv.wait(kv.pull(keys.contiguous(), v))
+        return v.view(-1, ln).double()
+
+    ent, rr = pull(torch.arange(N), el), pull(uniq + N, rl)
+    E, A, Rr, Ar = ent[:, :d], ent[:, d:], rr[:, :rl // 2], rr[:, rl // 2:]
+    rel = Rr[inv]
+    Es, Eo = E[s], E[o]
+
+    def rnd(x):
+        return x.to(torch.bfloat16).double() if emulate_bf16 else x
+
+    if cfg.algorithm == "ComplEx":
+        Q = torch.cat([complex_query(Es, rel, conj=False), complex_query(Eo, rel, conj=True)])
+    else:
+        Rm = rel.view(-1, d, d)
+        Q = torch.cat([torch.einsum("bi,bij->bj", Es, Rm), torch.einsum("bij,bj->bi", Rm, Eo)])
+    ans = torch.cat([o, s])
+    rows = torch.arange(ans.numel())
+    Qm, Em = rnd(Q), rnd(E)
+    Z = Qm @ Em.t()
+    lse = torch.logsumexp(Z, 1)
+    loss = float((lse - Z[rows, ans]).sum())
+    G = torch.exp(Z - lse.unsqueeze(1))
+    G[rows, ans] -= 1
+    Gm = rnd(G)
+    dQ, C = Gm @ Em, Gm.t() @ Qm
+    B = s.numel()
+    dqo, dqs = dQ[:B], dQ[B:]
+    if cfg.algorithm == "ComplEx":
+        h = d // 2
+        rre, rim, a, b, a2, b2 = rel[:, :h], rel[:, h:], dqo[:, :h], dqo[:, h:], dqs[:, :h], dqs[:, h:]
+        sre, sim, ore, oim = Es[:, :h], Es[:, h:], Eo[:, :h], Eo[:, h:]
+        ds = torch.cat([rre * a + rim * b, rre * b - rim * a], 1)
+        do = torch.cat([rre * a2 - rim * b2, rim * a2 + rre * b2], 1)
+        dr = torch.cat([sre * a + sim * b + ore * a2 + oim * b2, sre * b - sim * a + oim * a2 - ore * b2], 1)
+    else:
+        ds = torch.einsum("bij,bj->bi", Rm, dqo)
+        do = torch.einsum("bi,bij->bj", dqs, Rm)
+        dr = (torch.einsum("bi,bj->bij", Es, dqo) + torch.einsum("bi,bj->bij", dqs, Eo)).reshape(B, -1)
+    gE = C.clone()
+    gE.index_add_(0, s, ds + cfg.gamma_entity * Es)
+    gE.index_add_(0, o, do + cfg.gamma_entity * Eo)
+    gR = torch.zeros_like(Rr).index_add_(0, inv, dr + cfg.gamma_relation * rel)
+
+    def upd(g, a):
+        u = torch.where(g == 0, torch.zeros_like(g), -cfg.eta * g / torch.sqrt(a + g * g))
+        return torch.cat([u, g * g], 1).to(dt).contiguous().view(-1)
+
+    kv.wait(kv.push(torch.arange(N), upd(gE, A)))
+    kv.wait(kv.push((uniq + N).contiguous(), upd(gR, Ar)))
+    return loss
+
+
 TRANSE_MAX_DIM = 512
 TRANSE_MAX_NEG = 64
 _NORM_EPS = 1e-12
