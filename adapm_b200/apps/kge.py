@@ -25,9 +25,13 @@ def main(argv=None) -> int:
     ap.add_argument("--dataset", default=None, help="directory with train.del / valid.del / test.del (s r o per line)")
     ap.add_argument("--synthetic", type=int, default=0, help="number of synthetic training triples")
     ap.add_argument("--algorithm", default="ComplEx", choices=["ComplEx", "RESCAL", "TransE", "RotatE"])
-    ap.add_argument("--train_type", default="negative_sampling", choices=["negative_sampling", "1vsAll"],
+    ap.add_argument("--train_type", default="negative_sampling", choices=["negative_sampling", "1vsAll", "sampled_softmax"],
                     help="negative_sampling: BCE over neg_ratio corrupted subjects and objects per triple; 1vsAll "
-                         "(ComplEx, RESCAL): softmax cross-entropy of every query against all entities (neg_ratio unused)")
+                         "(ComplEx, RESCAL): softmax cross-entropy of every query against all entities (neg_ratio unused); "
+                         "sampled_softmax (ComplEx, RESCAL): softmax cross-entropy against the chunk's subjects and objects "
+                         "and --shared_negatives entities shared by the batch (neg_ratio unused)")
+    ap.add_argument("--shared_negatives", type=int, default=1024,
+                    help="sampled_softmax: entities sampled per step, shared by the whole batch")
     ap.add_argument("--transe_norm", type=int, default=1, choices=[1, 2], help="TransE: L1 or L2 distance")
     ap.add_argument("--margin", type=float, default=1.0,
                     help="TransE: margin of the ranking loss; RotatE: gamma of the sigmoid loss")
@@ -81,7 +85,8 @@ def main(argv=None) -> int:
                     read_ahead=args.signal_intent_ahead, sampling_scheme=getattr(args, "sampling.scheme") or "local",
                     signal_initial_relations_intent=bool(args.signal_initial_relations_intent), model_seed=args.model_seed,
                     deterministic=bool(args.deterministic), p_norm=args.transe_norm, margin=args.margin,
-                    adversarial_temperature=args.adversarial_temperature, train_type=args.train_type)
+                    adversarial_temperature=args.adversarial_temperature, train_type=args.train_type,
+                    shared_negatives=args.shared_negatives)
     if args.write_embeddings and not args.model_path:
         os.makedirs(args.write_embeddings, exist_ok=True)
         args.model_path = os.path.join(args.write_embeddings, "")
@@ -152,7 +157,7 @@ def main(argv=None) -> int:
         total = ps_allreduce(kv, cfg.loss_key, torch.tensor([bce, 0.0]))     # loss all-reduce through the PS
         if rank == 0:
             kind = {"TransE": "margin", "RotatE": "self-adversarial"}.get(cfg.algorithm, "bce")
-            kind = "cross-entropy" if cfg.train_type == "1vsAll" else kind
+            kind = "cross-entropy" if cfg.train_type in ("1vsAll", "sampled_softmax") else kind
             print(f"[kge] epoch {epoch}: {kind} loss {float(total[0]):.4f} ({time.time() - t0:.1f}s)", flush=True)
         if args.eval_freq > 0 and epoch % args.eval_freq == 0:
             ev = model.evaluate_distributed(va, known)

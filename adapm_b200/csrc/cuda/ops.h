@@ -101,6 +101,23 @@ void kge_1vsall_core(cudaStream_t stream, int model, const float* R, const Key* 
                      int N, int nrel, int B, int d, int chunk, float eta, float gamma_e, float gamma_r, void* workspace,
                      float* U, float* loss);
 
+// KGE sampled-softmax training for ComplEx and RESCAL on pulled rows (ops_kge_1vsall.cu): the B triples in chunks of
+// kKgeSharedChunk; chunk k scores its object queries (s, r, ?) and subject queries (?, r, o) against one list
+// [its subjects | its objects | the S shared negatives] with a softmax cross-entropy. R: the pulled rows [Ne entity rows
+// (2 d) | nrel relation rows]; s, o, rel: [Bp] indices into them, Bp = B padded to whole chunks (padding triples are
+// masked out of the loss and left out of every CSR); cand [nch][Lr]: the lists as entity indices, -1 for padding slots,
+// Lr = 2 * 128 + S padded to a multiple of 8; qorder [nch][2 * 128]: the queries of chunk k, object queries first, as
+// indices q < 2 Bp (object query of triple i: i, subject query: Bp + i). ent_off [Ne + 1] / ent_pos: per entity, its
+// occurrences in ascending order, p < nch * Lr the list column k * Lr + j, else the given entity of position
+// p - nch * Lr (2 i: subject of triple i, 2 i + 1: object); rel_off / rel_pos as in kge_1vsall_core. U: one AdaGrad
+// update per pulled row. No floating-point atomics. *loss += the 2 B cross-entropies.
+constexpr int kKgeSharedChunk = 128;
+size_t kge_shared_workspace_bytes(int B, int S, int d);
+void kge_shared_core(cudaStream_t stream, int model, const float* R, const Key* s, const Key* o, const int32_t* rel,
+                     const Key* cand, const Key* qorder, const int64_t* ent_off, const int32_t* ent_pos,
+                     const int64_t* rel_off, const int32_t* rel_pos, int Ne, int nrel, int B, int S, int d, float eta,
+                     float gamma_e, float gamma_r, void* workspace, float* U, float* loss);
+
 // matrix factorisation: fused pull + error + L2 + AdaGrad + push (ops_mf.cu)
 void mf_step(CudaBackend& be, cudaStream_t stream, const Key* row_keys, const Key* col_keys, const float* xs,
              const int* row_nnz, const int* col_nnz, int n, int rank, float eps, float lambda, float* loss_out,

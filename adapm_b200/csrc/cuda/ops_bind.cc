@@ -90,6 +90,16 @@ void bind(py::module_& m) {
                     ptr<const int64_t>(rel_off), ptr<const int32_t>(rel_pos), N, nrel, B, d, chunk, eta, gamma_e, gamma_r,
                     ptr<void>(ws), ptr<float>(U), ptr<float>(loss));
   });
+  m.def("kge_shared_workspace_bytes", [](int B, int S, int d) { return kge_shared_workspace_bytes(B, S, d); });
+  m.def("kge_shared_core", [](uintptr_t stream, int model, uintptr_t R, uintptr_t s, uintptr_t o, uintptr_t rel,
+                              uintptr_t cand, uintptr_t qorder, uintptr_t ent_off, uintptr_t ent_pos, uintptr_t rel_off,
+                              uintptr_t rel_pos, int Ne, int nrel, int B, int S, int d, float eta, float gamma_e,
+                              float gamma_r, uintptr_t ws, uintptr_t U, uintptr_t loss) {
+    kge_shared_core((cudaStream_t)stream, model, ptr<const float>(R), ptr<const Key>(s), ptr<const Key>(o),
+                    ptr<const int32_t>(rel), ptr<const Key>(cand), ptr<const Key>(qorder), ptr<const int64_t>(ent_off),
+                    ptr<const int32_t>(ent_pos), ptr<const int64_t>(rel_off), ptr<const int32_t>(rel_pos), Ne, nrel, B,
+                    S, d, eta, gamma_e, gamma_r, ptr<void>(ws), ptr<float>(U), ptr<float>(loss));
+  });
   m.def("gemm_nt_bf16", [](uintptr_t stream, uintptr_t A, uintptr_t B, int M, int N, int K, uintptr_t C, int ldc) {
     gemm_nt_bf16((cudaStream_t)stream, ptr<const void>(A), ptr<const void>(B), M, N, K, ptr<float>(C), ldc);
   });

@@ -31,6 +31,23 @@
 //   entity_kernel     per entity: C + its occurrences in position order -> AdaGrad update
 //   relation_kernel   per pulled relation: its triples in order -> AdaGrad update
 //   loss_kernel       *loss += the 2 B cross-entropies, summed in a fixed order
+//
+// Sampled softmax with shared negatives (kge_shared_core) runs the same rule against short lists instead of all
+// entities. The batch is padded to Bp = nch * 128 triples (padding triples are masked); chunk k's list is
+// [its 128 subjects | its 128 objects | the S negatives] (Lr columns, padded to a multiple of 8), and each of its 256
+// queries is scored against its own list only. The pulled rows are the step's distinct entities and relations. Per
+// chunk, as one batched launch each (grid dimension z over chunks, every operand at a fixed row stride, all of K in
+// one CTA, so no split-K):
+//     Z_k  [256, Lr] = Q_k E_k^T,   G_k = softmax - onehot over the live columns,
+//     dQ_k [256, d]  = G_k E_k,     C_k [Lr, d] = G_k^T Q_k
+// A column is live unless it is a padding slot, or holds the query's answer without being the answer's own slot.
+//   gemm_batched_kernel       P[z] = A_z B_z^T (the tile body of gemm_partial_kernel)
+//   gather_bf16_kernel        rows by index -> bf16 operand and / or its chunk-major transpose (lists, queries)
+//   kge_shared_lse_kernel     per query: logsumexp over the live columns (one warp, fixed order) and its cross-entropy
+//   kge_shared_grad_kernel    Z -> G (query order) and G^T (chunk-major, both sides of a chunk along K)
+//   kge_shared_entity_kernel  per distinct entity: its list columns of C in (chunk, column) order, then its
+//                             given-entity gradients in position order -> AdaGrad update
+// with query_kernel, given_kernel, relation_kernel and loss_kernel as above (batch stride Bp).
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
@@ -47,11 +64,11 @@ namespace {
 
 enum Model : int { COMPLEX = 0, RESCAL = 1 };
 
-// P[blockIdx.z][M][N] (fp32) = A[M, K] x B[N, K]^T (bf16, K-major) over the k-blocks of split blockIdx.z, one 128 x 128
-// tile per CTA. The host picks splits so that none is empty.
-__global__ void __launch_bounds__(tc::kGemmThreads, 1)
-gemm_partial_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N,
-                    int K, float* __restrict__ P) {
+// One 128 x 128 tile per CTA of the products gemm_partial_kernel (!BATCHED) and gemm_batched_kernel (BATCHED) compute:
+// the TMA producer warp loads the tile's k-blocks into the ring, the two wgmma consumer warpgroups store the fp32 tile.
+template <bool BATCHED>
+__device__ __forceinline__ void tile_product(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, int M, int N, int K,
+                                             int a_rows, int b_rows, int nb, float* __restrict__ P) {
   using namespace tc;
   constexpr int BK = 64;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -59,9 +76,11 @@ gemm_partial_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile_n = blockIdx.x, tile_m = blockIdx.y;
   const int total_kb = (K + BK - 1) / BK;
-  const int kb_per = (total_kb + (int)gridDim.z - 1) / (int)gridDim.z;
-  const int kb0 = (int)blockIdx.z * kb_per;
-  const int num_kb = min(kb_per, total_kb - kb0);
+  const int kb_per = BATCHED ? total_kb : (total_kb + (int)gridDim.z - 1) / (int)gridDim.z;
+  const int kb0 = BATCHED ? 0 : (int)blockIdx.z * kb_per;
+  const int num_kb = BATCHED ? total_kb : min(kb_per, total_kb - kb0);
+  const int a_row = BATCHED ? (int)blockIdx.z * a_rows + tile_m * BM : tile_m * BM;
+  const int b_row = BATCHED ? ((int)blockIdx.z % nb) * b_rows + tile_n * BN : tile_n * BN;
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(&sm.full_bar[s], 1); mbar_init(&sm.empty_bar[s], kConsumerWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -74,8 +93,8 @@ gemm_partial_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         const int s = kb % STAGES;
         mbar_wait(&sm.empty_bar[s], ((uint32_t)(kb / STAGES) & 1u) ^ 1u);
         mbar_expect_tx(&sm.full_bar[s], A_BYTES + B_BYTES);
-        tma_load_2d(sm.a[s], &tmap_a, &sm.full_bar[s], (kb0 + kb) * BK, tile_m * BM);
-        tma_load_2d(sm.b[s], &tmap_b, &sm.full_bar[s], (kb0 + kb) * BK, tile_n * BN);
+        tma_load_2d(sm.a[s], &tmap_a, &sm.full_bar[s], (kb0 + kb) * BK, a_row);
+        tma_load_2d(sm.b[s], &tmap_b, &sm.full_bar[s], (kb0 + kb) * BK, b_row);
       }
     }
   } else {
@@ -85,6 +104,23 @@ gemm_partial_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     store_fragment(d, 1.f, P + (size_t)blockIdx.z * M * N, N, tile_m * BM + wg * 64 + (warp & 3) * 16, tile_n * BN, M, N,
                    lane, false);
   }
+}
+
+// P[blockIdx.z][M][N] (fp32) = A[M, K] x B[N, K]^T (bf16, K-major) over the k-blocks of split blockIdx.z, one 128 x 128
+// tile per CTA. The host picks splits so that none is empty.
+__global__ void __launch_bounds__(tc::kGemmThreads, 1)
+gemm_partial_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N,
+                    int K, float* __restrict__ P) {
+  tile_product<false>(tmap_a, tmap_b, M, N, K, 0, 0, 1, P);
+}
+
+// Batched products over all of K: P[z][M][N] (fp32) = A_z [M, K] x B_z [N, K]^T for z = blockIdx.z, where A_z starts at
+// row z a_rows of A and B_z at row (z % nb) b_rows of B (bf16, K-major). A tile that runs past a batch's M or N rows
+// reads the next batch's rows (or TMA's zero fill) into output rows and columns that are not stored.
+__global__ void __launch_bounds__(tc::kGemmThreads, 1)
+gemm_batched_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N,
+                    int K, int a_rows, int b_rows, int nb, float* __restrict__ P) {
+  tile_product<true>(tmap_a, tmap_b, M, N, K, a_rows, b_rows, nb, P);
 }
 
 // Splits of K for gemm_partial: about two CTAs per SM of a 132-SM H100, at least 4 k-blocks per split, at most 64
@@ -111,6 +147,26 @@ void gemm_partial(cudaStream_t stream, const void* A, const void* B, int M, int 
   }
   const dim3 grid((N + tc::BN - 1) / tc::BN, (M + tc::BM - 1) / tc::BM, partial_splits(M, N, K));
   gemm_partial_kernel<<<grid, tc::kGemmThreads, smem, stream>>>(ma, mb, M, N, K, P);
+  ADAPM_COUNT_LAUNCH();
+  ADAPM_CUDA_CHECK(cudaGetLastError());
+}
+
+// P[z] (z < batches) = A_z B_z^T of gemm_batched_kernel; A holds a_total rows and B b_total rows of K values (K a
+// multiple of 8: 16-byte TMA row pitch).
+void gemm_batched(cudaStream_t stream, const void* A, long a_total, const void* B, long b_total, int M, int N, int K,
+                  int a_rows, int b_rows, int nb, int batches, float* P) {
+  ADAPM_CHECK(K % 8 == 0 && (((uintptr_t)A) & 15u) == 0 && (((uintptr_t)B) & 15u) == 0,
+              "kge_shared: GEMM operands must be 16-byte aligned with a K extent that is a multiple of 8");
+  const CUtensorMap ma = tc::make_map(A, a_total, K, tc::BM, tc::KIND_BF16);
+  const CUtensorMap mb = tc::make_map(B, b_total, K, tc::BN, tc::KIND_BF16);
+  const size_t smem = sizeof(tc::SmemLayout) + 1024;
+  static bool attr_set = false;
+  if (!attr_set) {
+    ADAPM_CUDA_CHECK(cudaFuncSetAttribute(gemm_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_set = true;
+  }
+  const dim3 grid((N + tc::BN - 1) / tc::BN, (M + tc::BM - 1) / tc::BM, batches);
+  gemm_batched_kernel<<<grid, tc::kGemmThreads, smem, stream>>>(ma, mb, M, N, K, a_rows, b_rows, nb, P);
   ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cudaGetLastError());
 }
@@ -351,6 +407,136 @@ __global__ void __launch_bounds__(32) loss_kernel(const float* __restrict__ qlos
   if (threadIdx.x == 0) *loss += t;
 }
 
+// ------------------------------------------------------------------ shared negatives (kge_shared_core)
+// Rows idx[r] (r < rows; row r itself when idx is null; zeros when idx[r] < 0) of X [.][ldx] fp32, first d values ->
+// Xb [rows][dpad] bf16 and XT in chunks of W rows: row r, column j at XT[(r / W) dpad W + j W + r % W]. A null output
+// is skipped; columns past d are zeros. 32 x 8 threads per 32 x 32 tile.
+__global__ void __launch_bounds__(256)
+gather_bf16_kernel(const float* __restrict__ X, int ldx, const Key* __restrict__ idx, int rows, int d, int dpad, int W,
+                   __nv_bfloat16* __restrict__ Xb, __nv_bfloat16* __restrict__ XT) {
+  __shared__ __nv_bfloat16 tile[32][33];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int j0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int rl = ty + 8 * k, r = r0 + rl, j = j0 + tx;
+    const Key src = r < rows ? (idx ? idx[r] : r) : -1;
+    const __nv_bfloat16 b = __float2bfloat16(src >= 0 && j < d ? X[(size_t)src * ldx + j] : 0.f);
+    if (Xb && r < rows && j < dpad) Xb[(size_t)r * dpad + j] = b;
+    tile[rl][tx] = b;
+  }
+  __syncthreads();
+  const int r = r0 + tx;
+  if (!XT || r >= rows) return;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int j = j0 + ty + 8 * k;
+    if (j < dpad) XT[(size_t)(r / W) * dpad * W + (size_t)j * W + r % W] = tile[tx][ty + 8 * k];
+  }
+}
+
+// Query q < 2 Bp of the padded batch (object queries, then subject queries; triple i sits in chunk i / 128 at slot
+// i % 128): its answer, and its positive column in the chunk's list [subjects | objects | negatives].
+struct SharedQuery {
+  int i, pos;
+  Key ans;
+  __device__ __forceinline__ SharedQuery(long q, int Bp, const Key* s, const Key* o) {
+    const bool obj = q < Bp;
+    i = obj ? (int)q : (int)(q - Bp);
+    ans = obj ? o[i] : s[i];
+    pos = (obj ? kKgeSharedChunk : 0) + i % kKgeSharedChunk;
+  }
+  // column j (entity c, -1 for a padding slot) takes part in the softmax: not padding, and not another copy of the answer
+  __device__ __forceinline__ bool live(Key c, int j) const { return c >= 0 && (j == pos || c != ans); }
+};
+
+// One warp per query q < 2 Bp: over its chunk's live columns, lse[q] = logsumexp of the scores Z[q] and qloss[q] = lse -
+// the positive column's score; queries of padding triples (i >= B) get zeros.
+__global__ void __launch_bounds__(256)
+kge_shared_lse_kernel(const float* __restrict__ Z, const Key* __restrict__ cand, const Key* __restrict__ s,
+                  const Key* __restrict__ o, int B, int Bp, int Lr, float* __restrict__ lse, float* __restrict__ qloss) {
+  const int lane = threadIdx.x & 31;
+  const long q = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (q >= 2L * Bp) return;
+  const SharedQuery sq(q, Bp, s, o);
+  if (sq.i >= B) {
+    if (lane == 0) lse[q] = qloss[q] = 0.f;
+    return;
+  }
+  const Key* c = cand + (size_t)(sq.i / kKgeSharedChunk) * Lr;
+  const float* z = Z + (size_t)q * Lr;
+  float m = -INFINITY;
+  for (int j = lane; j < Lr; j += 32)
+    if (sq.live(c[j], j)) m = fmaxf(m, z[j]);
+  m = warp_max(m);
+  float t = 0.f;
+  for (int j = lane; j < Lr; j += 32)
+    if (sq.live(c[j], j)) t += expf(z[j] - m);
+  t = warp_sum(t);
+  const float l = m + logf(t);
+  if (lane == 0) {
+    lse[q] = l;
+    qloss[q] = l - z[sq.pos];
+  }
+}
+
+// Z -> G = softmax - onehot(positive) over the live columns: Gb [2 Bp][Lr] in query order, and GT [nch][Lr][2 * 128]
+// whose chunk k holds, per list column, G of the chunk's object queries, then of its subject queries. Masked and padding
+// columns and the queries of padding triples are zeros. 32 x 32 tiles (32 queries of one chunk and one side).
+__global__ void __launch_bounds__(256)
+kge_shared_grad_kernel(const float* __restrict__ Z, const float* __restrict__ lse, const Key* __restrict__ cand,
+                   const Key* __restrict__ s, const Key* __restrict__ o, int B, int Bp, int Lr,
+                   __nv_bfloat16* __restrict__ Gb, __nv_bfloat16* __restrict__ GT) {
+  __shared__ __nv_bfloat16 tile[32][33];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int n0 = blockIdx.x * 32, b0 = blockIdx.y * 32;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int bl = ty + 8 * k, n = n0 + tx;
+    const long q = (long)b0 + bl;
+    const SharedQuery sq(q, Bp, s, o);
+    float g = 0.f;
+    if (sq.i < B && n < Lr && sq.live(cand[(size_t)(sq.i / kKgeSharedChunk) * Lr + n], n))
+      g = expf(Z[(size_t)q * Lr + n] - lse[q]) - (n == sq.pos ? 1.f : 0.f);
+    const __nv_bfloat16 gb = __float2bfloat16(g);
+    if (n < Lr) Gb[(size_t)q * Lr + n] = gb;
+    tile[bl][tx] = gb;
+  }
+  __syncthreads();
+  const bool obj = b0 < Bp;
+  const int i0 = obj ? b0 : b0 - Bp;
+  const size_t chunk = (size_t)(i0 / kKgeSharedChunk);
+  const int col = (obj ? 0 : kKgeSharedChunk) + i0 % kKgeSharedChunk + tx;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int n = n0 + ty + 8 * k;
+    if (n < Lr) GT[(chunk * Lr + n) * (2 * kKgeSharedChunk) + col] = tile[tx][ty + 8 * k];
+  }
+}
+
+// One warp per distinct entity u: g = its candidate columns' rows of C in (chunk, column) order, then its given-entity
+// gradients in position order (occurrence p < nC: row p of C [nch Lr][dpad], else row p - nC of GS [2 Bp][d]);
+// U row u = AdaGrad update.
+__global__ void __launch_bounds__(256)
+kge_shared_entity_kernel(const float* __restrict__ R, const float* __restrict__ C, const float* __restrict__ GS,
+                     const int64_t* __restrict__ ent_off, const int32_t* __restrict__ ent_pos, int Ne, int nC, int d,
+                     int dpad, float eta, float* __restrict__ U) {
+  const int lane = threadIdx.x & 31;
+  const long u = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (u >= Ne) return;
+  const int64_t p0 = ent_off[u], p1 = ent_off[u + 1];
+  const float* row = R + (size_t)u * 2 * d;
+  float* out = U + (size_t)u * 2 * d;
+  for (int k = lane; k < d; k += 32) {
+    float g = 0.f;
+    for (int64_t p = p0; p < p1; ++p) {
+      const int at = ent_pos[p];
+      g += at < nC ? C[(size_t)at * dpad + k] : GS[(size_t)(at - nC) * d + k];
+    }
+    adagrad(g, row[d + k], eta, out + k, out + d + k);
+  }
+}
+
 inline size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
 inline int pad8(int x) { return (x + 7) / 8 * 8; }
 
@@ -385,6 +571,37 @@ struct Layout {
         0};
     total = 0;
     for (int i = 0; i < 15; ++i) { off[i] = total; total += align_up(bytes[i]); }
+  }
+};
+
+// The workspace of kge_shared_core, carved in this order. Bp: B padded to whole chunks; Lr: the list length 2 * 128 + S
+// padded to a multiple of 8 (the K extent of G E).
+struct SharedLayout {
+  int dpad, Bp, nch, Lr;
+  size_t off[13];
+  size_t total;
+  SharedLayout(int B, int S, int d) {
+    dpad = pad8(d);
+    nch = (B + kKgeSharedChunk - 1) / kKgeSharedChunk;
+    Bp = nch * kKgeSharedChunk;
+    Lr = pad8(2 * kKgeSharedChunk + S);
+    const size_t q = 2 * (size_t)Bp, lists = (size_t)nch * Lr;
+    const size_t bytes[13] = {
+        lists * dpad * 2,                      //  0 Eb    [nch Lr][dpad] bf16: chunk k's list rows
+        lists * dpad * 2,                      //  1 ET    [nch][dpad][Lr] bf16
+        q * d * 4,                             //  2 Qf    [2 Bp][d] fp32
+        q * dpad * 2,                          //  3 Qb    [2 Bp][dpad] bf16
+        q * dpad * 2,                          //  4 QT    [nch][dpad][2 * 128] bf16
+        q * Lr * 4,                            //  5 Z     [2 Bp][Lr] fp32
+        q * 4,                                 //  6 lse   [2 Bp]
+        q * 4,                                 //  7 qloss [2 Bp]
+        q * Lr * 2,                            //  8 Gb    [2 Bp][Lr] bf16
+        lists * 2 * kKgeSharedChunk * 2,       //  9 GT    [nch][Lr][2 * 128] bf16
+        q * dpad * 4,                          // 10 dq    [2 Bp][dpad] fp32
+        lists * dpad * 4,                      // 11 C     [nch Lr][dpad] fp32
+        q * d * 4};                            // 12 GS    [2 Bp][d] fp32
+    total = 0;
+    for (int i = 0; i < 13; ++i) { off[i] = total; total += align_up(bytes[i]); }
   }
 };
 
@@ -447,6 +664,61 @@ void kge_1vsall_core(cudaStream_t stream, int model, const float* R, const Key* 
     relation_kernel<COMPLEX><<<nrel, 256, 0, stream>>>(R, s, o, rel_off, rel_pos, dq, N, B, d, dpad, eta, gamma_r, U);
   else relation_kernel<RESCAL><<<nrel, 256, 0, stream>>>(R, s, o, rel_off, rel_pos, dq, N, B, d, dpad, eta, gamma_r, U);
   loss_kernel<<<1, 32, 0, stream>>>(qloss, 2 * B, loss);
+  ADAPM_COUNT_LAUNCH(); ADAPM_COUNT_LAUNCH(); ADAPM_COUNT_LAUNCH(); ADAPM_COUNT_LAUNCH();
+  ADAPM_CUDA_CHECK(cudaGetLastError());
+}
+
+size_t kge_shared_workspace_bytes(int B, int S, int d) { return SharedLayout(B, S, d).total; }
+
+void kge_shared_core(cudaStream_t stream, int model, const float* R, const Key* s, const Key* o, const int32_t* rel,
+                     const Key* cand, const Key* qorder, const int64_t* ent_off, const int32_t* ent_pos,
+                     const int64_t* rel_off, const int32_t* rel_pos, int Ne, int nrel, int B, int S, int d, float eta,
+                     float gamma_e, float gamma_r, void* workspace, float* U, float* loss) {
+  ADAPM_CHECK(model == COMPLEX || model == RESCAL, "kge_shared: model must be ComplEx (0) or RESCAL (1)");
+  ADAPM_CHECK(Ne > 0 && B > 0 && nrel > 0 && S >= 0, "kge_shared: empty batch or entity set");
+  ADAPM_CHECK(d > 0 && d <= kKge1vsAllMaxDim && (model == RESCAL || d % 2 == 0), "kge_shared: embedding dimension out of range");
+  const SharedLayout L(B, S, d);
+  const int dpad = L.dpad, Bp = L.Bp, nch = L.nch, Lr = L.Lr;
+  char* w = static_cast<char*>(workspace);
+  auto* Eb = reinterpret_cast<__nv_bfloat16*>(w + L.off[0]);
+  auto* ET = reinterpret_cast<__nv_bfloat16*>(w + L.off[1]);
+  auto* Qf = reinterpret_cast<float*>(w + L.off[2]);
+  auto* Qb = reinterpret_cast<__nv_bfloat16*>(w + L.off[3]);
+  auto* QT = reinterpret_cast<__nv_bfloat16*>(w + L.off[4]);
+  auto* Z = reinterpret_cast<float*>(w + L.off[5]);
+  auto* lse = reinterpret_cast<float*>(w + L.off[6]);
+  auto* qloss = reinterpret_cast<float*>(w + L.off[7]);
+  auto* Gb = reinterpret_cast<__nv_bfloat16*>(w + L.off[8]);
+  auto* GT = reinterpret_cast<__nv_bfloat16*>(w + L.off[9]);
+  auto* dq = reinterpret_cast<float*>(w + L.off[10]);
+  auto* C = reinterpret_cast<float*>(w + L.off[11]);
+  auto* GS = reinterpret_cast<float*>(w + L.off[12]);
+  const int K2 = 2 * kKgeSharedChunk;          // queries per chunk: the K extent of G^T Q
+  const unsigned warps_q = (unsigned)((2L * Bp * 32 + 255) / 256);
+  if (model == COMPLEX) query_kernel<COMPLEX><<<warps_q, 256, 0, stream>>>(R, s, o, rel, Ne, Bp, d, Qf);
+  else query_kernel<RESCAL><<<warps_q, 256, 0, stream>>>(R, s, o, rel, Ne, Bp, d, Qf);
+  const unsigned jt = (unsigned)((dpad + 31) / 32);
+  gather_bf16_kernel<<<dim3(jt, (nch * Lr + 31) / 32), 256, 0, stream>>>(R, 2 * d, cand, nch * Lr, d, dpad, Lr, Eb, ET);
+  gather_bf16_kernel<<<dim3(jt, 2 * Bp / 32), 256, 0, stream>>>(Qf, d, nullptr, 2 * Bp, d, dpad, 1, Qb, nullptr);
+  gather_bf16_kernel<<<dim3(jt, 2 * Bp / 32), 256, 0, stream>>>(Qf, d, qorder, 2 * Bp, d, dpad, K2, nullptr, QT);
+  ADAPM_COUNT_LAUNCH(); ADAPM_COUNT_LAUNCH(); ADAPM_COUNT_LAUNCH(); ADAPM_COUNT_LAUNCH();
+  // Z = Q_k E_k^T: one batch per 128 queries of one side of chunk k (z % nch = k), K = dpad
+  gemm_batched(stream, Qb, 2L * Bp, Eb, (long)nch * Lr, kKgeSharedChunk, Lr, dpad, kKgeSharedChunk, Lr, nch, 2 * nch, Z);
+  kge_shared_lse_kernel<<<warps_q, 256, 0, stream>>>(Z, cand, s, o, B, Bp, Lr, lse, qloss);
+  kge_shared_grad_kernel<<<dim3((Lr + 31) / 32, 2 * Bp / 32), 256, 0, stream>>>(Z, lse, cand, s, o, B, Bp, Lr, Gb, GT);
+  ADAPM_COUNT_LAUNCH(); ADAPM_COUNT_LAUNCH();
+  // dQ = G_k E_k (K = Lr), in query order; C_k = G_k^T Q_k (K = the chunk's 256 queries), [nch Lr][dpad]
+  gemm_batched(stream, Gb, 2L * Bp, ET, (long)nch * dpad, kKgeSharedChunk, dpad, Lr, kKgeSharedChunk, dpad, nch, 2 * nch, dq);
+  gemm_batched(stream, GT, (long)nch * Lr, QT, (long)nch * dpad, Lr, dpad, K2, Lr, dpad, nch, nch, C);
+  const unsigned warps_b = (unsigned)(((long)Bp * 32 + 255) / 256);
+  if (model == COMPLEX) given_kernel<COMPLEX><<<warps_b, 256, 0, stream>>>(R, s, o, rel, dq, Ne, Bp, d, dpad, gamma_e, GS);
+  else given_kernel<RESCAL><<<warps_b, 256, 0, stream>>>(R, s, o, rel, dq, Ne, Bp, d, dpad, gamma_e, GS);
+  kge_shared_entity_kernel<<<(unsigned)(((long)Ne * 32 + 255) / 256), 256, 0, stream>>>(R, C, GS, ent_off, ent_pos, Ne,
+                                                                                     nch * Lr, d, dpad, eta, U);
+  if (model == COMPLEX)
+    relation_kernel<COMPLEX><<<nrel, 256, 0, stream>>>(R, s, o, rel_off, rel_pos, dq, Ne, Bp, d, dpad, eta, gamma_r, U);
+  else relation_kernel<RESCAL><<<nrel, 256, 0, stream>>>(R, s, o, rel_off, rel_pos, dq, Ne, Bp, d, dpad, eta, gamma_r, U);
+  loss_kernel<<<1, 32, 0, stream>>>(qloss, 2 * Bp, loss);
   ADAPM_COUNT_LAUNCH(); ADAPM_COUNT_LAUNCH(); ADAPM_COUNT_LAUNCH(); ADAPM_COUNT_LAUNCH();
   ADAPM_CUDA_CHECK(cudaGetLastError());
 }

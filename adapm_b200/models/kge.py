@@ -45,6 +45,14 @@ entity row gets one AdaGrad update per step (``ops.kge_1vsall_step`` on the tens
 ``ops.kge_1vsall_reference_step`` on the CPU backend and for float64 stores). ``neg_ratio`` is not used. Since every step
 reads every entity, several ranks signal one intent for all entity keys over ``[0, CLOCK_MAX)`` at initialisation.
 
+``KGEConfig.train_type = "sampled_softmax"`` (ComplEx and RESCAL) keeps that cross-entropy at any entity count: each step
+draws ``shared_negatives`` entities (the negative sampler's seed and ``local_only`` rule), and each chunk of 128 triples
+scores its queries against one list of its subjects, its objects and those shared negatives; other copies of a query's
+answer in the list are masked. The step touches only the batch's entities, the negatives and the batch's relations
+(``ops.kge_shared_step``: three per-chunk tensor-core contractions, cost linear in the batch and ``shared_negatives``,
+deterministic on one GPU; ``ops.kge_shared_reference_step`` on the CPU backend and for float64 stores). Intents are
+per batch, as for negative sampling. ``neg_ratio`` is not used.
+
 ``KGEConfig.deterministic`` selects the deterministic one-GPU variant of the fused kernels (start-of-step reads,
 fixed-point sums, bit-identical runs); the CPU backend accepts it and already follows the start-of-step rule.
 """
@@ -82,8 +90,11 @@ class KGEConfig:
     p_norm: int = 1                  # TransE only: L1 or L2 distance
     margin: float = 1.0              # TransE: margin of the ranking loss; RotatE: gamma of the sigmoid loss
     adversarial_temperature: float = 1.0   # RotatE only: alpha of the self-adversarial negative weights (0: uniform)
-    train_type: str = "negative_sampling"  # or "1vsAll" (ComplEx, RESCAL): cross-entropy over every entity
-    max_bytes: int = 1 << 30         # 1vsAll: device memory for one chunk of scores and G (ops.kge_1vsall_step)
+    train_type: str = "negative_sampling"  # or "1vsAll" (ComplEx, RESCAL): cross-entropy over every entity,
+    #                                          or "sampled_softmax" (ComplEx, RESCAL): over shared sampled negatives
+    shared_negatives: int = 1024     # sampled_softmax: entities drawn per step, shared by the whole batch
+    max_bytes: int = 1 << 30         # 1vsAll: device memory for one chunk of scores and G (ops.kge_1vsall_step);
+    #                                  sampled_softmax: the limit of the step's workspace (ops.kge_shared_step)
 
     @property
     def entity_len(self) -> int:
@@ -150,13 +161,18 @@ def load_triples(path: str) -> torch.Tensor:
 class KGE:
     def __init__(self, server, worker, cfg: KGEConfig):
         self.server, self.worker, self.cfg = server, worker, cfg
-        if cfg.train_type not in ("negative_sampling", "1vsAll"):
-            raise ValueError(f"train_type must be 'negative_sampling' or '1vsAll', got {cfg.train_type!r}")
-        if cfg.train_type == "1vsAll":
+        if cfg.train_type not in ("negative_sampling", "1vsAll", "sampled_softmax"):
+            raise ValueError("train_type must be 'negative_sampling', '1vsAll' or 'sampled_softmax', "
+                             f"got {cfg.train_type!r}")
+        if cfg.train_type != "negative_sampling":
             if cfg.algorithm not in ("ComplEx", "RESCAL"):
-                raise ValueError(f"1vsAll training is defined for ComplEx and RESCAL, not {cfg.algorithm}")
+                raise ValueError(f"{cfg.train_type} training is defined for ComplEx and RESCAL, not {cfg.algorithm}")
             if cfg.dropout_entity > 0 or cfg.dropout_relation > 0:
-                raise ValueError("dropout is not defined for 1vsAll training")
+                raise ValueError(f"dropout is not defined for {cfg.train_type} training")
+        if cfg.train_type == "sampled_softmax" and (isinstance(cfg.shared_negatives, bool)
+                                                    or int(cfg.shared_negatives) != cfg.shared_negatives
+                                                    or cfg.shared_negatives < 0):
+            raise ValueError(f"shared_negatives must be a non-negative integer, got {cfg.shared_negatives!r}")
         if cfg.algorithm == "RotatE":
             from ..ops import _check_rotate_shape
 
@@ -264,14 +280,19 @@ class KGE:
 
     def _negatives(self, B: int):
         """The step's seed and its ``[B, 2 * neg_ratio]`` uniform negative entities, in the layout of ``_expand``
-        (corrupted objects first): the device sampler on CUDA (local keys only under the local scheme on several ranks),
-        else the rank's generator."""
+        (corrupted objects first)."""
+        seed, neg = self._draw(B * 2 * self.cfg.neg_ratio)
+        return seed, neg.view(B, 2 * self.cfg.neg_ratio)
+
+    def _draw(self, n: int):
+        """The step's seed and ``n`` uniform entities: the device sampler on CUDA (local keys only under the local scheme
+        on several ranks), else the rank's generator."""
         cfg = self.cfg
         seed = (cfg.model_seed * 7 + self.server.my_rank() * 7919 + self.step_no) & 0xFFFFFFFFFFFF
         if self.cuda:
             local_only = cfg.sampling_scheme == "local" and self.server.num_servers() > 1
-            return seed, self.sampler.sample(B * 2 * cfg.neg_ratio, seed, local_only=local_only).view(B, 2 * cfg.neg_ratio)
-        return seed, torch.randint(0, cfg.num_entities, (B, 2 * cfg.neg_ratio), generator=self._gen)
+            return seed, self.sampler.sample(n, seed, local_only=local_only)
+        return seed, torch.randint(0, cfg.num_entities, (n,), generator=self._gen)
 
     def step(self, triples_host: torch.Tensor) -> torch.Tensor:
         """One batch of positive triples ([B,3] int64 CPU tensor, pinned for the e2e path): one fused launch on CUDA,
@@ -290,6 +311,16 @@ class KGE:
                                     cfg.gamma_relation, self.loss, cfg.max_bytes)
             else:
                 loss = ops.kge_1vsall_reference_step(self.worker, triples_host, cfg)
+            self.step_no += 1
+            return self.loss if self.cuda else torch.tensor([loss], dtype=torch.float32)
+        if cfg.train_type == "sampled_softmax":
+            _, neg = self._draw(int(cfg.shared_negatives))
+            if self.cuda:
+                ops.kge_shared_step(self.worker, tr[:, 0].contiguous(), (tr[:, 1] + ne).contiguous(),
+                                    tr[:, 2].contiguous(), neg, ne, cfg.algorithm, cfg.embed_dim, cfg.eta,
+                                    cfg.gamma_entity, cfg.gamma_relation, self.loss, cfg.max_bytes)
+            else:
+                loss = ops.kge_shared_reference_step(self.worker, triples_host, neg, cfg)
             self.step_no += 1
             return self.loss if self.cuda else torch.tensor([loss], dtype=torch.float32)
         seed, neg = self._negatives(tr.shape[0])

@@ -336,9 +336,9 @@ def _kge_1vsall_chunk(num_entities: int, queries: int, max_bytes: int) -> int:
     return min(chunk, (int(queries) + 127) // 128 * 128)
 
 
-def _check_kge_1vsall_shape(algorithm: str, embed_dim: int) -> None:
+def _check_kge_1vsall_shape(algorithm: str, embed_dim: int, kind: str = "1vsAll") -> None:
     if algorithm not in _KGE_1VSALL_MODELS:
-        raise ValueError(f"1vsAll training is defined for ComplEx and RESCAL, got {algorithm!r}")
+        raise ValueError(f"{kind} training is defined for ComplEx and RESCAL, got {algorithm!r}")
     if isinstance(embed_dim, bool) or int(embed_dim) != embed_dim or not 1 <= int(embed_dim) <= KGE_1VSALL_MAX_DIM:
         raise ValueError(f"embed_dim must be an integer in [1, {KGE_1VSALL_MAX_DIM}], got {embed_dim}")
     if algorithm == "ComplEx" and int(embed_dim) % 2:
@@ -423,8 +423,6 @@ def kge_1vsall_reference_step(kv, triples: torch.Tensor, cfg, emulate_bf16: bool
     ``KGEConfig`` (``algorithm`` ComplEx or RESCAL, ``num_entities``, ``embed_dim``, ``eta``, ``gamma_entity``,
     ``gamma_relation``). ``emulate_bf16`` rounds the operands of the three contractions (queries, entities, G) to bf16
     as the tensor-core path does. Returns the summed loss of the ``2 B`` queries."""
-    from ..models.kge import complex_query
-
     _check_kge_1vsall_shape(cfg.algorithm, cfg.embed_dim)
     d, N = cfg.embed_dim, cfg.num_entities
     dt = kv.server.dtype
@@ -450,11 +448,7 @@ def kge_1vsall_reference_step(kv, triples: torch.Tensor, cfg, emulate_bf16: bool
     def rnd(x):
         return x.to(torch.bfloat16).double() if emulate_bf16 else x
 
-    if cfg.algorithm == "ComplEx":
-        Q = torch.cat([complex_query(Es, rel, conj=False), complex_query(Eo, rel, conj=True)])
-    else:
-        Rm = rel.view(-1, d, d)
-        Q = torch.cat([torch.einsum("bi,bij->bj", Es, Rm), torch.einsum("bij,bj->bi", Rm, Eo)])
+    Q = _kge_queries(cfg, Es, Eo, rel)
     ans = torch.cat([o, s])
     rows = torch.arange(ans.numel())
     Qm, Em = rnd(Q), rnd(E)
@@ -465,7 +459,31 @@ def kge_1vsall_reference_step(kv, triples: torch.Tensor, cfg, emulate_bf16: bool
     G[rows, ans] -= 1
     Gm = rnd(G)
     dQ, C = Gm @ Em, Gm.t() @ Qm
-    B = s.numel()
+    ds, do, dr = _kge_query_grads(cfg, Es, Eo, rel, dQ)
+    gE = C.clone()
+    gE.index_add_(0, s, ds + cfg.gamma_entity * Es)
+    gE.index_add_(0, o, do + cfg.gamma_entity * Eo)
+    gR = torch.zeros_like(Rr).index_add_(0, inv, dr + cfg.gamma_relation * rel)
+    kv.wait(kv.push(torch.arange(N), _kge_adagrad_rows(cfg, gE, A, dt)))
+    kv.wait(kv.push((uniq + N).contiguous(), _kge_adagrad_rows(cfg, gR, Ar, dt)))
+    return loss
+
+
+def _kge_queries(cfg, Es, Eo, rel):
+    """[object queries; subject queries] of ``KGE._query`` for the triples with subject rows Es, object rows Eo and
+    relation rows rel (float64)"""
+    from ..models.kge import complex_query
+
+    if cfg.algorithm == "ComplEx":
+        return torch.cat([complex_query(Es, rel, conj=False), complex_query(Eo, rel, conj=True)])
+    Rm = rel.view(-1, cfg.embed_dim, cfg.embed_dim)
+    return torch.cat([torch.einsum("bi,bij->bj", Es, Rm), torch.einsum("bij,bj->bi", Rm, Eo)])
+
+
+def _kge_query_grads(cfg, Es, Eo, rel, dQ):
+    """The gradients (subject, object, relation) of the triples, given dQ = the loss's gradient w.r.t. the queries of
+    :func:`_kge_queries`, without L2"""
+    d, B = cfg.embed_dim, Es.shape[0]
     dqo, dqs = dQ[:B], dQ[B:]
     if cfg.algorithm == "ComplEx":
         h = d // 2
@@ -474,21 +492,190 @@ def kge_1vsall_reference_step(kv, triples: torch.Tensor, cfg, emulate_bf16: bool
         ds = torch.cat([rre * a + rim * b, rre * b - rim * a], 1)
         do = torch.cat([rre * a2 - rim * b2, rim * a2 + rre * b2], 1)
         dr = torch.cat([sre * a + sim * b + ore * a2 + oim * b2, sre * b - sim * a + oim * a2 - ore * b2], 1)
-    else:
-        ds = torch.einsum("bij,bj->bi", Rm, dqo)
-        do = torch.einsum("bi,bij->bj", dqs, Rm)
-        dr = (torch.einsum("bi,bj->bij", Es, dqo) + torch.einsum("bi,bj->bij", dqs, Eo)).reshape(B, -1)
-    gE = C.clone()
-    gE.index_add_(0, s, ds + cfg.gamma_entity * Es)
-    gE.index_add_(0, o, do + cfg.gamma_entity * Eo)
+        return ds, do, dr
+    Rm = rel.view(-1, d, d)
+    ds = torch.einsum("bij,bj->bi", Rm, dqo)
+    do = torch.einsum("bi,bij->bj", dqs, Rm)
+    dr = (torch.einsum("bi,bj->bij", Es, dqo) + torch.einsum("bi,bj->bij", dqs, Eo)).reshape(B, -1)
+    return ds, do, dr
+
+
+def _kge_adagrad_rows(cfg, g, a, dt):
+    """the flat additive updates [-eta g / sqrt(a + g^2) | g^2] of rows with gradients g and accumulators a"""
+    u = torch.where(g == 0, torch.zeros_like(g), -cfg.eta * g / torch.sqrt(a + g * g))
+    return torch.cat([u, g * g], 1).to(dt).contiguous().view(-1)
+
+
+KGE_SHARED_CHUNK = 128
+
+
+def _kge_row_lengths_ok(server, keys: torch.Tensor, length: int) -> bool:
+    lens = server._lens_t[keys.cpu()] if server._uniform_len is None else torch.full((1,), server._uniform_len)
+    return not bool((lens != length).any())
+
+
+def kge_shared_step(kv, subj: torch.Tensor, rel: torch.Tensor, obj: torch.Tensor, negatives: torch.Tensor,
+                    num_entities: int, algorithm: str, embed_dim: int, eta: float, gamma_entity: float,
+                    gamma_relation: float, loss: torch.Tensor, max_bytes: int = 1 << 30) -> None:
+    """Sampled-softmax training step of ComplEx or RESCAL with shared negatives (csrc/cuda/ops_kge_1vsall.cu) on the
+    store of the worker ``kv``.
+
+    The triples ``(subj[i], rel[i], obj[i])`` (entity keys in ``[0, num_entities)``, relation keys after them; CUDA
+    int64) are cut into chunks of ``KGE_SHARED_CHUNK`` (128) consecutive triples. Chunk k has one candidate list
+    ``[its subjects] ++ [its objects] ++ negatives`` (``negatives``: the S >= 0 entity keys shared by the whole batch;
+    they may repeat). Each triple's object query ``(s, r, ?)`` and subject query ``(?, r, o)`` (the query vectors of
+    ``KGE._query``) is scored against every column of its chunk's list, ``z_j = <q, e_j>``. The positive column is the
+    answer's own slot in the chunk's object (or subject) block; every other column holding the answer is masked. The
+    loss of a query is ``logsumexp(z over unmasked columns) - z_pos``; ``loss`` (CUDA float32[1]) is accumulated (+=)
+    with the sum over the ``2 B`` queries. The gradients, all from the rows at the start of the step, are
+    ``G = softmax - onehot`` (0 at masked columns) through the scores to the list's entities (``G^T Q``) and to the
+    queries (``G E``), carried back to the given entity and the relation as in :func:`kge_1vsall_step`; L2
+    (``gamma_entity`` on s and o, ``gamma_relation`` on r) is added once per triple, never to an entity that is only a
+    negative. Every distinct entity and relation of the step gets one AdaGrad update ``[-eta g / sqrt(a + g^2) | g^2]``
+    of the sum of all its occurrences; no other row changes. The cost is linear in B and S, whatever the entity count.
+
+    One Pull of the step's distinct entity and relation keys and one Push of their updates go through ``kv``, so the
+    step works in every protocol state (local, replica, peer, in flight). The three contractions run per chunk on the
+    tensor cores (bf16 operands, fp32 accumulation); ``kge_shared_reference_step(..., emulate_bf16=True)`` is the same
+    rule in float64. No floating-point atomics: on one GPU two runs with the same arguments give bit-identical rows and
+    loss. ``embed_dim`` is any integer up to ``KGE_1VSALL_MAX_DIM`` (1024), even for ComplEx. ``ValueError`` on another
+    algorithm, a bad ``embed_dim``, tensors of the wrong device, dtype, contiguity or length, keys out of range, row
+    lengths that do not match the model, a store that is not float32 on CUDA, or a workspace larger than
+    ``max_bytes``."""
+    _check_kge_1vsall_shape(algorithm, embed_dim, "sampled-softmax")
+    d, N = int(embed_dim), int(num_entities)
+    server = kv.server
+    if not 1 <= N < server.num_keys():
+        raise ValueError(f"num_entities must be in [1, {server.num_keys()}), got {num_entities}")
+    for t, name in ((subj, "subj"), (rel, "rel"), (obj, "obj"), (negatives, "negatives")):
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.int64 and t.is_contiguous()):
+            raise ValueError(f"{name} must be a contiguous CUDA int64 tensor")
+    B, S = subj.numel(), negatives.numel()
+    if not (rel.numel() == B and obj.numel() == B and B > 0 and negatives.dim() == 1):
+        raise ValueError("subj, rel and obj must have the same, non-zero length, and negatives must be one-dimensional")
+    if not (isinstance(loss, torch.Tensor) and loss.is_cuda and loss.dtype == torch.float32 and loss.numel() >= 1):
+        raise ValueError("loss must be a CUDA float32 tensor")
+    if server.backend != "cuda" or server.dtype != torch.float32:
+        raise ValueError("kge_shared_step needs a float32 CUDA store (kge_shared_reference_step is the other route)")
+    ws_bytes = _C.kge_shared_workspace_bytes(B, S, d)
+    if ws_bytes > int(max_bytes):
+        raise ValueError(f"max_bytes={max_bytes} is too small: B={B}, S={S}, d={d} need a workspace of {ws_bytes} bytes")
+    ents_all = torch.cat([subj, obj, negatives])
+    lo_e, hi_e, lo_r, hi_r = torch.stack([ents_all.min(), ents_all.max(), rel.min(), rel.max()]).tolist()
+    if lo_e < 0 or hi_e >= N:
+        raise ValueError(f"entity keys must be in [0, {N}), got [{lo_e}, {hi_e}]")
+    if lo_r < N or hi_r >= server.num_keys():
+        raise ValueError(f"relation keys must be in [{N}, {server.num_keys()}), got [{lo_r}, {hi_r}]")
+    rl = 2 * d * (d if algorithm == "RESCAL" else 1)
+    ents, einv = torch.unique(ents_all, return_inverse=True)
+    uniq, inv = torch.unique(rel, return_inverse=True)
+    if not (_kge_row_lengths_ok(server, ents, 2 * d) and _kge_row_lengths_ok(server, uniq, rl)):
+        raise ValueError(f"{algorithm} at embed_dim {d} needs entity rows of {2 * d} and relation rows of {rl} values")
+    dev = subj.device
+    ch = KGE_SHARED_CHUNK
+    nch = (B + ch - 1) // ch
+    Bp, Lr = nch * ch, (2 * ch + S + 7) // 8 * 8
+    ls, lo, ln = einv[:B], einv[B:2 * B], einv[2 * B:]
+    # the padded batch: padding triples point at row 0 and are masked (their list slots hold -1)
+    pad = torch.full((Bp - B,), -1, dtype=torch.int64, device=dev)
+    cand = torch.full((nch, Lr), -1, dtype=torch.int64, device=dev)
+    cand[:, :ch] = torch.cat([ls, pad]).view(nch, ch)
+    cand[:, ch:2 * ch] = torch.cat([lo, pad]).view(nch, ch)
+    cand[:, 2 * ch:2 * ch + S] = ln
+    s_p, o_p = torch.cat([ls, pad + 1]), torch.cat([lo, pad + 1])
+    rel_p = torch.cat([inv, pad + 1]).to(torch.int32)
+    base = torch.arange(Bp, dtype=torch.int64, device=dev).view(nch, ch)
+    qorder = torch.cat([base, base + Bp], 1).view(-1)
+    # occurrences: list columns in (chunk, column) order, then the given entities (2 i: subject, 2 i + 1: object)
+    occ = torch.cat([cand.view(-1), torch.stack([ls, lo], 1).view(-1)])
+    Ne = ents.numel()
+    occ = torch.where(occ < 0, Ne, occ)
+    ent_pos = torch.argsort(occ, stable=True).to(torch.int32)
+    ent_off = torch.zeros(Ne + 1, dtype=torch.int64, device=dev)
+    ent_off[1:] = torch.cumsum(torch.bincount(occ, minlength=Ne + 1)[:Ne], 0)
+    nrel = uniq.numel()
+    rel_pos = torch.argsort(inv, stable=True).to(torch.int32)
+    rel_off = torch.zeros(nrel + 1, dtype=torch.int64, device=dev)
+    rel_off[1:] = torch.cumsum(torch.bincount(inv, minlength=nrel), 0)
+    keys = torch.cat([ents, uniq])
+    R = torch.empty(Ne * 2 * d + nrel * rl, dtype=torch.float32, device=dev)
+    kv.wait(kv.pull(keys, R, True))
+    U = torch.empty_like(R)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    _C.kge_shared_core(_stream(subj), _KGE_1VSALL_MODELS[algorithm], R.data_ptr(), s_p.data_ptr(), o_p.data_ptr(),
+                       rel_p.data_ptr(), cand.data_ptr(), qorder.data_ptr(), ent_off.data_ptr(), ent_pos.data_ptr(),
+                       rel_off.data_ptr(), rel_pos.data_ptr(), Ne, nrel, B, S, d, float(eta), float(gamma_entity),
+                       float(gamma_relation), ws.data_ptr(), U.data_ptr(), loss.data_ptr())
+    kv.wait(kv.push(keys, U, True))
+
+
+def kge_shared_reference_step(kv, triples: torch.Tensor, negatives: torch.Tensor, cfg, emulate_bf16: bool = False) -> float:
+    """The rule of :func:`kge_shared_step` in float64 through Pull / Push on either backend: the CPU route of the model
+    (and of float64 stores) and the test oracle. ``triples``: [B, 3] (subject, relation id, object); ``negatives``: the
+    S >= 0 shared entity ids; ``cfg``: a ``KGEConfig`` (``algorithm`` ComplEx or RESCAL, ``num_entities``,
+    ``embed_dim``, ``eta``, ``gamma_entity``, ``gamma_relation``). ``emulate_bf16`` rounds the operands of the three
+    contractions (queries, list entities, G) to bf16 as the tensor-core path does. Returns the summed loss of the ``2 B``
+    queries."""
+    _check_kge_1vsall_shape(cfg.algorithm, cfg.embed_dim, "sampled-softmax")
+    N = cfg.num_entities
+    dt = kv.server.dtype
+    tr = torch.as_tensor(triples, dtype=torch.int64).view(-1, 3).cpu()
+    neg = torch.as_tensor(negatives, dtype=torch.int64).view(-1).cpu()
+    s, r, o = tr[:, 0], tr[:, 1], tr[:, 2]
+    ents_all = torch.cat([s, o, neg])
+    if tr.numel() == 0 or int(ents_all.min()) < 0 or int(ents_all.max()) >= N:
+        raise ValueError(f"triples must be non-empty with entity ids (and negatives) in [0, {N})")
+    if int(r.min()) < 0 or int(r.max()) >= cfg.num_relations:
+        raise ValueError(f"relation ids must be in [0, {cfg.num_relations})")
+    B = s.numel()
+    ents, einv = torch.unique(ents_all, return_inverse=True)
+    ls, lo, ln = einv[:B], einv[B:2 * B], einv[2 * B:]
+    uniq, inv = torch.unique(r, return_inverse=True)
+    rl = cfg.relation_len
+
+    def pull(keys, width):
+        v = torch.empty(keys.numel() * width, dtype=dt)
+        kv.wait(kv.pull(keys.contiguous(), v))
+        return v.view(-1, width).double()
+
+    ent, rr = pull(ents, 2 * cfg.embed_dim), pull(uniq + N, rl)
+    E, A, Rr, Ar = ent[:, :cfg.embed_dim], ent[:, cfg.embed_dim:], rr[:, :rl // 2], rr[:, rl // 2:]
+    rel = Rr[inv]
+    Es, Eo = E[ls], E[lo]
+
+    def rnd(x):
+        return x.to(torch.bfloat16).double() if emulate_bf16 else x
+
+    Q = _kge_queries(cfg, Es, Eo, rel)
+    Qm, Em = rnd(Q), rnd(E)
+    dQ = torch.zeros_like(Q)
+    gE = torch.zeros_like(E)
+    loss = 0.0
+    for c0 in range(0, B, KGE_SHARED_CHUNK):
+        idx = torch.arange(c0, min(B, c0 + KGE_SHARED_CHUNK))
+        n = idx.numel()
+        lst = torch.cat([ls[idx], lo[idx], ln])                  # the chunk's list: subjects, objects, negatives
+        qi = torch.cat([idx, idx + B])                           # its object queries, then its subject queries
+        ans = torch.cat([lo[idx], ls[idx]])
+        pos = torch.cat([n + torch.arange(n), torch.arange(n)])
+        rows = torch.arange(2 * n)
+        live = lst.view(1, -1) != ans.view(-1, 1)
+        live[rows, pos] = True
+        Ek = Em[lst]
+        Z = (Qm[qi] @ Ek.t()).masked_fill(~live, float("-inf"))
+        lse = torch.logsumexp(Z, 1)
+        loss += float((lse - Z[rows, pos]).sum())
+        G = torch.exp(Z - lse.unsqueeze(1))
+        G[rows, pos] -= 1
+        Gm = rnd(G)
+        dQ[qi] = Gm @ Ek
+        gE.index_add_(0, lst, Gm.t() @ Qm[qi])
+    ds, do, dr = _kge_query_grads(cfg, Es, Eo, rel, dQ)
+    gE.index_add_(0, ls, ds + cfg.gamma_entity * Es)
+    gE.index_add_(0, lo, do + cfg.gamma_entity * Eo)
     gR = torch.zeros_like(Rr).index_add_(0, inv, dr + cfg.gamma_relation * rel)
-
-    def upd(g, a):
-        u = torch.where(g == 0, torch.zeros_like(g), -cfg.eta * g / torch.sqrt(a + g * g))
-        return torch.cat([u, g * g], 1).to(dt).contiguous().view(-1)
-
-    kv.wait(kv.push(torch.arange(N), upd(gE, A)))
-    kv.wait(kv.push((uniq + N).contiguous(), upd(gR, Ar)))
+    kv.wait(kv.push(ents, _kge_adagrad_rows(cfg, gE, A, dt)))
+    kv.wait(kv.push((uniq + N).contiguous(), _kge_adagrad_rows(cfg, gR, Ar, dt)))
     return loss
 
 
