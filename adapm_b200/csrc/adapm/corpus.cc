@@ -133,8 +133,11 @@ void Corpus::encode(const std::string& path, int rank, int world) {
   const std::string buf = read_file(path);
   tokens_.clear();
   sent_off_.assign(1, 0);
+  sent_line_.clear();
+  num_lines_ = 0;
   std::string tmp;
   for_each_line(buf, [&](int64_t li, size_t b, size_t e) {
+    num_lines_ = li + 1;
     if (li % world != rank) return;
     const size_t before = tokens_.size();
     for_each_word(buf, b, e, [&](std::string_view w) {
@@ -142,14 +145,18 @@ void Corpus::encode(const std::string& path, int rank, int world) {
       auto it = index_->map.find(tmp);
       if (it != index_->map.end()) tokens_.push_back(it->second);
     });
-    if (tokens_.size() > before) sent_off_.push_back((int64_t)tokens_.size());
+    if (tokens_.size() > before) {
+      sent_off_.push_back((int64_t)tokens_.size());
+      sent_line_.push_back(li);
+    }
   });
 }
 
 // ------------------------------------------------------------------------------------- batch streams
 KeyBatchStream::KeyBatchStream(std::shared_ptr<Corpus> corpus, int window, double subsample, uint64_t seed,
                                int64_t batch_keys, int queue_depth)
-    : corpus_(std::move(corpus)), window_(window), subsample_(subsample), seed_(seed), batch_keys_(batch_keys) {
+    : corpus_(std::move(corpus)), window_(window), subsample_(subsample), seed_(seed), batch_keys_(batch_keys),
+      key_space_(2 * corpus_->vocab_size()) {
   ADAPM_CHECK(window_ >= 1 && batch_keys_ >= 1 && queue_depth >= 1, "batch stream: bad window / batch size / queue depth");
   ring_.resize((size_t)queue_depth);
   for (auto& sl : ring_) sl.keys.resize((size_t)batch_keys_);
@@ -204,6 +211,7 @@ bool KeyBatchStream::walk(uint64_t epoch, F&& fn) {
     }
     const int64_t L = (int64_t)s.size();
     if (L < 2) continue;
+    sentence_ = si;
     for (int64_t pos = 0; pos < L; ++pos) {
       const int64_t b = (int64_t)(rng.next() % (uint64_t)window_);   // window shrink in [0, window)
       const int64_t r = window_ - b;
@@ -216,7 +224,7 @@ bool KeyBatchStream::walk(uint64_t epoch, F&& fn) {
 
 bool KeyBatchStream::publish(std::vector<Key>& cur, int64_t valid) {
   // distinct keys of the batch (before taking the lock: this is the expensive part)
-  if (seen_.empty()) seen_.assign((size_t)(2 * corpus_->vocab_size()), 0u);
+  if (seen_.empty()) seen_.assign((size_t)key_space_, 0u);
   if (++seen_epoch_ == 0) { std::fill(seen_.begin(), seen_.end(), 0u); seen_epoch_ = 1; }
   uniq_.clear();
   for (int64_t i = 0; i < batch_keys_; ++i) {
@@ -334,6 +342,85 @@ void WindowStream::run(uint64_t epoch) {
     return true;
   });
   if (ok && n > 0) {         // pad a short last batch with windows that train nothing
+    std::fill(cur.begin() + n * cols, cur.end(), (Key)-1);
+    publish(cur, n);
+  }
+  finish();
+}
+
+// ------------------------------------------------------------------------------------- document streams
+DocPairStream::DocPairStream(std::shared_ptr<Corpus> corpus, int window, double subsample, int64_t batch_pairs,
+                             uint64_t seed, bool dbow_words, int queue_depth)
+    : KeyBatchStream(std::move(corpus), window, subsample, seed, 2 * batch_pairs, queue_depth), batch_(batch_pairs),
+      words_(dbow_words) {
+  ADAPM_CHECK(batch_ >= 1, "DocPairStream: bad batch size");
+  key_space_ = 2 * corpus_->vocab_size() + corpus_->num_lines();
+}
+
+DocPairStream::~DocPairStream() { stop(); }
+
+void DocPairStream::run(uint64_t epoch) {
+  std::vector<Key> cur((size_t)(2 * batch_));
+  const int64_t* lines = corpus_->sentence_lines();
+  const Key doc0 = 2 * (Key)corpus_->vocab_size();
+  int64_t n = 0;
+  auto publish_pairs = [&](int64_t valid) -> bool {
+    for (int64_t i = valid; i < batch_; ++i) {   // pad a short last batch by repeating its pairs, as PairStream does
+      cur[(size_t)i] = cur[(size_t)(i % valid)];
+      cur[(size_t)(batch_ + i)] = cur[(size_t)(batch_ + i % valid)];
+    }
+    return publish(cur, valid);
+  };
+  auto emit = [&](Key input, Key target) -> bool {
+    cur[(size_t)n] = input;
+    cur[(size_t)(batch_ + n)] = target;
+    if (++n < batch_) return true;
+    n = 0;
+    return publish_pairs(batch_);
+  };
+  const bool ok = walk(epoch, [&](const std::vector<int32_t>& s, int64_t pos, int64_t lo, int64_t hi) {
+    const Key target = 2 * (Key)s[(size_t)pos] + 1;
+    if (!emit(doc0 + lines[sentence_], target)) return false;
+    if (words_)
+      for (int64_t j = lo; j < hi; ++j)
+        if (j != pos && !emit(2 * (Key)s[(size_t)j], target)) return false;
+    return true;
+  });
+  if (ok && n > 0) publish_pairs(n);
+  finish();
+}
+
+DocWindowStream::DocWindowStream(std::shared_ptr<Corpus> corpus, int window, double subsample, int64_t batch_windows,
+                                 uint64_t seed, int queue_depth)
+    : KeyBatchStream(std::move(corpus), window, subsample, seed, batch_windows * (2 + 2 * (int64_t)window), queue_depth),
+      batch_(batch_windows) {
+  ADAPM_CHECK(window >= 1 && window <= kMaxWindow, "DocWindowStream: window must be in [1, 15]");
+  key_space_ = 2 * corpus_->vocab_size() + corpus_->num_lines();
+}
+
+DocWindowStream::~DocWindowStream() { stop(); }
+
+void DocWindowStream::run(uint64_t epoch) {
+  const int64_t cols = columns();
+  const int64_t* lines = corpus_->sentence_lines();
+  const Key doc0 = 2 * (Key)corpus_->vocab_size();
+  std::vector<Key> cur((size_t)batch_keys_);
+  int64_t n = 0;
+  const bool ok = walk(epoch, [&](const std::vector<int32_t>& s, int64_t pos, int64_t lo, int64_t hi) {
+    Key* r = cur.data() + n * cols;
+    r[0] = 2 * (Key)s[(size_t)pos] + 1;
+    r[1] = doc0 + lines[sentence_];
+    int64_t k = 2;
+    for (int64_t j = lo; j < hi; ++j)
+      if (j != pos) r[k++] = 2 * (Key)s[(size_t)j];
+    std::fill(r + k, r + cols, (Key)-1);
+    if (++n == batch_) {
+      n = 0;
+      return publish(cur, batch_);
+    }
+    return true;
+  });
+  if (ok && n > 0) {
     std::fill(cur.begin() + n * cols, cur.end(), (Key)-1);
     publish(cur, n);
   }

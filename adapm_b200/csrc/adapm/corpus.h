@@ -40,7 +40,8 @@ class Corpus {
   // ... or adopt an existing vocabulary (vocab_retrieve)
   static std::shared_ptr<Corpus> from_vocab(std::vector<std::string> words, std::vector<int64_t> counts);
 
-  // Pass 2: encode this rank's share of the file (line i belongs to rank i % world) as word ids.
+  // Pass 2: encode this rank's share of the file (line i belongs to rank i % world) as word ids. Lines without an
+  // in-vocabulary word are skipped; sentence_lines() keeps the 0-based file line of every encoded sentence.
   void encode(const std::string& path, int rank, int world);
 
   const std::vector<std::string>& words() const { return words_; }
@@ -50,6 +51,8 @@ class Corpus {
   int64_t num_sentences() const { return (int64_t)sent_off_.size() - 1; }
   const int32_t* tokens() const { return tokens_.data(); }
   const int64_t* sentence_offsets() const { return sent_off_.data(); }
+  const int64_t* sentence_lines() const { return sent_line_.data(); }
+  int64_t num_lines() const { return num_lines_; }   // lines of the encoded file, every rank's
   int64_t lookup(const std::string& w) const;   // -1 if unknown
 
  private:
@@ -58,6 +61,8 @@ class Corpus {
   std::vector<int64_t> counts_;
   std::vector<int32_t> tokens_;      // in-vocabulary word ids of this rank's sentences, concatenated
   std::vector<int64_t> sent_off_;    // sentence s = tokens_[sent_off_[s] .. sent_off_[s+1])
+  std::vector<int64_t> sent_line_;   // sentence s is line sent_line_[s] of the file
+  int64_t num_lines_ = 0;
   struct Index;
   std::shared_ptr<Index> index_;
 };
@@ -91,6 +96,8 @@ class KeyBatchStream {
   double subsample_;
   uint64_t seed_;
   int64_t batch_keys_;
+  int64_t key_space_;           // keys are < key_space_ (the deduplication table's size): 2 |V| unless a stream adds keys
+  int64_t sentence_ = -1;       // inside walk()'s fn: the index of the sentence being walked
   std::atomic<uint64_t> produced_{0};
 
  private:
@@ -137,6 +144,42 @@ class WindowStream : public KeyBatchStream {
   int64_t batch_windows() const { return batch_; }
   int64_t columns() const { return 1 + 2 * (int64_t)window_; }
   uint64_t windows_produced() const { return produced_.load(); }
+
+ private:
+  void run(uint64_t epoch) override;
+  int64_t batch_;
+};
+
+// Paragraph-vector (doc2vec) streams. Sentence s of the corpus is the document on file line l = sentence_lines()[s],
+// whose key is 2 |V| + l. Both walk the corpus with PairStream's draws (subsampling and window shrink), so they relate
+// to the word streams exactly:
+//  - DocPairStream: [2, batch_pairs] pairs for PV-DBOW. For every walked position it emits (doc key, syn1 key of the
+//    word) and then, with dbow_words, the position's skip-gram pairs in PairStream's order. Removing the document pairs
+//    leaves PairStream's pairs. A short last batch is padded by repeating its pairs.
+//  - DocWindowStream: [batch_windows, 2 + 2 window] windows for PV-DM: the centre's syn1 key, the doc key, then the
+//    contexts as WindowStream lays them out. Removing column 1 leaves WindowStream's windows. window <= 15; a short
+//    last batch is padded with windows whose centre is -1.
+class DocPairStream : public KeyBatchStream {
+ public:
+  DocPairStream(std::shared_ptr<Corpus> corpus, int window, double subsample, int64_t batch_pairs, uint64_t seed,
+                bool dbow_words, int queue_depth = 8);
+  ~DocPairStream() override;
+  int64_t batch_pairs() const { return batch_; }
+
+ private:
+  void run(uint64_t epoch) override;
+  int64_t batch_;
+  bool words_;
+};
+
+class DocWindowStream : public KeyBatchStream {
+ public:
+  static constexpr int kMaxWindow = 15;
+  DocWindowStream(std::shared_ptr<Corpus> corpus, int window, double subsample, int64_t batch_windows, uint64_t seed,
+                  int queue_depth = 8);
+  ~DocWindowStream() override;
+  int64_t batch_windows() const { return batch_; }
+  int64_t columns() const { return 2 + 2 * (int64_t)window_; }
 
  private:
   void run(uint64_t epoch) override;

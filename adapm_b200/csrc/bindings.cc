@@ -276,7 +276,9 @@ PYBIND11_MODULE(_C, m) {
       .def("num_sentences", &Corpus::num_sentences)
       .def("lookup", &Corpus::lookup)
       .def("tokens_ptr", [](Corpus& c) { return (uintptr_t)c.tokens(); })
-      .def("sentence_offsets_ptr", [](Corpus& c) { return (uintptr_t)c.sentence_offsets(); });
+      .def("sentence_offsets_ptr", [](Corpus& c) { return (uintptr_t)c.sentence_offsets(); })
+      .def("sentence_lines_ptr", [](Corpus& c) { return (uintptr_t)c.sentence_lines(); })
+      .def("num_lines", &Corpus::num_lines);
   py::class_<PairStream, std::shared_ptr<PairStream>>(m, "PairStream")
       .def(py::init<std::shared_ptr<Corpus>, int, double, int64_t, uint64_t, int>(), py::arg("corpus"), py::arg("window"),
            py::arg("subsample"), py::arg("batch_pairs"), py::arg("seed"), py::arg("queue_depth") = 8)
@@ -305,6 +307,31 @@ PYBIND11_MODULE(_C, m) {
       .def("columns", &WindowStream::columns)
       .def("windows_produced", &WindowStream::windows_produced);
   m.attr("window_stream_max_window") = WindowStream::kMaxWindow;
+  py::class_<DocPairStream, std::shared_ptr<DocPairStream>>(m, "DocPairStream")
+      .def(py::init<std::shared_ptr<Corpus>, int, double, int64_t, uint64_t, bool, int>(), py::arg("corpus"),
+           py::arg("window"), py::arg("subsample"), py::arg("batch_pairs"), py::arg("seed"), py::arg("dbow_words"),
+           py::arg("queue_depth") = 8)
+      .def("start_epoch", &DocPairStream::start_epoch, py::call_guard<py::gil_scoped_release>())
+      .def("next_with_unique", [](DocPairStream& p, uintptr_t out, uintptr_t uniq) {
+             int64_t n = 0;
+             int64_t valid;
+             { py::gil_scoped_release r; valid = p.next_with_unique(ptr<Key>(out), ptr<Key>(uniq), &n); }
+             return py::make_tuple(valid, n);
+           })
+      .def("batch_pairs", &DocPairStream::batch_pairs);
+  py::class_<DocWindowStream, std::shared_ptr<DocWindowStream>>(m, "DocWindowStream")
+      .def(py::init<std::shared_ptr<Corpus>, int, double, int64_t, uint64_t, int>(), py::arg("corpus"),
+           py::arg("window"), py::arg("subsample"), py::arg("batch_windows"), py::arg("seed"), py::arg("queue_depth") = 8)
+      .def("start_epoch", &DocWindowStream::start_epoch, py::call_guard<py::gil_scoped_release>())
+      .def("next_with_unique", [](DocWindowStream& p, uintptr_t out, uintptr_t uniq) {
+             int64_t n = 0;
+             int64_t valid;
+             { py::gil_scoped_release r; valid = p.next_with_unique(ptr<Key>(out), ptr<Key>(uniq), &n); }
+             return py::make_tuple(valid, n);
+           })
+      .def("batch_windows", &DocWindowStream::batch_windows)
+      .def("columns", &DocWindowStream::columns);
+  m.attr("doc_window_stream_max_window") = DocWindowStream::kMaxWindow;
 
   // host RPC (legacy SimpleApp capability, rpc.h)
   m.attr("kServerGroup") = (int)kServerGroup;

@@ -164,6 +164,21 @@ class Cooccurrence {
   int64_t lw_ = 1;
 };
 
+// paragraph-vector (doc2vec) inference (ops_doc2vec.cu; the rule is in its header): one epoch e of the documents
+// tokens[offsets[m] .. offsets[m + 1]) (word ids) with ids doc_ids[m], each trained on its own row of state [M, 2 d]
+// (embedding | AdaGrad; written at e = 0, read and written after) against the read-only store rows; negatives drawn by
+// the sampler table (kind, prob, alias, n_table, first, stride) as ops_sampler.cu draws them. loss (may be null) +=
+// the summed logistic loss; stats[2] += rows that could not be resolved. Limits: d a multiple of 4 in [4, 336],
+// 1 <= negative <= 31, PV-DM window in [1, 15]. One launch.
+constexpr int kDoc2VecMaxDim = 336;
+constexpr int kDoc2VecMaxTargets = 32;
+constexpr int kDoc2VecMaxWindow = 15;
+constexpr int kDoc2VecMaxWords = 10000;
+void doc2vec_infer_epoch(CudaBackend& be, cudaStream_t stream, const int64_t* tokens, const int64_t* offsets,
+                         const int64_t* doc_ids, int64_t M, bool dm, int d, int negative, int window, int epoch,
+                         float alpha, uint64_t seed, int kind, const float* prob, const int32_t* alias, int64_t n_table,
+                         Key first, Key stride, float* state, float* loss, unsigned long long* stats);
+
 // node2vec / DeepWalk random walks on a CSR graph (ops_walk.cu; the rule is in its header): walk w starts at
 // starts[w] and is numbered walk_nos[w]; out [n_walks, L] int64, -1 after a node without out-edges. cumw: the inclusive
 // prefix sums of the quantised weights per node (null: unweighted). second_order: rejection sampling with the 24-bit

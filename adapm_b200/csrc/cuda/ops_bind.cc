@@ -185,6 +185,19 @@ void bind(py::module_& m) {
       })
       .def("chunks", &Cooccurrence::chunks)
       .def("denominator", &Cooccurrence::denominator);
+  m.attr("doc2vec_max_dim") = kDoc2VecMaxDim;
+  m.attr("doc2vec_max_targets") = kDoc2VecMaxTargets;
+  m.attr("doc2vec_max_window") = kDoc2VecMaxWindow;
+  m.attr("doc2vec_max_words") = kDoc2VecMaxWords;
+  m.def("doc2vec_infer_epoch", [](uintptr_t be, uintptr_t stream, uintptr_t tokens, uintptr_t offsets, uintptr_t doc_ids,
+                                  int64_t M, bool dm, int d, int negative, int window, int epoch, float alpha,
+                                  uint64_t seed, int kind, uintptr_t prob, uintptr_t alias, int64_t n_table, int64_t first,
+                                  int64_t stride, uintptr_t state, uintptr_t loss, uintptr_t stats) {
+    doc2vec_infer_epoch(backend_of(be), (cudaStream_t)stream, ptr<const int64_t>(tokens), ptr<const int64_t>(offsets),
+                        ptr<const int64_t>(doc_ids), M, dm, d, negative, window, epoch, alpha, seed, kind,
+                        ptr<const float>(prob), ptr<const int32_t>(alias), n_table, first, stride, ptr<float>(state),
+                        ptr<float>(loss), ptr<unsigned long long>(stats));
+  });
   m.def("node2vec_walks", [](uintptr_t stream, uintptr_t offsets, uintptr_t nbrs, uintptr_t cumw, uintptr_t starts,
                              uintptr_t walk_nos, int64_t n_walks, int L, uint64_t seed, uint64_t epoch,
                              uint32_t thr_return, uint32_t thr_in, uint32_t thr_out, bool second_order, uintptr_t out) {

@@ -2459,3 +2459,197 @@ def alias_draw_probabilities(prob, alias) -> np.ndarray:
         np.add.at(A, to, c * (cnt >> 16))
         np.add.at(B, to, c * (cnt & 0xFFFF))
     return A * 2.0 ** -48 + B * 2.0 ** -64
+
+
+# ---------------------------------------------------------------------------------------------- doc2vec inference
+DOC2VEC_MAX_DIM = 336
+DOC2VEC_MAX_TARGETS = 32
+DOC2VEC_MAX_WINDOW = 15
+DOC2VEC_MAX_WORDS = 10000
+
+
+def _int_arg(x, name: str) -> int:
+    if isinstance(x, bool) or not isinstance(x, (int, np.integer)):
+        raise TypeError(f"{name} must be an integer, got {type(x).__name__}")
+    return int(x)
+
+
+def _check_doc2vec_args(dm, embed_dim, negative, window, epochs, alpha, min_alpha):
+    """Validates the scalar arguments of :func:`doc2vec_infer` (``ValueError`` / ``TypeError``)."""
+    d, neg, win, E = (_int_arg(embed_dim, "embed_dim"), _int_arg(negative, "negative"), _int_arg(window, "window"),
+                      _int_arg(epochs, "epochs"))
+    if not (4 <= d <= DOC2VEC_MAX_DIM and d % 4 == 0):
+        raise ValueError(f"embed_dim must be a multiple of 4 in [4, {DOC2VEC_MAX_DIM}], got {d}")
+    if not 1 <= neg <= DOC2VEC_MAX_TARGETS - 1:
+        raise ValueError(f"negative must be in [1, {DOC2VEC_MAX_TARGETS - 1}], got {neg}")
+    if dm and not 1 <= win <= DOC2VEC_MAX_WINDOW:
+        raise ValueError(f"PV-DM needs window in [1, {DOC2VEC_MAX_WINDOW}], got {win}")
+    if E < 1:
+        raise ValueError(f"epochs must be at least 1, got {E}")
+    a, ma = float(alpha), float(min_alpha)
+    if not (math.isfinite(a) and math.isfinite(ma) and 0.0 < ma <= a):
+        raise ValueError(f"need 0 < min_alpha <= alpha, got alpha {alpha}, min_alpha {min_alpha}")
+    return bool(dm), d, neg, win, E, a, ma
+
+
+def _check_doc2vec_docs(tokens: torch.Tensor, offsets: torch.Tensor, doc_ids: torch.Tensor, num_words: int):
+    """Checks the CSR documents on the host; returns (tokens, offsets, doc_ids) as int64 CPU tensors."""
+    for t, name in ((tokens, "tokens"), (offsets, "offsets"), (doc_ids, "doc_ids")):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.int64 or t.dim() != 1:
+            raise TypeError(f"{name} must be a 1-D int64 tensor")
+    tok, off, ids = tokens.cpu(), offsets.cpu(), doc_ids.cpu()
+    M = ids.numel()
+    if off.numel() != M + 1:
+        raise ValueError(f"offsets must have M + 1 = {M + 1} entries for {M} doc_ids, got {off.numel()}")
+    lens = off[1:] - off[:-1]
+    if int(off[0]) != 0 or int(off[-1]) != tok.numel() or bool((lens < 0).any()):
+        raise ValueError("offsets must start at 0, be monotone and end at the number of tokens")
+    if M and int(lens.max()) > DOC2VEC_MAX_WORDS:
+        raise ValueError(f"a document has {int(lens.max())} words, at most {DOC2VEC_MAX_WORDS} are allowed")
+    if tok.numel() and (int(tok.min()) < 0 or int(tok.max()) >= num_words):
+        raise ValueError(f"word ids must be in [0, {num_words})")
+    return tok, off, ids
+
+
+def _doc2vec_alphas(E: int, alpha: float, min_alpha: float):
+    return [alpha - e * (alpha - min_alpha) / max(1, E - 1) for e in range(E)]
+
+
+def doc2vec_infer(server, tokens: torch.Tensor, offsets: torch.Tensor, doc_ids: torch.Tensor, sampler, *, dm: bool,
+                  embed_dim: int, negative: int, window: int, epochs: int, alpha: float, min_alpha: float, seed: int,
+                  loss: Optional[torch.Tensor] = None, num_words: Optional[int] = None) -> torch.Tensor:
+    """Paragraph-vector inference on the device (csrc/cuda/ops_doc2vec.cu): one new vector per document, trained against
+    the store's frozen rows (word ``w``'s syn0 row is key ``2 w``, its syn1 row key ``2 w + 1``). Document ``m`` is the
+    word ids ``tokens[offsets[m]:offsets[m + 1]]`` (int64 CSR, ``offsets`` [M + 1]) with the id ``doc_ids[m]``;
+    ``sampler`` is the :class:`DeviceSampler` of the model's negatives. Returns float32 ``[M, embed_dim]``.
+
+    The rule (the kernel file's header; :func:`doc2vec_infer_reference` in float64): the vector starts at
+    ``(u - 0.5) / d`` from a counter hash of ``(seed, doc_ids[m], k)`` with AdaGrad state 1e-6; epoch ``e`` uses
+    ``alpha_e = alpha - e (alpha - min_alpha) / max(1, epochs - 1)`` and visits the positions in order, scoring the
+    word's syn1 row (label 1) and ``negative`` sampler draws (label 0; one equal to the word is skipped) against
+    ``h = v`` (PV-DBOW, ``dm=False``) or the mean of ``v`` and the syn0 rows of a window shrunk by a hash draw (PV-DM),
+    then ``v += alpha_e neu1e / sqrt(a + neu1e^2)``, ``a += neu1e^2``. Store rows are only read; a document's vector does
+    not depend on the other documents of the call. ``loss``: CUDA float32 [1], accumulated (+=) with the summed
+    logistic loss. Limits (checked before any launch, ``ValueError``): ``embed_dim`` a multiple of 4 in [4, 336],
+    ``1 <= negative <= 31``, PV-DM ``1 <= window <= 15``, ``epochs >= 1``, ``0 < min_alpha <= alpha``, at most 10 000
+    words per document, word ids outside ``[0, num_words)`` (default: every id whose rows are in the store);
+    ``TypeError`` for tensors of the wrong dtype or shape.
+    The documents are checked on the host, so device tensors cost a copy. One launch per epoch."""
+    dm, d, neg, win, E, a, ma = _check_doc2vec_args(dm, embed_dim, negative, window, epochs, alpha, min_alpha)
+    if not isinstance(sampler, DeviceSampler):
+        raise TypeError("sampler must be a DeviceSampler")
+    if loss is not None and not (loss.is_cuda and loss.dtype == torch.float32 and loss.numel() >= 1):
+        raise TypeError("loss must be a CUDA float32 tensor")
+    tok, off, ids = _check_doc2vec_docs(tokens, offsets, doc_ids,
+                                        server.num_keys() // 2 if num_words is None else int(num_words))
+    dev = server.device
+    M = ids.numel()
+    state = torch.empty(M, 2 * d, dtype=torch.float32, device=dev)
+    if M == 0:
+        return state[:, :d]
+    tok_d = tok.to(dev) if tok.numel() else torch.zeros(1, dtype=torch.int64, device=dev)
+    off_d, ids_d = off.to(dev), ids.to(dev)
+    own = _gather_stats(server, None, dev)
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    for e, ae in enumerate(_doc2vec_alphas(E, a, ma)):
+        _C.doc2vec_infer_epoch(server._impl.backend_handle(), stream, tok_d.data_ptr(), off_d.data_ptr(),
+                               ids_d.data_ptr(), M, dm, d, neg, win, e, float(ae), int(seed) & _U64, sampler.kind,
+                               sampler.prob.data_ptr(), sampler.alias.data_ptr(), sampler.n, sampler.first_key,
+                               sampler.key_stride, state.data_ptr(), loss.data_ptr() if loss is not None else 0,
+                               own.data_ptr() if own is not None else 0)
+    _gathered("doc2vec_infer", own, None)
+    return state[:, :d]
+
+
+def _doc2vec_base(seed: int, doc_ids: np.ndarray) -> np.ndarray:
+    return _mix64_np(np.uint64(_mix64_int(seed)) ^ doc_ids.astype(np.uint64))
+
+
+def doc2vec_initial_vectors(seed: int, doc_ids, d: int) -> np.ndarray:
+    """The documents' starting vectors of :func:`doc2vec_infer`, float32 ``[M, d]``: ``(u - 0.5) / d`` with
+    ``u = (mix64(base ^ (2^63 | k)) >> 40) 2^-24`` and ``base = mix64(mix64(seed) ^ doc_id)``, in float32 as the
+    kernel computes it."""
+    ids = np.asarray(doc_ids, dtype=np.int64).reshape(-1)
+    base = _doc2vec_base(seed, ids)
+    k = np.arange(d, dtype=np.uint64) | np.uint64(1 << 63)
+    u = (_mix64_np(base[:, None] ^ k[None, :]) >> np.uint64(40)).astype(np.float32) * np.float32(2.0 ** -24)
+    return (u - np.float32(0.5)) / np.float32(d)
+
+
+def doc2vec_infer_reference(kv, tokens, offsets, doc_ids, sampler, *, dm: bool, embed_dim: int, negative: int,
+                            window: int, epochs: int, alpha: float, min_alpha: float, seed: int,
+                            num_words: Optional[int] = None) -> tuple:
+    """The rule of :func:`doc2vec_infer` in float64 through Pull (any backend): the initial vectors and PV-DM shrinks
+    replayed in numpy, the negatives with the sampler's draw rule (:func:`sample_keys_reference`'s, seeded per document
+    and epoch). ``sampler``: a :class:`DeviceSampler`, or a dict with its ``kind``, ``prob``, ``alias``, ``n``,
+    ``first_key`` and ``key_stride``. Vectorised over documents, sequential over positions. Returns ``(vectors float64
+    [M, d] numpy, summed loss)``."""
+    dm, d, neg, win, E, a, ma = _check_doc2vec_args(dm, embed_dim, negative, window, epochs, alpha, min_alpha)
+    sp = sampler if isinstance(sampler, dict) else {k: getattr(sampler, k) for k in
+                                                    ("kind", "prob", "alias", "n", "first_key", "key_stride")}
+    prob = np.asarray(sp["prob"].cpu() if isinstance(sp["prob"], torch.Tensor) else sp["prob"], dtype=np.float32)
+    alias = np.asarray(sp["alias"].cpu() if isinstance(sp["alias"], torch.Tensor) else sp["alias"], dtype=np.int64)
+    tok, off, ids = (torch.as_tensor(np.asarray(x), dtype=torch.int64) if not isinstance(x, torch.Tensor) else x
+                     for x in (tokens, offsets, doc_ids))
+    tok, off, ids = _check_doc2vec_docs(tok, off, ids,
+                                        kv.server.num_keys() // 2 if num_words is None else int(num_words))
+    tok, off, ids = tok.numpy(), off.numpy(), ids.numpy()
+    M = ids.size
+    lens = np.diff(off)
+    v = doc2vec_initial_vectors(seed, ids, d).astype(np.float64)
+    acc = np.full((M, d), 1e-6, dtype=np.float32).astype(np.float64)
+    total = 0.0
+    if M == 0 or tok.size == 0:
+        return v, total
+    have_k = np.zeros(0, dtype=np.int64)
+    have_r = np.zeros((0, d))
+
+    def fetch(keys):
+        """the first d values of the store rows of keys (any shape), pulled once per distinct key"""
+        nonlocal have_k, have_r
+        miss = np.setdiff1d(keys, have_k)
+        if miss.size:
+            buf = torch.empty(miss.size * 2 * d, dtype=torch.float32)
+            kv.wait(kv.pull(torch.from_numpy(miss), buf))
+            have_k = np.concatenate([have_k, miss])
+            have_r = np.concatenate([have_r, buf.view(miss.size, 2 * d)[:, :d].double().numpy()])
+            order = np.argsort(have_k)
+            have_k, have_r = have_k[order], have_r[order]
+        return have_r[np.searchsorted(have_k, keys)]
+
+    base = _doc2vec_base(seed, ids)
+    kind, n_table, first, stride = int(sp["kind"]), int(sp["n"]), int(sp["first_key"]), int(sp["key_stride"])
+    Lmax = int(lens.max())
+    for e, ae in enumerate(_doc2vec_alphas(E, a, ma)):
+        es = _mix64_np(base ^ np.uint64((1 << 62) | e))
+        ss = _mix64_np(es)
+        for i in range(Lmax):
+            act = np.flatnonzero(lens > i)                                   # documents that have position i
+            pos_key = 2 * tok[off[act] + i] + 1
+            n = (np.uint64(i * neg) + np.arange(neg, dtype=np.uint64))[None, :]
+            h = _mix64_np(es[act, None] ^ (n * np.uint64(0x9E3779B97F4A7C15)))
+            draws = _sampler_draw(kind, h, prob, alias, n_table, first, stride)        # [A, neg]
+            tkeys = np.concatenate([pos_key[:, None], draws], 1)
+            valid = np.ones(tkeys.shape, dtype=bool)
+            valid[:, 1:] = draws != pos_key[:, None]
+            T = fetch(tkeys)                                                 # [A, 1 + neg, d]
+            hv = v[act].copy()
+            if dm:
+                r = win - (_mix64_np(ss[act] ^ np.uint64(i)) % np.uint64(win)).astype(np.int64)
+                for delta in range(-win, win + 1):                           # ascending context positions
+                    j = i + delta
+                    m = (delta != 0) & (np.abs(delta) <= r) & (j >= 0) & (j < lens[act])
+                    if m.any():
+                        hv[m] += fetch(2 * tok[off[act[m]] + j])
+                C = np.minimum(lens[act], i + r + 1) - np.maximum(0, i - r) - 1
+                hv /= (1 + C)[:, None]
+            f = np.einsum("ad,atd->at", hv, T)
+            label = np.zeros(f.shape)
+            label[:, 0] = 1
+            g = np.where(f > 6, label - 1, np.where(f < -6, label, label - 1 / (1 + np.exp(-f)))) * valid
+            z = np.clip(np.where(label > 0.5, f, -f), -6, 6)
+            total += float((np.log1p(np.exp(-z)) * valid).sum())
+            neu = np.einsum("at,atd->ad", g, T)
+            v[act] += ae * neu / np.sqrt(acc[act] + neu * neu)
+            acc[act] += neu * neu
+    return v, total

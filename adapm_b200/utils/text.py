@@ -241,6 +241,18 @@ class NativeCorpus:
         off = np.ctypeslib.as_array((ctypes.c_int64 * (ns + 1)).from_address(self._impl.sentence_offsets_ptr())).copy()
         return tok, off
 
+    def sentence_lines(self) -> np.ndarray:
+        """The 0-based file line of every encoded sentence (int64 numpy copy): lines without an in-vocabulary word are
+        not sentences, so sentence ``s`` is line ``sentence_lines()[s]``, the document ``s`` of paragraph vectors."""
+        import ctypes
+
+        ns = self.num_sentences()
+        return np.ctypeslib.as_array((ctypes.c_int64 * max(ns, 1)).from_address(self._impl.sentence_lines_ptr()))[:ns].copy()
+
+    def num_lines(self) -> int:
+        """Lines of the encoded file, every rank's: the number of documents."""
+        return self._impl.num_lines()
+
     def pair_batches(self, window: int, subsample: float, batch_pairs: int, seed: int, epoch: int = 0,
                      pin: bool = False, queue_depth: int = 8) -> Iterator[torch.Tensor]:
         """[2, batch_pairs] key batches of one epoch, generated by a background C++ thread. A short final batch is
@@ -273,6 +285,54 @@ class NativeCorpus:
         if not 1 <= window <= _C.window_stream_max_window:
             raise ValueError(f"window must be in [1, {_C.window_stream_max_window}], got {window}")
         ws = _C.WindowStream(self._impl, int(window), float(subsample), int(batch_windows), int(seed), int(queue_depth))
+        ws.start_epoch(int(epoch))
+        cols = ws.columns()
+        while True:
+            t = torch.empty(batch_windows, cols, dtype=torch.int64)
+            if pin:
+                t = t.pin_memory()
+            u = torch.empty(batch_windows * cols, dtype=torch.int64)
+            valid, n_u = ws.next_with_unique(t.data_ptr(), u.data_ptr())
+            if valid == 0:
+                return
+            t.valid_windows = int(valid)
+            t.unique_keys = u[:n_u]
+            yield t
+
+    def doc_pair_batches(self, window: int, subsample: float, batch_pairs: int, seed: int, dbow_words: bool,
+                         epoch: int = 0, pin: bool = False, queue_depth: int = 8) -> Iterator[torch.Tensor]:
+        """PV-DBOW key batches [2, batch_pairs] of one epoch (doc2vec), from a background C++ thread with the draws of
+        :meth:`pair_batches`. Every walked position gives the pair ``(2 V + line, 2 w + 1)`` of its document's key and its
+        word, followed with ``dbow_words`` by the position's skip-gram pairs as :meth:`pair_batches` emits them. A short
+        final batch is padded by repeating its pairs; ``valid_pairs`` and ``unique_keys`` as for :meth:`pair_batches`."""
+        from .. import _C
+
+        ps = _C.DocPairStream(self._impl, int(window), float(subsample), int(batch_pairs), int(seed), bool(dbow_words),
+                              int(queue_depth))
+        ps.start_epoch(int(epoch))
+        while True:
+            t = torch.empty(2, batch_pairs, dtype=torch.int64)
+            if pin:
+                t = t.pin_memory()
+            u = torch.empty(2 * batch_pairs, dtype=torch.int64)
+            valid, n_u = ps.next_with_unique(t.data_ptr(), u.data_ptr())
+            if valid == 0:
+                return
+            t.valid_pairs = int(valid)
+            t.unique_keys = u[:n_u]
+            yield t
+
+    def doc_window_batches(self, window: int, subsample: float, batch_windows: int, seed: int, epoch: int = 0,
+                           pin: bool = False, queue_depth: int = 8) -> Iterator[torch.Tensor]:
+        """PV-DM window batches [batch_windows, 2 + 2 * window] of one epoch (doc2vec): the centre's syn1 key, the
+        document's key ``2 V + line``, then the contexts as :meth:`window_batches` lays them out, with its draws.
+        ``window <= 15``. Padding, ``valid_windows`` and ``unique_keys`` as for :meth:`window_batches`."""
+        from .. import _C
+
+        if not 1 <= window <= _C.doc_window_stream_max_window:
+            raise ValueError(f"window must be in [1, {_C.doc_window_stream_max_window}], got {window}")
+        ws = _C.DocWindowStream(self._impl, int(window), float(subsample), int(batch_windows), int(seed),
+                                int(queue_depth))
         ws.start_epoch(int(epoch))
         cols = ws.columns()
         while True:
