@@ -265,6 +265,17 @@ void gather_dist_topk(CudaBackend& be, cudaStream_t stream, const float* q, cons
 // forward (1 launch): out[nbags, E] = pooled rows, each bag summed in fp32 in key order.
 // backward (4 launches, the radix sort counted as one): G_k = grad_scale * sum over the occurrences of k of
 // c_i * grad_out[bag(i)] in position order, then push [-lr G / sqrt(acc + G^2) | G^2] once per distinct key.
+// DLRM dot interaction (ops_dlrm.cu), fp32, one launch each way. z [B, E], e [B, F, E] (the pooled bags in place),
+// R [B, W] with W = E + F (F + 1) / 2 rounded up to 8: R = [z | <T_i, T_j> for j < i, row-major | 0] where
+// T = [z; e_0 .. e_{F-1}]. backward: dz = dR[:, :E] + dT_0, de_f = dT_{f+1} with dT_i = sum_{j != i} dZ_ij T_j.
+// 1 <= F, F + 1 <= 64, E % 4 == 0 in [4, 512], B * W < 2^31; 16-byte aligned pointers. Bit-identical reruns.
+constexpr int kDlrmMaxRows = 64;
+constexpr int kDlrmMaxDim = 512;
+void dlrm_interaction_forward(cudaStream_t stream, const float* z, const float* e, int64_t B, int F, int E, int W,
+                              float* R);
+void dlrm_interaction_backward(cudaStream_t stream, const float* dR, const float* z, const float* e, int64_t B, int F,
+                               int E, int W, float* dz, float* de);
+
 constexpr int kEmbBagMaxDim = 512;
 size_t embedding_bag_workspace_bytes(int64_t nnz, int E);
 void embedding_bag_forward(CudaBackend& be, cudaStream_t stream, const Key* keys, const int64_t* offsets,

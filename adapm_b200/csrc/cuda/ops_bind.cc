@@ -260,6 +260,17 @@ void bind(py::module_& m) {
                            ptr<const float>(weights), nnz, nbags, E, mean, ptr<const float>(grad_out), lr, grad_scale,
                            ptr<void>(ws), ws_bytes, ptr<unsigned long long>(stats));
   });
+  m.attr("dlrm_max_rows") = kDlrmMaxRows;
+  m.attr("dlrm_max_dim") = kDlrmMaxDim;
+  m.def("dlrm_interaction_forward", [](uintptr_t stream, uintptr_t z, uintptr_t e, int64_t B, int F, int E, int W,
+                                       uintptr_t R) {
+    dlrm_interaction_forward((cudaStream_t)stream, ptr<const float>(z), ptr<const float>(e), B, F, E, W, ptr<float>(R));
+  });
+  m.def("dlrm_interaction_backward", [](uintptr_t stream, uintptr_t dR, uintptr_t z, uintptr_t e, int64_t B, int F,
+                                        int E, int W, uintptr_t dz, uintptr_t de) {
+    dlrm_interaction_backward((cudaStream_t)stream, ptr<const float>(dR), ptr<const float>(z), ptr<const float>(e), B,
+                              F, E, W, ptr<float>(dz), ptr<float>(de));
+  });
   m.attr("ffm_max_fields") = kFfmMaxFields;
   m.attr("ffm_max_k") = kFfmMaxK;
   m.attr("ffm_max_fk") = kFfmMaxFk;

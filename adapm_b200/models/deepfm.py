@@ -73,14 +73,20 @@ class TensorCoreLinear(torch.autograd.Function):
 
 
 class DenseNet(nn.Module):
-    def __init__(self, cfg: DeepFMConfig, use_tensor_cores: bool):
+    """MLP with He-initialised weights from ``seed`` (default ``cfg.model_seed``); ``dims`` defaults to DeepFM's
+    ``F * k -> hidden... -> 1``. ReLU after every layer but the last (and after the last with ``relu_last``); a single
+    output column is returned as ``[B]``. The last layer runs in fp32, the others on the wgmma GEMM with
+    ``use_tensor_cores`` unless ``cfg.precision == 'fp32'``."""
+
+    def __init__(self, cfg, use_tensor_cores: bool, dims=None, relu_last: bool = False, seed=None):
         super().__init__()
-        dims = [cfg.num_fields * cfg.embed_dim] + list(cfg.hidden) + [1]
-        g = torch.Generator().manual_seed(cfg.model_seed)
+        if dims is None:
+            dims = [cfg.num_fields * cfg.embed_dim] + list(cfg.hidden) + [1]
+        g = torch.Generator().manual_seed(cfg.model_seed if seed is None else seed)
         self.w = nn.ParameterList([nn.Parameter(torch.randn(dims[i + 1], dims[i], generator=g) * (2.0 / dims[i]) ** 0.5)
                                    for i in range(len(dims) - 1)])
         self.b = nn.ParameterList([nn.Parameter(torch.zeros(dims[i + 1])) for i in range(len(dims) - 1)])
-        self.tc, self.precision = use_tensor_cores, cfg.precision
+        self.tc, self.precision, self.relu_last = use_tensor_cores, cfg.precision, relu_last
 
     def forward(self, x):
         for i, (w, b) in enumerate(zip(self.w, self.b)):
@@ -89,9 +95,9 @@ class DenseNet(nn.Module):
                 x = TensorCoreLinear.apply(x, w, self.precision) + b
             else:
                 x = x @ w.t() + b
-            if not last:
+            if not last or self.relu_last:
                 x = torch.relu(x)
-        return x.view(-1)
+        return x.view(-1) if x.shape[1] == 1 else x
 
 
 class DeepFM:

@@ -1901,6 +1901,123 @@ def embedding_bag_reference(table: torch.Tensor, keys: torch.Tensor, offsets: to
     return out, new
 
 
+DLRM_MAX_ROWS = 64          # F + 1 (the bottom-MLP output and the F fields)
+
+
+def dlrm_interaction_width(F: int, E: int) -> int:
+    """W, the width of :func:`dlrm_interaction`'s output: E + F (F + 1) / 2 rounded up to a multiple of 8."""
+    return (E + F * (F + 1) // 2 + 7) // 8 * 8
+
+
+def _check_dlrm_args(z, e):
+    for t, nm in ((z, "z"), (e, "e")):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.float32:
+            raise TypeError(f"{nm} must be a float32 tensor")
+    if z.dim() != 2 or e.dim() != 3:
+        raise ValueError(f"z must be [B, E] and e [B, F, E], got {tuple(z.shape)} and {tuple(e.shape)}")
+    if e.device != z.device:
+        raise TypeError(f"z and e must be on one device, got {z.device} and {e.device}")
+    B, E = z.shape
+    F = e.shape[1]
+    if e.shape[0] != B or e.shape[2] != E:
+        raise ValueError(f"e must be [B, F, E] = [{B}, F, {E}], got {tuple(e.shape)}")
+    if not 1 <= F <= DLRM_MAX_ROWS - 1:
+        raise ValueError(f"dlrm_interaction needs 1 <= F and F + 1 <= {DLRM_MAX_ROWS}, got F = {F}")
+    if E % 4 or not 4 <= E <= EMBEDDING_BAG_MAX_DIM:
+        raise ValueError(f"dlrm_interaction needs E a multiple of 4 in [4, {EMBEDDING_BAG_MAX_DIM}], got E = {E}")
+    W = dlrm_interaction_width(F, E)
+    if B * W >= 1 << 31:
+        raise ValueError(f"dlrm_interaction needs B * W < 2^31, got B = {B}, W = {W}")
+    return B, F, E, W
+
+
+def _dlrm_pairs(F: int, device):
+    return torch.tril_indices(F + 1, F + 1, offset=-1, device=device)
+
+
+def _dlrm_interaction_torch(z, e):
+    B, F, E, W = z.shape[0], e.shape[1], z.shape[1], dlrm_interaction_width(e.shape[1], z.shape[1])
+    T = torch.cat([z[:, None], e], 1)
+    Z = torch.bmm(T, T.transpose(1, 2))
+    i, j = _dlrm_pairs(F, z.device)
+    pad = z.new_zeros(B, W - E - i.numel())
+    return torch.cat([z, Z[:, i, j], pad], 1)
+
+
+class _DlrmInteractionFn(torch.autograd.Function):
+    """The fused route of :func:`dlrm_interaction`: one kernel each way (csrc/cuda/ops_dlrm.cu)."""
+
+    @staticmethod
+    def forward(ctx, z, e):
+        B, F, E, W = _check_dlrm_args(z, e)
+        z, e = _dlrm_aligned(z), _dlrm_aligned(e)
+        R = torch.empty(B, W, dtype=torch.float32, device=z.device)
+        _C.dlrm_interaction_forward(_stream(z), z.data_ptr(), e.data_ptr(), B, F, E, W, R.data_ptr())
+        ctx.save_for_backward(z, e)
+        return R
+
+    @staticmethod
+    def backward(ctx, dR):
+        z, e = ctx.saved_tensors
+        B, F, E = e.shape
+        dR = _dlrm_aligned(dR.to(torch.float32))
+        dz, de = torch.empty_like(z), torch.empty_like(e)
+        _C.dlrm_interaction_backward(_stream(dR), dR.data_ptr(), z.data_ptr(), e.data_ptr(), B, F, E,
+                                     dR.shape[1], dz.data_ptr(), de.data_ptr())
+        return dz, de
+
+
+def _dlrm_aligned(t: torch.Tensor) -> torch.Tensor:
+    """contiguous, with a 16-byte aligned start (the kernels read and write float4)"""
+    t = t.contiguous()
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
+def dlrm_interaction(z: torch.Tensor, e: torch.Tensor, impl: str = "auto") -> torch.Tensor:
+    """DLRM's dot interaction (Naumov et al., 2019): ``R [B, W]`` from the bottom-MLP output ``z`` float32 ``[B, E]``
+    and the pooled field embeddings ``e`` float32 ``[B, F, E]`` (as :class:`StoreEmbeddingBag` returns them, viewed
+    ``[B, F, E]``). With ``T = [z; e_0; ..; e_{F-1}]`` (``F + 1`` rows), ``R[:, :E] = z``, ``R[:, E + p]`` is the dot
+    product ``<T_i, T_j>`` of the p-th pair ``j < i`` in the order of ``torch.tril_indices(F + 1, F + 1, -1)``, and the
+    ``W - E - F (F + 1) / 2`` pad columns (:func:`dlrm_interaction_width`) are 0; their gradients are ignored.
+
+    Autograd reaches both ``z`` and ``e``. ``impl``: ``fused`` (CUDA tensors) - one kernel forward and one backward,
+    fp32 sums in a fixed order, bit-identical reruns; ``torch`` - ``cat``, ``bmm``, the ``tril`` gather and ``cat``
+    (CPU tensors, and the comparison arm of benchmarks/dlrm_bench.py); ``auto`` picks ``fused`` for CUDA tensors.
+    Limits: ``1 <= F``, ``F + 1 <= 64``, ``E`` a multiple of 4 in [4, 512], ``B * W < 2^31``."""
+    if impl not in ("auto", "fused", "torch"):
+        raise ValueError(f"impl must be 'auto', 'fused' or 'torch', got {impl!r}")
+    _check_dlrm_args(z, e)
+    if impl == "auto":
+        impl = "fused" if z.is_cuda else "torch"
+    if impl == "torch":
+        return _dlrm_interaction_torch(z, e)
+    if not z.is_cuda:
+        raise ValueError("impl='fused' needs CUDA tensors")
+    return _DlrmInteractionFn.apply(z, e)
+
+
+def dlrm_interaction_reference(z: torch.Tensor, e: torch.Tensor, grad_out: Optional[torch.Tensor] = None):
+    """The rule of :func:`dlrm_interaction` in float64 on the CPU (tests): ``(R, dz, de)``; ``dz`` and ``de`` are the
+    gradients for ``grad_out`` ``[B, W]`` (None without it)."""
+    z64, e64 = z.detach().cpu().double(), e.detach().cpu().double()
+    B, E = z64.shape
+    F = e64.shape[1]
+    W = dlrm_interaction_width(F, E)
+    T = torch.cat([z64[:, None], e64], 1)                        # [B, N, E]
+    i, j = _dlrm_pairs(F, "cpu")
+    R = torch.zeros(B, W, dtype=torch.float64)
+    R[:, :E] = z64
+    R[:, E:E + i.numel()] = (T[:, i] * T[:, j]).sum(-1)
+    if grad_out is None:
+        return R, None, None
+    g = grad_out.detach().cpu().double()
+    dZ = torch.zeros(B, F + 1, F + 1, dtype=torch.float64)
+    dZ[:, i, j] = g[:, E:E + i.numel()]
+    dZ = dZ + dZ.transpose(1, 2)
+    dT = torch.bmm(dZ, T)
+    return R, g[:, :E] + dT[:, 0], dT[:, 1:]
+
+
 FFM_MAX_FIELDS = 64
 FFM_MAX_K = 32
 FFM_MAX_FK = 512
