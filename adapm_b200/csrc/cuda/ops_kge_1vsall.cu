@@ -20,8 +20,8 @@
 // of the shape only (partial_splits), so it is the same on every H100. C sums its chunks in chunk order, every reduction (logsumexp, the loss,
 // the sum over a row's occurrences) runs in a fixed order, and every output row has one writer. On one GPU the same
 // inputs give bit-identical updates and loss. Kernels, in order (per chunk: z GEMM, lse, grad, dq / c GEMMs and sums):
-//   gemm_partial_kernel  P[z] = A B^T over split z's k-blocks (ops_gemm_wgmma.cu's tile: TMA producer warpgroup, two
-//                     wgmma consumer warpgroups)
+//   gemm_partial_kernel  P[z] = A B^T over split z's k-blocks (gemm_nt_bf16's tile, tc::tma_tile: TMA producer
+//                     warpgroup, two wgmma consumer warpgroups)
 //   query_kernel      Qf = queries of the pulled rows (fp32), one warp per query
 //   to_bf16_kernel    fp32 rows -> bf16 operand [rows, dpad] and its transpose (chunk-major), 32 x 32 tiles
 //   row_lse_kernel    per query: logsumexp over the N scores (one warp, fixed order) and its cross-entropy
@@ -64,54 +64,18 @@ namespace {
 
 enum Model : int { COMPLEX = 0, RESCAL = 1 };
 
-// One 128 x 128 tile per CTA of the products gemm_partial_kernel (!BATCHED) and gemm_batched_kernel (BATCHED) compute:
-// the TMA producer warp loads the tile's k-blocks into the ring, the two wgmma consumer warpgroups store the fp32 tile.
-template <bool BATCHED>
-__device__ __forceinline__ void tile_product(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, int M, int N, int K,
-                                             int a_rows, int b_rows, int nb, float* __restrict__ P) {
-  using namespace tc;
-  constexpr int BK = 64;
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
-  SmemLayout& sm = *reinterpret_cast<SmemLayout*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tile_n = blockIdx.x, tile_m = blockIdx.y;
-  const int total_kb = (K + BK - 1) / BK;
-  const int kb_per = BATCHED ? total_kb : (total_kb + (int)gridDim.z - 1) / (int)gridDim.z;
-  const int kb0 = BATCHED ? 0 : (int)blockIdx.z * kb_per;
-  const int num_kb = BATCHED ? total_kb : min(kb_per, total_kb - kb0);
-  const int a_row = BATCHED ? (int)blockIdx.z * a_rows + tile_m * BM : tile_m * BM;
-  const int b_row = BATCHED ? ((int)blockIdx.z % nb) * b_rows + tile_n * BN : tile_n * BN;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&sm.full_bar[s], 1); mbar_init(&sm.empty_bar[s], kConsumerWarps); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  __syncthreads();
-  if (warp < 4) {
-    if (threadIdx.x == 0) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        mbar_wait(&sm.empty_bar[s], ((uint32_t)(kb / STAGES) & 1u) ^ 1u);
-        mbar_expect_tx(&sm.full_bar[s], A_BYTES + B_BYTES);
-        tma_load_2d(sm.a[s], &tmap_a, &sm.full_bar[s], (kb0 + kb) * BK, a_row);
-        tma_load_2d(sm.b[s], &tmap_b, &sm.full_bar[s], (kb0 + kb) * BK, b_row);
-      }
-    }
-  } else {
-    const int wg = (warp >> 2) - 1;
-    float d[64];
-    consume_ring<KIND_BF16>(sm, num_kb, wg, lane, d);
-    store_fragment(d, 1.f, P + (size_t)blockIdx.z * M * N, N, tile_m * BM + wg * 64 + (warp & 3) * 16, tile_n * BN, M, N,
-                   lane, false);
-  }
-}
-
 // P[blockIdx.z][M][N] (fp32) = A[M, K] x B[N, K]^T (bf16, K-major) over the k-blocks of split blockIdx.z, one 128 x 128
 // tile per CTA. The host picks splits so that none is empty.
 __global__ void __launch_bounds__(tc::kGemmThreads, 1)
 gemm_partial_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N,
                     int K, float* __restrict__ P) {
-  tile_product<false>(tmap_a, tmap_b, M, N, K, 0, 0, 1, P);
+  using namespace tc;
+  const int tile_n = blockIdx.x, tile_m = blockIdx.y;
+  const KRange kr = k_split((K + BK<KIND_BF16> - 1) / BK<KIND_BF16>);
+  float d[64];
+  if (tma_tile<KIND_BF16>(tmap_a, tmap_b, tile_m * BM, tile_n * BN, kr.kb0, kr.num_kb, d))
+    store_fragment(d, 1.f, P + (size_t)blockIdx.z * M * N, N, tile_m * BM + frag_row0(threadIdx.x >> 5), tile_n * BN, M,
+                   N, threadIdx.x & 31, false);
 }
 
 // Batched products over all of K: P[z][M][N] (fp32) = A_z [M, K] x B_z [N, K]^T for z = blockIdx.z, where A_z starts at
@@ -120,7 +84,13 @@ gemm_partial_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
 __global__ void __launch_bounds__(tc::kGemmThreads, 1)
 gemm_batched_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N,
                     int K, int a_rows, int b_rows, int nb, float* __restrict__ P) {
-  tile_product<true>(tmap_a, tmap_b, M, N, K, a_rows, b_rows, nb, P);
+  using namespace tc;
+  const int tile_n = blockIdx.x, tile_m = blockIdx.y, z = blockIdx.z;
+  float d[64];
+  if (tma_tile<KIND_BF16>(tmap_a, tmap_b, z * a_rows + tile_m * BM, (z % nb) * b_rows + tile_n * BN, 0,
+                          (K + BK<KIND_BF16> - 1) / BK<KIND_BF16>, d))
+    store_fragment(d, 1.f, P + (size_t)z * M * N, N, tile_m * BM + frag_row0(threadIdx.x >> 5), tile_n * BN, M, N,
+                   threadIdx.x & 31, false);
 }
 
 // Splits of K for gemm_partial: about two CTAs per SM of a 132-SM H100, at least 4 k-blocks per split, at most 64
@@ -135,40 +105,20 @@ int partial_splits(int M, int N, int K) {
 
 // P[z] (z < partial_splits(M, N, K)) = the product over split z; K a multiple of 8 (16-byte TMA row pitch).
 void gemm_partial(cudaStream_t stream, const void* A, const void* B, int M, int N, int K, float* P) {
-  ADAPM_CHECK(K % 8 == 0 && (((uintptr_t)A) & 15u) == 0 && (((uintptr_t)B) & 15u) == 0,
-              "kge_1vsall: GEMM operands must be 16-byte aligned with a K extent that is a multiple of 8");
-  const CUtensorMap ma = tc::make_map(A, M, K, tc::BM, tc::KIND_BF16);
-  const CUtensorMap mb = tc::make_map(B, N, K, tc::BN, tc::KIND_BF16);
-  const size_t smem = sizeof(tc::SmemLayout) + 1024;
-  static bool attr_set = false;
-  if (!attr_set) {
-    ADAPM_CUDA_CHECK(cudaFuncSetAttribute(gemm_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  const CUtensorMap ma = tc::make_map("kge_1vsall", A, M, K, tc::BM, tc::KIND_BF16);
+  const CUtensorMap mb = tc::make_map("kge_1vsall", B, N, K, tc::BN, tc::KIND_BF16);
   const dim3 grid((N + tc::BN - 1) / tc::BN, (M + tc::BM - 1) / tc::BM, partial_splits(M, N, K));
-  gemm_partial_kernel<<<grid, tc::kGemmThreads, smem, stream>>>(ma, mb, M, N, K, P);
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_CUDA_CHECK(cudaGetLastError());
+  tc::launch<gemm_partial_kernel, tc::Ring<tc::STAGES>>(grid, stream, ma, mb, M, N, K, P);
 }
 
 // P[z] (z < batches) = A_z B_z^T of gemm_batched_kernel; A holds a_total rows and B b_total rows of K values (K a
 // multiple of 8: 16-byte TMA row pitch).
 void gemm_batched(cudaStream_t stream, const void* A, long a_total, const void* B, long b_total, int M, int N, int K,
                   int a_rows, int b_rows, int nb, int batches, float* P) {
-  ADAPM_CHECK(K % 8 == 0 && (((uintptr_t)A) & 15u) == 0 && (((uintptr_t)B) & 15u) == 0,
-              "kge_shared: GEMM operands must be 16-byte aligned with a K extent that is a multiple of 8");
-  const CUtensorMap ma = tc::make_map(A, a_total, K, tc::BM, tc::KIND_BF16);
-  const CUtensorMap mb = tc::make_map(B, b_total, K, tc::BN, tc::KIND_BF16);
-  const size_t smem = sizeof(tc::SmemLayout) + 1024;
-  static bool attr_set = false;
-  if (!attr_set) {
-    ADAPM_CUDA_CHECK(cudaFuncSetAttribute(gemm_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  const CUtensorMap ma = tc::make_map("kge_shared", A, a_total, K, tc::BM, tc::KIND_BF16);
+  const CUtensorMap mb = tc::make_map("kge_shared", B, b_total, K, tc::BN, tc::KIND_BF16);
   const dim3 grid((N + tc::BN - 1) / tc::BN, (M + tc::BM - 1) / tc::BM, batches);
-  gemm_batched_kernel<<<grid, tc::kGemmThreads, smem, stream>>>(ma, mb, M, N, K, a_rows, b_rows, nb, P);
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_CUDA_CHECK(cudaGetLastError());
+  tc::launch<gemm_batched_kernel, tc::Ring<tc::STAGES>>(grid, stream, ma, mb, M, N, K, a_rows, b_rows, nb, P);
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

@@ -37,21 +37,17 @@ using namespace tc;
 
 constexpr int TK_STAGES = 4;          // 128 KiB ring + 66 KiB of lists (a 6-stage ring would leave no room)
 constexpr int LSTRIDE = kTopkMax + 1; // padded list row: the 8 rows that a lane group scans sit in distinct banks
-constexpr int BK_ELEMS = 64;          // bf16 elements per 128-byte K-block row
 constexpr uint32_t NO_COL = 0xFFFFFFFFu;  // padding entry (-inf, NO_COL): loses to every eligible column
 constexpr int kMaxSlices = 2048;
 constexpr int kMergeWarps = 4;
 
 struct TopkSmem {
-  alignas(1024) unsigned char a[TK_STAGES][A_BYTES];
-  alignas(1024) unsigned char b[TK_STAGES][B_BYTES];
+  Ring<TK_STAGES> ring;
   float list_v[BM][LSTRIDE];
   uint32_t list_c[BM][LSTRIDE];
   float thr_v[BM];                    // the row's worst list entry = the score a new column has to beat
   uint32_t thr_c[BM];
   int worst[BM];                      // its position in the list
-  alignas(8) unsigned long long full_bar[TK_STAGES];
-  alignas(8) unsigned long long empty_bar[TK_STAGES];
 };
 
 struct TopkArgs {
@@ -63,62 +59,9 @@ struct TopkArgs {
   int* part_c;
 };
 
-// Gather thread t: k-block [k0, k0 + 64) of its store row -> bf16 -> row t of the swizzled K-major B tile (zeros past K
-// or for a null row; K % 4 == 0). The same conversion and layout as the staging in gather_gemm_kernel, which keeps its
-// inline copy so that its code stays as it is.
-__device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
-__device__ __forceinline__ void stage_row_bf16(unsigned char* tile, const Ctx& c, Key key, dev::GatherRow& row, int t,
-                                               int k0, int K) {
-  unsigned char* dst_row = tile + (size_t)t * ROW_BYTES;
-  float4 v[16];
-  do {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int k = k0 + 4 * j;
-      v[j] = (row.row && k < K) ? dev::ld_gather4(row, k) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-  } while (dev::gather_reread(c, key, row));
-  // 8 chunks of 8 bf16; chunk c goes to position c ^ (t & 7)  (128-byte swizzle)
-#pragma unroll
-  for (int ch = 0; ch < 8; ++ch) {
-    uint4 o;
-    o.x = pack_bf16(v[2 * ch].x, v[2 * ch].y);
-    o.y = pack_bf16(v[2 * ch].z, v[2 * ch].w);
-    o.z = pack_bf16(v[2 * ch + 1].x, v[2 * ch + 1].y);
-    o.w = pack_bf16(v[2 * ch + 1].z, v[2 * ch + 1].w);
-    *reinterpret_cast<uint4*>(dst_row + ((ch ^ (t & 7)) << 4)) = o;
-  }
-}
-
 // (v, c) comes before (tv, tc): higher score, or the same score and a smaller column. False for a NaN v.
 __device__ __forceinline__ bool beats(float v, uint32_t c, float tv, uint32_t tc) {
   return v > tv || (v == tv && c < tc);
-}
-
-// Consumer warpgroup `wg`: accumulate one tile over num_kb k-blocks. `it` counts k-blocks over all tiles of the CTA, so
-// stage and phase continue from the previous tile, and every stage is released once its wgmmas retired - including the
-// last stage of the tile, which consume_ring keeps.
-__device__ __forceinline__ void consume_tile(TopkSmem& sm, int num_kb, uint32_t& it, int wg, int lane, float (&d)[64]) {
-#pragma unroll
-  for (int i = 0; i < 64; ++i) d[i] = 0.f;
-  for (int kb = 0; kb < num_kb; ++kb, ++it) {
-    const int s = it % TK_STAGES;
-    mbar_wait(&sm.full_bar[s], (it / TK_STAGES) & 1u);
-    const uint32_t a_addr = smem_u32(sm.a[s]) + (uint32_t)(wg * 64 * ROW_BYTES);
-    const uint32_t b_addr = smem_u32(sm.b[s]);
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < ROW_BYTES / MMA_K_BYTES; ++k)
-      wgmma_m64n128<KIND_BF16>(d, wgmma_desc(a_addr + k * MMA_K_BYTES), wgmma_desc(b_addr + k * MMA_K_BYTES));
-    wgmma_commit();
-    wgmma_wait<1>();
-    if (kb > 0 && lane == 0) mbar_arrive(&sm.empty_bar[(it - 1) % TK_STAGES]);
-  }
-  wgmma_wait<0>();
-  if (lane == 0) mbar_arrive(&sm.empty_bar[(it - 1) % TK_STAGES]);
 }
 
 // the 16 rows of a consumer warp start with k padding entries each
@@ -245,52 +188,45 @@ __device__ __forceinline__ void write_partial(TopkSmem& sm, const TopkArgs& a, i
   }
 }
 
+// Consumer warps of both top-k kernels: the N tiles slice, slice + S, ... of M tile tile_m, accumulated tile after tile
+// from the ring and screened into the running lists, which then go to the workspace.
+__device__ __forceinline__ void topk_consume(TopkSmem& sm, const TopkArgs& a, int tile_m, int slice, int num_kb) {
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = (warp >> 2) - 1;
+  const int rbase = frag_row0(warp);
+  init_lists(sm, rbase, a.k, lane);
+  uint32_t it = 0;
+  float d[64];
+  for (int tn = slice; tn < (a.N + BN - 1) / BN; tn += a.S) {
+    consume<KIND_BF16>(sm.ring, num_kb, it, true, wg, lane, d);
+    topk_tile(sm, a, d, rbase, tile_m, tn * BN, lane);
+  }
+  write_partial(sm, a, rbase, tile_m, slice, lane);
+}
+
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_nt_topk_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                     const __grid_constant__ TopkArgs a) {
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
-  TopkSmem& sm = *reinterpret_cast<TopkSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  TopkSmem& sm = smem_as<TopkSmem>();
   const int tile_m = blockIdx.x, slice = blockIdx.y;
   const int n_tiles = (a.N + BN - 1) / BN;
-  const int num_kb = (a.K + BK_ELEMS - 1) / BK_ELEMS;
+  const int num_kb = (a.K + BK<KIND_BF16> - 1) / BK<KIND_BF16>;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < TK_STAGES; ++s) { mbar_init(&sm.full_bar[s], 1); mbar_init(&sm.empty_bar[s], kConsumerWarps); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_b) : "memory");
+    sm.ring.init(1);
+    prefetch_tensormap(&tmap_a);
+    prefetch_tensormap(&tmap_b);
   }
   __syncthreads();
 
-  if (warp < 4) {
-    // ===================== TMA producer: the ring runs across the tiles of the slice =====================
-    if (threadIdx.x == 0) {
-      uint32_t it = 0;
-      for (int tn = slice; tn < n_tiles; tn += a.S) {
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % TK_STAGES;
-          mbar_wait(&sm.empty_bar[s], ((it / TK_STAGES) & 1u) ^ 1u);  // first pass over the ring passes immediately
-          mbar_expect_tx(&sm.full_bar[s], A_BYTES + B_BYTES);
-          tma_load_2d(sm.a[s], &tmap_a, &sm.full_bar[s], kb * BK_ELEMS, tile_m * BM);
-          tma_load_2d(sm.b[s], &tmap_b, &sm.full_bar[s], kb * BK_ELEMS, tn * BN);
-        }
-      }
-    }
-  } else {
-    // ===================== consumers: wgmma -> registers -> running top-k =====================
-    const int wg = (warp >> 2) - 1;
-    const int rbase = wg * 64 + (warp & 3) * 16;
-    init_lists(sm, rbase, a.k, lane);
+  if (threadIdx.x >= 128) {
+    topk_consume(sm, a, tile_m, slice, num_kb);
+  } else if (threadIdx.x == 0) {
+    // TMA producer: the ring runs across the tiles of the slice
     uint32_t it = 0;
-    float d[64];
-    for (int tn = slice; tn < n_tiles; tn += a.S) {
-      consume_tile(sm, num_kb, it, wg, lane, d);
-      topk_tile(sm, a, d, rbase, tile_m, tn * BN, lane);
-    }
-    write_partial(sm, a, rbase, tile_m, slice, lane);
+    for (int tn = slice; tn < n_tiles; tn += a.S)
+      produce_tma<KIND_BF16>(sm.ring, tmap_a, tmap_b, tile_m * BM, tn * BN, 0, num_kb, it);
   }
 }
 
@@ -298,79 +234,29 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 gather_gemm_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ Ctx c,
                         const Key* __restrict__ keys, const __grid_constant__ TopkArgs a,
                         unsigned long long* __restrict__ stats) {
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
-  TopkSmem& sm = *reinterpret_cast<TopkSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  TopkSmem& sm = smem_as<TopkSmem>();
   const int tile_m = blockIdx.x, slice = blockIdx.y;
   const int n_tiles = (a.N + BN - 1) / BN;
-  const int num_kb = (a.K + BK_ELEMS - 1) / BK_ELEMS;
+  const int num_kb = (a.K + BK<KIND_BF16> - 1) / BK<KIND_BF16>;
   // The gather warps read store rows through the directory: this CTA counts in the grace epoch for all its tiles, so a
   // sync round that relocates rows waits for it (the host bounds the tiles per CTA through S).
   dev::cta_enter(c);
 
   if (threadIdx.x == 0) {
-    // full: 1 arrival (TMA expect_tx for the Q tile) + 4 arrivals (one per gather warp)
-    for (int s = 0; s < TK_STAGES; ++s) { mbar_init(&sm.full_bar[s], 5); mbar_init(&sm.empty_bar[s], kConsumerWarps); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_q) : "memory");
+    sm.ring.init(5);   // full: the TMA of the Q tile + one arrival per gather warp
+    prefetch_tensormap(&tmap_q);
   }
   __syncthreads();
 
-  if (warp < 4) {
-    // ===================== gatherers: store rows -> swizzled smem, tile after tile; thread 0 also TMAs Q ============
-    const int t = threadIdx.x;                // tile row handled by this thread (0..127)
-    unsigned nl = 0, nr = 0, nu = 0;
-    uint32_t it = 0;
-    for (int tn = slice; tn < n_tiles; tn += a.S) {
-      const int n = tn * BN + t;
-      const Key key = n < a.N ? keys[n] : 0;
-      dev::GatherRow row = {nullptr, nullptr, nullptr, nullptr, 0u, false};
-      if (n < a.N) {
-        row.row = dev::resolve_fast(c, key, class_of_key(c, key), &nl, &nr).row;
-        if (!row.row) {                          // transitional slot (relocation in flight)
-          row = dev::gather_locate(c, key);
-          if (!row.row) ++nu; else if (row.local) ++nl; else ++nr;
-        }
-      }
-      for (int kb = 0; kb < num_kb; ++kb, ++it) {
-        const int s = it % TK_STAGES;
-        mbar_wait(&sm.empty_bar[s], ((it / TK_STAGES) & 1u) ^ 1u);
-        if (t == 0) {
-          mbar_expect_tx(&sm.full_bar[s], A_BYTES);
-          tma_load_2d(sm.a[s], &tmap_q, &sm.full_bar[s], kb * BK_ELEMS, tile_m * BM);
-        }
-        stage_row_bf16(sm.b[s], c, key, row, t, kb * BK_ELEMS, a.K);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor core
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sm.full_bar[s]);
-      }
-    }
-    if (stats) {
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        nl += __shfl_xor_sync(0xffffffffu, nl, o); nr += __shfl_xor_sync(0xffffffffu, nr, o);
-        nu += __shfl_xor_sync(0xffffffffu, nu, o);
-      }
-      if (lane == 0) {
-        if (nl) atomicAdd(stats + 0, (unsigned long long)nl);
-        if (nr) atomicAdd(stats + 1, (unsigned long long)nr);
-        if (nu) atomicAdd(stats + 2, (unsigned long long)nu);   // unresolved rows, staged as zeros
-      }
-    }
+  if (threadIdx.x >= 128) {
+    topk_consume(sm, a, tile_m, slice, num_kb);
   } else {
-    // ===================== consumers: wgmma -> registers -> running top-k =====================
-    const int wg = (warp >> 2) - 1;
-    const int rbase = wg * 64 + (warp & 3) * 16;
-    init_lists(sm, rbase, a.k, lane);
+    // gatherers: store rows -> swizzled smem, tile after tile; thread 0 also TMAs Q
+    GatherStats st;
     uint32_t it = 0;
-    float d[64];
-    for (int tn = slice; tn < n_tiles; tn += a.S) {
-      consume_tile(sm, num_kb, it, wg, lane, d);
-      topk_tile(sm, a, d, rbase, tile_m, tn * BN, lane);
-    }
-    write_partial(sm, a, rbase, tile_m, slice, lane);
+    for (int tn = slice; tn < n_tiles; tn += a.S)
+      produce_gather(sm.ring, tmap_q, c, keys, tn * BN, a.N, a.K, tile_m * BM, num_kb, it, st);
+    st.flush(stats);
   }
   dev::cta_exit(c);
 }
@@ -416,18 +302,6 @@ topk_merge_kernel(const float* __restrict__ part_v, const int* __restrict__ part
   }
 }
 
-int num_sms() {
-  static int n = [] {
-    int dev = 0, v = 0;
-    ADAPM_CUDA_CHECK(cudaGetDevice(&dev));
-    ADAPM_CUDA_CHECK(cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev));
-    return v;
-  }();
-  return n;
-}
-
-size_t topk_smem() { return sizeof(TopkSmem) + 1024; }
-
 TopkArgs make_args(int M, int N, int K, int k, int S, const float* col_scale, const int64_t* ex_off, const int64_t* ex_cols,
                    float* part_v, int* part_c) {
   ADAPM_CHECK(k >= 1 && k <= kTopkMax, "topk: k must be in [1, " << kTopkMax << "]");
@@ -463,15 +337,9 @@ void gemm_nt_topk(cudaStream_t stream, const void* A, const void* B, int M, int 
   if (M == 0) return;
   const TopkArgs a = make_args(M, N, K, k, S, col_scale, ex_off, ex_cols, part_v, part_c);
   ADAPM_CHECK(N > 0, "gemm_nt_topk: no columns");
-  ADAPM_CHECK((K * 2) % 16 == 0, "gemm_nt_topk: the K extent must be a multiple of 16 bytes (TMA row pitch)");
-  ADAPM_CHECK((((uintptr_t)A) & 15u) == 0 && (((uintptr_t)B) & 15u) == 0, "gemm_nt_topk: operands must be 16-byte aligned");
-  CUtensorMap ma = make_map(A, M, K, BM, KIND_BF16);
-  CUtensorMap mb = make_map(B, N, K, BN, KIND_BF16);
-  set_max_dynamic_smem<gemm_nt_topk_kernel>((int)topk_smem());
-  dim3 grid((M + BM - 1) / BM, S);
-  gemm_nt_topk_kernel<<<grid, kGemmThreads, topk_smem(), stream>>>(ma, mb, a);
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_CUDA_CHECK(cudaGetLastError());
+  const CUtensorMap ma = make_map("gemm_nt_topk", A, M, K, BM, KIND_BF16);
+  const CUtensorMap mb = make_map("gemm_nt_topk", B, N, K, BN, KIND_BF16);
+  launch<gemm_nt_topk_kernel, TopkSmem>(dim3((M + BM - 1) / BM, S), stream, ma, mb, a);
   launch_merge(stream, a, out_v, out_i);
 }
 
@@ -489,15 +357,11 @@ void gather_gemm_topk(CudaBackend& be, cudaStream_t stream, const void* Q, const
   const TopkArgs a = make_args(M, N, K, k, S, col_scale, ex_off, ex_cols, part_v, part_c);
   ADAPM_CHECK(N > 0, "gather_gemm_topk: no keys");
   ADAPM_CHECK(K % 4 == 0, "gather_gemm_topk: the embedding length must be a multiple of 4");
-  ADAPM_CHECK(ldq % 8 == 0 && ldq >= K, "gather_gemm_topk: Q must be bf16 with a row pitch that is a multiple of 8 elements");
+  ADAPM_CHECK(ldq >= K, "gather_gemm_topk: Q's row pitch must be at least K");
   ADAPM_CHECK(be.ctx().L.val_bytes == 4, "the fused ops need float32 rows (Options::dtype)");
   be.track_stream(stream);
-  CUtensorMap mq = make_map(Q, M, ldq, BM, KIND_BF16);
-  set_max_dynamic_smem<gather_gemm_topk_kernel>((int)topk_smem());
-  dim3 grid((M + BM - 1) / BM, S);
-  gather_gemm_topk_kernel<<<grid, kGemmThreads, topk_smem(), stream>>>(mq, be.ctx(), keys, a, stats);
-  ADAPM_COUNT_LAUNCH();
-  ADAPM_CUDA_CHECK(cudaGetLastError());
+  const CUtensorMap mq = make_map("gather_gemm_topk", Q, M, ldq, BM, KIND_BF16);
+  launch<gather_gemm_topk_kernel, TopkSmem>(dim3((M + BM - 1) / BM, S), stream, mq, be.ctx(), keys, a, stats);
   launch_merge(stream, a, out_v, out_i);
 }
 

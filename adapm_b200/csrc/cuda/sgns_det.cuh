@@ -1,5 +1,5 @@
 // The deterministic one-GPU word2vec steps (SGNS: ops_sgns_tma.cu; CBOW and hierarchical softmax: ops_cbow.cu) and the
-// TMA rings of their kernels: mbarrier and bulk-copy helpers, the fixed-point scales, and one implementation of every
+// TMA rings of their kernels: bulk-copy helpers (the mbarriers are mbarrier.cuh's), the fixed-point scales, and one implementation of every
 // pass but the score pass. det_step runs a step: det_index gives each key a compact id, the op's score pass reads
 // start-of-step rows, det_group counts each key's entries and (after a scan) scatters them into a CSR grouped by key,
 // and the gather and finish passes apply them. The passes are generic over an entry source, which says what each entry
@@ -14,6 +14,7 @@
 
 #include "cuda_backend.h"
 #include "fx_accum.cuh"
+#include "mbarrier.cuh"
 #include "pm_kernels.cuh"
 
 namespace adapm {
@@ -29,27 +30,6 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(unsigned long long* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t parity) {
-  const uint32_t addr = smem_u32(bar);
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok) : "r"(addr), "r"(parity) : "memory");
-  } while (!ok);
-}
 // 1-D bulk copy global -> shared through the TMA engine; completes `bytes` on the mbarrier
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, unsigned long long* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
