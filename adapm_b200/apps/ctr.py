@@ -1,13 +1,15 @@
 """CTR application (BASELINE config #5) on the bindings-style API: DeepFM, a field-aware factorisation machine
 (``--model ffm``, libffm's model: one latent vector per field in every feature's row; ``--embed_dim`` is its k), or
 DLRM (``--model dlrm``: bottom MLP over the dense features, dot interaction, top MLP; synthetic planted data, or
-Criteo TSV files with ``--data`` / ``--test_data``).
+Criteo TSV files with ``--data`` / ``--test_data``), or DLRM-DCNv2 (``--model dlrm --interaction dcn``: a low-rank
+cross network of ``--cross_layers`` layers of rank ``--cross_rank`` instead of the dot interaction).
 
     python -m adapm_b200.launch -s 8 --backend cuda -m adapm_b200.apps.ctr -- --num_features 100000000
     python -m adapm_b200.apps.ctr --backend cpu --num_features 20000 --steps 30 --batch_size 512
     python -m adapm_b200.apps.ctr --backend cpu --num_features 20000 --steps 30 --batch_size 512 --multi_hot 3
     python -m adapm_b200.apps.ctr --backend cpu --model ffm --num_features 20000 --num_fields 8 --embed_dim 4 --steps 30
     python -m adapm_b200.apps.ctr --backend cpu --model dlrm --num_features 20000 --steps 30 --batch_size 512
+    python -m adapm_b200.apps.ctr --backend cpu --model dlrm --interaction dcn --cross_rank 64 --steps 30 --batch_size 512
 """
 from __future__ import annotations
 
@@ -48,8 +50,14 @@ def main(argv=None) -> int:
     ap.add_argument("--top", default="1024,1024,512,256", help="DLRM: hidden widths of the top MLP (W -> ... -> 1)")
     ap.add_argument("--data", default=None, help="DLRM: Criteo TSV training data (default: synthetic planted data)")
     ap.add_argument("--test_data", default=None, help="DLRM: Criteo TSV held-out data (needed with --data)")
+    ap.add_argument("--interaction", default="dot", choices=["dot", "dcn"],
+                    help="DLRM: dot interaction, or dcn (DLRM-DCNv2's low-rank cross network)")
+    ap.add_argument("--cross_layers", type=int, default=3, help="DLRM with --interaction dcn: cross layers")
+    ap.add_argument("--cross_rank", type=int, default=512, help="DLRM with --interaction dcn: rank of each layer")
     add_system_options(ap)
     args = ap.parse_args(strip_dashes(argv if argv is not None else sys.argv[1:]))
+    if args.interaction != "dot" and args.model != "dlrm":
+        ap.error(f"--interaction {args.interaction} needs --model dlrm")
     if args.model == "ffm":
         if args.multi_hot > 0:
             ap.error("--multi_hot is not supported with --model ffm (one id per field)")
@@ -163,7 +171,8 @@ def run_dlrm(args, bottom=(512, 256), top=(1024, 1024, 512, 256)) -> int:
     cfg = DLRMConfig(num_features=args.num_features, num_fields=num_fields, num_dense=num_dense,
                      embed_dim=args.embed_dim, bottom=bottom, top=top, lr_sparse=args.eta, batch_size=args.batch_size,
                      read_ahead=args.read_ahead, precision=args.precision, multi_hot=0 if args.data else args.multi_hot,
-                     pooling=args.pooling)
+                     pooling=args.pooling, interaction=args.interaction, cross_layers=args.cross_layers,
+                     cross_rank=args.cross_rank)
     ad.setup(cfg.num_features, 1)
     server = ad.Server(cfg.row_len, backend=args.backend, options=system_options(args))
     kv = ad.Worker(0, server)

@@ -276,6 +276,25 @@ void dlrm_interaction_forward(cudaStream_t stream, const float* z, const float* 
 void dlrm_interaction_backward(cudaStream_t stream, const float* dR, const float* z, const float* e, int64_t B, int F,
                                int E, int W, float* dz, float* de);
 
+// DCN-v2 low-rank cross network (ops_dcn.cu): x_{l+1} = x_0 * (W_l (V_l x_l) + b_l) + x_l, x_0 = [z | e] [B, N] from
+// z [B, E] and e [B, F, E] (N = (F + 1) E); V [L, r, N], W [L, N, r] (and the backward's Vt [L, N, r], Wt [L, r, N]) bf16,
+// b [L, N] fp32. N % 8 == 0, r % 8 == 0, 8 <= r <= 1024, 1 <= L <= 8, B * N < 2^31. Transposed buffers [*, pitch] have
+// pitch = B rounded up to 8. forward (1 + 2 L launches): x [B, N] fp32 = x_L; xb [B, N], hb [B, r] bf16 scratch; when
+// training (xt non-null) also xt [L, N, pitch] = x_l^T, ht [L, r, pitch] = h_l^T and ub [L, B, N] = u_l in bf16 for the
+// backward. backward: grad_out [B, N]; G, dx0 [B, N] fp32, Pb [B, N], Pt [N, pitch], dh [B, r], dht [r, pitch] bf16 and
+// ws (dcn_workspace_floats) scratch; writes dz, de, dV [L, r, N], dW [L, N, r], db [L, N]. No floating-point atomics:
+// bit-identical reruns on one GPU.
+constexpr int kDcnMaxLayers = 8;
+constexpr int kDcnMinRank = 8;
+constexpr int kDcnMaxRank = 1024;
+size_t dcn_workspace_floats(int B, int N, int r);
+void dcn_forward(cudaStream_t stream, const float* z, const float* e, int B, int E, int N, int r, int L, const void* V,
+                 const void* W, const float* b, void* xb, void* hb, float* x, void* xt, void* ht, void* ub);
+void dcn_backward(cudaStream_t stream, const float* z, const float* e, int B, int E, int N, int r, int L, const void* Vt,
+                  const void* Wt, const void* xt, const void* ht, const void* ub, const float* grad_out, float* G,
+                  float* dx0, void* Pb, void* Pt, void* dh, void* dht, float* ws, float* dz, float* de, float* dV,
+                  float* dW, float* db);
+
 constexpr int kEmbBagMaxDim = 512;
 size_t embedding_bag_workspace_bytes(int64_t nnz, int E);
 void embedding_bag_forward(CudaBackend& be, cudaStream_t stream, const Key* keys, const int64_t* offsets,

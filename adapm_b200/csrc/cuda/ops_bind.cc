@@ -271,6 +271,27 @@ void bind(py::module_& m) {
     dlrm_interaction_backward((cudaStream_t)stream, ptr<const float>(dR), ptr<const float>(z), ptr<const float>(e), B,
                               F, E, W, ptr<float>(dz), ptr<float>(de));
   });
+  m.attr("dcn_max_layers") = kDcnMaxLayers;
+  m.attr("dcn_min_rank") = kDcnMinRank;
+  m.attr("dcn_max_rank") = kDcnMaxRank;
+  m.def("dcn_workspace_floats", [](int B, int N, int r) { return dcn_workspace_floats(B, N, r); });
+  m.def("dcn_forward", [](uintptr_t stream, uintptr_t z, uintptr_t e, int B, int E, int N, int r, int L, uintptr_t V,
+                          uintptr_t W, uintptr_t b, uintptr_t xb, uintptr_t hb, uintptr_t x, uintptr_t xt, uintptr_t ht,
+                          uintptr_t ub) {
+    dcn_forward((cudaStream_t)stream, ptr<const float>(z), ptr<const float>(e), B, E, N, r, L, ptr<const void>(V),
+                ptr<const void>(W), ptr<const float>(b), ptr<void>(xb), ptr<void>(hb), ptr<float>(x), ptr<void>(xt),
+                ptr<void>(ht), ptr<void>(ub));
+  });
+  m.def("dcn_backward", [](uintptr_t stream, uintptr_t z, uintptr_t e, int B, int E, int N, int r, int L, uintptr_t Vt,
+                           uintptr_t Wt, uintptr_t xt, uintptr_t ht, uintptr_t ub, uintptr_t grad_out, uintptr_t G,
+                           uintptr_t dx0, uintptr_t Pb, uintptr_t Pt, uintptr_t dh, uintptr_t dht, uintptr_t ws,
+                           uintptr_t dz, uintptr_t de, uintptr_t dV, uintptr_t dW, uintptr_t db) {
+    dcn_backward((cudaStream_t)stream, ptr<const float>(z), ptr<const float>(e), B, E, N, r, L, ptr<const void>(Vt),
+                 ptr<const void>(Wt), ptr<const void>(xt), ptr<const void>(ht), ptr<const void>(ub),
+                 ptr<const float>(grad_out), ptr<float>(G), ptr<float>(dx0), ptr<void>(Pb), ptr<void>(Pt),
+                 ptr<void>(dh), ptr<void>(dht), ptr<float>(ws), ptr<float>(dz), ptr<float>(de), ptr<float>(dV),
+                 ptr<float>(dW), ptr<float>(db));
+  });
   m.attr("ffm_max_fields") = kFfmMaxFields;
   m.attr("ffm_max_k") = kFfmMaxK;
   m.attr("ffm_max_fk") = kFfmMaxFk;

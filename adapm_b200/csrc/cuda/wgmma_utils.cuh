@@ -358,16 +358,18 @@ inline EncodeTiledFn encode_fn() {
   return fn;
 }
 
-// row-major [rows, cols] matrix of 2-byte (bf16) or 1-byte (e4m3) elements,
+// row-major [rows, cols] matrix of 2-byte (bf16) or 1-byte (e4m3) elements, rows `pitch` elements apart (0: cols),
 // box = [box_rows, 128 bytes of K], 128-byte swizzle. `op` names the caller in the error for an operand that TMA cannot
-// read: its base must be 16-byte aligned and its row pitch a multiple of 16 bytes.
-inline CUtensorMap make_map(const char* op, const void* base, int64_t rows, int64_t cols, int box_rows, int kind) {
+// read: its base must be 16-byte aligned and its row pitch a multiple of 16 bytes. Columns past cols read as zeros.
+inline CUtensorMap make_map(const char* op, const void* base, int64_t rows, int64_t cols, int box_rows, int kind,
+                            int64_t pitch = 0) {
   CUtensorMap m;
   const int esz = kind == KIND_BF16 ? 2 : 1;
-  ADAPM_CHECK((reinterpret_cast<uintptr_t>(base) & 15u) == 0 && (cols * esz) % 16 == 0,
+  if (pitch == 0) pitch = cols;
+  ADAPM_CHECK((reinterpret_cast<uintptr_t>(base) & 15u) == 0 && (pitch * esz) % 16 == 0 && pitch >= cols,
               op << ": tensor-core operands must be 16-byte aligned, with rows a multiple of 16 bytes long");
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)cols * esz};
+  cuuint64_t strides[1] = {(cuuint64_t)pitch * esz};
   cuuint32_t box[2] = {(cuuint32_t)(ROW_BYTES / esz), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = encode_fn()(&m, kind == KIND_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8, 2,

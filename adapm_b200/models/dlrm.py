@@ -1,11 +1,14 @@
-"""CTR prediction with DLRM (Naumov et al., 2019) on the parameter manager: MLPerf's recommendation model.
+"""CTR prediction with DLRM (Naumov et al., 2019) on the parameter manager, and DLRM-DCNv2, MLPerf's recommendation
+model since 2023.
 
 * the sparse part - one row per feature id, ``[embedding (E) | AdaGrad (E)]`` - lives in the parameter manager; every
   (example, field) is a bag of ids pooled by ``ops.StoreEmbeddingBag`` (one id per bag for single-hot data), whose
   backward pushes one AdaGrad update per distinct id;
 * the dense features go through the bottom MLP (num_dense -> bottom... -> E, ReLU on every layer);
-* ``ops.dlrm_interaction`` forms ``[z | <T_i, T_j> for j < i]`` from ``T = [z; e_1 .. e_F]`` (one fused kernel each way
-  on a CUDA server), the top MLP (W -> top... -> 1) gives the logit, BCE-with-logits the loss;
+* ``interaction="dot"``: ``ops.dlrm_interaction`` forms ``[z | <T_i, T_j> for j < i]`` from ``T = [z; e_1 .. e_F]``
+  (one fused kernel each way on a CUDA server); ``interaction="dcn"``: ``ops.dcn_cross``, the low-rank cross network
+  of DCN-v2 (Wang et al., 2021) over ``x_0 = [z | e_1 .. e_F]`` (bf16 tensor-core GEMMs with fused elementwise work on
+  a CUDA server, fp32 on the torch route); the top MLP (W or N -> top... -> 1) gives the logit, BCE-with-logits the loss;
 * the MLPs are replicated, trained by Adam; their gradients are all-reduced with ``torch.distributed`` when available,
   as in DeepFM. On a CUDA server their linear layers run on the hand-written wgmma GEMM (``precision``).
 """
@@ -17,6 +20,7 @@ from typing import Optional
 
 import numpy as np
 import torch
+from torch import nn
 
 from .deepfm import DenseNet
 from .ffm import PLANT_DIM, PLANT_TYPES, logloss_auc
@@ -38,6 +42,9 @@ class DLRMConfig:
     multi_hot: int = 0                  # > 0: up to this many ids per field (synthetic_dlrm_batch); 0: one id per field
     pooling: str = "sum"                # sum | mean (multi-hot fields)
     model_seed: int = 1
+    interaction: str = "dot"            # dot | dcn (DLRM-DCNv2: low-rank cross network)
+    cross_layers: int = 3               # dcn: layers L
+    cross_rank: int = 512               # dcn: rank r of V_l [r, N] and W_l [N, r]
 
     @property
     def row_len(self) -> int:           # [embedding | AdaGrad]
@@ -49,27 +56,59 @@ class DLRMConfig:
 
         return dlrm_interaction_width(self.num_fields, self.embed_dim)
 
+    @property
+    def cross_width(self) -> int:       # N = (F + 1) E, the width of the cross network
+        return (self.num_fields + 1) * self.embed_dim
+
+
+class CrossNet(nn.Module):
+    """The parameters of DCN-v2's low-rank cross network (``ops.dcn_cross``): ``V [L, r, N]`` and ``W [L, N, r]``
+    Xavier-normal from ``seed``, ``b [L, N]`` zero."""
+
+    def __init__(self, N: int, rank: int, layers: int, seed: int):
+        super().__init__()
+        g = torch.Generator().manual_seed(seed)
+        std = (2.0 / (N + rank)) ** 0.5
+        self.V = nn.Parameter(torch.randn(layers, rank, N, generator=g) * std)
+        self.W = nn.Parameter(torch.randn(layers, N, rank, generator=g) * std)
+        self.b = nn.Parameter(torch.zeros(layers, N))
+
+    def forward(self, z, e, impl: str = "auto"):
+        from ..ops import dcn_cross
+
+        return dcn_cross(z, e, self.V, self.W, self.b, impl=impl)
+
 
 class DLRM:
     def __init__(self, server, worker, cfg: DLRMConfig, impl: str = "auto"):
-        """``impl`` selects the route of ``ops.dlrm_interaction`` (``auto``: the fused kernels on a CUDA server)."""
+        """``impl`` selects the route of ``ops.dlrm_interaction`` or ``ops.dcn_cross`` (``auto``: the fused kernels on a
+        CUDA server)."""
         from ..ops import StoreEmbeddingBag, dlrm_interaction_width
 
         if cfg.precision not in ("bf16", "fp8", "fp32"):
             raise ValueError(f"precision must be bf16, fp8 or fp32, got {cfg.precision!r}")
         if cfg.num_dense < 1:
             raise ValueError(f"num_dense must be >= 1, got {cfg.num_dense}")
+        if cfg.interaction not in ("dot", "dcn"):
+            raise ValueError(f"interaction must be dot or dcn, got {cfg.interaction!r}")
         self.server, self.worker, self.cfg, self.impl = server, worker, cfg, impl
         self.dev = server.device
         tc = server.backend == "cuda"
         E, W = cfg.embed_dim, dlrm_interaction_width(cfg.num_fields, cfg.embed_dim)
         self.bottom = DenseNet(cfg, tc, dims=[cfg.num_dense, *cfg.bottom, E], relu_last=True,
                                seed=cfg.model_seed).to(self.dev)
+        self.cross = None
+        if cfg.interaction == "dcn":
+            W = cfg.cross_width
+            self.cross = CrossNet(W, cfg.cross_rank, cfg.cross_layers, cfg.model_seed + 2).to(self.dev)
         self.top = DenseNet(cfg, tc, dims=[W, *cfg.top, 1], seed=cfg.model_seed + 1).to(self.dev)
-        self.opt = torch.optim.Adam([*self.bottom.parameters(), *self.top.parameters()], lr=cfg.lr_dense)
+        self.opt = torch.optim.Adam(self._dense_parameters(), lr=cfg.lr_dense)
         self.bag = StoreEmbeddingBag(server, worker, E, mode=cfg.pooling, lr=cfg.lr_sparse)
         self.step_no = 0
         self.rows_pushed = 0      # (key, row) updates applied so far (distinct feature rows per batch)
+
+    def _dense_parameters(self):
+        return [*self.bottom.parameters(), *self.top.parameters(), *(self.cross.parameters() if self.cross else ())]
 
     def init_model(self, chunk: int = 1 << 18) -> None:
         """Embeddings uniform in +-sqrt(1 / rows per field), accumulators 0; every rank initialises the keys it is home
@@ -116,6 +155,8 @@ class DLRM:
             raise ValueError(f"dense must be [{B}, {cfg.num_dense}], got {tuple(dense.shape)}")
         z = self.bottom(dense.to(self.dev, non_blocking=True).float())
         e = self.bag(keys, off).view(B, cfg.num_fields, cfg.embed_dim)
+        if self.cross is not None:
+            return self.top(self.cross(z, e, impl=self.impl)), B
         return self.top(dlrm_interaction(z, e, impl=self.impl)), B
 
     def step(self, dense: torch.Tensor, ids: torch.Tensor, labels: torch.Tensor,
@@ -130,7 +171,7 @@ class DLRM:
         self.opt.zero_grad(set_to_none=True)
         loss.backward()
         if torch.distributed.is_available() and torch.distributed.is_initialized() and self.server.num_servers() > 1:
-            for p in (*self.bottom.parameters(), *self.top.parameters()):
+            for p in self._dense_parameters():
                 torch.distributed.all_reduce(p.grad)
                 p.grad /= self.server.num_servers()
         self.opt.step()

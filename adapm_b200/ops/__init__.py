@@ -2018,6 +2018,172 @@ def dlrm_interaction_reference(z: torch.Tensor, e: torch.Tensor, grad_out: Optio
     return R, g[:, :E] + dT[:, 0], dT[:, 1:]
 
 
+DCN_MAX_LAYERS = 8
+DCN_MIN_RANK = 8
+DCN_MAX_RANK = 1024
+
+
+def _check_dcn_args(z, e, V, W, b, fused: bool):
+    """(B, E, N, r, L) of dcn_cross's arguments; ValueError / TypeError before anything is launched"""
+    for t, nm in ((z, "z"), (e, "e"), (V, "V"), (W, "W"), (b, "b")):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.float32:
+            raise TypeError(f"{nm} must be a float32 tensor")
+        if t.device != z.device:
+            raise TypeError(f"dcn_cross needs all tensors on one device, got {nm} on {t.device} and z on {z.device}")
+    if z.dim() != 2 or e.dim() != 3:
+        raise ValueError(f"z must be [B, E] and e [B, F, E], got {tuple(z.shape)} and {tuple(e.shape)}")
+    B, E = z.shape
+    F = e.shape[1]
+    if e.shape[0] != B or e.shape[2] != E or F < 1 or E < 1:
+        raise ValueError(f"e must be [B, F, E] = [{B}, F >= 1, {E}], got {tuple(e.shape)}")
+    N = (F + 1) * E
+    if V.dim() != 3 or V.shape[2] != N:
+        raise ValueError(f"V must be [L, r, N] with N = (F + 1) E = {N}, got {tuple(V.shape)}")
+    L, r = V.shape[0], V.shape[1]
+    if tuple(W.shape) != (L, N, r):
+        raise ValueError(f"W must be [L, N, r] = [{L}, {N}, {r}], got {tuple(W.shape)}")
+    if tuple(b.shape) != (L, N):
+        raise ValueError(f"b must be [L, N] = [{L}, {N}], got {tuple(b.shape)}")
+    if not 1 <= L <= DCN_MAX_LAYERS:
+        raise ValueError(f"dcn_cross needs 1 <= L <= {DCN_MAX_LAYERS}, got L = {L}")
+    if B * N >= 1 << 31:
+        raise ValueError(f"dcn_cross needs B * N < 2^31, got B = {B}, N = {N}")
+    if fused:
+        if B < 1:
+            raise ValueError("impl='fused' needs B >= 1")
+        if N % 8 or r % 8:
+            raise ValueError(f"impl='fused' needs N and r multiples of 8 (16-byte TMA rows), got N = {N}, r = {r}")
+        if not DCN_MIN_RANK <= r <= DCN_MAX_RANK:
+            raise ValueError(f"impl='fused' needs {DCN_MIN_RANK} <= r <= {DCN_MAX_RANK}, got r = {r}")
+        if not z.is_cuda:
+            raise ValueError("impl='fused' needs CUDA tensors")
+    return B, E, N, r, L
+
+
+def _dcn_cross_torch(z, e, V, W, b):
+    x0 = torch.cat([z, e.reshape(z.shape[0], -1)], 1)
+    x = x0
+    for l in range(V.shape[0]):
+        x = x0 * (torch.matmul(torch.matmul(x, V[l].t()), W[l].t()) + b[l]) + x
+    return x
+
+
+def _dcn_fused_forward(z, e, V16, W16, b, train: bool):
+    """x_L, and with ``train`` the bf16 tensors the backward reads: (x_l^T, h_l^T, u_l)"""
+    B, E = z.shape
+    L, r, N = V16.shape
+    P = (B + 7) // 8 * 8
+    dev = z.device
+    bf = dict(dtype=torch.bfloat16, device=dev)
+    x = torch.empty(B, N, dtype=torch.float32, device=dev)
+    xb, hb = torch.empty(B, N, **bf), torch.empty(B, r, **bf)
+    saved = (torch.empty(L, N, P, **bf), torch.empty(L, r, P, **bf), torch.empty(L, B, N, **bf)) if train else None
+    xt, ht, ub = (t.data_ptr() for t in saved) if train else (0, 0, 0)
+    _C.dcn_forward(_stream(z), z.data_ptr(), e.data_ptr(), B, E, N, r, L, V16.data_ptr(), W16.data_ptr(), b.data_ptr(),
+                   xb.data_ptr(), hb.data_ptr(), x.data_ptr(), xt, ht, ub)
+    return x, saved
+
+
+class _DcnCrossFn(torch.autograd.Function):
+    """The fused route of :func:`dcn_cross` (csrc/cuda/ops_dcn.cu): 1 + 2 L launches forward, and per layer an
+    elementwise pass, the db sum and four GEMMs backward."""
+
+    @staticmethod
+    def forward(ctx, z, e, V, W, b):
+        z, e, b = z.contiguous(), e.contiguous(), b.contiguous()
+        x, saved = _dcn_fused_forward(z, e, V.to(torch.bfloat16).contiguous(), W.to(torch.bfloat16).contiguous(), b,
+                                      train=True)
+        ctx.save_for_backward(z, e, V, W, *saved)
+        return x
+
+    @staticmethod
+    def backward(ctx, gx):
+        z, e, V, W, xt, ht, ub = ctx.saved_tensors
+        B, E = z.shape
+        L, r, N = V.shape
+        P = (B + 7) // 8 * 8
+        dev = z.device
+        Vt = V.transpose(1, 2).to(torch.bfloat16).contiguous()
+        Wt = W.transpose(1, 2).to(torch.bfloat16).contiguous()
+        gx = gx.to(torch.float32).contiguous()
+        bf = dict(dtype=torch.bfloat16, device=dev)
+        f32 = dict(dtype=torch.float32, device=dev)
+        G, dx0 = torch.empty(B, N, **f32), torch.empty(B, N, **f32)
+        Pb, Pt, dh, dht = torch.empty(B, N, **bf), torch.empty(N, P, **bf), torch.empty(B, r, **bf), torch.empty(r, P, **bf)
+        ws = torch.empty(_C.dcn_workspace_floats(B, N, r), **f32)
+        dz, de = torch.empty_like(z), torch.empty_like(e)
+        dV, dW, db = torch.empty(L, r, N, **f32), torch.empty(L, N, r, **f32), torch.empty(L, N, **f32)
+        _C.dcn_backward(_stream(gx), z.data_ptr(), e.data_ptr(), B, E, N, r, L, Vt.data_ptr(), Wt.data_ptr(),
+                        xt.data_ptr(), ht.data_ptr(), ub.data_ptr(), gx.data_ptr(), G.data_ptr(), dx0.data_ptr(),
+                        Pb.data_ptr(), Pt.data_ptr(), dh.data_ptr(), dht.data_ptr(), ws.data_ptr(), dz.data_ptr(),
+                        de.data_ptr(), dV.data_ptr(), dW.data_ptr(), db.data_ptr())
+        return dz, de, dV, dW, db
+
+
+def dcn_cross(z: torch.Tensor, e: torch.Tensor, V: torch.Tensor, W: torch.Tensor, b: torch.Tensor,
+              impl: str = "auto") -> torch.Tensor:
+    """DCN-v2's low-rank cross network (Wang et al., 2021; torchrec's ``LowRankCrossNet``) on DLRM's features:
+    ``x_L float32 [B, N]`` from ``x_0 = [z | e_0 | .. | e_{F-1}]`` (``N = (F + 1) E``) by the L layers
+    ``x_{l+1} = x_0 * (W_l (V_l x_l) + b_l) + x_l``.
+
+    ``z`` float32 ``[B, E]`` (the bottom-MLP output), ``e`` float32 ``[B, F, E]`` (the pooled fields, as for
+    :func:`dlrm_interaction`), ``V [L, r, N]``, ``W [L, N, r]``, ``b [L, N]`` float32. Autograd reaches all five.
+    ``impl``: ``fused`` (CUDA tensors) - the kernels of csrc/cuda/ops_dcn.cu, GEMMs on the tensor cores with bf16
+    operands and fp32 accumulation, the residual stream in fp32, bit-identical reruns; ``torch`` - the fp32 rule with
+    ``matmul`` (CPU tensors, and the comparison arm of benchmarks/dcn_bench.py); ``auto`` picks ``fused`` for CUDA
+    tensors. Limits: ``1 <= L <= 8``, ``B * N < 2^31``; on ``fused`` also ``B >= 1``, ``N`` and ``r`` multiples of 8,
+    ``8 <= r <= 1024``."""
+    if impl not in ("auto", "fused", "torch"):
+        raise ValueError(f"impl must be 'auto', 'fused' or 'torch', got {impl!r}")
+    if impl == "auto":
+        impl = "fused" if isinstance(z, torch.Tensor) and z.is_cuda else "torch"
+    _check_dcn_args(z, e, V, W, b, fused=impl == "fused")
+    if impl == "torch":
+        return _dcn_cross_torch(z, e, V, W, b)
+    if torch.is_grad_enabled() and any(t.requires_grad for t in (z, e, V, W, b)):
+        return _DcnCrossFn.apply(z, e, V, W, b)
+    return _dcn_fused_forward(z.contiguous(), e.contiguous(), V.to(torch.bfloat16).contiguous(),
+                              W.to(torch.bfloat16).contiguous(), b.contiguous(), train=False)[0]
+
+
+def dcn_cross_reference(z: torch.Tensor, e: torch.Tensor, V: torch.Tensor, W: torch.Tensor, b: torch.Tensor,
+                        grad_out: Optional[torch.Tensor] = None, bf16_operands: bool = False):
+    """The rule of :func:`dcn_cross` in float64 on the CPU (tests): ``(x_L, dz, de, dV, dW, db)``, the gradients for
+    ``grad_out [B, N]`` (None without it). With ``bf16_operands`` the values are rounded to bf16 where the fused route
+    rounds them: the GEMM operands x_l, h_l, V, W (forward) and P = G * x_0, dh, V, W (backward), and the saved u_l that
+    the backward multiplies G by; sums stay float64."""
+    def rb(t):
+        return t.to(torch.bfloat16).double() if bf16_operands else t
+
+    z64, e64 = z.detach().cpu().double(), e.detach().cpu().double()
+    V64, W64, b64 = V.detach().cpu().double(), W.detach().cpu().double(), b.detach().cpu().double()
+    B, E = z64.shape
+    x0 = torch.cat([z64, e64.reshape(B, -1)], 1)
+    x, xs, hs, us = x0, [], [], []
+    for l in range(V64.shape[0]):
+        xs.append(rb(x))
+        hs.append(rb(xs[-1] @ rb(V64[l]).t()))
+        u = hs[-1] @ rb(W64[l]).t() + b64[l]
+        us.append(rb(u))
+        x = x0 * u + x
+    if grad_out is None:
+        return x, None, None, None, None, None
+    G = grad_out.detach().cpu().double()
+    dx0 = torch.zeros_like(x0)
+    dV, dW, db = torch.zeros_like(V64), torch.zeros_like(W64), torch.zeros_like(b64)
+    for l in reversed(range(V64.shape[0])):
+        P = G * x0
+        dx0 += G * us[l]
+        db[l] = P.sum(0)
+        Pb = rb(P)
+        dh = rb(Pb @ rb(W64[l]))
+        dW[l] = Pb.t() @ hs[l]
+        dV[l] = dh.t() @ xs[l]
+        G = G + dh @ rb(V64[l])
+    dx0 += G
+    return x, dx0[:, :E], dx0[:, E:].reshape(e64.shape), dV, dW, db
+
+
 FFM_MAX_FIELDS = 64
 FFM_MAX_K = 32
 FFM_MAX_FK = 512
